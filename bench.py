@@ -9,7 +9,7 @@ Workloads (BASELINE.json `configs`; SURVEY.md 8(d) inputs, generators in se-ssd_
   frame-ring     configs[1]: car-only inference, batch 1 per launch, full path voxelise -> sparse 3-D encoder -> BEV neck/head ->
                  rotated NMS, seeded "ring-20k" clouds (KITTI-like 64-beam scan).  DEFAULT = the headline line.
   frame-uniform  same path on the "uniform-20k" input (SURVEY 8(d) primary input; over-dilates through the strided convs).
-  stress         configs[4] shape on one GPU per rank: "uniform-200k" clouds, batch 16 per launch, max_voxels 200000.
+  stress         configs[4] shape on one GPU per rank: "uniform-200k" clouds, batch 8 per launch (fits 80 GB), max_voxels 200000.
 The default line also carries `extra.uniform20k` and `extra.stress` sub-records (N=1 only; --no-extra skips them).
 
 One STEP = `--frames-per-step` frames pushed through `--streams` concurrent engines (one CUDA graph each).
@@ -51,6 +51,8 @@ def parse():
     ap.add_argument("--cg-deep", type=int, default=None, help="sparse conv pipeline: 1 deep / one CTA per SM, 0 two CTAs per SM (default: the engine's choice)")
     ap.add_argument("--quick", action="store_true", help="skip the e2e / roofline / cpu_baseline / extra legs (tuning runs)")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra.uniform20k / extra.stress sub-records")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps write what each engine returned for its last batch of the last step as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -60,8 +62,8 @@ WORKLOADS = {
                        name="examples/second car-only inference, batch 1, full voxel->sparse3d->BEV->IoU/NMS, synthetic ring-20k clouds"),
     "frame-uniform": dict(cloud="uniform", points=20000, batch=1, max_voxels=20000,
                           name="examples/second car-only inference, batch 1, full voxel->sparse3d->BEV->IoU/NMS, synthetic uniform-20k clouds"),
-    "stress": dict(cloud="uniform", points=200000, batch=16, max_voxels=200000,
-                   name="dense-scene stress: uniform-200k clouds, 0.05 m voxels, batch 16 per launch, full path"),
+    "stress": dict(cloud="uniform", points=200000, batch=8, max_voxels=200000,
+                   name="dense-scene stress: uniform-200k clouds, 0.05 m voxels, batch 8 per launch, full path"),
 }
 
 
@@ -87,7 +89,7 @@ def bench_weights(wl):
 
 # ------------------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -162,16 +164,11 @@ def run_reference(args):
     torch.set_num_threads(min(CPU_THREADS, os.cpu_count() or 1))
     lnp = oframe.layers_to_numpy(layers)
     mv = WORKLOADS[wl]["max_voxels"]
-    budget_s = 150.0
-    t0 = time.perf_counter()
     oframe.frame_detections(clouds[0], lnp, ssfa, head, anchors, max_voxels=mv)          # first frame: page-in, thread pools
-    t_first = time.perf_counter() - t0
-    warm = max(0, min(args.warmup - 1, int(0.25 * budget_s / max(t_first, 1e-3))))
+    warm = max(0, args.warmup - 1)
     for i in range(warm):
         oframe.frame_detections(clouds[(i + 1) % len(clouds)], lnp, ssfa, head, anchors, max_voxels=mv)
-    spent = time.perf_counter() - t0
-    per_frame = spent / (1 + warm)
-    steps = max(1, min(args.steps, int((budget_s - spent) / max(per_frame, 1e-3))))
+    steps = args.steps                                                                    # exactly --steps timed frames (~1 s each)
     stage = {}
     t0 = time.perf_counter()
     for i in range(steps):
@@ -333,6 +330,8 @@ def run_ours(args):
     ms_value = rig.timed(fn, args.steps)
     clocks = sampler.stop()
     value = world * F * args.steps / (ms_value / 1000.0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(rig, args.dump_outputs)
 
     if args.quick:
         if rank == 0:
@@ -372,7 +371,7 @@ def run_ours(args):
                 "data": "synthetic", "config": workload_config(wl),
                 "run": {"frames_per_step_per_gpu": F, "streams": S, "parallelism": "frame-sharded x%d, no collective" % world,
                         "timed_region_s": {"value": ms_value / 1000.0, "e2e": ms_e2e / 1000.0},
-                        "l2": "no explicit flush: per-frame activation working set (~0.4 GB) exceeds the 126 MB L2; inputs rotate over %d clouds" % args.pool},
+                        "l2": "no explicit flush: per-frame activation working set (~0.4 GB) exceeds the 50 MB L2; inputs rotate over %d clouds" % args.pool},
                 "e2e": {"value": e2e, "unit": "frames/s", "ms_per_step": ms_e2e / args.steps,
                         "h2d_bytes_per_step": rig.h2d // args.steps, "d2h_bytes_per_step": rig.d2h // args.steps},
                 "gpu_launches": int(rig.launches_per_batch) * (F // B) * args.steps,
@@ -387,7 +386,7 @@ def run_ours(args):
                                               "restatement, no CPU implementation exists in the reference)" % (n_cpu, stage)}
             line["parity_vs_oracle"] = parity_vs_oracle(rig, outs)
             if not args.no_extra and wl == "frame-ring":
-                # release the headline rig before building the next ones (stress needs ~90 GB)
+                # release the headline rig before building the next ones (stress needs ~45 GB)
                 del rig
                 torch.cuda.empty_cache()
                 line["extra"] = {"uniform20k": extra_uniform(args, dev), "stress": extra_stress(args, dev, peaks)}
@@ -397,13 +396,23 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
+def dump_outputs(rig, out_dir):
+    """What the HBM-resident timed loop computed in its last step: the packed detections [B, post_max, 8] (box3d_lidar 7 + score) and
+    the per-frame meta rows (count, candidates, ..., kept anchor indices) each engine returned for its last batch, as float32 / float64."""
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    for k, e in enumerate(rig.engines):
+        np.save(os.path.join(out_dir, "result_engine%02d.npy" % k), e.d_result.detach().cpu().numpy().astype(np.float32))
+        np.save(os.path.join(out_dir, "meta_engine%02d.npy" % k), e.d_meta.detach().cpu().numpy().astype(np.float64))
+
+
 def load_peaks():
     try:
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return {"hbm": float(p["hbm_gbs"]), "tf_burst": float(p["bf16_tflops"]), "tf_sustained": float(p.get("bf16_tflops_sustained", p["bf16_tflops"])),
                 "source": "MEASURED_PEAKS.json (of measured)"}
     except Exception:
-        return {"hbm": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "source": "B200_PROFILING.md fallback (of fallback)"}
+        return {"hbm": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "source": "H100 SXM datasheet (HBM3 3.35 TB/s, dense bf16 989 TFLOP/s)"}
 
 
 # ------------------------------------------------------------------------------------------------------------------ parity leg
@@ -470,34 +479,10 @@ def parity_vs_oracle(rig, outs):
 
 
 # ------------------------------------------------------------------------------------------------------------------ roofline leg
-def read_ncu_traffic(kernel_substr):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of the kernel from the newest committed profiles/r2*_ncu.txt summary
-    (written by scripts/ncu_summary.py from an `ncu --set full` capture); None when no capture of this round names the kernel."""
-    import glob
-    import re
-    best = None
-    for path in sorted(glob.glob(os.path.join(ROOT, "profiles", "r2*_ncu.txt"))):
-        try:
-            txt = open(path).read()
-        except OSError:
-            continue
-        for block in txt.split("== ")[1:]:
-            if kernel_substr not in block.splitlines()[0]:
-                continue
-            rd = re.search(r"dram__bytes_read\.sum\s+([0-9.]+) (\w+)", block)
-            wr = re.search(r"dram__bytes_write\.sum\s+([0-9.]+) (\w+)", block)
-            if rd and wr:
-                unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-                best = (float(rd.group(1)) * unit.get(rd.group(2), 1.0) + float(wr.group(1)) * unit.get(wr.group(2), 1.0),
-                        os.path.relpath(path, ROOT))
-                break
-    return best
-
-
 def dominant_kernel_roofline(e, peaks, reps=20):
     """The conv3x3 128->128 @200x176 layer (largest share of the step; 5 of the 13 neck launches have this shape), timed alone with
     CUDA events on the engine stream, through the same runner call the frame graph uses, L2 flushed before every launch.
-    Two-term fp16 split: THREE kind::f16 products per algorithmic MAC (fp32-level parity) => ceiling of `frac` against the bf16 peak is 1/3."""
+    Two-term fp16 split: THREE fp16 wgmma products per algorithmic MAC (fp32-level parity) => ceiling of `frac` against the bf16 peak is 1/3."""
     neck = e.neck
     flops = 2.0 * neck.batch * neck.h * neck.w * 128 * 128 * 9
     flush = torch.empty((64 * 1024 * 1024,), dtype=torch.float32, device=e.device)   # 256 MB > L2
@@ -515,11 +500,9 @@ def dominant_kernel_roofline(e, peaks, reps=20):
             e.stream.synchronize()
             ms.append(a.elapsed_time(b))
     t = float(np.mean(ms)) / 1000.0
-    tr = read_ncu_traffic(kern.split(" ")[0])
     return {"kernel": kern + ", conv3x3 128->128 @200x176 x batch %d" % neck.batch, "bound": "tensor", "achieved": flops / t / 1e12,
             "unit": "TFLOP/s", "peak": peaks["tf_burst"], "peak_source": peaks["source"] + ", bf16 burst (kernel timed alone)",
             "frac": flops / t / 1e12 / peaks["tf_burst"], "avg_launch_ms": t * 1000.0, "algorithmic_flops": flops,
-            "traffic": tr[0] if tr else None, "traffic_unit": "bytes/launch (ncu dram read + write)", "traffic_source": tr[1] if tr else None,
             "tensor_work_factor": 3,
             "timing": "CUDA events on the launch stream, L2 flushed (256 MB memset) before every launch, mean of %d" % reps}
 
@@ -568,7 +551,7 @@ def extra_uniform(args, dev):
 
 
 def extra_stress(args, dev, peaks):
-    """BASELINE configs[4] shape on this GPU: throughput through one batch-16 engine + the per-launch-group roofline fractions of the
+    """BASELINE configs[4] shape on this GPU: throughput through one batch-8 engine + the per-launch-group roofline fractions of the
     kernels north_star names (sparse-conv GEMM: tensor; rulebook / voxelise / dense scatter: HBM), from scripts/kernel_rooflines.py."""
     import kernel_rooflines as kr
     wl = "stress"
@@ -581,7 +564,7 @@ def extra_stress(args, dev, peaks):
     fn = rig.step_host(F)
     rig.timed(fn, 1)
     ms_h = rig.timed(fn, 5)
-    groups = kr.group_rooflines(rig.engines[0], rig.clouds[:16], iters=3)
+    groups = kr.group_rooflines(rig.engines[0], rig.clouds[:rig.B], iters=3)
     keep = [g for g in groups["groups"] if g["group"].startswith(("voxelize", "hash", "rulebook", "conv:", "split", "dense"))]
     tensor = [g for g in keep if g.get("bound") == "tensor" and g.get("impl") not in ("rows",)]
     hbm = [g for g in keep if g.get("bound") == "hbm"]

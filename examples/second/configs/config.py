@@ -1,4 +1,4 @@
-"""SE-SSD car detector on KITTI -- hot-path configuration for the B200 build.
+"""SE-SSD car detector on KITTI -- hot-path configuration for the H100 (sm_90a) build.
 
 Same variable names, registry type strings and hyper-parameters as the reference's examples/second/configs/config.py (which also
 loads unchanged through this repo's ``det3d`` package: tests/test_compat.py does that when the reference tree is present);

@@ -1,5 +1,5 @@
 /*
- * sessd_b200.h -- C ABI of the B200-native SE-SSD per-frame LiDAR hot path
+ * sessd_b200.h -- C ABI of the GPU-native (sm_90a) SE-SSD per-frame LiDAR hot path
  *                 (voxelise -> sparse 3-D conv encoder -> BEV neck/head -> rotated IoU / NMS).
  *
  * Conventions (all entry points):
@@ -28,7 +28,7 @@ extern "C" {
 #define SESSD_ECAPACITY (-2)
 #define SESSD_EWORKSPACE (-3)
 
-/* library / build information: returns e.g. "sessd_b200 0.1 sm_100a" */
+/* library / build information: returns e.g. "sessd_b200 0.1 (sm_90a)" */
 const char *sessd_version(void);
 /* number of kernel launches issued through this library since load (bench.py's gpu_launches claim) */
 long long sessd_launch_count(void);
@@ -149,8 +149,8 @@ int sessd_spconv_forward_rows_planes(const float *d_in_feat, int cin, const int 
                                      const float *d_amax_in, float gain, float shift_max, float *d_out_feat, void *d_out_planes, int cpo,
                                      float *d_out_info, void *stream);
 /* S4, the default tensor-core path of the Cin >= 32 layers (csrc/spconv_cg.cu): pair-proportional operand traffic -- the rows of the
- * neighbours that exist are copied by cp.async into the UMMA operand tiles (no row slot is spent on a missing neighbour), persistent CTAs,
- * tcgen05 kind::f16 with the two-term fp16 split of spconv_h2.cu (same weight tiles: ops.pack_weight_sp_h2).  Same contract as
+ * neighbours that exist are copied by cp.async into the wgmma operand tiles (no row slot is spent on a missing neighbour), persistent CTAs,
+ * fp16 wgmma with a two-term fp16 split of activations and weights (weight tiles: ops.pack_weight_sp_h2).  Same contract as
  * sessd_spconv_forward (spconv 1.x gather -> GEMM -> scatter-add at det3d/models/backbones/scn.py:106-149, + folded BN + ReLU).
  * The rulebook is passed as d_tiles = the per-tile pair lists sessd_rulebook_tile_lists() makes from the nbr table (once per rulebook).
  * d_in_planes [plane_rows][2][cp] fp16, x = (hi + lo) / d_in_info[1], d_in_info[0] = abs-max of the input tensor; outputs (each nullable, at
@@ -159,7 +159,7 @@ int sessd_spconv_forward_rows_planes(const float *d_in_feat, int cin, const int 
 int sessd_spconv_forward_cg(const void *d_in_planes, int cp, int plane_rows, const float *d_in_info, const void *d_tiles, int kvol,
                             const int *d_n_out, int max_out, const void *d_weight_h2, int cout, const float *d_scale, const float *d_shift,
                             int relu, float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, void *stream);
-/* 1: deep pipeline (twice the stages, one CTA per SM) for launches with fewer tiles than SMs (single frames); 0 (default): two CTAs per SM */
+/* 1: deep pipeline (twice the stages) for launches with fewer tiles than SMs (single frames); 0 (default): the shorter ring */
 void sessd_set_sp_cg_deep(int on);
 /* *d_amax = max(*d_amax, max |d_feat[i]|) over the first *d_n rows of a [max_rows, channels] fp32 tensor */
 int sessd_absmax_rows(const float *d_feat, const int *d_n, int max_rows, int channels, float *d_amax, void *stream);
@@ -192,8 +192,9 @@ int sessd_bev_conv(const float *d_in, const float *d_weight /*[ntaps, cin, cout]
  * BEV convs from PRE-SPLIT fp16 planes (csrc/bevconv_p2.cu): the neck's default path.  Activations travel between layers as
  * __half [2 (hi|lo)][batch][H][W][C] planes with x = (hi + lo) / S, S an exact power of two; every plane tensor has a device-side
  * info pair float[2] = {abs-max of the tensor (atomically raised by its producer; zero it once per frame), S}.  Same conv semantics
- * as sessd_bev_conv / sessd_bev_deconv_tc (rpn_v1.py:135-210, mg_head_sessd.py:202-230): in_stride 1 or 2, <= 9 taps, cin % 64 == 0,
- * cout % 8 == 0.  d_weight_h2 / d_scale as for sessd_bev_conv_h2.  gain / shift_max: |out| <= amax_in * gain + shift_max
+ * as sessd_bev_conv (rpn_v1.py:135-210, mg_head_sessd.py:202-230): in_stride 1 or 2, <= 9 taps, cin % 64 == 0,
+ * cout % 8 == 0.  d_weight_h2: __half [2 (hi|lo)][ntaps][cout_pad][cin] of 2^e[n] w
+ * (ops.pack_weight_h2); d_scale = folded BN scale * 2^-e[n].  gain / shift_max: |out| <= amax_in * gain + shift_max
  * (+ amax of the residual) with gain = max_n sum_{tap,c} |w[tap][c][n] * bn_scale[n]|: the producer derives the OUTPUT scale from
  * this bound before it writes the first element.  Outputs: fp32 NHWC (d_out_f32) and / or planes (d_out_planes + d_out_info). */
 int sessd_bev_conv_p2(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
@@ -205,9 +206,6 @@ int sessd_bev_deconv_p2(const void *d_in_planes, const float *d_in_info, const v
                         int relu, void *stream);
 /* fp32 [n] -> planes [2][n] scaled from d_info[0] (the tensor's abs-max, e.g. from sessd_absmax); writes the scale to d_info[1] */
 int sessd_bev_split_planes(const float *d_x, long long n, float *d_info, void *d_planes, void *stream);
-/* sessd_bev_conv_p2 / sessd_bev_deconv_p2: 0 (default) = CTA pairs (tcgen05 cta_group::2: one MMA spans two SMs, each CTA stages half of
- * every weight tile) for the layers with long K loops, single CTAs for the 1x1 convs; 1 / 2 = force single CTAs / pairs */
-void sessd_set_p2_cluster(int ctas_per_cluster);
 /* dense() (scn.py:184-187) straight into the planes the neck reads: d_amax = abs-max of the feature rows, d_info[2] <- {abs-max, S} */
 int sessd_sparse_to_dense_planes(const float *d_feat, int max_rows, const void *d_bitmap_index, int channels, sessd_grid grid,
                                  const float *d_amax, float *d_info, void *d_planes, void *stream);

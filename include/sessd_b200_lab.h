@@ -1,7 +1,7 @@
-/* sessd_b200_lab.h -- C ABI of libsessd_b200_lab.so: the NON-DEFAULT kernel variants and profiling probes kept for
- * cross-implementation tests and measurements (3xTF32 tcgen05 convs with SIMT gather, the TMA-gather4 sparse conv, the in-kernel-split
- * BEV conv, MMA / latency probes, ablation switches).  Nothing in the product path (libsessd_b200.so, sessd_b200.engine) links or
- * loads this library; it links against libsessd_b200.so for the launch counter only.  Same conventions as sessd_b200.h. */
+/* sessd_b200_lab.h -- C ABI of libsessd_b200_lab.so: the NON-DEFAULT BEV conv variants kept for cross-implementation tests
+ * (csrc/bevconv_split.cu): fp32 NHWC input split inside the wgmma kernel, either into 3xTF32 (tf32 wgmma) or into two-term fp16
+ * (fp16 wgmma).  Nothing in the product path (libsessd_b200.so, sessd_b200.engine) links or loads this library.  Same conventions as
+ * sessd_b200.h. */
 #ifndef SESSD_B200_LAB_H
 #define SESSD_B200_LAB_H
 
@@ -11,46 +11,21 @@
 extern "C" {
 #endif
 
-/* Tensor-core variant (tcgen05, 3xTF32) for (Cin, Cout) in {(32,32), (32,64), (64,64)}: d_weight_split is
- * [2 (hi|lo)][kvol][Cout][Cin] (K-major), hi = tf32-truncated weights, lo = w - hi. */
-int sessd_spconv_forward_tc(const float *d_in_feat, int cin, const int *d_nbr, int kvol, const int *d_n_out,
-                            int max_out, const float *d_weight_split, int cout, const float *d_scale,
-                            const float *d_shift, int relu, float *d_out_feat, void *stream);
-
-/* S4 (fp16-split tensor-core path with TMA gather; csrc/spconv_h2.cu).  Same contract as sessd_spconv_forward (spconv 1.x
- * gather -> GEMM -> scatter-add at det3d/models/backbones/scn.py:106-149, + folded BN + ReLU), but the input features are
- * read as fp16 (hi, lo) planes [plane_rows][2][cp] -- x = 2^-s (hi + lo), s chosen from *d_amax_in exactly like
- * sessd_bev_conv_h2 -- produced by sessd_split_h2 from the producing layer's fp32 rows; row `zero_row` of the planes must be
- * all zero (missing neighbours read it).  d_weight_h2: cp = 64: [kvol][2 (hi|lo)][cout][64] fp16, cp = 32:
- * [kvol][cout][hi 32 | lo 32] fp16 (Cin 16 zero-padded), every output channel scaled by a power of two 2^e[c];
- * d_scale[c] must be bn_scale[c] * 2^-e[c].  d_amax_out (nullable) receives the running abs-max of the output.
- * Supported (cp, cout): (32,16) (32,32) (32,64) (64,64). */
-int sessd_spconv_forward_h2(const void *d_in_planes, int cp, int plane_rows, int zero_row, const float *d_amax_in, const int *d_nbr,
-                            int kvol, const int *d_n_out, int max_out, const void *d_weight_h2, int cout, const float *d_scale,
-                            const float *d_shift, int relu, float *d_out_feat, float *d_amax_out, void *stream);
-/* fp32 rows -> the planes sessd_spconv_forward_h2 reads (scale from *d_amax, see sessd_absmax_rows) */
-int sessd_split_h2(const float *d_feat, const int *d_n, int max_rows, int channels, const float *d_amax, void *d_planes, int cp,
-                   void *stream);
-/* pipeline depth of sessd_spconv_forward_h2: 0 / 1 = two CTAs per SM x 2-4 stages (default), 2 = one CTA per SM x 4-8 stages */
-void sessd_set_sp_h2_depth(int mode);
-
-/* Tensor-core variant (tcgen05 + TMEM + TMA, 3xTF32 split for fp32-level accuracy): same contract (in_stride 1 or 2).
+/* 3xTF32 BEV conv (tf32 wgmma, three products per MAC): same contract as sessd_bev_conv (in_stride 1 or 2, cin % 64 == 0, cout % 8 == 0).
  * d_weight_split [2 (hi|lo)][ntaps][cout_pad][cin]: hi = weights truncated to tf32, lo = w - hi; cout_pad is a multiple of the
- * N tile (128; 32 when cout <= 32). */
+ * N tile (128; 32 when cout <= 32).  d_scale nullable (identity). */
 int sessd_bev_conv_tc(const float *d_in, const float *d_weight_split, int cout_pad, const float *d_scale,
                       const float *d_shift, const float *d_residual, float *d_out, const sessd_conv_desc *desc,
                       void *stream);
 
-/* ConvTranspose2d(k3, s2, p1, op1) + BN + ReLU (+ residual) in one launch (four output-parity classes as blockIdx.z);
- * d_weight_split [2][9][cout_pad][cin], tap = ky*3+kx of W[cin][cout][ky][kx]; output [batch, 2*in_h, 2*in_w, cout] NHWC
- * (rpn_v1.py:183-195). */
+/* ConvTranspose2d(k3, s2, p1, op1) + BN + ReLU (+ residual) in one launch; d_weight_split [2][9][cout_pad][cin],
+ * tap = ky*3+kx of W[cin][cout][ky][kx]; output [batch, 2*in_h, 2*in_w, cout] NHWC (rpn_v1.py:183-195). */
 int sessd_bev_deconv_tc(const float *d_in, const float *d_weight_split, int cout_pad, const float *d_scale,
                         const float *d_shift, const float *d_residual, float *d_out, int batch, int in_h, int in_w,
                         int cin, int cout, int relu, void *stream);
 
-/* fp16-split tensor-core variant (tcgen05 kind::f16, A operand in tensor memory, one halo patch per channel chunk): same contract as
- * sessd_bev_conv_tc for in_stride == 1, cin % 64 == 0 and tap lists whose reach fits a 10x18-pixel patch (else SESSD_EINVAL: use
- * sessd_bev_conv_tc).  Every fp32 operand is represented exactly-scaled as fp16 hi + fp16 lo (>= 22 significand bits, same as 3xTF32).
+/* fp16-split BEV conv from fp32 input (the split happens in shared memory): same contract as sessd_bev_conv_tc, in_stride 1 only
+ * (a stride-2 patch and its fp32 staging copy do not fit in shared memory: SESSD_EINVAL).
  * d_weight_h2: __half [2 (hi|lo)][ntaps][cout_pad][cin] of 2^e[n]*w (per output channel n; max |2^e w| in [2^10, 2^11));
  * d_scale (required) = folded BN scale * 2^-e[n].
  * d_amax_in  (nullable): device scalar >= max|in| -- selects the activation scaling 2^s; NULL = no scaling (|in| must stay < 65504).
@@ -61,29 +36,6 @@ int sessd_bev_conv_h2(const float *d_in, const void *d_weight_h2, int cout_pad, 
 int sessd_bev_deconv_h2(const float *d_in, const void *d_weight_h2, int cout_pad, const float *d_scale,
                         const float *d_shift, const float *d_residual, float *d_out, int batch, int in_h, int in_w,
                         int cin, int cout, int relu, const float *d_amax_in, float *d_amax_out, void *stream);
-
-/* profiling experiments only: ablation mask (1 no split work, 2 no MMAs, 4 no weight reloads, 8 no stores; results are garbage when
- * non-zero) and optional [ctas][8] int64 globaltimer stamps (start, split done, accumulators ready, end) */
-void sessd_set_h2_debug(int ablate_mask, void *d_stamps);
-/* tunable of sessd_bev_conv_tc: CTAs per thread-block cluster sharing the weight tiles through TMA multicast (1, 2 or 4) */
-void sessd_set_conv_cluster(int ctas_per_cluster);
-int sessd_get_conv_cluster(void);
-/* 1: A operand staged in shared memory, 2: A operand staged in tensor memory (less smem traffic) */
-void sessd_set_conv_variant(int variant);
-/* profiling experiments only: bit mask of pipeline stages to skip inside bev_conv_tc (results are garbage when non-zero) */
-void sessd_set_conv_ablate(int mask);
-/* profiling aid: sustained tcgen05.mma kind::tf32 rate (M=128, N=n) of one CTA per SM; mode bit0 = A from TMEM, bit1 = two rotating
- * accumulators; d_out[0..2] = issue cycles, cycles to retire, ns */
-int sessd_mma_probe(int n, int iters, int mode, long long *d_out, void *stream);
-/* profiling aid: handshake latencies in cycles (one CTA): d_out[0] tcgen05.commit->mbarrier, [1] two-warp mbarrier round trip,
- * [2] tcgen05.st x32 + wait, [3] / [4] one / four f16 MMAs (M128 N256 K16) + commit -> mbarrier, [5] tcgen05.ld x32 + wait,
- * [6] commit -> other warp -> arrive back round trip */
-/* kind::f16 SS probe: d_out[0] = issue cycles, [1] = cycles until retired for `iters` back-to-back M128 x N x K16 MMAs; mode & 3: 0 / 1 / 2 =
- * one / two / four accumulators in rotation, mode & 4: SWIZZLE_64B operand descriptors */
-int sessd_mma_probe_f16(int n, int iters, int mode, long long *d_out, void *stream);
-int sessd_latency_probe(int iters, long long *d_out, void *stream);
-/* profiling experiments only: device buffer [ctas][8] int64 receiving per-CTA globaltimer stamps of bev_conv_tc (NULL = off) */
-void sessd_set_conv_debug_buffer(void *d_buf);
 
 #ifdef __cplusplus
 }

@@ -1,5 +1,5 @@
-"""Per-kernel achieved rates against the B200 roofline, on BASELINE config #5's shape (dense-scene stress: uniform 200k-point
-clouds, batch 16 per launch, one GPU) and on config #2's shape (ring-20k, batch 1).  SURVEY.md 8(d): batch-1 frames are
+"""Per-kernel achieved rates against the GPU roofline, on BASELINE config #5's shape (dense-scene stress: uniform 200k-point
+clouds, batch 8 per launch, one GPU) and on config #2's shape (ring-20k, batch 1).  SURVEY.md 8(d): batch-1 frames are
 launch/latency-bound, so the roofline fractions of the bandwidth-bound kernels are quoted from the stress shape.
 
 Every launch group of the frame is bracketed by CUDA events on the engine stream (eager launches, median of --iters passes);
@@ -26,8 +26,8 @@ def load_peaks():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    return (float(peaks.get("hbm_gbs", 6650.0)), float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1400.0))),
-            "MEASURED_PEAKS.json (of measured)" if peaks else "B200_PROFILING.md fallback (of fallback)")
+    return (float(peaks.get("hbm_gbs", 3350.0)), float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0))),
+            "MEASURED_PEAKS.json (of measured)" if peaks else "H100 SXM datasheet (HBM3 3.35 TB/s, dense bf16 989 TFLOP/s)")
 
 
 def group_rooflines(eng, clouds, iters=5):
@@ -133,7 +133,7 @@ def main():
     from sessd_b200._lib import lib
     lib.sessd_set_sp_cg_deep(int(a.cg_deep))
     if a.shape == "stress":
-        B, N = a.batch or 16, a.points or 200000
+        B, N = a.batch or 8, a.points or 200000
         clouds = [synth.uniform_cloud(1000 + f, N) for f in range(B)]
         eng = FrameEngine(batch=B, max_points_per_frame=N, max_voxels=200000, growth=(1.0, 8.0, 8.0, 8.0, 8.0), sparse_tc=a.sparse_tc)
         kind = "uniform"

@@ -1,8 +1,8 @@
-"""Build libsessd_b200.so (hand-written CUDA for sm_100a + the C ABI of include/sessd_b200.h) IN-TREE.
+"""Build libsessd_b200.so (hand-written CUDA for sm_90a + the C ABI of include/sessd_b200.h) IN-TREE.
 
     python se-ssd_b200/build.py [--force]
 
-nvcc cross-compiles here without a GPU; the resulting .so is git-ignored but travels to the GPU box with gpurun.
+nvcc cross-compiles without a GPU; the resulting .so and the objects under build/ are git-ignored.
 Files that implement the rotated-box geometry are compiled with -fmad=false so that their fp32 arithmetic rounds
 like the CPU twin of the reference (see csrc/rotbox.cuh).
 """
@@ -15,10 +15,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libsessd_b200.so")
 LAB_OUT = os.path.join(HERE, "libsessd_b200_lab.so")
-# non-default kernel variants + probes (include/sessd_b200_lab.h): built into their own library, never loaded by the product path
-LAB = {"mma_probe.cu", "bevconv_tc.cu", "bevconv_h2.cu", "spconv_tc.cu", "spconv_h2.cu"}
+# non-default operand formats (include/sessd_b200_lab.h): built into their own library, never loaded by the product path
+LAB = {"bevconv_split.cu"}
 OBJ = os.path.join(HERE, "build")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"] + os.environ.get("SESSD_DEFINES", "").split()
 NO_FMA = {"iou3d.cu", "postproc.cu", "assign.cu", "odiou.cu"}
 

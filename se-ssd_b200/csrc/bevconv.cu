@@ -12,7 +12,7 @@
 //     zero-stuffed input that a naive "conv over the upsampled grid" would spend 75 % of its MACs on).
 // GEMM view: M = B*grid_h*grid_w pixels, N = Cout, K = ntaps*Cin.  CTA tile 128x128, BK = 16, 256 threads with 8x8
 // register micro-tiles, A rows gathered with zero-filling cp.async (3-stage pipeline), fp32 FMA accumulation.
-// This SIMT version is the fp32 numerics baseline; the tcgen05 (3xTF32) version shares this interface.
+// This SIMT version is the fp32 numerics baseline; the tensor-core versions read pre-split fp16 planes (bevconv_p2.cu).
 // Algorithmic bytes per layer: 4 (M Cin [read once per CTA column] + M Cout) ; FLOPs 2 M N K.
 #include <cuda_fp16.h>
 
@@ -236,7 +236,7 @@ extern "C" int sessd_absmax(const float *d_x, long long n, float *d_amax, void *
     if (!d_x || !d_amax || n < 0 || ((uintptr_t)d_x & 15)) return SESSD_EINVAL;
     if (n == 0) return 0;
     const long long n4 = n / 4;
-    const int blocks = (int)max(1LL, min((long long)148 * 8, (n4 + 255) / 256));
+    const int blocks = (int)max(1LL, min((long long)kNumSMs * 8, (n4 + 255) / 256));
     absmax_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float4 *>(d_x), n4, d_x + n4 * 4, (int)(n - n4 * 4), d_amax);
     ++g_launches;
     return last_error();

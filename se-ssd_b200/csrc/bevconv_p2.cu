@@ -1,489 +1,7 @@
-// bevconv_p2.cu -- BEV conv / deconv (+BN+ReLU+residual) on the 5th-gen tensor cores from PRE-SPLIT fp16 planes.
-//
-// Replaces the cuDNN conv blocks of det3d/models/necks/rpn_v1.py:135-210 and the 1x1 head convs of
-// det3d/models/bbox_heads/mg_head_sessd.py:202-230 (fp32 in, fp32 out, fp32 accumulate).  Same numerics as the lab library's bevconv_h2.cu
-// (x = (x_hi + x_lo) / S with fp16 hi / lo and an exact power-of-two scale S: 22+ significand bits; three kind::f16 products per MAC
-// accumulated in fp32 TMEM: a_hi*b_hi -> main0 / main1 alternating, a_hi*b_lo + a_lo*b_hi -> cross, summed in RN fp32 by the epilogue),
-// but the activations TRAVEL BETWEEN LAYERS as fp16 (hi, lo) planes [2][B*H*W][C] written by the producing layer's epilogue, so that
-//   * the main loop is pure TMA -> shared memory -> tcgen05.mma (SS form): no split warps, no in-kernel fp32 -> fp16 conversion, no
-//     tensor-memory A slots, no per-tap handshake between SIMT warps and the MMA issuer (the h2 kernel's tensor pipe was active 34 %
-//     of the time at batch 1 because its two-stage split -> TMEM -> MMA chain exposed every handshake latency);
-//   * the scale of an OUTPUT tensor has to be known before its first element is written: S_out comes from a rigorous bound
-//     |out| <= amax_in * G + max|shift| (+ amax_residual), G = max_n sum_k |w[k][n]| |bn_scale[n]| (host, at weight-load time) and
-//     amax_in = the measured abs-max of the input (device scalar, raised by the producer's epilogue).  The bound maps into
-//     [2^14, 2^15): fp16 keeps 22 bits of every element down to 2^-17 of the bound, far more slack than the bound is loose;
-//   * the weight tiles ([b_hi ; b_lo], 16 KB per (tap, 32-channel chunk)) are the dominant L2 -> SM traffic (589 KB per 128-pixel tile of
-//     a 3x3 128->128 layer against ~23 B/clk/SM the L2 delivers).  TMA multicast across a cluster of two did not help (every SM still
-//     receives every byte); CTA PAIRS do: with tcgen05 cta_group::2 ONE MMA spans two SMs (M = 256: 128 pixels per CTA) and each CTA stages
-//     only HALF of every weight tile (the N halves are concatenated by the instruction); all loads signal the leader's mbarriers
-//     (cp.async.bulk.tensor...cta_group::2), the leader's commits arrive in both CTAs.  Used where the K loop is long (3x3, stride-2, deconv);
-//     the 1x1 convs stay single-CTA;
-//   * the three loops (patch TMA, weight TMA, MMA issue) run warp-uniform with one ELECTED issuing lane, so descriptors and addresses stay
-//     in uniform registers (an `if (lane == 0)` around the loop made the issue thread, not the tensor pipe, the bottleneck).
-// Geometry: tile = 8 (u) x 16 (v) output pixels = 128 MMA rows, row = v*8 + u, so that one 8-row swizzle group = 8 consecutive u.
-// For every distinct tap shift along u (and v parity, strided convs) ONE copy of the input patch [v rows][8 u][32 channels] is
-// TMA-loaded per plane: a tap then addresses a canonical K-major SWIZZLE_64B operand at copy + v_shift * 512 B (group stride 512 B):
-// plain descriptors, no base-offset tricks.  u / v are mapped to (y, x) or (x, y), whichever tiles the map with fewer tiles.
-// Warps: 0 patch TMA, 1 weight TMA, 2 MMA issue (pair mode: the leader CTA's only), 3-10 epilogue (TMEM -> registers -> BN/ReLU/residual -> fp32 and / or
-// fp16 planes + running abs-max).
-#include <cuda_fp16.h>
-
-#include "tc_common.cuh"
+// bevconv_p2.cu -- C ABI of the BEV conv / deconv from pre-split fp16 planes (kernel and launcher: bevconv_p2.cuh).
+#include "bevconv_p2.cuh"
 
 namespace sessd {
-
-constexpr int kP2TileU = 8, kP2TileV = 16, kP2BM = 128;
-constexpr int kP2Chunk = 32;                              // channels per stage = one 64-byte SWIZZLE_64B row
-constexpr int kP2MaxCopies = 6, kP2MaxRowsV = 18;
-constexpr int kP2BStages = 6, kP2MaxBStages = 12;
-constexpr int kP2BStageBytes = 2 * 128 * 64;              // [X ; Y] planes, up to 128 rows of 64 B each
-constexpr int kP2BRing = kP2BStages * kP2BStageBytes;     // bytes of the weight-stage ring (pair mode: twice as many stages of half the size)
-constexpr int kP2Threads = 352;                           // 11 warps
-constexpr int kP2EpiWarps = 8;
-constexpr int kP2MaxSmem = 227 * 1024;
-
-struct P2Params {
-    int batch, cin, cout;
-    int in_stride;                     // 1 or 2 (input position = output position * in_stride + tap offset)
-    int out_h, out_w;                  // output tensor extent (pixels)
-    int grid_u, grid_v;                // output positions computed per class along u / v
-    int u_is_x;                        // 1: u = x, v = y;  0: u = y, v = x
-    int out_stride, nclass;
-    int cls_ntaps[4], cls_off_u[4], cls_off_v[4];
-    int tap_copy[4][9], tap_row[4][9], tap_w[4][9];      // per (class, tap): patch copy, first v row inside the copy, weight tap
-    int ncopies, rows_v;
-    int copy_u[kP2MaxCopies], copy_v[kP2MaxCopies];       // input coordinate of the copy's first element relative to (u0, v0) * in_stride
-    int copy_bytes, patch_bytes, npatch;                  // bytes of one copy plane, of one patch buffer (ncopies x 2 planes), 1 or 2 buffers
-    int relu, n_tile, nblocks;
-    int bstages, bstage_bytes;         // weight-stage ring: count and bytes per stage
-    int tiles_u, tiles_v, tiles, tgroups, total;          // pixel tiles, tile groups (CS tiles each), work items = nclass * nblocks * tgroups
-    int cls_order[4];
-    const float *in_info;              // [2] = {abs-max of the input tensor, scale S_in of its planes}
-    const float *resid_info;           // nullable [2]
-    float gain, shift_max;             // bound of the output: amax_in * gain + shift_max (+ amax_resid)
-    float *out_info;                   // [2] = {running abs-max of the output (atomicMax), S_out}
-    long long out_plane_stride;        // elements between the hi and the lo plane of the output
-    long long *dbg;                    // SESSD_P2_PROFILE only
-};
-
-__host__ __device__ constexpr uint32_t p2_idesc_f16(int M, int N) {
-    return (1u << 4) /*C=F32*/ | (0u << 7) /*A=F16*/ | (0u << 10) /*B=F16*/ | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__device__ __forceinline__ void p2_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-__device__ __forceinline__ void tma_load_5d(uint32_t smem_dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2, int c3, int c4) {
-    asm volatile(
-        "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];\n" ::"r"(smem_dst),
-        "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-        : "memory");
-}
-
-struct P2Item { int cls, n0, b, u0, v0, ntaps; };
-
-// -DSESSD_P2_PROFILE: per-CTA cycle counters of the waits of every role ([ctas][8] int64 via sessd_set_p2_dbg; lab measurements only)
-#ifdef SESSD_P2_PROFILE
-#define P2_WAIT(slot, stmt)                                                                              \
-    do {                                                                                                 \
-        const long long _t0 = clock64();                                                                 \
-        stmt;                                                                                            \
-        p2_acc[slot] += clock64() - _t0;                                                                 \
-    } while (0)
-#else
-#define P2_WAIT(slot, stmt) stmt
-#endif
-template <int CS>
-__device__ __forceinline__ P2Item p2_decode(const P2Params &p, int g, int crank) {
-    P2Item it;
-    const int per_cls = p.nblocks * p.tgroups;
-    const int cr = g / per_cls;
-    int rem = g - cr * per_cls;
-    const int nb = rem / p.tgroups;
-    int t = (rem - nb * p.tgroups) * CS + crank;              // padded tiles (t >= tiles) decode to b >= batch: loads zero-fill, stores are masked
-    it.cls = p.cls_order[cr];
-    it.n0 = nb * p.n_tile;
-    const int tu = t % p.tiles_u; t /= p.tiles_u;
-    const int tv = t % p.tiles_v;
-    it.b = t / p.tiles_v;
-    it.u0 = tu * kP2TileU; it.v0 = tv * kP2TileV;
-    it.ntaps = p.cls_ntaps[it.cls];
-    return it;
-}
-
-__device__ __forceinline__ void p2_tmem_ld16(uint32_t taddr, uint32_t *r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-
-template <int CS>
-__global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid_constant__ CUtensorMap map_a,
-                                                                   const __grid_constant__ CUtensorMap map_b,
-                                                                   const float *__restrict__ scale, const float *__restrict__ shift,
-                                                                   const float *__restrict__ resid, float *__restrict__ out_f32,
-                                                                   __half *__restrict__ out_planes, P2Params p) {
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char *tiles = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    unsigned char *patches = tiles + kP2BRing;
-    uint64_t *bars = (uint64_t *)(patches + p.npatch * p.patch_bytes);
-    uint64_t *patch_full = bars, *patch_empty = bars + 2, *b_full = bars + 4, *b_empty = bars + 4 + kP2MaxBStages;
-    uint64_t *acc_full = bars + 4 + 2 * kP2MaxBStages, *acc_free = acc_full + 1;
-    uint32_t *tmem_slot = (uint32_t *)(acc_free + 1);
-    uint32_t *s_aoff = tmem_slot + 2;                    // [4 classes][9 taps]
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) prefetch_tensormap(&map_a);    // descriptor fetches overlap barrier init / TMEM allocation / cluster syncs
-    if (threadIdx.x == 32) prefetch_tensormap(&map_b);
-#ifdef SESSD_P2_PROFILE
-    long long p2_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};      // per-thread wait counters, written once at the end
-    const long long p2_t0 = clock64();                   // timeline (second [ctas][8] block of dbg): 0 setup done, 1 MMA loop start, 2 MMA loop end,
-    long long p2_tl[8] = {0, 0, 0, 0, 0, 0, 0, 0};       // 3 first acc_full seen, 4 last epilogue done, 5 teardown done (clk since kernel entry)
-#endif
-    const uint32_t crank = (CS > 1) ? cluster_cta_rank() : 0u;
-    constexpr bool kPair = (CS == 2);
-    const int cluster_id = blockIdx.x / CS, nclusters = gridDim.x / CS;
-    const int nchunks = p.cin / kP2Chunk;
-    const uint32_t b_plane_bytes = (uint32_t)(p.n_tile / CS) * 64u;      // bytes of the b_hi (or b_lo) rows THIS CTA stages per (tap, chunk)
-
-    if (threadIdx.x == 0) {
-        // pair mode: the leader's "full" barriers collect one arrival per CTA (the leader's carries the byte count of BOTH CTAs' loads)
-        for (int s = 0; s < 2; ++s) { mbar_init(&patch_full[s], CS); mbar_init(&patch_empty[s], 1); }
-        for (int s = 0; s < p.bstages; ++s) { mbar_init(&b_full[s], CS); mbar_init(&b_empty[s], 1); }
-        mbar_init(acc_full, 1);
-        mbar_init(acc_free, kP2EpiWarps * CS);
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    }
-    if (kPair) cluster_sync_all();         // both CTAs are resident before the pair-wide TMEM allocation
-    if (warp == 2) {
-        if (kPair) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (kPair) cluster_sync_all();         // the peer's barriers are initialised before any remote arrive / peer-signalling load
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-#ifdef SESSD_P2_PROFILE
-    p2_tl[0] = clock64() - p2_t0;
-#endif
-
-    // Roles 0-2 run their loops with the WHOLE warp (warp-uniform trip counts and addresses stay in uniform registers) and issue the
-    // TMA / tcgen05 instructions from one elected lane.  Wrapping the loops in `if (lane == 0)` instead made every operand a vector
-    // register that has to be moved to the uniform file (R2UR) behind a divergence guard: ~890 clk per tap for 384 clk of MMA work --
-    // the issue thread, not the tensor pipe or the L2, bounded the first version (MMA thread busy 64 k of 73 k clk, waiting 8 k).
-    if (warp == 0) {
-        // ===================== activation patches: per (item, 32-channel chunk) ncopies x (hi, lo) boxes =====================
-        int pb = 0;
-        uint32_t pph = 0;
-        const uint32_t patches_u32 = smem_u32(patches);
-        for (int g = cluster_id; g < p.total; g += nclusters) {
-            const P2Item it = p2_decode<CS>(p, g, (int)crank);
-            const int bu = it.u0 * p.in_stride, bv = it.v0 * p.in_stride;
-            for (int cc = 0; cc < nchunks; ++cc) {
-                P2_WAIT(7, mbar_wait(&patch_empty[pb], pph ^ 1u));
-                if (elect_one()) {
-                    if (!kPair || crank == 0) mbar_expect_tx(&patch_full[pb], (uint32_t)(CS * p.patch_bytes));
-                    else mbar_arrive_remote(&patch_full[pb], 0);
-                    uint32_t dst = patches_u32 + (uint32_t)(pb * p.patch_bytes);
-                    for (int c = 0; c < p.ncopies; ++c, dst += 2u * (uint32_t)p.copy_bytes) {
-                        const int cu = bu + p.copy_u[c], cv = bv + p.copy_v[c];
-                        if (kPair) {
-                            tma_load_5d_pair(dst, &map_a, &patch_full[pb], cc * kP2Chunk, cu, cv, it.b, 0);
-                            tma_load_5d_pair(dst + (uint32_t)p.copy_bytes, &map_a, &patch_full[pb], cc * kP2Chunk, cu, cv, it.b, 1);
-                        } else {
-                            tma_load_5d(dst, &map_a, &patch_full[pb], cc * kP2Chunk, cu, cv, it.b, 0);
-                            tma_load_5d(dst + (uint32_t)p.copy_bytes, &map_a, &patch_full[pb], cc * kP2Chunk, cu, cv, it.b, 1);
-                        }
-                    }
-                }
-                __syncwarp();
-                if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== weight tiles: one stage per (item, chunk, tap) =====================
-        // single CTA: [b_hi ; b_lo] (128 + 128 rows) on even stages, [b_lo ; b_hi] on odd stages (every item has an even stage count);
-        // pair: this CTA's half of the output channels, always [b_hi half ; b_lo half] (64 + 64 rows)
-        int S = 0;
-        uint32_t bph = 0, par = 0;
-        const int rows = p.n_tile / CS;
-        for (int g = cluster_id; g < p.total; g += nclusters) {
-            const P2Item it = p2_decode<CS>(p, g, (int)crank);
-            const int n0 = it.n0 + (kPair ? (int)crank * rows : 0);
-            for (int cc = 0; cc < nchunks; ++cc)
-                for (int tap = 0; tap < it.ntaps; ++tap) {
-                    P2_WAIT(6, mbar_wait(&b_empty[S], bph ^ 1u));
-                    if (elect_one()) {
-                        unsigned char *st = tiles + S * p.bstage_bytes;
-                        const int wtap = p.tap_w[it.cls][tap];
-                        if (kPair) {
-                            if (crank == 0) mbar_expect_tx(&b_full[S], 4 * b_plane_bytes);
-                            else mbar_arrive_remote(&b_full[S], 0);
-                            tma_load_4d_pair(smem_u32(st), &map_b, &b_full[S], cc * kP2Chunk, n0, wtap, 0);
-                            tma_load_4d_pair(smem_u32(st) + b_plane_bytes, &map_b, &b_full[S], cc * kP2Chunk, n0, wtap, 1);
-                        } else {
-                            mbar_expect_tx(&b_full[S], 2 * b_plane_bytes);
-                            const uint32_t hi_off = par ? b_plane_bytes : 0u, lo_off = par ? 0u : b_plane_bytes;
-                            tma_load_4d(st + hi_off, &map_b, &b_full[S], cc * kP2Chunk, n0, wtap, 0);
-                            tma_load_4d(st + lo_off, &map_b, &b_full[S], cc * kP2Chunk, n0, wtap, 1);
-                        }
-                    }
-                    __syncwarp();
-                    par ^= 1u;
-                    if (++S == p.bstages) { S = 0; bph ^= 1u; }
-                }
-        }
-    } else if (warp == 2 && (!kPair || crank == 0)) {
-        // ===================== MMA issue (one elected lane; the warp walks the loops together; pair mode: the leader CTA only) =========
-        const uint32_t idesc1 = p2_idesc_f16(kP2BM * CS, p.n_tile), idesc2 = p2_idesc_f16(kP2BM * CS, 2 * p.n_tile);
-        const uint32_t acc_main0 = tmem_base, acc_cross = tmem_base + (uint32_t)p.n_tile, acc_main1 = tmem_base + 2 * (uint32_t)p.n_tile;
-        const uint64_t desc_hi = ((uint64_t)((512u >> 4) | (1u << 14) | (4u << 29))) << 32;      // SBO 512 B | version 1 | SWIZZLE_64B
-        const uint32_t lbo = 1u << 16;
-        const uint32_t tiles_lo = ((smem_u32(tiles) >> 4) & 0x3FFFu) | lbo;
-        const uint32_t patch_lo = ((smem_u32(patches) >> 4) & 0x3FFFu) | lbo;
-        const uint32_t plane_lo = b_plane_bytes >> 4;
-        const uint32_t copy_lo = (uint32_t)(p.copy_bytes >> 4), patch_sz = (uint32_t)(p.patch_bytes >> 4);
-        // operand offset of every (class, tap) inside a patch buffer, in 16-byte units
-        for (int idx = lane; idx < p.nclass * 9; idx += 32) {
-            const int c = idx / 9, t = idx - c * 9;
-            s_aoff[idx] = (uint32_t)((2 * p.tap_copy[c][t] * p.copy_bytes + p.tap_row[c][t] * 512) >> 4);
-        }
-        __syncwarp();
-        int S = 0, pb = 0, iter = 0;
-        uint32_t bph = 0, pph = 0, par = 0;
-        const int per_cls = p.nblocks * p.tgroups;
-#ifdef SESSD_P2_PROFILE
-        const long long t_begin = clock64();
-        p2_tl[1] = t_begin - p2_t0;
-#endif
-        for (int g = cluster_id; g < p.total; g += nclusters, ++iter) {
-            const int cls = p.cls_order[g / per_cls];
-            const int ntaps = p.cls_ntaps[cls];
-            const int nbj = nchunks * ntaps;
-            const uint32_t *aoff = s_aoff + cls * 9;
-            if (iter > 0) P2_WAIT(0, mbar_wait(acc_free, (uint32_t)(iter - 1) & 1u));   // the epilogue warps drained the previous item's accumulators
-            int lbj = 0;
-            for (int cc = 0; cc < nchunks; ++cc) {
-                P2_WAIT(1, mbar_wait(&patch_full[pb], pph));
-                const uint32_t pbase = patch_lo + (uint32_t)pb * patch_sz;
-#pragma unroll 1
-                for (int tap = 0; tap < ntaps; ++tap, ++lbj) {
-                    P2_WAIT(2, mbar_wait(&b_full[S], bph));
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint64_t da_hi = desc_hi | (uint64_t)(pbase + aoff[tap]);
-                        const uint64_t da_lo = da_hi + (uint64_t)copy_lo;
-                        const uint64_t dcat = desc_hi | (uint64_t)(tiles_lo + (uint32_t)(S * (p.bstage_bytes >> 4)));
-                        const uint64_t dbhi = dcat + (par ? plane_lo : 0u);
-                        const uint32_t d2 = par ? acc_cross : acc_main0;            // even stages: [main0|cross], odd stages: [cross|main1]
-                        if constexpr (kPair) {
-                            // TMEM columns (per CTA: its 128 pixels x all columns), h = n_tile / 2:
-                            //   [0, 2 n_tile)  = [main0 c<h | cross c<h | main0 c>=h | cross c>=h]: even taps, ONE N = 2 n_tile product
-                            //                    a_hi x [b_hi half ; b_lo half] (the two CTAs' halves are concatenated along N)
-                            //   [2 n_tile, 3 n_tile) = main1: odd taps, a_hi x b_hi  (two main accumulators halve the length of the truncating
-                            //                    accumulation chains, like the single-CTA path)
-                            //   [3 n_tile, 4 n_tile) = cross2: a_lo x b_hi (every tap) and a_hi x b_lo (odd taps)
-                            const uint32_t acc_m1 = tmem_base + 2 * (uint32_t)p.n_tile, acc_c2 = tmem_base + 3 * (uint32_t)p.n_tile;
-                            const uint64_t dblo = dcat + (uint64_t)plane_lo;
-                            // all K steps of one product before the next product (see the single-CTA path below)
-                            if (!par) {
-                                tc_mma_f16_pair(tmem_base, da_hi, dcat, idesc2, lbj != 0);
-                                tc_mma_f16_pair(tmem_base, da_hi + 2, dcat + 2, idesc2, 1);
-                            } else {
-                                tc_mma_f16_pair(acc_m1, da_hi, dcat, idesc1, lbj != 1);
-                                tc_mma_f16_pair(acc_m1, da_hi + 2, dcat + 2, idesc1, 1);
-                                tc_mma_f16_pair(acc_c2, da_hi, dblo, idesc1, 1);
-                                tc_mma_f16_pair(acc_c2, da_hi + 2, dblo + 2, idesc1, 1);
-                            }
-                            tc_mma_f16_pair(acc_c2, da_lo, dcat, idesc1, lbj != 0);
-                            tc_mma_f16_pair(acc_c2, da_lo + 2, dcat + 2, idesc1, 1);
-                            tc_commit_pair(&b_empty[S]);
-                            if (tap == ntaps - 1) tc_commit_pair(&patch_empty[pb]);
-                            if (lbj == nbj - 1) tc_commit_pair(acc_full);
-                        } else {
-                        // K = 16 per instruction = 32 bytes of the 64-byte row.  Both K steps of one product are issued before the next product:
-                        // consecutive MMAs of one shape into one accumulator pipeline, a switch to a product whose accumulator columns overlap the
-                        // previous one's drains the pipe
-                        if (lbj == 1) {
-                            p2_mma_f16(acc_main1, da_hi, dbhi, idesc1, 0);                // main1  = a_hi x b_hi (first write)
-                            p2_mma_f16(acc_cross, da_hi, dcat, idesc1, 1);                // cross += a_hi x b_lo
-                        } else {
-                            p2_mma_f16(d2, da_hi, dcat, idesc2, lbj != 0);                // [main|cross] (+)= a_hi x [b_hi;b_lo]
-                        }
-                        p2_mma_f16(d2, da_hi + 2, dcat + 2, idesc2, 1);
-                        p2_mma_f16(acc_cross, da_lo, dbhi, idesc1, 1);                    // cross += a_lo x b_hi
-                        p2_mma_f16(acc_cross, da_lo + 2, dbhi + 2, idesc1, 1);
-                        tc_commit(&b_empty[S]);
-                        if (tap == ntaps - 1) tc_commit(&patch_empty[pb]);
-                        if (lbj == nbj - 1) tc_commit(acc_full);
-                        }
-                    }
-                    __syncwarp();
-                    par ^= 1u;
-                    if (++S == p.bstages) { S = 0; bph ^= 1u; }
-                }
-                if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
-            }
-        }
-#ifdef SESSD_P2_PROFILE
-        p2_acc[3] = clock64() - t_begin; p2_acc[4] = iter; p2_tl[2] = clock64() - p2_t0;
-#endif
-    } else if (warp >= 3) {
-        // ===================== epilogue warps (3-10): TMEM -> registers, release the accumulators, BN / ReLU / residual / stores
-        const int q = warp & 3;                          // TMEM lane quadrant this warp may access
-        const int half = (warp - 3) >> 2;                // warps 3-6: first half of the N tile's columns, 7-10: second half
-        const int r = q * 32 + lane;
-        const int lv = r / kP2TileU, lu = r % kP2TileU;
-        const int ncol = p.n_tile >> 1;                  // 64 (n_tile 128) or 16 (n_tile 32)
-        const float amax_in = __ldg(p.in_info), s_in = __ldg(p.in_info + 1);
-        const float inv_sa = 1.f / s_in;                 // exact: power of two
-        float bound = amax_in * p.gain + p.shift_max;
-        if (p.resid_info) bound += __ldg(p.resid_info);
-        const float s_out = pow2_scale_for_bound(bound);
-        if (blockIdx.x == 0 && warp == 3 && lane == 0 && p.out_info) p.out_info[1] = s_out;
-        float vmax = 0.f;
-        const bool wide = (p.cout & 15) == 0 && (p.out_plane_stride & 15) == 0;     // plane rows are 32-byte aligned per 16-channel group
-        int iter = 0;
-        for (int g = cluster_id; g < p.total; g += nclusters, ++iter) {
-            const P2Item it = p2_decode<CS>(p, g, (int)crank);
-            float v[64];
-            if (lane == 0) { if (warp == 3) P2_WAIT(5, mbar_wait(acc_full, (uint32_t)iter & 1u)); else mbar_wait(acc_full, (uint32_t)iter & 1u); }
-            __syncwarp();
-            tc_fence_after();
-#ifdef SESSD_P2_PROFILE
-            if (iter == 0) p2_tl[3] = clock64() - p2_t0;
-#endif
-            // single CTA: [main0 | cross | main1], n_tile columns each; pair: [main c<h | cross c<h | main c>=h | cross c>=h | cross2], h = ncol
-            const uint32_t lane0 = tmem_base + ((uint32_t)(q * 32) << 16);
-            const uint32_t lane_base = lane0 + (uint32_t)(kPair ? half * 2 * ncol : half * ncol);
-            const uint32_t off_cr = (uint32_t)(kPair ? ncol : p.n_tile);
-            const uint32_t base_m1 = kPair ? lane0 + 2 * (uint32_t)p.n_tile + (uint32_t)(half * ncol) : lane_base + 2 * (uint32_t)p.n_tile;
-            const uint32_t base_c2 = lane0 + 3 * (uint32_t)p.n_tile + (uint32_t)(half * ncol);       // pair mode only
-#pragma unroll
-            for (int c0 = 0; c0 < 64; c0 += 16) {
-                if (c0 < ncol) {
-                    uint32_t m0[16], cr[16], m1[16];
-                    p2_tmem_ld16(lane_base + c0, m0);
-                    p2_tmem_ld16(lane_base + off_cr + c0, cr);
-                    p2_tmem_ld16(base_m1 + c0, m1);
-                    uint32_t c2[16];
-                    if (kPair) p2_tmem_ld16(base_c2 + c0, c2);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        if (kPair) v[c0 + i] = (__uint_as_float(m0[i]) + __uint_as_float(m1[i])) + (__uint_as_float(cr[i]) + __uint_as_float(c2[i]));
-                        else v[c0 + i] = (__uint_as_float(m0[i]) + __uint_as_float(cr[i])) + __uint_as_float(m1[i]);
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {                             // the next item's MMAs may overwrite the accumulators now
-                if (kPair && crank != 0) mbar_arrive_remote(acc_free, 0);
-                else mbar_arrive(acc_free);
-            }
-            const int gu = it.u0 + lu, gv = it.v0 + lv;
-            if (it.b < p.batch && gu < p.grid_u && gv < p.grid_v) {
-                const int ou = gu * p.out_stride + p.cls_off_u[it.cls], ov = gv * p.out_stride + p.cls_off_v[it.cls];
-                const int oy = p.u_is_x ? ov : ou, ox = p.u_is_x ? ou : ov;
-                const size_t opix = ((size_t)it.b * p.out_h + (size_t)oy) * p.out_w + (size_t)ox;
-                uint32_t hprev[4] = {0u, 0u, 0u, 0u}, lprev[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-                for (int i = 0; i < 64; i += 8) {
-                    const int n = it.n0 + half * ncol + i;
-                    if (i < ncol && n < p.cout) {
-                        float o[8];
-#pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            const float4 sc = *reinterpret_cast<const float4 *>(scale + n + 4 * h);
-                            float4 sh = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (shift) sh = *reinterpret_cast<const float4 *>(shift + n + 4 * h);
-                            o[4 * h + 0] = fmaf(v[i + 4 * h + 0] * inv_sa, sc.x, sh.x); o[4 * h + 1] = fmaf(v[i + 4 * h + 1] * inv_sa, sc.y, sh.y);
-                            o[4 * h + 2] = fmaf(v[i + 4 * h + 2] * inv_sa, sc.z, sh.z); o[4 * h + 3] = fmaf(v[i + 4 * h + 3] * inv_sa, sc.w, sh.w);
-                        }
-                        const size_t off = opix * p.cout + n;
-                        if (p.relu) {
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) o[j] = fmaxf(o[j], 0.f);
-                        }
-                        if (resid) {
-                            float rr[8];
-                            ldg256(resid + off, rr);
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) o[j] += rr[j];
-                        }
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) vmax = fmaxf(vmax, fabsf(o[j]));
-                        if (out_f32) stg256(out_f32 + off, reinterpret_cast<const uint32_t *>(o), reinterpret_cast<const uint32_t *>(o) + 4);
-                        if (out_planes) {
-                            __align__(16) __half2 hi[4], lo[4];
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const float x0 = o[2 * j] * s_out, x1 = o[2 * j + 1] * s_out;
-                                hi[j] = __floats2half2_rn(x0, x1);
-                                const float2 f = __half22float2(hi[j]);
-                                lo[j] = __floats2half2_rn(x0 - f.x, x1 - f.y);
-                            }
-                            if (!wide) {
-                                *reinterpret_cast<uint4 *>(out_planes + off) = *reinterpret_cast<const uint4 *>(hi);
-                                *reinterpret_cast<uint4 *>(out_planes + p.out_plane_stride + off) = *reinterpret_cast<const uint4 *>(lo);
-                            } else if ((i & 8) == 0) {       // first half of a 16-channel group: keep it for the 32-byte store
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) { hprev[j] = *reinterpret_cast<const uint32_t *>(&hi[j]); lprev[j] = *reinterpret_cast<const uint32_t *>(&lo[j]); }
-                            } else {
-                                stg256(out_planes + off - 8, hprev, reinterpret_cast<const uint32_t *>(hi));
-                                stg256(out_planes + p.out_plane_stride + off - 8, lprev, reinterpret_cast<const uint32_t *>(lo));
-                            }
-                        }
-                    }
-                }
-            }
-        }
-#ifdef SESSD_P2_PROFILE
-        p2_tl[4] = clock64() - p2_t0;
-#endif
-        if (p.out_info) {
-            const unsigned m = __reduce_max_sync(0xFFFFFFFFu, __float_as_uint(vmax));     // non-negative floats order like their bits
-            if (lane == 0 && m != 0u) atomicMax(reinterpret_cast<unsigned *>(p.out_info), m);
-        }
-    }
-#ifdef SESSD_P2_PROFILE
-    if (p.dbg && lane == 0 && warp <= 3) {
-        long long *d = p.dbg + (size_t)blockIdx.x * 8;
-        if (warp == 0) d[7] = p2_acc[7];
-        if (warp == 1) d[6] = p2_acc[6];
-        if (warp == 2) { d[0] = p2_acc[0]; d[1] = p2_acc[1]; d[2] = p2_acc[2]; d[3] = p2_acc[3]; d[4] = p2_acc[4]; }
-        if (warp == 3) d[5] = p2_acc[5];
-        long long *tl = p.dbg + (size_t)gridDim.x * 8 + (size_t)blockIdx.x * 8;
-        if (warp == 0) tl[0] = p2_tl[0];
-        if (warp == 2) { tl[1] = p2_tl[1]; tl[2] = p2_tl[2]; }
-        if (warp == 3) { tl[3] = p2_tl[3]; tl[4] = p2_tl[4]; tl[6] = clock64() - p2_t0; }
-    }
-#endif
-    tc_fence_before();
-    __syncthreads();
-    if (kPair) cluster_sync_all();         // nobody exits while the peer may still arrive on / load for this CTA
-    if (warp == 2) {
-        if (kPair) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "r"(512) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "r"(512) : "memory");
-    }
-}
 
 // fp32 rows [rows][C] -> fp16 (hi, lo) planes [2][rows][C] with the scale taken from info[0] (exact abs-max of the tensor); writes info[1]
 __global__ void __launch_bounds__(256) bev_split_planes_kernel(const float4 *__restrict__ x, long long n4, float *__restrict__ info,
@@ -504,167 +22,9 @@ __global__ void __launch_bounds__(256) bev_split_planes_kernel(const float4 *__r
     }
 }
 
-static int encode_map_nd(CUtensorMap *m, const void *base, int rank, const cuuint64_t *dims, const cuuint64_t *strides_bytes /*rank-1*/,
-                         const cuuint32_t *box, const cuuint32_t *estr, CUtensorMapSwizzle swz) {
-    EncodeTiledFn enc = get_tensor_map_encoder();
-    if (!enc) return SESSD_EINVAL;
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void *>(base), dims, strides_bytes, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS ? 0 : 700 + (int)r;
-}
-
-static long long *g_p2_dbg = nullptr;
-static int g_p2_cluster = 0;      // 0: CTA pairs (cta_group::2) for the layers with long K loops, single CTAs for the rest; 1 / 2: force
-
-// taps: per class (dy, dx, weight tap); fills the geometry of p and launches
-struct P2Taps { int n, dy[9], dx[9], w[9]; };
-
-static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d_in_info, const void *d_w, int w_taps, int cout_pad,
-                     const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info, float gain,
-                     float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, P2Params &p, const P2Taps *cls, int grid_h,
-                     int grid_w, void *stream) {
-    if (!d_in_planes || !d_in_info || !d_w || !d_scale || (!d_out_f32 && !d_out_planes)) return SESSD_EINVAL;
-    if (p.cin < 64 || p.cin % 64 || p.cout < 8 || p.cout % 8) return SESSD_EINVAL;      // even stage count per item; 16-byte plane stores
-    const int n_tile = p.cout <= 32 ? 32 : 128;
-    if (cout_pad % n_tile || cout_pad < p.cout) return SESSD_EINVAL;
-    // orientation: the in-group dimension u has the 8-pixel tile edge; pick the mapping with fewer tiles
-    const int t_ux = div_up(grid_w, kP2TileU) * div_up(grid_h, kP2TileV), t_uy = div_up(grid_h, kP2TileU) * div_up(grid_w, kP2TileV);
-    p.u_is_x = t_ux <= t_uy ? 1 : 0;
-    p.grid_u = p.u_is_x ? grid_w : grid_h;
-    p.grid_v = p.u_is_x ? grid_h : grid_w;
-    // patch copies: one per distinct (tap shift along u, tap shift along v modulo the input stride)
-    const int s = p.in_stride;
-    p.ncopies = 0;
-    int key_u[kP2MaxCopies], key_vm[kP2MaxCopies], vmin[kP2MaxCopies], vmax[kP2MaxCopies];
-    for (int c = 0; c < p.nclass; ++c)
-        for (int t = 0; t < cls[c].n; ++t) {
-            const int tu = p.u_is_x ? cls[c].dx[t] : cls[c].dy[t], tv = p.u_is_x ? cls[c].dy[t] : cls[c].dx[t];
-            const int vm = ((tv % s) + s) % s;
-            int k = 0;
-            for (; k < p.ncopies; ++k)
-                if (key_u[k] == tu && key_vm[k] == vm) break;
-            if (k == p.ncopies) {
-                if (p.ncopies == kP2MaxCopies) return SESSD_EINVAL;
-                key_u[k] = tu; key_vm[k] = vm; vmin[k] = tv; vmax[k] = tv;
-                ++p.ncopies;
-            }
-            vmin[k] = min(vmin[k], tv); vmax[k] = max(vmax[k], tv);
-        }
-    p.rows_v = 0;
-    for (int k = 0; k < p.ncopies; ++k) p.rows_v = max(p.rows_v, kP2TileV + (vmax[k] - vmin[k]) / s);
-    if (p.rows_v > kP2MaxRowsV) return SESSD_EINVAL;
-    for (int k = 0; k < p.ncopies; ++k) { p.copy_u[k] = key_u[k]; p.copy_v[k] = vmin[k]; }
-    for (int c = 0; c < p.nclass; ++c) {
-        p.cls_ntaps[c] = cls[c].n;
-        if ((cls[c].n * (p.cin / kP2Chunk)) & 1) return SESSD_EINVAL;
-        for (int t = 0; t < cls[c].n; ++t) {
-            const int tu = p.u_is_x ? cls[c].dx[t] : cls[c].dy[t], tv = p.u_is_x ? cls[c].dy[t] : cls[c].dx[t];
-            const int vm = ((tv % s) + s) % s;
-            int k = 0;
-            for (; k < p.ncopies; ++k)
-                if (key_u[k] == tu && key_vm[k] == vm) break;
-            p.tap_copy[c][t] = k;
-            p.tap_row[c][t] = (tv - vmin[k]) / s;
-            p.tap_w[c][t] = cls[c].w[t];
-        }
-    }
-    p.copy_bytes = p.rows_v * kP2TileU * 64;
-    p.patch_bytes = p.ncopies * 2 * p.copy_bytes;
-    const int fixed = kP2BRing + 1024 + 512;
-    p.npatch = (fixed + 2 * p.patch_bytes <= kP2MaxSmem) ? 2 : 1;
-    const int smem = fixed + p.npatch * p.patch_bytes;
-    if (smem > kP2MaxSmem) return SESSD_EINVAL;
-    // CTA pairs halve the weight bytes every SM pulls from the L2 and stages in shared memory (the two resources that bound the 3x3
-    // layers); the short K loops (1x1 convs: 4-8 tap-chunks per item) are dominated by per-item latencies, where a pair only adds
-    // cross-CTA handshakes (measured: 3x3 128->128 45.9 -> 39.7 us, 3x3 256->256 65.5 -> 51.2 us; 1x1 128->128 22.6 -> 23.6 us)
-    int kloop = 0;
-    for (int c = 0; c < p.nclass; ++c) kloop = max(kloop, cls[c].n * (p.cin / kP2Chunk));
-    const int cs = (g_p2_cluster == 2 || (g_p2_cluster == 0 && kloop >= 16)) ? 2 : 1;
-    CUtensorMap map_a, map_b;
-    {   // planes [2][B][H][W][C] fp16 viewed as {C, U, V, B, plane}
-        const cuuint64_t row_w = (cuuint64_t)p.cin * 2, row_h = (cuuint64_t)in_w * p.cin * 2;
-        const cuuint64_t dims[5] = {(cuuint64_t)p.cin, (cuuint64_t)(p.u_is_x ? in_w : in_h), (cuuint64_t)(p.u_is_x ? in_h : in_w),
-                                    (cuuint64_t)p.batch, 2};
-        const cuuint64_t strides[4] = {p.u_is_x ? row_w : row_h, p.u_is_x ? row_h : row_w, (cuuint64_t)in_h * in_w * p.cin * 2,
-                                       (cuuint64_t)p.batch * in_h * in_w * p.cin * 2};
-        const cuuint32_t box[5] = {kP2Chunk, (cuuint32_t)(kP2TileU * s), (cuuint32_t)(p.rows_v * s), 1, 1};
-        const cuuint32_t estr[5] = {1, (cuuint32_t)s, (cuuint32_t)s, 1, 1};
-        int rc = encode_map_nd(&map_a, d_in_planes, 5, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_64B);
-        if (rc) return rc;
-    }
-    {   // weights [2 (hi|lo)][taps][cout_pad][cin] fp16
-        const cuuint64_t dims[4] = {(cuuint64_t)p.cin, (cuuint64_t)cout_pad, (cuuint64_t)w_taps, 2};
-        const cuuint64_t strides[3] = {(cuuint64_t)p.cin * 2, (cuuint64_t)cout_pad * p.cin * 2, (cuuint64_t)w_taps * cout_pad * p.cin * 2};
-        const cuuint32_t box[4] = {kP2Chunk, (cuuint32_t)(n_tile / cs), 1, 1};
-        const cuuint32_t estr[4] = {1, 1, 1, 1};
-        int rc = encode_map_nd(&map_b, d_w, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_64B);
-        if (rc) return rc;
-    }
-    static bool attr_done = false;
-    if (!attr_done) {
-        SESSD_CUDA_TRY(cudaFuncSetAttribute(bev_conv_p2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2MaxSmem));
-        SESSD_CUDA_TRY(cudaFuncSetAttribute(bev_conv_p2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2MaxSmem));
-        attr_done = true;
-    }
-    p.n_tile = n_tile;
-    p.bstage_bytes = 2 * (n_tile / cs) * 64;
-    p.bstages = kP2BRing / p.bstage_bytes < kP2MaxBStages ? kP2BRing / p.bstage_bytes : kP2MaxBStages;
-    p.dbg = g_p2_dbg;
-    p.tiles_u = div_up(p.grid_u, kP2TileU);
-    p.tiles_v = div_up(p.grid_v, kP2TileV);
-    p.tiles = p.tiles_u * p.tiles_v * p.batch;
-    p.tgroups = div_up(p.tiles, cs);
-    p.nblocks = cout_pad / n_tile;
-    p.total = p.nclass * p.nblocks * p.tgroups;
-    for (int c = 0; c < p.nclass; ++c) p.cls_order[c] = c;
-    for (int i = 1; i < p.nclass; ++i)            // insertion sort by descending tap count (heavy items first)
-        for (int k = i; k > 0 && p.cls_ntaps[p.cls_order[k]] > p.cls_ntaps[p.cls_order[k - 1]]; --k) {
-            const int tmp = p.cls_order[k]; p.cls_order[k] = p.cls_order[k - 1]; p.cls_order[k - 1] = tmp;
-        }
-    p.in_info = d_in_info; p.resid_info = d_residual ? d_resid_info : nullptr;
-    if (d_residual && !d_resid_info) return SESSD_EINVAL;
-    p.gain = gain; p.shift_max = shift_max; p.out_info = d_out_info;
-    if (d_out_planes && !d_out_info) return SESSD_EINVAL;
-    p.out_plane_stride = (long long)p.batch * p.out_h * p.out_w * p.cout;
-    static int num_sms = 0;
-    if (!num_sms) {
-        int dev = 0;
-        SESSD_CUDA_TRY(cudaGetDevice(&dev));
-        SESSD_CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-    }
-    const int max_clusters = num_sms / cs;
-    const int nclusters = p.total < max_clusters ? p.total : max_clusters;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(nclusters * cs);
-    cfg.blockDim = dim3(kP2Threads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e;
-    if (cs == 2)
-        e = cudaLaunchKernelEx(&cfg, bev_conv_p2_kernel<2>, map_a, map_b, d_scale, d_shift, d_residual, d_out_f32, (__half *)d_out_planes, p);
-    else
-        e = cudaLaunchKernelEx(&cfg, bev_conv_p2_kernel<1>, map_a, map_b, d_scale, d_shift, d_residual, d_out_f32, (__half *)d_out_planes, p);
-    ++g_launches;
-    if (e != cudaSuccess) return (int)e;
-    return last_error();
-}
-
 }  // namespace sessd
 
 using namespace sessd;
-
-// 0 (default): CTA pairs (tcgen05 cta_group::2, each CTA stages half of every weight tile) where the K loop is long; 1 / 2: force
-extern "C" void sessd_set_p2_cluster(int cs) { sessd::g_p2_cluster = (cs == 1 || cs == 2) ? cs : 0; }
-
-
-#ifdef SESSD_P2_PROFILE
-extern "C" void sessd_set_p2_dbg(void *d) { sessd::g_p2_dbg = (long long *)d; }
-#endif
 
 // Conv2d (stride 1 or 2, arbitrary tap list) + folded BN + ReLU (+ residual) from fp16 (hi, lo) planes.
 //   d_in_planes  __half [2][batch][in_h][in_w][cin]; d_in_info [2] = {abs-max of the input, scale of its planes} (device);
@@ -676,25 +36,8 @@ extern "C" void sessd_set_p2_dbg(void *d) { sessd::g_p2_dbg = (long long *)d; }
 extern "C" int sessd_bev_conv_p2(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                                  const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                                  float *d_out_f32, void *d_out_planes, float *d_out_info, const sessd_conv_desc *desc, void *stream) {
-    if (!desc) return SESSD_EINVAL;
-    const sessd_conv_desc &d = *desc;
-    if (d.batch < 1 || d.ntaps < 1 || d.ntaps > 9 || (d.in_stride != 1 && d.in_stride != 2) || d.out_stride < 1 || d.grid_h < 1 || d.grid_w < 1)
-        return SESSD_EINVAL;
-    if ((d.grid_h - 1) * d.out_stride + d.out_off_y >= d.out_h || (d.grid_w - 1) * d.out_stride + d.out_off_x >= d.out_w) return SESSD_EINVAL;
-    P2Params p = {};
-    p.batch = d.batch; p.cin = d.cin; p.cout = d.cout; p.in_stride = d.in_stride;
-    p.out_h = d.out_h; p.out_w = d.out_w; p.out_stride = d.out_stride; p.relu = d.relu;
-    p.nclass = 1;
-    P2Taps t = {};
-    t.n = d.ntaps;
-    for (int i = 0; i < d.ntaps; ++i) { t.dy[i] = d.tap_dy[i]; t.dx[i] = d.tap_dx[i]; t.w[i] = i; }
-    // class offsets are expressed along (u, v) inside launch_p2 once the orientation is known: pass (y, x) through the first slots
-    const int off_y = d.out_off_y, off_x = d.out_off_x;
-    const int t_ux = div_up(d.grid_w, kP2TileU) * div_up(d.grid_h, kP2TileV), t_uy = div_up(d.grid_h, kP2TileU) * div_up(d.grid_w, kP2TileV);
-    const bool u_is_x = t_ux <= t_uy;
-    p.cls_off_u[0] = u_is_x ? off_x : off_y; p.cls_off_v[0] = u_is_x ? off_y : off_x;
-    return launch_p2(d_in_planes, d.in_h, d.in_w, d_in_info, d_weight_h2, d.ntaps, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
-                     shift_max, d_out_f32, d_out_planes, d_out_info, p, &t, d.grid_h, d.grid_w, stream);
+    return p2_conv<kP2Planes>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
+                              d_out_f32, d_out_planes, d_out_info, desc, stream);
 }
 
 // ConvTranspose2d(k3, s2, p1, op1) + BN + ReLU (+ residual), four output-parity classes in one launch; weights [2][9][cout_pad][cin],
@@ -703,31 +46,8 @@ extern "C" int sessd_bev_deconv_p2(const void *d_in_planes, const float *d_in_in
                                    const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                                    float *d_out_f32, void *d_out_planes, float *d_out_info, int batch, int in_h, int in_w, int cin, int cout,
                                    int relu, void *stream) {
-    if (batch < 1 || in_h < 1 || in_w < 1) return SESSD_EINVAL;
-    P2Params p = {};
-    p.batch = batch; p.cin = cin; p.cout = cout; p.in_stride = 1;
-    p.out_h = 2 * in_h; p.out_w = 2 * in_w; p.out_stride = 2; p.relu = relu;
-    p.nclass = 4;
-    P2Taps cls[4] = {};
-    const int t_ux = div_up(in_w, kP2TileU) * div_up(in_h, kP2TileV), t_uy = div_up(in_h, kP2TileU) * div_up(in_w, kP2TileV);
-    const bool u_is_x = t_ux <= t_uy;
-    for (int py = 0; py < 2; ++py)
-        for (int px = 0; px < 2; ++px) {
-            const int c = py * 2 + px;
-            p.cls_off_u[c] = u_is_x ? px : py; p.cls_off_v[c] = u_is_x ? py : px;
-            // out[2y+py] receives in[y+dy] * W[ky] with 2y+py = 2(y+dy) - 1 + ky:  py=0 -> (ky=1,dy=0);  py=1 -> (ky=0,dy=1), (ky=2,dy=0)
-            const int kys[2] = {py == 0 ? 1 : 0, 2}, dys[2] = {py == 0 ? 0 : 1, 0}, ny = py == 0 ? 1 : 2;
-            const int kxs[2] = {px == 0 ? 1 : 0, 2}, dxs[2] = {px == 0 ? 0 : 1, 0}, nx = px == 0 ? 1 : 2;
-            int t = 0;
-            for (int a = 0; a < ny; ++a)
-                for (int bb = 0; bb < nx; ++bb) {
-                    cls[c].dy[t] = dys[a]; cls[c].dx[t] = dxs[bb]; cls[c].w[t] = kys[a] * 3 + kxs[bb];
-                    ++t;
-                }
-            cls[c].n = t;
-        }
-    return launch_p2(d_in_planes, in_h, in_w, d_in_info, d_weight_h2, 9, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
-                     d_out_f32, d_out_planes, d_out_info, p, cls, in_h, in_w, stream);
+    return p2_deconv<kP2Planes>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
+                                d_out_f32, d_out_planes, d_out_info, batch, in_h, in_w, cin, cout, relu, stream);
 }
 
 // fp32 [n] (n % 4 == 0, 16-byte aligned) -> planes [2][n] fp16 scaled by the power of two that maps d_info[0] (the tensor's abs-max,

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for the sessd_b200 kernels (sm_100a only).
+// common.cuh -- shared device/host helpers for the sessd_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -8,7 +8,7 @@
 
 namespace sessd {
 
-constexpr int kNumSMs = 148;   // B200: 2 dies x 74 SMs; grids are sized in multiples of this
+constexpr int kNumSMs = 132;   // H100 SXM; grids are sized in multiples of this
 
 extern long long g_launches;   // counted per kernel launch (sessd_launch_count)
 

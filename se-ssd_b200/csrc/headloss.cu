@@ -145,7 +145,7 @@ __global__ void __launch_bounds__(32) headloss_finish_kernel(const float *__rest
     if (k == 7) losses[b * 8 + 7] = (float)counts[2 * b + 1];
 }
 
-constexpr int kHlBlocks = 74;      // per frame; x batch >= 1 wave on 148 SMs from batch 2
+constexpr int kHlBlocks = 74;      // per frame; x batch >= 1 wave on the 132 SMs of an H100 from batch 2
 
 }  // namespace sessd
 

@@ -1,4 +1,4 @@
-// iou3d.cu -- the iou3d_cuda operator family on B200: rotated BEV overlap / IoU / 3-D IoU matrices and the three
+// iou3d.cu -- the iou3d_cuda operator family on the GPU: rotated BEV overlap / IoU / 3-D IoU matrices and the three
 // NMS variants with the greedy reduction done ON DEVICE.
 //
 // Replaces det3d/core/iou3d/src/iou3d.cpp:34-281 and iou3d_kernel.cu:270-365,425-530.  Differences by design:

@@ -9,7 +9,7 @@
 namespace sessd {
 
 constexpr int kOdThreads = 128;
-constexpr int kOdBlocks = 148;
+constexpr int kOdBlocks = kNumSMs;
 
 __global__ void __launch_bounds__(kOdThreads) odiou_loss_kernel(const float *__restrict__ head, const float *__restrict__ anchors,
                                                                 const int *__restrict__ labels, const float *__restrict__ reg_targets, int batch,

@@ -1,4 +1,4 @@
-// rotbox.cuh -- rotated-rectangle BEV overlap / IoU device functions (sm_100a).
+// rotbox.cuh -- rotated-rectangle BEV overlap / IoU device functions (sm_90a).
 //
 // Same algorithm and fp32 operation order as the reference's box_overlap / iou_bev / iou_3d
 // (det3d/core/iou3d/src/iou3d_kernel.cu:125-268, CPU twin iou3d_cpu.cpp:126-254): rotate the four corners of each

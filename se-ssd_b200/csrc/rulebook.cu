@@ -1,4 +1,4 @@
-// rulebook.cu -- sparse-convolution rulebook ("indice pairs") construction on B200.
+// rulebook.cu -- sparse-convolution rulebook ("indice pairs") construction on the GPU.
 //
 // Replaces the indice-pair builders of spconv 1.x that det3d/models/backbones/scn.py:106-149,182-183 triggers
 // (one per SubM indice_key + one per strided SparseConv3d = 8 builds per forward).  spconv builds per-offset pair

@@ -11,7 +11,7 @@
 // BatchNorm scale/shift and ReLU and writes each output row exactly once -- no scatter-add, no atomics, no
 // intermediate buffers (spconv writes/reads 2 x sum(P_k) x C floats of gather/scatter buffers per layer).
 // Algorithmic HBM bytes per layer: 4 (N_in Cin + N_out Cout) + 4 kvol N_out (nbr) + 4 kvol Cin Cout (weights);
-// FLOPs: 2 sum(P_k) Cin Cout.  This SIMT fp32 version is the numerics baseline for the tcgen05 path.
+// FLOPs: 2 sum(P_k) Cin Cout.  This SIMT fp32 version is the numerics baseline for the tensor-core path.
 #include "common.cuh"
 
 namespace sessd {

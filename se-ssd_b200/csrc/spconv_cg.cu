@@ -1,30 +1,28 @@
-// spconv_cg.cu -- sparse 3-D convolution (SubM / strided, + folded BN + ReLU) on the tcgen05 tensor cores whose operand traffic is
-// proportional to the number of rulebook PAIRS: only the neighbour rows that exist are fetched.
+// spconv_cg.cu -- sparse 3-D convolution (SubM / strided, + folded BN + ReLU) on the Hopper tensor cores (wgmma) whose operand traffic
+// is proportional to the number of rulebook PAIRS: only the neighbour rows that exist are fetched.
 //
-// Replaces spconv 1.x's per-offset gather -> sgemm -> scatter-add used by det3d/models/backbones/scn.py:106-149 (SpMiddleFHD), like
-// the lab library's spconv_h2.cu (same numerics: fp16 (hi, lo) planes with an exact power-of-two scale, three kind::f16 products per MAC,
-// two main + one cross TMEM accumulator summed in RN fp32), but the 128-row A operand of a (tile, kernel offset) is no longer fetched
-// with 32-64 TMA gather4 instructions whose cost is per ROW SLOT, present or not (~5.5 clk per 128-byte row: at the 21 % neighbour fill of
-// the 32-channel layers 79 % of the row requests fetched zeros and the layer ran at 0.9 % of the tensor peak).  Here
+// Replaces spconv 1.x's per-offset gather -> sgemm -> scatter-add used by det3d/models/backbones/scn.py:106-149 (SpMiddleFHD).
+// Numerics: fp16 (hi, lo) planes with an exact power-of-two scale, three fp16 products per MAC (a_hi b_hi into the main accumulator,
+// a_hi b_lo + a_lo b_hi into the cross accumulator, both fp32), summed in RN fp32 by the epilogue.
 //   * the rulebook is regrouped ONCE per build (sessd_rulebook_tile_lists; a SubM rulebook serves 2-3 layers) into per-tile, per-offset
-//     lists of (input row, tile row) pairs + row masks; a tile's record (~3-8 KB) is copied to shared memory (compacting the neighbour
-//     table inside this kernel with shared-memory atomics cost 14.7 k clk per tile, a third of the tile's time);
-//   * eight producer warps copy the listed rows with 16-byte cp.async (LDGSTS: global/L2 -> shared, no registers, 2 clk per 128-byte row)
-//     straight into the K-major SWIZZLE_128B layout the UMMA descriptors address; rows without a neighbour are never touched;
+//     lists of (input row, tile row) pairs + row masks; a tile's record (~3-8 KB) is copied to shared memory;
+//   * eight producer warps copy the listed rows with 16-byte cp.async (global/L2 -> shared, no registers) straight into the K-major
+//     SWIZZLE_128B layout the wgmma descriptors address; rows without a neighbour are never touched;
 //   * a stage's missing rows must read as zeros: each producer warp remembers (registers) which of its rows of its stage hold data and
 //     clears (st.shared) only the rows that were valid for the stage's previous offset and are not for the new one -- the stages are
 //     zeroed once per CTA;
-//   * the 32-channel layers stage the weights as [b_hi rows ; b_lo rows] of 64 bytes (SWIZZLE_64B) so that one N = 2 Cout product gives
-//     the main and the a_hi x b_lo cross term (4 instead of 6 MMAs per offset: an SS-form MMA costs max(math, operand bytes / 128 B/clk));
-//   * CTAs are persistent (two per SM: one tile's epilogue overlaps the other's main loop), so barrier / TMEM / zero-fill setup is paid
-//     once, not per 128 rows;
+//   * the 32-channel layers stage the weights as [b_hi rows ; b_lo rows] of 64 bytes (SWIZZLE_64B), the 64-channel layers as
+//     [b_hi ; b_lo] tiles of 128-byte rows (SWIZZLE_128B);
+//   * two consumer warpgroups (64 tile rows each) issue the wgmmas of every offset, keep one offset's group in flight while they wait
+//     for the next stage, and run the epilogue from the accumulator registers;
+//   * CTAs are persistent (one per SM), so barrier / zero-fill setup is paid once, not per 128 rows;
 //   * the epilogue writes the NEXT layer's operand format directly -- fp16 (hi, lo) planes scaled by a power of two derived from a
 //     rigorous bound |out| <= amax_in * G + max|shift| (G from the weights, host; amax_in measured by the producing layer's epilogue) --
-//     and raises the output's abs-max: the separate split kernel (one read + one write of every feature tensor) is gone.
+//     and raises the output's abs-max: no separate split kernel.
 // Each stage has its own producer group (8 / kStages warps): the group copies, waits for ITS copies (cp.async.wait_all), makes them and
 // the clears visible to the async proxy (fence.proxy.async by the writing threads) and arrives on the stage's mbarrier, while the other
-// groups' fills are in flight -- kStages fills per CTA overlap and nobody hands data over on behalf of another thread.
-// Warps: 0-7 producers then epilogue (TMEM lane quadrant = warp & 3, column half = warp >> 2), 8 weight-tile TMA, 9 MMA issue.
+// groups' fills are in flight.
+// Warps: 0-7 producers, 8-15 consumers (warpgroups 2 and 3), 16 weight-tile TMA.
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -34,22 +32,22 @@ namespace sessd {
 constexpr int kCgBM = 128;
 constexpr int kCgMaxK = 27;
 constexpr int kCgProdWarps = 8;
-constexpr int kCgProdThreads = kCgProdWarps * 32;
-constexpr int kCgThreads = kCgProdThreads + 64;
+constexpr int kCgMmaWarps = 8;
+constexpr int kCgWeightWarp = kCgProdWarps + kCgMmaWarps;
+constexpr int kCgThreads = (kCgWeightWarp + 1) * 32;
 
-// DEEP = 1: twice the stages, one CTA per SM -- for launches whose tiles do not fill the machine twice over (a single frame: ~100 tiles on 148 SMs), where
-// a CTA is alone on its SM anyway and the layer's time is the serial chain of its tile's fills (latency-bound): more fills in flight shorten it
+// DEEP = 1: twice the stages -- for launches whose tiles do not fill the machine (a single frame: ~100 tiles on 132 SMs), where the
+// layer's time is the serial chain of a tile's fills (latency-bound): more fills in flight shorten it
 template <int CP, int COUT, int DEEP = 0>
 struct CgCfg {
     static constexpr bool kWide = (CP == 64);
     static constexpr int kATile = (kWide ? 2 : 1) * kCgBM * 128;              // bytes: [hi tile ; lo tile] (wide) or one [hi | lo] tile
-    static constexpr int kBTile = (kWide ? 2 : 1) * COUT * 128;
+    static constexpr int kBTile = (kWide ? 2 : 1) * COUT * 128;               // wide: [b_hi ; b_lo] of 128-byte rows; narrow: 64-byte rows
     static constexpr int kStage = kATile + (kBTile + 1023) / 1024 * 1024;
     static constexpr int kStages = (kWide ? 2 : 4) * (DEEP ? 2 : 1);           // must divide the 8 producer warps (one group per stage)
     static constexpr int kMeta = kCgBM * kCgMaxK * 4 /*lists*/ + kCgMaxK * 16 /*valid*/ + 32 * 4 /*cnt*/ + 33 * 4 /*klist, nact*/ + 32 * 4 /*off*/ +
-                                 (3 * kStages + 1) * 8 /*barriers*/ + 24;
+                                 3 * kStages * 8 /*barriers*/ + 24;
     static constexpr int kSmem = kStages * kStage + kMeta + 1024;
-    static constexpr int kTmemCols = (3 * COUT <= 128) ? 128 : 256;
     static constexpr int kCPO = COUT > 32 ? 64 : 32;                          // channels per plane row of the OUTPUT
 };
 
@@ -65,23 +63,9 @@ struct CgArgs {
     float *out_f32;                    // nullable [max_out][COUT]
     __half *out_planes;                // nullable [max_out (+1)][2][kCPO]
     float *out_info;                   // nullable {abs-max of the output (atomicMax), plane scale}
-    long long *dbg;                    // SESSD_CG_PROFILE only
 };
 
-__host__ __device__ constexpr uint32_t cg_idesc_f16(int M, int N) {
-    return (1u << 4) /*C=F32*/ | (0u << 7) /*A=F16*/ | (0u << 10) /*B=F16*/ | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__device__ __forceinline__ void cg_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// 16-byte global -> shared copy that bypasses L1 (allocating the gathered rows in L1 was measured: no hits worth the footprint)
+// 16-byte global -> shared copy that bypasses L1 (the gathered rows are not re-read from L1)
 __device__ __forceinline__ void cg_cp_async16(uint32_t smem_dst, const void *gsrc) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(smem_dst), "l"(gsrc) : "memory");
 }
@@ -90,41 +74,20 @@ __device__ __forceinline__ void cg_sts_zero16(uint32_t saddr) {
     asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};\n" ::"r"(saddr), "r"(0) : "memory");
 }
 
-__device__ __forceinline__ void cg_tmem_ld16(uint32_t taddr, uint32_t *r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+template <int COUT>
+__device__ __forceinline__ void cg_wgmma(float *d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    if constexpr (COUT == 32) wgmma_f16_n32(d, da, db, accumulate);
+    else wgmma_f16_n64(d, da, db, accumulate);
 }
 
-// -DSESSD_CG_PROFILE: per-CTA cycle counters ([ctas][16] int64 via sessd_set_cg_dbg; lab measurements only)
-//   0 mma wait full_b, 1 mma wait full_a, 2 mma loop total, 3 tiles, 4 wload wait empty, 5 producer(w0) wait empty, 6 producer(w0) loop total,
-//   7 epilogue wait acc_full (w0), 8 epilogue total (w0), 9 list build (t0), 10 kernel total (t0), 11 stage fills
-#ifdef SESSD_CG_PROFILE
-#define CG_T(var) const long long var = clock64()
-#define CG_ADD(slot, t0) do { cg_acc[slot] += clock64() - (t0); } while (0)
-#define CG_WAIT(slot, cond, stmt) do { const long long _t = clock64(); stmt; if (cond) cg_acc[slot] += clock64() - _t; } while (0)
-#else
-#define CG_T(var)
-#define CG_ADD(slot, t0)
-#define CG_WAIT(slot, cond, stmt) stmt
-#endif
-
 template <int CP, int COUT, int DEEP>
-__global__ void __launch_bounds__(kCgThreads, DEEP ? 1 : 2) spconv_cg_kernel(const __grid_constant__ CUtensorMap map_w, const CgArgs a) {
+__global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_constant__ CUtensorMap map_w, const CgArgs a) {
     using C = CgCfg<CP, COUT, DEEP>;
     const int n_out = min(*a.d_n_out, a.max_out);
     const int ntiles = (n_out + kCgBM - 1) / kCgBM;
-    if ((int)blockIdx.x >= ntiles) return;                       // whole CTA leaves together (before any barrier / TMEM use)
+    if ((int)blockIdx.x >= ntiles) return;                       // whole CTA leaves together (before any barrier use)
     const int kvol = a.kvol;
-#ifdef SESSD_CG_PROFILE
-    long long cg_acc[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};      // per-thread counters, written once at the end (no memory traffic in the loops)
-#endif
-    CG_T(t_kernel);
-    if (threadIdx.x == 8 * 32) prefetch_tensormap(&map_w);       // the weight-TMA warp's first load finds the descriptor cached
+    if (threadIdx.x == kCgWeightWarp * 32) prefetch_tensormap(&map_w);      // the weight-TMA warp's first load finds the descriptor cached
 
     extern __shared__ unsigned char smem_raw[];
     unsigned char *tiles = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -136,29 +99,19 @@ __global__ void __launch_bounds__(kCgThreads, DEEP ? 1 : 2) spconv_cg_kernel(con
     int *s_off = s_nact + 1;                                             // [32] first list entry of every offset
     uint64_t *bars = (uint64_t *)(((uintptr_t)(s_off + 32) + 7) & ~(uintptr_t)7);
     uint64_t *full_a = bars, *full_b = bars + C::kStages, *empty = bars + 2 * C::kStages;
-    uint64_t *acc_full = bars + 3 * C::kStages;
-    uint32_t *tmem_slot = (uint32_t *)(acc_full + 1);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t tiles_u32 = smem_u32(tiles);
 
     if (tid == 0) {
-        for (int s = 0; s < C::kStages; ++s) { mbar_init(&full_a[s], kCgProdWarps / C::kStages); mbar_init(&full_b[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(acc_full, 1);
+        for (int s = 0; s < C::kStages; ++s) { mbar_init(&full_a[s], kCgProdWarps / C::kStages); mbar_init(&full_b[s], 1); mbar_init(&empty[s], kCgMmaWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    }
-    if (warp == 9) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(tmem_slot)), "r"(C::kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
     }
     // every A tile starts as zeros (the B halves of the stages are always fully overwritten by the TMA)
     for (int s = 0; s < C::kStages; ++s)
         for (int o = tid * 16; o < C::kATile; o += kCgThreads * 16) cg_sts_zero16(tiles_u32 + (uint32_t)(s * C::kStage + o));
     cg_fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const float amax_in = __ldg(a.in_info), s_in = __ldg(a.in_info + 1);
     const float inv_act = 1.f / s_in;                            // exact: power of two
@@ -166,20 +119,19 @@ __global__ void __launch_bounds__(kCgThreads, DEEP ? 1 : 2) spconv_cg_kernel(con
     if (blockIdx.x == 0 && tid == 0 && a.out_info) a.out_info[1] = s_out;
     float vmax = 0.f;
     uint32_t dirty[4] = {0u, 0u, 0u, 0u};                        // rows of this warp's share of its stage that hold data (producer warps)
-    int st0 = 0, acc_it = 0;                                     // stage of this tile's first fill / accumulator hand-overs so far (all roles
-    uint32_t ph0 = 0;                                            // count alike); ph0 = phase bit of stage st0
+    int st0 = 0;                                                 // stage of this tile's first fill (all roles advance it alike)
+    uint32_t ph0 = 0;                                            // phase bit of stage st0
 
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int row0 = tile * kCgBM;
         const int rows = min(kCgBM, n_out - row0);
         // ---------------------------------------------------------------- the tile's per-offset pair lists (built once per rulebook by
         // sessd_rulebook_tile_lists: counts, row masks, (input row << 7 | tile row) entries grouped by offset) -> shared memory
-        CG_T(t_list);
         {
             const unsigned int *rec = a.tiles + (size_t)tile * (size_t)a.tile_stride;
             const int c = (int)__ldg(rec + lane);                        // every warp ranks the 32 counts itself: no extra block-wide sync
-            // the first list entries are requested together with the counts (one L2 round trip instead of two for tiles of <= 1280 pairs;
-            // the record is 160 + 128 kvol words long, so the speculative reads stay inside it)
+            // the first list entries are requested together with the counts (one L2 round trip instead of two for most tiles; the record
+            // is 160 + 128 kvol words long, so the speculative reads stay inside it)
             unsigned int spec[4];
 #pragma unroll
             for (int u = 0; u < 4; ++u) spec[u] = (tid + u * kCgThreads < 128 * kvol) ? __ldg(rec + 160 + tid + u * kCgThreads) : 0u;
@@ -200,112 +152,107 @@ __global__ void __launch_bounds__(kCgThreads, DEEP ? 1 : 2) spconv_cg_kernel(con
         }
         __syncthreads();
         const int nact = *s_nact;
-        if (tid == 0) { CG_ADD(9, t_list); }
 
-        // stage index / phase of this tile's first fill (all roles advance them alike)
-        if (warp == 9) {
-            // ===================== MMA issue (one elected lane; the warp walks the loop together: operands stay in uniform registers) ===
-            const uint32_t idesc = cg_idesc_f16(kCgBM, COUT);
-            const uint32_t idesc2 = cg_idesc_f16(kCgBM, 2 * COUT);
-            const uint64_t desc_hi = ((uint64_t)((1024u >> 4) | (1u << 14) | (2u << 29))) << 32;      // SBO | version | SWIZZLE_128B
-            const uint64_t desc_b64 = ((uint64_t)((512u >> 4) | (1u << 14) | (4u << 29))) << 32;      // narrow weight stages: SWIZZLE_64B rows
-            const uint32_t tiles_lo = ((tiles_u32 >> 4) & 0x3FFFu) | (1u << 16);
-            const uint32_t acc_main0 = tmem_base, acc_cross = tmem_base + COUT, acc_main1 = tmem_base + 2 * COUT;
-            tc_fence_after();                                    // the previous tile's epilogue read the accumulators before the CTA-wide sync
-            int s = st0;
-            uint32_t ph = ph0;
-            CG_T(t_mma);
-            for (int j = 0; j < nact; ++j) {
-                CG_WAIT(0, lane == 0, mbar_wait(&full_b[s], ph));
-                CG_WAIT(1, lane == 0, mbar_wait(&full_a[s], ph));
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint32_t st_lo = tiles_lo + (uint32_t)s * (C::kStage >> 4);
-                    const uint64_t dA = desc_hi | st_lo;
-                    const uint64_t dB = desc_hi | (st_lo + (C::kATile >> 4));
-                    if constexpr (C::kWide) {
-                        const uint64_t dAl = dA + ((kCgBM * 128) >> 4);
-                        const uint64_t dBh = dB + (((j & 1) ? COUT * 128 : 0) >> 4);       // the b_hi rows inside the [X ; Y] tile
-                        // all K steps of one product first, then the next product: consecutive MMAs of one shape into one accumulator pipeline,
-                        // a switch to a product whose accumulator columns OVERLAP the previous one's drains the pipe (one switch per offset, not per K step)
-                        if ((j & 1) == 0) {
-#pragma unroll
-                            for (int kk = 0; kk < 4; ++kk)
-                                cg_mma_f16(acc_main0, dA + 2 * kk, dB + 2 * kk, idesc2, (j != 0 || kk != 0) ? 1u : 0u);      // [main0|cross] (+)= a_hi x [b_hi;b_lo]
-                        } else {
-                            if (j == 1) {
-                                cg_mma_f16(acc_main1, dA, dBh, idesc, 0u);                                                 // main1  = a_hi x b_hi
-                                cg_mma_f16(acc_cross, dA, dB, idesc, 1u);                                                  // cross += a_hi x b_lo
-                            }
-#pragma unroll
-                            for (int kk = 0; kk < 4; ++kk)
-                                if (j != 1 || kk != 0) cg_mma_f16(acc_cross, dA + 2 * kk, dB + 2 * kk, idesc2, 1u);         // [cross|main1] += a_hi x [b_lo;b_hi]
-                        }
-#pragma unroll
-                        for (int kk = 0; kk < 4; ++kk) cg_mma_f16(acc_cross, dAl + 2 * kk, dBh + 2 * kk, idesc, 1u);        // cross += a_lo x b_hi
-                    } else {
-                        // narrow: A line = [hi 32 | lo 32] halves (SWIZZLE_128B); B stage = [b_hi rows ; b_lo rows] of 64 bytes each (SWIZZLE_64B),
-                        // [b_lo ; b_hi] on odd offsets: one N = 2 COUT product gives main and the a_hi x b_lo cross term together (4 instead of
-                        // 6 MMAs per offset: the A-operand reads from shared memory bound these layers)
-                        const uint64_t dBn = desc_b64 | (st_lo + (C::kATile >> 4));
-                        const uint64_t dBh = dBn + (((j & 1) ? COUT * 64 : 0) >> 4);
-                        if ((j & 1) == 0) {
-#pragma unroll
-                            for (int kk = 0; kk < 2; ++kk)
-                                cg_mma_f16(acc_main0, dA + 2 * kk, dBn + 2 * kk, idesc2, (j != 0 || kk != 0) ? 1u : 0u);   // [main0|cross] (+)= a_hi x [b_hi;b_lo]
-                        } else {
-                            if (j == 1) {
-                                cg_mma_f16(acc_main1, dA, dBh, idesc, 0u);                                                 // main1  = a_hi x b_hi
-                                cg_mma_f16(acc_cross, dA, dBn, idesc, 1u);                                                 // cross += a_hi x b_lo
-                            }
-#pragma unroll
-                            for (int kk = 0; kk < 2; ++kk)
-                                if (j != 1 || kk != 0) cg_mma_f16(acc_cross, dA + 2 * kk, dBn + 2 * kk, idesc2, 1u);        // [cross|main1] += a_hi x [b_lo;b_hi]
-                        }
-#pragma unroll
-                        for (int kk = 0; kk < 2; ++kk) cg_mma_f16(acc_cross, dA + 4 + 2 * kk, dBh + 2 * kk, idesc, 1u);     // cross += a_lo x b_hi
-                    }
-                    tc_commit(&empty[s]);
-                    if (j == nact - 1) tc_commit(acc_full);
-                }
-                __syncwarp();
-                if (++s == C::kStages) { s = 0; ph ^= 1u; }
-            }
-            if (lane == 0) { CG_ADD(2, t_mma); }
-#ifdef SESSD_CG_PROFILE
-            if (lane == 0) { cg_acc[3] += 1; cg_acc[11] += nact; }
-#endif
-        } else if (warp == 8) {
-            // ===================== weight tiles (TMA, one elected lane) =====================
+        if (warp == kCgWeightWarp) {
+            // ===================== weight tiles (TMA, one elected lane): [b_hi ; b_lo] =====================
             int s = st0;
             uint32_t ph = ph0;
             for (int j = 0; j < nact; ++j) {
                 const int k = s_klist[j];
-                CG_WAIT(4, lane == 0, mbar_wait(&empty[s], ph ^ 1u));
+                mbar_wait(&empty[s], ph ^ 1u);
                 if (elect_one()) {
                     mbar_expect_tx(&full_b[s], C::kBTile);
                     unsigned char *b_tile = tiles + s * C::kStage + C::kATile;
-                    if constexpr (C::kWide) {
-                        // [b_hi ; b_lo] on even steps, [b_lo ; b_hi] on odd steps (see the MMA issuer)
-                        tma_load_4d(b_tile + ((j & 1) ? COUT * 128 : 0), &map_w, &full_b[s], 0, 0, 0, k);
-                        tma_load_4d(b_tile + ((j & 1) ? 0 : COUT * 128), &map_w, &full_b[s], 0, 0, 1, k);
-                    } else {
-                        tma_load_4d(b_tile + ((j & 1) ? COUT * 64 : 0), &map_w, &full_b[s], 0, 0, 0, k);
-                        tma_load_4d(b_tile + ((j & 1) ? 0 : COUT * 64), &map_w, &full_b[s], 0, 0, 1, k);
-                    }
+                    tma_load_4d(b_tile, &map_w, &full_b[s], 0, 0, 0, k);
+                    tma_load_4d(b_tile + C::kBTile / 2, &map_w, &full_b[s], 0, 0, 1, k);
                 }
                 __syncwarp();
                 if (++s == C::kStages) { s = 0; ph ^= 1u; }
             }
+        } else if (warp >= kCgProdWarps) {
+            // ===================== consumers: wgmma per offset, then the epilogue from the accumulator registers =====================
+            const int cw = warp - kCgProdWarps, wg = cw >> 2, wq = cw & 3;
+            constexpr int kAcc = COUT / 2;
+            float acc_m[kAcc], acc_c[kAcc];
+#pragma unroll
+            for (int i = 0; i < kAcc; ++i) { acc_m[i] = 0.f; acc_c[i] = 0.f; }
+            const uint32_t a_rows = (uint32_t)(wg * 64 * 128);   // this warpgroup's 64 rows of the 128-byte-row A tile
+            int s = st0, prev = -1;
+            uint32_t ph = ph0;
+            for (int j = 0; j < nact; ++j) {
+                mbar_wait(&full_b[s], ph);
+                mbar_wait(&full_a[s], ph);
+                const uint32_t st = tiles_u32 + (uint32_t)(s * C::kStage);
+                const uint64_t dA = kDescSw128Hi | desc_lo(st + a_rows);
+                const uint32_t first = j != 0 ? 1u : 0u;
+                wgmma_fence();
+                if constexpr (C::kWide) {
+                    const uint64_t dAl = dA + ((kCgBM * 128) >> 4);
+                    const uint64_t dBh = kDescSw128Hi | desc_lo(st + C::kATile);
+                    const uint64_t dBl = dBh + ((COUT * 128) >> 4);
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk) cg_wgmma<COUT>(acc_m, dA + 2 * kk, dBh + 2 * kk, first | (kk != 0));      // main  += a_hi x b_hi
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk) cg_wgmma<COUT>(acc_c, dA + 2 * kk, dBl + 2 * kk, first | (kk != 0));      // cross += a_hi x b_lo
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk) cg_wgmma<COUT>(acc_c, dAl + 2 * kk, dBh + 2 * kk, 1u);                    // cross += a_lo x b_hi
+                } else {
+                    // A line = [hi 32 | lo 32] (SWIZZLE_128B); B stage = [b_hi rows ; b_lo rows] of 64 bytes each (SWIZZLE_64B)
+                    const uint64_t dBh = kDescSw64Hi | desc_lo(st + C::kATile);
+                    const uint64_t dBl = dBh + ((COUT * 64) >> 4);
+#pragma unroll
+                    for (int kk = 0; kk < 2; ++kk) cg_wgmma<COUT>(acc_m, dA + 2 * kk, dBh + 2 * kk, first | (kk != 0));
+#pragma unroll
+                    for (int kk = 0; kk < 2; ++kk) cg_wgmma<COUT>(acc_c, dA + 2 * kk, dBl + 2 * kk, first | (kk != 0));
+#pragma unroll
+                    for (int kk = 0; kk < 2; ++kk) cg_wgmma<COUT>(acc_c, dA + 4 + 2 * kk, dBh + 2 * kk, 1u);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                                 // the previous offset's products are done: its stage may be refilled
+                if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+                prev = s;
+                if (++s == C::kStages) { s = 0; ph ^= 1u; }
+            }
+            wgmma_wait<0>();
+            wgmma_fence_regs<kAcc>(acc_m);
+            wgmma_fence_regs<kAcc>(acc_c);
+            if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+            // BN / ReLU -> planes and / or fp32 rows; this thread holds rows r0 and r0 + 8, two adjacent channels per 8-channel group
+            const int r0 = wg * 64 + wq * 16 + (lane >> 2);
+            const int c2 = 2 * (lane & 3);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = r0 + 8 * h;
+                if (r >= rows) continue;
+                const size_t orow = (size_t)(row0 + r);
+#pragma unroll
+                for (int g = 0; g < COUT / 8; ++g) {
+                    const int n = 8 * g + c2, i = 4 * g + 2 * h;
+                    const float2 sc = __ldg(reinterpret_cast<const float2 *>(a.scale + n));
+                    const float2 sh = a.shift ? __ldg(reinterpret_cast<const float2 *>(a.shift + n)) : make_float2(0.f, 0.f);
+                    float o0 = fmaf((acc_m[i] + acc_c[i]) * inv_act, sc.x, sh.x);
+                    float o1 = fmaf((acc_m[i + 1] + acc_c[i + 1]) * inv_act, sc.y, sh.y);
+                    if (a.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+                    vmax = fmaxf(vmax, fmaxf(fabsf(o0), fabsf(o1)));
+                    if (a.out_f32) *reinterpret_cast<float2 *>(a.out_f32 + orow * COUT + n) = make_float2(o0, o1);
+                    if (a.out_planes) {
+                        const float x0 = o0 * s_out, x1 = o1 * s_out;
+                        const __half2 hi = __floats2half2_rn(x0, x1);
+                        const float2 f = __half22float2(hi);
+                        const __half2 lo = __floats2half2_rn(x0 - f.x, x1 - f.y);
+                        __half2 *dst = reinterpret_cast<__half2 *>(a.out_planes + orow * (2 * C::kCPO) + n);
+                        dst[0] = hi;
+                        dst[C::kCPO / 2] = lo;
+                    }
+                }
+            }
         } else {
             // ===================== producers: copy the rows that exist, clear the rows that stopped existing =====================
             // One producer GROUP per stage (kStages groups of 8 / kStages warps): a group fills only "its" stage, waits for its own copies
-            // (cp.async.wait_all), fences them into the async proxy and arrives; the other groups' fills are in flight meanwhile.  (With
-            // every warp working on every fill and cp.async.mbarrier.arrive.noinc as the hand-over, a warp's next shared-memory access
-            // queued behind the arrival, i.e. behind its outstanding copies: ~900 clk = one L2 round trip per fill, serialised.)
-            constexpr int kGroupWarps = kCgProdWarps / C::kStages;       // 2 (four stages) or 4 (two stages)
+            // (cp.async.wait_all), fences them into the async proxy and arrives; the other groups' fills are in flight meanwhile.
+            constexpr int kGroupWarps = kCgProdWarps / C::kStages;       // 1, 2 or 4
             constexpr int kGroupThreads = kGroupWarps * 32;
-            constexpr int kOwnRows = kCgBM / kGroupWarps;                // rows of the stage whose zero state this warp maintains: 64 or 32
+            constexpr int kOwnRows = kCgBM / kGroupWarps;                // rows of the stage whose zero state this warp maintains: 128, 64 or 32
             constexpr int kOwnWords = kOwnRows / 32;
             constexpr int kLanesPerRow = C::kWide ? 16 : 8;
             constexpr int kRowsPerPass = kGroupThreads / kLanesPerRow;
@@ -315,12 +262,11 @@ __global__ void __launch_bounds__(kCgThreads, DEEP ? 1 : 2) spconv_cg_kernel(con
             const int c = gtid % kLanesPerRow;
             const int half = c >> 3, cc = c & 7;                         // wide: chunk c of the 256-byte row = (hi | lo tile, 16-byte chunk)
             const uint32_t a_base = tiles_u32 + (uint32_t)(grp * C::kStage);
-            CG_T(t_prod);
             // this tile's fills that land in stage `grp`: j = j0, j0 + kStages, ...; the phase bit of fill j follows the ring position
             for (int j = (grp - st0 + C::kStages) % C::kStages; j < nact; j += C::kStages) {
                 const uint32_t ph = ph0 ^ ((uint32_t)((st0 + j) / C::kStages) & 1u);
                 const int k = s_klist[j];
-                if (lane == 0) CG_WAIT(5, warp == 0, mbar_wait(&empty[grp], ph ^ 1u));
+                if (lane == 0) mbar_wait(&empty[grp], ph ^ 1u);
                 __syncwarp();
 #pragma unroll
                 for (int w = 0; w < kOwnWords; ++w) {
@@ -350,8 +296,7 @@ __global__ void __launch_bounds__(kCgThreads, DEEP ? 1 : 2) spconv_cg_kernel(con
                     else
                         cg_cp_async16(a_base + r * 128u + (((uint32_t)cc ^ (r & 7u)) << 4), a.planes + src * 64 + cc * 8);
                 };
-                // four list entries per round: the shared-memory reads of a round are in flight together (the copies are `asm volatile`
-                // with a memory clobber, so the compiler keeps every read behind the previous copy otherwise: one LDS latency per row)
+                // four list entries per round: the shared-memory reads of a round are in flight together
                 int i = slot;
                 for (; i + 3 * kRowsPerPass < n; i += 4 * kRowsPerPass) {
                     const uint32_t e0 = lst[i], e1 = lst[i + kRowsPerPass], e2 = lst[i + 2 * kRowsPerPass], e3 = lst[i + 3 * kRowsPerPass];
@@ -359,115 +304,25 @@ __global__ void __launch_bounds__(kCgThreads, DEEP ? 1 : 2) spconv_cg_kernel(con
                 }
                 for (; i < n; i += kRowsPerPass) copy_row(lst[i]);
                 asm volatile("cp.async.wait_all;\n" ::: "memory");
-                cg_fence_proxy_async();                                  // copies and clears (generic proxy) -> visible to the tensor core (measured: free)
+                cg_fence_proxy_async();                                  // copies and clears (generic proxy) -> visible to the tensor core
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&full_a[grp]);
             }
-
-            if (tid == 0) { CG_ADD(6, t_prod); }
-            CG_T(t_epi);
-            // ===================== epilogue: TMEM -> registers -> BN / ReLU -> planes and / or fp32 rows =====================
-            const int q = warp & 3, hcol = warp >> 2;
-            constexpr int kNcol = COUT / 2;                              // 16 or 32 channels per thread
-            const int r = q * 32 + lane;
-            float v[kNcol];
-            if (nact > 0) {
-                if (lane == 0) CG_WAIT(7, warp == 0, mbar_wait(acc_full, (uint32_t)acc_it & 1u));
-                __syncwarp();
-                tc_fence_after();
-                const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(hcol * kNcol);
-#pragma unroll
-                for (int c0 = 0; c0 < kNcol; c0 += 16) {
-                    uint32_t m0[16], cr[16], m1[16];
-                    cg_tmem_ld16(lane_base + c0, m0);
-                    cg_tmem_ld16(lane_base + COUT + c0, cr);
-                    if (nact > 1) cg_tmem_ld16(lane_base + 2 * COUT + c0, m1);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        float t = __uint_as_float(m0[i]) + __uint_as_float(cr[i]);
-                        if (nact > 1) t += __uint_as_float(m1[i]);
-                        v[c0 + i] = t;
-                    }
-                }
-                tc_fence_before();                                       // the next tile's MMAs overwrite the accumulators after the CTA-wide sync
-            } else {
-#pragma unroll
-                for (int i = 0; i < kNcol; ++i) v[i] = 0.f;
-            }
-            if (r < rows) {
-                const size_t orow = (size_t)(row0 + r);
-                uint32_t hprev[4] = {0u, 0u, 0u, 0u}, lprev[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-                for (int i = 0; i < kNcol; i += 8) {
-                    const int n = hcol * kNcol + i;
-                    float o[8];
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const float4 sc = *reinterpret_cast<const float4 *>(a.scale + n + 4 * h);
-                        float4 sh = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (a.shift) sh = *reinterpret_cast<const float4 *>(a.shift + n + 4 * h);
-                        o[4 * h + 0] = fmaf(v[i + 4 * h + 0] * inv_act, sc.x, sh.x); o[4 * h + 1] = fmaf(v[i + 4 * h + 1] * inv_act, sc.y, sh.y);
-                        o[4 * h + 2] = fmaf(v[i + 4 * h + 2] * inv_act, sc.z, sh.z); o[4 * h + 3] = fmaf(v[i + 4 * h + 3] * inv_act, sc.w, sh.w);
-                    }
-                    if (a.relu) {
-#pragma unroll
-                        for (int t = 0; t < 8; ++t) o[t] = fmaxf(o[t], 0.f);
-                    }
-#pragma unroll
-                    for (int t = 0; t < 8; ++t) vmax = fmaxf(vmax, fabsf(o[t]));
-                    if (a.out_f32) stg256(a.out_f32 + orow * COUT + n, reinterpret_cast<const uint32_t *>(o), reinterpret_cast<const uint32_t *>(o) + 4);
-                    if (a.out_planes) {
-                        __align__(16) __half2 hi[4], lo[4];
-#pragma unroll
-                        for (int t = 0; t < 4; ++t) {
-                            const float x0 = o[2 * t] * s_out, x1 = o[2 * t + 1] * s_out;
-                            hi[t] = __floats2half2_rn(x0, x1);
-                            const float2 f = __half22float2(hi[t]);
-                            lo[t] = __floats2half2_rn(x0 - f.x, x1 - f.y);
-                        }
-                        // 32-byte stores (one full sector per lane): the first 8 channels of a 16-channel group wait for the second
-                        __half *dst = a.out_planes + orow * (2 * C::kCPO) + n;
-                        if ((i & 8) == 0) {
-#pragma unroll
-                            for (int t = 0; t < 4; ++t) { hprev[t] = *reinterpret_cast<const uint32_t *>(&hi[t]); lprev[t] = *reinterpret_cast<const uint32_t *>(&lo[t]); }
-                        } else {
-                            stg256(dst - 8, hprev, reinterpret_cast<const uint32_t *>(hi));
-                            stg256(dst - 8 + C::kCPO, lprev, reinterpret_cast<const uint32_t *>(lo));
-                        }
-                    }
-                }
-            }
-            if (tid == 0) { CG_ADD(8, t_epi); }
         }
         {   // advance the ring position by this tile's fills
             const int adv = st0 + nact;
             ph0 ^= (uint32_t)(adv / C::kStages) & 1u;
             st0 = adv % C::kStages;
         }
-        acc_it += nact > 0 ? 1 : 0;
         __syncthreads();                                         // lists are rebuilt next; every role is done reading them
     }
-    if (warp < kCgProdWarps && a.out_info) {
+    if (warp >= kCgProdWarps && warp < kCgWeightWarp && a.out_info) {
         const unsigned m = __reduce_max_sync(0xFFFFFFFFu, __float_as_uint(vmax));     // non-negative floats order like their bits
         if (lane == 0 && m != 0u) atomicMax(reinterpret_cast<unsigned *>(a.out_info), m);
     }
-    if (tid == 0) { CG_ADD(10, t_kernel); }
-#ifdef SESSD_CG_PROFILE
-    if (a.dbg && lane == 0 && (warp == 0 || warp >= 8)) {
-        long long *d = a.dbg + (size_t)blockIdx.x * 16;
-        if (warp == 9) { d[0] = cg_acc[0]; d[1] = cg_acc[1]; d[2] = cg_acc[2]; d[3] = cg_acc[3]; d[11] = cg_acc[11]; }
-        if (warp == 8) d[4] = cg_acc[4];
-        if (warp == 0) { d[5] = cg_acc[5]; d[6] = cg_acc[6]; d[7] = cg_acc[7]; d[8] = cg_acc[8]; d[9] = cg_acc[9]; d[10] = cg_acc[10]; }
-    }
-#endif
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 9) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "r"(C::kTmemCols) : "memory");
 }
 
-static long long *g_cg_dbg = nullptr;
-static int g_cg_deep = 0;          // 1: deep pipeline, one CTA per SM (sessd_set_sp_cg_deep)
+static int g_cg_deep = 0;          // 1: deep pipeline (sessd_set_sp_cg_deep)
 
 template <int CP, int COUT, int DEEP>
 static int launch_spconv_cg(const CgArgs &a, const void *w_h2, cudaStream_t st) {
@@ -503,8 +358,7 @@ static int launch_spconv_cg(const CgArgs &a, const void *w_h2, cudaStream_t st) 
         SESSD_CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
     }
     const int tiles = div_up(a.max_out, kCgBM);
-    const int per_sm = DEEP ? 1 : 2;
-    const int grid = tiles < per_sm * num_sms ? tiles : per_sm * num_sms;        // persistent
+    const int grid = tiles < num_sms ? tiles : num_sms;                          // persistent, one CTA per SM
     SESSD_LAUNCH((spconv_cg_kernel<CP, COUT, DEEP>), grid, kCgThreads, C::kSmem, st, map_w, a);
     return last_error();
 }
@@ -513,11 +367,8 @@ static int launch_spconv_cg(const CgArgs &a, const void *w_h2, cudaStream_t st) 
 
 using namespace sessd;
 
-#ifdef SESSD_CG_PROFILE
-extern "C" void sessd_set_cg_dbg(void *d) { sessd::g_cg_dbg = (long long *)d; }
-#endif
-// 1: twice the stages and one CTA per SM (launches with fewer tiles than SMs, e.g. single frames: the serial fill chain of a tile is latency-bound);
-// 0 (default): two CTAs per SM (many tiles: throughput)
+// 1: twice the stages (launches with fewer tiles than SMs, e.g. single frames: the serial fill chain of a tile is latency-bound);
+// 0 (default): the shorter ring (many tiles: throughput)
 extern "C" void sessd_set_sp_cg_deep(int on) { sessd::g_cg_deep = on ? 1 : 0; }
 
 // S4 (scn.py:106-149), pair-proportional tensor-core path.  d_in_planes [plane_rows][2][cp] fp16 with d_in_info = {abs-max, scale};
@@ -536,7 +387,7 @@ extern "C" int sessd_spconv_forward_cg(const void *d_in_planes, int cp, int plan
     CgArgs a;
     a.planes = (const __half *)d_in_planes; a.in_info = d_in_info; a.tiles = (const unsigned int *)d_tiles; a.tile_stride = 160 + 128 * kvol; a.d_n_out = d_n_out; a.kvol = kvol; a.max_out = max_out;
     a.relu = relu; a.scale = d_scale; a.shift = d_shift; a.gain = gain; a.shift_max = shift_max; a.out_f32 = d_out_f32;
-    a.out_planes = (__half *)d_out_planes; a.out_info = d_out_info; a.dbg = g_cg_dbg;
+    a.out_planes = (__half *)d_out_planes; a.out_info = d_out_info;
     cudaStream_t st = (cudaStream_t)stream;
 #define SESSD_CG_CASE(CPV, CO) \
     if (cp == CPV && cout == CO) return g_cg_deep ? launch_spconv_cg<CPV, CO, 1>(a, d_weight_h2, st) : launch_spconv_cg<CPV, CO, 0>(a, d_weight_h2, st);

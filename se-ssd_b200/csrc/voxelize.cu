@@ -1,4 +1,4 @@
-// voxelize.cu -- order-preserving hash-grid voxeliser with fused per-voxel mean (sm_100a).
+// voxelize.cu -- order-preserving hash-grid voxeliser with fused per-voxel mean (sm_90a).
 //
 // Replaces the sequential numba loop of det3d/ops/point_cloud/point_cloud_ops_v2.py:9-62 (called through
 // det3d/core/input/voxel_generator.py:24-32) and VoxelFeatureExtractorV3 (det3d/models/readers/voxel_encoder.py
@@ -275,7 +275,7 @@ static VoxWs carve(void *base, int max_total_points, int batch, const sessd_voxe
 
 using namespace sessd;
 
-extern "C" const char *sessd_version(void) { return "sessd_b200 0.1 (sm_100a)"; }
+extern "C" const char *sessd_version(void) { return "sessd_b200 0.1 (sm_90a)"; }
 extern "C" long long sessd_launch_count(void) { return g_launches; }
 
 extern "C" size_t sessd_voxelize_workspace_bytes(int max_total_points, int batch, const sessd_voxel_cfg *cfg) {

@@ -1,5 +1,5 @@
 """det3d -- the Det3D / SE-SSD registry + operator API surface for the per-frame LiDAR hot path, backed by the
-B200-native kernels of ``sessd_b200`` (libsessd_b200.so).
+GPU-native (sm_90a) kernels of ``sessd_b200`` (libsessd_b200.so).
 
 This package mirrors the names, signatures and error behaviour of the reference interfaces that
 ``examples/second/configs/config.py`` and ``tools/test.py`` bind (SURVEY.md 8b), so that the config loads unchanged and

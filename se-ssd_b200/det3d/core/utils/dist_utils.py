@@ -1,5 +1,5 @@
 """Gradient all-reduce of the DDP training loop (reference: det3d/core/utils/dist_utils.py:8-57, driven from
-det3d/torchie/apis/train_sessd.py:286-294).  Same entry points (``allreduce_grads``, ``DistOptimizerHook``); the B200-first path keeps
+det3d/torchie/apis/train_sessd.py:286-294).  Same entry points (``allreduce_grads``, ``DistOptimizerHook``); the GPU-native path keeps
 every gradient inside one contiguous arena (sessd_b200.train.ParamArena) so the collective runs IN PLACE on one buffer -- averaged inside
 NCCL over NVLink / NVSwitch -- instead of flatten -> all_reduce -> divide -> unflatten -> copy back per bucket."""
 import torch

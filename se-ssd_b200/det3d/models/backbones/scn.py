@@ -1,7 +1,7 @@
 """SpMiddleFHD sparse middle encoder (reference: det3d/models/backbones/scn.py:92-189).
 
 Same constructor, parameters and state-dict keys (``middle_conv.{0,3,...}.weight`` in spconv layout [kz,ky,kx,Cin,Cout],
-``middle_conv.{1,4,...}`` BatchNorm1d) so reference checkpoints load.  ``forward`` runs the fused B200 pipeline
+``middle_conv.{1,4,...}`` BatchNorm1d) so reference checkpoints load.  ``forward`` runs the fused CUDA pipeline
 (sessd_b200.runners.SpMiddleRunner): 8 deterministic rulebooks + 14 gather-GEMM launches with BN+ReLU in the epilogue + dense
 scatter, and returns the [B, 128, 200, 176] BEV tensor in channels-last memory (logically NCHW, like the reference's
 ``ret.view(N, C*D, H, W)``)."""

@@ -1,7 +1,7 @@
 """VoxelNet detector with the reference's call contract (det3d/models/detectors/voxelnet_sessd.py): ``forward(example, is_ema,
 return_loss)`` takes the collate_kitti batch dict (voxels, coordinates with a batch column, num_points, num_voxels, shape, anchors, calib,
 metadata; ``*_raw`` twins for the teacher branch) and returns per-frame detection dicts (``return_loss=False``), the head outputs
-(teacher branch) or the loss; every stage runs on the B200 kernels."""
+(teacher branch) or the loss; every stage runs on the sessd_b200 CUDA kernels."""
 from ..registry import DETECTORS
 from .single_stage import SingleStageDetector
 

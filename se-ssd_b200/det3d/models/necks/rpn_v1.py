@@ -2,12 +2,12 @@
 
 Identical module tree (hence identical state-dict keys: ``bottom_up_block_0.1.weight`` ...), identical constructor signature
 (``logger`` is dereferenced exactly like the reference does, :212).  ``forward`` (eval mode) executes the whole neck with the
-B200 kernels: 12 conv / deconv layers as NHWC implicit GEMMs on the tcgen05 tensor cores with BatchNorm + ReLU (+ the
+sessd_b200 kernels: 12 conv / deconv layers as NHWC implicit GEMMs on the wgmma tensor cores with BatchNorm + ReLU (+ the
 deconv_0 + trans_0 residual) fused into the epilogue, and one fused kernel for the two 1-channel attention convs, their BN, the
 2-way softmax and the weighted sum (:229-233)."""
 from torch import nn
 
-from sessd_b200.runners import SSFARunner
+from sessd_b200.runners import SSFAPlanesRunner
 
 from ..registry import NECKS
 from ..utils import build_norm_layer
@@ -65,7 +65,7 @@ class SSFA(nn.Module):
         b, c, h, w = x.shape
         key = (b, h, w, str(x.device))
         if self._runner is None or self._runner_key != key:
-            self._runner = SSFARunner(b, (h, w), x.device)
+            self._runner = SSFAPlanesRunner(b, (h, w), x.device)
             self._runner_key, self._weights_key = key, None
         wkey = tuple((p.data_ptr(), p._version) for p in self.parameters()) + tuple((t.data_ptr(), t._version) for t in self.buffers())
         if wkey != self._weights_key:

@@ -1,4 +1,4 @@
-"""sessd_b200 -- B200-native (sm_100a) implementation of the SE-SSD per-frame LiDAR hot path.
+"""sessd_b200 -- GPU-native (H100, sm_90a) implementation of the SE-SSD per-frame LiDAR hot path.
 
 Importing the package loads libsessd_b200.so through ctypes; there is no CPU or eager-PyTorch fallback: if the CUDA
 library has not been built the import fails."""

@@ -71,7 +71,6 @@ SIGNATURES = {
     "sessd_bev_conv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp]),
     "sessd_bev_deconv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "sessd_bev_split_planes": (_i, [_vp, _ll, _vp, _vp, _vp]),
-    "sessd_set_p2_cluster": (None, [_i]),
     "sessd_sparse_to_dense_planes": (_i, [_vp, _i, _vp, _i, Grid, _vp, _vp, _vp, _vp]),
     "sessd_ssfa_fuse_planes": (_i, [_vp, _vp, _vp, _vp, _f, _f, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "sessd_absmax": (_i, [_vp, C.c_longlong, _vp, _vp]),
@@ -101,25 +100,12 @@ SIGNATURES = {
 }
 
 
-# include/sessd_b200_lab.h: non-default kernel variants and probes (libsessd_b200_lab.so; loaded on first use, by tests / lab scripts only)
+# include/sessd_b200_lab.h: non-default BEV conv variants (libsessd_b200_lab.so; loaded on first use, by tests only)
 LAB_SIGNATURES = {
-    "sessd_spconv_forward_tc": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _vp]),
-    "sessd_set_sp_h2_depth": (None, [_i]),
-    "sessd_split_h2": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _vp]),
-    "sessd_spconv_forward_h2": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "sessd_bev_conv_tc": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp]),
     "sessd_bev_deconv_tc": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "sessd_bev_conv_h2": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp, _vp]),
     "sessd_bev_deconv_h2": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
-    "sessd_set_h2_debug": (None, [_i, _vp]),
-    "sessd_set_conv_cluster": (None, [_i]),
-    "sessd_get_conv_cluster": (_i, []),
-    "sessd_mma_probe": (_i, [_i, _i, _i, _vp, _vp]),
-    "sessd_mma_probe_f16": (_i, [_i, _i, _i, _vp, _vp]),
-    "sessd_latency_probe": (_i, [_i, _vp, _vp]),
-    "sessd_set_conv_ablate": (None, [_i]),
-    "sessd_set_conv_variant": (None, [_i]),
-    "sessd_set_conv_debug_buffer": (None, [_vp]),
 }
 
 

@@ -164,19 +164,11 @@ def spconv_forward_rows(in_feat, nbr, n_out, max_out, weight, scale, shift, relu
     return out
 
 
-def spconv_forward_tc(in_feat, nbr, n_out, max_out, weight_split, scale, shift, relu, out):
-    """weight_split [2, kvol, Cout, Cin] from pack_weight_tc(weight [kvol,Cin,Cout], Cout)."""
-    _two, kvol, cout, cin = weight_split.shape
-    check(lib.sessd_spconv_forward_tc(_p(in_feat), int(cin), _p(nbr), int(kvol), _p(n_out), int(max_out), _p(weight_split), int(cout),
-                                      _p(scale), _p(shift), int(bool(relu)), _p(out), _st()), "sessd_spconv_forward_tc")
-    return out
-
-
 def pack_weight_sp_h2(wp, cp, layout="cg"):
     """[kvol, Cin, Cout] (spconv layout, flattened offsets) -> (fp16 weight tiles of the tensor-core sparse convs, 2^-e[Cout]).
     Every output channel is scaled by the power of two that puts its largest |w| into [2^10, 2^11); hi = fp16_rn(2^e w),
     lo = fp16_rn(2^e w - hi).  cp = 64: [kvol, 2, Cout, 64]; cp = 32: layout "cg" (sessd_spconv_forward_cg): [kvol, 2, Cout, 32] (hi rows, then
-    lo rows), layout "h2" (lab sessd_spconv_forward_h2): [kvol, Cout, 64] with hi in columns [0, Cin), lo in [32, 32+Cin)."""
+    lo rows), layout "h2": [kvol, Cout, 64] with hi in columns [0, Cin), lo in [32, 32+Cin)."""
     kvol, cin, cout = wp.shape
     assert cp in (32, 64) and cin <= cp and (cp == 32 or cin == 64)
     wt = wp.permute(0, 2, 1).contiguous().to(torch.float32)                      # [kvol, Cout, Cin]
@@ -208,27 +200,7 @@ def absmax_rows(feat, n, max_rows, amax):
     return amax
 
 
-def split_h2(feat, n, max_rows, amax, planes):
-    cp = planes.shape[1] // 2
-    assert planes.shape[0] >= max_rows + 1 and planes.dtype == torch.float16
-    check(lib.sessd_split_h2(_p(feat), _p(n), int(max_rows), int(feat.shape[1]), _p(amax), _p(planes), int(cp), _st()), "sessd_split_h2")
-    return planes
-
-
 SP_H2_ZERO_MODE = 1      # missing neighbours: 0 = read the all-zero last row, 1 = row index -1 (TMA OOB fill), 2 = row index rows (OOB)
-
-
-def spconv_forward_h2(in_planes, amax_in, nbr, n_out, max_out, weight_h2, scale, shift, relu, out, amax_out=None):
-    """in_planes from split_h2 (its last row is the zero row); weight_h2 / scale from pack_weight_sp_h2 (scale = bn_scale * 2^-e)."""
-    cp = in_planes.shape[1] // 2
-    kvol = weight_h2.shape[0]
-    cout = weight_h2.shape[2] if cp == 64 else weight_h2.shape[1]
-    rows = in_planes.shape[0]
-    zero_row = (rows - 1, -1, rows)[SP_H2_ZERO_MODE]
-    check(lib.sessd_spconv_forward_h2(_p(in_planes), int(cp), int(rows), int(zero_row), _p(amax_in), _p(nbr), int(kvol), _p(n_out), int(max_out),
-                                      _p(weight_h2), int(cout), _p(scale), _p(shift), int(bool(relu)), _p(out), _p(amax_out), _st()),
-          "sessd_spconv_forward_h2")
-    return out
 
 
 def spconv_forward_rows_planes(in_feat, nbr, n_out, max_out, weight, scale, shift, relu, amax_in, gain, shift_max, out, out_planes, out_info):
@@ -344,7 +316,7 @@ def bev_deconv_tc(x, weight_split, scale, shift, residual, out, relu=True):
 
 
 def pack_weight_h2(wp, cout_pad):
-    """[taps, Cin, Cout] (SIMT packing) -> (planes fp16 [2, taps, cout_pad, Cin], exps [cout_pad] fp32 = 2^-e[n]) for sessd_bev_conv_h2:
+    """[taps, Cin, Cout] (SIMT packing) -> (planes fp16 [2, taps, cout_pad, Cin], exps [cout_pad] fp32 = 2^-e[n]) for sessd_bev_conv_p2 / _h2:
     every output channel is scaled by the power of two 2^e[n] that puts its largest |w| into [2^10, 2^11); hi = fp16_rn(2^e w),
     lo = fp16_rn(2^e w - hi).  The returned 2^-e[n] must be folded into the epilogue scale."""
     taps, cin, cout = wp.shape
@@ -400,11 +372,6 @@ def bev_deconv_p2(in_planes, in_info, weight_h2, scale, shift, residual, resid_i
                                   int(w), int(cin), int(cout), int(bool(relu)), _st()), "sessd_bev_deconv_p2")
 
 
-def set_p2_cluster(n):
-    """bev_conv_p2: 0 (default) = CTA pairs (cta_group::2) where the K loop is long, 1 / 2 = force single CTAs / pairs."""
-    lib.sessd_set_p2_cluster(int(n))
-
-
 def bev_split_planes(x, info, planes):
     """fp32 tensor -> planes with the scale from info[0] (its abs-max: call absmax(x, info[0:1]) first); info[1] <- scale"""
     check(lib.sessd_bev_split_planes(_p(x), int(x.numel()), _p(info), _p(planes), _st()), "sessd_bev_split_planes")
@@ -433,11 +400,6 @@ def absmax(x, amax):
     """amax[0] = max(amax[0], max|x|) on the current stream."""
     check(lib.sessd_absmax(_p(x), int(x.numel()), _p(amax), _st()), "sessd_absmax")
     return amax
-
-
-def set_conv_cluster(n):
-    """CTAs per cluster sharing weight tiles via TMA multicast in bev_conv_tc (1, 2 or 4)."""
-    lib.sessd_set_conv_cluster(int(n))
 
 
 def ssfa_fuse(x0, x1, w0, w1, s0, t0, s1, t1, out):

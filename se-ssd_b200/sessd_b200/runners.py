@@ -29,27 +29,27 @@ class SpMiddleRunner:
     # active-site growth bounds per level relative to the level-0 capacity (uniform 20k cloud: 3.4 / 5.2 / 4.3 / 2.6)
     GROWTH = (1.0, 4.0, 6.0, 5.0, 3.0)
     SPLIT = "fp16"
-    SPARSE_TC = "cg"          # tensor-core kernel of the Cin >= 32 layers: "cg" = pair-proportional cp.async gather, planes written by the
-                              # producing layer's epilogue (csrc/spconv_cg.cu); "h2" = TMA gather4 + separate split kernel (csrc/spconv_h2.cu)
+    SPARSE_TC = "cg"          # tensor-core kernel of the Cin >= 32 layers: pair-proportional cp.async gather, planes written by the
+                              # producing layer's epilogue (csrc/spconv_cg.cu)
     ROWS_SHAPES = ((4, 16), (16, 16), (16, 32), (32, 32))     # (Cin, Cout) whose whole weight tensor fits in shared memory
     ROWS_MAX_CIN = 16         # layers with Cin <= this run on the pair-proportional SIMT kernel (0: tensor-core kernels wherever possible)
     DENSE_GATHER = True       # dense() as one gather pass through the last level's bitmap index (False: memset + scatter)
 
     def __init__(self, batch, max_voxels_total, input_shape_xyz=(1408, 1600, 40), num_input_features=4, device="cuda",
                  growth=None, use_tc=True, split=None, rows_max_cin=None, sparse_tc=None, keep_f32=False):
-        """use_tc: run the layers on the tcgen05 tensor cores; False = fp32 SIMT baseline for all layers.
-        split: "fp16" = TMA-gather two-term fp16 split kernel (spconv_h2.cu) for every layer with Cin >= 16 (13 of 14 layers);
-               "tf32" = 3xTF32 kernel with SIMT gather warps (spconv_tc.cu) for the Cin >= 32 layers.  Default: SPLIT."""
+        """use_tc: run the Cin >= 32 layers on the tensor cores (fp16 wgmma with a two-term fp16 split, csrc/spconv_cg.cu) and the
+        narrow layers on the pair-proportional SIMT kernel; False = fp32 SIMT baseline for all layers.  split / sparse_tc: "fp16" / "cg",
+        the only tensor-core variant."""
         self.batch, self.device = batch, torch.device(device)
         self.use_tc = bool(use_tc)
         self.split = split or self.SPLIT
-        assert self.split in ("fp16", "tf32")
-        self.use_h2 = self.use_tc and self.split == "fp16"
+        assert self.split == "fp16", "the sparse tensor-core layers use the two-term fp16 split"
+        self.use_h2 = self.use_tc
         self.sparse_tc = sparse_tc or self.SPARSE_TC
-        assert self.sparse_tc in ("cg", "h2")
+        assert self.sparse_tc == "cg"
         self.keep_f32 = bool(keep_f32)      # cg layers also write their fp32 rows (tests compare per-layer features)
-        # per-layer kernel: "rows" = pair-proportional fp32 SIMT (narrow layers), "h2" = TMA-gather fp16-split tcgen05, "tc" = 3xTF32
-        # tcgen05 with SIMT gather warps, "simt" = the dense output-stationary fp32 baseline
+        # per-layer kernel: "rows" = pair-proportional fp32 SIMT (narrow layers), "cg" = pair-proportional fp16-split wgmma,
+        # "simt" = the dense output-stationary fp32 baseline
         self.rows_max_cin = (self.ROWS_MAX_CIN if rows_max_cin is None else int(rows_max_cin)) if self.use_tc else 0
         self.cin0 = num_input_features
         shape = (int(input_shape_xyz[2]) + 1, int(input_shape_xyz[1]), int(input_shape_xyz[0]))   # scn.py:179
@@ -90,16 +90,15 @@ class SpMiddleRunner:
         for p in self.plan:
             if self.use_tc and p["cin"] <= self.rows_max_cin and (p["cin"], p["cout"]) in self.ROWS_SHAPES:
                 p["impl"] = "rows"
-            elif self.use_h2 and p["cin"] >= 32 and self.sparse_tc == "cg":
+            elif self.use_h2 and p["cin"] >= 32:
                 p["impl"] = "cg"
-            elif self.use_h2 and p["cin"] >= 16:
-                p["impl"] = "h2"
-            elif self.use_tc and p["cin"] >= 32:
-                p["impl"] = "tc"
             else:
                 p["impl"] = "simt"
+        for li, p in enumerate(self.plan):
+            # a cg layer reads the planes its producer's epilogue writes: the pair-proportional kernels write them, the baseline does not
+            assert p["impl"] != "cg" or self.plan[li - 1]["impl"] in ("rows", "cg"), "rows_max_cin too small for the tensor-core chain"
         for li, p in enumerate(self.plan[:-1]):
-            if self.plan[li + 1]["impl"] in ("h2", "cg"):
+            if self.plan[li + 1]["impl"] == "cg":
                 cp = 64 if p["cout"] > 32 else 32
                 self.planes[li] = ops.alloc_planes(self.levels[p["lout"]]["cap"], cp, self.device)
                 assert self.planes[li].shape[0] <= (1 << 25)
@@ -149,11 +148,9 @@ class SpMiddleRunner:
             sc, sh = fold_bn(*[torch.as_tensor(l[k], device=self.device) for k in ("gamma", "beta", "mean", "var")], eps=float(l.get("eps", BN_EPS)))
             wp = w.reshape(-1, p["cin"], p["cout"]).contiguous()
             tc = None
-            if p["impl"] in ("h2", "cg"):
-                tiles, inv = ops.pack_weight_sp_h2(wp, 64 if p["cin"] > 32 else 32, layout=p["impl"])
+            if p["impl"] == "cg":
+                tiles, inv = ops.pack_weight_sp_h2(wp, 64 if p["cin"] > 32 else 32, layout="cg")
                 tc = (p["impl"], tiles, (sc * inv).contiguous())
-            elif p["impl"] == "tc":
-                tc = ops.pack_weight_tc(wp, p["cout"])
             p["gain"], p["shift_max"] = ops.conv_gain(wp, sc), float(sh.abs().max())
             self.weights.append((wp, sc, sh, tc))
 
@@ -204,32 +201,21 @@ class SpMiddleRunner:
             elif p["impl"] == "rows":
                 need_amax = self.planes[li] is not None or (nxt == "rows" and li + 2 < len(self.plan) and self.plan[li + 2]["impl"] == "cg")
                 x = ops.spconv_forward_rows(x, p["nbr"], n_out, cap_out, w, sc, sh, True, self.feats[li],
-                                            (self.info[li, 0:1] if nxt != "h2" else self.amax[li:li + 1]) if need_amax else None)
+                                            self.info[li, 0:1] if need_amax else None)
             elif isinstance(tc, tuple) and tc[0] == "cg":
                 last = nxt != "cg"
                 ops.spconv_forward_cg(self.planes[li - 1], self.info[li - 1], p["tiles"], n_out, cap_out, tc[1], tc[2], sh, True, p["gain"],
                                       p["shift_max"], self.feats[li] if (last or self.keep_f32) else None,
                                       None if last else self.planes[li], self.info[li])
                 x = self.feats[li]
-            elif isinstance(tc, tuple):
-                # fp16-split tensor-core layer: reads the (hi, lo) planes of its input, writes fp32 rows + the output's abs-max
-                x = ops.spconv_forward_h2(self.planes[li - 1], self.amax[li - 1:li], p["nbr"], n_out, cap_out, tc[1], tc[2], sh, True,
-                                          self.feats[li], self.amax[li:li + 1])
-            elif tc is not None:
-                x = ops.spconv_forward_tc(x, p["nbr"], n_out, cap_out, tc, sc, sh, True, self.feats[li])
             else:
                 x = ops.spconv_forward(x, p["nbr"], n_out, cap_out, w, sc, sh, True, self.feats[li])
-                if self.planes[li] is not None:
-                    ops.absmax_rows(x, n_out, cap_out, self.amax[li:li + 1])
             mark("conv:%d" % li)
-            if self.planes[li] is not None and nxt == "h2":
-                ops.split_h2(x, n_out, cap_out, self.amax[li:li + 1], self.planes[li])
-                mark("split:%d" % li)
         last = self.levels[-1]
         if dense_planes is not None:
             assert last["index_kind"] == 1 and self.use_h2
-            amax_last = self.info[len(self.plan) - 1, 0:1] if self.plan[-1]["impl"] == "cg" else self.amax[len(self.plan) - 1:len(self.plan)]
-            out = ops.sparse_to_dense_planes(x, last["index"], last["grid"], amax_last, dense_planes[1], dense_planes[0])
+            assert self.plan[-1]["impl"] == "cg"
+            out = ops.sparse_to_dense_planes(x, last["index"], last["grid"], self.info[len(self.plan) - 1, 0:1], dense_planes[1], dense_planes[0])
             mark("dense")
             return out
         if last["index_kind"] == 1 and self.DENSE_GATHER:
@@ -281,20 +267,32 @@ class HeadRunner:
     """The fused head GEMM alone (MultiGroupHead.forward)."""
 
     def __init__(self, batch, hw, device="cuda", use_tc=True, stride=24):
+        """use_tc: the fp16-split tensor-core conv (csrc/bevconv_p2.cu; the fp32 input is split into planes first); False = fp32 SIMT."""
         self.batch, self.h, self.w, self.stride, self.use_tc = batch, int(hw[0]), int(hw[1]), stride, use_tc
         self.out = torch.zeros((batch, self.h, self.w, stride), dtype=torch.float32, device=device)
         self.device = torch.device(device)
         self.w_simt = self.w_tc = self.bias = None
+        if use_tc:
+            self.x_planes = ops.alloc_bev_planes(batch, self.h, self.w, 128, self.device)
+            self.info = torch.zeros((2, 2), dtype=torch.float32, device=self.device)     # {abs-max, scale} of the input / the output
 
     def load_state(self, head_sd, prefix=""):
         self.w_simt, self.bias = pack_head(head_sd, prefix, self.device, self.stride)
-        self.w_tc = ops.pack_weight_tc(self.w_simt, 32) if self.use_tc else None
+        if self.use_tc:
+            planes, inv = ops.pack_weight_h2(self.w_simt, 32)
+            gain = ops.conv_gain(self.w_simt, torch.ones(self.stride, device=self.device))
+            self.w_tc = (planes, inv[: self.stride].contiguous(), gain, float(self.bias.abs().max()))
 
     def forward(self, x):
         H = (self.h, self.w)
         d = ops.conv_desc(self.batch, H, 128, H, self.stride, H, [(0, 0)], relu=False)
         if self.w_tc is not None:
-            return ops.bev_conv_tc(x, self.w_tc, None, self.bias, None, self.out, d)
+            planes, scale, gain, shift_max = self.w_tc
+            self.info.zero_()
+            ops.absmax(x, self.info[0, 0:1])
+            ops.bev_split_planes(x, self.info[0], self.x_planes)
+            ops.bev_conv_p2(self.x_planes, self.info[0], planes, scale, self.bias, None, None, gain, shift_max, self.out, None, self.info[1], d)
+            return self.out
         return ops.bev_conv(x, self.w_simt, None, self.bias, None, self.out, d)
 
 
@@ -306,7 +304,7 @@ class SSFARunner:
     TC_STRIDE2 = True     # run the stride-2 conv through the strided-TMA tensor-core path as well
 
     def __init__(self, batch, hw=(200, 176), device="cuda", use_tc=True, split="fp16"):
-        """use_tc: tcgen05 tensor-core convs (default); False = the fp32 SIMT baseline kernels.
+        """use_tc: tensor-core convs (default); False = the fp32 SIMT baseline kernels.
         split: "fp16" = two-term fp16 split (kind::f16, bevconv_h2.cu; the stride-2 conv stays on the tf32 kernel),
                "tf32" = 3xTF32 everywhere (bevconv_tc.cu)."""
         self.batch, self.h, self.w, self.device = batch, int(hw[0]), int(hw[1]), torch.device(device)
@@ -452,9 +450,9 @@ class SSFARunner:
             self._conv(name, x, out, H, H, 128, 128, ai=3, ao=2)
 
         if (name + ":h2") in self.params:
-            kern = "bev_conv_h2_kernel (tcgen05 kind::f16, two-term fp16 split)"
+            kern = "bev_conv_p2_kernel<.., kP2SplitF16> (fp32 input split to fp16 in shared memory, fp16 wgmma)"
         elif (name + ":tc") in self.params:
-            kern = "bev_conv_tc3_kernel (tcgen05 3xTF32)"
+            kern = "bev_conv_p2_kernel<.., kP2SplitTf32> (3xTF32, tf32 wgmma)"
         else:
             kern = "bev_conv_kernel (fp32 SIMT)"
         return launch, kern
@@ -475,7 +473,7 @@ class SSFARunner:
 class SSFAPlanesRunner:
     """SSFA neck (rpn_v1.py:220-235) + the fused 128->22(+2 pad) head GEMM (mg_head_sessd.py:202-230) on csrc/bevconv_p2.cu:
     activations travel between the layers as fp16 (hi, lo) planes written by the producing epilogue (the main loops are pure
-    TMA -> tcgen05), weight tiles are multicast over CTA pairs.  14 launches per forward: 13 convs (the stride-2 conv included)
+    TMA -> wgmma).  14 launches per forward: 13 convs (the stride-2 conv included)
     + the attention fusion; + abs-max and split when the input arrives as fp32 (module API) instead of planes (FrameEngine)."""
 
     HEAD_STRIDE = 24
@@ -600,4 +598,4 @@ class SSFAPlanesRunner:
         def launch():
             self._conv(name, "x0", "b0b", H, H, 128, 128)
 
-        return launch, "bev_conv_p2_kernel (tcgen05 kind::f16 from pre-split fp16 planes, two-term split, CTA pairs: cta_group::2)"
+        return launch, "bev_conv_p2_kernel (fp16 wgmma from pre-split fp16 planes, two-term split)"

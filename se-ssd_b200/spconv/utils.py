@@ -3,8 +3,8 @@ boost-based CPU helpers of spconv 1.x).  They are not on the SE-SSD hot path; us
 
 
 def rbbox_iou(*args, **kwargs):
-    raise NotImplementedError("spconv.utils.rbbox_iou is not part of the B200 hot path; use det3d.core.iou3d.iou3d_utils.boxes_iou_bev_gpu")
+    raise NotImplementedError("spconv.utils.rbbox_iou is not part of the CUDA hot path; use det3d.core.iou3d.iou3d_utils.boxes_iou_bev_gpu")
 
 
 def rbbox_intersection(*args, **kwargs):
-    raise NotImplementedError("spconv.utils.rbbox_intersection is not part of the B200 hot path")
+    raise NotImplementedError("spconv.utils.rbbox_intersection is not part of the CUDA hot path")

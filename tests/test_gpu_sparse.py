@@ -91,11 +91,8 @@ def _weights(seed=3):
     return weights.split_detector_state(sd)
 
 
-@pytest.mark.parametrize("use_tc,split,rows,kw", [(False, None, 0, {}), (True, "tf32", 0, {}), (True, "fp16", 0, dict(sparse_tc="h2")),
-                                                  (True, "fp16", 32, dict(sparse_tc="h2")), (True, "fp16", 16, dict(sparse_tc="h2")),
-                                                  (True, "fp16", 16, dict(sparse_tc="cg", keep_f32=True)), (True, "fp16", 16, {})],
-                         ids=["simt", "tcgen05-3xtf32", "tma-gather-fp16x2", "rows32+tma-gather", "rows16+tma-gather",
-                              "rows16+pair-gather+f32rows", "rows16+pair-gather(default)"])
+@pytest.mark.parametrize("use_tc,split,rows,kw", [(False, None, 0, {}), (True, "fp16", 16, dict(sparse_tc="cg", keep_f32=True)), (True, "fp16", 16, {})],
+                         ids=["simt", "rows16+pair-gather+f32rows", "rows16+pair-gather(default)"])
 def test_spmiddle_features_match_fp64_oracle(use_tc, split, rows, kw):
     from oracle import spconv_ref as S
     from sessd_b200 import synth
@@ -146,7 +143,7 @@ def test_full_size_rulebook_symmetry_and_conv_properties():
     """Size-independent properties at the stress shape (4 frames x 200 k points, ~0.8 M voxels, up to 3 M active sites):
     * SubM rulebook symmetry: nbr[o][k] = i  <=>  nbr[i][26-k] = o, centre offset = identity, rows in range;
     * strided levels: output coordinates strictly ascending in linear index (canonical order), every output has >= 1 input;
-    * the three sparse-conv implementations agree layer by layer (<= 1e-5 of the layer maximum) and are run-to-run deterministic (bitwise);
+    * the tensor-core and the SIMT sparse-conv implementations agree layer by layer (<= 1e-5 of the layer maximum) and are run-to-run deterministic (bitwise);
     * dense(): the one-pass gather equals memset + scatter bitwise."""
     from sessd_b200 import ops
     from sessd_b200.runners import SpMiddleRunner
@@ -186,7 +183,7 @@ def test_full_size_rulebook_symmetry_and_conv_properties():
     for li, a in enumerate(feats1):
         assert torch.equal(a, r.layer_output(li))
     counts = [int((n0 if p["lout"] == 0 else r.levels[p["lout"]]["n"]).item()) for p in r.plan]
-    for kw in (dict(split="tf32", rows_max_cin=0), dict(use_tc=False)):
+    for kw in (dict(use_tc=False),):
         q = SpMiddleRunner(B, B * 200000, device="cuda", growth=(1.0, 8.0, 8.0, 8.0, 8.0), **kw)
         q.load_weights(_weights()[0])
         dq = q.forward(vox.mean, vox.coors, n0)
@@ -222,23 +219,9 @@ def test_h2_sparse_conv_power_of_two_scaling_is_exact():
     w = torch.randn((27, 64, 64), device="cuda") * 0.05
     tiles, inv = ops.pack_weight_sp_h2(w, 64)
     sc = (torch.rand(64, device="cuda") + 0.5) * inv
-    outs = []
-    for mul in (1.0, 4.0):
-        xx = (x * mul).contiguous()
-        planes = ops.alloc_planes(cap, 64, "cuda")
-        amax = torch.zeros(2, device="cuda")
-        ops.absmax_rows(xx, n, cap, amax[0:1])
-        ops.split_h2(xx, n, cap, amax[0:1], planes)
-        out = torch.zeros((cap, 64), device="cuda")
-        ops.spconv_forward_h2(planes, amax[0:1], p["nbr"], n, cap, tiles, sc.contiguous(), None, True, out, amax[1:2])
-        torch.cuda.synchronize()
-        outs.append((out, float(amax[1])))
     nn = int(n.item())
     assert nn > 100000
-    assert torch.equal(outs[0][0][:nn] * 4.0, outs[1][0][:nn])
-    assert outs[0][1] * 4.0 == outs[1][1]
-    # the pair-gather kernel (default): same property with the bound-derived scale, fp32 rows and plane outputs; and it agrees with the
-    # TMA-gather kernel to rounding
+    # the pair-gather kernel (default): the property holds with the bound-derived scale, for fp32 rows and plane outputs
     gain = ops.conv_gain(w, sc / inv)
     tl = ops.rulebook_tile_lists(p["nbr"], n, cap, ops.alloc_tile_lists(cap, 27, "cuda"))
     cg = []
@@ -263,7 +246,6 @@ def test_h2_sparse_conv_power_of_two_scaling_is_exact():
         cg.append((out, float(oinfo[0])))
     assert torch.equal(cg[0][0][:nn] * 4.0, cg[1][0][:nn])
     assert cg[0][1] * 4.0 == cg[1][1]
-    assert float((cg[0][0][:nn] - outs[0][0][:nn]).abs().max()) <= 2e-6 * float(outs[0][0][:nn].abs().max())
 
 
 # ---------------------------------------------------------------------------------------------------- BASELINE shapes (SURVEY 8d)
