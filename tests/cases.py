@@ -203,3 +203,24 @@ def consistency_case():
     stu = {k: np.stack([out[0][0][k], out[1][0][k]], 0) for k in out[0][0]}
     tea = {k: np.stack([out[0][1][k], out[1][1][k]], 0) for k in out[0][1]}
     return stu, tea, anc, trans
+
+
+def assert_tile_lists_match(rec, nbr, n):
+    """sessd_rulebook_tile_lists records (uint32 [tiles, 160 + 128 kvol]) vs a numpy regrouping of the neighbour table nbr [>= n, kvol]
+    for its first n rows: per tile of 128 rows the pair count of every offset (zero for offsets >= kvol), the 128-bit row mask of every
+    offset and the (input row << 7 | tile row) entries offset by offset in ascending tile row -- bit-exact."""
+    kvol = nbr.shape[1]
+    assert rec.dtype == np.uint32 and rec.shape[1] == 160 + 128 * kvol
+    for t in range(-(-n // 128)):
+        rows = nbr[t * 128:min(n, (t + 1) * 128)]
+        pos = 160
+        for k in range(kvol):
+            valid = np.nonzero(rows[:, k] >= 0)[0]
+            assert rec[t, k] == len(valid), (t, k)
+            mask = np.zeros(4, np.uint64)
+            np.add.at(mask, valid >> 5, np.uint64(1) << (valid & 31).astype(np.uint64))      # distinct bits: sum == or
+            assert np.array_equal(rec[t, 32 + 4 * k:36 + 4 * k], mask), (t, k)
+            want = (rows[valid, k].astype(np.uint32) << np.uint32(7)) | valid.astype(np.uint32)
+            assert np.array_equal(rec[t, pos:pos + len(valid)], want), (t, k)
+            pos += len(valid)
+        assert not rec[t, kvol:32].any()

@@ -331,6 +331,7 @@ def test_features_uniform20k_match_fp64_oracle():
 def test_tile_lists_regroup_the_neighbour_table_exactly():
     """sessd_rulebook_tile_lists (the rulebook format of the pair-gather conv) vs a numpy regrouping of the same nbr table: counts, row masks
     and the (input row << 7 | tile row) entries per offset in ascending tile row -- bit-exact, SubM (kvol 27) and the (3,1,1) layer (kvol 3)."""
+    from cases import assert_tile_lists_match
     from sessd_b200 import ops, synth
     r, _feat, coors, _layers, _dense = _frame_through_runner(synth.ring_cloud(3, 20000))
     for p in (r.plan[3], r.plan[6], r.plan[13]):
@@ -339,21 +340,4 @@ def test_tile_lists_regroup_the_neighbour_table_exactly():
         cap = p["nbr"].shape[0]
         tl = ops.rulebook_tile_lists(p["nbr"], r.levels[p["lout"]]["n"], cap, ops.alloc_tile_lists(cap, kvol, "cuda"))
         torch.cuda.synchronize()
-        nbr = p["nbr"][:n].cpu().numpy()
-        rec = tl.cpu().numpy().view(np.uint32)
-        stride = rec.shape[1]
-        assert stride == 160 + 128 * kvol
-        for t in range(-(-n // 128)):
-            rows = nbr[t * 128:(t + 1) * 128]
-            pos = 160
-            for k in range(kvol):
-                valid = np.nonzero(rows[:, k] >= 0)[0]
-                assert rec[t, k] == len(valid), (t, k)
-                mask = np.zeros(4, np.uint32)
-                for rr in valid:
-                    mask[rr >> 5] |= np.uint32(1) << np.uint32(rr & 31)
-                assert np.array_equal(rec[t, 32 + 4 * k:36 + 4 * k], mask), (t, k)
-                want = (rows[valid, k].astype(np.uint32) << np.uint32(7)) | valid.astype(np.uint32)
-                assert np.array_equal(rec[t, pos:pos + len(valid)], want), (t, k)
-                pos += len(valid)
-            assert not rec[t, kvol:32].any()
+        assert_tile_lists_match(tl.cpu().numpy().view(np.uint32), p["nbr"][:n].cpu().numpy(), n)
