@@ -199,11 +199,22 @@ int sessd_bev_conv(const float *d_in, const float *d_weight /*[ntaps, cin, cout]
  * this bound before it writes the first element.  Outputs: fp32 NHWC (d_out_f32) and / or planes (d_out_planes + d_out_info). */
 int sessd_bev_conv_p2(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                       const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
-                      float *d_out_f32, void *d_out_planes, float *d_out_info, const sessd_conv_desc *desc, void *stream);
+                      float *d_out_f32, void *d_out_planes, float *d_out_info, const sessd_conv_desc *desc, const int *d_items,
+                      void *stream);
 int sessd_bev_deconv_p2(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                         const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                         float *d_out_f32, void *d_out_planes, float *d_out_info, int batch, int in_h, int in_w, int cin, int cout,
-                        int relu, void *stream);
+                        int relu, const int *d_items, void *stream);
+/* Constant-region skipping of the SSFA neck + head (csrc/bevskip.cu).  Where the last sparse level has no site, dense() writes exact
+ * zeros; every neck pixel whose receptive field lies in that empty space (and inside the map) then holds, bit for bit, the same value
+ * as every other such pixel of its output-parity class.  sessd_bev_skip_plan derives from the level's bitmap index, per neck launch
+ * (SKIP_LAUNCHES order of runners.SSFAPlanesRunner), the work items that must run plus one representative of the skipped ones, all on
+ * the device.  The conv / deconv run the list (d_items = the launch's record); sessd_bev_skip_fill then copies the representative's
+ * output into the skipped tiles.  sessd_bev_skip_plan_words: int32 words of the plan of a [batch, h, w] neck; offsets[13] <- the
+ * word offset of every launch record. */
+long long sessd_bev_skip_plan_words(int batch, int h, int w, int *offsets);
+int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, int *d_plan, void *stream);
+int sessd_bev_skip_fill(const int *d_record, float *d_out_f32, void *d_out_planes, int cout, void *stream);
 /* fp32 [n] -> planes [2][n] scaled from d_info[0] (the tensor's abs-max, e.g. from sessd_absmax); writes the scale to d_info[1] */
 int sessd_bev_split_planes(const float *d_x, long long n, float *d_info, void *d_planes, void *stream);
 /* dense() (scn.py:184-187) straight into the planes the neck reads: d_amax = abs-max of the feature rows, d_info[2] <- {abs-max, S} */

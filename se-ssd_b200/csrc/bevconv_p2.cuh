@@ -36,6 +36,8 @@ constexpr int kP2MmaWarps = 8;
 constexpr int kP2PatchWarp = 8, kP2WeightWarp = 9;
 constexpr int kP2Threads = 320;                           // 10 warps
 constexpr int kP2MaxSmem = 227 * 1024;
+// optional device item list (bevskip.cu): int32 record, word 0 = number of items to run, the item indices from word kP2ItemsHeader on
+constexpr int kP2ItemsHeader = 32;
 // operand source of the A side: pre-split fp16 planes (TMA straight into the operand layout), or an fp32 NHWC input that TMA stages in
 // shared memory and the consumer warpgroups split there -- into fp16 (hi, lo) with the power-of-two scale of its abs-max (32-channel
 // chunks), or into tf32 hi = truncate(x), lo = x - hi for three tf32 products (16-channel chunks, fp32 weights [2][taps][cout_pad][cin])
@@ -67,7 +69,12 @@ struct P2Params {
     float gain, shift_max;             // bound of the output: amax_in * gain + shift_max (+ amax_resid)
     float *out_info;                   // [2] = {running abs-max of the output (atomicMax), S_out}
     long long out_plane_stride;        // elements between the hi and the lo plane of the output
+    const int *items;                  // nullable: run only the listed work items (count + indices, see kP2ItemsHeader), else all p.total
 };
+
+// number of work items this launch runs and the k-th of them (every warp role walks the same sequence)
+__device__ __forceinline__ int p2_item_count(const P2Params &p) { return p.items ? __ldg(p.items) : p.total; }
+__device__ __forceinline__ int p2_item(const P2Params &p, int k) { return p.items ? __ldg(p.items + kP2ItemsHeader + k) : k; }
 
 struct P2Item { int cls, n0, b, u0, v0, ntaps; };
 
@@ -156,6 +163,7 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
     if (threadIdx.x == kP2PatchWarp * 32) prefetch_tensormap(&map_a);    // descriptor fetches overlap barrier init
     if (threadIdx.x == kP2WeightWarp * 32) prefetch_tensormap(&map_b);
     const int nchunks = p.cin / p.chunk;
+    const int nitems = p2_item_count(p);
     const uint32_t b_plane_bytes = (uint32_t)p.n_tile * 64u;      // bytes of the b_hi (or b_lo) rows per (tap, chunk)
 
     if (threadIdx.x == 0) {
@@ -175,8 +183,8 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
         int pb = 0;
         uint32_t pph = 0;
         const uint32_t patches_u32 = smem_u32(patches);
-        for (int g = blockIdx.x; g < p.total; g += gridDim.x) {
-            const P2Item it = p2_decode(p, g);
+        for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
+            const P2Item it = p2_decode(p, p2_item(p, k));
             const int bu = it.u0 * p.in_stride, bv = it.v0 * p.in_stride;
             for (int cc = 0; cc < nchunks; ++cc) {
                 mbar_wait(&patch_empty[pb], pph ^ 1u);
@@ -204,8 +212,8 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
         // ===================== weight tiles: one [b_hi ; b_lo] stage per (item, chunk, tap) =====================
         int S = 0;
         uint32_t bph = 0;
-        for (int g = blockIdx.x; g < p.total; g += gridDim.x) {
-            const P2Item it = p2_decode(p, g);
+        for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
+            const P2Item it = p2_decode(p, p2_item(p, k));
             for (int cc = 0; cc < nchunks; ++cc)
                 for (int tap = 0; tap < it.ntaps; ++tap) {
                     mbar_wait(&b_empty[S], bph ^ 1u);
@@ -241,7 +249,8 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
         const int per_cls = p.nblocks * p.tiles;
         int S = 0, pb = 0;
         uint32_t bph = 0, pph = 0;
-        for (int g = blockIdx.x; g < p.total; g += gridDim.x) {
+        for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
+            const int g = p2_item(p, k);
             const int cls = p.cls_order[g / per_cls];
             const int ntaps = p.cls_ntaps[cls];
             const uint32_t *aoff = s_aoff + cls * 9;
@@ -525,7 +534,8 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
 template <int MODE>
 static int p2_conv(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                    const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
-                   float *d_out_f32, void *d_out_planes, float *d_out_info, const sessd_conv_desc *desc, void *stream) {
+                   float *d_out_f32, void *d_out_planes, float *d_out_info, const sessd_conv_desc *desc, void *stream,
+                   const int *d_items = nullptr) {
     if (!desc) return SESSD_EINVAL;
     const sessd_conv_desc &d = *desc;
     if (d.batch < 1 || d.ntaps < 1 || d.ntaps > 9 || (d.in_stride != 1 && d.in_stride != 2) || d.out_stride < 1 || d.grid_h < 1 || d.grid_w < 1)
@@ -535,6 +545,7 @@ static int p2_conv(const void *d_in_planes, const float *d_in_info, const void *
     p.batch = d.batch; p.cin = d.cin; p.cout = d.cout; p.in_stride = d.in_stride;
     p.out_h = d.out_h; p.out_w = d.out_w; p.out_stride = d.out_stride; p.relu = d.relu;
     p.nclass = 1;
+    p.items = d_items;
     P2Taps t = {};
     t.n = d.ntaps;
     for (int i = 0; i < d.ntaps; ++i) { t.dy[i] = d.tap_dy[i]; t.dx[i] = d.tap_dx[i]; t.w[i] = i; }
@@ -551,12 +562,13 @@ template <int MODE>
 static int p2_deconv(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                      const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                      float *d_out_f32, void *d_out_planes, float *d_out_info, int batch, int in_h, int in_w, int cin, int cout,
-                     int relu, void *stream) {
+                     int relu, void *stream, const int *d_items = nullptr) {
     if (batch < 1 || in_h < 1 || in_w < 1) return SESSD_EINVAL;
     P2Params p = {};
     p.batch = batch; p.cin = cin; p.cout = cout; p.in_stride = 1;
     p.out_h = 2 * in_h; p.out_w = 2 * in_w; p.out_stride = 2; p.relu = relu;
     p.nclass = 4;
+    p.items = d_items;
     P2Taps cls[4] = {};
     const int t_ux = div_up(in_w, kP2TileU) * div_up(in_h, kP2TileV), t_uy = div_up(in_h, kP2TileU) * div_up(in_w, kP2TileV);
     const bool u_is_x = t_ux <= t_uy;

@@ -1,0 +1,363 @@
+// bevskip.cu -- constant-region skipping for the SSFA neck + head (runners.SSFAPlanesRunner) on the bevconv_p2 kernel.
+//
+// dense() writes exact zeros wherever the last sparse level has no site.  Over a receptive field that lies entirely in that empty space
+// and inside the map (zero padding makes the border differ), a conv sees the same operands, in the same order, at every output pixel of
+// one parity class, so the kernel's result there is one value per class, bit for bit; the layers after it inherit this.  The neck's maps
+// have period 1 (conv chains from the empty input) or 2 (the deconv's output-parity classes and what follows them).
+//
+// sessd_bev_skip_plan (one launch of one CTA per batch) marks, per frame, every pixel of every neck output that may differ from its class
+// constant ("non-constant": an active BEV site, an out-of-map tap, a non-constant tap or residual) as bit maps in shared memory.  Then,
+// per neck launch:
+//   * every work-item tile that holds a non-constant pixel or leaves the map (partial tiles always run) is flagged;
+//   * the first all-constant tile of each class is its representative: it runs like any other item, so its abs-max enters out_info;
+//   * the work items to run are compacted in the launcher's own item order (class by descending tap count, n-block, tile);
+//   * the skipped (class, tile) pairs are listed.
+// sessd_bev_skip_fill copies, after the launch, the representative's pixel at the same tile position into every skipped pixel.  Tile
+// origins are multiples of 8 (u) and 16 (v) along the class grid, so that pixel has the same parity.
+#include "bevconv_p2.cuh"
+
+namespace sessd {
+
+// record header (int32 words; the item list starts at kP2ItemsHeader, where bev_conv_p2_kernel reads it)
+enum {
+    kRecCount = 0, kRecSkipped = 1, kRecNclass = 2, kRecTiles = 3, kRecTilesU = 4, kRecTilesV = 5, kRecUisX = 6, kRecOutStride = 7,
+    kRecOutH = 8, kRecOutW = 9, kRecBatch = 10, kRecOffY = 11, kRecOffX = 15, kRecRep = 19, kRecSkipOff = 23, kRecFlagOff = 24
+};
+
+// bit maps of the plan kernel: the neck input, every layer output (t0 = x0 and t1 = x1 pixel for pixel: 1x1 convs) and two scratch maps
+enum { kMX, kMB0a, kMB0b, kMX0, kMM0, kMM1, kMO0, kMO1, kMOut, kMTmp, kMB1a, kMB1b, kMX1, kMTmpH, kNumMaps };
+constexpr int kNumFullMaps = kMTmp + 1;
+constexpr int kSkipLaunches = 13;
+constexpr int kSkipThreads = 1024;
+
+struct SkipLaunch {
+    int map;                                   // bit map of the launch's output
+    int nclass, nblocks, tiles_u, tiles_v, tiles, u_is_x, grid_u, grid_v, out_stride, out_h, out_w;
+    int off_y[4], off_x[4], order[4];
+    int rec, cap_items;                        // word offset of the launch record; nclass * nblocks * tiles
+};
+
+struct SkipPlan {
+    int batch, depth, h, w, h2, w2, nwf, nwh;  // nwf / nwh: 32-bit words per row of a full / half resolution map
+    SkipLaunch l[kSkipLaunches];
+};
+
+// the launcher's geometry (launch_p2 / p2_conv / p2_deconv): orientation, tiles, n-blocks and heavy-first class order
+static void skip_launch(SkipLaunch &L, int map, int batch, int grid_h, int grid_w, int out_h, int out_w, int cout, bool deconv) {
+    L.map = map;
+    const int t_ux = div_up(grid_w, kP2TileU) * div_up(grid_h, kP2TileV), t_uy = div_up(grid_h, kP2TileU) * div_up(grid_w, kP2TileV);
+    L.u_is_x = t_ux <= t_uy ? 1 : 0;
+    L.grid_u = L.u_is_x ? grid_w : grid_h;
+    L.grid_v = L.u_is_x ? grid_h : grid_w;
+    L.tiles_u = div_up(L.grid_u, kP2TileU);
+    L.tiles_v = div_up(L.grid_v, kP2TileV);
+    L.tiles = L.tiles_u * L.tiles_v * batch;
+    const int n_tile = cout <= 32 ? 32 : 128;
+    L.nblocks = div_up(cout, n_tile);
+    L.nclass = deconv ? 4 : 1;
+    L.out_stride = deconv ? 2 : 1;
+    L.out_h = out_h; L.out_w = out_w;
+    int ntaps[4];
+    for (int c = 0; c < 4; ++c) {
+        L.off_y[c] = deconv ? c >> 1 : 0;
+        L.off_x[c] = deconv ? c & 1 : 0;
+        ntaps[c] = deconv ? (1 + (c >> 1)) * (1 + (c & 1)) : 9;
+        L.order[c] = c;
+    }
+    for (int i = 1; i < L.nclass; ++i)
+        for (int k = i; k > 0 && ntaps[L.order[k]] > ntaps[L.order[k - 1]]; --k) {
+            const int tmp = L.order[k]; L.order[k] = L.order[k - 1]; L.order[k - 1] = tmp;
+        }
+    L.cap_items = L.nclass * L.nblocks * L.tiles;
+}
+
+// the SSFAPlanesRunner launch sequence (runners.SSFAPlanesRunner.SKIP_LAUNCHES); returns the plan's int32 words, or 0
+static long long skip_plan(SkipPlan &P, int batch, int h, int w) {
+    if (batch < 1 || h < 4 || w < 4 || (h & 1) || (w & 1)) return 0;
+    P.batch = batch; P.h = h; P.w = w; P.h2 = h / 2; P.w2 = w / 2;
+    P.nwf = div_up(w, 32); P.nwh = div_up(P.w2, 32);
+    const int h2 = P.h2, w2 = P.w2;
+    SkipLaunch *L = P.l;
+    skip_launch(L[0], kMB0a, batch, h, w, h, w, 128, false);        // bottom_up_block_0.1
+    skip_launch(L[1], kMB0b, batch, h, w, h, w, 128, false);        // bottom_up_block_0.4
+    skip_launch(L[2], kMX0, batch, h, w, h, w, 128, false);         // bottom_up_block_0.7
+    skip_launch(L[3], kMB1a, batch, h2, w2, h2, w2, 256, false);    // bottom_up_block_1.0 (stride 2)
+    skip_launch(L[4], kMB1b, batch, h2, w2, h2, w2, 256, false);    // bottom_up_block_1.3
+    skip_launch(L[5], kMX1, batch, h2, w2, h2, w2, 256, false);     // bottom_up_block_1.6
+    skip_launch(L[6], kMX0, batch, h, w, h, w, 128, false);         // trans_0.0 (1x1)
+    skip_launch(L[7], kMX1, batch, h2, w2, h2, w2, 256, false);     // trans_1.0 (1x1)
+    skip_launch(L[8], kMM0, batch, h2, w2, h, w, 128, true);        // deconv_block_0.0 (+ t0)
+    skip_launch(L[9], kMM1, batch, h2, w2, h, w, 128, true);        // deconv_block_1.0
+    skip_launch(L[10], kMO0, batch, h, w, h, w, 128, false);        // conv_0.0
+    skip_launch(L[11], kMO1, batch, h, w, h, w, 128, false);        // conv_1.0
+    skip_launch(L[12], kMOut, batch, h, w, h, w, 24, false);        // head (1x1 on the fused map)
+    long long words = 0;
+    for (int i = 0; i < kSkipLaunches; ++i) {
+        L[i].rec = (int)words;
+        words += kP2ItemsHeader + L[i].cap_items + 2LL * L[i].nclass * L[i].tiles;
+    }
+    return words;
+}
+
+struct BitMap {
+    uint32_t *w;
+    int h, wd, nw;
+    __device__ __forceinline__ bool get(int y, int x) const { return (w[y * nw + (x >> 5)] >> (x & 31)) & 1u; }
+    __device__ __forceinline__ uint32_t valid(int i) const {
+        const int rem = wd - 32 * i;
+        return rem >= 32 ? ~0u : ((1u << rem) - 1u);
+    }
+};
+
+// out = the non-constant pixels of a 3x3 / pad 1 conv of `in` (out-of-map taps count as non-constant); out may alias in
+__device__ void skip_dilate3(const BitMap &in, const BitMap &tmp, const BitMap &out) {
+    const int n = in.h * in.nw, last = (in.wd - 1) >> 5;
+    for (int idx = threadIdx.x; idx < n; idx += blockDim.x) {
+        const int y = idx / in.nw, i = idx - y * in.nw;
+        const uint32_t *r = in.w + y * in.nw;
+        const uint32_t c = r[i], l = i > 0 ? r[i - 1] : 0u, rr = i + 1 < in.nw ? r[i + 1] : 0u;
+        uint32_t hv = c | (c << 1) | (l >> 31) | (c >> 1) | (rr << 31);
+        if (i == 0) hv |= 1u;
+        if (i == last) hv |= 1u << ((in.wd - 1) & 31);
+        tmp.w[idx] = hv & in.valid(i);
+    }
+    __syncthreads();
+    for (int idx = threadIdx.x; idx < n; idx += blockDim.x) {
+        const int y = idx / in.nw, i = idx - y * in.nw;
+        out.w[idx] = (y == 0 || y == in.h - 1) ? in.valid(i) : (tmp.w[idx - in.nw] | tmp.w[idx] | tmp.w[idx + in.nw]);
+    }
+    __syncthreads();
+}
+
+// out(y, x) = f(y, x), one warp per 32-pixel word
+template <class F>
+__device__ void skip_map_from(const BitMap &out, F f) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    for (int idx = warp; idx < out.h * out.nw; idx += nwarps) {
+        const int y = idx / out.nw, x = (idx - y * out.nw) * 32 + lane;
+        const unsigned bits = __ballot_sync(0xFFFFFFFFu, x < out.wd && f(y, x));
+        if (lane == 0) out.w[idx] = bits;
+    }
+    __syncthreads();
+}
+
+// n predicates -> the indices i with pred(i) at out[0..count), in ascending order; returns count (every thread)
+template <class Pred>
+__device__ int skip_compact(int n, Pred pred, int *out, int *s_scan) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    int base = 0;
+    for (int start = 0; start < n; start += blockDim.x) {
+        const int i = start + threadIdx.x;
+        const bool v = i < n && pred(i);
+        const unsigned bal = __ballot_sync(0xFFFFFFFFu, v);
+        if (lane == 0) s_scan[warp] = __popc(bal);
+        __syncthreads();
+        if (warp == 0) {
+            const int own = lane < nwarps ? s_scan[lane] : 0;
+            int x = own;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int y = __shfl_up_sync(0xFFFFFFFFu, x, o);
+                if (lane >= o) x += y;
+            }
+            if (lane < nwarps) s_scan[lane] = x - own;
+            if (lane == 31) s_scan[32] = x;
+        }
+        __syncthreads();
+        if (v) out[base + s_scan[warp] + __popc(bal & ((1u << lane) - 1u))] = i;
+        base += s_scan[32];
+        __syncthreads();
+    }
+    return base;
+}
+
+__global__ void __launch_bounds__(kSkipThreads) bev_skip_plan_kernel(const uint2 *__restrict__ bitmap, int *__restrict__ plan, SkipPlan P) {
+    extern __shared__ uint32_t s_bits[];
+    __shared__ int s_scan[33], s_rep[4];
+    BitMap m[kNumMaps];
+    {
+        uint32_t *p = s_bits;
+        for (int i = 0; i < kNumMaps; ++i) {
+            const bool full = i < kNumFullMaps;
+            m[i].w = p; m[i].h = full ? P.h : P.h2; m[i].wd = full ? P.w : P.w2; m[i].nw = full ? P.nwf : P.nwh;
+            p += m[i].h * m[i].nw;
+        }
+    }
+    for (int b = 0; b < P.batch; ++b) {
+        // the neck input: a BEV cell is non-constant when any of its z slices holds a site of the last sparse level
+        // (one thread per 32-pixel word: the bits of a row segment are one funnel shift of two bitmap words per slice, all loads independent)
+        const BitMap X = m[kMX];
+        for (int idx = threadIdx.x; idx < X.h * X.nw; idx += blockDim.x) {
+            const int y = idx / X.nw, i = idx - y * X.nw;
+            const int nbits = min(32, X.wd - 32 * i);
+            uint32_t acc = 0u;
+            for (int z = 0; z < P.depth; ++z) {
+                const unsigned long long lin = (((unsigned long long)b * P.depth + z) * P.h + y) * P.w + 32 * i;
+                const unsigned sh = (unsigned)(lin & 31);
+                const uint32_t lo = __ldg(&bitmap[lin >> 5]).x, hi = sh + nbits > 32 ? __ldg(&bitmap[(lin >> 5) + 1]).x : 0u;
+                acc |= __funnelshift_r(lo, hi, sh);
+            }
+            X.w[idx] = acc & X.valid(i);
+        }
+        __syncthreads();
+        skip_dilate3(m[kMX], m[kMTmp], m[kMB0a]);
+        skip_dilate3(m[kMB0a], m[kMTmp], m[kMB0b]);
+        skip_dilate3(m[kMB0b], m[kMTmp], m[kMX0]);
+        skip_dilate3(m[kMX0], m[kMTmp], m[kMX]);                       // stride 2: the 3x3 neighbourhood of (2y, 2x)
+        {
+            const BitMap D = m[kMX];
+            skip_map_from(m[kMB1a], [&](int y, int x) { return D.get(2 * y, 2 * x); });
+        }
+        skip_dilate3(m[kMB1a], m[kMTmpH], m[kMB1b]);
+        skip_dilate3(m[kMB1b], m[kMTmpH], m[kMX1]);
+        {   // deconv: out[2g + p] reads in[g] and, for p = 1, in[g + 1] (per axis); m0 adds the residual t0 (= x0's pixels)
+            const BitMap T = m[kMX1], R = m[kMX0];
+            auto tget = [&](int gy, int gx) { return gy >= T.h || gx >= T.wd || T.get(gy, gx); };
+            auto dc = [&](int oy, int ox) {
+                const int py = oy & 1, px = ox & 1, gy = oy >> 1, gx = ox >> 1;
+                return tget(gy, gx) || (py && tget(gy + 1, gx)) || (px && tget(gy, gx + 1)) || (py && px && tget(gy + 1, gx + 1));
+            };
+            skip_map_from(m[kMM0], [&](int y, int x) { return dc(y, x) || R.get(y, x); });
+            skip_map_from(m[kMM1], dc);
+        }
+        skip_dilate3(m[kMM0], m[kMTmp], m[kMO0]);
+        skip_dilate3(m[kMM1], m[kMTmp], m[kMO1]);
+        for (int i = threadIdx.x; i < P.h * P.nwf; i += blockDim.x) m[kMOut].w[i] = m[kMO0].w[i] | m[kMO1].w[i];
+        __syncthreads();
+        // per launch and class: flag the tiles of this frame that must run
+        for (int li = 0; li < kSkipLaunches; ++li) {
+            const SkipLaunch &L = P.l[li];
+            const BitMap &o = m[L.map];
+            int *flags = plan + L.rec + kP2ItemsHeader + L.cap_items + L.nclass * L.tiles;
+            const int per_frame = L.tiles_u * L.tiles_v;
+            for (int idx = threadIdx.x; idx < L.nclass * per_frame; idx += blockDim.x) {
+                const int c = idx / per_frame, tf = idx - c * per_frame;
+                const int tu = tf % L.tiles_u, tv = tf / L.tiles_u;
+                const int u0 = tu * kP2TileU, v0 = tv * kP2TileV;
+                bool run = u0 + kP2TileU > L.grid_u || v0 + kP2TileV > L.grid_v;      // partial tile
+                if (!run && L.out_stride == 1) {     // the tile is one aligned 8- or 16-bit field of 16 or 8 rows
+                    const int y0 = L.u_is_x ? v0 : u0, x0 = L.u_is_x ? u0 : v0;
+                    const int ny = L.u_is_x ? kP2TileV : kP2TileU, nx = L.u_is_x ? kP2TileU : kP2TileV;
+                    const uint32_t field = (1u << nx) - 1u;
+                    for (int y = y0; y < y0 + ny && !run; ++y) run = (o.w[y * o.nw + (x0 >> 5)] >> (x0 & 31)) & field;
+                } else if (!run) {
+                    for (int r = 0; r < kP2TileU * kP2TileV && !run; ++r) {
+                        const int gu = u0 + (r & 7), gv = v0 + (r >> 3);
+                        const int gy = L.u_is_x ? gv : gu, gx = L.u_is_x ? gu : gv;
+                        run = o.get(gy * L.out_stride + L.off_y[c], gx * L.out_stride + L.off_x[c]);
+                    }
+                }
+                flags[c * L.tiles + b * per_frame + tf] = run ? 1 : 0;
+            }
+        }
+        __syncthreads();
+    }
+    // per launch: representatives, the item list, the skipped list, the header
+    for (int li = 0; li < kSkipLaunches; ++li) {
+        const SkipLaunch &L = P.l[li];
+        int *rec = plan + L.rec;
+        int *items = rec + kP2ItemsHeader, *skipped = items + L.cap_items;
+        const int *flags = skipped + L.nclass * L.tiles;
+        if (threadIdx.x < 4) s_rep[threadIdx.x] = 0x7FFFFFFF;
+        __syncthreads();
+        for (int e = threadIdx.x; e < L.nclass * L.tiles; e += blockDim.x)
+            if (!flags[e]) atomicMin(&s_rep[e / L.tiles], e % L.tiles);
+        __syncthreads();
+        const int per_cls = L.nblocks * L.tiles;
+        const int count = skip_compact(L.cap_items, [&](int g) {
+            const int cls = L.order[g / per_cls], t = g % L.tiles;
+            return flags[cls * L.tiles + t] != 0 || t == s_rep[cls];
+        }, items, s_scan);
+        const int nskip = skip_compact(L.nclass * L.tiles, [&](int e) {
+            return flags[e] == 0 && e % L.tiles != s_rep[e / L.tiles];
+        }, skipped, s_scan);
+        if (threadIdx.x == 0) {
+            rec[kRecCount] = count; rec[kRecSkipped] = nskip;
+            rec[kRecNclass] = L.nclass; rec[kRecTiles] = L.tiles; rec[kRecTilesU] = L.tiles_u; rec[kRecTilesV] = L.tiles_v;
+            rec[kRecUisX] = L.u_is_x; rec[kRecOutStride] = L.out_stride; rec[kRecOutH] = L.out_h; rec[kRecOutW] = L.out_w;
+            rec[kRecBatch] = P.batch;
+            for (int c = 0; c < 4; ++c) {
+                rec[kRecOffY + c] = L.off_y[c]; rec[kRecOffX + c] = L.off_x[c];
+                rec[kRecRep + c] = c < L.nclass && s_rep[c] != 0x7FFFFFFF ? s_rep[c] : -1;
+            }
+            rec[kRecSkipOff] = kP2ItemsHeader + L.cap_items;
+            rec[kRecFlagOff] = kP2ItemsHeader + L.cap_items + L.nclass * L.tiles;
+        }
+        __syncthreads();
+    }
+}
+
+// every pixel of a skipped tile <- the pixel at the same tile position of its class's representative (fp32 and / or both planes)
+__global__ void __launch_bounds__(256) bev_skip_fill_kernel(const int *__restrict__ rec, float *__restrict__ out_f32,
+                                                            __half *__restrict__ out_planes, int cout) {
+    const int nskip = __ldg(rec + kRecSkipped);
+    if ((int)blockIdx.x >= nskip) return;
+    const int tiles = __ldg(rec + kRecTiles), tiles_u = __ldg(rec + kRecTilesU), tiles_v = __ldg(rec + kRecTilesV);
+    const int u_is_x = __ldg(rec + kRecUisX), os = __ldg(rec + kRecOutStride), out_h = __ldg(rec + kRecOutH), out_w = __ldg(rec + kRecOutW);
+    const long long plane_stride = (long long)__ldg(rec + kRecBatch) * out_h * out_w * cout;
+    const int *skipped = rec + __ldg(rec + kRecSkipOff);
+    for (int e = blockIdx.x; e < nskip; e += gridDim.x) {
+        const int ent = __ldg(skipped + e);
+        const int c = ent / tiles, t = ent - c * tiles, r = __ldg(rec + kRecRep + c);
+        const int oy0 = __ldg(rec + kRecOffY + c), ox0 = __ldg(rec + kRecOffX + c);
+        auto pixel = [&](int tt, int lu, int lv) -> size_t {
+            const int tu = tt % tiles_u, rest = tt / tiles_u, tv = rest % tiles_v, b = rest / tiles_v;
+            const int gu = tu * kP2TileU + lu, gv = tv * kP2TileV + lv;
+            const int gy = u_is_x ? gv : gu, gx = u_is_x ? gu : gv;
+            return ((size_t)b * out_h + (size_t)(gy * os + oy0)) * out_w + (size_t)(gx * os + ox0);
+        };
+        if (out_f32) {
+            const int q = cout / 4;
+            for (int i = threadIdx.x; i < kP2TileU * kP2TileV * q; i += blockDim.x) {
+                const int px = i / q, j = i - px * q;
+                const float4 v = reinterpret_cast<const float4 *>(out_f32 + pixel(r, px & 7, px >> 3) * cout)[j];
+                reinterpret_cast<float4 *>(out_f32 + pixel(t, px & 7, px >> 3) * cout)[j] = v;
+            }
+        }
+        if (out_planes) {
+            const int q = cout / 8, n = kP2TileU * kP2TileV * q;
+            for (int i = threadIdx.x; i < 2 * n; i += blockDim.x) {
+                const int pl = i / n, k = i - pl * n, px = k / q, j = k - px * q;
+                const __half *src = out_planes + pl * plane_stride + pixel(r, px & 7, px >> 3) * cout;
+                __half *dst = out_planes + pl * plane_stride + pixel(t, px & 7, px >> 3) * cout;
+                reinterpret_cast<uint4 *>(dst)[j] = reinterpret_cast<const uint4 *>(src)[j];
+            }
+        }
+    }
+}
+
+}  // namespace sessd
+
+using namespace sessd;
+
+extern "C" long long sessd_bev_skip_plan_words(int batch, int h, int w, int *offsets) {
+    SkipPlan P;
+    const long long words = skip_plan(P, batch, h, w);
+    if (words && offsets)
+        for (int i = 0; i < kSkipLaunches; ++i) offsets[i] = P.l[i].rec;
+    return words;
+}
+
+// d_bitmap_index: the last sparse level's bitmap index (grid = that level: shape = {D, h, w}); d_plan: sessd_bev_skip_plan_words(B, h, w)
+extern "C" int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, int *d_plan, void *stream) {
+    if (!d_bitmap_index || !d_plan || grid.shape[0] < 1) return SESSD_EINVAL;
+    SkipPlan P;
+    if (!skip_plan(P, grid.batch, grid.shape[1], grid.shape[2])) return SESSD_EINVAL;
+    P.depth = grid.shape[0];
+    const int smem = 4 * (kNumFullMaps * P.h * P.nwf + (kNumMaps - kNumFullMaps) * P.h2 * P.nwh);
+    if (smem > 200 * 1024) return SESSD_EINVAL;
+    static int attr_smem = 48 * 1024;     // opt in to what the maps need (the static shared memory counts against the same limit)
+    if (smem > attr_smem) {
+        SESSD_CUDA_TRY(cudaFuncSetAttribute(bev_skip_plan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        attr_smem = smem;
+    }
+    SESSD_LAUNCH(bev_skip_plan_kernel, 1, kSkipThreads, smem, (cudaStream_t)stream, (const uint2 *)d_bitmap_index, d_plan, P);
+    return last_error();
+}
+
+// after the launch that ran d_record's items: fill its skipped tiles in d_out_f32 [B][H][W][cout] and / or d_out_planes [2][B][H][W][cout]
+extern "C" int sessd_bev_skip_fill(const int *d_record, float *d_out_f32, void *d_out_planes, int cout, void *stream) {
+    if (!d_record || (!d_out_f32 && !d_out_planes) || cout < 8 || cout % 8) return SESSD_EINVAL;
+    SESSD_LAUNCH(bev_skip_fill_kernel, 2 * kNumSMs, 256, 0, (cudaStream_t)stream, d_record, d_out_f32, (__half *)d_out_planes, cout);
+    return last_error();
+}

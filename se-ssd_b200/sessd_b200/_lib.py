@@ -68,8 +68,11 @@ SIGNATURES = {
     "sessd_sparse_to_dense_indexed": (_i, [_vp, _i, _vp, _i, Grid, _vp, _vp]),
     "sessd_sparse_to_dense": (_i, [_vp, _vp, _vp, _i, _i, Grid, _vp, _vp]),
     "sessd_bev_conv": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp]),
-    "sessd_bev_conv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp]),
-    "sessd_bev_deconv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "sessd_bev_conv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp]),
+    "sessd_bev_deconv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "sessd_bev_skip_plan_words": (_ll, [_i, _i, _i, _I3]),
+    "sessd_bev_skip_plan": (_i, [_vp, Grid, _vp, _vp]),
+    "sessd_bev_skip_fill": (_i, [_vp, _vp, _vp, _i, _vp]),
     "sessd_bev_split_planes": (_i, [_vp, _ll, _vp, _vp, _vp]),
     "sessd_sparse_to_dense_planes": (_i, [_vp, _i, _vp, _i, Grid, _vp, _vp, _vp, _vp]),
     "sessd_ssfa_fuse_planes": (_i, [_vp, _vp, _vp, _vp, _f, _f, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -18,7 +18,9 @@ from .runners import SpMiddleRunner, SSFAPlanesRunner, SSFARunner
 class FrameEngine:
     def __init__(self, batch=1, max_points_per_frame=32768, voxel_size=synth.VOXEL_SIZE, pc_range=synth.PC_RANGE,
                  max_points_per_voxel=5, max_voxels=20000, device="cuda", post_kwargs=None, growth=None, use_tc=True, sparse_split=None, rows_max_cin=None,
-                 neck="planes", sparse_tc=None):
+                 neck="planes", sparse_tc=None, skip_constant=True):
+        """skip_constant: the planes neck computes only the tiles whose receptive field reaches a LiDAR site or the map border and fills
+        the rest with their bit-identical empty-space constant (runners.SSFAPlanesRunner)"""
         self.batch, self.device = int(batch), torch.device(device)
         self.max_points = int(max_points_per_frame) * self.batch
         self.vcfg = ops.make_voxel_cfg(voxel_size, pc_range, max_points_per_voxel, max_voxels)
@@ -34,7 +36,7 @@ class FrameEngine:
                                      sparse_tc=sparse_tc)
         self.neck_planes = neck == "planes" and use_tc
         if self.neck_planes:
-            self.neck = SSFAPlanesRunner(self.batch, (self.grid_xyz[1] // 8, self.grid_xyz[0] // 8), dev)
+            self.neck = SSFAPlanesRunner(self.batch, (self.grid_xyz[1] // 8, self.grid_xyz[0] // 8), dev, skip_constant=skip_constant)
         else:
             self.neck = SSFARunner(self.batch, (self.grid_xyz[1] // 8, self.grid_xyz[0] // 8), dev, use_tc=use_tc)
         self.anchors = None
@@ -77,7 +79,8 @@ class FrameEngine:
         if self.neck_planes:       # dense() writes the fp16 (hi, lo) planes of the neck input directly
             self.neck.info.zero_()
             self.middle.forward(self.vox.mean, self.vox.coors, n0, mark=mark, dense_planes=(self.neck.planes["x"], self.neck.info[0]))
-            _, head = self.neck.forward(None, mark=mark)
+            last = self.middle.levels[-1]
+            _, head = self.neck.forward(None, mark=mark, occupancy=(last["index"], last["grid"]))
         else:
             dense = self.middle.forward(self.vox.mean, self.vox.coors, n0, mark=mark)
             _, head = self.neck.forward(dense, mark=mark)

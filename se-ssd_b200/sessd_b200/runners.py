@@ -474,13 +474,19 @@ class SSFAPlanesRunner:
     """SSFA neck (rpn_v1.py:220-235) + the fused 128->22(+2 pad) head GEMM (mg_head_sessd.py:202-230) on csrc/bevconv_p2.cu:
     activations travel between the layers as fp16 (hi, lo) planes written by the producing epilogue (the main loops are pure
     TMA -> wgmma).  14 launches per forward: 13 convs (the stride-2 conv included)
-    + the attention fusion; + abs-max and split when the input arrives as fp32 (module API) instead of planes (FrameEngine)."""
+    + the attention fusion; + abs-max and split when the input arrives as fp32 (module API) instead of planes (FrameEngine).
+    With skip_constant and the sparse occupancy (FrameEngine): + one skip-plan launch and one fill launch after each conv / deconv."""
 
     HEAD_STRIDE = 24
     # info slots (each {abs-max, scale}); the whole table is zeroed once per forward
     SLOT = dict(x=0, b0a=1, b0b=2, x0=3, b1a=4, b1b=5, x1=6, t1=7, m0=8, m1=9, out=10, t0=11, o0=12, o1=13, head=14)
+    # the conv / deconv launches of one forward, in the order of the skip plan's records (csrc/bevskip.cu)
+    SKIP_LAUNCHES = ("bottom_up_block_0.1", "bottom_up_block_0.4", "bottom_up_block_0.7", "bottom_up_block_1.0", "bottom_up_block_1.3",
+                     "bottom_up_block_1.6", "trans_0.0", "trans_1.0", "deconv_block_0.0", "deconv_block_1.0", "conv_0.0", "conv_1.0", "head")
 
-    def __init__(self, batch, hw=(200, 176), device="cuda"):
+    def __init__(self, batch, hw=(200, 176), device="cuda", skip_constant=False):
+        """skip_constant: when forward() gets the occupancy of the last sparse level, run only the work items whose output can differ
+        from the empty-space constant of its class and fill the others with it (bit-identical to the dense neck, csrc/bevskip.cu)"""
         self.batch, self.h, self.w, self.device = batch, int(hw[0]), int(hw[1]), torch.device(device)
         h, w, h2, w2 = self.h, self.w, self.h // 2, self.w // 2
         pl = lambda hh, ww, c: ops.alloc_bev_planes(batch, hh, ww, c, self.device)     # noqa: E731
@@ -490,6 +496,8 @@ class SSFAPlanesRunner:
         self.buf = dict(t0=z(h, w, 128), o0=z(h, w, 128), o1=z(h, w, 128), out=z(h, w, 128), head=z(h, w, self.HEAD_STRIDE))
         self.info = torch.zeros((16, 2), dtype=torch.float32, device=self.device)
         self.params = None
+        self.skip_constant = bool(skip_constant)
+        self.skip = ops.BevSkipPlan(batch, h, w, self.device) if self.skip_constant else None
 
     def _info(self, name):
         return self.info[self.SLOT[name]]
@@ -528,22 +536,34 @@ class SSFAPlanesRunner:
                              gain=ops.conv_gain(hw, torch.ones(self.HEAD_STRIDE, device=dev)), shift_max=float(hb.abs().max()))
         self.params = P
 
-    def _conv(self, name, src, dst, in_hw, out_hw, cin, cout, stride=1, relu=True, f32=None):
-        """src: name of the input planes; dst: name of the output planes (or None); f32: name of an fp32 output buffer (or None)"""
+    def _conv(self, name, src, dst, in_hw, out_hw, cin, cout, stride=1, relu=True, f32=None, skip=False):
+        """src: name of the input planes; dst: name of the output planes (or None); f32: name of an fp32 output buffer (or None);
+        skip: run the work items of this launch's skip-plan record, then fill the skipped tiles"""
         q = self.params[name]
         d = ops.conv_desc(self.batch, in_hw, cin, out_hw, cout, out_hw, q["taps"], in_stride=stride, relu=relu)
         out_name = dst if dst is not None else f32
+        out_f32 = self.buf[f32] if f32 is not None else None
+        out_planes = self.planes[dst] if dst is not None else None
+        rec = self.skip.record(self.SKIP_LAUNCHES.index(name)) if skip else None
         ops.bev_conv_p2(self.planes[src], self._info(src), q["w"], q["scale"], q["shift"], None, None, q["gain"], q["shift_max"],
-                        self.buf[f32] if f32 is not None else None, self.planes[dst] if dst is not None else None, self._info(out_name), d)
+                        out_f32, out_planes, self._info(out_name), d, items=rec)
+        if skip:
+            self.skip.fill(self.SKIP_LAUNCHES.index(name), out_f32, out_planes, cout)
 
-    def _deconv(self, name, src, dst, residual=None):
+    def _deconv(self, name, src, dst, residual=None, skip=False):
         q = self.params[name]
+        rec = self.skip.record(self.SKIP_LAUNCHES.index(name)) if skip else None
         ops.bev_deconv_p2(self.planes[src], self._info(src), q["w"], q["scale"], q["shift"], self.buf[residual] if residual else None,
-                          self._info(residual) if residual else None, q["gain"], q["shift_max"], None, self.planes[dst], self._info(dst), True)
+                          self._info(residual) if residual else None, q["gain"], q["shift_max"], None, self.planes[dst], self._info(dst), True,
+                          items=rec)
+        if skip:
+            self.skip.fill(self.SKIP_LAUNCHES.index(name), None, self.planes[dst], self.planes[dst].shape[-1])
 
-    def forward(self, x=None, mark=None):
+    def forward(self, x=None, mark=None, occupancy=None):
         """x: NHWC fp32 [B,200,176,128] (converted to planes here) or None when self.planes['x'] / info slot 'x' were filled by the
-        producer (FrameEngine: dense() writes the planes directly).  Returns (neck out NHWC fp32, head NHWC fp32 [B,200,176,24])."""
+        producer (FrameEngine: dense() writes the planes directly).  Returns (neck out NHWC fp32, head NHWC fp32 [B,200,176,24]).
+        occupancy: (bitmap index, grid) of the last sparse level whose dense() made the input (FrameEngine); with skip_constant, the
+        launches then skip the tiles of the empty space (the input must be exactly zero wherever that level has no site)."""
         assert self.params is not None, "load_state first"
         mark = mark or (lambda label: None)
         H, H2 = (self.h, self.w), (self.h // 2, self.w // 2)
@@ -551,9 +571,15 @@ class SSFAPlanesRunner:
             self.info.zero_()
             ops.absmax(x, self.info[0, 0:1])
             ops.bev_split_planes(x, self.info[0], self.planes["x"])
+        skip = self.skip_constant and occupancy is not None
+        if skip:
+            index, grid = occupancy
+            assert (grid.batch, grid.shape[1], grid.shape[2]) == (self.batch, self.h, self.w), "occupancy of another map"
+            self.skip.build(index, grid)
+            mark("neck:skip_plan")
 
         def conv(name, *a, **kw):
-            self._conv(name, *a, **kw)
+            self._conv(name, *a, skip=skip, **kw)
             mark("neck:" + name)
 
         conv("bottom_up_block_0.1", "x", "b0a", H, H, 128, 128)
@@ -564,9 +590,9 @@ class SSFAPlanesRunner:
         conv("bottom_up_block_1.6", "b1b", "x1", H2, H2, 256, 256)
         conv("trans_0.0", "x0", None, H, H, 128, 128, f32="t0")
         conv("trans_1.0", "x1", "t1", H2, H2, 256, 256)
-        self._deconv("deconv_block_0.0", "t1", "m0", residual="t0")
+        self._deconv("deconv_block_0.0", "t1", "m0", residual="t0", skip=skip)
         mark("neck:deconv_block_0.0")
-        self._deconv("deconv_block_1.0", "t1", "m1")
+        self._deconv("deconv_block_1.0", "t1", "m1", skip=skip)
         mark("neck:deconv_block_1.0")
         conv("conv_0.0", "m0", None, H, H, 128, 128, f32="o0")
         conv("conv_1.0", "m1", None, H, H, 128, 128, f32="o1")
@@ -577,13 +603,13 @@ class SSFAPlanesRunner:
         if "head" not in self.params:
             mark("neck:fuse+head")
             return self.buf["out"], None
-        self.head()
+        self.head(skip=skip)
         mark("neck:fuse+head")
         return self.buf["out"], self.buf["head"]
 
-    def head(self):
+    def head(self, skip=False):
         H = (self.h, self.w)
-        self._conv("head", "out", None, H, H, 128, self.HEAD_STRIDE, relu=False, f32="head")
+        self._conv("head", "out", None, H, H, 128, self.HEAD_STRIDE, relu=False, f32="head", skip=skip)
         return self.buf["head"]
 
     def activation(self, name):
