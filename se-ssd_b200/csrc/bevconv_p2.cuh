@@ -30,7 +30,7 @@ namespace sessd {
 constexpr int kP2TileU = 8, kP2TileV = 16;
 constexpr int kP2MaxCopies = 6, kP2MaxRowsV = 18;
 constexpr int kP2BStages = 6, kP2MaxBStages = 12;
-constexpr int kP2BStageBytes = 2 * 128 * 64;              // [b_hi ; b_lo] planes, up to 128 rows of 64 B each
+constexpr int kP2BStageBytes = 2 * 128 * 64;              // [b_lo ; b_hi] planes, up to 128 rows of 64 B each
 constexpr int kP2BRing = kP2BStages * kP2BStageBytes;     // bytes of the weight-stage ring
 constexpr int kP2MmaWarps = 8;
 constexpr int kP2PatchWarp = 8, kP2WeightWarp = 9;
@@ -95,15 +95,45 @@ __device__ __forceinline__ P2Item p2_decode(const P2Params &p, int g) {
     return it;
 }
 
-template <int NT, int MODE>
+// N output columns: NT (one plane of the weight stage) or, fp16 only, 2 NT (the whole [b_lo ; b_hi] stage)
+template <int N, int MODE>
 __device__ __forceinline__ void p2_wgmma(float *d, uint64_t da, uint64_t db, uint32_t accumulate) {
     if constexpr (MODE == kP2SplitTf32) {
-        if constexpr (NT == 32) wgmma_tf32_n32(d, da, db, accumulate);
+        if constexpr (N == 32) wgmma_tf32_n32(d, da, db, accumulate);
         else wgmma_tf32_n128(d, da, db, accumulate);
     } else {
-        if constexpr (NT == 32) wgmma_f16_n32(d, da, db, accumulate);
-        else wgmma_f16_n128(d, da, db, accumulate);
+        if constexpr (N == 32) wgmma_f16_n32(d, da, db, accumulate);
+        else if constexpr (N == 64) wgmma_f16_n64(d, da, db, accumulate);
+        else if constexpr (N == 128) wgmma_f16_n128(d, da, db, accumulate);
+        else wgmma_f16_n256(d, da, db, accumulate);
     }
+}
+
+// 4 x 4 transpose of 2-float pairs inside each quad of lanes (q = lane & 3, the four lanes of one accumulator row): on entry pair g
+// is s[4 g], s[4 g + 1] = channels 8 g + 2 q, + 1 of a 32-channel block; on exit v[0..8) = channels 8 q .. 8 q + 7.  Two xor
+// exchanges, all lanes of the warp take part.
+__device__ __forceinline__ void p2_quad_transpose(const float *s, int q, float v[8]) {
+    const bool odd = q & 1, up = q & 2;
+    float a[2][2][2];      // [k][b][e]: pair of group (q & 1) + 2 k held by lane (q & ~1) | b
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const float even_g = s[4 * (2 * k) + e], odd_g = s[4 * (2 * k + 1) + e];
+            const float keep = odd ? odd_g : even_g;
+            const float recv = __shfl_xor_sync(0xFFFFFFFFu, odd ? even_g : odd_g, 1);
+            a[k][0][e] = odd ? recv : keep;
+            a[k][1][e] = odd ? keep : recv;
+        }
+#pragma unroll
+    for (int b = 0; b < 2; ++b)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const float keep = up ? a[1][b][e] : a[0][b][e];
+            const float recv = __shfl_xor_sync(0xFFFFFFFFu, up ? a[0][b][e] : a[1][b][e], 2);
+            v[2 * b + e] = up ? recv : keep;           // from lane b
+            v[2 * (2 + b) + e] = up ? keep : recv;     // from lane 2 + b
+        }
 }
 
 __device__ __forceinline__ float p2_tf32_rn(float x) {
@@ -209,7 +239,7 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
             }
         }
     } else if (warp == kP2WeightWarp) {
-        // ===================== weight tiles: one [b_hi ; b_lo] stage per (item, chunk, tap) =====================
+        // ===================== weight tiles: one [b_lo ; b_hi] stage per (item, chunk, tap) =====================
         int S = 0;
         uint32_t bph = 0;
         for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
@@ -221,8 +251,8 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
                         unsigned char *st = tiles + S * p.bstage_bytes;
                         const int wtap = p.tap_w[it.cls][tap];
                         mbar_expect_tx(&b_full[S], 2 * b_plane_bytes);
-                        tma_load_4d(st, &map_b, &b_full[S], cc * p.chunk, it.n0, wtap, 0);
-                        tma_load_4d(st + b_plane_bytes, &map_b, &b_full[S], cc * p.chunk, it.n0, wtap, 1);
+                        tma_load_4d(st + b_plane_bytes, &map_b, &b_full[S], cc * p.chunk, it.n0, wtap, 0);
+                        tma_load_4d(st, &map_b, &b_full[S], cc * p.chunk, it.n0, wtap, 1);
                     }
                     __syncwarp();
                     if (++S == p.bstages) { S = 0; bph ^= 1u; }
@@ -254,9 +284,12 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
             const int cls = p.cls_order[g / per_cls];
             const int ntaps = p.cls_ntaps[cls];
             const uint32_t *aoff = s_aoff + cls * 9;
-            float acc_m[kAcc], acc_c[kAcc], tot[MODE == kP2SplitTf32 ? kAcc : 1];
+            // acc[0, kAcc): cross a_hi x b_lo + a_lo x b_hi, acc[kAcc, NT): main a_hi x b_hi -- the fragment of an m64n(2 NT) over the
+            // whole [b_lo ; b_hi] weight stage.  The cross half comes first: ptxas serializes every wgmma of the kernel when one of them
+            // accumulates into a part of another's fragment that does not start at its first register.
+            float acc[NT], tot[MODE == kP2SplitTf32 ? kAcc : 1];
 #pragma unroll
-            for (int i = 0; i < kAcc; ++i) { acc_m[i] = 0.f; acc_c[i] = 0.f; }
+            for (int i = 0; i < NT; ++i) acc[i] = 0.f;
 #pragma unroll
             for (int i = 0; i < (MODE == kP2SplitTf32 ? kAcc : 1); ++i) tot[i] = 0.f;
             int prevS = -1, prev_pb = -1;
@@ -271,26 +304,33 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
                     mbar_wait(&b_full[S], bph);
                     if constexpr (MODE == kP2SplitTf32) {
                         // the weights' lo plane rounded to the nearest tf32 in place (the tensor core would truncate it)
-                        float *wl = reinterpret_cast<float *>(tiles + S * p.bstage_bytes + b_plane_bytes);
+                        float *wl = reinterpret_cast<float *>(tiles + S * p.bstage_bytes);
                         for (int i = threadIdx.x; i < (int)(b_plane_bytes / 4); i += kP2MmaWarps * 32) wl[i] = p2_tf32_rn(wl[i]);
                         asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
                         asm volatile("bar.sync 1, %0;\n" ::"n"(kP2MmaWarps * 32) : "memory");
                     }
                     const uint64_t da_hi = kDescSw64Hi | (uint64_t)(pbase + aoff[tap]);
                     const uint64_t da_lo = da_hi + (uint64_t)copy_lo;
-                    const uint64_t db_hi = kDescSw64Hi | (uint64_t)(tiles_lo + (uint32_t)(S * (p.bstage_bytes >> 4)));
-                    const uint64_t db_lo = db_hi + (uint64_t)plane_lo;
-                    const uint32_t acc = first ? 0u : 1u;
+                    const uint64_t db_lo = kDescSw64Hi | (uint64_t)(tiles_lo + (uint32_t)(S * (p.bstage_bytes >> 4)));
+                    const uint64_t db_hi = db_lo + (uint64_t)plane_lo;
+                    const uint32_t accum = first ? 0u : 1u;
                     // K = 16 fp16 / 8 tf32 per instruction = 32 bytes of the 64-byte row
                     wgmma_fence();
                     // tf32: the main accumulator restarts every chunk (its chunk partial is added into `tot` in RN fp32 below)
-                    const uint32_t acc_main = MODE == kP2SplitTf32 ? (tap != 0 ? 1u : 0u) : acc;
-                    p2_wgmma<NT, MODE>(acc_m, da_hi, db_hi, acc_main);       // main  (+)= a_hi x b_hi
-                    p2_wgmma<NT, MODE>(acc_m, da_hi + 2, db_hi + 2, 1u);
-                    p2_wgmma<NT, MODE>(acc_c, da_hi, db_lo, acc);            // cross (+)= a_hi x b_lo
-                    p2_wgmma<NT, MODE>(acc_c, da_hi + 2, db_lo + 2, 1u);
-                    p2_wgmma<NT, MODE>(acc_c, da_lo, db_hi, 1u);             // cross  += a_lo x b_hi
-                    p2_wgmma<NT, MODE>(acc_c, da_lo + 2, db_hi + 2, 1u);
+                    const uint32_t acc_main = MODE == kP2SplitTf32 ? (tap != 0 ? 1u : 0u) : accum;
+                    if constexpr (MODE == kP2Planes) {
+                        // one m64n(2 NT) per k16 over the stacked stage: cross (+)= a_hi x b_lo and main (+)= a_hi x b_hi read a_hi once.
+                        // Each accumulator sums in the order of the three-product sequence below (the lab modes' bitwise reference).
+                        p2_wgmma<2 * NT, MODE>(acc, da_hi, db_lo, accum);
+                        p2_wgmma<2 * NT, MODE>(acc, da_hi + 2, db_lo + 2, 1u);
+                    } else {
+                        p2_wgmma<NT, MODE>(acc + kAcc, da_hi, db_hi, acc_main);       // main  (+)= a_hi x b_hi
+                        p2_wgmma<NT, MODE>(acc + kAcc, da_hi + 2, db_hi + 2, 1u);
+                        p2_wgmma<NT, MODE>(acc, da_hi, db_lo, accum);                 // cross (+)= a_hi x b_lo
+                        p2_wgmma<NT, MODE>(acc, da_hi + 2, db_lo + 2, 1u);
+                    }
+                    p2_wgmma<NT, MODE>(acc, da_lo, db_hi, 1u);                        // cross  += a_lo x b_hi
+                    p2_wgmma<NT, MODE>(acc, da_lo + 2, db_hi + 2, 1u);
                     wgmma_commit();
                     first = false;
                     wgmma_wait<1>();                                         // the previous step's operands are no longer read
@@ -313,59 +353,101 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
                     }
                     prevS = prev_pb = -1;
                     if constexpr (MODE == kP2SplitTf32) {
-                        wgmma_fence_regs<kAcc>(acc_m);
+                        wgmma_fence_regs<kAcc>(acc + kAcc);
 #pragma unroll
-                        for (int i = 0; i < kAcc; ++i) tot[i] += acc_m[i];
+                        for (int i = 0; i < kAcc; ++i) tot[i] += acc[kAcc + i];
                     }
                 }
                 if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
             }
             wgmma_wait<0>();
-            wgmma_fence_regs<kAcc>(acc_m);
-            wgmma_fence_regs<kAcc>(acc_c);
+            wgmma_fence_regs<NT>(acc);
             if (lane == 0) {
                 if (prevS >= 0) mbar_arrive(&b_empty[prevS]);
                 if (prev_pb >= 0) mbar_arrive(&patch_empty[prev_pb]);
             }
-            // epilogue: this thread holds tile rows r0 and r0 + 8, two adjacent channels of every 8-channel group
+            // epilogue: this thread holds tile rows r0 and r0 + 8, two adjacent channels of every 8-channel group; a transpose inside
+            // each quad of lanes (one row) gives every lane 8 whole channels, stored 16 bytes at a time
+#pragma unroll
+            for (int i = 0; i < kAcc; ++i) acc[i] = (MODE == kP2SplitTf32 ? tot[i] : acc[kAcc + i]) + acc[i];      // main + cross
             const P2Item it = p2_decode(p, g);
+            const int q = lane & 3;
             const int r0 = wg * 64 + wq * 16 + (lane >> 2);
-            const int c2 = 2 * (lane & 3);
+            bool rows_ok[2];
+            size_t opixs[2];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int r = r0 + 8 * h;
                 const int lv = r / kP2TileU, lu = r % kP2TileU;
                 const int gu = it.u0 + lu, gv = it.v0 + lv;
-                if (it.b >= p.batch || gu >= p.grid_u || gv >= p.grid_v) continue;
+                rows_ok[h] = it.b < p.batch && gu < p.grid_u && gv < p.grid_v;      // the same in the four lanes of a quad
                 const int ou = gu * p.out_stride + p.cls_off_u[it.cls], ov = gv * p.out_stride + p.cls_off_v[it.cls];
                 const int oy = p.u_is_x ? ov : ou, ox = p.u_is_x ? ou : ov;
-                const size_t opix = ((size_t)it.b * p.out_h + (size_t)oy) * p.out_w + (size_t)ox;
+                opixs[h] = ((size_t)it.b * p.out_h + (size_t)oy) * p.out_w + (size_t)ox;
+            }
 #pragma unroll
-                for (int gi = 0; gi < NT / 8; ++gi) {
-                    const int n = it.n0 + 8 * gi + c2, i = 4 * gi + 2 * h;
-                    if (n >= p.cout) continue;                          // cout % 8 == 0: both channels of the pair exist or neither
-                    const float2 sc = scale ? __ldg(reinterpret_cast<const float2 *>(scale + n)) : make_float2(1.f, 1.f);
-                    const float2 sh = shift ? __ldg(reinterpret_cast<const float2 *>(shift + n)) : make_float2(0.f, 0.f);
-                    const float m0 = MODE == kP2SplitTf32 ? tot[i] : acc_m[i], m1 = MODE == kP2SplitTf32 ? tot[i + 1] : acc_m[i + 1];
-                    float o0 = fmaf((m0 + acc_c[i]) * inv_sa, sc.x, sh.x);
-                    float o1 = fmaf((m1 + acc_c[i + 1]) * inv_sa, sc.y, sh.y);
-                    if (p.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+            for (int j = 0; j < NT / 32; ++j)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const bool row_ok = rows_ok[h];
+                    const size_t opix = opixs[h];
+                    float v[8], o[8] = {};
+                    p2_quad_transpose(acc + 16 * j + 2 * h, q, v);
+                    const int n = it.n0 + 32 * j + 8 * q;      // this lane's 8 channels; cout % 8 == 0: all exist or none
                     const size_t off = opix * p.cout + n;
-                    if (resid) {
-                        const float2 rr = __ldg(reinterpret_cast<const float2 *>(resid + off));
-                        o0 += rr.x; o1 += rr.y;
+                    if (row_ok && n < p.cout) {
+                        float sc[8], sh[8];
+#pragma unroll
+                        for (int t = 0; t < 8; t += 4) {
+                            const float4 a = scale ? __ldg(reinterpret_cast<const float4 *>(scale + n + t)) : make_float4(1.f, 1.f, 1.f, 1.f);
+                            const float4 b = shift ? __ldg(reinterpret_cast<const float4 *>(shift + n + t)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                            sc[t] = a.x; sc[t + 1] = a.y; sc[t + 2] = a.z; sc[t + 3] = a.w;
+                            sh[t] = b.x; sh[t + 1] = b.y; sh[t + 2] = b.z; sh[t + 3] = b.w;
+                        }
+#pragma unroll
+                        for (int t = 0; t < 8; ++t) {
+                            o[t] = fmaf(v[t] * inv_sa, sc[t], sh[t]);
+                            if (p.relu) o[t] = fmaxf(o[t], 0.f);
+                        }
+                        if (resid) {
+#pragma unroll
+                            for (int t = 0; t < 8; t += 4) {
+                                const float4 rr = __ldg(reinterpret_cast<const float4 *>(resid + off + t));
+                                o[t] += rr.x; o[t + 1] += rr.y; o[t + 2] += rr.z; o[t + 3] += rr.w;
+                            }
+                        }
+#pragma unroll
+                        for (int t = 0; t < 8; ++t) vmax = fmaxf(vmax, fabsf(o[t]));
+                        if (out_planes) {
+                            __align__(16) __half2 hi[4], lo[4];
+#pragma unroll
+                            for (int t = 0; t < 4; ++t) {
+                                const float x0 = o[2 * t] * s_out, x1 = o[2 * t + 1] * s_out;
+                                hi[t] = __floats2half2_rn(x0, x1);
+                                const float2 f = __half22float2(hi[t]);
+                                lo[t] = __floats2half2_rn(x0 - f.x, x1 - f.y);
+                            }
+                            *reinterpret_cast<uint4 *>(out_planes + off) = *reinterpret_cast<const uint4 *>(hi);
+                            *reinterpret_cast<uint4 *>(out_planes + p.out_plane_stride + off) = *reinterpret_cast<const uint4 *>(lo);
+                        }
                     }
-                    vmax = fmaxf(vmax, fmaxf(fabsf(o0), fabsf(o1)));
-                    if (out_f32) *reinterpret_cast<float2 *>(out_f32 + off) = make_float2(o0, o1);
-                    if (out_planes) {
-                        const float x0 = o0 * s_out, x1 = o1 * s_out;
-                        const __half2 hi = __floats2half2_rn(x0, x1);
-                        const float2 f = __half22float2(hi);
-                        *reinterpret_cast<__half2 *>(out_planes + off) = hi;
-                        *reinterpret_cast<__half2 *>(out_planes + p.out_plane_stride + off) = __floats2half2_rn(x0 - f.x, x1 - f.y);
+                    if (out_f32) {
+                        // lanes q and q ^ 2 trade half groups, so that each of the two stores of a quad covers 16 whole channels
+                        // (groups 0-1, then 2-3 of the block): lane q keeps half (q >> 1) of group q, gets the same half of group q ^ 2
+                        const bool up = q & 2;
+                        float keep[4], recv[4];
+#pragma unroll
+                        for (int t = 0; t < 4; ++t) {
+                            keep[t] = up ? o[4 + t] : o[t];
+                            recv[t] = __shfl_xor_sync(0xFFFFFFFFu, up ? o[t] : o[4 + t], 2);
+                        }
+                        const int n_lo = it.n0 + 32 * j + 8 * (q & 1), c_lo = n_lo + 4 * (q >> 1);
+                        const float4 w_lo = up ? make_float4(recv[0], recv[1], recv[2], recv[3]) : make_float4(keep[0], keep[1], keep[2], keep[3]);
+                        const float4 w_hi = up ? make_float4(keep[0], keep[1], keep[2], keep[3]) : make_float4(recv[0], recv[1], recv[2], recv[3]);
+                        if (row_ok && n_lo < p.cout) *reinterpret_cast<float4 *>(out_f32 + opix * p.cout + c_lo) = w_lo;
+                        if (row_ok && n_lo + 16 < p.cout) *reinterpret_cast<float4 *>(out_f32 + opix * p.cout + c_lo + 16) = w_hi;
                     }
                 }
-            }
         }
         if (p.out_info) {
             const unsigned m = __reduce_max_sync(0xFFFFFFFFu, __float_as_uint(vmax));     // non-negative floats order like their bits
@@ -398,7 +480,10 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
     if (!d_in_planes || !d_w || (!d_out_f32 && !d_out_planes)) return SESSD_EINVAL;
     if (MODE == kP2Planes && (!d_in_info || !d_scale)) return SESSD_EINVAL;
     if (MODE != kP2Planes && d_out_planes) return SESSD_EINVAL;
-    if (p.cin < 64 || p.cin % 64 || p.cout < 8 || p.cout % 8) return SESSD_EINVAL;      // whole 64-channel groups; 8-byte stores
+    if (p.cin < 64 || p.cin % 64 || p.cout < 8 || p.cout % 8) return SESSD_EINVAL;      // whole 64-channel groups; 8-channel stores
+    // the epilogue reads and writes 16 bytes at a time
+    if (((uintptr_t)d_scale | (uintptr_t)d_shift | (uintptr_t)d_residual | (uintptr_t)d_out_f32 | (uintptr_t)d_out_planes) & 15)
+        return SESSD_EINVAL;
     const int n_tile = p.cout <= 32 ? 32 : 128;
     if (cout_pad % n_tile || cout_pad < p.cout) return SESSD_EINVAL;
     // orientation: the in-group dimension u has the 8-pixel tile edge; pick the mapping with fewer tiles
