@@ -279,7 +279,9 @@ int sessd_postprocess_packed(const float *d_head, const float *d_anchors, const 
                              const int *d_status, void *workspace, size_t workspace_bytes, void *stream);
 
 /* stand-alone rotated NMS on [n,5] (x,y,w,l,r) + scores: box_torch_ops.rotate_nms semantics
- * (top-k pre_max by score, greedy, keep <= post_max); d_keep [post_max] i32 indices into the input */
+ * (top-k pre_max by score, greedy, keep <= post_max); d_keep [post_max] i32 indices into the input.
+ * Scores may have either sign and are ordered as floats, -0 == +0; equal scores keep the lower index first.
+ * NaN / Inf scores are out of scope. */
 size_t sessd_rotate_nms_workspace_bytes(int max_boxes, int pre_max);
 int sessd_rotate_nms(const float *d_boxes5, const float *d_scores, const int *d_n, int max_boxes, int pre_max,
                      int post_max, float iou_thresh, int ge, int *d_keep, int *d_num_keep, void *workspace,

@@ -70,6 +70,15 @@ __device__ __forceinline__ unsigned long long make_key(float score, int idx) {
     if (sb & 0x80000000u) sb = 0;   // -0 / negative garbage sorts last
     return ((unsigned long long)sb << 32) | (unsigned int)(0xFFFFFFFFu - (unsigned int)idx);
 }
+// stand-alone NMS: scores of any sign (raw logits, say). The high word is the float's bits mapped monotonically onto unsigned:
+// non-negative floats set the sign bit, negative ones flip every bit; -0 counts as +0 so that the two tie and fall back to index
+// order. Order-preserving over all finite floats; NaN / Inf scores are out of scope. key_score() does not apply to these keys.
+__device__ __forceinline__ unsigned long long make_key_signed(float score, int idx) {
+    unsigned int sb = __float_as_uint(score);
+    if (sb == 0x80000000u) sb = 0u;
+    sb = (sb & 0x80000000u) ? ~sb : (sb | 0x80000000u);
+    return ((unsigned long long)sb << 32) | (unsigned int)(0xFFFFFFFFu - (unsigned int)idx);
+}
 __device__ __forceinline__ int key_index(unsigned long long k) { return (int)(0xFFFFFFFFu - (unsigned int)(k & 0xFFFFFFFFull)); }
 __device__ __forceinline__ float key_score(unsigned long long k) { return __uint_as_float((unsigned int)(k >> 32)); }
 
@@ -115,7 +124,7 @@ __global__ void __launch_bounds__(256) post_score_kernel(const float *__restrict
 __global__ void __launch_bounds__(256) keys_from_scores_kernel(const float *__restrict__ scores, const int *__restrict__ d_n,
                                                                int max_n, unsigned long long *__restrict__ cand, int *__restrict__ ncand) {
     const int n = min(*d_n, max_n);
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) cand[i] = make_key(scores[i], i);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) cand[i] = make_key_signed(scores[i], i);
     if (blockIdx.x == 0 && threadIdx.x == 0) *ncand = n;
 }
 
