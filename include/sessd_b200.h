@@ -136,7 +136,7 @@ int sessd_sparse_to_dense_indexed(const float *d_feat, int max_rows, const void 
 
 /* S4, narrow layers (Cin <= 32; csrc/spconv_rows.cu): same contract and arguments as sessd_spconv_forward, fp32 SIMT, but the work is
  * proportional to the number of rulebook PAIRS instead of N_out x kvol row slots (a warp owns 8 output rows and visits only their valid
- * neighbours).  d_amax_out (nullable) receives the running abs-max of the output.  (Cin, Cout): (4,16) (16,16) (16,32) (32,32) (32,64). */
+ * neighbours).  d_amax_out (nullable) receives the running abs-max of the output.  (Cin, Cout): (4,16) (16,16) (16,32) (32,16) (32,32). */
 int sessd_spconv_forward_rows(const float *d_in_feat, int cin, const int *d_nbr, int kvol, const int *d_n_out, int max_out,
                               const float *d_weight, int cout, const float *d_scale, const float *d_shift, int relu,
                               float *d_out_feat, float *d_amax_out, void *stream);
@@ -155,7 +155,7 @@ int sessd_spconv_forward_rows_planes(const float *d_in_feat, int cin, const int 
  * The rulebook is passed as d_tiles = the per-tile pair lists sessd_rulebook_tile_lists() makes from the nbr table (once per rulebook).
  * d_in_planes [plane_rows][2][cp] fp16, x = (hi + lo) / d_in_info[1], d_in_info[0] = abs-max of the input tensor; outputs (each nullable, at
  * least one): fp32 rows [max_out][cout]; planes [>= max_out][2][cout <= 32 ? 32 : 64] with d_out_info = {abs-max of the output (atomicMax; zero
- * it once per frame), S_out}, S_out from the bound d_in_info[0] * gain + shift_max as above.  Supported (cp, cout): (32,32) (32,64) (64,64). */
+ * it once per frame), S_out}, S_out from the bound d_in_info[0] * gain + shift_max as above.  Supported (cp, cout): (32,32) (32,64) (64,32) (64,64). */
 int sessd_spconv_forward_cg(const void *d_in_planes, int cp, int plane_rows, const float *d_in_info, const void *d_tiles, int kvol,
                             const int *d_n_out, int max_out, const void *d_weight_h2, int cout, const float *d_scale, const float *d_shift,
                             int relu, float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, void *stream);
@@ -163,6 +163,33 @@ int sessd_spconv_forward_cg(const void *d_in_planes, int cp, int plane_rows, con
 void sessd_set_sp_cg_deep(int on);
 /* *d_amax = max(*d_amax, max |d_feat[i]|) over the first *d_n rows of a [max_rows, channels] fp32 tensor */
 int sessd_absmax_rows(const float *d_feat, const int *d_n, int max_rows, int channels, float *d_amax, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Backward of the sparse convs (csrc/spconv_grad.cu; training of SpMiddleFHD).  The data gradient is the forward kernels run with
+ * re-packed weights over the same table (SubM: W'[k] = W[K-1-k]^T) or over the transposed table (strided: W[k]^T); the weight gradient
+ * gW[k] = sum over the pairs of offset k of in[i]^T gout[o] reads the forward rulebook's tile lists.
+ * ------------------------------------------------------------------------------------------------ */
+/* nbr [max_out, kvol] -> nbr_t [max_in, kvol]: nbr_t[i, k] = o where nbr[o, k] = i (o < *d_n_out), else -1 (every row of nbr_t is written) */
+int sessd_rulebook_transpose(const int *d_nbr, int kvol, const int *d_n_out, int max_out, int max_in, int *d_nbr_t, void *stream);
+/* fp32 rows [max_rows, channels] -> fp16 (hi, lo) planes [rows][2][cp] at S = the power of two that maps d_info[0] (the abs-max of the
+ * tensor, sessd_absmax_rows) into [2^14, 2^15); d_info[1] <- S.  Rows >= *d_n are untouched; channels [channels, cp) are written as zero. */
+int sessd_sparse_split_planes(const float *d_x, const int *d_n, int max_rows, int channels, float *d_info, void *d_planes, int cp, void *stream);
+/* adjoint of sessd_sparse_to_dense: d_out[r][c] = d_grad[b, y, x, c*D + z] for (b, z, y, x) = d_coors[r], r < *d_n */
+int sessd_dense_grad_gather(const float *d_grad, const int *d_coors, const int *d_n, int max_rows, int channels, sessd_grid grid,
+                            float *d_out, void *stream);
+/* weight gradient: work items (offset, fixed range of tiles) -- sessd_spconv_wgrad_items(max_out, kvol) of them, a function of the
+ * arguments only -- each write an fp32 partial [Cin][Cout] to the workspace; a reduce sums the partials of every offset in ascending item
+ * order: bitwise run-to-run deterministic, no float atomics.  d_gw [kvol][Cin][Cout] fp32.  _items: SESSD_EINVAL on invalid arguments. */
+int sessd_spconv_wgrad_items(int max_out, int kvol);
+size_t sessd_spconv_wgrad_workspace_bytes(int max_out, int kvol, int cin, int cout);
+/* Cin <= 16 (fp32 SIMT): d_in_feat [*, cin] fp32, d_gout [max_out, cout] fp32.  (Cin, Cout): (4,16) (16,16) (16,32). */
+int sessd_spconv_wgrad_rows(const float *d_in_feat, int cin, const float *d_gout, int cout, const void *d_tiles, int kvol,
+                            const int *d_n_out, int max_out, float *d_gw, void *d_ws, size_t ws_bytes, void *stream);
+/* Cin >= 32 (tensor cores, fp16 mma with the three-product split): d_in_planes [*][2][cp] with d_in_info = {abs-max, S_in}, d_g_planes
+ * [max_out][2][cout] with d_g_info = {abs-max, S_g} (sessd_sparse_split_planes); gW = sum / S_in / S_g.  (cp, cout): (32,32) (32,64) (64,64). */
+int sessd_spconv_wgrad_cg(const void *d_in_planes, int cp, const float *d_in_info, const void *d_g_planes, int cout, const float *d_g_info,
+                          const void *d_tiles, int kvol, const int *d_n_out, int max_out, float *d_gw, void *d_ws, size_t ws_bytes,
+                          void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * N1/H1: BEV neck (SSFA) + head.  Replaces the cuDNN conv/deconv + BatchNorm2d + ReLU blocks of

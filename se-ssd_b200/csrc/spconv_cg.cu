@@ -375,7 +375,7 @@ extern "C" void sessd_set_sp_cg_deep(int on) { sessd::g_cg_deep = on ? 1 : 0; }
 // weights / d_scale from ops.pack_weight_sp_h2 (cp = 64: [kvol][2][Cout][64], cp = 32: [kvol][2][Cout][32]; d_scale = BN scale *
 // 2^-e[c]); gain / shift_max bound the output (see the header).  Outputs (each nullable, at least one): fp32 rows [max_out][cout],
 // planes [>= max_out][2][cout <= 32 ? 32 : 64] + d_out_info = {abs-max (zero it once per frame), scale}.
-// Supported (cp, cout): (32,32), (32,64), (64,64).
+// Supported (cp, cout): (32,32), (32,64), (64,32), (64,64).
 extern "C" int sessd_spconv_forward_cg(const void *d_in_planes, int cp, int plane_rows, const float *d_in_info, const void *d_tiles, int kvol,
                                        const int *d_n_out, int max_out, const void *d_weight_h2, int cout, const float *d_scale,
                                        const float *d_shift, int relu, float gain, float shift_max, float *d_out_f32, void *d_out_planes,
@@ -393,6 +393,7 @@ extern "C" int sessd_spconv_forward_cg(const void *d_in_planes, int cp, int plan
     if (cp == CPV && cout == CO) return g_cg_deep ? launch_spconv_cg<CPV, CO, 1>(a, d_weight_h2, st) : launch_spconv_cg<CPV, CO, 0>(a, d_weight_h2, st);
     SESSD_CG_CASE(32, 32)
     SESSD_CG_CASE(32, 64)
+    SESSD_CG_CASE(64, 32)     // data gradient of the 32 -> 64 strided layer
     SESSD_CG_CASE(64, 64)
 #undef SESSD_CG_CASE
     return SESSD_EINVAL;

@@ -221,13 +221,14 @@ static int rows_dispatch(const float *d_in_feat, int cin, const int *d_nbr, int 
     RW_CASE(4, 16);
     RW_CASE(16, 16);
     RW_CASE(16, 32);
+    RW_CASE(32, 16);     // data gradient of the 16 -> 32 strided layer
     RW_CASE(32, 32);
 #undef RW_CASE
     return SESSD_EINVAL;
 }
 
 // Same arguments as sessd_spconv_forward plus d_amax_out (nullable): running abs-max of the output.  Supported (Cin, Cout): (4,16),
-// (16,16), (16,32), (32,32) -- the whole weight tensor must fit in shared memory.
+// (16,16), (16,32), (32,16), (32,32) -- the whole weight tensor must fit in shared memory.
 extern "C" int sessd_spconv_forward_rows(const float *d_in_feat, int cin, const int *d_nbr, int kvol, const int *d_n_out, int max_out,
                                          const float *d_weight, int cout, const float *d_scale, const float *d_shift, int relu,
                                          float *d_out_feat, float *d_amax_out, void *stream) {

@@ -4,13 +4,16 @@ Same constructor, parameters and state-dict keys (``middle_conv.{0,3,...}.weight
 ``middle_conv.{1,4,...}`` BatchNorm1d) so reference checkpoints load.  ``forward`` runs the fused CUDA pipeline
 (sessd_b200.runners.SpMiddleRunner): 8 deterministic rulebooks + 14 gather-GEMM launches with BN+ReLU in the epilogue + dense
 scatter, and returns the [B, 128, 200, 176] BEV tensor in channels-last memory (logically NCHW, like the reference's
-``ret.view(N, C*D, H, W)``)."""
+``ret.view(N, C*D, H, W)``).  In ``.train()`` it runs the reference's own forward instead -- ``middle_conv`` layer by layer with the
+convs differentiable on the same kernels (sessd_b200.sparse_grad), BatchNorm1d with batch statistics -- and returns the same tensor with
+an autograd graph down to every conv weight and BN parameter."""
 import numpy as np
 import spconv
 import torch
 from spconv import SparseConv3d, SubMConv3d
 from torch import nn
 
+from sessd_b200 import sparse_grad
 from sessd_b200.runners import SPMIDDLE_LAYERS, SpMiddleRunner
 
 from ..registry import BACKBONES
@@ -53,9 +56,16 @@ class SpMiddleFHD(nn.Module):
                             mean=bn.running_mean, var=bn.running_var, eps=float(bn.eps)))
         return out
 
+    def forward_train(self, voxel_features, coors, batch_size, input_shape):
+        """scn.py:176-189 with batch-statistics BatchNorm (the module's train mode; also the SE-SSD teacher's no-grad forward)"""
+        sparse_shape = [int(v) for v in np.array(input_shape).reshape(-1)[:3][::-1] + np.array([1, 0, 0])]
+        ret = spconv.SparseConvTensor(voxel_features.float().contiguous(), coors.int().contiguous(), sparse_shape, int(batch_size))
+        ret = sparse_grad.encoder_forward(self.middle_conv, ret)
+        return sparse_grad.dense(ret)                                     # [N, C*D, H, W], channels-last memory
+
     def forward(self, voxel_features, coors, batch_size, input_shape):
         if self.training:
-            raise NotImplementedError("SpMiddleFHD: only the inference path is built (call .eval()); training is a 'next' row")
+            return self.forward_train(voxel_features, coors, batch_size, input_shape)
         grid_xyz = [int(v) for v in np.array(input_shape).reshape(-1)[:3]]
         coors = coors.int().contiguous()
         n = int(coors.shape[0])

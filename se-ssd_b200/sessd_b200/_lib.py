@@ -65,6 +65,13 @@ SIGNATURES = {
     "sessd_spconv_forward_cg": (_i, [_vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _f, _f, _vp, _vp, _vp, _vp]),
     "sessd_set_sp_cg_deep": (None, [_i]),
     "sessd_absmax_rows": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
+    "sessd_rulebook_transpose": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp]),
+    "sessd_sparse_split_planes": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _vp]),
+    "sessd_dense_grad_gather": (_i, [_vp, _vp, _vp, _i, _i, Grid, _vp, _vp]),
+    "sessd_spconv_wgrad_items": (_i, [_i, _i]),
+    "sessd_spconv_wgrad_workspace_bytes": (_sz, [_i, _i, _i, _i]),
+    "sessd_spconv_wgrad_rows": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
+    "sessd_spconv_wgrad_cg": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
     "sessd_sparse_to_dense_indexed": (_i, [_vp, _i, _vp, _i, Grid, _vp, _vp]),
     "sessd_sparse_to_dense": (_i, [_vp, _vp, _vp, _i, _i, Grid, _vp, _vp]),
     "sessd_bev_conv": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp]),

@@ -244,6 +244,66 @@ def set_sp_cg_deep(on):
     lib.sessd_set_sp_cg_deep(int(on))
 
 
+# ---- backward of the sparse convs (csrc/spconv_grad.cu) -------------------------------------------------------------------------
+def rulebook_transpose(nbr, n_out, max_out, max_in, nbr_t=None):
+    """nbr [max_out, kvol] -> nbr_t [max_in, kvol]: nbr_t[i, k] = o where nbr[o, k] = i, else -1 (strided layers' data gradient)"""
+    kvol = int(nbr.shape[1])
+    if nbr_t is None:
+        nbr_t = torch.empty((int(max_in), kvol), dtype=torch.int32, device=nbr.device)
+    check(lib.sessd_rulebook_transpose(_p(nbr), kvol, _p(n_out), int(max_out), int(max_in), _p(nbr_t), _st()), "sessd_rulebook_transpose")
+    return nbr_t
+
+
+def sparse_split_planes(x, n, max_rows, info, planes):
+    """fp32 rows [max_rows, C] -> fp16 (hi, lo) planes [rows, 2 * cp] at the power-of-two scale of info[0] (abs-max: absmax_rows first);
+    info[1] <- the scale"""
+    check(lib.sessd_sparse_split_planes(_p(x), _p(n), int(max_rows), int(x.shape[1]), _p(info), _p(planes), int(planes.shape[1] // 2), _st()),
+          "sessd_sparse_split_planes")
+    return planes
+
+
+def dense_grad_gather(grad, coors, n, max_rows, grid, channels, out=None):
+    """adjoint of sparse_to_dense: grad NHWC [B, H, W, C*D] (contiguous) -> rows [max_rows, C] (rows >= n untouched)"""
+    if out is None:
+        out = torch.empty((int(max_rows), int(channels)), dtype=torch.float32, device=grad.device)
+    check(lib.sessd_dense_grad_gather(_p(grad), _p(coors), _p(n), int(max_rows), int(channels), grid, _p(out), _st()), "sessd_dense_grad_gather")
+    return out
+
+
+def wgrad_items(max_out, kvol):
+    """work items of one weight-gradient launch (a function of max_out and kvol only)"""
+    return int(lib.sessd_spconv_wgrad_items(int(max_out), int(kvol)))
+
+
+def wgrad_workspace(max_out, kvol, cin, cout, device):
+    return torch.empty((int(lib.sessd_spconv_wgrad_workspace_bytes(int(max_out), int(kvol), int(cin), int(cout))),), dtype=torch.uint8,
+                       device=device)
+
+
+def spconv_wgrad_rows(in_feat, gout, tiles, n_out, max_out, kvol, gw=None, ws=None):
+    """fp32 weight gradient [kvol, Cin, Cout] of the narrow layers (Cin <= 16) from the forward rulebook's tile lists"""
+    cin, cout = int(in_feat.shape[1]), int(gout.shape[1])
+    if gw is None:
+        gw = torch.empty((int(kvol), cin, cout), dtype=torch.float32, device=gout.device)
+    if ws is None:
+        ws = wgrad_workspace(max_out, kvol, cin, cout, gout.device)
+    check(lib.sessd_spconv_wgrad_rows(_p(in_feat), cin, _p(gout), cout, _p(tiles), int(kvol), _p(n_out), int(max_out), _p(gw), _p(ws), ws.numel(),
+                                      _st()), "sessd_spconv_wgrad_rows")
+    return gw
+
+
+def spconv_wgrad_cg(in_planes, in_info, g_planes, g_info, tiles, n_out, max_out, kvol, gw=None, ws=None):
+    """tensor-core weight gradient [kvol, Cp, Cout] from the input planes (+ {abs-max, scale}) and the gradient planes (sparse_split_planes)"""
+    cp, cout = int(in_planes.shape[1] // 2), int(g_planes.shape[1] // 2)
+    if gw is None:
+        gw = torch.empty((int(kvol), cp, cout), dtype=torch.float32, device=g_planes.device)
+    if ws is None:
+        ws = wgrad_workspace(max_out, kvol, cp, cout, g_planes.device)
+    check(lib.sessd_spconv_wgrad_cg(_p(in_planes), cp, _p(in_info), _p(g_planes), cout, _p(g_info), _p(tiles), int(kvol), _p(n_out), int(max_out),
+                                    _p(gw), _p(ws), ws.numel(), _st()), "sessd_spconv_wgrad_cg")
+    return gw
+
+
 def sparse_planes_to_float(planes, info, channels):
     """(hi + lo) / S of sparse feature planes [rows, 2 * cp] as fp32 [rows, channels] (tests / debugging)"""
     cp = planes.shape[1] // 2

@@ -3,7 +3,8 @@
 reference (requirements.txt:28) whose source is not part of it; the semantics implemented here are spconv 1.x's published
 ones: weight layout [kz,ky,kx,Cin,Cout], cross-correlation pairs, SubM convs keep the input index set, regular sparse convs emit
 every reachable output site, ``dense()`` returns [B, C, D, H, W].  Output rows of SparseConv3d are in ascending linear index
-(spconv's own order is atomics-dependent).  Inference only: the modules do not build an autograd graph (training is a "next" row).
+(spconv's own order is atomics-dependent).  The modules do not build an autograd graph; SpMiddleFHD in train mode differentiates
+through the same rulebooks with sessd_b200.sparse_grad.
 """
 import math
 
@@ -116,9 +117,10 @@ class _SparseConvBase(SparseModule):
     def packed_weight(self):
         return self.weight.detach().reshape(-1, self.in_channels, self.out_channels).contiguous().float()
 
-    @torch.no_grad()
-    def forward(self, x):
-        assert isinstance(x, SparseConvTensor)
+    def rulebook(self, x):
+        """The output index set of this conv on ``x`` and its neighbour table (a SubM table is shared through ``x.indice_dict`` by the
+        layers of an ``indice_key``): (output SparseConvTensor without features, nbr [cap, kvol] int32, device row count [1], cap).
+        Used by ``forward`` and by the training path (sessd_b200.sparse_grad)."""
         kind, index = x._ensure_index()
         n_in = x.indices.shape[0]
         kvol = int(np.prod(self.kernel_size))
@@ -136,11 +138,11 @@ class _SparseConvBase(SparseModule):
             ogrid = ops.make_grid(x.batch_size, oshape)
             cells = x.batch_size * int(np.prod(oshape))
             cap = max(1, min(cells, n_in * kvol))
-            bitmap, scratch = ops.bitmap_alloc(ogrid, x.features.device)
-            ocoors = torch.empty((cap, 4), dtype=torch.int32, device=x.features.device)
-            n_out_t = torch.zeros((1,), dtype=torch.int32, device=x.features.device)
-            nbr = torch.empty((cap, kvol), dtype=torch.int32, device=x.features.device)
-            status = torch.zeros((1,), dtype=torch.int32, device=x.features.device)
+            bitmap, scratch = ops.bitmap_alloc(ogrid, x.indices.device)
+            ocoors = torch.empty((cap, 4), dtype=torch.int32, device=x.indices.device)
+            n_out_t = torch.zeros((1,), dtype=torch.int32, device=x.indices.device)
+            nbr = torch.empty((cap, kvol), dtype=torch.int32, device=x.indices.device)
+            status = torch.zeros((1,), dtype=torch.int32, device=x.indices.device)
             ops.strided_rulebook(x.indices, x._n(), max(n_in, 1), x._grid(), kind, index, self.kernel_size, self.stride,
                                  self.padding, ogrid, bitmap, scratch, ocoors, n_out_t, cap, nbr, status)
             n_out = int(n_out_t.item())            # data-dependent size crosses to the host here (module-level API only)
@@ -149,6 +151,12 @@ class _SparseConvBase(SparseModule):
             cap = max(n_out, 1)
             nbr = nbr[:cap]
         out.indice_dict = x.indice_dict
+        return out, nbr, n_out_t, cap
+
+    @torch.no_grad()
+    def forward(self, x):
+        assert isinstance(x, SparseConvTensor)
+        out, nbr, n_out_t, cap = self.rulebook(x)
         feat = ops.spconv_forward(x.features.detach().float().contiguous(), nbr, n_out_t, cap, self.packed_weight(), None,
                                   self.bias.detach().float() if self.bias is not None else None, False)
         out.features = feat[: out.indices.shape[0]]
