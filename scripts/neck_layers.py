@@ -17,31 +17,9 @@ for _p in (ROOT, os.path.join(ROOT, "se-ssd_b200")):
 
 
 def launches(neck):
-    """(name, closure(skip)) of the 13 launches, with the arguments of SSFAPlanesRunner.forward"""
-    H, H2 = (neck.h, neck.w), (neck.h // 2, neck.w // 2)
-    conv = {
-        "bottom_up_block_0.1": ("x", "b0a", H, H, 128, 128, {}),
-        "bottom_up_block_0.4": ("b0a", "b0b", H, H, 128, 128, {}),
-        "bottom_up_block_0.7": ("b0b", "x0", H, H, 128, 128, {}),
-        "bottom_up_block_1.0": ("x0", "b1a", H, H2, 128, 256, dict(stride=2)),
-        "bottom_up_block_1.3": ("b1a", "b1b", H2, H2, 256, 256, {}),
-        "bottom_up_block_1.6": ("b1b", "x1", H2, H2, 256, 256, {}),
-        "trans_0.0": ("x0", None, H, H, 128, 128, dict(f32="t0")),
-        "trans_1.0": ("x1", "t1", H2, H2, 256, 256, {}),
-        "conv_0.0": ("m0", None, H, H, 128, 128, dict(f32="o0")),
-        "conv_1.0": ("m1", None, H, H, 128, 128, dict(f32="o1")),
-        "head": ("out", None, H, H, 128, neck.HEAD_STRIDE, dict(relu=False, f32="head")),
-    }
-    deconv = {"deconv_block_0.0": ("t1", "m0", dict(residual="t0")), "deconv_block_1.0": ("t1", "m1", {})}
-    out = []
-    for name in neck.SKIP_LAUNCHES:
-        if name in conv:
-            src, dst, ih, oh, ci, co, kw = conv[name]
-            out.append((name, lambda skip, a=(name, src, dst, ih, oh, ci, co), kw=kw: neck._conv(*a, skip=skip, **kw)))
-        else:
-            src, dst, kw = deconv[name]
-            out.append((name, lambda skip, a=(name, src, dst), kw=kw: neck._deconv(*a, skip=skip, **kw)))
-    return out
+    """(name, closure(skip)) of the 13 launches of SSFAPlanesRunner.forward"""
+    from sessd_data.layers import SSFA_LAUNCHES
+    return [(L.name, lambda skip, L=L: neck._launch(L, skip)) for L in SSFA_LAUNCHES]
 
 
 def main():

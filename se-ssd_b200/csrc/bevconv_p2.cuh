@@ -76,17 +76,21 @@ struct P2Params {
 __device__ __forceinline__ int p2_item_count(const P2Params &p) { return p.items ? __ldg(p.items) : p.total; }
 __device__ __forceinline__ int p2_item(const P2Params &p, int k) { return p.items ? __ldg(p.items + kP2ItemsHeader + k) : k; }
 
+// work item g -> (class rank in the heavy-first order, n-block, pixel tile): the item encoding of the kernel and of the skip planner
+struct P2ItemIndex { int rank, nb, t; };
+__host__ __device__ __forceinline__ P2ItemIndex p2_item_index(int g, int nblocks, int tiles) {
+    const int rank = g / (nblocks * tiles), rem = g - rank * (nblocks * tiles), nb = rem / tiles;
+    return {rank, nb, rem - nb * tiles};
+}
+
 struct P2Item { int cls, n0, b, u0, v0, ntaps; };
 
 __device__ __forceinline__ P2Item p2_decode(const P2Params &p, int g) {
     P2Item it;
-    const int per_cls = p.nblocks * p.tiles;
-    const int cr = g / per_cls;
-    int rem = g - cr * per_cls;
-    const int nb = rem / p.tiles;
-    int t = rem - nb * p.tiles;
-    it.cls = p.cls_order[cr];
-    it.n0 = nb * p.n_tile;
+    const P2ItemIndex ix = p2_item_index(g, p.nblocks, p.tiles);
+    int t = ix.t;
+    it.cls = p.cls_order[ix.rank];
+    it.n0 = ix.nb * p.n_tile;
     const int tu = t % p.tiles_u; t /= p.tiles_u;
     const int tv = t % p.tiles_v;
     it.b = t / p.tiles_v;
@@ -466,8 +470,58 @@ static int encode_map_nd(CUtensorMap *m, const void *base, int rank, const cuuin
     return r == CUDA_SUCCESS ? 0 : 700 + (int)r;
 }
 
-// taps: per class (dy, dx, weight tap); fills the geometry of p and launches
-struct P2Taps { int n, dy[9], dx[9], w[9]; };
+// per class: the taps (dy, dx, weight tap) and the (y, x) offset of its output positions (output = grid position * out_stride + offset)
+struct P2Taps { int n, dy[9], dx[9], w[9], off_y, off_x; };
+
+// ConvTranspose2d(k3, s2, p1, op1) as four output-parity classes c = 2 py + px over the input grid, output offset (py, px):
+// out[2y+py] receives in[y+dy] * W[ky] with 2y+py = 2(y+dy) - 1 + ky, i.e. ky = py + 1 - 2 dy for dy = py .. 0 (the same along x)
+static void p2_deconv_classes(P2Taps cls[4]) {
+    for (int c = 0; c < 4; ++c) {
+        P2Taps &k = cls[c];
+        k = {};
+        k.off_y = c >> 1; k.off_x = c & 1;
+        for (int dy = k.off_y; dy >= 0; --dy)
+            for (int dx = k.off_x; dx >= 0; --dx, ++k.n) {
+                k.dy[k.n] = dy; k.dx[k.n] = dx; k.w[k.n] = (k.off_y + 1 - 2 * dy) * 3 + (k.off_x + 1 - 2 * dx);
+            }
+    }
+}
+
+constexpr int p2_n_tile(int cout) { return cout <= 32 ? 32 : 128; }      // output channels per work item
+
+// The work items of one launch (the launcher's and the skip planner's): the class grid cut into 8 (u) x 16 (v) pixel tiles, u / v
+// mapped to (y, x) or (x, y), whichever gives fewer tiles; n-blocks of n_tile channels over the packed weight width cout_pad; classes
+// heavy first (descending tap count).  Item g = (rank * nblocks + n-block) * tiles + tile, tile = (b * tiles_v + tv) * tiles_u + tu.
+struct P2Geometry {
+    int u_is_x, grid_u, grid_v, tiles_u, tiles_v, tiles;
+    int n_tile, nblocks, nclass, total;
+    int ntaps[4], off_u[4], off_v[4], order[4];
+};
+
+static int p2_geometry(P2Geometry &g, int batch, int grid_h, int grid_w, int cout, int cout_pad, const P2Taps *cls, int nclass) {
+    g = {};
+    if (batch < 1 || grid_h < 1 || grid_w < 1 || cout < 8 || cout % 8) return SESSD_EINVAL;      // 8-channel stores
+    g.n_tile = p2_n_tile(cout);
+    if (cout_pad % g.n_tile || cout_pad < cout) return SESSD_EINVAL;
+    // orientation: the in-group dimension u has the 8-pixel tile edge; pick the mapping with fewer tiles
+    g.u_is_x = div_up(grid_w, kP2TileU) * div_up(grid_h, kP2TileV) <= div_up(grid_h, kP2TileU) * div_up(grid_w, kP2TileV);
+    g.grid_u = g.u_is_x ? grid_w : grid_h; g.grid_v = g.u_is_x ? grid_h : grid_w;
+    g.tiles_u = div_up(g.grid_u, kP2TileU); g.tiles_v = div_up(g.grid_v, kP2TileV);
+    g.tiles = g.tiles_u * g.tiles_v * batch;
+    g.nblocks = cout_pad / g.n_tile;
+    g.nclass = nclass; g.total = nclass * g.nblocks * g.tiles;
+    for (int c = 0; c < nclass; ++c) {
+        g.ntaps[c] = cls[c].n;
+        g.off_u[c] = g.u_is_x ? cls[c].off_x : cls[c].off_y;
+        g.off_v[c] = g.u_is_x ? cls[c].off_y : cls[c].off_x;
+        g.order[c] = c;
+    }
+    for (int i = 1; i < nclass; ++i)            // insertion sort by descending tap count
+        for (int k = i; k > 0 && g.ntaps[g.order[k]] > g.ntaps[g.order[k - 1]]; --k) {
+            const int tmp = g.order[k]; g.order[k] = g.order[k - 1]; g.order[k - 1] = tmp;
+        }
+    return 0;
+}
 
 // MODE kP2Planes: d_in = fp16 planes [2][B][H][W][C], d_in_info = {abs-max, S}; split modes: d_in = fp32 NHWC, d_in_info = the input's
 // abs-max (split fp16; nullable) or unused (tf32), weights fp32 [2][taps][cout_pad][cin] in the tf32 mode; d_out_info is {abs-max, S_out}
@@ -475,22 +529,25 @@ struct P2Taps { int n, dy[9], dx[9], w[9]; };
 template <int MODE>
 static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d_in_info, const void *d_w, int w_taps, int cout_pad,
                      const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info, float gain,
-                     float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, P2Params &p, const P2Taps *cls, int grid_h,
-                     int grid_w, void *stream) {
+                     float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, P2Params &p, const P2Taps *cls, int nclass,
+                     int grid_h, int grid_w, void *stream) {
     if (!d_in_planes || !d_w || (!d_out_f32 && !d_out_planes)) return SESSD_EINVAL;
     if (MODE == kP2Planes && (!d_in_info || !d_scale)) return SESSD_EINVAL;
     if (MODE != kP2Planes && d_out_planes) return SESSD_EINVAL;
-    if (p.cin < 64 || p.cin % 64 || p.cout < 8 || p.cout % 8) return SESSD_EINVAL;      // whole 64-channel groups; 8-channel stores
+    if (p.cin < 64 || p.cin % 64) return SESSD_EINVAL;      // whole 64-channel groups
     // the epilogue reads and writes 16 bytes at a time
     if (((uintptr_t)d_scale | (uintptr_t)d_shift | (uintptr_t)d_residual | (uintptr_t)d_out_f32 | (uintptr_t)d_out_planes) & 15)
         return SESSD_EINVAL;
-    const int n_tile = p.cout <= 32 ? 32 : 128;
-    if (cout_pad % n_tile || cout_pad < p.cout) return SESSD_EINVAL;
-    // orientation: the in-group dimension u has the 8-pixel tile edge; pick the mapping with fewer tiles
-    const int t_ux = div_up(grid_w, kP2TileU) * div_up(grid_h, kP2TileV), t_uy = div_up(grid_h, kP2TileU) * div_up(grid_w, kP2TileV);
-    p.u_is_x = t_ux <= t_uy ? 1 : 0;
-    p.grid_u = p.u_is_x ? grid_w : grid_h;
-    p.grid_v = p.u_is_x ? grid_h : grid_w;
+    P2Geometry g;
+    if (p2_geometry(g, p.batch, grid_h, grid_w, p.cout, cout_pad, cls, nclass)) return SESSD_EINVAL;
+    // a skip-plan record numbers the items of the width the runner packs: any other width decodes them to other classes / n-blocks
+    if (p.items && cout_pad != div_up(p.cout, g.n_tile) * g.n_tile) return SESSD_EINVAL;
+    p.u_is_x = g.u_is_x; p.grid_u = g.grid_u; p.grid_v = g.grid_v;
+    p.tiles_u = g.tiles_u; p.tiles_v = g.tiles_v; p.tiles = g.tiles;
+    p.n_tile = g.n_tile; p.nblocks = g.nblocks; p.nclass = g.nclass; p.total = g.total;
+    for (int c = 0; c < 4; ++c) {
+        p.cls_ntaps[c] = g.ntaps[c]; p.cls_off_u[c] = g.off_u[c]; p.cls_off_v[c] = g.off_v[c]; p.cls_order[c] = g.order[c];
+    }
     // patch copies: one per distinct (tap shift along u, tap shift along v modulo the input stride)
     const int s = p.in_stride;
     p.ncopies = 0;
@@ -514,7 +571,6 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
     if (p.rows_v > kP2MaxRowsV) return SESSD_EINVAL;
     for (int k = 0; k < p.ncopies; ++k) { p.copy_u[k] = key_u[k]; p.copy_v[k] = vmin[k]; }
     for (int c = 0; c < p.nclass; ++c) {
-        p.cls_ntaps[c] = cls[c].n;
         for (int t = 0; t < cls[c].n; ++t) {
             const int tu = p.u_is_x ? cls[c].dx[t] : cls[c].dy[t], tv = p.u_is_x ? cls[c].dy[t] : cls[c].dx[t];
             const int vm = ((tv % s) + s) % s;
@@ -532,7 +588,7 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
     // fp32 staging: 32 channels = 128-byte rows (split fp16) or 16 channels = 64-byte rows (tf32)
     p.staging_bytes = MODE == kP2Planes ? 0 : p.ncopies * p.rows_v * kP2TileU * p.chunk * 4;
     p.load_bytes = MODE == kP2Planes ? p.patch_bytes : p.staging_bytes;
-    const int per_buf = p.patch_bytes + p.staging_bytes, bstage = 2 * (p.cout <= 32 ? 32 : 128) * 64;
+    const int per_buf = p.patch_bytes + p.staging_bytes, bstage = 2 * p.n_tile * 64;
     // weight ring: kP2BRing when it fits next to two patch buffers or one, else shrunk (>= 2 stages) next to one buffer
     p.bring_bytes = kP2BRing;
     p.npatch = (kP2BRing + 1536 + 2 * per_buf <= kP2MaxSmem) ? 2 : 1;
@@ -565,7 +621,7 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
     {   // weights [2 (hi|lo)][taps][cout_pad][cin] fp16 (fp32 tf32 split in the tf32 mode): 64-byte rows of one K stage
         const cuuint64_t dims[4] = {(cuuint64_t)p.cin, (cuuint64_t)cout_pad, (cuuint64_t)w_taps, 2};
         const cuuint64_t strides[3] = {(cuuint64_t)p.cin * es, (cuuint64_t)cout_pad * p.cin * es, (cuuint64_t)w_taps * cout_pad * p.cin * es};
-        const cuuint32_t box[4] = {(cuuint32_t)p.chunk, (cuuint32_t)n_tile, 1, 1};
+        const cuuint32_t box[4] = {(cuuint32_t)p.chunk, (cuuint32_t)p.n_tile, 1, 1};
         const cuuint32_t estr[4] = {1, 1, 1, 1};
         int rc = encode_map_nd(&map_b, d_w, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_64B,
                                MODE == kP2SplitTf32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
@@ -577,19 +633,8 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
         SESSD_CUDA_TRY(cudaFuncSetAttribute(bev_conv_p2_kernel<128, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2MaxSmem));
         attr_done = true;
     }
-    p.n_tile = n_tile;
-    p.bstage_bytes = 2 * n_tile * 64;
+    p.bstage_bytes = bstage;
     p.bstages = p.bring_bytes / p.bstage_bytes < kP2MaxBStages ? p.bring_bytes / p.bstage_bytes : kP2MaxBStages;
-    p.tiles_u = div_up(p.grid_u, kP2TileU);
-    p.tiles_v = div_up(p.grid_v, kP2TileV);
-    p.tiles = p.tiles_u * p.tiles_v * p.batch;
-    p.nblocks = cout_pad / n_tile;
-    p.total = p.nclass * p.nblocks * p.tiles;
-    for (int c = 0; c < p.nclass; ++c) p.cls_order[c] = c;
-    for (int i = 1; i < p.nclass; ++i)            // insertion sort by descending tap count (heavy items first)
-        for (int k = i; k > 0 && p.cls_ntaps[p.cls_order[k]] > p.cls_ntaps[p.cls_order[k - 1]]; --k) {
-            const int tmp = p.cls_order[k]; p.cls_order[k] = p.cls_order[k - 1]; p.cls_order[k - 1] = tmp;
-        }
     p.in_info = MODE == kP2Planes ? d_in_info : nullptr;
     p.in_amax = MODE == kP2SplitF16 ? d_in_info : nullptr;
     p.resid_info = d_residual ? d_resid_info : nullptr;
@@ -605,7 +650,7 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
         SESSD_CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
     }
     const int grid = p.total < num_sms ? p.total : num_sms;                 // persistent, one CTA per SM
-    if (n_tile == 32)
+    if (p.n_tile == 32)
         SESSD_LAUNCH((bev_conv_p2_kernel<32, MODE>), grid, kP2Threads, smem, (cudaStream_t)stream, map_a, map_b, d_scale, d_shift, d_residual, d_out_f32,
                      (__half *)d_out_planes, p);
     else
@@ -623,24 +668,17 @@ static int p2_conv(const void *d_in_planes, const float *d_in_info, const void *
                    const int *d_items = nullptr) {
     if (!desc) return SESSD_EINVAL;
     const sessd_conv_desc &d = *desc;
-    if (d.batch < 1 || d.ntaps < 1 || d.ntaps > 9 || (d.in_stride != 1 && d.in_stride != 2) || d.out_stride < 1 || d.grid_h < 1 || d.grid_w < 1)
-        return SESSD_EINVAL;
+    if (d.ntaps < 1 || d.ntaps > 9 || (d.in_stride != 1 && d.in_stride != 2) || d.out_stride < 1) return SESSD_EINVAL;
     if ((d.grid_h - 1) * d.out_stride + d.out_off_y >= d.out_h || (d.grid_w - 1) * d.out_stride + d.out_off_x >= d.out_w) return SESSD_EINVAL;
     P2Params p = {};
     p.batch = d.batch; p.cin = d.cin; p.cout = d.cout; p.in_stride = d.in_stride;
     p.out_h = d.out_h; p.out_w = d.out_w; p.out_stride = d.out_stride; p.relu = d.relu;
-    p.nclass = 1;
     p.items = d_items;
     P2Taps t = {};
-    t.n = d.ntaps;
+    t.n = d.ntaps; t.off_y = d.out_off_y; t.off_x = d.out_off_x;
     for (int i = 0; i < d.ntaps; ++i) { t.dy[i] = d.tap_dy[i]; t.dx[i] = d.tap_dx[i]; t.w[i] = i; }
-    // class offsets are expressed along (u, v) inside launch_p2 once the orientation is known: pass (y, x) through the first slots
-    const int off_y = d.out_off_y, off_x = d.out_off_x;
-    const int t_ux = div_up(d.grid_w, kP2TileU) * div_up(d.grid_h, kP2TileV), t_uy = div_up(d.grid_h, kP2TileU) * div_up(d.grid_w, kP2TileV);
-    const bool u_is_x = t_ux <= t_uy;
-    p.cls_off_u[0] = u_is_x ? off_x : off_y; p.cls_off_v[0] = u_is_x ? off_y : off_x;
     return launch_p2<MODE>(d_in_planes, d.in_h, d.in_w, d_in_info, d_weight_h2, d.ntaps, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
-                     shift_max, d_out_f32, d_out_planes, d_out_info, p, &t, d.grid_h, d.grid_w, stream);
+                     shift_max, d_out_f32, d_out_planes, d_out_info, p, &t, 1, d.grid_h, d.grid_w, stream);
 }
 
 template <int MODE>
@@ -648,32 +686,14 @@ static int p2_deconv(const void *d_in_planes, const float *d_in_info, const void
                      const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                      float *d_out_f32, void *d_out_planes, float *d_out_info, int batch, int in_h, int in_w, int cin, int cout,
                      int relu, void *stream, const int *d_items = nullptr) {
-    if (batch < 1 || in_h < 1 || in_w < 1) return SESSD_EINVAL;
     P2Params p = {};
     p.batch = batch; p.cin = cin; p.cout = cout; p.in_stride = 1;
     p.out_h = 2 * in_h; p.out_w = 2 * in_w; p.out_stride = 2; p.relu = relu;
-    p.nclass = 4;
     p.items = d_items;
-    P2Taps cls[4] = {};
-    const int t_ux = div_up(in_w, kP2TileU) * div_up(in_h, kP2TileV), t_uy = div_up(in_h, kP2TileU) * div_up(in_w, kP2TileV);
-    const bool u_is_x = t_ux <= t_uy;
-    for (int py = 0; py < 2; ++py)
-        for (int px = 0; px < 2; ++px) {
-            const int c = py * 2 + px;
-            p.cls_off_u[c] = u_is_x ? px : py; p.cls_off_v[c] = u_is_x ? py : px;
-            // out[2y+py] receives in[y+dy] * W[ky] with 2y+py = 2(y+dy) - 1 + ky:  py=0 -> (ky=1,dy=0);  py=1 -> (ky=0,dy=1), (ky=2,dy=0)
-            const int kys[2] = {py == 0 ? 1 : 0, 2}, dys[2] = {py == 0 ? 0 : 1, 0}, ny = py == 0 ? 1 : 2;
-            const int kxs[2] = {px == 0 ? 1 : 0, 2}, dxs[2] = {px == 0 ? 0 : 1, 0}, nx = px == 0 ? 1 : 2;
-            int t = 0;
-            for (int a = 0; a < ny; ++a)
-                for (int bb = 0; bb < nx; ++bb) {
-                    cls[c].dy[t] = dys[a]; cls[c].dx[t] = dxs[bb]; cls[c].w[t] = kys[a] * 3 + kxs[bb];
-                    ++t;
-                }
-            cls[c].n = t;
-        }
+    P2Taps cls[4];
+    p2_deconv_classes(cls);
     return launch_p2<MODE>(d_in_planes, in_h, in_w, d_in_info, d_weight_h2, 9, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
-                     d_out_f32, d_out_planes, d_out_info, p, cls, in_h, in_w, stream);
+                     d_out_f32, d_out_planes, d_out_info, p, cls, 4, in_h, in_w, stream);
 }
 
 }  // namespace sessd

@@ -30,11 +30,10 @@ constexpr int kNumFullMaps = kMTmp + 1;
 constexpr int kSkipLaunches = 13;
 constexpr int kSkipThreads = 1024;
 
-struct SkipLaunch {
+struct SkipLaunch : P2Geometry {             // the launcher's work items (p2_geometry)
     int map;                                   // bit map of the launch's output
-    int nclass, nblocks, tiles_u, tiles_v, tiles, u_is_x, grid_u, grid_v, out_stride, out_h, out_w;
-    int off_y[4], off_x[4], order[4];
-    int rec, cap_items;                        // word offset of the launch record; nclass * nblocks * tiles
+    int out_stride, out_h, out_w;
+    int rec;                                   // word offset of the launch record
 };
 
 struct SkipPlan {
@@ -42,33 +41,15 @@ struct SkipPlan {
     SkipLaunch l[kSkipLaunches];
 };
 
-// the launcher's geometry (launch_p2 / p2_conv / p2_deconv): orientation, tiles, n-blocks and heavy-first class order
-static void skip_launch(SkipLaunch &L, int map, int batch, int grid_h, int grid_w, int out_h, int out_w, int cout, bool deconv) {
+// one launch of the plan, with the launcher's geometry at the weight width the runner packs (round_up(cout, n_tile))
+static int skip_launch(SkipLaunch &L, int map, int batch, int grid_h, int grid_w, int out_h, int out_w, int cout, bool deconv) {
+    P2Taps cls[4] = {};
+    if (deconv) p2_deconv_classes(cls);
+    else cls[0].n = 1;                         // a conv is one class: its taps do not enter the item order
     L.map = map;
-    const int t_ux = div_up(grid_w, kP2TileU) * div_up(grid_h, kP2TileV), t_uy = div_up(grid_h, kP2TileU) * div_up(grid_w, kP2TileV);
-    L.u_is_x = t_ux <= t_uy ? 1 : 0;
-    L.grid_u = L.u_is_x ? grid_w : grid_h;
-    L.grid_v = L.u_is_x ? grid_h : grid_w;
-    L.tiles_u = div_up(L.grid_u, kP2TileU);
-    L.tiles_v = div_up(L.grid_v, kP2TileV);
-    L.tiles = L.tiles_u * L.tiles_v * batch;
-    const int n_tile = cout <= 32 ? 32 : 128;
-    L.nblocks = div_up(cout, n_tile);
-    L.nclass = deconv ? 4 : 1;
     L.out_stride = deconv ? 2 : 1;
     L.out_h = out_h; L.out_w = out_w;
-    int ntaps[4];
-    for (int c = 0; c < 4; ++c) {
-        L.off_y[c] = deconv ? c >> 1 : 0;
-        L.off_x[c] = deconv ? c & 1 : 0;
-        ntaps[c] = deconv ? (1 + (c >> 1)) * (1 + (c & 1)) : 9;
-        L.order[c] = c;
-    }
-    for (int i = 1; i < L.nclass; ++i)
-        for (int k = i; k > 0 && ntaps[L.order[k]] > ntaps[L.order[k - 1]]; --k) {
-            const int tmp = L.order[k]; L.order[k] = L.order[k - 1]; L.order[k - 1] = tmp;
-        }
-    L.cap_items = L.nclass * L.nblocks * L.tiles;
+    return p2_geometry(L, batch, grid_h, grid_w, cout, div_up(cout, p2_n_tile(cout)) * p2_n_tile(cout), cls, deconv ? 4 : 1);
 }
 
 // the SSFAPlanesRunner launch sequence (runners.SSFAPlanesRunner.SKIP_LAUNCHES); returns the plan's int32 words, or 0
@@ -78,25 +59,25 @@ static long long skip_plan(SkipPlan &P, int batch, int h, int w) {
     P.nwf = div_up(w, 32); P.nwh = div_up(P.w2, 32);
     const int h2 = P.h2, w2 = P.w2;
     SkipLaunch *L = P.l;
-    skip_launch(L[0], kMB0a, batch, h, w, h, w, 128, false);        // bottom_up_block_0.1
-    skip_launch(L[1], kMB0b, batch, h, w, h, w, 128, false);        // bottom_up_block_0.4
-    skip_launch(L[2], kMX0, batch, h, w, h, w, 128, false);         // bottom_up_block_0.7
-    skip_launch(L[3], kMB1a, batch, h2, w2, h2, w2, 256, false);    // bottom_up_block_1.0 (stride 2)
-    skip_launch(L[4], kMB1b, batch, h2, w2, h2, w2, 256, false);    // bottom_up_block_1.3
-    skip_launch(L[5], kMX1, batch, h2, w2, h2, w2, 256, false);     // bottom_up_block_1.6
-    skip_launch(L[6], kMX0, batch, h, w, h, w, 128, false);         // trans_0.0 (1x1)
-    skip_launch(L[7], kMX1, batch, h2, w2, h2, w2, 256, false);     // trans_1.0 (1x1)
-    skip_launch(L[8], kMM0, batch, h2, w2, h, w, 128, true);        // deconv_block_0.0 (+ t0)
-    skip_launch(L[9], kMM1, batch, h2, w2, h, w, 128, true);        // deconv_block_1.0
-    skip_launch(L[10], kMO0, batch, h, w, h, w, 128, false);        // conv_0.0
-    skip_launch(L[11], kMO1, batch, h, w, h, w, 128, false);        // conv_1.0
-    skip_launch(L[12], kMOut, batch, h, w, h, w, 24, false);        // head (1x1 on the fused map)
+    const int rc = skip_launch(L[0], kMB0a, batch, h, w, h, w, 128, false)     // bottom_up_block_0.1
+                 | skip_launch(L[1], kMB0b, batch, h, w, h, w, 128, false)     // bottom_up_block_0.4
+                 | skip_launch(L[2], kMX0, batch, h, w, h, w, 128, false)      // bottom_up_block_0.7
+                 | skip_launch(L[3], kMB1a, batch, h2, w2, h2, w2, 256, false) // bottom_up_block_1.0 (stride 2)
+                 | skip_launch(L[4], kMB1b, batch, h2, w2, h2, w2, 256, false) // bottom_up_block_1.3
+                 | skip_launch(L[5], kMX1, batch, h2, w2, h2, w2, 256, false)  // bottom_up_block_1.6
+                 | skip_launch(L[6], kMX0, batch, h, w, h, w, 128, false)      // trans_0.0 (1x1)
+                 | skip_launch(L[7], kMX1, batch, h2, w2, h2, w2, 256, false)  // trans_1.0 (1x1)
+                 | skip_launch(L[8], kMM0, batch, h2, w2, h, w, 128, true)     // deconv_block_0.0 (+ t0)
+                 | skip_launch(L[9], kMM1, batch, h2, w2, h, w, 128, true)     // deconv_block_1.0
+                 | skip_launch(L[10], kMO0, batch, h, w, h, w, 128, false)     // conv_0.0
+                 | skip_launch(L[11], kMO1, batch, h, w, h, w, 128, false)     // conv_1.0
+                 | skip_launch(L[12], kMOut, batch, h, w, h, w, 24, false);    // head (1x1 on the fused map)
     long long words = 0;
     for (int i = 0; i < kSkipLaunches; ++i) {
         L[i].rec = (int)words;
-        words += kP2ItemsHeader + L[i].cap_items + 2LL * L[i].nclass * L[i].tiles;
+        words += kP2ItemsHeader + L[i].total + 2LL * L[i].nclass * L[i].tiles;
     }
-    return words;
+    return rc ? 0 : words;
 }
 
 struct BitMap {
@@ -228,7 +209,7 @@ __global__ void __launch_bounds__(kSkipThreads) bev_skip_plan_kernel(const uint2
         for (int li = 0; li < kSkipLaunches; ++li) {
             const SkipLaunch &L = P.l[li];
             const BitMap &o = m[L.map];
-            int *flags = plan + L.rec + kP2ItemsHeader + L.cap_items + L.nclass * L.tiles;
+            int *flags = plan + L.rec + kP2ItemsHeader + L.total + L.nclass * L.tiles;
             const int per_frame = L.tiles_u * L.tiles_v;
             for (int idx = threadIdx.x; idx < L.nclass * per_frame; idx += blockDim.x) {
                 const int c = idx / per_frame, tf = idx - c * per_frame;
@@ -242,9 +223,8 @@ __global__ void __launch_bounds__(kSkipThreads) bev_skip_plan_kernel(const uint2
                     for (int y = y0; y < y0 + ny && !run; ++y) run = (o.w[y * o.nw + (x0 >> 5)] >> (x0 & 31)) & field;
                 } else if (!run) {
                     for (int r = 0; r < kP2TileU * kP2TileV && !run; ++r) {
-                        const int gu = u0 + (r & 7), gv = v0 + (r >> 3);
-                        const int gy = L.u_is_x ? gv : gu, gx = L.u_is_x ? gu : gv;
-                        run = o.get(gy * L.out_stride + L.off_y[c], gx * L.out_stride + L.off_x[c]);
+                        const int ou = (u0 + (r & 7)) * L.out_stride + L.off_u[c], ov = (v0 + (r >> 3)) * L.out_stride + L.off_v[c];
+                        run = L.u_is_x ? o.get(ov, ou) : o.get(ou, ov);
                     }
                 }
                 flags[c * L.tiles + b * per_frame + tf] = run ? 1 : 0;
@@ -256,17 +236,16 @@ __global__ void __launch_bounds__(kSkipThreads) bev_skip_plan_kernel(const uint2
     for (int li = 0; li < kSkipLaunches; ++li) {
         const SkipLaunch &L = P.l[li];
         int *rec = plan + L.rec;
-        int *items = rec + kP2ItemsHeader, *skipped = items + L.cap_items;
+        int *items = rec + kP2ItemsHeader, *skipped = items + L.total;
         const int *flags = skipped + L.nclass * L.tiles;
         if (threadIdx.x < 4) s_rep[threadIdx.x] = 0x7FFFFFFF;
         __syncthreads();
         for (int e = threadIdx.x; e < L.nclass * L.tiles; e += blockDim.x)
             if (!flags[e]) atomicMin(&s_rep[e / L.tiles], e % L.tiles);
         __syncthreads();
-        const int per_cls = L.nblocks * L.tiles;
-        const int count = skip_compact(L.cap_items, [&](int g) {
-            const int cls = L.order[g / per_cls], t = g % L.tiles;
-            return flags[cls * L.tiles + t] != 0 || t == s_rep[cls];
+        const int count = skip_compact(L.total, [&](int g) {
+            const P2ItemIndex ix = p2_item_index(g, L.nblocks, L.tiles);
+            return flags[L.order[ix.rank] * L.tiles + ix.t] != 0 || ix.t == s_rep[L.order[ix.rank]];
         }, items, s_scan);
         const int nskip = skip_compact(L.nclass * L.tiles, [&](int e) {
             return flags[e] == 0 && e % L.tiles != s_rep[e / L.tiles];
@@ -277,11 +256,11 @@ __global__ void __launch_bounds__(kSkipThreads) bev_skip_plan_kernel(const uint2
             rec[kRecUisX] = L.u_is_x; rec[kRecOutStride] = L.out_stride; rec[kRecOutH] = L.out_h; rec[kRecOutW] = L.out_w;
             rec[kRecBatch] = P.batch;
             for (int c = 0; c < 4; ++c) {
-                rec[kRecOffY + c] = L.off_y[c]; rec[kRecOffX + c] = L.off_x[c];
+                rec[kRecOffY + c] = L.u_is_x ? L.off_v[c] : L.off_u[c]; rec[kRecOffX + c] = L.u_is_x ? L.off_u[c] : L.off_v[c];
                 rec[kRecRep + c] = c < L.nclass && s_rep[c] != 0x7FFFFFFF ? s_rep[c] : -1;
             }
-            rec[kRecSkipOff] = kP2ItemsHeader + L.cap_items;
-            rec[kRecFlagOff] = kP2ItemsHeader + L.cap_items + L.nclass * L.tiles;
+            rec[kRecSkipOff] = kP2ItemsHeader + L.total;
+            rec[kRecFlagOff] = kP2ItemsHeader + L.total + L.nclass * L.tiles;
         }
         __syncthreads();
     }

@@ -1,4 +1,4 @@
-"""BEV necks on the hot path: the SSFA block of SE-SSD (runs on csrc/bevconv_h2.cu through sessd_b200.runners.SSFARunner)."""
+"""BEV necks on the hot path: the SSFA block of SE-SSD (runs on csrc/bevconv_p2.cu through sessd_b200.runners.SSFAPlanesRunner)."""
 from .rpn_v1 import SSFA
 
 __all__ = ["SSFA"]

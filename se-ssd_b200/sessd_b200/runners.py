@@ -8,6 +8,7 @@ import math
 
 import torch
 from sessd_data.layers import SPMIDDLE_LAYERS  # (kind, cout, ksize, stride, padding, indice_key)   scn.py:106-149
+from sessd_data.layers import SSFA_LAUNCHES, ssfa_extents
 
 from . import ops
 
@@ -263,6 +264,63 @@ def pack_head(head_sd, prefix, device, stride=24):
     return hw.contiguous(), hb.contiguous()
 
 
+def fold_ssfa_bn(sd, conv_name, device, eps=BN_EPS):
+    """folded (scale, shift) of the BatchNorm2d that follows an SSFA conv: module blk.(i+1) of the conv blk.i (rpn_v1.py:135-210)"""
+    blk, idx = conv_name.rsplit(".", 1)
+    b = "%s.%d." % (blk, int(idx) + 1)
+    return fold_bn(*(sd[b + k].to(device, torch.float32) for k in ("weight", "bias", "running_mean", "running_var")), eps=eps)
+
+
+def pack_h2(wp, scale, shift, cout_pad):
+    """[taps, Cin, Cout] weight + folded BN (scale None: 1) -> the fp16-split launch parameters of bev_conv_p2 / _h2: weight planes,
+    epilogue scale (BN scale x the planes' 2^-e[n]), shift, and gain / shift_max of the output bound"""
+    planes, inv = ops.pack_weight_h2(wp, cout_pad)
+    scale = torch.ones(wp.shape[2], device=wp.device) if scale is None else scale
+    return dict(w=planes, scale=(scale * inv[:scale.numel()]).contiguous(), shift=shift.contiguous(), gain=ops.conv_gain(wp, scale),
+                shift_max=float(shift.abs().max()))
+
+
+def _cout_pad(cout):
+    """packed weight width of a BEV conv: whole n-tiles of bev_conv_p2 (32 channels up to 32, else 128), as the skip plan assumes"""
+    n_tile = 32 if cout <= 32 else 128
+    return -(-cout // n_tile) * n_tile
+
+
+def ssfa_weights(ssfa_sd, head_sd, head_prefix, device, bn_eps=BN_EPS):
+    """yields (launch, weight [taps, Cin, Cout], taps, BN scale, BN shift) in SSFA_LAUNCHES order: convs in the tap-list packing (taps
+    (dy, dx) relative to the output pixel), deconvs in the plain 9-tap packing of W[cin][cout][ky][kx] (taps None), the head (only with
+    head_sd) with scale None and its bias as the shift"""
+    for L in SSFA_LAUNCHES:
+        if L.name == "head":
+            if head_sd is not None:
+                hw, hb = pack_head(head_sd, head_prefix, device, L.cout)
+                yield L, hw, [(0, 0)], None, hb
+            continue
+        wt = ssfa_sd[L.name + ".weight"].to(device, torch.float32)
+        if L.kind == "conv":
+            wp, taps = _pack_conv(wt)
+            taps = [(dy - L.k // 2, dx - L.k // 2) for dy, dx in taps]
+        else:
+            wp, taps = wt.permute(2, 3, 0, 1).reshape(9, L.cin, L.cout).contiguous(), None
+        yield (L, wp, taps) + fold_ssfa_bn(ssfa_sd, L.name, device, bn_eps)
+
+
+def ssfa_fuse_weights(ssfa_sd, device, bn_eps=BN_EPS):
+    """{w_0.0 / w_1.0: (weight [128], BN scale, BN shift)} of the attention fusion's 1x1 128 -> 1 convs"""
+    out = {}
+    for name in ("w_0.0", "w_1.0"):
+        sc, sh = fold_ssfa_bn(ssfa_sd, name, device, bn_eps)
+        out[name] = (ssfa_sd[name + ".weight"].to(device, torch.float32).reshape(-1).contiguous(), float(sc[0]), float(sh[0]))
+    return out
+
+
+# {abs-max, scale} slot of every SSFA tensor: the neck input, the launch outputs the planes runner keeps as planes, the fused map, then the
+# fp32 outputs (SSFARunner's abs-max slots have the same numbers)
+SSFA_SLOT = {n: i for i, n in enumerate(["x"] + [L.dst for L in SSFA_LAUNCHES if not L.f32] + ["out"] + [L.dst for L in SSFA_LAUNCHES if L.f32])}
+_SSFA_INPUTS = {L.src for L in SSFA_LAUNCHES}        # tensors a later launch reads (the fp16 split needs their abs-max)
+_SSFA = {L.name: L for L in SSFA_LAUNCHES}
+
+
 class HeadRunner:
     """The fused head GEMM alone (MultiGroupHead.forward)."""
 
@@ -279,25 +337,25 @@ class HeadRunner:
     def load_state(self, head_sd, prefix=""):
         self.w_simt, self.bias = pack_head(head_sd, prefix, self.device, self.stride)
         if self.use_tc:
-            planes, inv = ops.pack_weight_h2(self.w_simt, 32)
-            gain = ops.conv_gain(self.w_simt, torch.ones(self.stride, device=self.device))
-            self.w_tc = (planes, inv[: self.stride].contiguous(), gain, float(self.bias.abs().max()))
+            self.w_tc = pack_h2(self.w_simt, None, self.bias, _cout_pad(self.stride))
 
     def forward(self, x):
         H = (self.h, self.w)
         d = ops.conv_desc(self.batch, H, 128, H, self.stride, H, [(0, 0)], relu=False)
         if self.w_tc is not None:
-            planes, scale, gain, shift_max = self.w_tc
+            q = self.w_tc
             self.info.zero_()
             ops.absmax(x, self.info[0, 0:1])
             ops.bev_split_planes(x, self.info[0], self.x_planes)
-            ops.bev_conv_p2(self.x_planes, self.info[0], planes, scale, self.bias, None, None, gain, shift_max, self.out, None, self.info[1], d)
+            ops.bev_conv_p2(self.x_planes, self.info[0], q["w"], q["scale"], q["shift"], None, None, q["gain"], q["shift_max"], self.out, None,
+                            self.info[1], d)
             return self.out
         return ops.bev_conv(x, self.w_simt, None, self.bias, None, self.out, d)
 
 
 class SSFARunner:
-    """SSFA neck (rpn_v1.py:220-235) + the fused 128->22(+2 pad) head GEMM (mg_head_sessd.py:202-230)."""
+    """SSFA neck (rpn_v1.py:220-235) + the fused 128->22(+2 pad) head GEMM (mg_head_sessd.py:202-230) from fp32 activations: the lab
+    formats of bev_conv_p2_kernel, or the fp32 SIMT baseline."""
 
     HEAD_STRIDE = 24
 
@@ -305,96 +363,63 @@ class SSFARunner:
 
     def __init__(self, batch, hw=(200, 176), device="cuda", use_tc=True, split="fp16"):
         """use_tc: tensor-core convs (default); False = the fp32 SIMT baseline kernels.
-        split: "fp16" = two-term fp16 split (kind::f16, bevconv_h2.cu; the stride-2 conv stays on the tf32 kernel),
-               "tf32" = 3xTF32 everywhere (bevconv_tc.cu)."""
+        split: "fp16" = two-term fp16 split of the fp32 input inside the kernel (bev_conv_p2_kernel<.., kP2SplitF16>, bevconv_split.cu;
+               the stride-2 conv stays on the tf32 mode), "tf32" = 3xTF32 everywhere (kP2SplitTf32, bevconv_split.cu)."""
         self.batch, self.h, self.w, self.device = batch, int(hw[0]), int(hw[1]), torch.device(device)
         self.use_tc = bool(use_tc)
         assert split in ("fp16", "tf32")
         self.use_h2 = self.use_tc and split == "fp16"
-        self.amax = torch.zeros(16, dtype=torch.float32, device=self.device)     # per-tensor abs-max scalars (fp16 split scaling)
-        h, w, h2, w2 = self.h, self.w, self.h // 2, self.w // 2
-        z = lambda hh, ww, c: torch.zeros((batch, hh, ww, c), dtype=torch.float32, device=self.device)  # noqa: E731
-        self.buf = dict(b0a=z(h, w, 128), b0b=z(h, w, 128), x0=z(h, w, 128), b1a=z(h2, w2, 256), b1b=z(h2, w2, 256),
-                        x1=z(h2, w2, 256), t0=z(h, w, 128), t1=z(h2, w2, 256), m0=z(h, w, 128), m1=z(h, w, 128),
-                        o0=z(h, w, 128), o1=z(h, w, 128), out=z(h, w, 128), head=z(h, w, self.HEAD_STRIDE))
+        self.amax = torch.zeros(16, dtype=torch.float32, device=self.device)     # abs-max scalars (fp16 split scaling), SSFA_SLOT numbering
+        z = lambda hw_, c: torch.zeros((batch,) + hw_ + (c,), dtype=torch.float32, device=self.device)  # noqa: E731
+        self.buf = {L.dst: z(ssfa_extents(L, self.h, self.w)[1], L.cout) for L in SSFA_LAUNCHES}
+        self.buf["out"] = z((self.h, self.w), 128)
         self.params = None
 
     def load_state(self, ssfa_sd, head_sd=None, head_prefix="tasks.0.", bn_eps=BN_EPS):
         """bn_eps: eps of the neck's BatchNorm2d layers (rpn_v1.py:131-132 uses 1e-3; pass the module's own value otherwise)."""
-        dev = self.device
-        g = lambda k: ssfa_sd[k].to(dev, torch.float32)   # noqa: E731
-        P = {}
-
-        def bn(conv_name):
-            blk, idx = conv_name.rsplit(".", 1)
-            b = "%s.%d" % (blk, int(idx) + 1)
-            return fold_bn(g(b + ".weight"), g(b + ".bias"), g(b + ".running_mean"), g(b + ".running_var"), eps=bn_eps)
-
-        for name, pad in (("bottom_up_block_0.1", 1), ("bottom_up_block_0.4", 1), ("bottom_up_block_0.7", 1),
-                          ("bottom_up_block_1.0", 1), ("bottom_up_block_1.3", 1), ("bottom_up_block_1.6", 1),
-                          ("trans_0.0", 0), ("trans_1.0", 0), ("conv_0.0", 1), ("conv_1.0", 1)):
-            wp, taps = _pack_conv(g(name + ".weight"))
-            P[name] = (wp, [(dy - pad, dx - pad) for dy, dx in taps]) + bn(name)
-            if self.use_h2 and name != "bottom_up_block_1.0":
-                planes, inv = ops.pack_weight_h2(wp, -(-wp.shape[2] // 128) * 128)
-                sc_, sh_ = bn(name)
-                P[name + ":h2"] = (planes, (sc_ * inv[:sc_.numel()]).contiguous(), sh_)
-            elif self.use_tc and (self.TC_STRIDE2 or name != "bottom_up_block_1.0"):
-                P[name + ":tc"] = ops.pack_weight_tc(wp, -(-wp.shape[2] // 128) * 128)
-        for name in ("deconv_block_0.0", "deconv_block_1.0"):
-            classes = _deconv_classes(g(name + ".weight"))
-            P[name] = (classes,) + bn(name)
-            if self.use_tc:     # one launch for the four parity classes: plain 9-tap packing of W[cin][cout][ky][kx]
-                wd = g(name + ".weight")
-                w9 = wd.permute(2, 3, 0, 1).reshape(9, wd.shape[0], wd.shape[1]).contiguous()
-                if self.use_h2:
-                    planes, inv = ops.pack_weight_h2(w9, 128)
-                    sc_, sh_ = bn(name)
-                    P[name + ":h2"] = (planes, (sc_ * inv[:sc_.numel()]).contiguous(), sh_)
-                else:
-                    P[name + ":tc"] = ops.pack_weight_tc(w9, 128)
-        for name in ("w_0.0", "w_1.0"):
-            sc, sh = bn(name)
-            P[name] = (g(name + ".weight").reshape(-1).contiguous(), float(sc[0]), float(sh[0]))
-        if head_sd is not None:
-            hw, hb = pack_head(head_sd, head_prefix, dev, self.HEAD_STRIDE)
-            P["head"] = (hw, hb)
-            if self.use_h2:
-                planes, inv = ops.pack_weight_h2(hw, 32)
-                P["head:h2"] = (planes, inv.contiguous())
-            elif self.use_tc:
-                P["head:tc"] = ops.pack_weight_tc(hw, 32)
+        P = ssfa_fuse_weights(ssfa_sd, self.device, bn_eps)
+        for L, wp, taps, sc, sh in ssfa_weights(ssfa_sd, head_sd, head_prefix, self.device, bn_eps):
+            if L.kind == "conv":
+                P[L.name] = (wp, taps, sc, sh)
+            else:       # SIMT: four parity-class convs; tensor cores: one launch over the 9-tap packing
+                P[L.name] = (_deconv_classes(wp.reshape(3, 3, L.cin, L.cout).permute(2, 3, 0, 1)), sc, sh)
+            if self.use_h2 and L.stride == 1:
+                P[L.name + ":h2"] = pack_h2(wp, sc, sh, _cout_pad(L.cout))
+            elif self.use_tc and (self.TC_STRIDE2 or L.stride == 1):
+                P[L.name + ":tc"] = ops.pack_weight_tc(wp, _cout_pad(L.cout))
         self.params = P
 
-    def _am(self, i):
-        return None if i is None else self.amax[i:i + 1]
+    def _am(self, name):
+        return None if name is None else self.amax[SSFA_SLOT[name]:SSFA_SLOT[name] + 1]
 
-    def _conv(self, name, x, out, in_hw, out_hw, cin, cout, stride=1, relu=True, ai=None, ao=None):
-        """ai / ao: slots of self.amax holding the abs-max of the input / receiving the abs-max of the output (fp16-split scaling)."""
-        wp, taps, sc, sh = self.params[name]
-        d = ops.conv_desc(self.batch, in_hw, cin, out_hw, cout, out_hw, taps, in_stride=stride, relu=relu)
-        if (name + ":h2") in self.params:
-            planes, sc2, sh2 = self.params[name + ":h2"]
-            return ops.bev_conv_h2(x, planes, sc2, sh2, None, out, d, self._am(ai), self._am(ao))
-        if (name + ":tc") in self.params:
-            ops.bev_conv_tc(x, self.params[name + ":tc"], sc, sh, None, out, d)
+    def _launch(self, L, x, out, ai=None, ao=None):
+        """launch L from x into out.  ai / ao: tensors whose abs-max slot holds the abs-max of the input (default: L's input) / receives
+        the abs-max of the output (fp16-split scaling)"""
+        in_hw, out_hw = ssfa_extents(L, self.h, self.w)
+        resid = self.buf[L.residual] if L.residual else None
+        h2, tc = self.params.get(L.name + ":h2"), self.params.get(L.name + ":tc")
+        if L.kind == "conv":
+            wp, taps, sc, sh = self.params[L.name]
+            d = ops.conv_desc(self.batch, in_hw, L.cin, out_hw, L.cout, out_hw, taps, in_stride=L.stride, relu=L.relu)
+            if h2 is not None:
+                ops.bev_conv_h2(x, h2["w"], h2["scale"], h2["shift"], resid, out, d, self._am(ai or L.src), self._am(ao))
+            elif tc is not None:
+                ops.bev_conv_tc(x, tc, sc, sh, resid, out, d)
+            else:
+                ops.bev_conv(x, wp, sc, sh, resid, out, d)
         else:
-            ops.bev_conv(x, wp, sc, sh, None, out, d)
-        if self.use_h2 and ao is not None:
+            classes, sc, sh = self.params[L.name]
+            if h2 is not None:
+                ops.bev_deconv_h2(x, h2["w"], h2["scale"], h2["shift"], resid, out, L.relu, self._am(ai or L.src), self._am(ao))
+            elif tc is not None:
+                ops.bev_deconv_tc(x, tc, sc, sh, resid, out, relu=L.relu)
+            else:
+                for py, px, wp, taps in classes:
+                    d = ops.conv_desc(self.batch, in_hw, L.cin, out_hw, L.cout, in_hw, taps, in_stride=1, out_stride=2, out_off=(py, px),
+                                      relu=L.relu)
+                    ops.bev_conv(x, wp, sc, sh, resid, out, d)
+        if h2 is None and self.use_h2 and ao is not None:
             ops.absmax(out, self._am(ao))
-        return out
-
-    def _deconv(self, name, x, out, in_hw, out_hw, cin, cout, residual=None, ai=None, ao=None):
-        classes, sc, sh = self.params[name]
-        if (name + ":h2") in self.params:
-            planes, sc2, sh2 = self.params[name + ":h2"]
-            return ops.bev_deconv_h2(x, planes, sc2, sh2, residual, out, True, self._am(ai), self._am(ao))
-        tc = self.params.get(name + ":tc")
-        if tc is not None:
-            return ops.bev_deconv_tc(x, tc, sc, sh, residual, out, relu=True)
-        for py, px, wp, taps in classes:
-            d = ops.conv_desc(self.batch, in_hw, cin, out_hw, cout, in_hw, taps, in_stride=1, out_stride=2, out_off=(py, px), relu=True)
-            ops.bev_conv(x, wp, sc, sh, residual, out, d)
         return out
 
     def forward(self, x, mark=None):
@@ -403,36 +428,17 @@ class SSFARunner:
         assert self.params is not None, "load_state first"
         mark = mark or (lambda label: None)
         b = self.buf
-        H, H2 = (self.h, self.w), (self.h // 2, self.w // 2)
-
-        def conv(name, *a, **kw):
-            self._conv(name, *a, **kw)
-            mark("neck:" + name)
-
-        def deconv(name, *a, **kw):
-            self._deconv(name, *a, **kw)
-            mark("neck:" + name)
-
-        if self.use_h2:      # abs-max scalars: 0 x, 1 b0a, 2 b0b, 3 x0, 4 b1a, 5 b1b, 6 x1, 7 t1, 8 m0, 9 m1, 10 out
+        if self.use_h2:
             self.amax.zero_()
-            ops.absmax(x, self._am(0))
-        conv("bottom_up_block_0.1", x, b["b0a"], H, H, 128, 128, ai=0, ao=1)
-        conv("bottom_up_block_0.4", b["b0a"], b["b0b"], H, H, 128, 128, ai=1, ao=2)
-        conv("bottom_up_block_0.7", b["b0b"], b["x0"], H, H, 128, 128, ai=2, ao=3)
-        conv("bottom_up_block_1.0", b["x0"], b["b1a"], H, H2, 128, 256, stride=2, ai=3, ao=4)
-        conv("bottom_up_block_1.3", b["b1a"], b["b1b"], H2, H2, 256, 256, ai=4, ao=5)
-        conv("bottom_up_block_1.6", b["b1b"], b["x1"], H2, H2, 256, 256, ai=5, ao=6)
-        conv("trans_0.0", b["x0"], b["t0"], H, H, 128, 128, ai=3)
-        conv("trans_1.0", b["x1"], b["t1"], H2, H2, 256, 256, ai=6, ao=7)
-        deconv("deconv_block_0.0", b["t1"], b["m0"], H2, H, 256, 128, residual=b["t0"], ai=7, ao=8)
-        deconv("deconv_block_1.0", b["t1"], b["m1"], H2, H, 256, 128, ai=7, ao=9)
-        conv("conv_0.0", b["m0"], b["o0"], H, H, 128, 128, ai=8)
-        conv("conv_1.0", b["m1"], b["o1"], H, H, 128, 128, ai=9)
+            ops.absmax(x, self._am("x"))
+        for L in SSFA_LAUNCHES[:-1]:
+            self._launch(L, x if L.src == "x" else b[L.src], b[L.dst], ao=L.dst if L.dst in _SSFA_INPUTS else None)
+            mark("neck:" + L.name)
         w0, s0, t0 = self.params["w_0.0"]
         w1, s1, t1 = self.params["w_1.0"]
         ops.ssfa_fuse(b["o0"], b["o1"], w0, w1, s0, t0, s1, t1, b["out"])
         if self.use_h2 and "head" in self.params:
-            ops.absmax(b["out"], self._am(10))
+            ops.absmax(b["out"], self._am("out"))
         if "head" not in self.params:
             mark("neck:fuse+head")
             return b["out"], None
@@ -443,11 +449,9 @@ class SSFARunner:
     def bench_layer(self, name="bottom_up_block_0.4"):
         """(launch closure, kernel description) of one 3x3 128->128 layer on the buffers / abs-max slots a frame uses (valid after any
         forward): what bench.py times alone for the `roofline` object."""
-        H = (self.h, self.w)
-        x, out = self.buf["x0"], self.buf["b0b"]
 
         def launch():
-            self._conv(name, x, out, H, H, 128, 128, ai=3, ao=2)
+            self._launch(_SSFA[name], self.buf["x0"], self.buf["b0b"], ai="x0", ao="b0b")
 
         if (name + ":h2") in self.params:
             kern = "bev_conv_p2_kernel<.., kP2SplitF16> (fp32 input split to fp16 in shared memory, fp16 wgmma)"
@@ -458,15 +462,7 @@ class SSFARunner:
         return launch, kern
 
     def head(self, x):
-        hw, hb = self.params["head"]
-        H = (self.h, self.w)
-        d = ops.conv_desc(self.batch, H, 128, H, self.HEAD_STRIDE, H, [(0, 0)], relu=False)
-        if "head:h2" in self.params:
-            planes, inv = self.params["head:h2"]
-            return ops.bev_conv_h2(x, planes, inv, hb, None, self.buf["head"], d, self._am(10), None)
-        if "head:tc" in self.params:
-            return ops.bev_conv_tc(x, self.params["head:tc"], None, hb, None, self.buf["head"], d)
-        return ops.bev_conv(x, hw, None, hb, None, self.buf["head"], d)
+        return self._launch(SSFA_LAUNCHES[-1], x, self.buf["head"])
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -479,85 +475,51 @@ class SSFAPlanesRunner:
 
     HEAD_STRIDE = 24
     # info slots (each {abs-max, scale}); the whole table is zeroed once per forward
-    SLOT = dict(x=0, b0a=1, b0b=2, x0=3, b1a=4, b1b=5, x1=6, t1=7, m0=8, m1=9, out=10, t0=11, o0=12, o1=13, head=14)
+    SLOT = SSFA_SLOT
     # the conv / deconv launches of one forward, in the order of the skip plan's records (csrc/bevskip.cu)
-    SKIP_LAUNCHES = ("bottom_up_block_0.1", "bottom_up_block_0.4", "bottom_up_block_0.7", "bottom_up_block_1.0", "bottom_up_block_1.3",
-                     "bottom_up_block_1.6", "trans_0.0", "trans_1.0", "deconv_block_0.0", "deconv_block_1.0", "conv_0.0", "conv_1.0", "head")
+    SKIP_LAUNCHES = tuple(L.name for L in SSFA_LAUNCHES)
 
     def __init__(self, batch, hw=(200, 176), device="cuda", skip_constant=False):
         """skip_constant: when forward() gets the occupancy of the last sparse level, run only the work items whose output can differ
         from the empty-space constant of its class and fill the others with it (bit-identical to the dense neck, csrc/bevskip.cu)"""
         self.batch, self.h, self.w, self.device = batch, int(hw[0]), int(hw[1]), torch.device(device)
-        h, w, h2, w2 = self.h, self.w, self.h // 2, self.w // 2
-        pl = lambda hh, ww, c: ops.alloc_bev_planes(batch, hh, ww, c, self.device)     # noqa: E731
-        z = lambda hh, ww, c: torch.zeros((batch, hh, ww, c), dtype=torch.float32, device=self.device)  # noqa: E731
-        self.planes = dict(x=pl(h, w, 128), b0a=pl(h, w, 128), b0b=pl(h, w, 128), x0=pl(h, w, 128), b1a=pl(h2, w2, 256), b1b=pl(h2, w2, 256),
-                           x1=pl(h2, w2, 256), t1=pl(h2, w2, 256), m0=pl(h, w, 128), m1=pl(h, w, 128), out=pl(h, w, 128))
-        self.buf = dict(t0=z(h, w, 128), o0=z(h, w, 128), o1=z(h, w, 128), out=z(h, w, 128), head=z(h, w, self.HEAD_STRIDE))
+        pl = lambda hw_, c: ops.alloc_bev_planes(batch, hw_[0], hw_[1], c, self.device)     # noqa: E731
+        z = lambda hw_, c: torch.zeros((batch,) + hw_ + (c,), dtype=torch.float32, device=self.device)  # noqa: E731
+        H, ext = (self.h, self.w), lambda L: ssfa_extents(L, self.h, self.w)[1]     # noqa: E731
+        self.planes = dict(x=pl(H, 128), **{L.dst: pl(ext(L), L.cout) for L in SSFA_LAUNCHES if not L.f32}, out=pl(H, 128))
+        self.buf = dict(**{L.dst: z(ext(L), L.cout) for L in SSFA_LAUNCHES[:-1] if L.f32}, out=z(H, 128), head=z(H, self.HEAD_STRIDE))
         self.info = torch.zeros((16, 2), dtype=torch.float32, device=self.device)
         self.params = None
         self.skip_constant = bool(skip_constant)
-        self.skip = ops.BevSkipPlan(batch, h, w, self.device) if self.skip_constant else None
+        self.skip = ops.BevSkipPlan(batch, self.h, self.w, self.device) if self.skip_constant else None
 
     def _info(self, name):
         return self.info[self.SLOT[name]]
 
     def load_state(self, ssfa_sd, head_sd=None, head_prefix="tasks.0.", bn_eps=BN_EPS):
-        dev = self.device
-        g = lambda k: ssfa_sd[k].to(dev, torch.float32)   # noqa: E731
-        P = {}
-
-        def bn(conv_name):
-            blk, idx = conv_name.rsplit(".", 1)
-            b = "%s.%d" % (blk, int(idx) + 1)
-            return fold_bn(g(b + ".weight"), g(b + ".bias"), g(b + ".running_mean"), g(b + ".running_var"), eps=bn_eps)
-
-        def pack(name, wp, taps, cout_pad):
-            sc, sh = bn(name)
-            planes, inv = ops.pack_weight_h2(wp, cout_pad)
-            P[name] = dict(w=planes, taps=taps, scale=(sc * inv[:sc.numel()]).contiguous(), shift=sh.contiguous(),
-                           gain=ops.conv_gain(wp, sc), shift_max=float(sh.abs().max()))
-
-        for name, pad in (("bottom_up_block_0.1", 1), ("bottom_up_block_0.4", 1), ("bottom_up_block_0.7", 1), ("bottom_up_block_1.0", 1),
-                          ("bottom_up_block_1.3", 1), ("bottom_up_block_1.6", 1), ("trans_0.0", 0), ("trans_1.0", 0), ("conv_0.0", 1),
-                          ("conv_1.0", 1)):
-            wp, taps = _pack_conv(g(name + ".weight"))
-            pack(name, wp, [(dy - pad, dx - pad) for dy, dx in taps], -(-wp.shape[2] // 128) * 128)
-        for name in ("deconv_block_0.0", "deconv_block_1.0"):       # plain 9-tap packing of W[cin][cout][ky][kx]
-            wd = g(name + ".weight")
-            pack(name, wd.permute(2, 3, 0, 1).reshape(9, wd.shape[0], wd.shape[1]).contiguous(), None, 128)
-        for name in ("w_0.0", "w_1.0"):
-            sc, sh = bn(name)
-            P[name] = (g(name + ".weight").reshape(-1).contiguous(), float(sc[0]), float(sh[0]))
-        if head_sd is not None:
-            hw, hb = pack_head(head_sd, head_prefix, dev, self.HEAD_STRIDE)
-            planes, inv = ops.pack_weight_h2(hw, 32)
-            P["head"] = dict(w=planes, taps=[(0, 0)], scale=inv[: self.HEAD_STRIDE].contiguous(), shift=hb.contiguous(),
-                             gain=ops.conv_gain(hw, torch.ones(self.HEAD_STRIDE, device=dev)), shift_max=float(hb.abs().max()))
+        P = ssfa_fuse_weights(ssfa_sd, self.device, bn_eps)
+        for L, wp, taps, sc, sh in ssfa_weights(ssfa_sd, head_sd, head_prefix, self.device, bn_eps):
+            P[L.name] = dict(pack_h2(wp, sc, sh, _cout_pad(L.cout)), taps=taps)
         self.params = P
 
-    def _conv(self, name, src, dst, in_hw, out_hw, cin, cout, stride=1, relu=True, f32=None, skip=False):
-        """src: name of the input planes; dst: name of the output planes (or None); f32: name of an fp32 output buffer (or None);
-        skip: run the work items of this launch's skip-plan record, then fill the skipped tiles"""
-        q = self.params[name]
-        d = ops.conv_desc(self.batch, in_hw, cin, out_hw, cout, out_hw, q["taps"], in_stride=stride, relu=relu)
-        out_name = dst if dst is not None else f32
-        out_f32 = self.buf[f32] if f32 is not None else None
-        out_planes = self.planes[dst] if dst is not None else None
-        rec = self.skip.record(self.SKIP_LAUNCHES.index(name)) if skip else None
-        ops.bev_conv_p2(self.planes[src], self._info(src), q["w"], q["scale"], q["shift"], None, None, q["gain"], q["shift_max"],
-                        out_f32, out_planes, self._info(out_name), d, items=rec)
+    def _launch(self, L, skip=False):
+        """launch L from its input planes into its output planes or fp32 buffer.  skip: run the work items of this launch's skip-plan
+        record, then fill the skipped tiles"""
+        q = self.params[L.name]
+        out_f32, out_planes = (self.buf[L.dst], None) if L.f32 else (None, self.planes[L.dst])
+        resid, resid_info = (self.buf[L.residual], self._info(L.residual)) if L.residual else (None, None)
+        i = self.SKIP_LAUNCHES.index(L.name)
+        rec = self.skip.record(i) if skip else None
+        if L.kind == "conv":
+            in_hw, out_hw = ssfa_extents(L, self.h, self.w)
+            d = ops.conv_desc(self.batch, in_hw, L.cin, out_hw, L.cout, out_hw, q["taps"], in_stride=L.stride, relu=L.relu)
+            ops.bev_conv_p2(self.planes[L.src], self._info(L.src), q["w"], q["scale"], q["shift"], resid, resid_info, q["gain"],
+                            q["shift_max"], out_f32, out_planes, self._info(L.dst), d, items=rec)
+        else:
+            ops.bev_deconv_p2(self.planes[L.src], self._info(L.src), q["w"], q["scale"], q["shift"], resid, resid_info, q["gain"],
+                              q["shift_max"], out_f32, out_planes, self._info(L.dst), L.relu, items=rec)
         if skip:
-            self.skip.fill(self.SKIP_LAUNCHES.index(name), out_f32, out_planes, cout)
-
-    def _deconv(self, name, src, dst, residual=None, skip=False):
-        q = self.params[name]
-        rec = self.skip.record(self.SKIP_LAUNCHES.index(name)) if skip else None
-        ops.bev_deconv_p2(self.planes[src], self._info(src), q["w"], q["scale"], q["shift"], self.buf[residual] if residual else None,
-                          self._info(residual) if residual else None, q["gain"], q["shift_max"], None, self.planes[dst], self._info(dst), True,
-                          items=rec)
-        if skip:
-            self.skip.fill(self.SKIP_LAUNCHES.index(name), None, self.planes[dst], self.planes[dst].shape[-1])
+            self.skip.fill(i, out_f32, out_planes, L.cout)
 
     def forward(self, x=None, mark=None, occupancy=None):
         """x: NHWC fp32 [B,200,176,128] (converted to planes here) or None when self.planes['x'] / info slot 'x' were filled by the
@@ -566,7 +528,6 @@ class SSFAPlanesRunner:
         launches then skip the tiles of the empty space (the input must be exactly zero wherever that level has no site)."""
         assert self.params is not None, "load_state first"
         mark = mark or (lambda label: None)
-        H, H2 = (self.h, self.w), (self.h // 2, self.w // 2)
         if x is not None:
             self.info.zero_()
             ops.absmax(x, self.info[0, 0:1])
@@ -577,25 +538,9 @@ class SSFAPlanesRunner:
             assert (grid.batch, grid.shape[1], grid.shape[2]) == (self.batch, self.h, self.w), "occupancy of another map"
             self.skip.build(index, grid)
             mark("neck:skip_plan")
-
-        def conv(name, *a, **kw):
-            self._conv(name, *a, skip=skip, **kw)
-            mark("neck:" + name)
-
-        conv("bottom_up_block_0.1", "x", "b0a", H, H, 128, 128)
-        conv("bottom_up_block_0.4", "b0a", "b0b", H, H, 128, 128)
-        conv("bottom_up_block_0.7", "b0b", "x0", H, H, 128, 128)
-        conv("bottom_up_block_1.0", "x0", "b1a", H, H2, 128, 256, stride=2)
-        conv("bottom_up_block_1.3", "b1a", "b1b", H2, H2, 256, 256)
-        conv("bottom_up_block_1.6", "b1b", "x1", H2, H2, 256, 256)
-        conv("trans_0.0", "x0", None, H, H, 128, 128, f32="t0")
-        conv("trans_1.0", "x1", "t1", H2, H2, 256, 256)
-        self._deconv("deconv_block_0.0", "t1", "m0", residual="t0", skip=skip)
-        mark("neck:deconv_block_0.0")
-        self._deconv("deconv_block_1.0", "t1", "m1", skip=skip)
-        mark("neck:deconv_block_1.0")
-        conv("conv_0.0", "m0", None, H, H, 128, 128, f32="o0")
-        conv("conv_1.0", "m1", None, H, H, 128, 128, f32="o1")
+        for L in SSFA_LAUNCHES[:-1]:
+            self._launch(L, skip)
+            mark("neck:" + L.name)
         w0, s0, t0 = self.params["w_0.0"]
         w1, s1, t1 = self.params["w_1.0"]
         ops.ssfa_fuse_planes(self.buf["o0"], self.buf["o1"], w0, w1, s0, t0, s1, t1, self.buf["out"], self._info("o0"), self._info("o1"),
@@ -608,8 +553,7 @@ class SSFAPlanesRunner:
         return self.buf["out"], self.buf["head"]
 
     def head(self, skip=False):
-        H = (self.h, self.w)
-        self._conv("head", "out", None, H, H, 128, self.HEAD_STRIDE, relu=False, f32="head", skip=skip)
+        self._launch(SSFA_LAUNCHES[-1], skip)
         return self.buf["head"]
 
     def activation(self, name):
@@ -619,9 +563,7 @@ class SSFAPlanesRunner:
         return ops.planes_to_float(self.planes[name], self._info(name))
 
     def bench_layer(self, name="bottom_up_block_0.4"):
-        H = (self.h, self.w)
-
         def launch():
-            self._conv(name, "x0", "b0b", H, H, 128, 128)
+            self._launch(_SSFA[name]._replace(src="x0", dst="b0b"))
 
         return launch, "bev_conv_p2_kernel (fp16 wgmma from pre-split fp16 planes, two-term split)"

@@ -886,10 +886,11 @@ def test_p2_zero_map_is_exact():
 def test_p2_refuses_launches_beyond_its_limits():
     """descriptors the launcher cannot run return an error (ops.check raises) without a launch and leave the output alone; the expected
     refusals are those of p2_plan (test_launcher_limits_restated): > 6 patch copies, > 18 patch rows, > 9 taps, cin % 64, cout % 8, and
-    the stride-2 3x3 h2 conv at n_tile 128 (its fp32 staging leaves room for one weight stage)"""
+    the stride-2 3x3 h2 conv at n_tile 128 (its fp32 staging leaves room for one weight stage); and a skip-plan item list with weights
+    wider than round_up(cout, n_tile), whose item numbers would decode to other classes / n-blocks (conv and deconv)"""
     from sessd_b200 import _lib, ops
     bad = [dict(taps=[(0, dx) for dx in range(-3, 4)]), dict(taps=[(-2, 0), (0, 0), (1, 0)]), dict(taps=TAPS3 + [(2, 2)]),
-           dict(cin=96), dict(cout=44, cout_pad=128)]
+           dict(cin=96), dict(cout=44, cout_pad=128), dict(cout_pad=256, items=True)]
     for kw in bad:
         cin, cout = kw.get("cin", 64), kw.get("cout", 64)
         taps = kw.get("taps", TAPS3)
@@ -899,12 +900,19 @@ def test_p2_refuses_launches_beyond_its_limits():
         w = torch.zeros((2, len(taps), kw.get("cout_pad", 128), cin), dtype=torch.float16, device="cuda")
         sc = torch.ones(kw.get("cout_pad", 128), device="cuda")
         buf, out = _guarded((1, 16, 16, cout), torch.float32)
-        if len(taps) <= 9:
-            assert p2_plan("p2", cin, cout, kw.get("cout_pad", 128), [[(dy, dx, t) for t, (dy, dx) in enumerate(taps)]], 1, 16, 16, 1) is None
+        items = torch.zeros(64, dtype=torch.int32, device="cuda") if kw.get("items") else None
+        if len(taps) <= 9:      # beyond the geometry's limits, or (with items) a geometry that runs without the item list
+            assert (p2_plan("p2", cin, cout, kw.get("cout_pad", 128), [[(dy, dx, t) for t, (dy, dx) in enumerate(taps)]], 1, 16, 16, 1)
+                    is None) == (items is None)
         d = ops.conv_desc(1, (16, 16), cin, (16, 16), cout, (16, 16), taps)
         n0 = _lib.launch_count()
         with pytest.raises(_lib.SessdError):
-            ops.bev_conv_p2(planes, info, w, sc, None, None, None, 1.0, 0.0, out, None, torch.zeros(2, device="cuda"), d)
+            ops.bev_conv_p2(planes, info, w, sc, None, None, None, 1.0, 0.0, out, None, torch.zeros(2, device="cuda"), d, items=items)
+        if items is not None:
+            dbuf, dout = _guarded((1, 32, 32, cout), torch.float32)
+            with pytest.raises(_lib.SessdError):
+                ops.bev_deconv_p2(planes, info, w, sc, None, None, None, 1.0, 0.0, dout, None, torch.zeros(2, device="cuda"), items=items)
+            assert bool(_is_sentinel(dbuf).all())
         torch.cuda.synchronize()
         assert _lib.launch_count() == n0 and bool(_is_sentinel(buf).all()), kw
         del case

@@ -96,6 +96,27 @@ def test_conv_and_deconv_tap_packing_equals_torch():
     assert torch.allclose(full.permute(0, 3, 1, 2), ref, atol=1e-12)
 
 
+def test_skip_plan_records_follow_the_ssfa_launch_table():
+    """the C skip planner (csrc/bevskip.cu) lays out one record per launch of sessd_data.layers.SSFA_LAUNCHES, in table order, each of
+    32 + nclass * nblocks * tiles + 2 * nclass * tiles words under the launcher's geometry (restated by tests/skip_model.py)"""
+    import ctypes as C
+    import skip_model as sm
+    from sessd_b200._lib import lib
+    from sessd_b200.runners import SSFAPlanesRunner
+    from sessd_data.layers import SSFA_LAUNCHES, ssfa_extents
+    assert tuple(L.name for L in SSFA_LAUNCHES) == SSFAPlanesRunner.SKIP_LAUNCHES
+    assert tuple((L.dst, L.kind == "deconv", L.cout) for L in SSFA_LAUNCHES) == sm.LAUNCHES
+    for batch, h, w in ((1, 200, 176), (2, 48, 64), (1, 24, 16)):
+        offsets = (C.c_int * len(SSFA_LAUNCHES))()
+        words = lib.sessd_bev_skip_plan_words(batch, h, w, offsets)
+        expect = [0]
+        for L in SSFA_LAUNCHES:
+            src, dst = ssfa_extents(L, h, w)
+            g = sm.geometry(batch, *(src if L.kind == "deconv" else dst), L.cout, L.kind == "deconv")
+            expect.append(expect[-1] + sm.HEADER + g["nclass"] * g["nblocks"] * g["tiles"] + 2 * g["nclass"] * g["tiles"])
+        assert list(offsets) == expect[:-1] and words == expect[-1], (batch, h, w)
+
+
 def test_weight_split_and_bn_fold():
     from sessd_b200 import weights
     from sessd_b200.runners import SPMIDDLE_LAYERS, fold_bn
