@@ -127,7 +127,6 @@ def main():
     ap.add_argument("--batch", type=int, default=None)
     ap.add_argument("--points", type=int, default=None)
     ap.add_argument("--iters", type=int, default=5)
-    ap.add_argument("--sparse-tc", default=None, choices=["cg", "h2"], help="tensor-core kernel of the Cin >= 32 sparse layers (default: the runner's)")
     ap.add_argument("--cg-deep", type=int, default=0, help="1: deep pipeline, one CTA per SM")
     a = ap.parse_args()
     from sessd_b200._lib import lib
@@ -135,18 +134,17 @@ def main():
     if a.shape == "stress":
         B, N = a.batch or 8, a.points or 200000
         clouds = [synth.uniform_cloud(1000 + f, N) for f in range(B)]
-        eng = FrameEngine(batch=B, max_points_per_frame=N, max_voxels=200000, growth=(1.0, 8.0, 8.0, 8.0, 8.0), sparse_tc=a.sparse_tc)
+        eng = FrameEngine(batch=B, max_points_per_frame=N, max_voxels=200000, growth=(1.0, 8.0, 8.0, 8.0, 8.0))
         kind = "uniform"
     else:
         B, N = a.batch or 1, a.points or 20000
         kind = "ring" if a.shape == "frame" else "uniform"
         clouds = [(synth.ring_cloud if kind == "ring" else synth.uniform_cloud)(f, N) for f in range(B)]
-        eng = FrameEngine(batch=B, max_points_per_frame=max(c.shape[0] for c in clouds), sparse_tc=a.sparse_tc)
+        eng = FrameEngine(batch=B, max_points_per_frame=max(c.shape[0] for c in clouds))
     layers, ssfa, head = weights.bench_detector_state(kind, 0)
     eng.load_weights(layers, ssfa, head, weights.kitti_car_anchors())
     out = group_rooflines(eng, clouds, a.iters)
     out["shape"] = a.shape
-    out["sparse_tc"] = eng.middle.sparse_tc
     out["cg_deep"] = int(a.cg_deep)
     print(json.dumps(out))
 

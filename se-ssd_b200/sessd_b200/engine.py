@@ -17,9 +17,10 @@ from .runners import SpMiddleRunner, SSFAPlanesRunner, SSFARunner
 
 class FrameEngine:
     def __init__(self, batch=1, max_points_per_frame=32768, voxel_size=synth.VOXEL_SIZE, pc_range=synth.PC_RANGE,
-                 max_points_per_voxel=5, max_voxels=20000, device="cuda", post_kwargs=None, growth=None, use_tc=True, sparse_split=None, rows_max_cin=None,
-                 neck="planes", sparse_tc=None, skip_constant=True):
-        """skip_constant: the planes neck computes only the tiles whose receptive field reaches a LiDAR site or the map border and fills
+                 max_points_per_voxel=5, max_voxels=20000, device="cuda", post_kwargs=None, growth=None, use_tc=True, neck="planes",
+                 skip_constant=True):
+        """use_tc: tensor-core kernels in the sparse encoder (runners.SpMiddleRunner) and the neck; False = their fp32 SIMT baselines.
+        skip_constant: the planes neck computes only the tiles whose receptive field reaches a LiDAR site or the map border and fills
         the rest with their bit-identical empty-space constant (runners.SSFAPlanesRunner)"""
         self.batch, self.device = int(batch), torch.device(device)
         self.max_points = int(max_points_per_frame) * self.batch
@@ -32,8 +33,7 @@ class FrameEngine:
         self.d_points = torch.zeros((self.max_points, 4), dtype=torch.float32, device=dev)
         self.d_off = torch.zeros((self.batch + 1,), dtype=torch.int32, device=dev)
         self.vox = ops.VoxelBuffers(self.vcfg, self.batch, self.max_points, dev, with_mean=True)
-        self.middle = SpMiddleRunner(self.batch, self.batch * max_voxels, self.grid_xyz, 4, dev, growth=growth, use_tc=use_tc, split=sparse_split, rows_max_cin=rows_max_cin,
-                                     sparse_tc=sparse_tc)
+        self.middle = SpMiddleRunner(self.batch, self.batch * max_voxels, self.grid_xyz, 4, dev, growth=growth, use_tc=use_tc)
         self.neck_planes = neck == "planes" and use_tc
         if self.neck_planes:
             self.neck = SSFAPlanesRunner(self.batch, (self.grid_xyz[1] // 8, self.grid_xyz[0] // 8), dev, skip_constant=skip_constant)

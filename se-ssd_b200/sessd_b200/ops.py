@@ -164,30 +164,24 @@ def spconv_forward_rows(in_feat, nbr, n_out, max_out, weight, scale, shift, relu
     return out
 
 
-def pack_weight_sp_h2(wp, cp, layout="cg"):
-    """[kvol, Cin, Cout] (spconv layout, flattened offsets) -> (fp16 weight tiles of the tensor-core sparse convs, 2^-e[Cout]).
-    Every output channel is scaled by the power of two that puts its largest |w| into [2^10, 2^11); hi = fp16_rn(2^e w),
-    lo = fp16_rn(2^e w - hi).  cp = 64: [kvol, 2, Cout, 64]; cp = 32: layout "cg" (sessd_spconv_forward_cg): [kvol, 2, Cout, 32] (hi rows, then
-    lo rows), layout "h2": [kvol, Cout, 64] with hi in columns [0, Cin), lo in [32, 32+Cin)."""
-    kvol, cin, cout = wp.shape
-    assert cp in (32, 64) and cin <= cp and (cp == 32 or cin == 64)
-    wt = wp.permute(0, 2, 1).contiguous().to(torch.float32)                      # [kvol, Cout, Cin]
+def _fp16_split(wt):
+    """[taps, Cout, Cin] fp32 -> (hi, lo, 2^-e[Cout]): every output channel is scaled by the power of two 2^e[n] that puts its largest
+    |w| into [2^10, 2^11); hi = fp16_rn(2^e w), lo = fp16_rn(2^e w - hi)"""
     amax = wt.abs().amax(dim=(0, 2))
-    _, ex = torch.frexp(amax)
+    _, ex = torch.frexp(amax)                       # amax = m * 2^ex, m in [0.5, 1)
     e = torch.where(amax > 0, 11 - ex, torch.zeros_like(ex)).clamp(-100, 100).to(torch.float32)
     ws = wt * torch.exp2(e)[None, :, None]
     hi = ws.to(torch.float16)
-    lo = (ws - hi.to(torch.float32)).to(torch.float16)
-    if cp == 64:
-        tiles = torch.stack([hi, lo], 1).contiguous()                            # [kvol, 2, Cout, 64]
-    elif layout == "cg":
-        assert cin == 32
-        tiles = torch.stack([hi, lo], 1).contiguous()                            # [kvol, 2, Cout, 32]
-    else:
-        tiles = torch.zeros((kvol, cout, 64), dtype=torch.float16, device=wp.device)
-        tiles[:, :, :cin] = hi
-        tiles[:, :, 32:32 + cin] = lo
-    return tiles, torch.exp2(-e).contiguous()
+    return hi, (ws - hi.to(torch.float32)).to(torch.float16), torch.exp2(-e).contiguous()
+
+
+def pack_weight_sp_h2(wp, cp):
+    """[kvol, Cin, Cout] (spconv layout, flattened offsets) -> (fp16 weight tiles [kvol, 2 (hi, lo), Cout, cp] of
+    sessd_spconv_forward_cg, 2^-e[Cout]) at the plane width cp = Cin of the layer's input (32 or 64); the fp16 split of _fp16_split."""
+    kvol, cin, cout = wp.shape
+    assert cp in (32, 64) and cin == cp
+    hi, lo, inv = _fp16_split(wp.permute(0, 2, 1).contiguous().to(torch.float32))
+    return torch.stack([hi, lo], 1).contiguous(), inv
 
 
 def alloc_planes(max_rows, cp, device):
@@ -198,9 +192,6 @@ def alloc_planes(max_rows, cp, device):
 def absmax_rows(feat, n, max_rows, amax):
     check(lib.sessd_absmax_rows(_p(feat), _p(n), int(max_rows), int(feat.shape[1]), _p(amax), _st()), "sessd_absmax_rows")
     return amax
-
-
-SP_H2_ZERO_MODE = 1      # missing neighbours: 0 = read the all-zero last row, 1 = row index -1 (TMA OOB fill), 2 = row index rows (OOB)
 
 
 def spconv_forward_rows_planes(in_feat, nbr, n_out, max_out, weight, scale, shift, relu, amax_in, gain, shift_max, out, out_planes, out_info):
@@ -377,18 +368,12 @@ def bev_deconv_tc(x, weight_split, scale, shift, residual, out, relu=True):
 
 def pack_weight_h2(wp, cout_pad):
     """[taps, Cin, Cout] (SIMT packing) -> (planes fp16 [2, taps, cout_pad, Cin], exps [cout_pad] fp32 = 2^-e[n]) for sessd_bev_conv_p2 / _h2:
-    every output channel is scaled by the power of two 2^e[n] that puts its largest |w| into [2^10, 2^11); hi = fp16_rn(2^e w),
-    lo = fp16_rn(2^e w - hi).  The returned 2^-e[n] must be folded into the epilogue scale."""
+    the fp16 split of _fp16_split over the zero-padded weight.  The returned 2^-e[n] must be folded into the epilogue scale."""
     taps, cin, cout = wp.shape
     wt = torch.zeros((taps, cout_pad, cin), dtype=torch.float32, device=wp.device)
     wt[:, :cout] = wp.permute(0, 2, 1)
-    amax = wt.abs().amax(dim=(0, 2))
-    _, ex = torch.frexp(amax)                       # amax = m * 2^ex, m in [0.5, 1)
-    e = torch.where(amax > 0, 11 - ex, torch.zeros_like(ex)).clamp(-100, 100).to(torch.float32)
-    ws = wt * torch.exp2(e)[None, :, None]
-    hi = ws.to(torch.float16)
-    lo = (ws - hi.to(torch.float32)).to(torch.float16)
-    return torch.stack([hi, lo], 0).contiguous(), torch.exp2(-e).contiguous()
+    hi, lo, inv = _fp16_split(wt)
+    return torch.stack([hi, lo], 0).contiguous(), inv
 
 
 def bev_conv_h2(x, weight_h2, scale, shift, residual, out, desc, amax_in=None, amax_out=None):

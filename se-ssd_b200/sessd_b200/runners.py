@@ -24,105 +24,98 @@ def fold_bn(gamma, beta, mean, var, eps=BN_EPS):
     return scale.contiguous(), shift.contiguous()
 
 
+def sparse_impl(cin, use_tc=True):
+    """kernel of a sparse conv with cin input channels.  use_tc: "rows" (pair-proportional fp32 SIMT, csrc/spconv_rows.cu) up to 16
+    channels, "cg" (pair-proportional gather + fp16 wgmma with a two-term fp16 split, csrc/spconv_cg.cu) above; otherwise "simt" (the
+    output-stationary fp32 baseline, csrc/spconv.cu) for every layer"""
+    if not use_tc:
+        return "simt"
+    return "rows" if cin <= 16 else "cg"
+
+
+def plane_width(channels):
+    """cp of the fp16 (hi, lo) planes [rows, 2 cp] of a sparse feature tensor, and of the weight tiles of the cg layer that reads them"""
+    return 32 if channels <= 32 else 64
+
+
+def spmiddle_plan(use_tc=True, keep_f32=False, cin0=4):
+    """One record per conv of SpMiddleFHD (SPMIDDLE_LAYERS): its kernel and the operands it reads and writes.
+      kind, key, ks, st, pd, cin, cout: the layer;  lin / lout: its input / output level (a strided conv opens the next level)
+      rb: its rulebook, the SubM indice key or "sp<lout>" for a strided conv;  build_rb: this layer builds it (the first to use it)
+      tile_lists: (with build_rb) the per-tile pair lists are made from it, because a cg layer gathers over it
+      impl: "rows" / "cg" / "simt" (sparse_impl);  cp_in: width of the input planes and of the packed weight of a cg layer, None for
+        the layers that read fp32 rows
+      cp_out: width of the output planes the layer writes for a cg successor, or None;  out_f32: it writes fp32 rows
+      out_info: it writes its {abs-max, scale} info slot: every cg layer and every layer that writes planes; a rows layer without planes
+        writes only the abs-max, for a successor that derives its planes' scale from that bound"""
+    plan, cin, lvl = [], cin0, 0
+    for kind, cout, ks, st, pd, key in SPMIDDLE_LAYERS:
+        lout = lvl if kind == "subm" else lvl + 1
+        rb = key if kind == "subm" else "sp%d" % lout
+        impl = sparse_impl(cin, use_tc)
+        plan.append(dict(kind=kind, key=key, ks=ks, st=st, pd=pd, cin=cin, cout=cout, lin=lvl, lout=lout, rb=rb,
+                         build_rb=all(p["rb"] != rb for p in plan), impl=impl, cp_in=plane_width(cin) if impl == "cg" else None))
+        cin, lvl = cout, lout
+    nxt = {}
+    for p in reversed(plan):
+        p["tile_lists"] = p["build_rb"] and any(q["impl"] == "cg" for q in plan if q["rb"] == p["rb"])
+        p["cp_out"] = nxt.get("cp_in")
+        p["out_f32"] = keep_f32 or p["cp_out"] is None
+        p["out_info"] = p["impl"] == "cg" or p["cp_out"] is not None or (nxt.get("impl") == "rows" and nxt["cp_out"] is not None)
+        nxt = p
+    return plan
+
+
 class SpMiddleRunner:
-    """SpMiddleFHD forward (scn.py:176-189): 4 SubM rulebooks + 4 strided rulebooks + 14 fused conv launches + dense()."""
+    """SpMiddleFHD forward (scn.py:176-189): 4 SubM rulebooks + 4 strided rulebooks + 14 fused conv launches + dense(), as laid
+    out by spmiddle_plan."""
 
     # active-site growth bounds per level relative to the level-0 capacity (uniform 20k cloud: 3.4 / 5.2 / 4.3 / 2.6)
     GROWTH = (1.0, 4.0, 6.0, 5.0, 3.0)
-    SPLIT = "fp16"
-    SPARSE_TC = "cg"          # tensor-core kernel of the Cin >= 32 layers: pair-proportional cp.async gather, planes written by the
-                              # producing layer's epilogue (csrc/spconv_cg.cu)
-    ROWS_SHAPES = ((4, 16), (16, 16), (16, 32), (32, 32))     # (Cin, Cout) whose whole weight tensor fits in shared memory
-    ROWS_MAX_CIN = 16         # layers with Cin <= this run on the pair-proportional SIMT kernel (0: tensor-core kernels wherever possible)
-    DENSE_GATHER = True       # dense() as one gather pass through the last level's bitmap index (False: memset + scatter)
 
     def __init__(self, batch, max_voxels_total, input_shape_xyz=(1408, 1600, 40), num_input_features=4, device="cuda",
-                 growth=None, use_tc=True, split=None, rows_max_cin=None, sparse_tc=None, keep_f32=False):
-        """use_tc: run the Cin >= 32 layers on the tensor cores (fp16 wgmma with a two-term fp16 split, csrc/spconv_cg.cu) and the
-        narrow layers on the pair-proportional SIMT kernel; False = fp32 SIMT baseline for all layers.  split / sparse_tc: "fp16" / "cg",
-        the only tensor-core variant."""
+                 growth=None, use_tc=True, keep_f32=False):
+        """use_tc: the narrow layers on the pair-proportional fp32 SIMT kernel and the others on the tensor cores, activations handed
+        from layer to layer as fp16 (hi, lo) planes; False = the fp32 SIMT baseline for every layer (sparse_impl).
+        keep_f32: the layers that hand planes to the next one write their fp32 rows as well (tests compare per-layer features)."""
         self.batch, self.device = batch, torch.device(device)
-        self.use_tc = bool(use_tc)
-        self.split = split or self.SPLIT
-        assert self.split == "fp16", "the sparse tensor-core layers use the two-term fp16 split"
-        self.use_h2 = self.use_tc
-        self.sparse_tc = sparse_tc or self.SPARSE_TC
-        assert self.sparse_tc == "cg"
-        self.keep_f32 = bool(keep_f32)      # cg layers also write their fp32 rows (tests compare per-layer features)
-        # per-layer kernel: "rows" = pair-proportional fp32 SIMT (narrow layers), "cg" = pair-proportional fp16-split wgmma,
-        # "simt" = the dense output-stationary fp32 baseline
-        self.rows_max_cin = (self.ROWS_MAX_CIN if rows_max_cin is None else int(rows_max_cin)) if self.use_tc else 0
-        self.cin0 = num_input_features
+        self.use_tc, self.keep_f32 = bool(use_tc), bool(keep_f32)
         shape = (int(input_shape_xyz[2]) + 1, int(input_shape_xyz[1]), int(input_shape_xyz[0]))   # scn.py:179
         growth = growth or self.GROWTH
         self.levels = []       # dicts: shape, cap, grid, coors, n, index_kind, index, scratch
-        self.plan = []         # per layer: (kind, level_in, level_out, nbr tensor, cin, cout)
-        lvl = 0
         self._add_level(shape, int(max_voxels_total), hash_index=True)
-        cin = num_input_features
-        subm_nbr = {}
-        for li, (kind, cout, ks, st, pd, key) in enumerate(SPMIDDLE_LAYERS):
-            kvol = ks[0] * ks[1] * ks[2]
-            if kind == "subm":
-                if key not in subm_nbr:
-                    subm_nbr[key] = torch.empty((self.levels[lvl]["cap"], kvol), dtype=torch.int32, device=self.device)
-                self.plan.append(dict(kind=kind, lin=lvl, lout=lvl, nbr=subm_nbr[key], cin=cin, cout=cout, ks=ks, st=st, pd=pd,
-                                      key=key, first=len([p for p in self.plan if p.get("key") == key]) == 0))
-            else:
-                oshape = conv_out_shape(self.levels[lvl]["shape"], ks, st, pd)
+        self.plan = spmiddle_plan(self.use_tc, self.keep_f32, num_input_features)
+        rulebooks = {}         # rb -> (neighbour table, tile lists or None), shared by the layers of a SubM key
+        for p in self.plan:
+            if p["kind"] != "subm":
+                oshape = conv_out_shape(self.levels[p["lin"]]["shape"], p["ks"], p["st"], p["pd"])
                 cells = batch * oshape[0] * oshape[1] * oshape[2]
-                cap = min(cells, int(math.ceil(max_voxels_total * growth[lvl + 1])))
-                self._add_level(oshape, cap, hash_index=False)
-                nbr = torch.empty((cap, kvol), dtype=torch.int32, device=self.device)
-                self.plan.append(dict(kind=kind, lin=lvl, lout=lvl + 1, nbr=nbr, cin=cin, cout=cout, ks=ks, st=st, pd=pd, key=None))
-                lvl += 1
-            cin = cout
-        self.feats = [torch.zeros((self.levels[p["lout"]]["cap"], p["cout"]), dtype=torch.float32, device=self.device)
-                      for p in self.plan]
+                self._add_level(oshape, min(cells, int(math.ceil(max_voxels_total * growth[p["lout"]]))), hash_index=False)
+            if p["build_rb"]:
+                cap, kvol = self.levels[p["lout"]]["cap"], p["ks"][0] * p["ks"][1] * p["ks"][2]
+                rulebooks[p["rb"]] = (torch.empty((cap, kvol), dtype=torch.int32, device=self.device),
+                                      ops.alloc_tile_lists(cap, kvol, self.device) if p["tile_lists"] else None)
+            p["nbr"], p["tiles"] = rulebooks[p["rb"]]
+        caps = [self.levels[p["lout"]]["cap"] for p in self.plan]
+        self.feats = [torch.zeros((cap, p["cout"]), dtype=torch.float32, device=self.device) if p["out_f32"] else None
+                      for p, cap in zip(self.plan, caps)]
+        self.planes = [ops.alloc_planes(cap, p["cp_out"], self.device) if p["cp_out"] else None for p, cap in zip(self.plan, caps)]
+        # a cg layer's tile lists address its input plane rows with 25 bits (input row << 7 | tile row)
+        assert all(pl is None or pl.shape[0] <= (1 << 25) for pl in self.planes)
         last = self.levels[-1]
         self.out_channels = self.plan[-1]["cout"] * last["shape"][0]
         self.dense = torch.zeros((batch, last["shape"][1], last["shape"][2], self.out_channels), dtype=torch.float32,
                                  device=self.device)
         self.status = torch.zeros((1,), dtype=torch.int32, device=self.device)
         self.weights = None
-        # fp16-split path: (hi, lo) planes of every layer output that feeds a tensor-core layer + one abs-max scalar per tensor
-        self.planes = [None] * len(self.plan)
-        self.amax = torch.zeros((len(self.plan) + 1,), dtype=torch.float32, device=self.device)
-        for p in self.plan:
-            if self.use_tc and p["cin"] <= self.rows_max_cin and (p["cin"], p["cout"]) in self.ROWS_SHAPES:
-                p["impl"] = "rows"
-            elif self.use_h2 and p["cin"] >= 32:
-                p["impl"] = "cg"
-            else:
-                p["impl"] = "simt"
-        for li, p in enumerate(self.plan):
-            # a cg layer reads the planes its producer's epilogue writes: the pair-proportional kernels write them, the baseline does not
-            assert p["impl"] != "cg" or self.plan[li - 1]["impl"] in ("rows", "cg"), "rows_max_cin too small for the tensor-core chain"
-        for li, p in enumerate(self.plan[:-1]):
-            if self.plan[li + 1]["impl"] == "cg":
-                cp = 64 if p["cout"] > 32 else 32
-                self.planes[li] = ops.alloc_planes(self.levels[p["lout"]]["cap"], cp, self.device)
-                assert self.planes[li].shape[0] <= (1 << 25)
-        # per-tile pair lists of every rulebook a cg layer reads (one per nbr table; a SubM rulebook is shared by its layers)
-        for p in self.plan:
-            p["tiles"] = None
-        by_nbr = {}
-        for p in self.plan:
-            if p["impl"] == "cg":
-                key = p["nbr"].data_ptr()
-                if key not in by_nbr:
-                    by_nbr[key] = ops.alloc_tile_lists(p["nbr"].shape[0], p["nbr"].shape[1], self.device)
-                p["tiles"] = by_nbr[key]
-        # {abs-max, plane scale} of every layer output (cg chain: written by the producing layer's epilogue)
+        # {abs-max, plane scale} of every layer output (out_info)
         self.info = torch.zeros((len(self.plan), 2), dtype=torch.float32, device=self.device)
 
     def layer_output(self, li):
         """fp32 rows [cap, Cout] of layer li's output after forward(): the fp32 buffer when the layer wrote it, else rebuilt from the fp16
-        (hi, lo) planes the next layer reads (exact: x = (hi + lo) / S) -- tests / debugging."""
+        (hi, lo) planes it wrote (exact: x = (hi + lo) / S) -- tests / debugging."""
         p = self.plan[li]
-        nxt = self.plan[li + 1]["impl"] if li + 1 < len(self.plan) else None
-        planes_only = (not self.keep_f32) and nxt == "cg" and p["impl"] in ("cg", "rows")
-        if not planes_only:
+        if p["out_f32"]:
             return self.feats[li]
         return ops.sparse_planes_to_float(self.planes[li][:-1], self.info[li], p["cout"])
 
@@ -148,12 +141,12 @@ class SpMiddleRunner:
             assert tuple(w.shape) == (*p["ks"], p["cin"], p["cout"]), (w.shape, p)
             sc, sh = fold_bn(*[torch.as_tensor(l[k], device=self.device) for k in ("gamma", "beta", "mean", "var")], eps=float(l.get("eps", BN_EPS)))
             wp = w.reshape(-1, p["cin"], p["cout"]).contiguous()
-            tc = None
-            if p["impl"] == "cg":
-                tiles, inv = ops.pack_weight_sp_h2(wp, 64 if p["cin"] > 32 else 32, layout="cg")
-                tc = (p["impl"], tiles, (sc * inv).contiguous())
             p["gain"], p["shift_max"] = ops.conv_gain(wp, sc), float(sh.abs().max())
-            self.weights.append((wp, sc, sh, tc))
+            if p["impl"] == "cg":      # fp16 (hi, lo) weight tiles; their per-channel 2^-e folds into the BN scale
+                tiles, inv = ops.pack_weight_sp_h2(wp, p["cp_in"])
+                self.weights.append((tiles, (sc * inv).contiguous(), sh))
+            else:
+                self.weights.append((wp, sc, sh))
 
     def forward(self, feat0, coors0, n0, mark=None, dense_planes=None):
         """feat0 [cap0, Cin] f32, coors0 [cap0,4] i32 (b,z,y,x), n0 [1] i32 (device).  Returns dense NHWC.
@@ -163,66 +156,49 @@ class SpMiddleRunner:
         mark = mark or (lambda label: None)
         assert self.weights is not None, "load_weights first"
         L0 = self.levels[0]
-        assert coors0.shape[0] <= L0["cap"] or True
         cap0 = min(coors0.shape[0], L0["cap"])
         L0["coors"], L0["n_ext"] = coors0, n0
         ops.hash_build(coors0, n0, cap0, L0["grid"], L0["index"])
         mark("hash_build")
-        if self.use_h2:
-            self.amax.zero_()
+        if self.use_tc:
             self.info.zero_()
         x = feat0
         for li, p in enumerate(self.plan):
             lin, lout = self.levels[p["lin"]], self.levels[p["lout"]]
             n_in = lin["n_ext"] if p["lin"] == 0 else lin["n"]
             cap_in = cap0 if p["lin"] == 0 else lin["cap"]
-            if p["kind"] == "subm":
-                if p["first"]:
+            n_out, cap_out = (n_in, cap_in) if p["kind"] == "subm" else (lout["n"], lout["cap"])
+            if p["build_rb"]:
+                if p["kind"] == "subm":
                     ops.subm_rulebook(lin["coors"], n_in, cap_in, lin["grid"], p["ks"], lin["index_kind"], lin["index"], p["nbr"])
-                    tl = next((q["tiles"] for q in self.plan if q.get("key") == p["key"] and q["tiles"] is not None), None)
-                    if tl is not None:
-                        ops.rulebook_tile_lists(p["nbr"], n_in, cap_in, tl)
-                    mark("rulebook:%s" % p["key"])
-                n_out, cap_out = n_in, cap_in
-            else:
-                ops.strided_rulebook(lin["coors"], n_in, cap_in, lin["grid"], lin["index_kind"], lin["index"], p["ks"], p["st"],
-                                     p["pd"], lout["grid"], lout["index"], lout["scratch"], lout["coors"], lout["n"], lout["cap"],
-                                     p["nbr"], self.status)
-                n_out, cap_out = lout["n"], lout["cap"]
+                else:
+                    ops.strided_rulebook(lin["coors"], n_in, cap_in, lin["grid"], lin["index_kind"], lin["index"], p["ks"], p["st"],
+                                         p["pd"], lout["grid"], lout["index"], lout["scratch"], lout["coors"], lout["n"], lout["cap"],
+                                         p["nbr"], self.status)
                 if p["tiles"] is not None:
                     ops.rulebook_tile_lists(p["nbr"], n_out, cap_out, p["tiles"])
-                mark("rulebook:sp%d" % p["lout"])
-            w, sc, sh, tc = self.weights[li]
-            nxt = self.plan[li + 1]["impl"] if li + 1 < len(self.plan) else None
-            if p["impl"] == "rows" and nxt == "cg":
-                # last SIMT layer before the tensor-core chain: writes the planes the next layer reads (scale from the bound on its output)
+                mark("rulebook:" + p["rb"])
+            w, sc, sh = self.weights[li]
+            out = self.feats[li]
+            if p["impl"] == "rows" and p["cp_out"]:
+                # the planes' scale comes from the bound on the output: the input's abs-max (info slot of layer li - 1) x gain + shift_max
                 ops.spconv_forward_rows_planes(x, p["nbr"], n_out, cap_out, w, sc, sh, True, self.info[li - 1, 0:1], p["gain"], p["shift_max"],
-                                               self.feats[li] if self.keep_f32 else None, self.planes[li], self.info[li])
-                x = self.feats[li]
+                                               out, self.planes[li], self.info[li])
             elif p["impl"] == "rows":
-                need_amax = self.planes[li] is not None or (nxt == "rows" and li + 2 < len(self.plan) and self.plan[li + 2]["impl"] == "cg")
-                x = ops.spconv_forward_rows(x, p["nbr"], n_out, cap_out, w, sc, sh, True, self.feats[li],
-                                            self.info[li, 0:1] if need_amax else None)
-            elif isinstance(tc, tuple) and tc[0] == "cg":
-                last = nxt != "cg"
-                ops.spconv_forward_cg(self.planes[li - 1], self.info[li - 1], p["tiles"], n_out, cap_out, tc[1], tc[2], sh, True, p["gain"],
-                                      p["shift_max"], self.feats[li] if (last or self.keep_f32) else None,
-                                      None if last else self.planes[li], self.info[li])
-                x = self.feats[li]
+                ops.spconv_forward_rows(x, p["nbr"], n_out, cap_out, w, sc, sh, True, out, self.info[li, 0:1] if p["out_info"] else None)
+            elif p["impl"] == "cg":
+                ops.spconv_forward_cg(self.planes[li - 1], self.info[li - 1], p["tiles"], n_out, cap_out, w, sc, sh, True, p["gain"],
+                                      p["shift_max"], out, self.planes[li], self.info[li])
             else:
-                x = ops.spconv_forward(x, p["nbr"], n_out, cap_out, w, sc, sh, True, self.feats[li])
+                ops.spconv_forward(x, p["nbr"], n_out, cap_out, w, sc, sh, True, out)
             mark("conv:%d" % li)
+            x = out
         last = self.levels[-1]
         if dense_planes is not None:
-            assert last["index_kind"] == 1 and self.use_h2
-            assert self.plan[-1]["impl"] == "cg"
-            out = ops.sparse_to_dense_planes(x, last["index"], last["grid"], self.info[len(self.plan) - 1, 0:1], dense_planes[1], dense_planes[0])
-            mark("dense")
-            return out
-        if last["index_kind"] == 1 and self.DENSE_GATHER:
-            out = ops.sparse_to_dense_indexed(x, last["index"], last["grid"], self.dense)
+            assert self.plan[-1]["out_info"], "the planes' scale needs the last layer's abs-max (use_tc)"
+            out = ops.sparse_to_dense_planes(x, last["index"], last["grid"], self.info[-1, 0:1], dense_planes[1], dense_planes[0])
         else:
-            out = ops.sparse_to_dense(x, last["coors"], last["n"], last["cap"], last["grid"], self.dense)
+            out = ops.sparse_to_dense_indexed(x, last["index"], last["grid"], self.dense)
         mark("dense")
         return out
 

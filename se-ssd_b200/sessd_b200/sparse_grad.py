@@ -1,11 +1,12 @@
 """Autograd through the sparse middle encoder (SpMiddleFHD in train mode, det3d/models/backbones/scn.py:176-189).
 
 One conv of ``middle_conv`` is one ``SparseConvFunction``; BatchNorm1d and ReLU stay the torch modules they are (batch statistics and
-running-stat updates exactly as the reference), and ``dense()`` is ``DenseFunction``.  Per layer (``impl``):
+running-stat updates exactly as the reference), and ``dense()`` is ``DenseFunction``.  Per layer (``impl``, ``conv_impl``: runners.sparse_impl, the rule
+of the inference runner):
 
 * ``rows`` (Cin <= 16): forward on the fp32 pair-proportional kernel (spconv_rows.cu), data gradient on the same kernel with re-packed
   weights, weight gradient on the fp32 SIMT wgrad kernel;
-* ``cg`` (Cin >= 32): the input rows are split into fp16 (hi, lo) planes (sparse_split_planes) for the tensor-core forward
+* ``cg`` (the wider layers): the input rows are split into fp16 (hi, lo) planes (sparse_split_planes) for the tensor-core forward
   (spconv_cg.cu), the output gradient likewise for the data gradient (the forward kernel again) and the tensor-core wgrad kernel.
 
 Data gradient through the forward kernels: a SubM layer's table is point-symmetric, so the same table / tile lists serve with
@@ -14,9 +15,10 @@ Rulebooks, nbr_t and tile lists are built once per rulebook (``ConvRulebook``) a
 import torch
 
 from . import ops
+from .runners import plane_width, sparse_impl
 from .train import subm_dgrad_weight
 
-ROWS_MAX_CIN = 16
+conv_impl = sparse_impl     # kernel of a training conv: the inference runner's rule, with the tensor-core kernels
 
 
 class ConvRulebook:
@@ -63,10 +65,6 @@ class ConvRulebook:
         return out
 
 
-def conv_impl(cin):
-    return "rows" if cin <= ROWS_MAX_CIN else "cg"
-
-
 def _split(x, n_t, n):
     """fp32 rows [n, C] -> (planes [n + 1, 2 C], info {abs-max, scale}); the extra row stays zero"""
     c = int(x.shape[1])
@@ -96,7 +94,7 @@ class SparseConvFunction(torch.autograd.Function):
             saved = (feat,)
         else:
             planes, info = _split(x, rb.n_in_t, rb.n_in)
-            w_h2, inv = ops.pack_weight_sp_h2(w, cin, layout="cg")
+            w_h2, inv = ops.pack_weight_sp_h2(w, plane_width(cin))
             ops.spconv_forward_cg(planes, info, rb.tiles(), rb.n_out_t, rb.cap_out, w_h2, inv, None, False, 0.0, 0.0, out, None, None)
             saved = (planes, info)
         # through save_for_backward: an in-place change of the input or the weight between forward and backward raises
@@ -134,7 +132,7 @@ class SparseConvFunction(torch.autograd.Function):
                 planes, info = saved
                 gw = ops.spconv_wgrad_cg(planes, info, g_planes, g_info, rb.tiles(), rb.n_out_t, rb.cap_out, kvol).reshape(w5.shape)
             if want_x:
-                wd_h2, inv = ops.pack_weight_sp_h2(wd, cout, layout="cg")
+                wd_h2, inv = ops.pack_weight_sp_h2(wd, plane_width(cout))
                 ops.spconv_forward_cg(g_planes, g_info, tiles, rb.n_in_t, rb.cap_in, wd_h2, inv, None, False, 0.0, 0.0, gin, None, None)
                 gfeat = gin[:rb.n_in]
         return gfeat, gw, None

@@ -91,9 +91,9 @@ def _weights(seed=3):
     return weights.split_detector_state(sd)
 
 
-@pytest.mark.parametrize("use_tc,split,rows,kw", [(False, None, 0, {}), (True, "fp16", 16, dict(sparse_tc="cg", keep_f32=True)), (True, "fp16", 16, {})],
-                         ids=["simt", "rows16+pair-gather+f32rows", "rows16+pair-gather(default)"])
-def test_spmiddle_features_match_fp64_oracle(use_tc, split, rows, kw):
+@pytest.mark.parametrize("use_tc,kw", [(False, {}), (True, dict(keep_f32=True)), (True, {})],
+                         ids=["simt14", "rows3+cg11+f32rows", "rows3+cg11(default)"])
+def test_spmiddle_features_match_fp64_oracle(use_tc, kw):
     from oracle import spconv_ref as S
     from sessd_b200 import synth
     from sessd_b200.runners import SpMiddleRunner
@@ -105,10 +105,9 @@ def test_spmiddle_features_match_fp64_oracle(use_tc, split, rows, kw):
                    var=l["var"].numpy()) for l in layers]
     trace = []
     ref = S.spmiddle_forward(feat, coors, 1, (1408, 1600, 40), params, np.float64, trace)   # [1,128,200,176]
-    r = SpMiddleRunner(1, n, device="cuda", use_tc=use_tc, split=split, rows_max_cin=rows, **kw)
-    assert [p["impl"] for p in r.plan].count("rows") == {0: 0, 16: 3, 32: 5}[rows]
-    if use_tc and split == "fp16" and rows == 16:
-        assert [p["impl"] for p in r.plan].count(kw.get("sparse_tc", "cg")) == 11
+    r = SpMiddleRunner(1, n, device="cuda", use_tc=use_tc, **kw)
+    impls = [p["impl"] for p in r.plan]
+    assert (impls.count("rows"), impls.count("cg"), impls.count("simt")) == ((3, 11, 0) if use_tc else (0, 0, 14))
     r.load_weights(layers)
     dense = r.forward(torch.from_numpy(feat).cuda(), torch.from_numpy(coors).cuda(), torch.tensor([n], dtype=torch.int32, device="cuda"))
     torch.cuda.synchronize()

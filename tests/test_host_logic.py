@@ -156,28 +156,58 @@ def test_frame_sharding_two_ranks_gloo(tmp_path):
     assert out.stdout.count("ok") == 2
 
 
-def test_sparse_fp16_split_weight_packing_layout_and_precision():
-    """ops.pack_weight_sp_h2: tile layouts the TMA maps of spconv_h2.cu assume, per-channel power-of-two scales, hi + lo == scaled weight
-    to fp16-split precision (22+ significand bits)."""
+def test_sparse_cg_weight_packing_layout_and_precision():
+    """ops.pack_weight_sp_h2: the tile layout of the pair-gather kernel (spconv_cg.cu), per-channel power-of-two scales, hi + lo == scaled
+    weight to fp16-split precision (22+ significand bits)."""
     from sessd_b200 import ops
     g = torch.Generator().manual_seed(3)
-    for cin, cout, cp, layout in ((64, 64, 64, "cg"), (32, 32, 32, "cg"), (32, 64, 32, "cg"), (32, 32, 32, "h2"), (16, 32, 32, "h2")):
+    for cin, cout, cp in ((64, 64, 64), (32, 32, 32), (32, 64, 32)):
         w = torch.randn(27, cin, cout, generator=g) * torch.logspace(-3, 1, cout)[None, None, :]      # channel scales over 4 decades
-        tiles, inv = ops.pack_weight_sp_h2(w, cp, layout=layout)
+        tiles, inv = ops.pack_weight_sp_h2(w, cp)
         assert tiles.dtype == torch.float16 and inv.shape == (cout,)
         ex = torch.log2(inv)
         assert torch.equal(ex, ex.round())                                   # exact powers of two
         scaled = w.permute(0, 2, 1) / inv[None, :, None]                     # [kvol, cout, cin] * 2^e
         assert float(scaled.abs().amax()) < 2048.0 and float(scaled.abs().amax(dim=(0, 2)).min()) >= 1024.0
-        if cp == 64 or layout == "cg":                                       # [kvol, 2 (hi | lo), Cout, Cin]: the pair-gather kernel's tiles
-            assert tuple(tiles.shape) == (27, 2, cout, cin)
-            hi, lo = tiles[:, 0].float(), tiles[:, 1].float()
-        else:
-            assert tuple(tiles.shape) == (27, cout, 64)
-            hi, lo = tiles[:, :, :cin].float(), tiles[:, :, 32:32 + cin].float()
-            assert not tiles[:, :, cin:32].any() and not tiles[:, :, 32 + cin:].any()     # zero padding of the 16-channel layers
+        assert tuple(tiles.shape) == (27, 2, cout, cin)                      # [kvol, 2 (hi | lo), Cout, Cin]
+        hi, lo = tiles[:, 0].float(), tiles[:, 1].float()
         err = (hi + lo - scaled).abs().max() / scaled.abs().max()
         assert float(err) < 2.0 ** -21
+
+
+def test_spmiddle_layer_plan_pins_each_conv_kernel_and_operands():
+    """runners.spmiddle_plan for both modes against the per-layer choices of the runner it replaced, written out by hand; and the
+    training path (sparse_grad on the SpMiddleFHD module's convs) picks the plan's kernel and plane width for every layer."""
+    import spconv
+    from det3d.models.backbones.scn import SpMiddleFHD
+    from sessd_b200 import sparse_grad
+    from sessd_b200.runners import plane_width, spmiddle_plan
+    lout = [0, 0, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4]
+    builders = dict(subm0=0, sp1=2, subm1=3, sp2=5, subm2=6, sp3=9, subm3=10, sp4=13)     # rulebook -> the layer that builds it
+    # (impl, cp_in, cp_out, out_f32 without keep_f32, out_info) per layer: layer 1 publishes the abs-max that layer 2 scales its planes
+    # by (spconv_forward_rows_planes), the cg chain hands planes on, and the last layer writes fp32 rows for dense()
+    tc = ([("rows", None, None, True, False), ("rows", None, None, True, True), ("rows", None, 32, False, True)]
+          + [("cg", 32, 32, False, True)] * 2 + [("cg", 32, 64, False, True)] + [("cg", 64, 64, False, True)] * 7
+          + [("cg", 64, None, True, True)])
+    for use_tc, keep_f32 in ((True, False), (True, True), (False, False), (False, True)):
+        plan = spmiddle_plan(use_tc, keep_f32)
+        expect = tc if use_tc else [("simt", None, None, True, False)] * 14
+        got = [(p["impl"], p["cp_in"], p["cp_out"], p["out_f32"], p["out_info"]) for p in plan]
+        assert got == [(i, ci, co, f or keep_f32, a) for i, ci, co, f, a in expect], (use_tc, keep_f32)
+        assert [p["lout"] for p in plan] == lout and [p["lin"] for p in plan] == [0] + lout[:-1]
+        assert {p["rb"]: li for li, p in enumerate(plan) if p["build_rb"]} == builders
+        assert [p["rb"] for p in plan] == ["subm0"] * 2 + ["sp1"] + ["subm1"] * 2 + ["sp2"] + ["subm2"] * 3 + ["sp3"] + ["subm3"] * 3 + ["sp4"]
+        tiles = {p["rb"] for p in plan if p["tile_lists"]}
+        assert tiles == ({"subm1", "sp2", "subm2", "sp3", "subm3", "sp4"} if use_tc else set())
+        assert all(p["build_rb"] for p in plan if p["tile_lists"])
+    plan = spmiddle_plan()
+    convs = [m for m in SpMiddleFHD(num_input_features=4).middle_conv._modules.values() if isinstance(m, spconv.SparseModule)]
+    assert len(convs) == len(plan)
+    for m, p in zip(convs, plan):
+        assert (m.in_channels, m.out_channels, m.subm) == (p["cin"], p["cout"], p["kind"] == "subm")
+        assert sparse_grad.conv_impl(m.in_channels) == p["impl"]
+        if p["impl"] == "cg":
+            assert plane_width(m.in_channels) == p["cp_in"] == m.in_channels
 
 
 def test_checkpoint_reads_reference_written_file(golden_dir):
