@@ -128,13 +128,16 @@ def bn_relu(x, gamma, beta, mean, var, eps=1e-3, relu=True):
     return np.maximum(y, 0) if relu else y
 
 
-def spmiddle_forward(voxel_features, coors, batch_size, input_shape_xyz, params, dtype=np.float64, trace=None):
+def spmiddle_forward(voxel_features, coors, batch_size, input_shape_xyz, params, dtype=np.float64, trace=None, caps=None):
     """scn.py:176-189.  params: list of dicts {weight [kz,ky,kx,Cin,Cout], gamma, beta, mean, var}.
+    caps: optional per-level capacities (index = level, 1..4; None = unbounded): a strided layer keeps only the first caps[level]
+    output sites in canonical order, as a capacity-bounded device level does after an overflow.
     Returns the dense BEV tensor [B, 128, 200, 176] (NCHW, channel = c*D + d)."""
     shape = tuple(int(v) for v in (np.array(input_shape_xyz)[::-1] + np.array([1, 0, 0])))
     feat = voxel_features.astype(dtype)
     cur = coors.astype(np.int32)
     books = {}
+    level = 0
     for li, (kind, _cin, _cout, ks, st, pd, key) in enumerate(SPMIDDLE_FHD_LAYERS):
         p = params[li]
         w = p["weight"].reshape(-1, p["weight"].shape[3], p["weight"].shape[4])
@@ -144,6 +147,9 @@ def spmiddle_forward(voxel_features, coors, batch_size, input_shape_xyz, params,
             nbr = books[key]
         else:
             oc, oshape = strided_out_coors(cur, shape, ks, st, pd)
+            level += 1
+            if caps is not None and caps[level] is not None:
+                oc = oc[:caps[level]]
             nbr = neighbor_table(cur, shape, oc, ks, st, pd)
             cur, shape = oc, oshape
         feat = conv_from_nbr(feat, nbr, w, dtype)

@@ -177,8 +177,11 @@ struct PrefixStore {
     __device__ __forceinline__ void operator()(long long i, int ex, int) const { words[i].y = (unsigned int)ex; }
 };
 
-// strided conv, step 3: emit output coordinates in ascending linear index, clamp the count
-__global__ void __launch_bounds__(256) enumerate_kernel(const uint2 *__restrict__ bitmap, long long nwords, GridDims gout,
+// strided conv, step 3: emit output coordinates in ascending linear index, clamp the count.  On overflow (more sites than max_out) the
+// level keeps its first max_out sites in canonical order: the thread that owns a word also clears the bits ranked >= max_out, so every
+// later lookup through the bitmap index (SubM rulebook, next strided rulebook, dense gather, skip plan) sees exactly the kept sites and
+// never returns a row >= max_out.  The ranks of the kept bits are unchanged.
+__global__ void __launch_bounds__(256) enumerate_kernel(uint2 *__restrict__ bitmap, long long nwords, GridDims gout,
                                                         const int *__restrict__ d_total, int max_out, int4 *__restrict__ out_coors,
                                                         int *__restrict__ d_n_out, int *__restrict__ d_status) {
     if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -191,23 +194,27 @@ __global__ void __launch_bounds__(256) enumerate_kernel(const uint2 *__restrict_
         const uint2 e = bitmap[w];
         unsigned int bits = e.x;
         int pos = (int)e.y;
+        if ((long long)pos + __popc(bits) > max_out) {    // overflow: keep the lowest (max_out - pos) bits, if any
+            unsigned int keep = 0u;
+            for (int r = pos; r < max_out && bits; ++r) { keep |= bits & (0u - bits); bits &= bits - 1; }
+            bits = keep;
+            bitmap[w].x = keep;
+        }
         while (bits) {
             const int b = __ffs(bits) - 1;
             bits &= bits - 1;
-            if (pos < max_out) {
-                if (small) {                               // < 2^32 cells (every level below the input grid): 32-bit divisions
-                    unsigned int lin = (unsigned int)w * 32u + (unsigned int)b;
-                    const unsigned int q1 = lin / (unsigned int)gout.W, x = lin - q1 * (unsigned int)gout.W;
-                    const unsigned int q2 = q1 / (unsigned int)gout.H, y = q1 - q2 * (unsigned int)gout.H;
-                    const unsigned int q3 = q2 / (unsigned int)gout.D, z = q2 - q3 * (unsigned int)gout.D;
-                    out_coors[pos] = make_int4((int)q3, (int)z, (int)y, (int)x);
-                } else {
-                    unsigned long long lin = (unsigned long long)w * 32 + b;
-                    const int x = (int)(lin % gout.W); lin /= gout.W;
-                    const int y = (int)(lin % gout.H); lin /= gout.H;
-                    const int z = (int)(lin % gout.D); lin /= gout.D;
-                    out_coors[pos] = make_int4((int)lin, z, y, x);
-                }
+            if (small) {                                   // < 2^32 cells (every level below the input grid): 32-bit divisions
+                unsigned int lin = (unsigned int)w * 32u + (unsigned int)b;
+                const unsigned int q1 = lin / (unsigned int)gout.W, x = lin - q1 * (unsigned int)gout.W;
+                const unsigned int q2 = q1 / (unsigned int)gout.H, y = q1 - q2 * (unsigned int)gout.H;
+                const unsigned int q3 = q2 / (unsigned int)gout.D, z = q2 - q3 * (unsigned int)gout.D;
+                out_coors[pos] = make_int4((int)q3, (int)z, (int)y, (int)x);
+            } else {
+                unsigned long long lin = (unsigned long long)w * 32 + b;
+                const int x = (int)(lin % gout.W); lin /= gout.W;
+                const int y = (int)(lin % gout.H); lin /= gout.H;
+                const int z = (int)(lin % gout.D); lin /= gout.D;
+                out_coors[pos] = make_int4((int)lin, z, y, x);
             }
             ++pos;
         }

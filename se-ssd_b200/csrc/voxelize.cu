@@ -290,6 +290,13 @@ extern "C" int sessd_voxelize(const float *d_points, const int *d_frame_off, int
     if (batch < 1 || batch > 4096 || max_total_points < 1 || cfg->max_points < 1 || cfg->max_voxels < 1 || cfg->num_feat < 3)
         return SESSD_EINVAL;
     if ((long long)max_total_points >= (1ll << kHashValBits)) return SESSD_ECAPACITY;
+    // the hash key (frame, cell) must fit the 40 bits above the point index, or distinct cells would alias: batch * cells < 2^40
+    unsigned long long keys = (unsigned long long)batch;
+    for (int j = 0; j < 3; ++j) {
+        const unsigned long long g = cfg->grid[j] > 0 ? (unsigned long long)cfg->grid[j] : 0ull;
+        if (g && keys > ((1ull << (64 - kHashValBits)) - 1) / g) return SESSD_ECAPACITY;
+        keys *= g;
+    }
     VoxWs w = carve(workspace, max_total_points, batch, cfg);
     if (w.bytes > workspace_bytes) return SESSD_EWORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;
