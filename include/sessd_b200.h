@@ -242,6 +242,21 @@ int sessd_bev_deconv_p2(const void *d_in_planes, const float *d_in_info, const v
 long long sessd_bev_skip_plan_words(int batch, int h, int w, int *offsets);
 int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, int *d_plan, void *stream);
 int sessd_bev_skip_fill(const int *d_record, float *d_out_f32, void *d_out_planes, int cout, void *stream);
+/* Weight gradient of a BEV conv (csrc/bevgrad.cu; training of the neck and head, rpn_v1.py:135-210, mg_head_sessd.py:202-215):
+ *    d_gw[t][ci][co] = sum_{b, y, x} in[b, y*is + dy[t], x*is + dx[t], ci] * g[b, y, x, co]     (zero outside the input)
+ * for the tap list, stride and extents of the forward's descriptor (out_stride 1, no offset, grid = the output extent; relu ignored).
+ * d_in_planes __half [2][batch][in_h][in_w][cin] with d_in_info = {abs-max, S_in} (the planes the forward read); d_g_planes __half
+ * [2][batch][out_h][out_w][cout] with d_g_info = {abs-max, S_g} (sessd_absmax + sessd_bev_split_planes of the output gradient).
+ * cin % 128 == 0; cout % 128 == 0 or cout == 64 (the head's 24-channel gradient zero-padded, as its data gradient needs).  Tensor cores,
+ * fp16 mma with the three-product split, divided by S_in S_g.  A deconv (k3, s2, p1, op1) is the stride-2 conv with the roles swapped:
+ * in = its output gradient, g = its input; its gradient is d_gw transposed.  Work items (tap, channel blocks, fixed pixel range) --
+ * sessd_bev_wgrad_items(desc) of them, a function of the descriptor only -- each write an fp32 partial to the workspace, and a reduce
+ * sums them in ascending item order: bitwise run-to-run deterministic, no float atomics.  _items: SESSD_EINVAL on an invalid descriptor;
+ * _workspace_bytes: 0 then. */
+int sessd_bev_wgrad_items(const sessd_conv_desc *desc);
+size_t sessd_bev_wgrad_workspace_bytes(const sessd_conv_desc *desc);
+int sessd_bev_wgrad(const void *d_in_planes, const float *d_in_info, const void *d_g_planes, const float *d_g_info,
+                    const sessd_conv_desc *desc, float *d_gw, void *d_ws, size_t ws_bytes, void *stream);
 /* fp32 [n] -> planes [2][n] scaled from d_info[0] (the tensor's abs-max, e.g. from sessd_absmax); writes the scale to d_info[1] */
 int sessd_bev_split_planes(const float *d_x, long long n, float *d_info, void *d_planes, void *stream);
 /* dense() (scn.py:184-187) straight into the planes the neck reads: d_amax = abs-max of the feature rows, d_info[2] <- {abs-max, S} */

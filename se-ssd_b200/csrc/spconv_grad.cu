@@ -17,7 +17,7 @@
 //     a_hi g_lo + a_lo g_hi into the cross accumulator, fp32), summed RN once per item; the reduce divides by S_in S_g (exact).
 #include <cuda_fp16.h>
 
-#include "common.cuh"
+#include "tc_common.cuh"
 
 namespace sessd {
 
@@ -100,22 +100,6 @@ __global__ void __launch_bounds__(kGrThreads) wgrad_rows_kernel(const float *__r
 }
 
 // ---------------------------------------------------------------------------------------------------------------- tensor-core wgrad
-__device__ __forceinline__ void mma_f16_16816(float *d, const uint32_t *a, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-__device__ __forceinline__ void wg_cp_async16(uint32_t dst, const void *src, bool valid) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");   // 0: zero fill
-}
-__device__ __forceinline__ void ldsm_x4_trans(uint32_t *r, uint32_t addr) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x2_trans(uint32_t *r, uint32_t addr) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];\n" : "=r"(r[0]), "=r"(r[1]) : "r"(addr));
-}
-
 // CP input channels (plane width), COUT output channels (= the gradient plane width).  Eight warps tile the [CP][COUT] result in m16 slabs
 // x NT n8 tiles each.  A round stages up to kGrKC pairs PAIR-MAJOR, exactly as the planes lie in global memory: [hi | lo][pair][channel],
 // 16-byte cp.async per 8 channels (slots past the round's pairs are zero-filled by the copy itself), double-buffered so the next round's

@@ -7,7 +7,8 @@
   -> range mask in five kernels with no host round trip (sessd_postprocess); the reference syncs to the host twice per frame
   (box_torch_ops.py:536, mg_head_sessd.py:1026) and clips polygons on one CPU thread.
 * ``loss``     : the assembled SE-SSD head loss (supervised terms + ODIoU on the device, consistency loss against the teacher); value and
-  gradient w.r.t. the packed head tensor.  The encoder / neck backward below it is a "next" row."""
+  gradient w.r.t. the packed head tensor.  In train mode the packed tensor carries a graph to the head's input and its convs' weights
+  and biases (sessd_b200.bev_grad), so ``loss.backward()`` reaches the neck and the encoder below it."""
 import logging
 import math
 
@@ -16,7 +17,7 @@ import torch
 from torch import nn
 
 from det3d.core.bbox.geometry import frustum_planes
-from sessd_b200 import ops
+from sessd_b200 import bev_grad, ops
 from sessd_b200.runners import HeadRunner
 
 from ..builder import build_loss
@@ -56,6 +57,8 @@ class Head(nn.Module):
         """x logical NCHW [B,128,H,W] -> packed NHWC [B,H,W,24] = [box 14 | cls 2 | dir 4 | iou 2 | pad 2]."""
         if not (self.use_dir and self.conv_box.out_channels == 14 and self.conv_cls.out_channels == 2 and self.conv_dir.out_channels == 4):
             raise NotImplementedError("the fused head kernel is built for the car head: 2 anchors x (7 box, 1 cls, 2 dir, 1 iou)")
+        if self.training:       # differentiable w.r.t. x and the four convs' weights and biases (sessd_b200.bev_grad); a fresh tensor
+            return bev_grad.head_forward(self, x)
         b, c, h, w = x.shape
         key = (b, h, w, str(x.device))
         if self._runner is None or self._runner_key != key:
@@ -70,7 +73,9 @@ class Head(nn.Module):
     def forward(self, x):
         # a fresh tensor per call (like the reference): the runner's output buffer is overwritten by the next forward, and the SE-SSD
         # teacher / student flow runs two forwards before either result is consumed
-        packed = self.packed_forward(x).clone()
+        packed = self.packed_forward(x)
+        if not self.training:
+            packed = packed.clone()
         ret = {"box_preds": packed[..., 0:14].contiguous(), "cls_preds": packed[..., 14:16].contiguous()}
         if self.use_dir:
             ret["dir_cls_preds"] = packed[..., 16:20].contiguous()
@@ -185,8 +190,8 @@ class MultiGroupHead(nn.Module):
         trainer_sessd.py:267) and the teacher's own supervised terms on the raw targets (``*_ema``, :810-884).  Values and the gradient
         w.r.t. the packed head tensor come from one device pass (csrc/headloss.cu, odiou.cu); ``loss`` is a torch scalar whose backward
         hands that gradient to ``preds_dicts[0]['_packed']``'s graph, and ``consistency_loss`` is differentiable through
-        ``box_preds / cls_preds / iou_preds`` by torch autograd.  Returns the reference's key -> [per-task value] dict.  The backward of the
-        encoder / neck below the head tensor is a 'next' row (DESIGN.md §8): a head tensor produced by ``Head.forward`` carries no graph."""
+        ``box_preds / cls_preds / iou_preds`` by torch autograd.  Returns the reference's key -> [per-task value] dict.  A head tensor
+        produced by ``Head.forward`` in train mode carries the graph of the head, the neck and the encoder (in eval mode none)."""
         if len(preds_dicts) != 1:
             raise NotImplementedError("the fused loss kernels are built for the single-task (car) head")
         merged = {}

@@ -4,9 +4,11 @@ Identical module tree (hence identical state-dict keys: ``bottom_up_block_0.1.we
 (``logger`` is dereferenced exactly like the reference does, :212).  ``forward`` (eval mode) executes the whole neck with the
 sessd_b200 kernels: 12 conv / deconv layers as NHWC implicit GEMMs on the wgmma tensor cores with BatchNorm + ReLU (+ the
 deconv_0 + trans_0 residual) fused into the epilogue, and one fused kernel for the two 1-channel attention convs, their BN, the
-2-way softmax and the weighted sum (:229-233)."""
+2-way softmax and the weighted sum (:229-233).  In train mode ``forward`` runs the reference forward (:220-235) layer by layer instead:
+the convs on the same kernels through an autograd Function, BatchNorm2d with batch statistics (sessd_b200.bev_grad)."""
 from torch import nn
 
+from sessd_b200 import bev_grad
 from sessd_b200.runners import SSFAPlanesRunner
 
 from ..registry import NECKS
@@ -60,8 +62,8 @@ class SSFA(nn.Module):
                 nn.init.xavier_uniform_(m.weight)
 
     def forward(self, x):
-        if self.training:
-            raise NotImplementedError("SSFA: only the inference path is built (call .eval()); training is a 'next' row")
+        if self.training:       # the reference forward layer by layer, differentiable (sessd_b200.bev_grad); BatchNorm2d with batch statistics
+            return bev_grad.ssfa_forward(self, x)
         b, c, h, w = x.shape
         key = (b, h, w, str(x.device))
         if self._runner is None or self._runner_key != key:

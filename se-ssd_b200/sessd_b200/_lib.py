@@ -80,6 +80,9 @@ SIGNATURES = {
     "sessd_bev_skip_plan_words": (_ll, [_i, _i, _i, _I3]),
     "sessd_bev_skip_plan": (_i, [_vp, Grid, _vp, _vp]),
     "sessd_bev_skip_fill": (_i, [_vp, _vp, _vp, _i, _vp]),
+    "sessd_bev_wgrad_items": (_i, [C.POINTER(ConvDesc)]),
+    "sessd_bev_wgrad_workspace_bytes": (_sz, [C.POINTER(ConvDesc)]),
+    "sessd_bev_wgrad": (_i, [_vp, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp, _sz, _vp]),
     "sessd_bev_split_planes": (_i, [_vp, _ll, _vp, _vp, _vp]),
     "sessd_sparse_to_dense_planes": (_i, [_vp, _i, _vp, _i, Grid, _vp, _vp, _vp, _vp]),
     "sessd_ssfa_fuse_planes": (_i, [_vp, _vp, _vp, _vp, _f, _f, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),

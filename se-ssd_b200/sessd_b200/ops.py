@@ -452,6 +452,25 @@ def bev_split_planes(x, info, planes):
     return planes
 
 
+def bev_wgrad_workspace(desc, device):
+    n = int(lib.sessd_bev_wgrad_workspace_bytes(C.byref(desc)))
+    if n == 0:
+        raise ValueError("sessd_bev_wgrad: no weight gradient for this descriptor")
+    return torch.empty((n,), dtype=torch.uint8, device=device)
+
+
+def bev_wgrad(in_planes, in_info, g_planes, g_info, desc, gw=None, ws=None):
+    """weight gradient [ntaps, Cin, Cout] fp32 of the conv of ``desc`` (csrc/bevgrad.cu) from the input planes the forward read and the
+    planes of the output gradient (absmax + bev_split_planes)"""
+    if gw is None:
+        gw = torch.empty((desc.ntaps, desc.cin, desc.cout), dtype=torch.float32, device=g_planes.device)
+    if ws is None:
+        ws = bev_wgrad_workspace(desc, g_planes.device)
+    check(lib.sessd_bev_wgrad(_p(in_planes), _p(in_info), _p(g_planes), _p(g_info), C.byref(desc), _p(gw), _p(ws), ws.numel(), _st()),
+          "sessd_bev_wgrad")
+    return gw
+
+
 def planes_to_float(planes, info):
     """(hi + lo) / S as fp32 (tests / debugging)"""
     return (planes[0].float() + planes[1].float()) / info[1]
