@@ -20,6 +20,7 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "tile_lists.cuh"
 
 namespace sessd {
 
@@ -291,13 +292,8 @@ static GridDims to_dims(sessd_grid g) { GridDims d; d.B = g.batch; d.D = g.shape
 
 
 // ---------------------------------------------------------------------------------------------------------------------------------
-// Tile lists: the neighbour table regrouped for the pair-proportional tensor-core conv (spconv_cg.cu).  One record per tile of 128
-// output rows: [0, 32) pair count per kernel offset, [32, 32 + 4 kvol) 128-bit row mask per offset, [160, 160 + pairs) the pairs of
-// offset 0, then of offset 1, ... each (input row << 7) | tile row, ascending tile row.  Built once per rulebook (a SubM rulebook serves
-// 2-3 layers); deterministic (warp ballots + popcount ranks, no atomics).
-constexpr int kTlRows = 128, kTlHeader = 160;
-__host__ __device__ constexpr int tile_list_stride(int kvol) { return kTlHeader + kTlRows * kvol; }
-
+// Tile lists: the neighbour table regrouped for the pair-proportional tensor-core conv (spconv_cg.cu), record format in tile_lists.cuh.
+// Built once per rulebook (a SubM rulebook serves 2-3 layers); deterministic (warp ballots + popcount ranks, no atomics).
 template <int KV>
 __global__ void __launch_bounds__(kTlRows) tile_lists_kernel(const int *__restrict__ nbr, int kvol_, const int *__restrict__ d_n_out, int max_out,
                                                              unsigned int *__restrict__ tiles) {
@@ -328,14 +324,14 @@ __global__ void __launch_bounds__(kTlRows) tile_lists_kernel(const int *__restri
     __syncthreads();
     unsigned int *rec = tiles + (size_t)blockIdx.x * tile_list_stride(kvol);
     if (r < 32) rec[r] = (unsigned int)(s_off[r + 1] - s_off[r]);
-    for (int e = r; e < kvol * 4; e += kTlRows) rec[32 + e] = s_mask[e >> 2][e & 3];
+    for (int e = r; e < kvol * 4; e += kTlRows) rec[kTlMask + e] = s_mask[e >> 2][e & 3];
     const unsigned int lt = (1u << lane) - 1u;
 #pragma unroll
     for (int k = 0; k < (KV ? KV : 27); ++k) {
         if (k < kvol && v[k] >= 0) {
             int pos = s_off[k] + __popc(s_mask[k][warp] & lt);
             for (int w = 0; w < warp; ++w) pos += __popc(s_mask[k][w]);
-            rec[kTlHeader + pos] = ((unsigned int)v[k] << 7) | (unsigned int)r;
+            rec[kTlHeader + pos] = tl_entry(v[k], r);
         }
     }
 }

@@ -26,6 +26,7 @@
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
+#include "tile_lists.cuh"
 
 namespace sessd {
 
@@ -131,10 +132,10 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
             const unsigned int *rec = a.tiles + (size_t)tile * (size_t)a.tile_stride;
             const int c = (int)__ldg(rec + lane);                        // every warp ranks the 32 counts itself: no extra block-wide sync
             // the first list entries are requested together with the counts (one L2 round trip instead of two for most tiles; the record
-            // is 160 + 128 kvol words long, so the speculative reads stay inside it)
+            // is tile_list_stride(kvol) words long, so the speculative reads stay inside it)
             unsigned int spec[4];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) spec[u] = (tid + u * kCgThreads < 128 * kvol) ? __ldg(rec + 160 + tid + u * kCgThreads) : 0u;
+            for (int u = 0; u < 4; ++u) spec[u] = (tid + u * kCgThreads < kTlRows * kvol) ? __ldg(rec + kTlHeader + tid + u * kCgThreads) : 0u;
             const int incl = warp_incl_scan(c, lane);
             const int total = __shfl_sync(0xffffffffu, incl, 31);
             if (warp == 0) {
@@ -144,11 +145,11 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
                 if (c > 0) s_klist[__popc(m & ((1u << lane) - 1u))] = lane;
                 if (lane == 0) *s_nact = __popc(m);
             }
-            if (tid < kvol * 4) s_valid[tid] = __ldg(rec + 32 + tid);
+            if (tid < kvol * 4) s_valid[tid] = __ldg(rec + kTlMask + tid);
 #pragma unroll
             for (int u = 0; u < 4; ++u)
                 if (tid + u * kCgThreads < total) s_list[tid + u * kCgThreads] = spec[u];
-            for (int e = tid + 4 * kCgThreads; e < total; e += kCgThreads) s_list[e] = __ldg(rec + 160 + e);
+            for (int e = tid + 4 * kCgThreads; e < total; e += kCgThreads) s_list[e] = __ldg(rec + kTlHeader + e);
         }
         __syncthreads();
         const int nact = *s_nact;
@@ -288,8 +289,8 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
                 const int n = s_cnt[k];
                 const uint32_t *lst = s_list + s_off[k];
                 auto copy_row = [&](uint32_t e) {
-                    const uint32_t r = e & 127u;
-                    const size_t src = (size_t)(e >> 7);
+                    const uint32_t r = tl_tile_row(e);
+                    const size_t src = (size_t)tl_in_row(e);
                     if constexpr (C::kWide)
                         cg_cp_async16(a_base + (uint32_t)half * (kCgBM * 128) + r * 128u + (((uint32_t)cc ^ (r & 7u)) << 4),
                                       a.planes + src * 128 + half * 64 + cc * 8);
@@ -385,7 +386,7 @@ extern "C" int sessd_spconv_forward_cg(const void *d_in_planes, int cp, int plan
         return SESSD_EINVAL;
     if (d_out_planes && !d_out_info) return SESSD_EINVAL;
     CgArgs a;
-    a.planes = (const __half *)d_in_planes; a.in_info = d_in_info; a.tiles = (const unsigned int *)d_tiles; a.tile_stride = 160 + 128 * kvol; a.d_n_out = d_n_out; a.kvol = kvol; a.max_out = max_out;
+    a.planes = (const __half *)d_in_planes; a.in_info = d_in_info; a.tiles = (const unsigned int *)d_tiles; a.tile_stride = tile_list_stride(kvol); a.d_n_out = d_n_out; a.kvol = kvol; a.max_out = max_out;
     a.relu = relu; a.scale = d_scale; a.shift = d_shift; a.gain = gain; a.shift_max = shift_max; a.out_f32 = d_out_f32;
     a.out_planes = (__half *)d_out_planes; a.out_info = d_out_info;
     cudaStream_t st = (cudaStream_t)stream;

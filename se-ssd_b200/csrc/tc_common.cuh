@@ -73,24 +73,6 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
-// ---- warp MMA (mma.sync) fed by cp.async + ldmatrix.trans: the weight-gradient kernels, whose K dimension (pairs, pixels) is the
-// leading dimension of both operands in shared memory
-__device__ __forceinline__ void mma_f16_16816(float *d, const uint32_t *a, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-__device__ __forceinline__ void wg_cp_async16(uint32_t dst, const void *src, bool valid) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");   // 0: zero fill
-}
-__device__ __forceinline__ void ldsm_x4_trans(uint32_t *r, uint32_t addr) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x2_trans(uint32_t *r, uint32_t addr) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];\n" : "=r"(r[0]), "=r"(r[1]) : "r"(addr));
-}
-
 // ---- warpgroup MMA (wgmma): four consecutive warps, the first one's index a multiple of four, issue together
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
