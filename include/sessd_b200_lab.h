@@ -1,7 +1,7 @@
 /* sessd_b200_lab.h -- C ABI of libsessd_b200_lab.so: the NON-DEFAULT BEV conv variants kept for cross-implementation tests
  * (csrc/bevconv_split.cu): fp32 NHWC input split inside the wgmma kernel, either into 3xTF32 (tf32 wgmma) or into two-term fp16
- * (fp16 wgmma).  Nothing in the product path (libsessd_b200.so, sessd_b200.engine) links or loads this library.  Same conventions as
- * sessd_b200.h. */
+ * (fp16 wgmma); and a clock-counting build of the product's planes kernel for stall profiles.  Nothing in the product path
+ * (libsessd_b200.so, sessd_b200.engine) links or loads this library.  Same conventions as sessd_b200.h. */
 #ifndef SESSD_B200_LAB_H
 #define SESSD_B200_LAB_H
 
@@ -36,6 +36,19 @@ int sessd_bev_conv_h2(const float *d_in, const void *d_weight_h2, int cout_pad, 
 int sessd_bev_deconv_h2(const float *d_in, const void *d_weight_h2, int cout_pad, const float *d_scale,
                         const float *d_shift, const float *d_residual, float *d_out, int batch, int in_h, int in_w,
                         int cin, int cout, int relu, const float *d_amax_in, float *d_amax_out, void *stream);
+
+/* Stall profile of the product's planes conv / deconv (sessd_bev_conv_p2 / sessd_bev_deconv_p2, same arguments and results): the
+ * kernel's clock counters are written to d_prof, int64 [grid][16] with grid = min(work items, SMs); word order in csrc/bevconv_p2.cuh
+ * (P2Prof).  For measurement only: the counters cost clocks of their own. */
+int sessd_bev_conv_p2_profile(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
+                              const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
+                              float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info,
+                              const sessd_conv_desc *desc, const int *d_items, long long *d_prof, void *stream);
+int sessd_bev_deconv_p2_profile(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
+                                const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
+                                float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, int batch,
+                                int in_h, int in_w, int cin, int cout, int relu, const int *d_items, long long *d_prof,
+                                void *stream);
 
 #ifdef __cplusplus
 }

@@ -70,6 +70,25 @@ struct P2Params {
     float *out_info;                   // [2] = {running abs-max of the output (atomicMax), S_out}
     long long out_plane_stride;        // elements between the hi and the lo plane of the output
     const int *items;                  // nullable: run only the listed work items (count + indices, see kP2ItemsHeader), else all p.total
+    long long *prof;                   // PROFILE instantiations only: [grid][kP2ProfWords] clock counters (P2Prof)
+};
+
+// Stall profile of the PROFILE instantiations (lab library): each CTA writes its clock64() counts to record blockIdx.x of p.prof.
+// Consumer counters come from thread 0 (warpgroup 0), the producer counters from lane 0 of warps 8 and 9.
+enum P2Prof {
+    kProfCta,           // clocks from the end of the set-up to the end of the consumer loop
+    kProfItems,         // work items run
+    kProfSteps,         // tap steps (one [b_lo ; b_hi] stage each)
+    kProfItemClk,       // clocks inside the item loop (main loop + epilogue)
+    kProfBFull,         // clocks waiting on b_full
+    kProfPatchFull,     // clocks waiting on patch_full
+    kProfMmaWait,       // clocks inside wgmma_wait (in-loop and the drain before the epilogue)
+    kProfEpilogue,      // clocks of the epilogue (after the drain)
+    kProfPatchEmpty,    // patch producer: clocks waiting on patch_empty
+    kProfPatchTotal,    // patch producer: clocks of its whole loop
+    kProfBEmpty,        // weight producer: clocks waiting on b_empty
+    kProfBTotal,        // weight producer: clocks of its whole loop
+    kP2ProfWords = 16
 };
 
 // number of work items this launch runs and the k-th of them (every warp role walks the same sequence)
@@ -140,6 +159,17 @@ __device__ __forceinline__ void p2_quad_transpose(const float *s, int q, float v
         }
 }
 
+// PROFILE only: clock64() at the start of a timed span, and the span's clocks added to clk (no code otherwise)
+template <bool PROFILE>
+__device__ __forceinline__ long long p2_tick() {
+    if constexpr (PROFILE) return clock64();
+    return 0;
+}
+template <bool PROFILE>
+__device__ __forceinline__ void p2_tock(long long &clk, long long t0) {
+    if constexpr (PROFILE) clk += clock64() - t0;
+}
+
 __device__ __forceinline__ float p2_tf32_rn(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -179,7 +209,7 @@ __device__ __forceinline__ void p2_split_patch(const P2Params &p, const unsigned
     asm volatile("bar.sync 1, %0;\n" ::"n"(kP2MmaWarps * 32) : "memory");
 }
 
-template <int NT, int MODE>
+template <int NT, int MODE, bool PROFILE = false>
 __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                    const __grid_constant__ CUtensorMap map_b,
                                                                    const float *__restrict__ scale, const float *__restrict__ shift,
@@ -192,6 +222,9 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
     uint64_t *bars = (uint64_t *)(staging + p.npatch * p.staging_bytes);
     uint64_t *patch_full = bars, *patch_empty = bars + 2, *b_full = bars + 4, *b_empty = bars + 4 + kP2MaxBStages;
     uint32_t *s_aoff = (uint32_t *)(b_empty + kP2MaxBStages);      // [4 classes][9 taps]
+    // the epilogue's folded BN scale and shift, [p.cout] each: read from shared memory, so that no epilogue step waits on a global load
+    // behind the main loops' TMA traffic
+    float *s_scale = (float *)(((uintptr_t)(s_aoff + 4 * 9) + 15) & ~(uintptr_t)15), *s_shift = s_scale + p.cout;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == kP2PatchWarp * 32) prefetch_tensormap(&map_a);    // descriptor fetches overlap barrier init
@@ -210,7 +243,14 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
         const int c = idx / 9, t = idx - c * 9;
         s_aoff[idx] = (uint32_t)((2 * p.tap_copy[c][t] * p.copy_bytes + p.tap_row[c][t] * 512) >> 4);
     }
+    for (int n = threadIdx.x; n < p.cout; n += blockDim.x) {
+        s_scale[n] = scale ? __ldg(scale + n) : 1.f;
+        s_shift[n] = shift ? __ldg(shift + n) : 0.f;
+    }
     __syncthreads();
+    long long clk[kP2ProfWords] = {};          // PROFILE only (P2Prof)
+    const long long t_start = p2_tick<PROFILE>();
+    long long *prof_rec = PROFILE ? p.prof + (size_t)blockIdx.x * kP2ProfWords : nullptr;
 
     if (warp == kP2PatchWarp) {
         // ===================== activation patches: per (item, 32-channel chunk) ncopies x (hi, lo) boxes =====================
@@ -221,7 +261,7 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
             const P2Item it = p2_decode(p, p2_item(p, k));
             const int bu = it.u0 * p.in_stride, bv = it.v0 * p.in_stride;
             for (int cc = 0; cc < nchunks; ++cc) {
-                mbar_wait(&patch_empty[pb], pph ^ 1u);
+                { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&patch_empty[pb], pph ^ 1u); p2_tock<PROFILE>(clk[kProfPatchEmpty], t0); }
                 if (elect_one()) {
                     mbar_expect_tx(&patch_full[pb], (uint32_t)p.load_bytes);
                     if constexpr (MODE == kP2Planes) {
@@ -242,6 +282,11 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
                 if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
             }
         }
+        if constexpr (PROFILE)
+            if (lane == 0) {
+                prof_rec[kProfPatchEmpty] = clk[kProfPatchEmpty];
+                prof_rec[kProfPatchTotal] = clock64() - t_start;
+            }
     } else if (warp == kP2WeightWarp) {
         // ===================== weight tiles: one [b_lo ; b_hi] stage per (item, chunk, tap) =====================
         int S = 0;
@@ -250,7 +295,7 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
             const P2Item it = p2_decode(p, p2_item(p, k));
             for (int cc = 0; cc < nchunks; ++cc)
                 for (int tap = 0; tap < it.ntaps; ++tap) {
-                    mbar_wait(&b_empty[S], bph ^ 1u);
+                    { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&b_empty[S], bph ^ 1u); p2_tock<PROFILE>(clk[kProfBEmpty], t0); }
                     if (elect_one()) {
                         unsigned char *st = tiles + S * p.bstage_bytes;
                         const int wtap = p.tap_w[it.cls][tap];
@@ -262,6 +307,11 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
                     if (++S == p.bstages) { S = 0; bph ^= 1u; }
                 }
         }
+        if constexpr (PROFILE)
+            if (lane == 0) {
+                prof_rec[kProfBEmpty] = clk[kProfBEmpty];
+                prof_rec[kProfBTotal] = clock64() - t_start;
+            }
     } else {
         // ===================== consumers (warps 0-7): wgmma over (chunk, tap), then BN / ReLU / residual / stores =====================
         const int wg = warp >> 2, wq = warp & 3;
@@ -284,6 +334,7 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
         int S = 0, pb = 0;
         uint32_t bph = 0, pph = 0;
         for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
+            const long long t_item = p2_tick<PROFILE>();
             const int g = p2_item(p, k);
             const int cls = p.cls_order[g / per_cls];
             const int ntaps = p.cls_ntaps[cls];
@@ -299,13 +350,13 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
             int prevS = -1, prev_pb = -1;
             bool first = true;
             for (int cc = 0; cc < nchunks; ++cc) {
-                mbar_wait(&patch_full[pb], pph);
+                { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&patch_full[pb], pph); p2_tock<PROFILE>(clk[kProfPatchFull], t0); }
                 if constexpr (MODE != kP2Planes)
                     p2_split_patch<MODE>(p, staging + pb * p.staging_bytes, patches + pb * p.patch_bytes, s_in, threadIdx.x);
                 const uint32_t pbase = patch_lo + (uint32_t)pb * patch_sz;
 #pragma unroll 1
                 for (int tap = 0; tap < ntaps; ++tap) {
-                    mbar_wait(&b_full[S], bph);
+                    { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&b_full[S], bph); p2_tock<PROFILE>(clk[kProfBFull], t0); }
                     if constexpr (MODE == kP2SplitTf32) {
                         // the weights' lo plane rounded to the nearest tf32 in place (the tensor core would truncate it)
                         float *wl = reinterpret_cast<float *>(tiles + S * p.bstage_bytes);
@@ -337,7 +388,9 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
                     p2_wgmma<NT, MODE>(acc, da_lo + 2, db_hi + 2, 1u);
                     wgmma_commit();
                     first = false;
-                    wgmma_wait<1>();                                         // the previous step's operands are no longer read
+                    if constexpr (PROFILE) ++clk[kProfSteps];
+                    // the previous step's operands are no longer read
+                    { const long long t0 = p2_tick<PROFILE>(); wgmma_wait<1>(); p2_tock<PROFILE>(clk[kProfMmaWait], t0); }
                     if (lane == 0) {
                         if (prevS >= 0) mbar_arrive(&b_empty[prevS]);
                         if (prev_pb >= 0) mbar_arrive(&patch_empty[prev_pb]);
@@ -350,7 +403,7 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
                     // one patch buffer: the next chunk's patch can only land once this one is released, so release it now rather
                     // than after the next chunk's first step (that step would wait for the patch forever); tf32: drain the chunk
                     // and fold its main partial
-                    wgmma_wait<0>();
+                    { const long long t0 = p2_tick<PROFILE>(); wgmma_wait<0>(); p2_tock<PROFILE>(clk[kProfMmaWait], t0); }
                     if (lane == 0) {
                         mbar_arrive(&b_empty[prevS]);
                         mbar_arrive(&patch_empty[pb]);
@@ -364,7 +417,8 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
                 }
                 if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
             }
-            wgmma_wait<0>();
+            { const long long t0 = p2_tick<PROFILE>(); wgmma_wait<0>(); p2_tock<PROFILE>(clk[kProfMmaWait], t0); }
+            const long long t_epi = p2_tick<PROFILE>();
             wgmma_fence_regs<NT>(acc);
             if (lane == 0) {
                 if (prevS >= 0) mbar_arrive(&b_empty[prevS]);
@@ -403,8 +457,8 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
                         float sc[8], sh[8];
 #pragma unroll
                         for (int t = 0; t < 8; t += 4) {
-                            const float4 a = scale ? __ldg(reinterpret_cast<const float4 *>(scale + n + t)) : make_float4(1.f, 1.f, 1.f, 1.f);
-                            const float4 b = shift ? __ldg(reinterpret_cast<const float4 *>(shift + n + t)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                            const float4 a = *reinterpret_cast<const float4 *>(s_scale + n + t);
+                            const float4 b = *reinterpret_cast<const float4 *>(s_shift + n + t);
                             sc[t] = a.x; sc[t + 1] = a.y; sc[t + 2] = a.z; sc[t + 3] = a.w;
                             sh[t] = b.x; sh[t + 1] = b.y; sh[t + 2] = b.z; sh[t + 3] = b.w;
                         }
@@ -452,7 +506,18 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
                         if (row_ok && n_lo + 16 < p.cout) *reinterpret_cast<float4 *>(out_f32 + opix * p.cout + c_lo + 16) = w_hi;
                     }
                 }
+            if constexpr (PROFILE) {
+                const long long t_end = clock64();
+                clk[kProfEpilogue] += t_end - t_epi;
+                clk[kProfItemClk] += t_end - t_item;
+                ++clk[kProfItems];
+            }
         }
+        if constexpr (PROFILE)
+            if (threadIdx.x == 0) {
+                clk[kProfCta] = clock64() - t_start;
+                for (int w = kProfCta; w <= kProfEpilogue; ++w) prof_rec[w] = clk[w];
+            }
         if (p.out_info) {
             const unsigned m = __reduce_max_sync(0xFFFFFFFFu, __float_as_uint(vmax));     // non-negative floats order like their bits
             if (lane == 0 && m != 0u) atomicMax(reinterpret_cast<unsigned *>(p.out_info), m);
@@ -526,7 +591,7 @@ static int p2_geometry(P2Geometry &g, int batch, int grid_h, int grid_w, int cou
 // MODE kP2Planes: d_in = fp16 planes [2][B][H][W][C], d_in_info = {abs-max, S}; split modes: d_in = fp32 NHWC, d_in_info = the input's
 // abs-max (split fp16; nullable) or unused (tf32), weights fp32 [2][taps][cout_pad][cin] in the tf32 mode; d_out_info is {abs-max, S_out}
 // in the planes mode and a single running abs-max otherwise
-template <int MODE>
+template <int MODE, bool PROFILE = false>
 static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d_in_info, const void *d_w, int w_taps, int cout_pad,
                      const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info, float gain,
                      float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, P2Params &p, const P2Taps *cls, int nclass,
@@ -591,10 +656,12 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
     const int per_buf = p.patch_bytes + p.staging_bytes, bstage = 2 * p.n_tile * 64;
     // weight ring: kP2BRing when it fits next to two patch buffers or one, else shrunk (>= 2 stages) next to one buffer
     p.bring_bytes = kP2BRing;
-    p.npatch = (kP2BRing + 1536 + 2 * per_buf <= kP2MaxSmem) ? 2 : 1;
-    if (kP2BRing + 1536 + per_buf > kP2MaxSmem) p.bring_bytes = (kP2MaxSmem - 1536 - per_buf) / bstage * bstage;
+    // after the ring and the patch buffers: barriers and tap offsets (1536 B with the 1 KB alignment slack), then scale / shift
+    const int tail = 1536 + 16 + 2 * 4 * p.cout;
+    p.npatch = (kP2BRing + tail + 2 * per_buf <= kP2MaxSmem) ? 2 : 1;
+    if (kP2BRing + tail + per_buf > kP2MaxSmem) p.bring_bytes = (kP2MaxSmem - tail - per_buf) / bstage * bstage;
     if (p.bring_bytes < 2 * bstage) return SESSD_EINVAL;
-    const int smem = p.bring_bytes + 1536 + p.npatch * per_buf;
+    const int smem = p.bring_bytes + tail + p.npatch * per_buf;
     CUtensorMap map_a, map_b;
     const cuuint64_t es = MODE == kP2SplitTf32 ? 4 : 2;               // weight element bytes
     if (MODE != kP2Planes) {   // fp32 NHWC [B][H][W][C] viewed as {C, U, V, B, 1}, staged unswizzled
@@ -629,8 +696,8 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
     }
     static bool attr_done = false;
     if (!attr_done) {
-        SESSD_CUDA_TRY(cudaFuncSetAttribute(bev_conv_p2_kernel<32, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2MaxSmem));
-        SESSD_CUDA_TRY(cudaFuncSetAttribute(bev_conv_p2_kernel<128, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2MaxSmem));
+        SESSD_CUDA_TRY(cudaFuncSetAttribute(bev_conv_p2_kernel<32, MODE, PROFILE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2MaxSmem));
+        SESSD_CUDA_TRY(cudaFuncSetAttribute(bev_conv_p2_kernel<128, MODE, PROFILE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2MaxSmem));
         attr_done = true;
     }
     p.bstage_bytes = bstage;
@@ -651,22 +718,22 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
     }
     const int grid = p.total < num_sms ? p.total : num_sms;                 // persistent, one CTA per SM
     if (p.n_tile == 32)
-        SESSD_LAUNCH((bev_conv_p2_kernel<32, MODE>), grid, kP2Threads, smem, (cudaStream_t)stream, map_a, map_b, d_scale, d_shift, d_residual, d_out_f32,
+        SESSD_LAUNCH((bev_conv_p2_kernel<32, MODE, PROFILE>), grid, kP2Threads, smem, (cudaStream_t)stream, map_a, map_b, d_scale, d_shift, d_residual, d_out_f32,
                      (__half *)d_out_planes, p);
     else
-        SESSD_LAUNCH((bev_conv_p2_kernel<128, MODE>), grid, kP2Threads, smem, (cudaStream_t)stream, map_a, map_b, d_scale, d_shift, d_residual, d_out_f32,
+        SESSD_LAUNCH((bev_conv_p2_kernel<128, MODE, PROFILE>), grid, kP2Threads, smem, (cudaStream_t)stream, map_a, map_b, d_scale, d_shift, d_residual, d_out_f32,
                      (__half *)d_out_planes, p);
     return last_error();
 }
 
 
-// one tap-list conv (sessd_conv_desc) / the four-class deconv through launch_p2<MODE>
-template <int MODE>
+// one tap-list conv (sessd_conv_desc) / the four-class deconv through launch_p2<MODE, PROFILE>; d_prof: [grid][kP2ProfWords] (PROFILE)
+template <int MODE, bool PROFILE = false>
 static int p2_conv(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                    const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                    float *d_out_f32, void *d_out_planes, float *d_out_info, const sessd_conv_desc *desc, void *stream,
-                   const int *d_items = nullptr) {
-    if (!desc) return SESSD_EINVAL;
+                   const int *d_items = nullptr, long long *d_prof = nullptr) {
+    if (!desc || (PROFILE && !d_prof)) return SESSD_EINVAL;
     const sessd_conv_desc &d = *desc;
     if (d.ntaps < 1 || d.ntaps > 9 || (d.in_stride != 1 && d.in_stride != 2) || d.out_stride < 1) return SESSD_EINVAL;
     if ((d.grid_h - 1) * d.out_stride + d.out_off_y >= d.out_h || (d.grid_w - 1) * d.out_stride + d.out_off_x >= d.out_w) return SESSD_EINVAL;
@@ -674,25 +741,28 @@ static int p2_conv(const void *d_in_planes, const float *d_in_info, const void *
     p.batch = d.batch; p.cin = d.cin; p.cout = d.cout; p.in_stride = d.in_stride;
     p.out_h = d.out_h; p.out_w = d.out_w; p.out_stride = d.out_stride; p.relu = d.relu;
     p.items = d_items;
+    p.prof = d_prof;
     P2Taps t = {};
     t.n = d.ntaps; t.off_y = d.out_off_y; t.off_x = d.out_off_x;
     for (int i = 0; i < d.ntaps; ++i) { t.dy[i] = d.tap_dy[i]; t.dx[i] = d.tap_dx[i]; t.w[i] = i; }
-    return launch_p2<MODE>(d_in_planes, d.in_h, d.in_w, d_in_info, d_weight_h2, d.ntaps, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
+    return launch_p2<MODE, PROFILE>(d_in_planes, d.in_h, d.in_w, d_in_info, d_weight_h2, d.ntaps, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
                      shift_max, d_out_f32, d_out_planes, d_out_info, p, &t, 1, d.grid_h, d.grid_w, stream);
 }
 
-template <int MODE>
+template <int MODE, bool PROFILE = false>
 static int p2_deconv(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                      const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                      float *d_out_f32, void *d_out_planes, float *d_out_info, int batch, int in_h, int in_w, int cin, int cout,
-                     int relu, void *stream, const int *d_items = nullptr) {
+                     int relu, void *stream, const int *d_items = nullptr, long long *d_prof = nullptr) {
+    if (PROFILE && !d_prof) return SESSD_EINVAL;
     P2Params p = {};
     p.batch = batch; p.cin = cin; p.cout = cout; p.in_stride = 1;
     p.out_h = 2 * in_h; p.out_w = 2 * in_w; p.out_stride = 2; p.relu = relu;
     p.items = d_items;
+    p.prof = d_prof;
     P2Taps cls[4];
     p2_deconv_classes(cls);
-    return launch_p2<MODE>(d_in_planes, in_h, in_w, d_in_info, d_weight_h2, 9, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
+    return launch_p2<MODE, PROFILE>(d_in_planes, in_h, in_w, d_in_info, d_weight_h2, 9, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
                      d_out_f32, d_out_planes, d_out_info, p, cls, 4, in_h, in_w, stream);
 }
 
