@@ -50,6 +50,15 @@ int sessd_bev_deconv_p2_profile(const void *d_in_planes, const float *d_in_info,
                                 int in_h, int in_w, int cin, int cout, int relu, const int *d_items, long long *d_prof,
                                 void *stream);
 
+/* Loader-only probe of sessd_bev_conv_p2_profile's launch: the two TMA producer warps run unchanged, the consumers wait on the full
+ * barriers and release them without issuing wgmma or an epilogue, so the launch's time is what the loads alone take (no output is
+ * written; d_prof as above).  smem_a != 0 plans a stride-1 conv's patches as shared-memory A descriptors would need them, one copy
+ * per tap shift along u, instead of the single copy the register-fed A reads: the traffic of these launches before and after. */
+int sessd_bev_conv_p2_loads(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
+                            const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
+                            float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info,
+                            const sessd_conv_desc *desc, const int *d_items, int smem_a, long long *d_prof, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,7 +10,12 @@ b_full / patch_full / wgmma_wait and in the epilogue, the producers' shares wait
 per tap step against the tensor-core floor (6 * n_tile clocks: 128 px x 32 cin x 3 n_tile fp16 FMA at 2048 FMA/clk/SM).  The card's
 name, power limit and SM clocks are read in the same run.  The counters cost clocks of their own: the µs here are not bench numbers.
 
-    python scripts/p2_stall_profile.py --out FILE [--reps 20] [--engines 12] [--frames 8]
+--loads adds the L2 -> SM ceiling of the 3x3 128 -> 128 launch: the launch alone and dense through the loader-only probe
+(sessd_bev_conv_p2_loads: the TMA producers run unchanged, the consumers only wait on the full barriers and release them), once with
+the three patch copies shared-memory A descriptors would need and once with the single copy the register-fed A reads.  Bytes are counted
+from the shapes (per item and 32-channel chunk: the patch boxes plus nine 16 KB weight stages); reported per clock and SM and as TB/s.
+
+    python scripts/p2_stall_profile.py --out FILE [--reps 20] [--engines 12] [--frames 8] [--loads]
 """
 import argparse
 import ctypes as C
@@ -47,6 +52,7 @@ class Profiler:
         from sessd_b200 import ops
         self.torch, self.ops, self.device, self.num_sms = torch, ops, device, num_sms
         self.bufs, self.key = {}, None
+        self.loads_smem_a = None      # 0 / 1: route conv() to the loader-only probe with that patch plan, counters filed under self.key
         ops.bev_conv_p2, ops.bev_deconv_p2 = self.conv, self.deconv
 
     def buf(self):
@@ -57,6 +63,12 @@ class Profiler:
     def conv(self, in_planes, in_info, weight_h2, scale, shift, residual, resid_info, gain, shift_max, out_f32, out_planes, out_info, desc,
              items=None):
         o = self.ops
+        if self.loads_smem_a is not None:
+            o.check(o.lib.sessd_bev_conv_p2_loads(o._p(in_planes), o._p(in_info), o._p(weight_h2), int(weight_h2.shape[2]), o._p(scale),
+                                                  o._p(shift), o._p(residual), o._p(resid_info), float(gain), float(shift_max), o._p(out_f32),
+                                                  o._p(out_planes), o._p(out_info), C.byref(desc), o._p(items), int(self.loads_smem_a),
+                                                  o._p(self.buf()), o._st()), "sessd_bev_conv_p2_loads")
+            return
         o.check(o.lib.sessd_bev_conv_p2_profile(o._p(in_planes), o._p(in_info), o._p(weight_h2), int(weight_h2.shape[2]), o._p(scale),
                                                 o._p(shift), o._p(residual), o._p(resid_info), float(gain), float(shift_max), o._p(out_f32),
                                                 o._p(out_planes), o._p(out_info), C.byref(desc), o._p(items), o._p(self.buf()), o._st()),
@@ -77,7 +89,8 @@ class Profiler:
         orig = neck._launch
 
         def launch(L, skip=False):
-            self.key = (eng_id, L.name, "skip" if skip else "dense")
+            if self.loads_smem_a is None:
+                self.key = (eng_id, L.name, "skip" if skip else "dense")
             orig(L, skip)
 
         neck._launch = launch
@@ -110,6 +123,7 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--engines", type=int, default=12)
     ap.add_argument("--frames", type=int, default=8, help="frames per engine in the concurrent leg")
+    ap.add_argument("--loads", action="store_true", help="also measure the loader-only ceiling of the 3x3 128->128 launch")
     a = ap.parse_args()
 
     import numpy as np
@@ -153,6 +167,31 @@ def main():
                 s["sm_mhz_from_clock64"] = s["cta_clk_max"] / us if us > 0 else None
                 rec[mode] = s
             res["alone"][L.name] = rec
+        if a.loads:
+            # the 3x3 128 -> 128 launch: per (item, chunk) 2 planes x 18 x (8 + 2) rows (one copy) or 3 copies x 2 x 18 x 8 rows of
+            # 64 B, plus 9 weight stages of 2 x 128 rows of 64 B
+            L = next(L for L in SSFA_LAUNCHES if L.kind == "conv" and L.cin == 128 and L.cout == 128 and L.k == 3 and L.stride == 1)
+            res["loads"] = dict(launch=L.name)
+            for smem_a, patch in ((1, 3 * 2 * 18 * 8 * 64), (0, 2 * 18 * 10 * 64)):
+                prof.loads_smem_a = smem_a
+                prof.key = (0, L.name, "loads%d" % smem_a)
+                for _ in range(3):
+                    eng.neck._launch(L, False)
+                t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                t0.record(eng.stream)
+                for _ in range(a.reps):
+                    eng.neck._launch(L, False)
+                t1.record(eng.stream)
+                eng.stream.synchronize()
+                us = t0.elapsed_time(t1) * 1000.0 / a.reps
+                r = prof.bufs[prof.key].cpu().numpy().astype(np.float64)
+                item_bytes = (L.cin // 32) * (patch + 9 * 2 * 128 * 64)
+                act = r[:, ITEMS] > 0
+                res["loads"]["smem_a" if smem_a else "reg_a"] = dict(
+                    us=us, items=int(r[:, ITEMS].sum()), bytes_per_item=item_bytes, patch_bytes_per_chunk=patch,
+                    bytes_per_clk_per_sm=float((r[act, ITEMS] * item_bytes / r[act, CTA]).mean()),
+                    tb_per_s=float(r[:, ITEMS].sum() * item_bytes / (us * 1e-6) / 1e12))
+            prof.loads_smem_a = None
     clock_probe = gpu_info()
     del eng
     torch.cuda.synchronize()
@@ -213,6 +252,11 @@ def main():
         print("  %-20s clk/step main %.0f (floor %d), with epilogue %.0f; consumer %s; producers %s" % (
             k, t["clk_per_step_main"], t["floor_clk_per_step"], t["clk_per_step_with_epilogue"],
             {x: round(v, 3) for x, v in t["consumer_share"].items()}, {x: round(v, 3) for x, v in t["producer_share"].items()}))
+    if a.loads:
+        for k in ("smem_a", "reg_a"):
+            r = res["loads"][k]
+            print("  loader-only %-6s %s: %.1f us, %d B per item, %.1f B/clk/SM, %.2f TB/s" % (
+                k, res["loads"]["launch"], r["us"], r["bytes_per_item"], r["bytes_per_clk_per_sm"], r["tb_per_s"]))
     print("  alone totals (us): %s; concurrent frames/s while profiled: %.0f" % (res["alone_total_us"], res["concurrent_frames_per_s_profiled"]))
 
 

@@ -18,8 +18,12 @@
 // the input patch [v rows][8 u][32 channels] is TMA-loaded per plane: a tap then addresses a canonical K-major SWIZZLE_64B operand at
 // copy + v_shift * 512 B (group stride 512 B): plain descriptors, no base-offset tricks.  u / v are mapped to (y, x) or (x, y),
 // whichever tiles the map with fewer tiles.
+// Stride-1 launches from planes (REGA) feed A from registers instead: ONE patch [rows_v][pitch_u = 8 + the taps' u extent][32 channels]
+// per plane serves every tap, because ldmatrix takes one address per row and so reads the 16 tile rows of a warp at any row shift of
+// the swizzled patch, where a shared-memory descriptor needs whole 8-row swizzle groups.  A 3x3 patch is 2 x 18 x 10 rows instead of
+// 3 x 2 x 18 x 8; the wgmma's, their order and the accumulators are the same (bit-identical outputs).
 // Warps: 0-7 consumers (two warpgroups: wgmma issue, then BN/ReLU/residual -> fp32 and / or fp16 planes + running abs-max from the
-// accumulator registers), 8 patch TMA, 9 weight TMA.
+// accumulator registers), 8 patch TMA, 9 weight TMA (REGA: and 10, 11, which only complete the producers' warpgroup).
 #pragma once
 #include <cuda_fp16.h>
 
@@ -29,12 +33,18 @@ namespace sessd {
 
 constexpr int kP2TileU = 8, kP2TileV = 16;
 constexpr int kP2MaxCopies = 6, kP2MaxRowsV = 18;
+// weight-stage ring ([b_lo ; b_hi] planes of n_tile 64-byte rows each per stage): as many stages as fit next to the patch buffers, at
+// most kP2MaxBStages; two patch buffers when that leaves at least kP2BStages stages
 constexpr int kP2BStages = 6, kP2MaxBStages = 12;
-constexpr int kP2BStageBytes = 2 * 128 * 64;              // [b_lo ; b_hi] planes, up to 128 rows of 64 B each
-constexpr int kP2BRing = kP2BStages * kP2BStageBytes;     // bytes of the weight-stage ring
 constexpr int kP2MmaWarps = 8;
 constexpr int kP2PatchWarp = 8, kP2WeightWarp = 9;
 constexpr int kP2Threads = 320;                           // 10 warps
+// REGA: 12 warps, so that the producers' warpgroup (warps 8-11; 10 and 11 do nothing else) is whole and can hand registers to the two
+// consumer warpgroups, which hold the A fragments next to the accumulators.  The CTA owns 384 x 168 registers (what ptxas gives a
+// 384-thread kernel) and no more: the consumers' 8 x 32 x (232 - 168) must not exceed the producers' 4 x 32 x (168 - 40), or the
+// raise never returns.
+constexpr int kP2ThreadsRegA = 384, kP2RegsConsumer = 232, kP2RegsProducer = 40;
+static_assert(2 * (kP2RegsConsumer - 168) <= 168 - kP2RegsProducer, "the consumers take what the producers release");
 constexpr int kP2MaxSmem = 227 * 1024;
 // optional device item list (bevskip.cu): int32 record, word 0 = number of items to run, the item indices from word kP2ItemsHeader on
 constexpr int kP2ItemsHeader = 32;
@@ -42,6 +52,9 @@ constexpr int kP2ItemsHeader = 32;
 // shared memory and the consumer warpgroups split there -- into fp16 (hi, lo) with the power-of-two scale of its abs-max (32-channel
 // chunks), or into tf32 hi = truncate(x), lo = x - hi for three tf32 products (16-channel chunks, fp32 weights [2][taps][cout_pad][cin])
 enum { kP2Planes = 0, kP2SplitF16 = 1, kP2SplitTf32 = 2 };
+// lab instantiations: the product kernel with clock counters (P2Prof), or with counters and consumers that only wait on the full
+// barriers and release them -- no wgmma, no epilogue: what the two TMA producers alone can pull from L2
+enum { kP2NoProbe = 0, kP2ProbeClocks = 1, kP2ProbeLoads = 2 };
 
 struct P2Params {
     int batch, cin, cout;
@@ -51,8 +64,9 @@ struct P2Params {
     int u_is_x;                        // 1: u = x, v = y;  0: u = y, v = x
     int out_stride, nclass;
     int cls_ntaps[4], cls_off_u[4], cls_off_v[4];
-    int tap_copy[4][9], tap_row[4][9], tap_w[4][9];      // per (class, tap): patch copy, first v row inside the copy, weight tap
-    int ncopies, rows_v;
+    // per (class, tap): patch copy, first v row inside the copy (REGA: first patch row, v * pitch_u + u), weight tap
+    int tap_copy[4][9], tap_row[4][9], tap_w[4][9];
+    int ncopies, rows_v, pitch_u;                         // copies, v rows and u positions per v row (8; REGA: 8 + the taps' u extent) of a copy
     int copy_u[kP2MaxCopies], copy_v[kP2MaxCopies];       // input coordinate of the copy's first element relative to (u0, v0) * in_stride
     int copy_bytes, patch_bytes, npatch;                  // bytes of one copy plane, of one patch buffer (ncopies x 2 planes), 1 or 2 buffers
     int chunk;                         // input channels per K stage: 32 (fp16 operands) or 16 (tf32 operands); 64-byte operand rows either way
@@ -70,10 +84,10 @@ struct P2Params {
     float *out_info;                   // [2] = {running abs-max of the output (atomicMax), S_out}
     long long out_plane_stride;        // elements between the hi and the lo plane of the output
     const int *items;                  // nullable: run only the listed work items (count + indices, see kP2ItemsHeader), else all p.total
-    long long *prof;                   // PROFILE instantiations only: [grid][kP2ProfWords] clock counters (P2Prof)
+    long long *prof;                   // probe instantiations only: [grid][kP2ProfWords] clock counters (P2Prof)
 };
 
-// Stall profile of the PROFILE instantiations (lab library): each CTA writes its clock64() counts to record blockIdx.x of p.prof.
+// Stall profile of the probe instantiations (lab library): each CTA writes its clock64() counts to record blockIdx.x of p.prof.
 // Consumer counters come from thread 0 (warpgroup 0), the producer counters from lane 0 of warps 8 and 9.
 enum P2Prof {
     kProfCta,           // clocks from the end of the set-up to the end of the consumer loop
@@ -130,6 +144,15 @@ __device__ __forceinline__ void p2_wgmma(float *d, uint64_t da, uint64_t db, uin
         else if constexpr (N == 128) wgmma_f16_n128(d, da, db, accumulate);
         else wgmma_f16_n256(d, da, db, accumulate);
     }
+}
+
+// the same with the A fragment (one k16 of this warp's 16 rows, ldsm_x4) in registers
+template <int N>
+__device__ __forceinline__ void p2_wgmma_ra(float *d, const uint32_t *a, uint64_t db, uint32_t accumulate) {
+    if constexpr (N == 32) wgmma_f16_ra_n32(d, a, db, accumulate);
+    else if constexpr (N == 64) wgmma_f16_ra_n64(d, a, db, accumulate);
+    else if constexpr (N == 128) wgmma_f16_ra_n128(d, a, db, accumulate);
+    else wgmma_f16_ra_n256(d, a, db, accumulate);
 }
 
 // 4 x 4 transpose of 2-float pairs inside each quad of lanes (q = lane & 3, the four lanes of one accumulator row): on entry pair g
@@ -209,12 +232,14 @@ __device__ __forceinline__ void p2_split_patch(const P2Params &p, const unsigned
     asm volatile("bar.sync 1, %0;\n" ::"n"(kP2MmaWarps * 32) : "memory");
 }
 
-template <int NT, int MODE, bool PROFILE = false>
-__global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid_constant__ CUtensorMap map_a,
+template <int NT, int MODE, bool REGA = false, int PROBE = kP2NoProbe>
+__global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_conv_p2_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                    const __grid_constant__ CUtensorMap map_b,
                                                                    const float *__restrict__ scale, const float *__restrict__ shift,
                                                                    const float *__restrict__ resid, float *__restrict__ out_f32,
                                                                    __half *__restrict__ out_planes, P2Params p) {
+    static_assert(!REGA || MODE == kP2Planes, "register-fed A reads the TMA-written planes");
+    constexpr bool PROFILE = PROBE != kP2NoProbe, LOADS_ONLY = PROBE == kP2ProbeLoads;
     extern __shared__ unsigned char smem_raw[];
     unsigned char *tiles = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     unsigned char *patches = tiles + p.bring_bytes;
@@ -238,10 +263,10 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
         for (int s = 0; s < p.bstages; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], kP2MmaWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
     }
-    // operand offset of every (class, tap) inside a patch buffer, in 16-byte units
+    // operand offset of every (class, tap) inside a patch buffer, in 16-byte units (REGA: in patch rows)
     for (int idx = threadIdx.x; idx < p.nclass * 9; idx += blockDim.x) {
         const int c = idx / 9, t = idx - c * 9;
-        s_aoff[idx] = (uint32_t)((2 * p.tap_copy[c][t] * p.copy_bytes + p.tap_row[c][t] * 512) >> 4);
+        s_aoff[idx] = REGA ? (uint32_t)p.tap_row[c][t] : (uint32_t)((2 * p.tap_copy[c][t] * p.copy_bytes + p.tap_row[c][t] * 512) >> 4);
     }
     for (int n = threadIdx.x; n < p.cout; n += blockDim.x) {
         s_scale[n] = scale ? __ldg(scale + n) : 1.f;
@@ -252,67 +277,71 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
     const long long t_start = p2_tick<PROFILE>();
     long long *prof_rec = PROFILE ? p.prof + (size_t)blockIdx.x * kP2ProfWords : nullptr;
 
-    if (warp == kP2PatchWarp) {
-        // ===================== activation patches: per (item, 32-channel chunk) ncopies x (hi, lo) boxes =====================
-        int pb = 0;
-        uint32_t pph = 0;
-        const uint32_t patches_u32 = smem_u32(patches);
-        for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
-            const P2Item it = p2_decode(p, p2_item(p, k));
-            const int bu = it.u0 * p.in_stride, bv = it.v0 * p.in_stride;
-            for (int cc = 0; cc < nchunks; ++cc) {
-                { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&patch_empty[pb], pph ^ 1u); p2_tock<PROFILE>(clk[kProfPatchEmpty], t0); }
-                if (elect_one()) {
-                    mbar_expect_tx(&patch_full[pb], (uint32_t)p.load_bytes);
-                    if constexpr (MODE == kP2Planes) {
-                        uint32_t dst = patches_u32 + (uint32_t)(pb * p.patch_bytes);
-                        for (int c = 0; c < p.ncopies; ++c, dst += 2u * (uint32_t)p.copy_bytes) {
-                            const int cu = bu + p.copy_u[c], cv = bv + p.copy_v[c];
-                            tma_load_5d(dst, &map_a, &patch_full[pb], cc * p.chunk, cu, cv, it.b, 0);
-                            tma_load_5d(dst + (uint32_t)p.copy_bytes, &map_a, &patch_full[pb], cc * p.chunk, cu, cv, it.b, 1);
-                        }
-                    } else {
-                        const uint32_t copy_in = (uint32_t)(p.staging_bytes / p.ncopies);
-                        uint32_t dst = smem_u32(staging) + (uint32_t)(pb * p.staging_bytes);
-                        for (int c = 0; c < p.ncopies; ++c, dst += copy_in)
-                            tma_load_5d(dst, &map_a, &patch_full[pb], cc * p.chunk, bu + p.copy_u[c], bv + p.copy_v[c], it.b, 0);
-                    }
-                }
-                __syncwarp();
-                if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
-            }
-        }
-        if constexpr (PROFILE)
-            if (lane == 0) {
-                prof_rec[kProfPatchEmpty] = clk[kProfPatchEmpty];
-                prof_rec[kProfPatchTotal] = clock64() - t_start;
-            }
-    } else if (warp == kP2WeightWarp) {
-        // ===================== weight tiles: one [b_lo ; b_hi] stage per (item, chunk, tap) =====================
-        int S = 0;
-        uint32_t bph = 0;
-        for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
-            const P2Item it = p2_decode(p, p2_item(p, k));
-            for (int cc = 0; cc < nchunks; ++cc)
-                for (int tap = 0; tap < it.ntaps; ++tap) {
-                    { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&b_empty[S], bph ^ 1u); p2_tock<PROFILE>(clk[kProfBEmpty], t0); }
+    if (warp >= kP2MmaWarps) {
+        if constexpr (REGA) setmaxnreg_dec<kP2RegsProducer>();
+        if (warp == kP2PatchWarp) {
+            // ===================== activation patches: per (item, 32-channel chunk) ncopies x (hi, lo) boxes =====================
+            int pb = 0;
+            uint32_t pph = 0;
+            const uint32_t patches_u32 = smem_u32(patches);
+            for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
+                const P2Item it = p2_decode(p, p2_item(p, k));
+                const int bu = it.u0 * p.in_stride, bv = it.v0 * p.in_stride;
+                for (int cc = 0; cc < nchunks; ++cc) {
+                    { const long long t0 = p2_tick<PROFILE>(); mbar_wait<REGA>(&patch_empty[pb], pph ^ 1u); p2_tock<PROFILE>(clk[kProfPatchEmpty], t0); }
                     if (elect_one()) {
-                        unsigned char *st = tiles + S * p.bstage_bytes;
-                        const int wtap = p.tap_w[it.cls][tap];
-                        mbar_expect_tx(&b_full[S], 2 * b_plane_bytes);
-                        tma_load_4d(st + b_plane_bytes, &map_b, &b_full[S], cc * p.chunk, it.n0, wtap, 0);
-                        tma_load_4d(st, &map_b, &b_full[S], cc * p.chunk, it.n0, wtap, 1);
+                        mbar_expect_tx(&patch_full[pb], (uint32_t)p.load_bytes);
+                        if constexpr (MODE == kP2Planes) {
+                            uint32_t dst = patches_u32 + (uint32_t)(pb * p.patch_bytes);
+                            for (int c = 0; c < p.ncopies; ++c, dst += 2u * (uint32_t)p.copy_bytes) {
+                                const int cu = bu + p.copy_u[c], cv = bv + p.copy_v[c];
+                                tma_load_5d(dst, &map_a, &patch_full[pb], cc * p.chunk, cu, cv, it.b, 0);
+                                tma_load_5d(dst + (uint32_t)p.copy_bytes, &map_a, &patch_full[pb], cc * p.chunk, cu, cv, it.b, 1);
+                            }
+                        } else {
+                            const uint32_t copy_in = (uint32_t)(p.staging_bytes / p.ncopies);
+                            uint32_t dst = smem_u32(staging) + (uint32_t)(pb * p.staging_bytes);
+                            for (int c = 0; c < p.ncopies; ++c, dst += copy_in)
+                                tma_load_5d(dst, &map_a, &patch_full[pb], cc * p.chunk, bu + p.copy_u[c], bv + p.copy_v[c], it.b, 0);
+                        }
                     }
                     __syncwarp();
-                    if (++S == p.bstages) { S = 0; bph ^= 1u; }
+                    if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
+                }
+            }
+            if constexpr (PROFILE)
+                if (lane == 0) {
+                    prof_rec[kProfPatchEmpty] = clk[kProfPatchEmpty];
+                    prof_rec[kProfPatchTotal] = clock64() - t_start;
+                }
+        } else if (warp == kP2WeightWarp) {
+            // ===================== weight tiles: one [b_lo ; b_hi] stage per (item, chunk, tap) =====================
+            int S = 0;
+            uint32_t bph = 0;
+            for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
+                const P2Item it = p2_decode(p, p2_item(p, k));
+                for (int cc = 0; cc < nchunks; ++cc)
+                    for (int tap = 0; tap < it.ntaps; ++tap) {
+                        { const long long t0 = p2_tick<PROFILE>(); mbar_wait<REGA>(&b_empty[S], bph ^ 1u); p2_tock<PROFILE>(clk[kProfBEmpty], t0); }
+                        if (elect_one()) {
+                            unsigned char *st = tiles + S * p.bstage_bytes;
+                            const int wtap = p.tap_w[it.cls][tap];
+                            mbar_expect_tx(&b_full[S], 2 * b_plane_bytes);
+                            tma_load_4d(st + b_plane_bytes, &map_b, &b_full[S], cc * p.chunk, it.n0, wtap, 0);
+                            tma_load_4d(st, &map_b, &b_full[S], cc * p.chunk, it.n0, wtap, 1);
+                        }
+                        __syncwarp();
+                        if (++S == p.bstages) { S = 0; bph ^= 1u; }
+                    }
+            }
+            if constexpr (PROFILE)
+                if (lane == 0) {
+                    prof_rec[kProfBEmpty] = clk[kProfBEmpty];
+                    prof_rec[kProfBTotal] = clock64() - t_start;
                 }
         }
-        if constexpr (PROFILE)
-            if (lane == 0) {
-                prof_rec[kProfBEmpty] = clk[kProfBEmpty];
-                prof_rec[kProfBTotal] = clock64() - t_start;
-            }
     } else {
+        if constexpr (REGA) setmaxnreg_inc<kP2RegsConsumer>();
         // ===================== consumers (warps 0-7): wgmma over (chunk, tap), then BN / ReLU / residual / stores =====================
         const int wg = warp >> 2, wq = warp & 3;
         constexpr int kAcc = NT / 2;
@@ -321,6 +350,10 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
         const uint32_t patch_lo = desc_lo(smem_u32(patches)) + a_rows;
         const uint32_t plane_lo = b_plane_bytes >> 4;
         const uint32_t copy_lo = (uint32_t)(p.copy_bytes >> 4), patch_sz = (uint32_t)(p.patch_bytes >> 4);
+        // REGA: lane l gives ldmatrix the address of row l % 8 of matrix l / 8 -- matrices 0, 1 = tile rows 0-7, 8-15 of this warp's
+        // 16 (one v row of 8 u each), matrices 2, 3 the same rows 16 bytes on.  Its patch row before the tap's shift, and 16-byte chunk:
+        const uint32_t a_row = (uint32_t)((wg * 8 + wq * 2 + ((lane >> 3) & 1)) * p.pitch_u + (lane & 7)), a_chunk = (uint32_t)(lane >> 4);
+        const uint32_t patches_u32 = smem_u32(patches);
         float amax_in = 0.f, s_in = 1.f;
         if constexpr (MODE == kP2Planes) { amax_in = __ldg(p.in_info); s_in = __ldg(p.in_info + 1); }
         if constexpr (MODE == kP2SplitF16) if (p.in_amax) { amax_in = __ldg(p.in_amax); s_in = pow2_scale_for_bound(amax_in); }
@@ -349,73 +382,138 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
             for (int i = 0; i < (MODE == kP2SplitTf32 ? kAcc : 1); ++i) tot[i] = 0.f;
             int prevS = -1, prev_pb = -1;
             bool first = true;
-            for (int cc = 0; cc < nchunks; ++cc) {
-                { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&patch_full[pb], pph); p2_tock<PROFILE>(clk[kProfPatchFull], t0); }
-                if constexpr (MODE != kP2Planes)
-                    p2_split_patch<MODE>(p, staging + pb * p.staging_bytes, patches + pb * p.patch_bytes, s_in, threadIdx.x);
-                const uint32_t pbase = patch_lo + (uint32_t)pb * patch_sz;
-#pragma unroll 1
-                for (int tap = 0; tap < ntaps; ++tap) {
-                    { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&b_full[S], bph); p2_tock<PROFILE>(clk[kProfBFull], t0); }
-                    if constexpr (MODE == kP2SplitTf32) {
-                        // the weights' lo plane rounded to the nearest tf32 in place (the tensor core would truncate it)
-                        float *wl = reinterpret_cast<float *>(tiles + S * p.bstage_bytes);
-                        for (int i = threadIdx.x; i < (int)(b_plane_bytes / 4); i += kP2MmaWarps * 32) wl[i] = p2_tf32_rn(wl[i]);
-                        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-                        asm volatile("bar.sync 1, %0;\n" ::"n"(kP2MmaWarps * 32) : "memory");
+            if constexpr (REGA) {
+                // the A fragments of a tap step, {a_hi k 0-15, a_hi k 16-31, a_lo k 0-15, a_lo k 16-31}.  Two sets, taken in turn: the
+                // tensor core reads a step's set until the wgmma_wait<1> of the NEXT step has retired the step.
+                uint32_t frag[2][16];
+                int tap = 0;
+                uint32_t pbase = 0;
+                // the A fragments of the step at (pb, tap) -> fa
+                auto load_frags = [&](uint32_t *fa) {
+                    if (tap == 0) {
+                        { const long long t0 = p2_tick<PROFILE>(); mbar_wait<REGA>(&patch_full[pb], pph); p2_tock<PROFILE>(clk[kProfPatchFull], t0); }
+                        pbase = patches_u32 + (uint32_t)(pb * p.patch_bytes);
                     }
-                    const uint64_t da_hi = kDescSw64Hi | (uint64_t)(pbase + aoff[tap]);
-                    const uint64_t da_lo = da_hi + (uint64_t)copy_lo;
+                    if constexpr (!LOADS_ONLY) {
+                        // patch row r is 64 bytes at r * 64, its 16-byte chunk j at j ^ ((r >> 1) & 3) (SWIZZLE_64B); k 16-31 = chunk + 2
+                        const uint32_t r = a_row + aoff[tap];
+                        const uint32_t a_hi = pbase + r * 64u + ((a_chunk ^ ((r >> 1) & 3u)) << 4), a_lo = a_hi + (uint32_t)p.copy_bytes;
+                        ldsm_x4(fa, a_hi);
+                        ldsm_x4(fa + 4, a_hi ^ 32u);
+                        ldsm_x4(fa + 8, a_lo);
+                        ldsm_x4(fa + 12, a_lo ^ 32u);
+                    }
+                };
+                // one tap step from the fragments fa: the planes sequence of the descriptor path below, its a_hi and its a_lo instructions
+                // as two groups; between them, once the previous step has retired, the next step's fragments load into that step's set fn,
+                // so that their latency runs under the a_lo group's issue
+                auto step_ra = [&](const uint32_t *fa, uint32_t *fn, bool more) {
+                    { const long long t0 = p2_tick<PROFILE>(); mbar_wait<REGA>(&b_full[S], bph); p2_tock<PROFILE>(clk[kProfBFull], t0); }
                     const uint64_t db_lo = kDescSw64Hi | (uint64_t)(tiles_lo + (uint32_t)(S * (p.bstage_bytes >> 4)));
                     const uint64_t db_hi = db_lo + (uint64_t)plane_lo;
-                    const uint32_t accum = first ? 0u : 1u;
-                    // K = 16 fp16 / 8 tf32 per instruction = 32 bytes of the 64-byte row
-                    wgmma_fence();
-                    // tf32: the main accumulator restarts every chunk (its chunk partial is added into `tot` in RN fp32 below)
-                    const uint32_t acc_main = MODE == kP2SplitTf32 ? (tap != 0 ? 1u : 0u) : accum;
-                    if constexpr (MODE == kP2Planes) {
-                        // one m64n(2 NT) per k16 over the stacked stage: cross (+)= a_hi x b_lo and main (+)= a_hi x b_hi read a_hi once.
-                        // Each accumulator sums in the order of the three-product sequence below (the lab modes' bitwise reference).
-                        p2_wgmma<2 * NT, MODE>(acc, da_hi, db_lo, accum);
-                        p2_wgmma<2 * NT, MODE>(acc, da_hi + 2, db_lo + 2, 1u);
-                    } else {
-                        p2_wgmma<NT, MODE>(acc + kAcc, da_hi, db_hi, acc_main);       // main  (+)= a_hi x b_hi
-                        p2_wgmma<NT, MODE>(acc + kAcc, da_hi + 2, db_hi + 2, 1u);
-                        p2_wgmma<NT, MODE>(acc, da_hi, db_lo, accum);                 // cross (+)= a_hi x b_lo
-                        p2_wgmma<NT, MODE>(acc, da_hi + 2, db_lo + 2, 1u);
+                    if constexpr (!LOADS_ONLY) {
+                        wgmma_fence();
+                        p2_wgmma_ra<2 * NT>(acc, fa, db_lo, first ? 0u : 1u);
+                        p2_wgmma_ra<2 * NT>(acc, fa + 4, db_lo + 2, 1u);
+                        wgmma_commit();
                     }
-                    p2_wgmma<NT, MODE>(acc, da_lo, db_hi, 1u);                        // cross  += a_lo x b_hi
-                    p2_wgmma<NT, MODE>(acc, da_lo + 2, db_hi + 2, 1u);
-                    wgmma_commit();
                     first = false;
                     if constexpr (PROFILE) ++clk[kProfSteps];
-                    // the previous step's operands are no longer read
+                    // all but this step's a_hi group has retired: the previous step's stage and fragment set are free
                     { const long long t0 = p2_tick<PROFILE>(); wgmma_wait<1>(); p2_tock<PROFILE>(clk[kProfMmaWait], t0); }
-                    if (lane == 0) {
-                        if (prevS >= 0) mbar_arrive(&b_empty[prevS]);
-                        if (prev_pb >= 0) mbar_arrive(&patch_empty[prev_pb]);
-                    }
+                    if (lane == 0 && prevS >= 0) mbar_arrive(&b_empty[prevS]);
                     prevS = S;
-                    prev_pb = (tap == ntaps - 1) ? pb : -1;
                     if (++S == p.bstages) { S = 0; bph ^= 1u; }
-                }
-                if (p.npatch == 1 || MODE == kP2SplitTf32) {
-                    // one patch buffer: the next chunk's patch can only land once this one is released, so release it now rather
-                    // than after the next chunk's first step (that step would wait for the patch forever); tf32: drain the chunk
-                    // and fold its main partial
-                    { const long long t0 = p2_tick<PROFILE>(); wgmma_wait<0>(); p2_tock<PROFILE>(clk[kProfMmaWait], t0); }
-                    if (lane == 0) {
-                        mbar_arrive(&b_empty[prevS]);
-                        mbar_arrive(&patch_empty[pb]);
+                    if (++tap == ntaps) {      // the chunk's last fragments are in registers: its patch is free
+                        tap = 0;
+                        if (lane == 0) mbar_arrive(&patch_empty[pb]);
+                        if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
                     }
-                    prevS = prev_pb = -1;
-                    if constexpr (MODE == kP2SplitTf32) {
-                        wgmma_fence_regs<kAcc>(acc + kAcc);
+                    if (more) load_frags(fn);
+                    if constexpr (!LOADS_ONLY) {
+                        wgmma_fence();
+                        p2_wgmma_ra<NT>(acc, fa + 8, db_hi, 1u);                          // cross  += a_lo x b_hi
+                        p2_wgmma_ra<NT>(acc, fa + 12, db_hi + 2, 1u);
+                        wgmma_commit();
+                    }
+                };
+                const int nsteps = nchunks * ntaps;
+                load_frags(frag[0]);
+#pragma unroll 1
+                for (int st = 0; st + 1 < nsteps; st += 2) { step_ra(frag[0], frag[1], true); step_ra(frag[1], frag[0], st + 2 < nsteps); }
+                if (nsteps & 1) step_ra(frag[0], frag[1], false);
+            } else {
+                for (int cc = 0; cc < nchunks; ++cc) {
+                    { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&patch_full[pb], pph); p2_tock<PROFILE>(clk[kProfPatchFull], t0); }
+                    if constexpr (MODE != kP2Planes)
+                        p2_split_patch<MODE>(p, staging + pb * p.staging_bytes, patches + pb * p.patch_bytes, s_in, threadIdx.x);
+                    const uint32_t pbase = patch_lo + (uint32_t)pb * patch_sz;
+#pragma unroll 1
+                    for (int tap = 0; tap < ntaps; ++tap) {
+                        { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&b_full[S], bph); p2_tock<PROFILE>(clk[kProfBFull], t0); }
+                        if constexpr (MODE == kP2SplitTf32) {
+                            // the weights' lo plane rounded to the nearest tf32 in place (the tensor core would truncate it)
+                            float *wl = reinterpret_cast<float *>(tiles + S * p.bstage_bytes);
+                            for (int i = threadIdx.x; i < (int)(b_plane_bytes / 4); i += kP2MmaWarps * 32) wl[i] = p2_tf32_rn(wl[i]);
+                            asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+                            asm volatile("bar.sync 1, %0;\n" ::"n"(kP2MmaWarps * 32) : "memory");
+                        }
+                        if constexpr (!LOADS_ONLY) {
+                            const uint64_t da_hi = kDescSw64Hi | (uint64_t)(pbase + aoff[tap]);
+                            const uint64_t da_lo = da_hi + (uint64_t)copy_lo;
+                            const uint64_t db_lo = kDescSw64Hi | (uint64_t)(tiles_lo + (uint32_t)(S * (p.bstage_bytes >> 4)));
+                            const uint64_t db_hi = db_lo + (uint64_t)plane_lo;
+                            const uint32_t accum = first ? 0u : 1u;
+                            // K = 16 fp16 / 8 tf32 per instruction = 32 bytes of the 64-byte row
+                            wgmma_fence();
+                            // tf32: the main accumulator restarts every chunk (its chunk partial is added into `tot` in RN fp32 below)
+                            const uint32_t acc_main = MODE == kP2SplitTf32 ? (tap != 0 ? 1u : 0u) : accum;
+                            if constexpr (MODE == kP2Planes) {
+                                // one m64n(2 NT) per k16 over the stacked stage: cross (+)= a_hi x b_lo and main (+)= a_hi x b_hi read
+                                // a_hi once.  Each accumulator sums in the order of the three-product sequence below (the lab modes'
+                                // bitwise reference).
+                                p2_wgmma<2 * NT, MODE>(acc, da_hi, db_lo, accum);
+                                p2_wgmma<2 * NT, MODE>(acc, da_hi + 2, db_lo + 2, 1u);
+                            } else {
+                                p2_wgmma<NT, MODE>(acc + kAcc, da_hi, db_hi, acc_main);       // main  (+)= a_hi x b_hi
+                                p2_wgmma<NT, MODE>(acc + kAcc, da_hi + 2, db_hi + 2, 1u);
+                                p2_wgmma<NT, MODE>(acc, da_hi, db_lo, accum);                 // cross (+)= a_hi x b_lo
+                                p2_wgmma<NT, MODE>(acc, da_hi + 2, db_lo + 2, 1u);
+                            }
+                            p2_wgmma<NT, MODE>(acc, da_lo, db_hi, 1u);                        // cross  += a_lo x b_hi
+                            p2_wgmma<NT, MODE>(acc, da_lo + 2, db_hi + 2, 1u);
+                            wgmma_commit();
+                        }
+                        first = false;
+                        if constexpr (PROFILE) ++clk[kProfSteps];
+                        // the previous step's operands are no longer read
+                        { const long long t0 = p2_tick<PROFILE>(); wgmma_wait<1>(); p2_tock<PROFILE>(clk[kProfMmaWait], t0); }
+                        if (lane == 0) {
+                            if (prevS >= 0) mbar_arrive(&b_empty[prevS]);
+                            if (prev_pb >= 0) mbar_arrive(&patch_empty[prev_pb]);
+                        }
+                        prevS = S;
+                        prev_pb = (tap == ntaps - 1) ? pb : -1;
+                        if (++S == p.bstages) { S = 0; bph ^= 1u; }
+                    }
+                    if (p.npatch == 1 || MODE == kP2SplitTf32) {
+                        // one patch buffer: the next chunk's patch can only land once this one is released, so release it now rather
+                        // than after the next chunk's first step (that step would wait for the patch forever); tf32: drain the chunk
+                        // and fold its main partial
+                        { const long long t0 = p2_tick<PROFILE>(); wgmma_wait<0>(); p2_tock<PROFILE>(clk[kProfMmaWait], t0); }
+                        if (lane == 0) {
+                            mbar_arrive(&b_empty[prevS]);
+                            mbar_arrive(&patch_empty[pb]);
+                        }
+                        prevS = prev_pb = -1;
+                        if constexpr (MODE == kP2SplitTf32) {
+                            wgmma_fence_regs<kAcc>(acc + kAcc);
 #pragma unroll
-                        for (int i = 0; i < kAcc; ++i) tot[i] += acc[kAcc + i];
+                            for (int i = 0; i < kAcc; ++i) tot[i] += acc[kAcc + i];
+                        }
                     }
+                    if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
                 }
-                if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
             }
             { const long long t0 = p2_tick<PROFILE>(); wgmma_wait<0>(); p2_tock<PROFILE>(clk[kProfMmaWait], t0); }
             const long long t_epi = p2_tick<PROFILE>();
@@ -444,7 +542,7 @@ __global__ void __launch_bounds__(kP2Threads, 1) bev_conv_p2_kernel(const __grid
                 opixs[h] = ((size_t)it.b * p.out_h + (size_t)oy) * p.out_w + (size_t)ox;
             }
 #pragma unroll
-            for (int j = 0; j < NT / 32; ++j)
+            for (int j = 0; j < (LOADS_ONLY ? 0 : NT / 32); ++j)      // the loads probe has nothing to store
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const bool row_ok = rows_ok[h];
@@ -591,14 +689,15 @@ static int p2_geometry(P2Geometry &g, int batch, int grid_h, int grid_w, int cou
 // MODE kP2Planes: d_in = fp16 planes [2][B][H][W][C], d_in_info = {abs-max, S}; split modes: d_in = fp32 NHWC, d_in_info = the input's
 // abs-max (split fp16; nullable) or unused (tf32), weights fp32 [2][taps][cout_pad][cin] in the tf32 mode; d_out_info is {abs-max, S_out}
 // in the planes mode and a single running abs-max otherwise
-template <int MODE, bool PROFILE = false>
+template <int MODE, int PROBE = kP2NoProbe>
 static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d_in_info, const void *d_w, int w_taps, int cout_pad,
                      const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info, float gain,
                      float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, P2Params &p, const P2Taps *cls, int nclass,
-                     int grid_h, int grid_w, void *stream) {
+                     int grid_h, int grid_w, bool reg_a, void *stream) {
     if (!d_in_planes || !d_w || (!d_out_f32 && !d_out_planes)) return SESSD_EINVAL;
     if (MODE == kP2Planes && (!d_in_info || !d_scale)) return SESSD_EINVAL;
     if (MODE != kP2Planes && d_out_planes) return SESSD_EINVAL;
+    if (reg_a && (MODE != kP2Planes || p.in_stride != 1)) return SESSD_EINVAL;
     if (p.cin < 64 || p.cin % 64) return SESSD_EINVAL;      // whole 64-channel groups
     // the epilogue reads and writes 16 bytes at a time
     if (((uintptr_t)d_scale | (uintptr_t)d_shift | (uintptr_t)d_residual | (uintptr_t)d_out_f32 | (uintptr_t)d_out_planes) & 15)
@@ -632,9 +731,21 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
             vmin[k] = min(vmin[k], tv); vmax[k] = max(vmax[k], tv);
         }
     p.rows_v = 0;
+    p.pitch_u = kP2TileU;
     for (int k = 0; k < p.ncopies; ++k) p.rows_v = max(p.rows_v, kP2TileV + (vmax[k] - vmin[k]) / s);
     if (p.rows_v > kP2MaxRowsV) return SESSD_EINVAL;
     for (int k = 0; k < p.ncopies; ++k) { p.copy_u[k] = key_u[k]; p.copy_v[k] = vmin[k]; }
+    if (reg_a) {      // the same taps from one copy: from their least shift, wide and tall enough for their greatest (one TMA box)
+        int umin = key_u[0], umax = key_u[0];
+        for (int k = 1; k < p.ncopies; ++k) {
+            umin = min(umin, key_u[k]); umax = max(umax, key_u[k]);
+            vmin[0] = min(vmin[0], vmin[k]); vmax[0] = max(vmax[0], vmax[k]);
+        }
+        p.ncopies = 1;
+        p.copy_u[0] = umin; p.copy_v[0] = vmin[0];
+        p.pitch_u = kP2TileU + umax - umin; p.rows_v = kP2TileV + vmax[0] - vmin[0];
+        if (p.pitch_u > 256 || p.rows_v > 256) return SESSD_EINVAL;
+    }
     for (int c = 0; c < p.nclass; ++c) {
         for (int t = 0; t < cls[c].n; ++t) {
             const int tu = p.u_is_x ? cls[c].dx[t] : cls[c].dy[t], tv = p.u_is_x ? cls[c].dy[t] : cls[c].dx[t];
@@ -642,25 +753,26 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
             int k = 0;
             for (; k < p.ncopies; ++k)
                 if (key_u[k] == tu && key_vm[k] == vm) break;
-            p.tap_copy[c][t] = k;
-            p.tap_row[c][t] = (tv - vmin[k]) / s;
+            p.tap_copy[c][t] = reg_a ? 0 : k;
+            p.tap_row[c][t] = reg_a ? (tv - p.copy_v[0]) * p.pitch_u + (tu - p.copy_u[0]) : (tv - vmin[k]) / s;
             p.tap_w[c][t] = cls[c].w[t];
         }
     }
     p.chunk = MODE == kP2SplitTf32 ? 16 : 32;
-    p.copy_bytes = p.rows_v * kP2TileU * 64;
+    p.copy_bytes = (p.rows_v * p.pitch_u * 64 + 511) & ~511;      // whole 512-byte swizzle periods: every copy starts one
     p.patch_bytes = p.ncopies * 2 * p.copy_bytes;
     // fp32 staging: 32 channels = 128-byte rows (split fp16) or 16 channels = 64-byte rows (tf32)
     p.staging_bytes = MODE == kP2Planes ? 0 : p.ncopies * p.rows_v * kP2TileU * p.chunk * 4;
-    p.load_bytes = MODE == kP2Planes ? p.patch_bytes : p.staging_bytes;
+    p.load_bytes = MODE == kP2Planes ? p.ncopies * 2 * p.rows_v * p.pitch_u * 64 : p.staging_bytes;
     const int per_buf = p.patch_bytes + p.staging_bytes, bstage = 2 * p.n_tile * 64;
-    // weight ring: kP2BRing when it fits next to two patch buffers or one, else shrunk (>= 2 stages) next to one buffer
-    p.bring_bytes = kP2BRing;
     // after the ring and the patch buffers: barriers and tap offsets (1536 B with the 1 KB alignment slack), then scale / shift
     const int tail = 1536 + 16 + 2 * 4 * p.cout;
-    p.npatch = (kP2BRing + tail + 2 * per_buf <= kP2MaxSmem) ? 2 : 1;
-    if (kP2BRing + tail + per_buf > kP2MaxSmem) p.bring_bytes = (kP2MaxSmem - tail - per_buf) / bstage * bstage;
-    if (p.bring_bytes < 2 * bstage) return SESSD_EINVAL;
+    // two patch buffers when kP2BStages weight stages fit next to them, else one; then every stage that fits (>= 2), up to kP2MaxBStages
+    p.npatch = (kP2BStages * bstage + tail + 2 * per_buf <= kP2MaxSmem) ? 2 : 1;
+    p.bstage_bytes = bstage;
+    p.bstages = min((kP2MaxSmem - tail - p.npatch * per_buf) / bstage, kP2MaxBStages);
+    if (p.bstages < 2) return SESSD_EINVAL;
+    p.bring_bytes = p.bstages * bstage;
     const int smem = p.bring_bytes + tail + p.npatch * per_buf;
     CUtensorMap map_a, map_b;
     const cuuint64_t es = MODE == kP2SplitTf32 ? 4 : 2;               // weight element bytes
@@ -680,7 +792,7 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
                                     (cuuint64_t)p.batch, 2};
         const cuuint64_t strides[4] = {p.u_is_x ? row_w : row_h, p.u_is_x ? row_h : row_w, (cuuint64_t)in_h * in_w * p.cin * 2,
                                        (cuuint64_t)p.batch * in_h * in_w * p.cin * 2};
-        const cuuint32_t box[5] = {(cuuint32_t)p.chunk, (cuuint32_t)(kP2TileU * s), (cuuint32_t)(p.rows_v * s), 1, 1};
+        const cuuint32_t box[5] = {(cuuint32_t)p.chunk, (cuuint32_t)(p.pitch_u * s), (cuuint32_t)(p.rows_v * s), 1, 1};
         const cuuint32_t estr[5] = {1, (cuuint32_t)s, (cuuint32_t)s, 1, 1};
         int rc = encode_map_nd(&map_a, d_in_planes, 5, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_64B);
         if (rc) return rc;
@@ -694,14 +806,16 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
                                MODE == kP2SplitTf32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
         if (rc) return rc;
     }
-    static bool attr_done = false;
-    if (!attr_done) {
-        SESSD_CUDA_TRY(cudaFuncSetAttribute(bev_conv_p2_kernel<32, MODE, PROFILE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2MaxSmem));
-        SESSD_CUDA_TRY(cudaFuncSetAttribute(bev_conv_p2_kernel<128, MODE, PROFILE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2MaxSmem));
-        attr_done = true;
+    // A from registers only in the planes mode: the split modes write their operand planes from the consumer threads
+    constexpr bool kRegA = MODE == kP2Planes;
+    auto kernel = bev_conv_p2_kernel<128, MODE, false, PROBE>;
+    if (p.n_tile == 32) kernel = reg_a ? bev_conv_p2_kernel<32, MODE, kRegA, PROBE> : bev_conv_p2_kernel<32, MODE, false, PROBE>;
+    else if (reg_a) kernel = bev_conv_p2_kernel<128, MODE, kRegA, PROBE>;
+    static bool attr_done[2][2] = {};
+    if (!attr_done[p.n_tile == 32][reg_a]) {
+        SESSD_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2MaxSmem));
+        attr_done[p.n_tile == 32][reg_a] = true;
     }
-    p.bstage_bytes = bstage;
-    p.bstages = p.bring_bytes / p.bstage_bytes < kP2MaxBStages ? p.bring_bytes / p.bstage_bytes : kP2MaxBStages;
     p.in_info = MODE == kP2Planes ? d_in_info : nullptr;
     p.in_amax = MODE == kP2SplitF16 ? d_in_info : nullptr;
     p.resid_info = d_residual ? d_resid_info : nullptr;
@@ -717,23 +831,21 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
         SESSD_CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
     }
     const int grid = p.total < num_sms ? p.total : num_sms;                 // persistent, one CTA per SM
-    if (p.n_tile == 32)
-        SESSD_LAUNCH((bev_conv_p2_kernel<32, MODE, PROFILE>), grid, kP2Threads, smem, (cudaStream_t)stream, map_a, map_b, d_scale, d_shift, d_residual, d_out_f32,
-                     (__half *)d_out_planes, p);
-    else
-        SESSD_LAUNCH((bev_conv_p2_kernel<128, MODE, PROFILE>), grid, kP2Threads, smem, (cudaStream_t)stream, map_a, map_b, d_scale, d_shift, d_residual, d_out_f32,
-                     (__half *)d_out_planes, p);
+    SESSD_LAUNCH(kernel, grid, reg_a ? kP2ThreadsRegA : kP2Threads, smem, (cudaStream_t)stream, map_a, map_b, d_scale, d_shift, d_residual, d_out_f32,
+                 (__half *)d_out_planes, p);
     return last_error();
 }
 
 
-// one tap-list conv (sessd_conv_desc) / the four-class deconv through launch_p2<MODE, PROFILE>; d_prof: [grid][kP2ProfWords] (PROFILE)
-template <int MODE, bool PROFILE = false>
+// one tap-list conv (sessd_conv_desc) / the four-class deconv through launch_p2<MODE, PROBE>; d_prof: [grid][kP2ProfWords] (probes).
+// Stride-1 launches from planes take A from registers (one patch copy); smem_a (the loads probe) plans them for the shared-memory
+// descriptors instead, for comparison.
+template <int MODE, int PROBE = kP2NoProbe>
 static int p2_conv(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                    const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                    float *d_out_f32, void *d_out_planes, float *d_out_info, const sessd_conv_desc *desc, void *stream,
-                   const int *d_items = nullptr, long long *d_prof = nullptr) {
-    if (!desc || (PROFILE && !d_prof)) return SESSD_EINVAL;
+                   const int *d_items = nullptr, long long *d_prof = nullptr, bool smem_a = false) {
+    if (!desc || (PROBE != kP2NoProbe && !d_prof)) return SESSD_EINVAL;
     const sessd_conv_desc &d = *desc;
     if (d.ntaps < 1 || d.ntaps > 9 || (d.in_stride != 1 && d.in_stride != 2) || d.out_stride < 1) return SESSD_EINVAL;
     if ((d.grid_h - 1) * d.out_stride + d.out_off_y >= d.out_h || (d.grid_w - 1) * d.out_stride + d.out_off_x >= d.out_w) return SESSD_EINVAL;
@@ -745,16 +857,17 @@ static int p2_conv(const void *d_in_planes, const float *d_in_info, const void *
     P2Taps t = {};
     t.n = d.ntaps; t.off_y = d.out_off_y; t.off_x = d.out_off_x;
     for (int i = 0; i < d.ntaps; ++i) { t.dy[i] = d.tap_dy[i]; t.dx[i] = d.tap_dx[i]; t.w[i] = i; }
-    return launch_p2<MODE, PROFILE>(d_in_planes, d.in_h, d.in_w, d_in_info, d_weight_h2, d.ntaps, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
-                     shift_max, d_out_f32, d_out_planes, d_out_info, p, &t, 1, d.grid_h, d.grid_w, stream);
+    return launch_p2<MODE, PROBE>(d_in_planes, d.in_h, d.in_w, d_in_info, d_weight_h2, d.ntaps, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
+                     shift_max, d_out_f32, d_out_planes, d_out_info, p, &t, 1, d.grid_h, d.grid_w, MODE == kP2Planes && d.in_stride == 1 && !smem_a,
+                     stream);
 }
 
-template <int MODE, bool PROFILE = false>
+template <int MODE, int PROBE = kP2NoProbe>
 static int p2_deconv(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                      const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                      float *d_out_f32, void *d_out_planes, float *d_out_info, int batch, int in_h, int in_w, int cin, int cout,
                      int relu, void *stream, const int *d_items = nullptr, long long *d_prof = nullptr) {
-    if (PROFILE && !d_prof) return SESSD_EINVAL;
+    if (PROBE != kP2NoProbe && !d_prof) return SESSD_EINVAL;
     P2Params p = {};
     p.batch = batch; p.cin = cin; p.cout = cout; p.in_stride = 1;
     p.out_h = 2 * in_h; p.out_w = 2 * in_w; p.out_stride = 2; p.relu = relu;
@@ -762,8 +875,8 @@ static int p2_deconv(const void *d_in_planes, const float *d_in_info, const void
     p.prof = d_prof;
     P2Taps cls[4];
     p2_deconv_classes(cls);
-    return launch_p2<MODE, PROFILE>(d_in_planes, in_h, in_w, d_in_info, d_weight_h2, 9, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
-                     d_out_f32, d_out_planes, d_out_info, p, cls, 4, in_h, in_w, stream);
+    return launch_p2<MODE, PROBE>(d_in_planes, in_h, in_w, d_in_info, d_weight_h2, 9, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
+                     d_out_f32, d_out_planes, d_out_info, p, cls, 4, in_h, in_w, MODE == kP2Planes, stream);
 }
 
 }  // namespace sessd

@@ -42,13 +42,13 @@ extern "C" int sessd_bev_deconv_h2(const float *d_in, const void *d_weight_h2, i
 }
 
 // Stall profile of the product's planes kernel (scripts/p2_stall_profile.py): sessd_bev_conv_p2 / sessd_bev_deconv_p2 with the clock
-// counters of the PROFILE instantiation written to d_prof, [grid][kP2ProfWords] int64 (P2Prof, grid = min(work items, SMs)).
+// counters of the kP2ProbeClocks instantiation written to d_prof, [grid][kP2ProfWords] int64 (P2Prof, grid = min(work items, SMs)).
 extern "C" int sessd_bev_conv_p2_profile(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
                                          const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
                                          float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info,
                                          const sessd_conv_desc *desc, const int *d_items, long long *d_prof, void *stream) {
-    return p2_conv<kP2Planes, true>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
-                                    d_out_f32, d_out_planes, d_out_info, desc, stream, d_items, d_prof);
+    return p2_conv<kP2Planes, kP2ProbeClocks>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
+                                              shift_max, d_out_f32, d_out_planes, d_out_info, desc, stream, d_items, d_prof);
 }
 
 extern "C" int sessd_bev_deconv_p2_profile(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
@@ -56,7 +56,18 @@ extern "C" int sessd_bev_deconv_p2_profile(const void *d_in_planes, const float 
                                            float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, int batch,
                                            int in_h, int in_w, int cin, int cout, int relu, const int *d_items, long long *d_prof,
                                            void *stream) {
-    return p2_deconv<kP2Planes, true>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
-                                      shift_max, d_out_f32, d_out_planes, d_out_info, batch, in_h, in_w, cin, cout, relu, stream, d_items,
-                                      d_prof);
+    return p2_deconv<kP2Planes, kP2ProbeClocks>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
+                                                shift_max, d_out_f32, d_out_planes, d_out_info, batch, in_h, in_w, cin, cout, relu, stream,
+                                                d_items, d_prof);
+}
+
+// The loader-only probe: the launch of sessd_bev_conv_p2_profile with consumers that wait on the full barriers and release them,
+// no wgmma and no epilogue (no output is written).  smem_a != 0 plans a stride-1 conv's patches as shared-memory A descriptors would
+// need them (one copy per tap shift along u), the plan these launches had before A came from registers.
+extern "C" int sessd_bev_conv_p2_loads(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
+                                       const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
+                                       float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info,
+                                       const sessd_conv_desc *desc, const int *d_items, int smem_a, long long *d_prof, void *stream) {
+    return p2_conv<kP2Planes, kP2ProbeLoads>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
+                                             shift_max, d_out_f32, d_out_planes, d_out_info, desc, stream, d_items, d_prof, smem_a != 0);
 }

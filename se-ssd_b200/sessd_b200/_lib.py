@@ -122,6 +122,7 @@ LAB_SIGNATURES = {
     "sessd_bev_conv_p2_profile": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp, _vp]),
     "sessd_bev_deconv_p2_profile": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp,
                                          _vp]),
+    "sessd_bev_conv_p2_loads": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _i, _vp, _vp]),
 }
 
 
