@@ -410,10 +410,25 @@ int sessd_head_loss(const float *d_head, const float *d_anchors, const int *d_la
  *                 launch (a = alpha, b = 1 - alpha), and the 1 / world_size scaling after the gradient all-reduce
  *                 (det3d/core/utils/dist_utils.py:8-29) with d_x = NULL;
  * sessd_adamw_step -- Adam with decoupled weight decay (the fastai true_wd step of det3d/solver/fastai_optim.py == torch.optim.AdamW).
+ * sessd_grad_sqnorm -- the gradient clip of det3d/torchie/trainer/hooks/optimizer.py:35-62 (clip_grad_norm_(params, max_norm=35,
+ *                 norm_type=2), optimizer_config of examples/second/configs/config.py:257-260) without a host round trip: d_out[0] =
+ *                 total_norm (fp32, sqrt of an fp64 sum, rounded once), d_out[1] = clip_coef = min(1, max_norm / (total_norm + 1e-6)),
+ *                 both on the device.  Bitwise deterministic run to run and across SM counts (the chunking depends on n only), so DDP
+ *                 ranks holding the same all-reduced arena clip identically.  d_workspace: sessd_grad_sqnorm_workspace_bytes(n) bytes,
+ *                 zero-filled once before first use, one stream at a time.
+ * sessd_adamw_clip_ema_step -- sessd_adamw_step (the same kernel) with the gradient scaled by *d_clip_coef and stored back, and the
+ *                 teacher EMA of det3d/torchie/trainer/trainer_sessd.py:315-318 (ema = alpha ema + (1 - alpha) p_new, with a = (float)alpha,
+ *                 b = (float)(1 - alpha) as sessd_axpby takes them) in the same pass; d_clip_coef and d_ema are nullable.  beta1 is the
+ *                 one-cycle momentum of the step (det3d/solver/learning_schedules_fastai.py:7-100); bias corrections use it.
  * ------------------------------------------------------------------------------------------------ */
 int sessd_axpby(float *d_y, const float *d_x, float a, float b, long long n, void *stream);
 int sessd_adamw_step(float *d_param, const float *d_grad, float *d_exp_avg, float *d_exp_avg_sq, long long n, float lr, float beta1,
                      float beta2, float eps, float weight_decay, int step, void *stream);
+size_t sessd_grad_sqnorm_workspace_bytes(long long n);
+int sessd_grad_sqnorm(const float *d_x, long long n, float max_norm, float *d_out, void *d_workspace, void *stream);
+int sessd_adamw_clip_ema_step(float *d_param, float *d_grad, float *d_exp_avg, float *d_exp_avg_sq, long long n, float lr, float beta1,
+                              float beta2, float eps, float weight_decay, int step, const float *d_clip_coef, float *d_ema, double ema_alpha,
+                              void *stream);
 
 #ifdef __cplusplus
 }

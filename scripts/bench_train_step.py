@@ -5,7 +5,10 @@ and weight-gradient times of the BevConvFunction on that launch's shapes (CUDA e
 gradient into planes) with TFLOP/s from FLOPs computed from the shapes (each of the three products counted as the launch's forward FLOPs),
 and a torch.profiler kernel table of one step from a separate run.
 
-    python scripts/bench_train_step.py [--batch 8] [--steps 20] [--warmup 5] [--layer-reps 10]
+    python scripts/bench_train_step.py [--batch 8] [--steps 20] [--warmup 5] [--layer-reps 10] [--recipe]
+
+--recipe runs the reference's optimiser recipe: the one-cycle lr / momentum schedule before each step, and clip (max-norm 35), AdamW
+and the teacher EMA as one fused device pass (ArenaAdamW.step(max_grad_norm=35, ema=..., global_step=...)).
 """
 import argparse
 import copy
@@ -63,6 +66,7 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--layer-reps", type=int, default=10)
+    ap.add_argument("--recipe", action="store_true")
     a = ap.parse_args()
     from det3d.models import build_detector
     from det3d.torchie import Config
@@ -88,11 +92,20 @@ def main():
         gts.append(gt)
     ex = synth.train_batch(cfg, clouds, gts)
     state = dict(n=0)
+    if a.recipe:
+        from det3d.solver import OneCycle
+        sched = OneCycle(opt, a.steps + a.warmup + 3, 0.003, [0.95, 0.85], 10.0, 0.4)
 
     def step():
         arena.zero_grad()
+        if a.recipe:
+            sched.step(state["n"])
         out = batch_processor_inline(model, ema, ex, consistency_weight=1.0, train_mode=True)
         out["loss"].backward()
+        if a.recipe:
+            opt.step(max_grad_norm=35.0, ema=arena_ema, global_step=state["n"])
+            state["n"] += 1
+            return
         opt.step()
         state["n"] += 1
         update_ema_variables(arena, arena_ema, state["n"])
@@ -137,7 +150,7 @@ def main():
             kernels[ev.key] = dict(calls=int(ev.count), us=round(float(ev.device_time_total), 1))
     tops = dict(sorted(kernels.items(), key=lambda kv: -kv[1]["us"])[:30])
     name, pl = card()
-    print(json.dumps(dict(gpu=name, power_limit=pl, sm_clock_mhz_now_max=sm_clock, batch=a.batch, step_ms=step_ms,
+    print(json.dumps(dict(gpu=name, power_limit=pl, sm_clock_mhz_now_max=sm_clock, batch=a.batch, recipe=a.recipe, step_ms=step_ms,
                           neck_head_fwd_gflop=round(neck_gflop, 2), neck_head_bwd_gflop=round(2 * neck_gflop, 2),
                           neck_fwd_ms=round(sum(l["fwd_ms"] for l in layers), 3),
                           neck_dgrad_ms=round(sum(l["dgrad_ms"] for l in layers), 3),

@@ -5,6 +5,8 @@ NCCL over NVLink / NVSwitch -- instead of flatten -> all_reduce -> divide -> unf
 import torch
 import torch.distributed as dist
 
+from ...torchie.trainer.hooks.optimizer import clip_and_step
+
 
 def _grads(params):
     return [p.grad for p in params if p.requires_grad and p.grad is not None]
@@ -64,7 +66,9 @@ def allreduce_grads(params, coalesce=True, bucket_size_mb=-1):
 
 
 class DistOptimizerHook(object):
-    """after_train_iter: zero_grad -> backward -> allreduce_grads -> (clip) -> optimizer.step, like the reference hook."""
+    """after_train_iter: zero_grad -> backward -> allreduce_grads -> (clip) -> optimizer.step, like the reference hook.  Over an ArenaAdamW
+    that owns the model's gradient arena the L2 clip runs inside its step: a deterministic norm of the all-reduced arena, identical on
+    every rank (det3d.torchie.trainer.hooks.optimizer.clip_and_step)."""
 
     def __init__(self, grad_clip=None, coalesce=True, bucket_size_mb=-1):
         self.grad_clip, self.coalesce, self.bucket_size_mb = grad_clip, coalesce, bucket_size_mb
@@ -76,6 +80,4 @@ class DistOptimizerHook(object):
         runner.optimizer.zero_grad()
         runner.outputs["loss"].backward()
         allreduce_grads(runner.model.parameters(), self.coalesce, self.bucket_size_mb)
-        if self.grad_clip is not None:
-            self.clip_grads(runner.model.parameters())
-        runner.optimizer.step()
+        clip_and_step(runner.optimizer, runner.model.parameters(), self.grad_clip)

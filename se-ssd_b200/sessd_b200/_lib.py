@@ -108,6 +108,9 @@ SIGNATURES = {
     "sessd_iou_pred_loss": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _vp, _vp, _vp, _sz, _vp]),
     "sessd_axpby": (_i, [_vp, _vp, _f, _f, _ll, _vp]),
     "sessd_adamw_step": (_i, [_vp, _vp, _vp, _vp, _ll, _f, _f, _f, _f, _f, _i, _vp]),
+    "sessd_grad_sqnorm_workspace_bytes": (_sz, [_ll]),
+    "sessd_grad_sqnorm": (_i, [_vp, _ll, _f, _vp, _vp, _vp]),
+    "sessd_adamw_clip_ema_step": (_i, [_vp, _vp, _vp, _vp, _ll, _f, _f, _f, _f, _f, _i, _vp, _vp, C.c_double, _vp]),
     "sessd_assign_workspace_bytes": (_sz, [_i, _i, _i]),
     "sessd_assign_targets": (_i, [_vp, _i, _vp, _vp, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
