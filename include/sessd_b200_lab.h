@@ -1,7 +1,8 @@
-/* sessd_b200_lab.h -- C ABI of libsessd_b200_lab.so: the NON-DEFAULT BEV conv variants kept for cross-implementation tests
- * (csrc/bevconv_split.cu): fp32 NHWC input split inside the wgmma kernel, either into 3xTF32 (tf32 wgmma) or into two-term fp16
- * (fp16 wgmma); and a clock-counting build of the product's planes kernel for stall profiles.  Nothing in the product path
- * (libsessd_b200.so, sessd_b200.engine) links or loads this library.  Same conventions as sessd_b200.h. */
+/* sessd_b200_lab.h -- C ABI of libsessd_b200_lab.so (csrc/bevconv_split.cu): the BEV conv with its fp32 NHWC input split into two-term
+ * fp16 inside the wgmma kernel and three separate products per MAC, the bitwise reference of the product kernel's folded wgmma
+ * (tests/test_gpu_bev_p2_vs_h2.py); clock-counting and loader-only builds of the product's planes kernel for stall profiles; and the
+ * launcher's plan, for the tests' restatement of it.  Nothing in the product path (libsessd_b200.so, sessd_b200.engine) links or
+ * loads this library.  Same conventions as sessd_b200.h. */
 #ifndef SESSD_B200_LAB_H
 #define SESSD_B200_LAB_H
 
@@ -11,21 +12,9 @@
 extern "C" {
 #endif
 
-/* 3xTF32 BEV conv (tf32 wgmma, three products per MAC): same contract as sessd_bev_conv (in_stride 1 or 2, cin % 64 == 0, cout % 8 == 0).
- * d_weight_split [2 (hi|lo)][ntaps][cout_pad][cin]: hi = weights truncated to tf32, lo = w - hi; cout_pad is a multiple of the
- * N tile (128; 32 when cout <= 32).  d_scale nullable (identity). */
-int sessd_bev_conv_tc(const float *d_in, const float *d_weight_split, int cout_pad, const float *d_scale,
-                      const float *d_shift, const float *d_residual, float *d_out, const sessd_conv_desc *desc,
-                      void *stream);
-
-/* ConvTranspose2d(k3, s2, p1, op1) + BN + ReLU (+ residual) in one launch; d_weight_split [2][9][cout_pad][cin],
- * tap = ky*3+kx of W[cin][cout][ky][kx]; output [batch, 2*in_h, 2*in_w, cout] NHWC (rpn_v1.py:183-195). */
-int sessd_bev_deconv_tc(const float *d_in, const float *d_weight_split, int cout_pad, const float *d_scale,
-                        const float *d_shift, const float *d_residual, float *d_out, int batch, int in_h, int in_w,
-                        int cin, int cout, int relu, void *stream);
-
-/* fp16-split BEV conv from fp32 input (the split happens in shared memory): same contract as sessd_bev_conv_tc, in_stride 1 only
- * (a stride-2 patch and its fp32 staging copy do not fit in shared memory: SESSD_EINVAL).
+/* fp16-split BEV conv from fp32 input (the split happens in shared memory): in_stride 1 or 2, cin % 64 == 0, cout % 8 == 0; a stride-2
+ * 3x3 patch and its fp32 staging copy leave room for the weight ring only at cout_pad 32 (else SESSD_EINVAL).  cout_pad is a multiple of
+ * the N tile (128; 32 when cout <= 32).
  * d_weight_h2: __half [2 (hi|lo)][ntaps][cout_pad][cin] of 2^e[n]*w (per output channel n; max |2^e w| in [2^10, 2^11));
  * d_scale (required) = folded BN scale * 2^-e[n].
  * d_amax_in  (nullable): device scalar >= max|in| -- selects the activation scaling 2^s; NULL = no scaling (|in| must stay < 65504).
@@ -58,6 +47,12 @@ int sessd_bev_conv_p2_loads(const void *d_in_planes, const float *d_in_info, con
                             const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
                             float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info,
                             const sessd_conv_desc *desc, const int *d_items, int smem_a, long long *d_prof, void *stream);
+
+/* The launch plan of the conv desc (deconv != 0: of the deconv of desc's batch, in_h, in_w, cin and cout) as sessd_bev_conv_p2 (split 0;
+ * smem_a as for sessd_bev_conv_p2_loads) or sessd_bev_conv_h2 (split != 0) would launch it, without launching: plan[19] =
+ * {u_is_x, n_tile, nblocks, tiles, total, ncopies, rows_v, pitch_u, npatch, bstages, dynamic shared memory bytes, taps of class 0-3,
+ * class order 0-3} (0 past the launch's classes).  SESSD_EINVAL where the launcher refuses the launch.  Touches no device. */
+int sessd_bev_p2_plan(const sessd_conv_desc *desc, int deconv, int cout_pad, int split, int smem_a, int *plan);
 
 #ifdef __cplusplus
 }

@@ -1,5 +1,6 @@
 // bevconv_p2.cuh -- BEV conv / deconv (+BN+ReLU+residual) on the Hopper tensor cores (wgmma) from PRE-SPLIT fp16 planes
-// (the product's default path, bevconv_p2.cu) or from an fp32 input split inside the kernel (the lab formats, bevconv_split.cu).
+// (the product's default path, bevconv_p2.cu) or from an fp32 input split into fp16 planes inside the kernel (the lab's h2 mode,
+// bevconv_split.cu: the bitwise reference of the folded wgmma, three separate products per MAC).
 //
 // Replaces the cuDNN conv blocks of det3d/models/necks/rpn_v1.py:135-210 and the 1x1 head convs of
 // det3d/models/bbox_heads/mg_head_sessd.py:202-230 (fp32 in, fp32 out, fp32 accumulate).  Numerics: x = (x_hi + x_lo) / S with fp16
@@ -46,12 +47,12 @@ constexpr int kP2Threads = 320;                           // 10 warps
 constexpr int kP2ThreadsRegA = 384, kP2RegsConsumer = 232, kP2RegsProducer = 40;
 static_assert(2 * (kP2RegsConsumer - 168) <= 168 - kP2RegsProducer, "the consumers take what the producers release");
 constexpr int kP2MaxSmem = 227 * 1024;
+constexpr int kP2Chunk = 32;                              // input channels per K stage: one 64-byte fp16 operand row
 // optional device item list (bevskip.cu): int32 record, word 0 = number of items to run, the item indices from word kP2ItemsHeader on
 constexpr int kP2ItemsHeader = 32;
 // operand source of the A side: pre-split fp16 planes (TMA straight into the operand layout), or an fp32 NHWC input that TMA stages in
-// shared memory and the consumer warpgroups split there -- into fp16 (hi, lo) with the power-of-two scale of its abs-max (32-channel
-// chunks), or into tf32 hi = truncate(x), lo = x - hi for three tf32 products (16-channel chunks, fp32 weights [2][taps][cout_pad][cin])
-enum { kP2Planes = 0, kP2SplitF16 = 1, kP2SplitTf32 = 2 };
+// shared memory and the consumer warpgroups split there into fp16 (hi, lo) with the power-of-two scale of its abs-max
+enum { kP2Planes = 0, kP2SplitF16 = 1 };
 // lab instantiations: the product kernel with clock counters (P2Prof), or with counters and consumers that only wait on the full
 // barriers and release them -- no wgmma, no epilogue: what the two TMA producers alone can pull from L2
 enum { kP2NoProbe = 0, kP2ProbeClocks = 1, kP2ProbeLoads = 2 };
@@ -69,8 +70,7 @@ struct P2Params {
     int ncopies, rows_v, pitch_u;                         // copies, v rows and u positions per v row (8; REGA: 8 + the taps' u extent) of a copy
     int copy_u[kP2MaxCopies], copy_v[kP2MaxCopies];       // input coordinate of the copy's first element relative to (u0, v0) * in_stride
     int copy_bytes, patch_bytes, npatch;                  // bytes of one copy plane, of one patch buffer (ncopies x 2 planes), 1 or 2 buffers
-    int chunk;                         // input channels per K stage: 32 (fp16 operands) or 16 (tf32 operands); 64-byte operand rows either way
-    int load_bytes, staging_bytes;     // TMA bytes per patch buffer; fp32 staging bytes per patch buffer (split modes, else 0)
+    int load_bytes, staging_bytes;     // TMA bytes per patch buffer; fp32 staging bytes per patch buffer (split mode, else 0)
     int bring_bytes;                   // bytes of the weight-stage ring
     int out_info_scale;                // 1: out_info = {abs-max, S_out} (planes chain); 0: out_info is a single running abs-max
     const float *in_amax;              // split fp16 mode: abs-max of the fp32 input (nullable: scale 1)
@@ -132,18 +132,13 @@ __device__ __forceinline__ P2Item p2_decode(const P2Params &p, int g) {
     return it;
 }
 
-// N output columns: NT (one plane of the weight stage) or, fp16 only, 2 NT (the whole [b_lo ; b_hi] stage)
-template <int N, int MODE>
+// N output columns: NT (one plane of the weight stage) or 2 NT (the whole [b_lo ; b_hi] stage)
+template <int N>
 __device__ __forceinline__ void p2_wgmma(float *d, uint64_t da, uint64_t db, uint32_t accumulate) {
-    if constexpr (MODE == kP2SplitTf32) {
-        if constexpr (N == 32) wgmma_tf32_n32(d, da, db, accumulate);
-        else wgmma_tf32_n128(d, da, db, accumulate);
-    } else {
-        if constexpr (N == 32) wgmma_f16_n32(d, da, db, accumulate);
-        else if constexpr (N == 64) wgmma_f16_n64(d, da, db, accumulate);
-        else if constexpr (N == 128) wgmma_f16_n128(d, da, db, accumulate);
-        else wgmma_f16_n256(d, da, db, accumulate);
-    }
+    if constexpr (N == 32) wgmma_f16_n32(d, da, db, accumulate);
+    else if constexpr (N == 64) wgmma_f16_n64(d, da, db, accumulate);
+    else if constexpr (N == 128) wgmma_f16_n128(d, da, db, accumulate);
+    else wgmma_f16_n256(d, da, db, accumulate);
 }
 
 // the same with the A fragment (one k16 of this warp's 16 rows, ldsm_x4) in registers
@@ -193,15 +188,8 @@ __device__ __forceinline__ void p2_tock(long long &clk, long long t0) {
     if constexpr (PROFILE) clk += clock64() - t0;
 }
 
-__device__ __forceinline__ float p2_tf32_rn(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return __uint_as_float(r);
-}
-
-// split modes: the fp32 staging copy of patch buffer pb -> the (hi, lo) operand planes in the SWIZZLE_64B layout (16-byte chunk j of a
+// split mode: the fp32 staging copy of patch buffer pb -> the (hi, lo) operand planes in the SWIZZLE_64B layout (16-byte chunk j of a
 // 64-byte row r lands at chunk j ^ ((r >> 1) & 3)); run by the 256 consumer threads, which then sync among themselves
-template <int MODE>
 __device__ __forceinline__ void p2_split_patch(const P2Params &p, const unsigned char *staging, unsigned char *planes, float s_in, int ctid) {
     const int rows = p.rows_v * kP2TileU;
     const int copy_in = p.staging_bytes / p.ncopies;
@@ -209,24 +197,15 @@ __device__ __forceinline__ void p2_split_patch(const P2Params &p, const unsigned
     for (int i = ctid; i < items; i += kP2MmaWarps * 32) {
         const int j = i & 3, r = (i >> 2) % rows, c = (i >> 2) / rows;
         unsigned char *hi = planes + 2 * c * p.copy_bytes + r * 64 + ((j ^ ((r >> 1) & 3)) << 4);
-        if constexpr (MODE == kP2SplitF16) {          // 32 fp32 per staging row -> 8 of them per 16-byte fp16 chunk
-            const float4 *src = reinterpret_cast<const float4 *>(staging + c * copy_in + r * 128 + j * 32);
-            const float4 a = src[0], b = src[1];
-            const float x[8] = {a.x * s_in, a.y * s_in, a.z * s_in, a.w * s_in, b.x * s_in, b.y * s_in, b.z * s_in, b.w * s_in};
-            __align__(16) __half h[8], l[8];
+        // 32 fp32 per staging row -> 8 of them per 16-byte fp16 chunk
+        const float4 *src = reinterpret_cast<const float4 *>(staging + c * copy_in + r * 128 + j * 32);
+        const float4 a = src[0], b = src[1];
+        const float x[8] = {a.x * s_in, a.y * s_in, a.z * s_in, a.w * s_in, b.x * s_in, b.y * s_in, b.z * s_in, b.w * s_in};
+        __align__(16) __half h[8], l[8];
 #pragma unroll
-            for (int t = 0; t < 8; ++t) { h[t] = __float2half_rn(x[t]); l[t] = __float2half_rn(x[t] - __half2float(h[t])); }
-            *reinterpret_cast<uint4 *>(hi) = *reinterpret_cast<const uint4 *>(h);
-            *reinterpret_cast<uint4 *>(hi + p.copy_bytes) = *reinterpret_cast<const uint4 *>(l);
-        } else {                                      // 16 fp32 per staging row -> 4 of them per 16-byte tf32 chunk
-            const float4 x = *reinterpret_cast<const float4 *>(staging + c * copy_in + r * 64 + j * 16);
-            const float4 h = make_float4(__uint_as_float(__float_as_uint(x.x) & ~0x1FFFu), __uint_as_float(__float_as_uint(x.y) & ~0x1FFFu),
-                                         __uint_as_float(__float_as_uint(x.z) & ~0x1FFFu), __uint_as_float(__float_as_uint(x.w) & ~0x1FFFu));
-            *reinterpret_cast<float4 *>(hi) = h;
-            // lo rounded to the nearest tf32 here: the tensor core would truncate it (a bias that grows with K)
-            *reinterpret_cast<float4 *>(hi + p.copy_bytes) = make_float4(p2_tf32_rn(x.x - h.x), p2_tf32_rn(x.y - h.y), p2_tf32_rn(x.z - h.z),
-                                                                         p2_tf32_rn(x.w - h.w));
-        }
+        for (int t = 0; t < 8; ++t) { h[t] = __float2half_rn(x[t]); l[t] = __float2half_rn(x[t] - __half2float(h[t])); }
+        *reinterpret_cast<uint4 *>(hi) = *reinterpret_cast<const uint4 *>(h);
+        *reinterpret_cast<uint4 *>(hi + p.copy_bytes) = *reinterpret_cast<const uint4 *>(l);
     }
     asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");      // generic-proxy writes -> visible to wgmma
     asm volatile("bar.sync 1, %0;\n" ::"n"(kP2MmaWarps * 32) : "memory");
@@ -254,7 +233,7 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == kP2PatchWarp * 32) prefetch_tensormap(&map_a);    // descriptor fetches overlap barrier init
     if (threadIdx.x == kP2WeightWarp * 32) prefetch_tensormap(&map_b);
-    const int nchunks = p.cin / p.chunk;
+    const int nchunks = p.cin / kP2Chunk;
     const int nitems = p2_item_count(p);
     const uint32_t b_plane_bytes = (uint32_t)p.n_tile * 64u;      // bytes of the b_hi (or b_lo) rows per (tap, chunk)
 
@@ -295,14 +274,14 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
                             uint32_t dst = patches_u32 + (uint32_t)(pb * p.patch_bytes);
                             for (int c = 0; c < p.ncopies; ++c, dst += 2u * (uint32_t)p.copy_bytes) {
                                 const int cu = bu + p.copy_u[c], cv = bv + p.copy_v[c];
-                                tma_load_5d(dst, &map_a, &patch_full[pb], cc * p.chunk, cu, cv, it.b, 0);
-                                tma_load_5d(dst + (uint32_t)p.copy_bytes, &map_a, &patch_full[pb], cc * p.chunk, cu, cv, it.b, 1);
+                                tma_load_5d(dst, &map_a, &patch_full[pb], cc * kP2Chunk, cu, cv, it.b, 0);
+                                tma_load_5d(dst + (uint32_t)p.copy_bytes, &map_a, &patch_full[pb], cc * kP2Chunk, cu, cv, it.b, 1);
                             }
                         } else {
                             const uint32_t copy_in = (uint32_t)(p.staging_bytes / p.ncopies);
                             uint32_t dst = smem_u32(staging) + (uint32_t)(pb * p.staging_bytes);
                             for (int c = 0; c < p.ncopies; ++c, dst += copy_in)
-                                tma_load_5d(dst, &map_a, &patch_full[pb], cc * p.chunk, bu + p.copy_u[c], bv + p.copy_v[c], it.b, 0);
+                                tma_load_5d(dst, &map_a, &patch_full[pb], cc * kP2Chunk, bu + p.copy_u[c], bv + p.copy_v[c], it.b, 0);
                         }
                     }
                     __syncwarp();
@@ -327,8 +306,8 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
                             unsigned char *st = tiles + S * p.bstage_bytes;
                             const int wtap = p.tap_w[it.cls][tap];
                             mbar_expect_tx(&b_full[S], 2 * b_plane_bytes);
-                            tma_load_4d(st + b_plane_bytes, &map_b, &b_full[S], cc * p.chunk, it.n0, wtap, 0);
-                            tma_load_4d(st, &map_b, &b_full[S], cc * p.chunk, it.n0, wtap, 1);
+                            tma_load_4d(st + b_plane_bytes, &map_b, &b_full[S], cc * kP2Chunk, it.n0, wtap, 0);
+                            tma_load_4d(st, &map_b, &b_full[S], cc * kP2Chunk, it.n0, wtap, 1);
                         }
                         __syncwarp();
                         if (++S == p.bstages) { S = 0; bph ^= 1u; }
@@ -375,11 +354,9 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
             // acc[0, kAcc): cross a_hi x b_lo + a_lo x b_hi, acc[kAcc, NT): main a_hi x b_hi -- the fragment of an m64n(2 NT) over the
             // whole [b_lo ; b_hi] weight stage.  The cross half comes first: ptxas serializes every wgmma of the kernel when one of them
             // accumulates into a part of another's fragment that does not start at its first register.
-            float acc[NT], tot[MODE == kP2SplitTf32 ? kAcc : 1];
+            float acc[NT];
 #pragma unroll
             for (int i = 0; i < NT; ++i) acc[i] = 0.f;
-#pragma unroll
-            for (int i = 0; i < (MODE == kP2SplitTf32 ? kAcc : 1); ++i) tot[i] = 0.f;
             int prevS = -1, prev_pb = -1;
             bool first = true;
             if constexpr (REGA) {
@@ -445,43 +422,34 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
             } else {
                 for (int cc = 0; cc < nchunks; ++cc) {
                     { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&patch_full[pb], pph); p2_tock<PROFILE>(clk[kProfPatchFull], t0); }
-                    if constexpr (MODE != kP2Planes)
-                        p2_split_patch<MODE>(p, staging + pb * p.staging_bytes, patches + pb * p.patch_bytes, s_in, threadIdx.x);
+                    if constexpr (MODE == kP2SplitF16)
+                        p2_split_patch(p, staging + pb * p.staging_bytes, patches + pb * p.patch_bytes, s_in, threadIdx.x);
                     const uint32_t pbase = patch_lo + (uint32_t)pb * patch_sz;
 #pragma unroll 1
                     for (int tap = 0; tap < ntaps; ++tap) {
                         { const long long t0 = p2_tick<PROFILE>(); mbar_wait(&b_full[S], bph); p2_tock<PROFILE>(clk[kProfBFull], t0); }
-                        if constexpr (MODE == kP2SplitTf32) {
-                            // the weights' lo plane rounded to the nearest tf32 in place (the tensor core would truncate it)
-                            float *wl = reinterpret_cast<float *>(tiles + S * p.bstage_bytes);
-                            for (int i = threadIdx.x; i < (int)(b_plane_bytes / 4); i += kP2MmaWarps * 32) wl[i] = p2_tf32_rn(wl[i]);
-                            asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-                            asm volatile("bar.sync 1, %0;\n" ::"n"(kP2MmaWarps * 32) : "memory");
-                        }
                         if constexpr (!LOADS_ONLY) {
                             const uint64_t da_hi = kDescSw64Hi | (uint64_t)(pbase + aoff[tap]);
                             const uint64_t da_lo = da_hi + (uint64_t)copy_lo;
                             const uint64_t db_lo = kDescSw64Hi | (uint64_t)(tiles_lo + (uint32_t)(S * (p.bstage_bytes >> 4)));
                             const uint64_t db_hi = db_lo + (uint64_t)plane_lo;
                             const uint32_t accum = first ? 0u : 1u;
-                            // K = 16 fp16 / 8 tf32 per instruction = 32 bytes of the 64-byte row
+                            // K = 16 fp16 per instruction = 32 bytes of the 64-byte row
                             wgmma_fence();
-                            // tf32: the main accumulator restarts every chunk (its chunk partial is added into `tot` in RN fp32 below)
-                            const uint32_t acc_main = MODE == kP2SplitTf32 ? (tap != 0 ? 1u : 0u) : accum;
                             if constexpr (MODE == kP2Planes) {
                                 // one m64n(2 NT) per k16 over the stacked stage: cross (+)= a_hi x b_lo and main (+)= a_hi x b_hi read
-                                // a_hi once.  Each accumulator sums in the order of the three-product sequence below (the lab modes'
+                                // a_hi once.  Each accumulator sums in the order of the three-product sequence below (the h2 mode's
                                 // bitwise reference).
-                                p2_wgmma<2 * NT, MODE>(acc, da_hi, db_lo, accum);
-                                p2_wgmma<2 * NT, MODE>(acc, da_hi + 2, db_lo + 2, 1u);
+                                p2_wgmma<2 * NT>(acc, da_hi, db_lo, accum);
+                                p2_wgmma<2 * NT>(acc, da_hi + 2, db_lo + 2, 1u);
                             } else {
-                                p2_wgmma<NT, MODE>(acc + kAcc, da_hi, db_hi, acc_main);       // main  (+)= a_hi x b_hi
-                                p2_wgmma<NT, MODE>(acc + kAcc, da_hi + 2, db_hi + 2, 1u);
-                                p2_wgmma<NT, MODE>(acc, da_hi, db_lo, accum);                 // cross (+)= a_hi x b_lo
-                                p2_wgmma<NT, MODE>(acc, da_hi + 2, db_lo + 2, 1u);
+                                p2_wgmma<NT>(acc + kAcc, da_hi, db_hi, accum);       // main  (+)= a_hi x b_hi
+                                p2_wgmma<NT>(acc + kAcc, da_hi + 2, db_hi + 2, 1u);
+                                p2_wgmma<NT>(acc, da_hi, db_lo, accum);              // cross (+)= a_hi x b_lo
+                                p2_wgmma<NT>(acc, da_hi + 2, db_lo + 2, 1u);
                             }
-                            p2_wgmma<NT, MODE>(acc, da_lo, db_hi, 1u);                        // cross  += a_lo x b_hi
-                            p2_wgmma<NT, MODE>(acc, da_lo + 2, db_hi + 2, 1u);
+                            p2_wgmma<NT>(acc, da_lo, db_hi, 1u);                     // cross  += a_lo x b_hi
+                            p2_wgmma<NT>(acc, da_lo + 2, db_hi + 2, 1u);
                             wgmma_commit();
                         }
                         first = false;
@@ -496,21 +464,15 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
                         prev_pb = (tap == ntaps - 1) ? pb : -1;
                         if (++S == p.bstages) { S = 0; bph ^= 1u; }
                     }
-                    if (p.npatch == 1 || MODE == kP2SplitTf32) {
+                    if (p.npatch == 1) {
                         // one patch buffer: the next chunk's patch can only land once this one is released, so release it now rather
-                        // than after the next chunk's first step (that step would wait for the patch forever); tf32: drain the chunk
-                        // and fold its main partial
+                        // than after the next chunk's first step (that step would wait for the patch forever)
                         { const long long t0 = p2_tick<PROFILE>(); wgmma_wait<0>(); p2_tock<PROFILE>(clk[kProfMmaWait], t0); }
                         if (lane == 0) {
                             mbar_arrive(&b_empty[prevS]);
                             mbar_arrive(&patch_empty[pb]);
                         }
                         prevS = prev_pb = -1;
-                        if constexpr (MODE == kP2SplitTf32) {
-                            wgmma_fence_regs<kAcc>(acc + kAcc);
-#pragma unroll
-                            for (int i = 0; i < kAcc; ++i) tot[i] += acc[kAcc + i];
-                        }
                     }
                     if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
                 }
@@ -525,7 +487,7 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
             // epilogue: this thread holds tile rows r0 and r0 + 8, two adjacent channels of every 8-channel group; a transpose inside
             // each quad of lanes (one row) gives every lane 8 whole channels, stored 16 bytes at a time
 #pragma unroll
-            for (int i = 0; i < kAcc; ++i) acc[i] = (MODE == kP2SplitTf32 ? tot[i] : acc[kAcc + i]) + acc[i];      // main + cross
+            for (int i = 0; i < kAcc; ++i) acc[i] = acc[kAcc + i] + acc[i];      // main + cross
             const P2Item it = p2_decode(p, g);
             const int q = lane & 3;
             const int r0 = wg * 64 + wq * 16 + (lane >> 2);
@@ -686,26 +648,14 @@ static int p2_geometry(P2Geometry &g, int batch, int grid_h, int grid_w, int cou
     return 0;
 }
 
-// MODE kP2Planes: d_in = fp16 planes [2][B][H][W][C], d_in_info = {abs-max, S}; split modes: d_in = fp32 NHWC, d_in_info = the input's
-// abs-max (split fp16; nullable) or unused (tf32), weights fp32 [2][taps][cout_pad][cin] in the tf32 mode; d_out_info is {abs-max, S_out}
-// in the planes mode and a single running abs-max otherwise
-template <int MODE, int PROBE = kP2NoProbe>
-static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d_in_info, const void *d_w, int w_taps, int cout_pad,
-                     const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info, float gain,
-                     float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, P2Params &p, const P2Taps *cls, int nclass,
-                     int grid_h, int grid_w, bool reg_a, void *stream) {
-    if (!d_in_planes || !d_w || (!d_out_f32 && !d_out_planes)) return SESSD_EINVAL;
-    if (MODE == kP2Planes && (!d_in_info || !d_scale)) return SESSD_EINVAL;
-    if (MODE != kP2Planes && d_out_planes) return SESSD_EINVAL;
-    if (reg_a && (MODE != kP2Planes || p.in_stride != 1)) return SESSD_EINVAL;
+// The launch plan: work-item geometry (p2_geometry), the patch copies and every (class, tap)'s copy, row and weight tap, and the
+// shared-memory split between the patch buffers and the weight-stage ring.  Reads p.batch, p.cin, p.cout and p.in_stride, fills the
+// plan fields of p and *smem (dynamic shared memory bytes), or returns SESSD_EINVAL for a launch the kernel cannot run.  Host only.
+static int p2_plan(P2Params &p, const P2Taps *cls, int nclass, int grid_h, int grid_w, int cout_pad, int mode, bool reg_a, int *smem) {
+    if (reg_a && (mode != kP2Planes || p.in_stride != 1)) return SESSD_EINVAL;
     if (p.cin < 64 || p.cin % 64) return SESSD_EINVAL;      // whole 64-channel groups
-    // the epilogue reads and writes 16 bytes at a time
-    if (((uintptr_t)d_scale | (uintptr_t)d_shift | (uintptr_t)d_residual | (uintptr_t)d_out_f32 | (uintptr_t)d_out_planes) & 15)
-        return SESSD_EINVAL;
     P2Geometry g;
     if (p2_geometry(g, p.batch, grid_h, grid_w, p.cout, cout_pad, cls, nclass)) return SESSD_EINVAL;
-    // a skip-plan record numbers the items of the width the runner packs: any other width decodes them to other classes / n-blocks
-    if (p.items && cout_pad != div_up(p.cout, g.n_tile) * g.n_tile) return SESSD_EINVAL;
     p.u_is_x = g.u_is_x; p.grid_u = g.grid_u; p.grid_v = g.grid_v;
     p.tiles_u = g.tiles_u; p.tiles_v = g.tiles_v; p.tiles = g.tiles;
     p.n_tile = g.n_tile; p.nblocks = g.nblocks; p.nclass = g.nclass; p.total = g.total;
@@ -758,12 +708,11 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
             p.tap_w[c][t] = cls[c].w[t];
         }
     }
-    p.chunk = MODE == kP2SplitTf32 ? 16 : 32;
     p.copy_bytes = (p.rows_v * p.pitch_u * 64 + 511) & ~511;      // whole 512-byte swizzle periods: every copy starts one
     p.patch_bytes = p.ncopies * 2 * p.copy_bytes;
-    // fp32 staging: 32 channels = 128-byte rows (split fp16) or 16 channels = 64-byte rows (tf32)
-    p.staging_bytes = MODE == kP2Planes ? 0 : p.ncopies * p.rows_v * kP2TileU * p.chunk * 4;
-    p.load_bytes = MODE == kP2Planes ? p.ncopies * 2 * p.rows_v * p.pitch_u * 64 : p.staging_bytes;
+    // fp32 staging (split mode): 32 channels = 128-byte rows
+    p.staging_bytes = mode == kP2Planes ? 0 : p.ncopies * p.rows_v * kP2TileU * kP2Chunk * 4;
+    p.load_bytes = mode == kP2Planes ? p.ncopies * 2 * p.rows_v * p.pitch_u * 64 : p.staging_bytes;
     const int per_buf = p.patch_bytes + p.staging_bytes, bstage = 2 * p.n_tile * 64;
     // after the ring and the patch buffers: barriers and tap offsets (1536 B with the 1 KB alignment slack), then scale / shift
     const int tail = 1536 + 16 + 2 * 4 * p.cout;
@@ -773,16 +722,36 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
     p.bstages = min((kP2MaxSmem - tail - p.npatch * per_buf) / bstage, kP2MaxBStages);
     if (p.bstages < 2) return SESSD_EINVAL;
     p.bring_bytes = p.bstages * bstage;
-    const int smem = p.bring_bytes + tail + p.npatch * per_buf;
+    *smem = p.bring_bytes + tail + p.npatch * per_buf;
+    return 0;
+}
+
+// MODE kP2Planes: d_in = fp16 planes [2][B][H][W][C], d_in_info = {abs-max, S}; kP2SplitF16: d_in = fp32 NHWC, d_in_info = the input's
+// abs-max (nullable); d_out_info is {abs-max, S_out} in the planes mode and a single running abs-max otherwise
+template <int MODE, int PROBE = kP2NoProbe>
+static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d_in_info, const void *d_w, int w_taps, int cout_pad,
+                     const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info, float gain,
+                     float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, P2Params &p, const P2Taps *cls, int nclass,
+                     int grid_h, int grid_w, bool reg_a, void *stream) {
+    if (!d_in_planes || !d_w || (!d_out_f32 && !d_out_planes)) return SESSD_EINVAL;
+    if (MODE == kP2Planes && (!d_in_info || !d_scale)) return SESSD_EINVAL;
+    if (MODE != kP2Planes && d_out_planes) return SESSD_EINVAL;
+    // the epilogue reads and writes 16 bytes at a time
+    if (((uintptr_t)d_scale | (uintptr_t)d_shift | (uintptr_t)d_residual | (uintptr_t)d_out_f32 | (uintptr_t)d_out_planes) & 15)
+        return SESSD_EINVAL;
+    int smem = 0;
+    if (p2_plan(p, cls, nclass, grid_h, grid_w, cout_pad, MODE, reg_a, &smem)) return SESSD_EINVAL;
+    // a skip-plan record numbers the items of the width the runner packs: any other width decodes them to other classes / n-blocks
+    if (p.items && cout_pad != div_up(p.cout, p.n_tile) * p.n_tile) return SESSD_EINVAL;
+    const int s = p.in_stride;
     CUtensorMap map_a, map_b;
-    const cuuint64_t es = MODE == kP2SplitTf32 ? 4 : 2;               // weight element bytes
     if (MODE != kP2Planes) {   // fp32 NHWC [B][H][W][C] viewed as {C, U, V, B, 1}, staged unswizzled
         const cuuint64_t row_w = (cuuint64_t)p.cin * 4, row_h = (cuuint64_t)in_w * p.cin * 4;
         const cuuint64_t dims[5] = {(cuuint64_t)p.cin, (cuuint64_t)(p.u_is_x ? in_w : in_h), (cuuint64_t)(p.u_is_x ? in_h : in_w),
                                     (cuuint64_t)p.batch, 1};
         const cuuint64_t strides[4] = {p.u_is_x ? row_w : row_h, p.u_is_x ? row_h : row_w, (cuuint64_t)in_h * in_w * p.cin * 4,
                                        (cuuint64_t)p.batch * in_h * in_w * p.cin * 4};
-        const cuuint32_t box[5] = {(cuuint32_t)p.chunk, (cuuint32_t)(kP2TileU * s), (cuuint32_t)(p.rows_v * s), 1, 1};
+        const cuuint32_t box[5] = {(cuuint32_t)kP2Chunk, (cuuint32_t)(kP2TileU * s), (cuuint32_t)(p.rows_v * s), 1, 1};
         const cuuint32_t estr[5] = {1, (cuuint32_t)s, (cuuint32_t)s, 1, 1};
         int rc = encode_map_nd(&map_a, d_in_planes, 5, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
         if (rc) return rc;
@@ -792,21 +761,20 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
                                     (cuuint64_t)p.batch, 2};
         const cuuint64_t strides[4] = {p.u_is_x ? row_w : row_h, p.u_is_x ? row_h : row_w, (cuuint64_t)in_h * in_w * p.cin * 2,
                                        (cuuint64_t)p.batch * in_h * in_w * p.cin * 2};
-        const cuuint32_t box[5] = {(cuuint32_t)p.chunk, (cuuint32_t)(p.pitch_u * s), (cuuint32_t)(p.rows_v * s), 1, 1};
+        const cuuint32_t box[5] = {(cuuint32_t)kP2Chunk, (cuuint32_t)(p.pitch_u * s), (cuuint32_t)(p.rows_v * s), 1, 1};
         const cuuint32_t estr[5] = {1, (cuuint32_t)s, (cuuint32_t)s, 1, 1};
         int rc = encode_map_nd(&map_a, d_in_planes, 5, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_64B);
         if (rc) return rc;
     }
-    {   // weights [2 (hi|lo)][taps][cout_pad][cin] fp16 (fp32 tf32 split in the tf32 mode): 64-byte rows of one K stage
+    {   // weights [2 (hi|lo)][taps][cout_pad][cin] fp16: 64-byte rows of one K stage
         const cuuint64_t dims[4] = {(cuuint64_t)p.cin, (cuuint64_t)cout_pad, (cuuint64_t)w_taps, 2};
-        const cuuint64_t strides[3] = {(cuuint64_t)p.cin * es, (cuuint64_t)cout_pad * p.cin * es, (cuuint64_t)w_taps * cout_pad * p.cin * es};
-        const cuuint32_t box[4] = {(cuuint32_t)p.chunk, (cuuint32_t)p.n_tile, 1, 1};
+        const cuuint64_t strides[3] = {(cuuint64_t)p.cin * 2, (cuuint64_t)cout_pad * p.cin * 2, (cuuint64_t)w_taps * cout_pad * p.cin * 2};
+        const cuuint32_t box[4] = {(cuuint32_t)kP2Chunk, (cuuint32_t)p.n_tile, 1, 1};
         const cuuint32_t estr[4] = {1, 1, 1, 1};
-        int rc = encode_map_nd(&map_b, d_w, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_64B,
-                               MODE == kP2SplitTf32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+        int rc = encode_map_nd(&map_b, d_w, 4, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_64B);
         if (rc) return rc;
     }
-    // A from registers only in the planes mode: the split modes write their operand planes from the consumer threads
+    // A from registers only in the planes mode: the split mode writes its operand planes from the consumer threads
     constexpr bool kRegA = MODE == kP2Planes;
     auto kernel = bev_conv_p2_kernel<128, MODE, false, PROBE>;
     if (p.n_tile == 32) kernel = reg_a ? bev_conv_p2_kernel<32, MODE, kRegA, PROBE> : bev_conv_p2_kernel<32, MODE, false, PROBE>;
@@ -837,6 +805,26 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
 }
 
 
+// the fields of P2Params that describe a tap-list conv (sessd_conv_desc) / the four-class deconv, and its tap classes
+static int p2_conv_params(const sessd_conv_desc &d, P2Params &p, P2Taps &t) {
+    if (d.ntaps < 1 || d.ntaps > 9 || (d.in_stride != 1 && d.in_stride != 2) || d.out_stride < 1) return SESSD_EINVAL;
+    if ((d.grid_h - 1) * d.out_stride + d.out_off_y >= d.out_h || (d.grid_w - 1) * d.out_stride + d.out_off_x >= d.out_w) return SESSD_EINVAL;
+    p = {};
+    p.batch = d.batch; p.cin = d.cin; p.cout = d.cout; p.in_stride = d.in_stride;
+    p.out_h = d.out_h; p.out_w = d.out_w; p.out_stride = d.out_stride; p.relu = d.relu;
+    t = {};
+    t.n = d.ntaps; t.off_y = d.out_off_y; t.off_x = d.out_off_x;
+    for (int i = 0; i < d.ntaps; ++i) { t.dy[i] = d.tap_dy[i]; t.dx[i] = d.tap_dx[i]; t.w[i] = i; }
+    return 0;
+}
+
+static void p2_deconv_params(int batch, int in_h, int in_w, int cin, int cout, int relu, P2Params &p, P2Taps cls[4]) {
+    p = {};
+    p.batch = batch; p.cin = cin; p.cout = cout; p.in_stride = 1;
+    p.out_h = 2 * in_h; p.out_w = 2 * in_w; p.out_stride = 2; p.relu = relu;
+    p2_deconv_classes(cls);
+}
+
 // one tap-list conv (sessd_conv_desc) / the four-class deconv through launch_p2<MODE, PROBE>; d_prof: [grid][kP2ProfWords] (probes).
 // Stride-1 launches from planes take A from registers (one patch copy); smem_a (the loads probe) plans them for the shared-memory
 // descriptors instead, for comparison.
@@ -847,16 +835,11 @@ static int p2_conv(const void *d_in_planes, const float *d_in_info, const void *
                    const int *d_items = nullptr, long long *d_prof = nullptr, bool smem_a = false) {
     if (!desc || (PROBE != kP2NoProbe && !d_prof)) return SESSD_EINVAL;
     const sessd_conv_desc &d = *desc;
-    if (d.ntaps < 1 || d.ntaps > 9 || (d.in_stride != 1 && d.in_stride != 2) || d.out_stride < 1) return SESSD_EINVAL;
-    if ((d.grid_h - 1) * d.out_stride + d.out_off_y >= d.out_h || (d.grid_w - 1) * d.out_stride + d.out_off_x >= d.out_w) return SESSD_EINVAL;
-    P2Params p = {};
-    p.batch = d.batch; p.cin = d.cin; p.cout = d.cout; p.in_stride = d.in_stride;
-    p.out_h = d.out_h; p.out_w = d.out_w; p.out_stride = d.out_stride; p.relu = d.relu;
+    P2Params p;
+    P2Taps t;
+    if (p2_conv_params(d, p, t)) return SESSD_EINVAL;
     p.items = d_items;
     p.prof = d_prof;
-    P2Taps t = {};
-    t.n = d.ntaps; t.off_y = d.out_off_y; t.off_x = d.out_off_x;
-    for (int i = 0; i < d.ntaps; ++i) { t.dy[i] = d.tap_dy[i]; t.dx[i] = d.tap_dx[i]; t.w[i] = i; }
     return launch_p2<MODE, PROBE>(d_in_planes, d.in_h, d.in_w, d_in_info, d_weight_h2, d.ntaps, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
                      shift_max, d_out_f32, d_out_planes, d_out_info, p, &t, 1, d.grid_h, d.grid_w, MODE == kP2Planes && d.in_stride == 1 && !smem_a,
                      stream);
@@ -868,13 +851,11 @@ static int p2_deconv(const void *d_in_planes, const float *d_in_info, const void
                      float *d_out_f32, void *d_out_planes, float *d_out_info, int batch, int in_h, int in_w, int cin, int cout,
                      int relu, void *stream, const int *d_items = nullptr, long long *d_prof = nullptr) {
     if (PROBE != kP2NoProbe && !d_prof) return SESSD_EINVAL;
-    P2Params p = {};
-    p.batch = batch; p.cin = cin; p.cout = cout; p.in_stride = 1;
-    p.out_h = 2 * in_h; p.out_w = 2 * in_w; p.out_stride = 2; p.relu = relu;
+    P2Params p;
+    P2Taps cls[4];
+    p2_deconv_params(batch, in_h, in_w, cin, cout, relu, p, cls);
     p.items = d_items;
     p.prof = d_prof;
-    P2Taps cls[4];
-    p2_deconv_classes(cls);
     return launch_p2<MODE, PROBE>(d_in_planes, in_h, in_w, d_in_info, d_weight_h2, 9, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
                      d_out_f32, d_out_planes, d_out_info, p, cls, 4, in_h, in_w, MODE == kP2Planes, stream);
 }

@@ -1,29 +1,15 @@
-// bevconv_split.cu -- the lab formats of the BEV conv / deconv (include/sessd_b200_lab.h): fp32 NHWC input split inside the wgmma kernel
-// of bevconv_p2.cuh.  TMA stages the fp32 patch in shared memory and the consumer warpgroups split it there:
-//   * sessd_bev_conv_tc / sessd_bev_deconv_tc: 3xTF32 -- x = tf32(x) + (x - tf32(x)), fp32 weights pre-split the same way (ops.pack_weight_tc);
-//     three tf32 wgmma products per MAC (hi hi, hi lo, lo hi) over 16-channel stages;
-//   * sessd_bev_conv_h2 / sessd_bev_deconv_h2: x * 2^s = fp16 hi + fp16 lo with 2^s from the input's abs-max, fp16 weights of
-//     ops.pack_weight_h2; three fp16 wgmma products over 32-channel stages.
+// bevconv_split.cu -- the lab library's builds of the wgmma kernel of bevconv_p2.cuh (include/sessd_b200_lab.h):
+//   * sessd_bev_conv_h2 / sessd_bev_deconv_h2: fp32 NHWC input split inside the kernel -- TMA stages the fp32 patch in shared memory and
+//     the consumer warpgroups split it there into x * 2^s = fp16 hi + fp16 lo (2^s from the input's abs-max); fp16 weights of
+//     ops.pack_weight_h2; three separate fp16 wgmma products per MAC over 32-channel stages.  The product kernel's folded
+//     a_hi x [b_lo ; b_hi] wgmma must sum the same products in the same order: this mode is its bitwise reference;
+//   * the clock-counting and loader-only probes of the product's planes kernel (stall profiles);
+//   * sessd_bev_p2_plan: the launcher's plan, host only (tests compare their restatement of it against this).
 #include "bevconv_p2.cuh"
 
 #include "../../include/sessd_b200_lab.h"
 
 using namespace sessd;
-
-extern "C" int sessd_bev_conv_tc(const float *d_in, const float *d_weight_split, int cout_pad, const float *d_scale, const float *d_shift,
-                                 const float *d_residual, float *d_out, const sessd_conv_desc *desc, void *stream) {
-    if (!d_in || !d_out) return SESSD_EINVAL;
-    return p2_conv<kP2SplitTf32>(d_in, nullptr, d_weight_split, cout_pad, d_scale, d_shift, d_residual, nullptr, 0.f, 0.f, d_out, nullptr, nullptr,
-                                 desc, stream);
-}
-
-extern "C" int sessd_bev_deconv_tc(const float *d_in, const float *d_weight_split, int cout_pad, const float *d_scale, const float *d_shift,
-                                   const float *d_residual, float *d_out, int batch, int in_h, int in_w, int cin, int cout, int relu,
-                                   void *stream) {
-    if (!d_in || !d_out) return SESSD_EINVAL;
-    return p2_deconv<kP2SplitTf32>(d_in, nullptr, d_weight_split, cout_pad, d_scale, d_shift, d_residual, nullptr, 0.f, 0.f, d_out, nullptr,
-                                   nullptr, batch, in_h, in_w, cin, cout, relu, stream);
-}
 
 extern "C" int sessd_bev_conv_h2(const float *d_in, const void *d_weight_h2, int cout_pad, const float *d_scale, const float *d_shift,
                                  const float *d_residual, float *d_out, const sessd_conv_desc *desc, const float *d_amax_in,
@@ -70,4 +56,23 @@ extern "C" int sessd_bev_conv_p2_loads(const void *d_in_planes, const float *d_i
                                        const sessd_conv_desc *desc, const int *d_items, int smem_a, long long *d_prof, void *stream) {
     return p2_conv<kP2Planes, kP2ProbeLoads>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
                                              shift_max, d_out_f32, d_out_planes, d_out_info, desc, stream, d_items, d_prof, smem_a != 0);
+}
+
+// The plan p2_conv / p2_deconv would launch with (p2_plan), word order in sessd_b200_lab.h.  No device call.
+extern "C" int sessd_bev_p2_plan(const sessd_conv_desc *desc, int deconv, int cout_pad, int split, int smem_a, int *plan) {
+    if (!desc || !plan) return SESSD_EINVAL;
+    const sessd_conv_desc &d = *desc;
+    P2Params p;
+    P2Taps cls[4];
+    if (deconv) p2_deconv_params(d.batch, d.in_h, d.in_w, d.cin, d.cout, d.relu, p, cls);
+    else if (p2_conv_params(d, p, cls[0])) return SESSD_EINVAL;
+    const int mode = split ? kP2SplitF16 : kP2Planes;
+    const bool reg_a = mode == kP2Planes && (deconv || (d.in_stride == 1 && !smem_a));
+    int smem = 0;
+    if (p2_plan(p, cls, deconv ? 4 : 1, deconv ? d.in_h : d.grid_h, deconv ? d.in_w : d.grid_w, cout_pad, mode, reg_a, &smem))
+        return SESSD_EINVAL;
+    const int rec[11] = {p.u_is_x, p.n_tile, p.nblocks, p.tiles, p.total, p.ncopies, p.rows_v, p.pitch_u, p.npatch, p.bstages, smem};
+    for (int i = 0; i < 11; ++i) plan[i] = rec[i];
+    for (int c = 0; c < 4; ++c) { plan[11 + c] = p.cls_ntaps[c]; plan[15 + c] = p.cls_order[c]; }      // 0 past the classes
+    return 0;
 }

@@ -116,16 +116,16 @@ SIGNATURES = {
 }
 
 
-# include/sessd_b200_lab.h: non-default BEV conv variants (libsessd_b200_lab.so; loaded on first use, by tests only)
+# include/sessd_b200_lab.h: the in-kernel fp16 split, the probes and the launch plan of the BEV conv (libsessd_b200_lab.so; loaded on first
+# use, by tests and scripts only)
 LAB_SIGNATURES = {
-    "sessd_bev_conv_tc": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp]),
-    "sessd_bev_deconv_tc": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "sessd_bev_conv_h2": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp, _vp]),
     "sessd_bev_deconv_h2": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "sessd_bev_conv_p2_profile": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp, _vp]),
     "sessd_bev_deconv_p2_profile": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp,
                                          _vp]),
     "sessd_bev_conv_p2_loads": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _i, _vp, _vp]),
+    "sessd_bev_p2_plan": (_i, [C.POINTER(ConvDesc), _i, _i, _i, _i, _I3]),
 }
 
 

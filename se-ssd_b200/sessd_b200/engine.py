@@ -17,7 +17,7 @@ from .runners import SpMiddleRunner, SSFAPlanesRunner, SSFARunner
 
 class FrameEngine:
     def __init__(self, batch=1, max_points_per_frame=32768, voxel_size=synth.VOXEL_SIZE, pc_range=synth.PC_RANGE,
-                 max_points_per_voxel=5, max_voxels=20000, device="cuda", post_kwargs=None, growth=None, use_tc=True, neck="planes",
+                 max_points_per_voxel=5, max_voxels=20000, device="cuda", post_kwargs=None, growth=None, use_tc=True,
                  skip_constant=True):
         """use_tc: tensor-core kernels in the sparse encoder (runners.SpMiddleRunner) and the neck; False = their fp32 SIMT baselines.
         skip_constant: the planes neck computes only the tiles whose receptive field reaches a LiDAR site or the map border and fills
@@ -34,11 +34,11 @@ class FrameEngine:
         self.d_off = torch.zeros((self.batch + 1,), dtype=torch.int32, device=dev)
         self.vox = ops.VoxelBuffers(self.vcfg, self.batch, self.max_points, dev, with_mean=True)
         self.middle = SpMiddleRunner(self.batch, self.batch * max_voxels, self.grid_xyz, 4, dev, growth=growth, use_tc=use_tc)
-        self.neck_planes = neck == "planes" and use_tc
+        self.neck_planes = bool(use_tc)
         if self.neck_planes:
             self.neck = SSFAPlanesRunner(self.batch, (self.grid_xyz[1] // 8, self.grid_xyz[0] // 8), dev, skip_constant=skip_constant)
         else:
-            self.neck = SSFARunner(self.batch, (self.grid_xyz[1] // 8, self.grid_xyz[0] // 8), dev, use_tc=use_tc)
+            self.neck = SSFARunner(self.batch, (self.grid_xyz[1] // 8, self.grid_xyz[0] // 8), dev, use_tc=False)
         self.anchors = None
         pk = dict(batch=self.batch, head_stride=SSFARunner.HEAD_STRIDE)
         pk.update(post_kwargs or {})

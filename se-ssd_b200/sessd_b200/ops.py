@@ -336,36 +336,6 @@ def bev_conv(x, weight, scale, shift, residual, out, desc):
     return out
 
 
-def split_tf32(w):
-    """w -> (hi, lo): hi = w truncated to tf32 (13 low mantissa bits cleared), lo = w - hi (exact in fp32)."""
-    hi = (w.contiguous().view(torch.int32) & -8192).view(torch.float32)
-    return hi, w - hi
-
-
-def pack_weight_tc(wp, cout_pad):
-    """[taps, Cin, Cout] (SIMT packing) -> [2, taps, cout_pad, Cin] K-major hi/lo planes for sessd_bev_conv_tc."""
-    taps, cin, cout = wp.shape
-    wt = torch.zeros((taps, cout_pad, cin), dtype=torch.float32, device=wp.device)
-    wt[:, :cout] = wp.permute(0, 2, 1)
-    hi, lo = split_tf32(wt)
-    return torch.stack([hi, lo], 0).contiguous()
-
-
-def bev_conv_tc(x, weight_split, scale, shift, residual, out, desc):
-    check(lib.sessd_bev_conv_tc(_p(x), _p(weight_split), int(weight_split.shape[2]), _p(scale), _p(shift), _p(residual), _p(out),
-                                C.byref(desc), _st()), "sessd_bev_conv_tc")
-    return out
-
-
-def bev_deconv_tc(x, weight_split, scale, shift, residual, out, relu=True):
-    """ConvTranspose2d(k3,s2,p1,op1)+BN+ReLU(+residual): x [B,H,W,Cin] -> out [B,2H,2W,Cout]; weight_split from
-    pack_weight_tc(W.permute(2,3,0,1).reshape(9,Cin,Cout), cout_pad)."""
-    b, h, w, cin = x.shape
-    check(lib.sessd_bev_deconv_tc(_p(x), _p(weight_split), int(weight_split.shape[2]), _p(scale), _p(shift), _p(residual), _p(out),
-                                  int(b), int(h), int(w), int(cin), int(out.shape[-1]), int(bool(relu)), _st()), "sessd_bev_deconv_tc")
-    return out
-
-
 def pack_weight_h2(wp, cout_pad):
     """[taps, Cin, Cout] (SIMT packing) -> (planes fp16 [2, taps, cout_pad, Cin], exps [cout_pad] fp32 = 2^-e[n]) for sessd_bev_conv_p2 / _h2:
     the fp16 split of _fp16_split over the zero-padded weight.  The returned 2^-e[n] must be folded into the epilogue scale."""
@@ -383,7 +353,8 @@ def bev_conv_h2(x, weight_h2, scale, shift, residual, out, desc, amax_in=None, a
 
 
 def bev_deconv_h2(x, weight_h2, scale, shift, residual, out, relu=True, amax_in=None, amax_out=None):
-    """fp16-split twin of bev_deconv_tc; weight_h2 from pack_weight_h2(W.permute(2,3,0,1).reshape(9,Cin,Cout), cout_pad)."""
+    """ConvTranspose2d(k3,s2,p1,op1)+BN+ReLU(+residual) with the fp16 split in the kernel: x [B,H,W,Cin] -> out [B,2H,2W,Cout];
+    weight_h2 from pack_weight_h2(W.permute(2,3,0,1).reshape(9,Cin,Cout), cout_pad)."""
     b, h, w, cin = x.shape
     check(lib.sessd_bev_deconv_h2(_p(x), _p(weight_h2), int(weight_h2.shape[2]), _p(scale), _p(shift), _p(residual), _p(out),
                                   int(b), int(h), int(w), int(cin), int(out.shape[-1]), int(bool(relu)), _p(amax_in), _p(amax_out), _st()),

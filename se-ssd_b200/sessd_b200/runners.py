@@ -330,21 +330,16 @@ class HeadRunner:
 
 
 class SSFARunner:
-    """SSFA neck (rpn_v1.py:220-235) + the fused 128->22(+2 pad) head GEMM (mg_head_sessd.py:202-230) from fp32 activations: the lab
-    formats of bev_conv_p2_kernel, or the fp32 SIMT baseline."""
+    """SSFA neck (rpn_v1.py:220-235) + the fused 128->22(+2 pad) head GEMM (mg_head_sessd.py:202-230) from fp32 activations, on the
+    fp32 SIMT baseline kernels, or (use_tc) with the stride-1 launches on the lab's h2 mode of bev_conv_p2_kernel (the fp32 input split
+    into fp16 planes inside the kernel, bevconv_split.cu) and the stride-2 conv on the SIMT kernel: a stride-2 3x3 patch and its fp32
+    staging copy leave the h2 mode no room for the weight ring at 128 output channels per tile."""
 
     HEAD_STRIDE = 24
 
-    TC_STRIDE2 = True     # run the stride-2 conv through the strided-TMA tensor-core path as well
-
-    def __init__(self, batch, hw=(200, 176), device="cuda", use_tc=True, split="fp16"):
-        """use_tc: tensor-core convs (default); False = the fp32 SIMT baseline kernels.
-        split: "fp16" = two-term fp16 split of the fp32 input inside the kernel (bev_conv_p2_kernel<.., kP2SplitF16>, bevconv_split.cu;
-               the stride-2 conv stays on the tf32 mode), "tf32" = 3xTF32 everywhere (kP2SplitTf32, bevconv_split.cu)."""
+    def __init__(self, batch, hw=(200, 176), device="cuda", use_tc=True):
         self.batch, self.h, self.w, self.device = batch, int(hw[0]), int(hw[1]), torch.device(device)
         self.use_tc = bool(use_tc)
-        assert split in ("fp16", "tf32")
-        self.use_h2 = self.use_tc and split == "fp16"
         self.amax = torch.zeros(16, dtype=torch.float32, device=self.device)     # abs-max scalars (fp16 split scaling), SSFA_SLOT numbering
         z = lambda hw_, c: torch.zeros((batch,) + hw_ + (c,), dtype=torch.float32, device=self.device)  # noqa: E731
         self.buf = {L.dst: z(ssfa_extents(L, self.h, self.w)[1], L.cout) for L in SSFA_LAUNCHES}
@@ -359,10 +354,8 @@ class SSFARunner:
                 P[L.name] = (wp, taps, sc, sh)
             else:       # SIMT: four parity-class convs; tensor cores: one launch over the 9-tap packing
                 P[L.name] = (_deconv_classes(wp.reshape(3, 3, L.cin, L.cout).permute(2, 3, 0, 1)), sc, sh)
-            if self.use_h2 and L.stride == 1:
+            if self.use_tc and L.stride == 1:
                 P[L.name + ":h2"] = pack_h2(wp, sc, sh, _cout_pad(L.cout))
-            elif self.use_tc and (self.TC_STRIDE2 or L.stride == 1):
-                P[L.name + ":tc"] = ops.pack_weight_tc(wp, _cout_pad(L.cout))
         self.params = P
 
     def _am(self, name):
@@ -373,28 +366,24 @@ class SSFARunner:
         the abs-max of the output (fp16-split scaling)"""
         in_hw, out_hw = ssfa_extents(L, self.h, self.w)
         resid = self.buf[L.residual] if L.residual else None
-        h2, tc = self.params.get(L.name + ":h2"), self.params.get(L.name + ":tc")
+        h2 = self.params.get(L.name + ":h2")
         if L.kind == "conv":
             wp, taps, sc, sh = self.params[L.name]
             d = ops.conv_desc(self.batch, in_hw, L.cin, out_hw, L.cout, out_hw, taps, in_stride=L.stride, relu=L.relu)
             if h2 is not None:
                 ops.bev_conv_h2(x, h2["w"], h2["scale"], h2["shift"], resid, out, d, self._am(ai or L.src), self._am(ao))
-            elif tc is not None:
-                ops.bev_conv_tc(x, tc, sc, sh, resid, out, d)
             else:
                 ops.bev_conv(x, wp, sc, sh, resid, out, d)
         else:
             classes, sc, sh = self.params[L.name]
             if h2 is not None:
                 ops.bev_deconv_h2(x, h2["w"], h2["scale"], h2["shift"], resid, out, L.relu, self._am(ai or L.src), self._am(ao))
-            elif tc is not None:
-                ops.bev_deconv_tc(x, tc, sc, sh, resid, out, relu=L.relu)
             else:
                 for py, px, wp, taps in classes:
                     d = ops.conv_desc(self.batch, in_hw, L.cin, out_hw, L.cout, in_hw, taps, in_stride=1, out_stride=2, out_off=(py, px),
                                       relu=L.relu)
                     ops.bev_conv(x, wp, sc, sh, resid, out, d)
-        if h2 is None and self.use_h2 and ao is not None:
+        if h2 is None and self.use_tc and ao is not None:
             ops.absmax(out, self._am(ao))
         return out
 
@@ -404,7 +393,7 @@ class SSFARunner:
         assert self.params is not None, "load_state first"
         mark = mark or (lambda label: None)
         b = self.buf
-        if self.use_h2:
+        if self.use_tc:
             self.amax.zero_()
             ops.absmax(x, self._am("x"))
         for L in SSFA_LAUNCHES[:-1]:
@@ -413,7 +402,7 @@ class SSFARunner:
         w0, s0, t0 = self.params["w_0.0"]
         w1, s1, t1 = self.params["w_1.0"]
         ops.ssfa_fuse(b["o0"], b["o1"], w0, w1, s0, t0, s1, t1, b["out"])
-        if self.use_h2 and "head" in self.params:
+        if self.use_tc and "head" in self.params:
             ops.absmax(b["out"], self._am("out"))
         if "head" not in self.params:
             mark("neck:fuse+head")
@@ -431,8 +420,6 @@ class SSFARunner:
 
         if (name + ":h2") in self.params:
             kern = "bev_conv_p2_kernel<.., kP2SplitF16> (fp32 input split to fp16 in shared memory, fp16 wgmma)"
-        elif (name + ":tc") in self.params:
-            kern = "bev_conv_p2_kernel<.., kP2SplitTf32> (3xTF32, tf32 wgmma)"
         else:
             kern = "bev_conv_kernel (fp32 SIMT)"
         return launch, kern

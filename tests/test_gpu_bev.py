@@ -14,14 +14,14 @@ def _rel(a, b):
     return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-30))
 
 
-MODES = ["simt", "tf32x3", "fp16x2", "planes"]   # fp32 SIMT baseline | 3xTF32 weights | fp16 split of fp32 inputs | pre-split planes (default)
+MODES = ["simt", "fp16x2", "planes"]   # fp32 SIMT baseline | fp16 split of fp32 inputs | pre-split planes (default)
 
 
 def _runner(batch, hw, mode):
     from sessd_b200.runners import SSFAPlanesRunner, SSFARunner
     if mode == "planes":
         return SSFAPlanesRunner(batch, hw, "cuda")
-    return SSFARunner(batch, hw, "cuda", use_tc=mode != "simt", split="tf32" if mode == "tf32x3" else "fp16")
+    return SSFARunner(batch, hw, "cuda", use_tc=mode != "simt")
 
 
 def _act(r, name):
@@ -107,9 +107,7 @@ def test_single_conv_vs_fp64(mode, cin, cout, k, hw):
     out = torch.zeros((b, hw[0], hw[1], cout), device="cuda")
     d = ops.conv_desc(b, hw, cin, hw, cout, hw, taps, relu=True)
     cout_pad = 32 if cout <= 32 else -(-cout // 128) * 128
-    if mode == "tf32x3":
-        ops.bev_conv_tc(xd, ops.pack_weight_tc(wp.cuda(), cout_pad), sc.cuda(), sh.cuda(), rd, out, d)
-    elif mode == "planes":
+    if mode == "planes":
         planes, inv = ops.pack_weight_h2(wp.cuda(), cout_pad)
         xp, info = _to_planes(xd)
         rinfo = torch.zeros(2, device="cuda")
@@ -135,14 +133,6 @@ def test_single_conv_vs_fp64(mode, cin, cout, k, hw):
     got = out.permute(0, 3, 1, 2).cpu().double()
     err = float((got - ref).abs().max() / ref.abs().max())
     assert err < 5e-6, err
-
-
-def test_tf32_split_is_exact():
-    from sessd_b200 import ops
-    w = torch.randn(4096, generator=torch.Generator().manual_seed(1))
-    hi, lo = ops.split_tf32(w)
-    assert torch.equal(hi + lo, w)
-    assert int((hi.view(torch.int32) & 8191).abs().max()) == 0
 
 
 def test_fp16_split_range_and_precision():
@@ -202,7 +192,7 @@ def test_planes_conv_full_shapes_vs_fp64(k, stride, hw):
     assert err < 5e-6, err
 
 
-@pytest.mark.parametrize("split", ["tf32", "fp16", "planes"])
+@pytest.mark.parametrize("split", ["fp16", "planes"])
 @pytest.mark.parametrize("hw", [(13, 17), (100, 88)])
 def test_deconv_single_launch_vs_fp64(hw, split):
     """ConvTranspose2d(k3,s2,p1,op1)+BN+ReLU+residual as one 4-class tensor-core launch."""
@@ -220,9 +210,7 @@ def test_deconv_single_launch_vs_fp64(hw, split):
     w9 = w.permute(2, 3, 0, 1).reshape(9, cin, cout).contiguous().cuda()
     out = torch.zeros((b, 2 * hw[0], 2 * hw[1], cout), device="cuda")
     xd, rd = x.permute(0, 2, 3, 1).contiguous().cuda(), res.permute(0, 2, 3, 1).contiguous().cuda()
-    if split == "tf32":
-        ops.bev_deconv_tc(xd, ops.pack_weight_tc(w9, 128), sc.cuda(), sh.cuda(), rd, out)
-    elif split == "planes":
+    if split == "planes":
         planes, inv = ops.pack_weight_h2(w9, 128)
         xp, info = _to_planes(xd)
         rinfo = torch.zeros(2, device="cuda")

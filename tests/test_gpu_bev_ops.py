@@ -27,13 +27,6 @@ planes outputs [2][B][H][W][C] at S_out = pow2_scale_for_bound(bound), bound = a
   checked at 2^-22 bound.  |o| <= bound gives |o S_out| < 2^15, so |hi| <= 2^15: the fp16 rounding of a value within 8 of 2^15 IS
   2^15 (the spacing there is 16), so |hi| < 2^15 does not follow; 2^15 is far below fp16's 65504 and (hi, lo) stays exact.
 bev_conv_h2 / bev_deconv_h2 (lab): the same bounds, with the input split inside the kernel at pow2_scale_for_bound(amax_in).
-bev_conv_tc / bev_deconv_tc (lab, 3xTF32): x_hi = x truncated to tf32, x_lo = rna_tf32(x - x_hi); the weights' hi planes truncated,
-  their lo planes rna_tf32(w - w_hi) (rounded in shared memory by the kernel).  Products of tf32 operands are exact in fp32.  Per 16-channel
-  chunk and tap the main accumulator takes two k=8 steps and the cross one four, and the main partial is folded into an fp32 total per
-  chunk (one rounding each): G = P Cin / 4 + Cin / 16 steps, and
-    |got - emul| <= c 2^-23 (G + 2) |bn| magA + 2^-23 |sh| (+ 2^-23 (|relu(emul)| + |r|))
-  vs fp64: |x - x_hi| < 2^-10 |x| and the lo rounding loses <= 2^-11 of that, for x and w alike; the dropped x_lo w_lo is <= 2^-20 |x||w|:
-  <= 2^-19 |x| |w| per product, checked with a 2x margin: + 2^-18 |bn| sum |x| |w|.
 
 Plane producers: bev_split_planes, sparse_to_dense_planes and the planes of ssfa_fuse_planes are a power-of-two scaling and two fp16
 roundings: restated bit for bit in numpy.  absmax is exact.  ssfa_fuse_planes' fp32 output vs fp64, per pixel with C channels:
@@ -43,11 +36,13 @@ roundings: restated bit for bit in numpy.  absmax is exact.  ssfa_fuse_planes' f
   relative, and the rounded l_0 - max adds <= u |l_0 - l_1| a_0 <= 0.3 u: |da| <= (|dl_0| + |dl_1|) / 4 + 16 u.  The output
   x_0 a_0 + x_1 a_1 adds two roundings: |dout| <= (|x_0| + |x_1|) (|da| + 2 u).
 
-Launch schedule (bev_conv_p2.cuh, restated in p2_plan / ring_starts): total = nclass nblocks tiles work items, classes ordered by
-descending tap count, on min(total, SMs) persistent CTAs; an item takes nchunks ntaps steps of the weight ring.  nchunks is even
-(Cin is a multiple of 64, chunks are 32 channels; 16 in tf32, where nchunks is a multiple of 4), so items start only at even stages
-(stage 0 of a 4-stage tf32 ring); the sweep is checked to start items at every such stage with both phases for the 6-, 12- and 4-stage
-rings, and to run both one and two patch buffers.
+Launch schedule (bev_conv_p2.cuh, restated in p2_plan / ring_starts and checked against the launcher's own plan, sessd_bev_p2_plan):
+total = nclass nblocks tiles work items, classes ordered by descending tap count, on min(total, SMs) persistent CTAs; an item takes
+nchunks ntaps steps of the weight ring.  nchunks is even (Cin is a multiple of 64, chunks are 32 channels), so an item starts after an
+even number s of steps of its CTA, at (stage, phase) = (s mod B, (s div B) mod 2) of a B-stage ring: B of the 2 B positions (even
+stages with both phases for even B, every stage with the phase of its parity for odd B).  The planes launches of the sweep build the
+11- (3x3 convs and deconvs), 12- (1x1 and n_tile 32) and 7-stage (stride-2 convs) rings and are checked to start items at every one
+of those positions, and to run both one and two patch buffers.
 
 Each tolerance is shown to catch a subtly wrong kernel on the CPU (negative controls).  Smallest ratio of error to bound over the control
 cases (vs the emulation bound / vs the fp64 bound): cross products dropped 10 / 4.5, one tap read from the neighbouring tile at a tile
@@ -55,10 +50,9 @@ edge 1.2e4 / 6.3e3, previous item's accumulator carried into one tile 4.8e4 / 1.
 3.9e6 / 4.3e4, two taps' weights swapped 2.1e4 / 9.9e3; lo output plane dropped vs the planes bound 16; the residual's share left out
 of the output scale: max |hi| / 2^15 = 1.3.
 Largest ratios measured on one H100 80GB HBM3 (400 W power limit): p2 vs emulation 0.50, p2 vs fp64 0.50, p2 planes 0.38; h2 vs
-emulation 0.46, vs fp64 0.44; tf32 vs emulation 0.39, vs fp64 0.38; ssfa_fuse vs fp64 0.08.
+emulation 0.46, vs fp64 0.44; ssfa_fuse vs fp64 0.08.
 """
 import ctypes as C
-import math
 
 import numpy as np
 import pytest
@@ -78,7 +72,7 @@ TILE_U, TILE_V = 8, 16
 MAX_COPIES, MAX_ROWS_V = 6, 18
 BSTAGES, MAX_BSTAGES = 6, 12
 MAX_SMEM = 227 * 1024
-BRING = BSTAGES * 2 * 128 * 64
+CHUNK = 32
 TAPS3 = [(dy, dx) for dy in (-1, 0, 1) for dx in (-1, 0, 1)]
 TAPS1 = [(0, 0)]
 
@@ -104,8 +98,9 @@ def deconv_classes():
     return out
 
 
-def p2_plan(mode, cin, cout, cout_pad, classes, stride, grid_h, grid_w, batch):
-    """launch_p2's geometry for a mode ("p2", "h2", "tc"): None where the launcher refuses the launch"""
+def p2_plan(mode, cin, cout, cout_pad, classes, stride, grid_h, grid_w, batch, smem_a=False):
+    """p2_plan of bevconv_p2.cuh for a mode ("p2": planes, "h2": fp16 split in the kernel): None where the launcher refuses the launch.
+    Stride-1 planes launches read A from registers out of one patch copy (smem_a: the loads probe's descriptor plan instead)."""
     if cin < 64 or cin % 64 or cout < 8 or cout % 8:
         return None
     n_tile = 32 if cout <= 32 else 128
@@ -125,23 +120,27 @@ def p2_plan(mode, cin, cout, cout_pad, classes, stride, grid_h, grid_w, batch):
     rows_v = max(TILE_V + (hi - lo) // stride for lo, hi in keys.values())
     if rows_v > MAX_ROWS_V:
         return None
-    chunk = 16 if mode == "tc" else 32
-    ncopies = len(keys)
-    patch = ncopies * 2 * rows_v * TILE_U * 64
-    staging = 0 if mode == "p2" else ncopies * rows_v * TILE_U * chunk * 4
-    per_buf, bstage = patch + staging, 2 * n_tile * 64
-    bring = BRING
-    npatch = 2 if BRING + 1536 + 2 * per_buf <= MAX_SMEM else 1
-    if BRING + 1536 + per_buf > MAX_SMEM:
-        bring = (MAX_SMEM - 1536 - per_buf) // bstage * bstage
-    if bring < 2 * bstage:
+    ncopies, pitch_u = len(keys), TILE_U
+    if mode == "p2" and stride == 1 and not smem_a:       # one copy: from the taps' least shift, wide and tall enough for their greatest
+        us, vs = [u for u, _ in keys], [v for lohi in keys.values() for v in lohi]
+        ncopies, pitch_u, rows_v = 1, TILE_U + max(us) - min(us), TILE_V + max(vs) - min(vs)
+        if pitch_u > 256 or rows_v > 256:
+            return None
+    per_buf = ncopies * 2 * cdiv(rows_v * pitch_u * 64, 512) * 512                  # fp16 (hi, lo) copies in whole 512-byte periods
+    if mode == "h2":
+        per_buf += ncopies * rows_v * TILE_U * CHUNK * 4                              # fp32 staging
+    bstage, tail = 2 * n_tile * 64, 1536 + 16 + 2 * 4 * cout                          # barriers, tap offsets, BN scale and shift
+    npatch = 2 if BSTAGES * bstage + tail + 2 * per_buf <= MAX_SMEM else 1
+    bstages = min((MAX_SMEM - tail - npatch * per_buf) // bstage, MAX_BSTAGES)
+    if bstages < 2:
         return None
     grid_u, grid_v = (grid_w, grid_h) if u_is_x else (grid_h, grid_w)
     tiles = cdiv(grid_u, TILE_U) * cdiv(grid_v, TILE_V) * batch
     ntaps = [len(c) for c in classes]
-    return dict(u_is_x=u_is_x, ncopies=ncopies, rows_v=rows_v, npatch=npatch, bstages=min(bring // bstage, MAX_BSTAGES),
-                nchunks=cin // chunk, nblocks=cout_pad // n_tile, tiles=tiles, total=len(classes) * (cout_pad // n_tile) * tiles,
-                ntaps=ntaps, order=sorted(range(len(classes)), key=lambda c: -ntaps[c]))
+    return dict(u_is_x=u_is_x, n_tile=n_tile, nblocks=cout_pad // n_tile, tiles=tiles, total=len(classes) * (cout_pad // n_tile) * tiles,
+                ncopies=ncopies, rows_v=rows_v, pitch_u=pitch_u, npatch=npatch, bstages=bstages,
+                smem=bstages * bstage + tail + npatch * per_buf, ntaps=ntaps, order=sorted(range(len(classes)), key=lambda c: -ntaps[c]),
+                nchunks=cin // CHUNK)
 
 
 def ring_starts(plan, num_sms=NUM_SMS):
@@ -159,10 +158,9 @@ def ring_starts(plan, num_sms=NUM_SMS):
     return seen
 
 
-def reachable_starts(bstages, mode):
-    """every item is a multiple of nchunks steps: even (fp16 chunks), a multiple of 4 (tf32 chunks)"""
-    step = math.gcd(bstages, 4 if mode == "tc" else 2)
-    return {(s, p) for s in range(0, bstages, step) for p in (0, 1)}
+def reachable_starts(bstages):
+    """every item is a multiple of nchunks steps, an even number: an item starts after s steps of its CTA, s even, s mod 2 bstages"""
+    return {(s % bstages, s // bstages) for s in range(0, 2 * bstages, 2)}
 
 
 # ------------------------------------------------------------------------------------------------------------------ crafted maps
@@ -317,48 +315,30 @@ def output_scale(amax, gain, shift_max, amax_r=None):
     return s, float(fused)
 
 
-def tf32_trunc(v):
-    return (np.asarray(v, np.float32).view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
-
-
-def tf32_rna(v):
-    """cvt.rna.tf32.f32: nearest tf32, ties away from zero (finite inputs)"""
-    return ((np.asarray(v, np.float32).view(np.uint32) + np.uint32(0x1000)) & np.uint32(0xFFFFE000)).view(np.float32)
-
-
 class Emu:
-    """What a BEV kernel multiplies for a BevCase, in fp64 on `dev`, plus the tolerances of the module docstring.  mode "p2" / "h2":
-    fp16 planes (a_planes: the device's input planes, else the restated split); "tc": 3xTF32."""
+    """What a BEV kernel multiplies for a BevCase (fp16 planes: a_planes = the device's input planes, else the restated split), in fp64
+    on `dev`, plus the tolerances of the module docstring."""
 
-    def __init__(self, case, dev, mode="p2", a_planes=None):
+    def __init__(self, case, dev, a_planes=None):
         from sessd_b200 import ops
-        self.case, self.dev, self.mode = case, dev, mode
+        self.case, self.dev = case, dev
         d64 = lambda a: torch.as_tensor(np.asarray(a, np.float64), device=dev)       # noqa: E731
         self.amax_in = float(np.abs(case.x).max())
         wp = torch.from_numpy(case.w)
-        if mode == "tc":
-            self.s_in = 1.0
-            hi = tf32_trunc(case.x)
-            a_hi, a_lo = hi, tf32_rna(case.x - hi)
-            wt = ops.pack_weight_tc(wp, case.cout_pad).numpy()[:, :, :case.cout].transpose(0, 1, 3, 2)   # [2][T][Cin][Cout]
-            b_hi, b_lo = wt[0], tf32_rna(wt[1])
-            self.wsplit = ops.pack_weight_tc(wp, case.cout_pad)
-            self.sc = case.bn.astype(np.float64)
-        else:
-            self.s_in = pow2_scale_for_bound(self.amax_in)
-            a_hi, a_lo = split16(case.x, self.s_in) if a_planes is None else a_planes
-            planes, inv = ops.pack_weight_h2(wp, case.cout_pad)
-            self.w_h2, self.inv = planes, inv
-            t = planes.numpy()[:, :, :case.cout].transpose(0, 1, 3, 2)                                # [2][T][Cin][Cout]
-            b_hi, b_lo = t[0], t[1]
-            self.sc32 = (torch.from_numpy(case.bn) * inv[:case.cout]).numpy()
-            self.sc = self.sc32.astype(np.float64)
+        self.s_in = pow2_scale_for_bound(self.amax_in)
+        a_hi, a_lo = split16(case.x, self.s_in) if a_planes is None else a_planes
+        planes, inv = ops.pack_weight_h2(wp, case.cout_pad)
+        self.w_h2, self.inv = planes, inv
+        t = planes.numpy()[:, :, :case.cout].transpose(0, 1, 3, 2)                                # [2][T][Cin][Cout]
+        b_hi, b_lo = t[0], t[1]
+        self.sc32 = (torch.from_numpy(case.bn) * inv[:case.cout]).numpy()
+        self.sc = self.sc32.astype(np.float64)
         self.A_hi, self.A_lo, self.B_hi, self.B_lo = d64(a_hi), d64(a_lo), d64(b_hi), d64(b_lo)
         self.acc0 = self.acc()
         mag = tap_conv(case, self.A_hi.abs(), self.B_hi.abs() + self.B_lo.abs()) + tap_conv(case, self.A_lo.abs(), self.B_hi.abs())
         ones = torch.ones((case.batch,) + case.in_hw + (1,), dtype=torch.float64, device=dev)
         self.P = tap_conv(case, ones, torch.ones((self.B_hi.shape[0], 1, 1), dtype=torch.float64, device=dev))
-        g = 2 * self.P * case.cin / 16 if mode != "tc" else self.P * case.cin / 4 + case.cin / 16
+        g = 2 * self.P * case.cin / 16
         sc, shv = d64(self.sc), d64(case.shv)
         self.magA = mag
         self.emul0 = self.emul()
@@ -368,13 +348,9 @@ class Emu:
             self.tol_e = self.tol_e + 2.0 ** -23 * ((self.emul0 - r).abs() + r.abs())
         x64, w64 = d64(case.x), d64(case.w)
         aw = w64.abs()
-        if mode == "tc":
-            split = tap_conv(case, x64.abs(), aw)
-            self.tol_64 = self.tol_e + 2.0 ** -18 * d64(case.bn).abs() * split
-        else:
-            split = (self.amax_in * tap_conv(case, ones, aw.sum(1, keepdim=True))
-                     + tap_conv(case, x64.abs().sum(3, keepdim=True), torch.ones_like(aw[:, :1, :1])) * aw.amax(dim=(0, 1)))
-            self.tol_64 = self.tol_e + 2.0 ** -20 * d64(case.bn).abs() * split
+        split = (self.amax_in * tap_conv(case, ones, aw.sum(1, keepdim=True))
+                 + tap_conv(case, x64.abs().sum(3, keepdim=True), torch.ones_like(aw[:, :1, :1])) * aw.amax(dim=(0, 1)))
+        self.tol_64 = self.tol_e + 2.0 ** -20 * d64(case.bn).abs() * split
         self.ref = self.finish(tap_conv(case, x64, w64), d64(case.bn), 1.0)
 
     @property
@@ -530,7 +506,10 @@ def _p2_specs():
          dict(kind="deconv", pattern="zero", batch=1, in_hw=(8, 16), cin=192, cout=24, resid=True),
          dict(kind="deconv", pattern="dense", batch=1, in_hw=(17, 40), cin=128, cout=136, resid=True),
          dict(kind="deconv", pattern="dense", batch=1, in_hw=(100, 88), cin=256, cout=128, resid=True),
-         dict(kind="deconv", pattern="sparse", batch=2, in_hw=(1, 15), cin=64, cout=8, relu=False)]
+         dict(kind="deconv", pattern="sparse", batch=2, in_hw=(1, 15), cin=64, cout=8, relu=False),
+         # ring coverage (module docstring): 3 items per CTA of 4 steps on the 11-stage ring, 7 items of 18 steps on the 7-stage ring
+         dict(kind="conv", pattern="dense", batch=4, in_hw=(96, 96), cin=64, cout=128, taps=[(0, 0), (0, 1)], resid=True),
+         dict(kind="conv", pattern="dense", batch=4, in_hw=(160, 160), cin=64, cout=256, cout_pad=512, stride=2)]
     for i, d in enumerate(s):
         d.setdefault("seed", 500 + i)
         d.setdefault("shift", i % 3 != 2)
@@ -544,29 +523,45 @@ def _case(spec, **kw):
 
 
 def _lab_specs():
-    """(mode, spec) subset for the lab formats; each mode includes its shrunk-ring / single-patch-buffer configurations"""
+    """(mode, spec) subset for the lab's h2 mode, incl. its shrunk-ring / single-patch-buffer configurations"""
     sp = _p2_specs()
-    return [("h2", sp[1]), ("h2", sp[3]), ("h2", dict(sp[13], cout=32)), ("h2", sp[18]), ("h2", sp[21]),
-            ("tc", sp[0]), ("tc", sp[11]), ("tc", dict(sp[12], batch=2, in_hw=(200, 176), cout=128)), ("tc", sp[16]), ("tc", sp[19])]
+    return [("h2", sp[1]), ("h2", sp[3]), ("h2", dict(sp[13], cout=32)), ("h2", sp[18]), ("h2", sp[21])]
+
+
+P2_RINGS = (7, 11, 12)          # the weight rings the planes launches build: stride-2 3x3 convs, 3x3 convs and deconvs, the rest
+
+
+def _sweep_plans():
+    """(mode, kind, stride, plan) of every launch of the sweep and the lab subset"""
+    out = []
+    for mode, s in [("p2", s) for s in _p2_specs()] + _lab_specs():
+        c = _case(s)
+        out.append((mode, c.kind, c.stride, c.plan(mode)))
+        assert out[-1][3] is not None, c.label()
+    return out
+
+
+def _ring_coverage(plans, num_sms):
+    """{bstages: (stage, phase) starts} of the planes launches among plans; asserts that every launch starts only at reachable positions"""
+    seen = {}
+    for mode, _, _, p in plans:
+        starts = ring_starts(p, num_sms)
+        assert starts <= reachable_starts(p["bstages"]), (mode, p)
+        if mode == "p2":
+            seen.setdefault(p["bstages"], set()).update(starts)
+    assert sorted(seen) == list(P2_RINGS)
+    return seen
 
 
 def test_schedule_reaches_every_ring_position_and_both_patch_paths():
-    """The sweep's launches (restated launcher arithmetic) start work items at every reachable weight-ring stage with both phases, for
-    the 6-stage ring (n_tile 128), the 12-stage ring (n_tile 32) and the shrunk 4-stage tf32 ring; they run one and two patch buffers
-    and both tile orientations of conv, stride-2 conv and deconv."""
-    seen, npatch, orient = {}, set(), set()
-    runs = [("p2", _case(s)) for s in _p2_specs()] + [(m, _case(s)) for m, s in _lab_specs()]
-    for mode, c in runs:
-        p = c.plan(mode)
-        assert p is not None, c.label()
-        starts = ring_starts(p)
-        assert starts <= reachable_starts(p["bstages"], mode), (c.label(), p["bstages"])
-        seen.setdefault((p["bstages"], mode == "tc"), set()).update(starts)
-        npatch.add(p["npatch"])
-        orient.add((c.kind, c.stride, p["u_is_x"]))
-    for bstages, tc in ((6, False), (12, False), (4, True)):
-        assert seen.get((bstages, tc), set()) == reachable_starts(bstages, "tc" if tc else "p2"), (bstages, sorted(seen.get((bstages, tc), ())))
-    assert npatch == {1, 2}
+    """The sweep's planes launches (restated launcher arithmetic) start work items at every reachable position of each weight ring they
+    build (7, 11 and 12 stages); the sweep runs one and two patch buffers and both tile orientations of conv, stride-2 conv and deconv."""
+    plans = _sweep_plans()
+    seen = _ring_coverage(plans, NUM_SMS)
+    for bstages in P2_RINGS:
+        assert seen[bstages] == reachable_starts(bstages), (bstages, sorted(reachable_starts(bstages) - seen[bstages]))
+    assert {p["npatch"] for _, _, _, p in plans} == {1, 2}
+    orient = {(kind, stride, p["u_is_x"]) for _, kind, stride, p in plans}
     assert {(k, s, u) for k in ("conv",) for s in (1, 2) for u in (0, 1)} | {("deconv", 1, 0), ("deconv", 1, 1)} <= orient
 
 
@@ -582,7 +577,8 @@ def test_launcher_limits_restated():
     -- while n_tile 32 (4 KB stages) still fits five."""
     cls = lambda taps: [[(dy, dx, t) for t, (dy, dx) in enumerate(taps)]]      # noqa: E731
     assert p2_plan("p2", 64, 64, 128, cls([(0, dx) for dx in range(-3, 4)]), 1, 16, 16, 1) is None                  # 7 copies
-    assert p2_plan("p2", 64, 64, 128, cls([(0, dx) for dx in range(-3, 3)]), 1, 16, 16, 1)["ncopies"] == 6
+    assert p2_plan("p2", 64, 64, 128, cls([(0, dx) for dx in range(-3, 3)]), 1, 16, 16, 1, smem_a=True)["ncopies"] == 6
+    assert p2_plan("p2", 64, 64, 128, cls([(0, dx) for dx in range(-3, 3)]), 1, 16, 16, 1)["ncopies"] == 1
     assert p2_plan("p2", 64, 64, 128, cls([(dy, 0) for dy in (-2, 0, 1)]), 1, 16, 16, 1) is None                    # 19 rows
     assert p2_plan("p2", 64, 64, 128, cls([(dy, 0) for dy in (-1, 0, 1)]), 1, 16, 16, 1)["rows_v"] == 18
     assert p2_plan("p2", 96, 64, 128, cls(TAPS3), 1, 16, 16, 1) is None
@@ -590,10 +586,49 @@ def test_launcher_limits_restated():
     assert p2_plan("h2", 128, 128, 128, cls(TAPS3), 2, 16, 16, 1) is None
     p = p2_plan("h2", 128, 32, 32, cls(TAPS3), 2, 16, 16, 1)
     assert (p["npatch"], p["bstages"], p["ncopies"], p["rows_v"]) == (1, 5, 6, 17)
-    p = p2_plan("tc", 128, 128, 128, cls(TAPS3), 2, 16, 16, 1)
-    assert (p["npatch"], p["bstages"]) == (1, 4)
     assert p2_plan("p2", 128, 128, 128, cls(TAPS3), 2, 16, 16, 1)["npatch"] == 1
     assert p2_plan("p2", 128, 128, 128, cls(TAPS3), 1, 16, 16, 1)["npatch"] == 2
+
+
+PLAN_WORDS = ("u_is_x", "n_tile", "nblocks", "tiles", "total", "ncopies", "rows_v", "pitch_u", "npatch", "bstages", "smem")
+
+
+def launcher_plan(case, mode, smem_a=False):
+    """the launcher's own plan of a case (sessd_bev_p2_plan: lab library, no device call) in p2_plan's terms, or None where it refuses"""
+    from sessd_b200 import _lib, ops
+    d = case.desc() if case.kind == "conv" else ops.conv_desc(case.batch, case.in_hw, case.cin, case.out_hw, case.cout, case.grid, [])
+    rec = (C.c_int * 19)()
+    if _lib.lib.sessd_bev_p2_plan(C.byref(d), int(case.kind == "deconv"), case.cout_pad, int(mode == "h2"), int(smem_a), rec) != 0:
+        return None
+    n = len(case.classes)
+    assert list(rec[11 + n:15]) == [0] * (4 - n) and list(rec[15 + n:]) == [0] * (4 - n)
+    return dict(zip(PLAN_WORDS, rec[:11]), ntaps=list(rec[11:11 + n]), order=list(rec[15:15 + n]))
+
+
+def test_plan_restatement_matches_the_launcher():
+    """p2_plan field by field against the launcher's plan for every sweep and lab launch (the sweep's stride-1 convs also as the loads
+    probe's descriptor plan), and for the refusals of test_launcher_limits_restated and the launches next to them"""
+    sweep = [_case(s) for s in _p2_specs()]
+    runs = [("p2", c, False) for c in sweep] + [(m, _case(s), False) for m, s in _lab_specs()]
+    runs += [("p2", c, True) for c in sweep if c.kind == "conv" and c.stride == 1]
+    for mode, cin, cout, cout_pad, taps, stride in (("p2", 64, 64, 128, [(0, dx) for dx in range(-3, 4)], 1),       # 7 copies
+                                                    ("p2", 64, 64, 128, [(0, dx) for dx in range(-3, 3)], 1),
+                                                    ("p2", 64, 64, 128, [(-2, 0), (0, 0), (1, 0)], 1),              # 19 rows
+                                                    ("p2", 64, 64, 128, [(-1, 0), (0, 0), (1, 0)], 1),
+                                                    ("p2", 96, 64, 128, TAPS3, 1), ("p2", 64, 44, 128, TAPS3, 1),
+                                                    ("h2", 128, 128, 128, TAPS3, 2), ("h2", 128, 32, 32, TAPS3, 2),
+                                                    ("p2", 128, 128, 128, TAPS3, 2), ("p2", 128, 128, 128, TAPS3, 1)):
+        runs.append((mode, BevCase("conv", "zero", 1, (16 * stride, 16 * stride), cin, cout, 0, taps=taps, stride=stride, cout_pad=cout_pad),
+                     False))
+    refused = 0
+    for mode, c, smem_a in runs:
+        want = p2_plan(mode, c.cin, c.cout, c.cout_pad, c.classes, c.stride, c.grid[0], c.grid[1], c.batch, smem_a)
+        got = launcher_plan(c, mode, smem_a)
+        refused += got is None
+        if want is not None:
+            want = {k: want[k] for k in PLAN_WORDS + ("ntaps", "order")}
+        assert got == want, (mode, c.label(), smem_a)
+    assert refused == 5
 
 
 def test_crafted_maps_have_their_shape():
@@ -612,9 +647,6 @@ def test_crafted_maps_have_their_shape():
 def test_split_restatements():
     for b, want in ((1.0, 2.0 ** 14), (2.0 ** 14, 1.0), (0.0, 1.0), (np.inf, 1.0), (2.0 ** -126, 2.0 ** 125), (1e-40, 1.0), (1e30, 2.0 ** -85)):
         assert pow2_scale_for_bound(b) == want, b
-    v = np.float32([1.0, 1.0 + 2.0 ** -10, -(1.0 + 3 * 2.0 ** -12), 3 * 2.0 ** -20, 1.0 + 2.0 ** -11])     # tf32 ulp at 1: 2^-10
-    assert np.array_equal(tf32_trunc(v), np.float32([1.0, 1.0 + 2.0 ** -10, -1.0, 3 * 2.0 ** -20, 1.0]))
-    assert np.array_equal(tf32_rna(v), np.float32([1.0, 1.0 + 2.0 ** -10, -(1.0 + 2.0 ** -10), 3 * 2.0 ** -20, 1.0 + 2.0 ** -10]))
 
 
 def _control_cases():
@@ -628,11 +660,10 @@ def _control_cases():
 
 def test_split_bounds_hold_for_the_exact_emulation():
     """Positive controls of the derivations: the fp64 emulation (a kernel without accumulation error) is within the split's own error of
-    fp64 for the planes and tf32 splits, and the fp16 (hi, lo) epilogue restated in numpy meets the planes bound."""
+    fp64 for the planes split, and the fp16 (hi, lo) epilogue restated in numpy meets the planes bound."""
     for case in _control_cases():
-        for mode in ("p2", "tc"):
-            emu = Emu(case, "cpu", mode)
-            assert ratio(emu.emul0, emu.ref, emu.tol_64 - emu.tol_e) <= 0.5, (case.label(), mode)
+        emu = Emu(case, "cpu")
+        assert ratio(emu.emul0, emu.ref, emu.tol_64 - emu.tol_e) <= 0.5, case.label()
         o = emu.emul0.numpy().astype(np.float32)
         s, bound = output_scale(emu.amax_in, case.gain, case.shift_max, case.amax_r if case.r is not None else None)
         hi, lo = split16(o, s)
@@ -748,7 +779,7 @@ def _check_p2(case, worst):
     a_hi, a_lo = planes_in[0].cpu().numpy(), planes_in[1].cpu().numpy()
     rh, rl = split16(case.x, s_in)
     assert float(info_in[1]) == s_in and np.array_equal(a_hi.view(np.int16), rh.view(np.int16)) and np.array_equal(a_lo.view(np.int16), rl.view(np.int16))
-    emu = Emu(case, "cuda", "p2", (a_hi, a_lo))
+    emu = Emu(case, "cuda", (a_hi, a_lo))
     gain, shift_max = case.gain, case.shift_max
     w, sc = emu.w_h2.cuda(), _dev(emu.sc32)
     sh = None if case.sh is None else _dev(case.sh)
@@ -800,13 +831,10 @@ def test_p2_kernels_match_emulation_and_fp64(spec):
 @gpu
 def test_p2_sweep_schedule_on_this_device():
     """the ring-position coverage of the CPU schedule test, recomputed with this device's SM count (the launcher's grid size)"""
-    props = torch.cuda.get_device_properties(0)
-    seen = {}
-    for mode, c in [("p2", _case(s)) for s in _P2] + [(m, _case(s)) for m, s in _lab_specs()]:
-        p = c.plan(mode)
-        seen.setdefault((p["bstages"], mode == "tc"), set()).update(ring_starts(p, props.multi_processor_count))
-    for bstages, tc in ((6, False), (12, False), (4, True)):
-        assert seen[(bstages, tc)] == reachable_starts(bstages, "tc" if tc else "p2"), (props.multi_processor_count, bstages)
+    num_sms = torch.cuda.get_device_properties(0).multi_processor_count
+    seen = _ring_coverage(_sweep_plans(), num_sms)
+    for bstages in P2_RINGS:
+        assert seen[bstages] == reachable_starts(bstages), (num_sms, bstages, sorted(reachable_starts(bstages) - seen[bstages]))
 
 
 @gpu
@@ -939,13 +967,13 @@ _LAB = _lab_specs()
 @gpu
 @pytest.mark.parametrize("mode,spec", _LAB, ids=["%s-%s" % (m, _case(s).label()) for m, s in _LAB])
 def test_lab_modes_match_emulation_and_fp64(mode, spec):
-    """bev_conv_h2 / _deconv_h2 (fp16 split in the kernel) and bev_conv_tc / _deconv_tc (3xTF32) on a subset of the sweep, incl. the
-    single-patch-buffer and shrunk-ring configurations: fp32 within the bounds of their split, exact on empty receptive fields, run to
-    run bitwise, the h2 running abs-max exact, guards and unowned pixels untouched"""
+    """bev_conv_h2 / _deconv_h2 (fp16 split in the kernel) on a subset of the sweep, incl. the single-patch-buffer and shrunk-ring
+    configurations: fp32 within the bounds of the split, exact on empty receptive fields, run to run bitwise, the running abs-max exact,
+    guards and unowned pixels untouched"""
     from sessd_b200 import ops
     case = _case(spec)
     assert case.plan(mode) is not None
-    emu = Emu(case, "cuda", mode)
+    emu = Emu(case, "cuda")
     xd = _dev(case.x)
     sh = None if case.sh is None else _dev(case.sh)
     rd = None if case.r is None else _dev(case.r)
@@ -954,27 +982,19 @@ def test_lab_modes_match_emulation_and_fp64(mode, spec):
     for _ in range(2):
         buf, out = _guarded(oshape, torch.float32)
         amax_out = torch.zeros(1, device="cuda")
-        if mode == "h2":
-            amax_in = torch.tensor([emu.amax_in], device="cuda")
-            w, sc = emu.w_h2.cuda(), _dev(emu.sc32)
-            if case.kind == "conv":
-                ops.bev_conv_h2(xd, w, sc, sh, rd, out, case.desc(), amax_in, amax_out)
-            else:
-                ops.bev_deconv_h2(xd, w, sc, sh, rd, out, case.relu, amax_in, amax_out)
+        amax_in = torch.tensor([emu.amax_in], device="cuda")
+        w, sc = emu.w_h2.cuda(), _dev(emu.sc32)
+        if case.kind == "conv":
+            ops.bev_conv_h2(xd, w, sc, sh, rd, out, case.desc(), amax_in, amax_out)
         else:
-            w = emu.wsplit.cuda()
-            if case.kind == "conv":
-                ops.bev_conv_tc(xd, w, _dev(case.bn), sh, rd, out, case.desc())
-            else:
-                ops.bev_deconv_tc(xd, w, _dev(case.bn), sh, rd, out, case.relu)
+            ops.bev_deconv_h2(xd, w, sc, sh, rd, out, case.relu, amax_in, amax_out)
         outs.append((buf, out, amax_out))
     torch.cuda.synchronize()
     assert torch.equal(_bits(outs[0][1]), _bits(outs[1][1]))
     got = _on_grid(outs[0][1], case)
     worst = {}
     _check_common(case, emu, [(b, o) for b, o, _ in outs], got, worst)
-    if mode == "h2":
-        assert float(outs[0][2][0]) == float(got.abs().max())
+    assert float(outs[0][2][0]) == float(got.abs().max())
     _report(worst, "%s %s" % (mode, case.label()))
 
 
