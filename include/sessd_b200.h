@@ -430,6 +430,60 @@ int sessd_adamw_clip_ema_step(float *d_param, float *d_grad, float *d_exp_avg, f
                               float beta2, float eps, float weight_decay, int step, const float *d_clip_coef, float *d_ema, double ema_alpha,
                               void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * KITTI object evaluation (csrc/kitti_eval.cu): det3d/datasets/kitti/kitti.py convert_detection_to_kitti_annos and
+ * det3d/datasets/kitti/eval.py eval_class_v3 on flat arrays.  The precision of every step is written down in the kernel file.
+ *
+ * A box record is SESSD_KITTI_REC doubles: bbox x0 y0 x1 y1, alpha, location x y z, dimensions (l h w), rotation_y, then the score
+ * (detections) or the truncation (ground truth).  Class codes: the index into the evaluation's class list (car 0, pedestrian 1,
+ * bicycle 2, truck 3, bus 4, trailer 5, construction_vehicle 6, motorcycle 7, barrier 8, traffic_cone 9, cyclist 10) of the
+ * lower-cased name, SESSD_KITTI_PERSON_SITTING, SESSD_KITTI_VAN (the neighbour classes of pedestrian and car), -1 for any other
+ * name.  DontCare boxes (names "DontCare" / "ignore") are passed once more, as 2D boxes, in their own CSR list.
+ *
+ * sessd_kitti_convert_detections -- one thread per lidar detection (x y z w l h ry, fp32): camera record, image box, alpha; boxes
+ *     outside the image are dropped and the rest kept in input order, frame f's kept records at d_rec[d_off[f] ...] (the input's
+ *     slots) and their count in d_cnt[f].  d_calib [F, 24] fp64: rows 0-2 of R0_rect . Tr_velo_to_cam, rows 0-2 of P2;
+ *     d_image_hw [F, 2] (height, width).  d_code[j] = d_label_code[label] (-1 for labels outside [0, num_labels)).  capacity =
+ *     d_off[F].  workspace: sessd_kitti_convert_workspace_bytes(capacity).
+ * sessd_kitti_overlaps -- the block-diagonal overlap of one metric (0 2D, 1 BEV, 2 3D): frame f's [dt_cnt[f], n_gt_f] block, row
+ *     stride n_gt_f, at d_overlaps + ov_off[f].  z_axis / z_center: (1, 1.0) for KITTI camera boxes, (2, 0.5) for lidar boxes.
+ * sessd_kitti_eval -- overlaps, both matching passes, get_thresholds and the curves of one metric for num_configs configs d_cfg
+ *     [n, 2] = (class code, difficulty 0-2) with d_min_overlap [n].  Outputs per config: d_thresholds / d_precision / d_aos [n, 41]
+ *     (zero past d_num_thresholds[c]), d_map [n, 4] = R11 precision, R40 precision, R11 AOS, R40 AOS (get_mAP / get_mAP_v2, in
+ *     percent).  A config with no valid ground truth has no thresholds and AP 0.  max_frame_dt: the largest dt_off[f+1] - dt_off[f]
+ *     (SESSD_ECAPACITY above 1024).  total_gt = gt_off[F]; overlap_elems = ov_off[F].  Bitwise deterministic run to run.  The
+ *     workspace holds the overlaps, 2 x num_configs x total_gt fp64 scores and, with compute_aos, one fp64 similarity per (config,
+ *     threshold, frame) for the frame-ordered sum: num_configs x 41 x F doubles (133 MB for 108 configs over 3769 frames).
+ * ------------------------------------------------------------------------------------------------ */
+#define SESSD_KITTI_REC 13
+#define SESSD_KITTI_PERSON_SITTING 11
+#define SESSD_KITTI_VAN 12
+typedef struct {
+    int num_frames;
+    const int *gt_off;        /* [F+1] CSR of ground-truth boxes */
+    const double *gt;         /* [n_gt, SESSD_KITTI_REC] */
+    const int *gt_code;       /* [n_gt] */
+    const int *gt_occluded;   /* [n_gt] */
+    const int *dc_off;        /* [F+1] CSR of DontCare boxes */
+    const double *dc;         /* [n_dc, 4] (may be NULL when there are none) */
+    const int *dt_off;        /* [F+1] CSR capacity of detections */
+    const int *dt_cnt;        /* [F] detections held by frame f (<= its capacity) */
+    const double *dt;         /* [dt_off[F], SESSD_KITTI_REC] */
+    const int *dt_code;       /* [dt_off[F]] */
+    const long long *ov_off;  /* [F+1] start of frame f's overlap block; block f holds at least dt_cnt[f] * n_gt_f values */
+} SessdKittiFrames;
+size_t sessd_kitti_convert_workspace_bytes(long long capacity);
+int sessd_kitti_convert_detections(const float *d_boxes7, const float *d_scores, const int *d_labels, const int *d_off, int num_frames,
+                                   long long capacity, const double *d_calib, const int *d_image_hw, const int *d_label_code,
+                                   int num_labels, double *d_rec, int *d_label, int *d_code, int *d_cnt, void *workspace,
+                                   size_t workspace_bytes, void *stream);
+int sessd_kitti_overlaps(const SessdKittiFrames *frames, int metric, int z_axis, double z_center, double *d_overlaps, void *stream);
+size_t sessd_kitti_eval_workspace_bytes(int num_frames, long long total_gt, long long overlap_elems, int num_configs, int compute_aos);
+int sessd_kitti_eval(const SessdKittiFrames *frames, int max_frame_dt, int metric, int z_axis, double z_center, int num_configs,
+                     const int *d_cfg, const double *d_min_overlap, int compute_aos, long long total_gt, long long overlap_elems,
+                     double *d_thresholds, int *d_num_thresholds, double *d_precision, double *d_aos, double *d_map, void *workspace,
+                     size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

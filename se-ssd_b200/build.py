@@ -20,7 +20,7 @@ LAB = {"bevconv_split.cu"}
 OBJ = os.path.join(HERE, "build")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"] + os.environ.get("SESSD_DEFINES", "").split()
-NO_FMA = {"iou3d.cu", "postproc.cu", "assign.cu", "odiou.cu"}
+NO_FMA = {"iou3d.cu", "postproc.cu", "assign.cu", "odiou.cu", "kitti_eval.cu"}
 
 
 def sources():

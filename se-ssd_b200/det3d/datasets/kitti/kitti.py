@@ -1,0 +1,103 @@
+"""KittiDataset mirror: the evaluation side of det3d/datasets/kitti/kitti.py (ground truth, detection -> KITTI camera annotations,
+`evaluation`), running on the device.  Loading frames (`__getitem__` / `get_sensor_data`) needs the reference's pipeline, which
+this mirror does not carry."""
+import pickle
+
+from sessd_b200 import kitti_eval as ke
+
+from ..registry import DATASETS
+from .eval import _has_alpha, evaluate_all
+
+
+@DATASETS.register_module
+class KittiDataset:
+    NumPointFeatures = 4
+
+    def __init__(self, root_path, info_path, cfg=None, pipeline=None, class_names=None, test_mode=False, **kwargs):
+        assert info_path is not None
+        self._root_path = root_path
+        self._info_path = info_path
+        self.pipeline = pipeline
+        self.test_mode = test_mode
+        with open(info_path, "rb") as f:
+            self._kitti_infos = pickle.load(f)
+        self._num_point_features = KittiDataset.NumPointFeatures
+        self._class_names = class_names
+        self.labeled = kwargs.get("labeled", True)
+        self.plane_dir = root_path + "/training/planes"
+        self._device_gt = None       # packed ground truth; it does not change between epochs
+        self._device_calib = None
+
+    def __len__(self):
+        return len(self._kitti_infos)
+
+    @property
+    def num_point_features(self):
+        return self._num_point_features
+
+    @property
+    def ground_truth_annotations(self):
+        if "annos" not in self._kitti_infos[0]:
+            return None
+        return [info["annos"] for info in self._kitti_infos]
+
+    def _gt(self):
+        if self._device_gt is None:
+            self._device_gt = ke.DeviceGT(self.ground_truth_annotations)
+        return self._device_gt
+
+    def _frames_of(self, detection, partial):
+        gt_idx = [str(info["image"]["image_idx"]) for info in self._kitti_infos]
+        keys = list(detection.keys()) if partial else gt_idx
+        if partial:
+            calib = ke.DeviceCalib([self._kitti_infos[gt_idx.index(k)] for k in keys])
+        else:
+            if self._device_calib is None:
+                self._device_calib = ke.DeviceCalib(self._kitti_infos)
+            calib = self._device_calib
+        dets = [(detection[k]["box3d_lidar"], detection[k]["scores"], detection[k]["label_preds"]) for k in keys]
+        dt, labels = ke.convert_detections(dets, calib, self._class_names)
+        return keys, dt, labels
+
+    def _annos(self, detection, keys, dt, labels):
+        annos = ke.dt_annos_from_device(dt, labels, self._class_names)
+        for a, k in zip(annos, keys):
+            a["metadata"] = detection[k]["metadata"]
+        return annos
+
+    def convert_detection_to_kitti_annos(self, detection, partial=False):
+        """detection: {image_idx string: {"box3d_lidar", "scores", "label_preds", "metadata"}}, tensors on any device.  Boxes whose
+        image box lies outside the image are dropped, the rest clipped to it."""
+        keys, dt, labels = self._frames_of(detection, partial)
+        return self._annos(detection, keys, dt, labels)
+
+    def evaluation(self, detections, output_dir=None, get_results=True):
+        """KITTI camera boxes: z_axis 1, z_center 1.0.  Returns (results, dt_annos); nothing is copied to the host before the
+        kernels have run, then one copy brings the curves back and one builds dt_annos."""
+        keys, dt, labels = self._frames_of(detections, False)
+        results = None
+        if get_results:
+            frames = ke.Frames(self._gt(), dt)
+            official, official_2, coco = evaluate_all(frames, self._class_names, True, z_axis=1, z_center=1.0)
+        dt_annos = self._annos(detections, keys, dt, labels)
+        if get_results:
+            if not _has_alpha(dt_annos):
+                official, official_2, coco = (_drop_aos(r) for r in (official, official_2, coco))
+            results = {"results": {"official_AP_11": official["result"]},
+                       "results_2": {"official_AP_40": official_2["result"]},
+                       "detail": {"eval.kitti": {"official": official["detail"], "coco": coco["detail"]}}}
+        return results, dt_annos
+
+    def __getitem__(self, idx):
+        raise NotImplementedError("KittiDataset mirror: loading frames needs the reference's data pipeline, which is not part of "
+                                  "this package; it provides ground truth and evaluation only")
+
+    def get_sensor_data(self, idx, with_image=False, with_gp=False, by_index=False):
+        raise NotImplementedError("KittiDataset mirror: loading frames needs the reference's data pipeline, which is not part of "
+                                  "this package; it provides ground truth and evaluation only")
+
+
+def _drop_aos(r):
+    lines = [ln for ln in r["result"].split("\n") if not ln.startswith("aos  AP:")]
+    detail = {c: {k: v for k, v in d.items() if k != "aos"} for c, d in r["detail"].items()}
+    return {"result": "\n".join(lines), "detail": detail}

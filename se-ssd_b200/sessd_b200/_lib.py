@@ -39,6 +39,12 @@ class PostCfg(C.Structure):
                 ("direction_offset", C.c_float), ("use_frustum", C.c_int)]
 
 
+class KittiFrames(C.Structure):
+    _fields_ = [("num_frames", C.c_int), ("gt_off", C.c_void_p), ("gt", C.c_void_p), ("gt_code", C.c_void_p),
+                ("gt_occluded", C.c_void_p), ("dc_off", C.c_void_p), ("dc", C.c_void_p), ("dt_off", C.c_void_p),
+                ("dt_cnt", C.c_void_p), ("dt", C.c_void_p), ("dt_code", C.c_void_p), ("ov_off", C.c_void_p)]
+
+
 _vp, _i, _f, _sz, _ll = C.c_void_p, C.c_int, C.c_float, C.c_size_t, C.c_longlong
 _I3 = C.POINTER(C.c_int)
 
@@ -113,6 +119,12 @@ SIGNATURES = {
     "sessd_adamw_clip_ema_step": (_i, [_vp, _vp, _vp, _vp, _ll, _f, _f, _f, _f, _f, _i, _vp, _vp, C.c_double, _vp]),
     "sessd_assign_workspace_bytes": (_sz, [_i, _i, _i]),
     "sessd_assign_targets": (_i, [_vp, _i, _vp, _vp, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "sessd_kitti_convert_workspace_bytes": (_sz, [_ll]),
+    "sessd_kitti_convert_detections": (_i, [_vp, _vp, _vp, _vp, _i, _ll, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "sessd_kitti_overlaps": (_i, [C.POINTER(KittiFrames), _i, _i, C.c_double, _vp, _vp]),
+    "sessd_kitti_eval_workspace_bytes": (_sz, [_i, _ll, _ll, _i, _i]),
+    "sessd_kitti_eval": (_i, [C.POINTER(KittiFrames), _i, _i, _i, C.c_double, _i, _vp, _vp, _i, _ll, _ll, _vp, _vp, _vp, _vp, _vp, _vp,
+                              _sz, _vp]),
 }
 
 
