@@ -194,12 +194,12 @@ int sessd_spconv_wgrad_cg(const void *d_in_planes, int cp, const float *d_in_inf
 /* ------------------------------------------------------------------------------------------------
  * N1/H1: BEV neck (SSFA) + head.  Replaces the cuDNN conv/deconv + BatchNorm2d + ReLU blocks of
  * det3d/models/necks/rpn_v1.py:135-235 and the four 1x1 convs of
- * det3d/models/bbox_heads/mg_head_sessd.py:202-230.  Activations are NHWC fp32.
- * One call = one tap-list convolution:  out[b, oy*os+py, ox*os+px, :] =
+ * det3d/models/bbox_heads/mg_head_sessd.py:202-230.  Tensors are NHWC.
+ * ------------------------------------------------------------------------------------------------ */
+/* One tap-list convolution:  out[b, oy*os+py, ox*os+px, :] =
  *    epilogue( sum_t in[b, oy*is + dy[t], ox*is + dx[t], :] @ W[t] )   (zero outside the input)
  * with epilogue y = acc*scale + shift (nullable), optional ReLU, optional residual add AFTER the ReLU
- * (rpn_v1.py:225: deconv_block_0(x_trans_1) + x_trans_0).
- * ------------------------------------------------------------------------------------------------ */
+ * (rpn_v1.py:225: deconv_block_0(x_trans_1) + x_trans_0). */
 typedef struct {
     int batch, in_h, in_w, cin;       /* input tensor  [batch, in_h, in_w, cin]  */
     int out_h, out_w, cout;           /* output tensor [batch, out_h, out_w, cout] */
@@ -211,15 +211,11 @@ typedef struct {
     int relu;
 } sessd_conv_desc;
 
-int sessd_bev_conv(const float *d_in, const float *d_weight /*[ntaps, cin, cout]*/, const float *d_scale,
-                   const float *d_shift, const float *d_residual /*nullable, same shape as out*/, float *d_out,
-                   const sessd_conv_desc *desc, void *stream);
-
 /* ------------------------------------------------------------------------------------------------
  * BEV convs from PRE-SPLIT fp16 planes (csrc/bevconv_p2.cu): the neck's default path.  Activations travel between layers as
  * __half [2 (hi|lo)][batch][H][W][C] planes with x = (hi + lo) / S, S an exact power of two; every plane tensor has a device-side
- * info pair float[2] = {abs-max of the tensor (atomically raised by its producer; zero it once per frame), S}.  Same conv semantics
- * as sessd_bev_conv (rpn_v1.py:135-210, mg_head_sessd.py:202-230): in_stride 1 or 2, <= 9 taps, cin % 64 == 0,
+ * info pair float[2] = {abs-max of the tensor (atomically raised by its producer; zero it once per frame), S}.  sessd_bev_conv_p2
+ * runs the tap-list conv of sessd_conv_desc (rpn_v1.py:135-210, mg_head_sessd.py:202-230): in_stride 1 or 2, <= 9 taps, cin % 64 == 0,
  * cout % 8 == 0.  d_weight_h2: __half [2 (hi|lo)][ntaps][cout_pad][cin] of 2^e[n] w
  * (ops.pack_weight_h2); d_scale = folded BN scale * 2^-e[n].  gain / shift_max: |out| <= amax_in * gain + shift_max
  * (+ amax of the residual) with gain = max_n sum_{tap,c} |w[tap][c][n] * bn_scale[n]|: the producer derives the OUTPUT scale from
@@ -262,19 +258,15 @@ int sessd_bev_split_planes(const float *d_x, long long n, float *d_info, void *d
 /* dense() (scn.py:184-187) straight into the planes the neck reads: d_amax = abs-max of the feature rows, d_info[2] <- {abs-max, S} */
 int sessd_sparse_to_dense_planes(const float *d_feat, int max_rows, const void *d_bitmap_index, int channels, sessd_grid grid,
                                  const float *d_amax, float *d_info, void *d_planes, void *stream);
-/* sessd_ssfa_fuse that also (d_out nullable: only) writes the fused map as planes; d_info0 / d_info1 [2]: abs-max of x0 / x1 */
+/* SSFA tail (rpn_v1.py:229-233): w_k = BN(conv1x1_{128->1}(x_k)) with d_w0 / d_w1 [C] and (s_k, t_k) the folded BN; softmax over the
+ * pair; weighted sum of x0 and x1.  Writes the fused map as planes (d_planes + d_out_info) and, when d_out is set, as fp32;
+ * d_info0 / d_info1 [2]: abs-max of x0 / x1 */
 int sessd_ssfa_fuse_planes(const float *d_x0, const float *d_x1, const float *d_w0, const float *d_w1, float s0, float t0, float s1,
                            float t1, int num_pixels, int channels, float *d_out, const float *d_info0, const float *d_info1,
                            float *d_out_info, void *d_planes, void *stream);
 
 /* *d_amax = max(*d_amax, max_i |d_x[i]|)  (for tensors produced by kernels without an abs-max epilogue) */
 int sessd_absmax(const float *d_x, long long n, float *d_amax, void *stream);
-
-
-/* SSFA tail (rpn_v1.py:229-233): w_k = BN(conv1x1_{128->1}(x_k)); softmax over the pair; weighted sum */
-int sessd_ssfa_fuse(const float *d_x0, const float *d_x1, const float *d_w0 /*[C]*/, const float *d_w1,
-                    float s0, float t0, float s1, float t1, int num_pixels, int channels, float *d_out,
-                    void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * P1/P2/P3: decode -> sigmoid -> threshold -> IoU-rectified score -> top-k -> rotated NMS -> direction fix ->

@@ -1,7 +1,7 @@
 // bevgrad.cu -- weight gradient of the BEV neck and head convs (training of SSFA, det3d/models/necks/rpn_v1.py:135-210, and of the
 // head's 1x1 convs, det3d/models/bbox_heads/mg_head_sessd.py:202-215).
 //
-// Tap-list form of the forward (sessd_bev_conv): out[b, y, x] = sum_t in[b, y s + dy_t, x s + dx_t] @ W[t]   (zero outside the input)
+// Tap-list form of the forward (sessd_conv_desc): out[b, y, x] = sum_t in[b, y s + dy_t, x s + dx_t] @ W[t]   (zero outside the input)
 //   wgrad  gW[t][ci][co] = sum_{b, y, x} in[b, y s + dy_t, x s + dx_t, ci] g[b, y, x, co]   -- here;
 //   dgrad  is the forward kernels (bevconv_p2.cu) with re-packed weights, no kernel of its own (sessd_b200/bev_grad.py).
 // The deconv (k3, s2, p1, op1) has no mode of its own: its weight gradient is the stride-2 conv's with the roles swapped (input = the

@@ -80,7 +80,6 @@ SIGNATURES = {
     "sessd_spconv_wgrad_cg": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
     "sessd_sparse_to_dense_indexed": (_i, [_vp, _i, _vp, _i, Grid, _vp, _vp]),
     "sessd_sparse_to_dense": (_i, [_vp, _vp, _vp, _i, _i, Grid, _vp, _vp]),
-    "sessd_bev_conv": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp]),
     "sessd_bev_conv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp]),
     "sessd_bev_deconv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "sessd_bev_skip_plan_words": (_ll, [_i, _i, _i, _I3]),
@@ -93,7 +92,6 @@ SIGNATURES = {
     "sessd_sparse_to_dense_planes": (_i, [_vp, _i, _vp, _i, Grid, _vp, _vp, _vp, _vp]),
     "sessd_ssfa_fuse_planes": (_i, [_vp, _vp, _vp, _vp, _f, _f, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "sessd_absmax": (_i, [_vp, C.c_longlong, _vp, _vp]),
-    "sessd_ssfa_fuse": (_i, [_vp, _vp, _vp, _vp, _f, _f, _f, _f, _i, _i, _vp, _vp]),
     "sessd_postprocess_workspace_bytes": (_sz, [C.POINTER(PostCfg)]),
     "sessd_postprocess": (_i, [_vp, _vp, _vp, C.POINTER(PostCfg), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "sessd_postprocess_packed": (_i, [_vp, _vp, _vp, C.POINTER(PostCfg), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),

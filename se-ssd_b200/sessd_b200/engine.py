@@ -12,16 +12,14 @@ import numpy as np
 import torch
 
 from . import ops, synth
-from .runners import SpMiddleRunner, SSFAPlanesRunner, SSFARunner
+from .runners import SpMiddleRunner, SSFAPlanesRunner
 
 
 class FrameEngine:
     def __init__(self, batch=1, max_points_per_frame=32768, voxel_size=synth.VOXEL_SIZE, pc_range=synth.PC_RANGE,
-                 max_points_per_voxel=5, max_voxels=20000, device="cuda", post_kwargs=None, growth=None, use_tc=True,
-                 skip_constant=True):
-        """use_tc: tensor-core kernels in the sparse encoder (runners.SpMiddleRunner) and the neck; False = their fp32 SIMT baselines.
-        skip_constant: the planes neck computes only the tiles whose receptive field reaches a LiDAR site or the map border and fills
-        the rest with their bit-identical empty-space constant (runners.SSFAPlanesRunner)"""
+                 max_points_per_voxel=5, max_voxels=20000, device="cuda", post_kwargs=None, growth=None, skip_constant=True):
+        """skip_constant: the neck computes only the tiles whose receptive field reaches a LiDAR site or the map border and fills the
+        rest with their bit-identical empty-space constant (runners.SSFAPlanesRunner)"""
         self.batch, self.device = int(batch), torch.device(device)
         self.max_points = int(max_points_per_frame) * self.batch
         self.vcfg = ops.make_voxel_cfg(voxel_size, pc_range, max_points_per_voxel, max_voxels)
@@ -33,14 +31,10 @@ class FrameEngine:
         self.d_points = torch.zeros((self.max_points, 4), dtype=torch.float32, device=dev)
         self.d_off = torch.zeros((self.batch + 1,), dtype=torch.int32, device=dev)
         self.vox = ops.VoxelBuffers(self.vcfg, self.batch, self.max_points, dev, with_mean=True)
-        self.middle = SpMiddleRunner(self.batch, self.batch * max_voxels, self.grid_xyz, 4, dev, growth=growth, use_tc=use_tc)
-        self.neck_planes = bool(use_tc)
-        if self.neck_planes:
-            self.neck = SSFAPlanesRunner(self.batch, (self.grid_xyz[1] // 8, self.grid_xyz[0] // 8), dev, skip_constant=skip_constant)
-        else:
-            self.neck = SSFARunner(self.batch, (self.grid_xyz[1] // 8, self.grid_xyz[0] // 8), dev, use_tc=False)
+        self.middle = SpMiddleRunner(self.batch, self.batch * max_voxels, self.grid_xyz, 4, dev, growth=growth)
+        self.neck = SSFAPlanesRunner(self.batch, (self.grid_xyz[1] // 8, self.grid_xyz[0] // 8), dev, skip_constant=skip_constant)
         self.anchors = None
-        pk = dict(batch=self.batch, head_stride=SSFARunner.HEAD_STRIDE)
+        pk = dict(batch=self.batch, head_stride=SSFAPlanesRunner.HEAD_STRIDE)
         pk.update(post_kwargs or {})
         self.pcfg = ops.make_post_cfg(**pk)
         self.post = ops.PostBuffers(self.pcfg, dev)
@@ -74,16 +68,12 @@ class FrameEngine:
 
     def sparse_and_neck(self, mark=None):
         """sparse encoder + dense() + neck + head on the current stream; returns the head map.  mark(label) is called after every
-        launch group (profiling)."""
+        launch group (profiling).  dense() writes the fp16 (hi, lo) planes of the neck input directly."""
         n0 = self.vox.num_voxels[self.batch:self.batch + 1]
-        if self.neck_planes:       # dense() writes the fp16 (hi, lo) planes of the neck input directly
-            self.neck.info.zero_()
-            self.middle.forward(self.vox.mean, self.vox.coors, n0, mark=mark, dense_planes=(self.neck.planes["x"], self.neck.info[0]))
-            last = self.middle.levels[-1]
-            _, head = self.neck.forward(None, mark=mark, occupancy=(last["index"], last["grid"]))
-        else:
-            dense = self.middle.forward(self.vox.mean, self.vox.coors, n0, mark=mark)
-            _, head = self.neck.forward(dense, mark=mark)
+        self.neck.info.zero_()
+        self.middle.forward(self.vox.mean, self.vox.coors, n0, mark=mark, dense_planes=(self.neck.planes["x"], self.neck.info[0]))
+        last = self.middle.levels[-1]
+        _, head = self.neck.forward(None, mark=mark, occupancy=(last["index"], last["grid"]))
         return head
 
     def _step_body(self):

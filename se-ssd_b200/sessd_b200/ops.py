@@ -331,13 +331,8 @@ def conv_desc(batch, in_hw, cin, out_hw, cout, grid_hw, taps, in_stride=1, out_s
     return d
 
 
-def bev_conv(x, weight, scale, shift, residual, out, desc):
-    check(lib.sessd_bev_conv(_p(x), _p(weight), _p(scale), _p(shift), _p(residual), _p(out), C.byref(desc), _st()), "sessd_bev_conv")
-    return out
-
-
 def pack_weight_h2(wp, cout_pad):
-    """[taps, Cin, Cout] (SIMT packing) -> (planes fp16 [2, taps, cout_pad, Cin], exps [cout_pad] fp32 = 2^-e[n]) for sessd_bev_conv_p2 / _h2:
+    """[taps, Cin, Cout] (tap-list packing) -> (planes fp16 [2, taps, cout_pad, Cin], exps [cout_pad] fp32 = 2^-e[n]) for sessd_bev_conv_p2 / _h2:
     the fp16 split of _fp16_split over the zero-padded weight.  The returned 2^-e[n] must be folded into the epilogue scale."""
     taps, cin, cout = wp.shape
     wt = torch.zeros((taps, cout_pad, cin), dtype=torch.float32, device=wp.device)
@@ -464,13 +459,6 @@ def absmax(x, amax):
     """amax[0] = max(amax[0], max|x|) on the current stream."""
     check(lib.sessd_absmax(_p(x), int(x.numel()), _p(amax), _st()), "sessd_absmax")
     return amax
-
-
-def ssfa_fuse(x0, x1, w0, w1, s0, t0, s1, t1, out):
-    npix = x0.numel() // x0.shape[-1]
-    check(lib.sessd_ssfa_fuse(_p(x0), _p(x1), _p(w0), _p(w1), float(s0), float(t0), float(s1), float(t1), int(npix), int(x0.shape[-1]),
-                              _p(out), _st()), "sessd_ssfa_fuse")
-    return out
 
 
 # ------------------------------------------------------------------------------------------------ post-processing

@@ -211,22 +211,6 @@ def _pack_conv(w):
     return packed, [(ky, kx) for ky in range(kh) for kx in range(kw)]
 
 
-def _deconv_classes(w):
-    """nn.ConvTranspose2d(k3,s2,p1,op1) weight [Cin,Cout,3,3] -> 4 parity classes: (py, px, packed [T,Cin,Cout], taps)."""
-    out = []
-    for py in (0, 1):
-        for px in (0, 1):
-            kys = [(1, 0)] if py == 0 else [(0, 1), (2, 0)]     # (ky, dy): iy = y + dy
-            kxs = [(1, 0)] if px == 0 else [(0, 1), (2, 0)]
-            taps, mats = [], []
-            for ky, dy in kys:
-                for kx, dx in kxs:
-                    taps.append((dy, dx))
-                    mats.append(w[:, :, ky, kx])
-            out.append((py, px, torch.stack(mats, 0).contiguous(), taps))
-    return out
-
-
 def pack_head(head_sd, prefix, device, stride=24):
     """Four 1x1 head convs (mg_head_sessd.py:202-215) -> one [1,128,stride] GEMM weight + bias, channel layout
     [box 14 | cls 2 | dir 4 | iou 2 | zero pad]."""
@@ -290,142 +274,37 @@ def ssfa_fuse_weights(ssfa_sd, device, bn_eps=BN_EPS):
     return out
 
 
-# {abs-max, scale} slot of every SSFA tensor: the neck input, the launch outputs the planes runner keeps as planes, the fused map, then the
-# fp32 outputs (SSFARunner's abs-max slots have the same numbers)
+# {abs-max, scale} slot of every SSFA tensor: the neck input, the launch outputs kept as planes, the fused map, then the fp32 outputs
 SSFA_SLOT = {n: i for i, n in enumerate(["x"] + [L.dst for L in SSFA_LAUNCHES if not L.f32] + ["out"] + [L.dst for L in SSFA_LAUNCHES if L.f32])}
-_SSFA_INPUTS = {L.src for L in SSFA_LAUNCHES}        # tensors a later launch reads (the fp16 split needs their abs-max)
 _SSFA = {L.name: L for L in SSFA_LAUNCHES}
 
 
 class HeadRunner:
-    """The fused head GEMM alone (MultiGroupHead.forward)."""
+    """The fused head GEMM alone (MultiGroupHead.forward) on the fp16-split tensor-core conv (csrc/bevconv_p2.cu; the fp32 input is
+    split into planes first)."""
 
-    def __init__(self, batch, hw, device="cuda", use_tc=True, stride=24):
-        """use_tc: the fp16-split tensor-core conv (csrc/bevconv_p2.cu; the fp32 input is split into planes first); False = fp32 SIMT."""
-        self.batch, self.h, self.w, self.stride, self.use_tc = batch, int(hw[0]), int(hw[1]), stride, use_tc
+    def __init__(self, batch, hw, device="cuda", stride=24):
+        self.batch, self.h, self.w, self.stride = batch, int(hw[0]), int(hw[1]), stride
         self.out = torch.zeros((batch, self.h, self.w, stride), dtype=torch.float32, device=device)
         self.device = torch.device(device)
-        self.w_simt = self.w_tc = self.bias = None
-        if use_tc:
-            self.x_planes = ops.alloc_bev_planes(batch, self.h, self.w, 128, self.device)
-            self.info = torch.zeros((2, 2), dtype=torch.float32, device=self.device)     # {abs-max, scale} of the input / the output
+        self.params = None
+        self.x_planes = ops.alloc_bev_planes(batch, self.h, self.w, 128, self.device)
+        self.info = torch.zeros((2, 2), dtype=torch.float32, device=self.device)     # {abs-max, scale} of the input / the output
 
     def load_state(self, head_sd, prefix=""):
-        self.w_simt, self.bias = pack_head(head_sd, prefix, self.device, self.stride)
-        if self.use_tc:
-            self.w_tc = pack_h2(self.w_simt, None, self.bias, _cout_pad(self.stride))
+        w, bias = pack_head(head_sd, prefix, self.device, self.stride)
+        self.params = pack_h2(w, None, bias, _cout_pad(self.stride))
 
     def forward(self, x):
         H = (self.h, self.w)
         d = ops.conv_desc(self.batch, H, 128, H, self.stride, H, [(0, 0)], relu=False)
-        if self.w_tc is not None:
-            q = self.w_tc
-            self.info.zero_()
-            ops.absmax(x, self.info[0, 0:1])
-            ops.bev_split_planes(x, self.info[0], self.x_planes)
-            ops.bev_conv_p2(self.x_planes, self.info[0], q["w"], q["scale"], q["shift"], None, None, q["gain"], q["shift_max"], self.out, None,
-                            self.info[1], d)
-            return self.out
-        return ops.bev_conv(x, self.w_simt, None, self.bias, None, self.out, d)
-
-
-class SSFARunner:
-    """SSFA neck (rpn_v1.py:220-235) + the fused 128->22(+2 pad) head GEMM (mg_head_sessd.py:202-230) from fp32 activations, on the
-    fp32 SIMT baseline kernels, or (use_tc) with the stride-1 launches on the lab's h2 mode of bev_conv_p2_kernel (the fp32 input split
-    into fp16 planes inside the kernel, bevconv_split.cu) and the stride-2 conv on the SIMT kernel: a stride-2 3x3 patch and its fp32
-    staging copy leave the h2 mode no room for the weight ring at 128 output channels per tile."""
-
-    HEAD_STRIDE = 24
-
-    def __init__(self, batch, hw=(200, 176), device="cuda", use_tc=True):
-        self.batch, self.h, self.w, self.device = batch, int(hw[0]), int(hw[1]), torch.device(device)
-        self.use_tc = bool(use_tc)
-        self.amax = torch.zeros(16, dtype=torch.float32, device=self.device)     # abs-max scalars (fp16 split scaling), SSFA_SLOT numbering
-        z = lambda hw_, c: torch.zeros((batch,) + hw_ + (c,), dtype=torch.float32, device=self.device)  # noqa: E731
-        self.buf = {L.dst: z(ssfa_extents(L, self.h, self.w)[1], L.cout) for L in SSFA_LAUNCHES}
-        self.buf["out"] = z((self.h, self.w), 128)
-        self.params = None
-
-    def load_state(self, ssfa_sd, head_sd=None, head_prefix="tasks.0.", bn_eps=BN_EPS):
-        """bn_eps: eps of the neck's BatchNorm2d layers (rpn_v1.py:131-132 uses 1e-3; pass the module's own value otherwise)."""
-        P = ssfa_fuse_weights(ssfa_sd, self.device, bn_eps)
-        for L, wp, taps, sc, sh in ssfa_weights(ssfa_sd, head_sd, head_prefix, self.device, bn_eps):
-            if L.kind == "conv":
-                P[L.name] = (wp, taps, sc, sh)
-            else:       # SIMT: four parity-class convs; tensor cores: one launch over the 9-tap packing
-                P[L.name] = (_deconv_classes(wp.reshape(3, 3, L.cin, L.cout).permute(2, 3, 0, 1)), sc, sh)
-            if self.use_tc and L.stride == 1:
-                P[L.name + ":h2"] = pack_h2(wp, sc, sh, _cout_pad(L.cout))
-        self.params = P
-
-    def _am(self, name):
-        return None if name is None else self.amax[SSFA_SLOT[name]:SSFA_SLOT[name] + 1]
-
-    def _launch(self, L, x, out, ai=None, ao=None):
-        """launch L from x into out.  ai / ao: tensors whose abs-max slot holds the abs-max of the input (default: L's input) / receives
-        the abs-max of the output (fp16-split scaling)"""
-        in_hw, out_hw = ssfa_extents(L, self.h, self.w)
-        resid = self.buf[L.residual] if L.residual else None
-        h2 = self.params.get(L.name + ":h2")
-        if L.kind == "conv":
-            wp, taps, sc, sh = self.params[L.name]
-            d = ops.conv_desc(self.batch, in_hw, L.cin, out_hw, L.cout, out_hw, taps, in_stride=L.stride, relu=L.relu)
-            if h2 is not None:
-                ops.bev_conv_h2(x, h2["w"], h2["scale"], h2["shift"], resid, out, d, self._am(ai or L.src), self._am(ao))
-            else:
-                ops.bev_conv(x, wp, sc, sh, resid, out, d)
-        else:
-            classes, sc, sh = self.params[L.name]
-            if h2 is not None:
-                ops.bev_deconv_h2(x, h2["w"], h2["scale"], h2["shift"], resid, out, L.relu, self._am(ai or L.src), self._am(ao))
-            else:
-                for py, px, wp, taps in classes:
-                    d = ops.conv_desc(self.batch, in_hw, L.cin, out_hw, L.cout, in_hw, taps, in_stride=1, out_stride=2, out_off=(py, px),
-                                      relu=L.relu)
-                    ops.bev_conv(x, wp, sc, sh, resid, out, d)
-        if h2 is None and self.use_tc and ao is not None:
-            ops.absmax(out, self._am(ao))
-        return out
-
-    def forward(self, x, mark=None):
-        """x NHWC [B,200,176,128] -> (neck out NHWC [B,200,176,128], head NHWC [B,200,176,24]).
-        mark: optional callable(label) invoked after every layer (profiling scripts record a CUDA event there)."""
-        assert self.params is not None, "load_state first"
-        mark = mark or (lambda label: None)
-        b = self.buf
-        if self.use_tc:
-            self.amax.zero_()
-            ops.absmax(x, self._am("x"))
-        for L in SSFA_LAUNCHES[:-1]:
-            self._launch(L, x if L.src == "x" else b[L.src], b[L.dst], ao=L.dst if L.dst in _SSFA_INPUTS else None)
-            mark("neck:" + L.name)
-        w0, s0, t0 = self.params["w_0.0"]
-        w1, s1, t1 = self.params["w_1.0"]
-        ops.ssfa_fuse(b["o0"], b["o1"], w0, w1, s0, t0, s1, t1, b["out"])
-        if self.use_tc and "head" in self.params:
-            ops.absmax(b["out"], self._am("out"))
-        if "head" not in self.params:
-            mark("neck:fuse+head")
-            return b["out"], None
-        self.head(b["out"])
-        mark("neck:fuse+head")
-        return b["out"], b["head"]
-
-    def bench_layer(self, name="bottom_up_block_0.4"):
-        """(launch closure, kernel description) of one 3x3 128->128 layer on the buffers / abs-max slots a frame uses (valid after any
-        forward): what bench.py times alone for the `roofline` object."""
-
-        def launch():
-            self._launch(_SSFA[name], self.buf["x0"], self.buf["b0b"], ai="x0", ao="b0b")
-
-        if (name + ":h2") in self.params:
-            kern = "bev_conv_p2_kernel<.., kP2SplitF16> (fp32 input split to fp16 in shared memory, fp16 wgmma)"
-        else:
-            kern = "bev_conv_kernel (fp32 SIMT)"
-        return launch, kern
-
-    def head(self, x):
-        return self._launch(SSFA_LAUNCHES[-1], x, self.buf["head"])
+        q = self.params
+        self.info.zero_()
+        ops.absmax(x, self.info[0, 0:1])
+        ops.bev_split_planes(x, self.info[0], self.x_planes)
+        ops.bev_conv_p2(self.x_planes, self.info[0], q["w"], q["scale"], q["shift"], None, None, q["gain"], q["shift_max"], self.out, None,
+                        self.info[1], d)
+        return self.out
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -460,6 +339,7 @@ class SSFAPlanesRunner:
         return self.info[self.SLOT[name]]
 
     def load_state(self, ssfa_sd, head_sd=None, head_prefix="tasks.0.", bn_eps=BN_EPS):
+        """bn_eps: eps of the neck's BatchNorm2d layers (rpn_v1.py:131-132 uses 1e-3; pass the module's own value otherwise)."""
         P = ssfa_fuse_weights(ssfa_sd, self.device, bn_eps)
         for L, wp, taps, sc, sh in ssfa_weights(ssfa_sd, head_sd, head_prefix, self.device, bn_eps):
             P[L.name] = dict(pack_h2(wp, sc, sh, _cout_pad(L.cout)), taps=taps)
@@ -526,6 +406,9 @@ class SSFAPlanesRunner:
         return ops.planes_to_float(self.planes[name], self._info(name))
 
     def bench_layer(self, name="bottom_up_block_0.4"):
+        """(launch closure, kernel description) of one 3x3 128->128 layer on the planes / info slots a frame uses (valid after any
+        forward): what bench.py times alone for the `roofline` object."""
+
         def launch():
             self._launch(_SSFA[name]._replace(src="x0", dst="b0b"))
 

@@ -1,7 +1,7 @@
 """fp64 torch restatements of the BEV neck / head backward (csrc/bevgrad.cu, sessd_b200/bev_grad.py); shared by
 tests/test_bev_grad_model.py (CPU) and tests/test_gpu_bev_grad.py.
 
-* ``tap_conv``: the forward kernels' tap-list conv (sessd_bev_conv semantics) at the index level, NHWC;
+* ``tap_conv``: the forward kernels' tap-list conv (sessd_conv_desc semantics) at the index level, NHWC;
 * ``wgrad_index``: what sessd_bev_wgrad computes, gW[t][ci][co] = sum_{b,y,x} X[b, y s + dy_t, x s + dx_t, ci] G[b, y, x, co];
 * ``bg_geometry``: its work-item decomposition (the item count is a function of the descriptor only);
 * ``ssfa_train_ref`` / ``head_ref``: rpn_v1.py:220-235 written out with train-mode BatchNorm2d, and the four head convs, in fp64 torch."""

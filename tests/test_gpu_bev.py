@@ -14,20 +14,6 @@ def _rel(a, b):
     return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-30))
 
 
-MODES = ["simt", "fp16x2", "planes"]   # fp32 SIMT baseline | fp16 split of fp32 inputs | pre-split planes (default)
-
-
-def _runner(batch, hw, mode):
-    from sessd_b200.runners import SSFAPlanesRunner, SSFARunner
-    if mode == "planes":
-        return SSFAPlanesRunner(batch, hw, "cuda")
-    return SSFARunner(batch, hw, "cuda", use_tc=mode != "simt")
-
-
-def _act(r, name):
-    return r.activation(name) if hasattr(r, "activation") else r.buf[name]
-
-
 def _to_planes(xd):
     """fp32 NHWC device tensor -> (planes [2,B,H,W,C], info [2])"""
     from sessd_b200 import ops
@@ -38,16 +24,15 @@ def _to_planes(xd):
     return planes, info
 
 
-@pytest.mark.parametrize("mode", MODES)
-def test_ssfa_and_head_match_reference_golden(golden_dir, mode):
+def test_ssfa_and_head_match_reference_golden(golden_dir):
     from oracle import bev_ref
-    from sessd_b200.runners import SSFARunner
+    from sessd_b200.runners import SSFAPlanesRunner
     g = np.load(os.path.join(golden_dir, "ssfa_head_case.npz"))
     sd = bev_ref.ssfa_random_state(7)
     hsd = bev_ref.head_random_state(9, prefix="tasks.0.")
     gen = torch.Generator().manual_seed(8)
     x = torch.relu(torch.randn(1, 128, 24, 16, generator=gen))
-    r = _runner(1, (24, 16), mode)
+    r = SSFAPlanesRunner(1, (24, 16), "cuda")
     r.load_state(sd, hsd)
     out, head = r.forward(x.permute(0, 2, 3, 1).contiguous().cuda())
     torch.cuda.synchronize()
@@ -64,27 +49,26 @@ def test_ssfa_and_head_match_reference_golden(golden_dir, mode):
     assert _rel(h[..., 20:22], g["iou_preds"]) < TOL
 
 
-@pytest.mark.parametrize("mode", MODES)
-def test_ssfa_intermediates_match_oracle_fp64_batch2(mode):
+def test_ssfa_intermediates_match_oracle_fp64_batch2():
     from oracle import bev_ref
-    from sessd_b200.runners import SSFARunner
+    from sessd_b200.runners import SSFAPlanesRunner
     sd = bev_ref.ssfa_random_state(17)
     hsd = bev_ref.head_random_state(19)
     gen = torch.Generator().manual_seed(18)
     x = torch.relu(torch.randn(2, 128, 40, 48, generator=gen))
     trace = {}
     ref = bev_ref.ssfa_forward(x.double(), {k: v.double() if v.is_floating_point() else v for k, v in sd.items()}, trace)
-    r = _runner(2, (40, 48), mode)
+    r = SSFAPlanesRunner(2, (40, 48), "cuda")
     r.load_state(sd, hsd)
     out, _ = r.forward(x.permute(0, 2, 3, 1).contiguous().cuda())
     torch.cuda.synchronize()
     for mine, theirs in (("x0", "x0"), ("x1", "x1"), ("t0", "t0"), ("t1", "t1"), ("m0", "m0"), ("m1", "m1"), ("o0", "o0"), ("o1", "o1")):
-        got = _act(r, mine).permute(0, 3, 1, 2).cpu().numpy()
+        got = r.activation(mine).permute(0, 3, 1, 2).cpu().numpy()
         assert _rel(got, trace[theirs].numpy()) < 2e-5, mine
     assert _rel(out.permute(0, 3, 1, 2).cpu().numpy(), ref.numpy()) < 2e-5
 
 
-@pytest.mark.parametrize("mode", MODES)
+@pytest.mark.parametrize("mode", ["fp16x2", "planes"])   # fp16 split of fp32 inputs (lab h2) | pre-split planes (default)
 @pytest.mark.parametrize("cin,cout,k,hw", [(128, 128, 3, (21, 37)), (256, 256, 3, (9, 50)), (128, 128, 1, (8, 16)), (256, 256, 1, (13, 17)),
                                            (128, 24, 1, (20, 33))])
 def test_single_conv_vs_fp64(mode, cin, cout, k, hw):
@@ -120,16 +104,13 @@ def test_single_conv_vs_fp64(mode, cin, cout, k, hw):
         assert float(oinfo[0]) == float(out.abs().max())
         back = ops.planes_to_float(oplanes, oinfo)
         assert float((back - out).abs().max()) <= 4e-7 * float(out.abs().max()), "planes output differs from the fp32 output"
-    elif mode == "fp16x2":
+    else:
         planes, inv = ops.pack_weight_h2(wp.cuda(), cout_pad)
         amax = torch.zeros(2, device="cuda")
         ops.absmax(xd, amax[0:1])
         ops.bev_conv_h2(xd, planes, sc.cuda() * inv[:cout], sh.cuda(), rd, out, d, amax[0:1], amax[1:2])
         torch.cuda.synchronize()
         assert float(amax[0]) == float(xd.abs().max()) and float(amax[1]) == float(out.abs().max())
-    else:
-        ops.bev_conv(xd, wp.cuda(), sc.cuda(), sh.cuda(), rd, out, d)
-    torch.cuda.synchronize()
     got = out.permute(0, 3, 1, 2).cpu().double()
     err = float((got - ref).abs().max() / ref.abs().max())
     assert err < 5e-6, err
