@@ -358,6 +358,56 @@ int sessd_assign_targets(const float *d_anchors, int num_anchors, const float *d
                          void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Training augmentation: per-object noise, global flip / rotation / scaling, shuffle (csrc/augment.cu).  Replaces the numba loops of det3d/core/sampler/preprocess.py that
+ * noise_per_object_v4_ (:614-658, called from det3d/datasets/pipelines/preprocess.py:110-121) runs on every training frame.  The random
+ * draws are made on the host (sessd_b200/augment.py, a numpy RandomState in the reference's order); these calls are pure functions
+ * of the boxes and the draws, evaluated in fp64 like the reference (see the file header for the rounding).
+ * sessd_box_collision -- box_collision_test (:944-1027, clockwise): d_out[i, j] = 1 when BEV corner set i of d_boxes [n, 4, 2] and j of
+ *     d_qboxes [k, 4, 2] (fp64, box2d_to_corner_jit order) collide: standup pre-test, segment crossing, containment either way.
+ * sessd_noise_per_box -- noise_per_box (:579-611) over a padded batch: d_gt_boxes [batch, max_gt, 7] f32 (x y z w l h r), d_num_gt
+ *     [batch] (device), d_valid [batch, max_gt] u8 (gt_boxes_mask: the box's class is a target class), d_loc_noise [batch, max_gt,
+ *     num_try, 3] and d_rot_noise [batch, max_gt, num_try] fp64 (the draws), context = data_aug_with_context (<= 0: none; > 0 enlarges
+ *     w and l).  d_selected [batch, max_gt] i32: the try each valid box takes, -1 when every try collides, for invalid boxes and for
+ *     the padding.  max_gt <= SESSD_AUGMENT_MAX_GT, num_try <= SESSD_AUGMENT_MAX_TRY (SESSD_ECAPACITY above); no workspace.
+ * ------------------------------------------------------------------------------------------------ */
+#define SESSD_AUGMENT_MAX_GT 256
+#define SESSD_AUGMENT_MAX_TRY 128
+int sessd_box_collision(const double *d_boxes, int n, const double *d_qboxes, int k, uint8_t *d_out, void *stream);
+int sessd_noise_per_box(const float *d_gt_boxes, const int *d_num_gt, const uint8_t *d_valid, int batch, int max_gt,
+                        const double *d_loc_noise, const double *d_rot_noise, int num_try, double context, int *d_selected,
+                        void *stream);
+/* sessd_augment_points -- points_transform_ (:545-560) with the membership of points_in_convex_polygon_3d_jit (:634-646), the raw
+ *     twin (pipelines/preprocess.py:131), random_flip_v2 / global_rotation_v3 / global_scaling_v3 (:896-941) and the shuffle
+ *     (pipelines/preprocess.py:159-161) in one pass.  d_points [*, 4] f32 with d_frame_off [batch + 1] (device); max_frame_points: the
+ *     largest frame (sizes the grid); boxes, valid and draws as for sessd_noise_per_box and its d_selected; d_global [batch, 5] f32 =
+ *     fp32 cos, fp32 sin of the global angle, fp32 scale, flip (0 / 1), fp32 angle; d_perm [*] i32: frame-local permutation, student
+ *     row k of frame f = point d_perm[off + k] of the frame; d_labeled [batch] u8 (nullable: all labelled; an unlabelled frame is
+ *     shuffled, flipped, rotated and scaled only, pipelines/preprocess.py:163-167).  A point moves with the first VALID box holding it
+ *     (pre-noise boxes).  Outputs: d_points_raw (nullable) = the noised points before the global stages, unshuffled (rows of unlabelled
+ *     frames untouched); d_points_out = the student's points.  d_points, d_points_raw and d_points_out are read / written as float4
+ *     rows and must be 16-byte aligned (SESSD_EINVAL otherwise).  d_perm must hold a permutation of [0, n_f) per frame; a row whose
+ *     entry is out of range is left unwritten (never an out-of-bounds access).
+ * sessd_augment_boxes -- box3d_transform_ (:562-567), the valid-box selection, the global stages on the boxes, then the bookkeeping of
+ *     Voxelization / AssignTarget (pipelines/preprocess.py:200-205, :290-330): both sets keep the boxes that are valid and in d_target
+ *     (u8 [batch, max_gt], nullable: all), the student's set also drops the boxes with no BEV corner strictly inside range_bev (HOST
+ *     float[4] x0 y0 x1 y1, filter_gt_box_outside_range); angles -> limit_period(r, 0.5, 2 pi); compacted in index order into
+ *     d_boxes_raw / d_boxes_out [batch, max_gt, 7] (zero padded) with d_num_raw / d_num_out [batch]: the layout sessd_assign_targets reads. */
+/* sessd_points_in_boxes -- points_in_rbbox / points_in_convex_polygon_3d_jit over center_to_corner_box3d(origin 0.5) faces, as the
+ *     point pass tests membership and as GT-AUG's point removal needs it: d_mask [n, m] u8 = point i (d_points rows of point_stride floats,
+ *     x y z first) inside box j of d_boxes [m, 7] f32, w and l enlarged by context when it is positive.  The test is |R^T (p - c)| < dims/2
+ *     in fp64: the reference's face-plane test holds the same points except within rounding of a face. */
+int sessd_points_in_boxes(const float *d_points, int n, int point_stride, const float *d_boxes, int m, double context, uint8_t *d_mask,
+                          void *stream);
+int sessd_augment_points(const float *d_points, const int *d_frame_off, int batch, int max_frame_points, const float *d_gt_boxes,
+                         const int *d_num_gt, const uint8_t *d_valid, int max_gt, const double *d_loc_noise, const double *d_rot_noise,
+                         int num_try, const int *d_selected, double context, const float *d_global, const int *d_perm,
+                         const uint8_t *d_labeled, float *d_points_raw, float *d_points_out, void *stream);
+int sessd_augment_boxes(const float *d_gt_boxes, const int *d_num_gt, const uint8_t *d_valid, const uint8_t *d_target, int batch,
+                        int max_gt, const double *d_loc_noise, const double *d_rot_noise, int num_try, const int *d_selected,
+                        const float *d_global, const float *range_bev, float *d_boxes_raw, int *d_num_raw, float *d_boxes_out,
+                        int *d_num_out, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * SURVEY.md 8(f) row 1, first slice of the training step: the supervised SSD-head loss terms, value AND gradient in one pass.
  * Replaces (for the terms without the teacher model) det3d/models/bbox_heads/mg_head_sessd.py:706-760:
  * prepare_loss_weights/NormByNumPositives (:525-572), SigmoidFocalLoss (det3d/models/losses/losses.py:345-420, gamma = 2),

@@ -117,6 +117,11 @@ SIGNATURES = {
     "sessd_adamw_clip_ema_step": (_i, [_vp, _vp, _vp, _vp, _ll, _f, _f, _f, _f, _f, _i, _vp, _vp, C.c_double, _vp]),
     "sessd_assign_workspace_bytes": (_sz, [_i, _i, _i]),
     "sessd_assign_targets": (_i, [_vp, _i, _vp, _vp, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "sessd_box_collision": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
+    "sessd_noise_per_box": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _i, C.c_double, _vp, _vp]),
+    "sessd_points_in_boxes": (_i, [_vp, _i, _i, _vp, _i, C.c_double, _vp, _vp]),
+    "sessd_augment_points": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _i, _vp, C.c_double, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "sessd_augment_boxes": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, C.POINTER(C.c_float), _vp, _vp, _vp, _vp, _vp]),
     "sessd_kitti_convert_workspace_bytes": (_sz, [_ll]),
     "sessd_kitti_convert_detections": (_i, [_vp, _vp, _vp, _vp, _i, _ll, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "sessd_kitti_overlaps": (_i, [C.POINTER(KittiFrames), _i, _i, C.c_double, _vp, _vp]),

@@ -1,0 +1,294 @@
+"""SE-SSD training-frame augmentation on the device: per-object box noise with collision tests, global flip / rotation / scaling, the
+point shuffle and the teacher's un-augmented twin (reference: det3d/datasets/pipelines/preprocess.py:68-175, Preprocess.__call__, and the
+numba loops of det3d/core/sampler/preprocess.py it calls).
+
+Every random number is drawn on the host by ``draw_augmentation`` with a numpy ``RandomState``, with the reference's calls in the
+reference's order; the kernels of csrc/augment.cu are pure functions of the points, the boxes and those draws, so each stage is
+comparable with the reference's own function run on the same seed.
+
+Not built here (see DESIGN §7): GT-database sampling (GT-AUG, before the per-object noise) and shape-aware augmentation (SA-DA,
+``pyramid_augment_v0``, between the global scaling and the shuffle).  The reference's ``Preprocess`` always runs both, so this module
+registers no ``Preprocess`` pipeline; ``build_train_batch`` (the collated batch) and ``augment_batch`` (the augmented points and
+boxes) are their own entry points.
+"""
+from dataclasses import dataclass, field
+
+import numpy as np
+import torch
+
+from . import ops
+
+NUM_TRY = 100                                   # noise_per_object_v4_(num_try=100), pipelines/preprocess.py:118
+MAX_GT = 256                                    # SESSD_AUGMENT_MAX_GT (include/sessd_b200.h)
+
+
+@dataclass
+class AugmentConfig:
+    """the train_preprocessor values the augmentation reads (examples/second/configs/config.py train_preprocessor)"""
+    gt_loc_noise: tuple = (1.0, 1.0, 0.5)
+    gt_rot_noise: tuple = (-0.785, 0.785)
+    global_rot_noise: tuple = (-0.785, 0.785)
+    global_scale_noise: tuple = (0.95, 1.05)
+    data_aug_with_context: float = -1.0
+    class_names: tuple = ("Car", "Van")
+    shuffle_points: bool = True
+    target_class_ids: tuple = (1, 2)            # AssignTarget: [1, 2] with enable_similar_type, else [1]
+    range_bev: tuple = (0.0, -40.0, 70.4, 40.0)  # filter_gt_box_outside_range over pc_range[[0, 1, 3, 4]] (Voxelization)
+
+    @classmethod
+    def from_config(cls, cfg):
+        """from a loaded det3d Config: cfg.train_preprocessor, cfg.voxel_generator.range, cfg.train_cfg.assigner"""
+        tp = cfg.train_preprocessor
+        names = list(tp.class_names)                # the reference appends 'Van' to the config's own list; this copies it
+        similar = bool(tp.get("enable_similar_type", False))
+        if similar and "Car" in names:
+            names.append("Van")
+        rg = [float(v) for v in cfg.voxel_generator.range]
+        similar_assign = bool(cfg.train_cfg.assigner.get("enable_similar_type", False))
+        ctx = tp.get("data_aug_with_context", -1)
+        return cls(gt_loc_noise=tuple(float(v) for v in tp.gt_loc_noise), gt_rot_noise=tuple(float(v) for v in tp.gt_rot_noise),
+                   global_rot_noise=_pair(tp.global_rot_noise), global_scale_noise=tuple(float(v) for v in tp.global_scale_noise),
+                   data_aug_with_context=float(ctx), class_names=tuple(names), shuffle_points=bool(tp.get("shuffle_points", False)),
+                   target_class_ids=(1, 2) if similar_assign else (1,), range_bev=(rg[0], rg[1], rg[3], rg[4]))
+
+
+def _pair(r):
+    """global_rotation_v3: a scalar r means [-r, r]"""
+    if isinstance(r, (list, tuple)):
+        return float(r[0]), float(r[1])
+    return -float(r), float(r)
+
+
+@dataclass
+class FrameDraws:
+    loc: np.ndarray          # [M, NUM_TRY, 3] fp64
+    rot: np.ndarray          # [M, NUM_TRY] fp64
+    flip: bool
+    rotation: float
+    scale: float
+    perm: np.ndarray         # [N] int64
+
+
+@dataclass
+class Draws:
+    frames: list = field(default_factory=list)
+
+    def transformation(self):
+        """the per-frame ``transformation`` dicts of Preprocess (pipelines/preprocess.py:140) that consistency_loss undoes"""
+        return [dict(flipped=f.flip, noise_rotation=f.rotation, noise_scale=f.scale) for f in self.frames]
+
+
+def draw_augmentation(rs, frames, cfg):
+    """Draw every random number of the augmentation on the host, per frame, with the reference's calls in the reference's order.
+
+    frames: per frame (num_points, num_boxes, labeled).  Labelled frames: ``normal(scale=gt_loc_noise, size=[M, 100, 3])`` and
+    ``uniform(*gt_rot_noise, size=[M, 100])`` (noise_per_object_v4_), ``choice([False, True], replace=False, p=[0.5, 0.5])``
+    (random_flip_v2), ``uniform`` for the global rotation and for the scale, then ``choice(arange(n), n, replace=False)`` (the shuffle,
+    when shuffle_points).  Unlabelled frames: the shuffle first, then flip, rotation and scale.
+
+    GT-AUG (before the noise) and SA-DA (between the scaling and the shuffle) are not built and draw nothing, so a seeded stream matches
+    the reference stage by stage, not over the whole of its Preprocess (which runs both)."""
+    out = Draws()
+    loc_std = np.array(cfg.gt_loc_noise, dtype=np.float32)          # noise_per_object_v4_: np.array(center_noise_std, gt_boxes.dtype)
+    for n, m, labeled in frames:
+        n, m = int(n), int(m)
+        if labeled:
+            loc = rs.normal(scale=loc_std, size=[m, NUM_TRY, 3])
+            rot = rs.uniform(cfg.gt_rot_noise[0], cfg.gt_rot_noise[1], size=[m, NUM_TRY])
+            flip, rotation, scale = _global_draws(rs, cfg)
+            perm = _shuffle(rs, n, cfg)
+        else:
+            loc, rot = np.zeros((0, NUM_TRY, 3)), np.zeros((0, NUM_TRY))
+            perm = _shuffle(rs, n, cfg)
+            flip, rotation, scale = _global_draws(rs, cfg)
+        out.frames.append(FrameDraws(loc, rot, flip, rotation, scale, perm))
+    return out
+
+
+def _global_draws(rs, cfg):
+    flip = bool(rs.choice([False, True], replace=False, p=[0.5, 0.5]))
+    rotation = float(rs.uniform(cfg.global_rot_noise[0], cfg.global_rot_noise[1]))
+    scale = float(rs.uniform(cfg.global_scale_noise[0], cfg.global_scale_noise[1]))
+    return flip, rotation, scale
+
+
+def _shuffle(rs, n, cfg):
+    if not cfg.shuffle_points:
+        return np.arange(n)
+    return rs.choice(np.arange(n), n, replace=False)
+
+
+def global_row(d):
+    """fp32 (cos, sin, scale, flip, angle) as rotation_points_single_angle / global_scaling_v3 / random_flip_v2 round them"""
+    return np.array([np.float32(np.cos(d.rotation)), np.float32(np.sin(d.rotation)), np.float32(d.scale), 1.0 if d.flip else 0.0,
+                     np.float32(d.rotation)], np.float32)
+
+
+def _pack(arrays):
+    """one host buffer for all inputs (one host-to-device copy per batch); returns (bytes, [(offset, dtype, shape)])"""
+    layout, off = [], 0
+    for a in arrays:
+        layout.append((off, a.dtype, a.shape))
+        off += -(-a.nbytes // 16) * 16
+    buf = np.zeros(max(off, 16), np.uint8)
+    for (o, _, _), a in zip(layout, arrays):
+        buf[o:o + a.nbytes] = np.ascontiguousarray(a).view(np.uint8).reshape(-1)
+    return buf, layout
+
+
+def _unpack(dev, layout):
+    out = []
+    for o, dt, shape in layout:
+        n = int(np.prod(shape)) * np.dtype(dt).itemsize
+        out.append(dev[o:o + n].view(getattr(torch, np.dtype(dt).name)).view(*shape) if n else
+                   torch.empty(shape, dtype=getattr(torch, np.dtype(dt).name), device=dev.device))
+    return out
+
+
+def augment_batch(cfg, clouds, gt_boxes, gt_names, draws, labeled=None, device="cuda"):
+    """Augment a batch of frames on the device.  clouds: per frame [N, 4] f32; gt_boxes: per frame [M, 7] (x y z w l h r); gt_names: per
+    frame [M] class names (DontCare / ignore already dropped, as Preprocess does first); draws: draw_augmentation's output for
+    (len(cloud), len(boxes), labeled) of every frame; labeled: per frame, None = all labelled.
+
+    Returns a dict of device tensors: ``points`` (the student's [P, 4]: noised, flipped, rotated, scaled, shuffled), ``points_raw``
+    (the teacher's twin: noised, unshuffled; an unlabelled frame's rows are its input), ``frame_off`` [B+1], ``gt_boxes`` / ``num_gt`` (the student's boxes after the range
+    filter) and ``gt_boxes_raw`` / ``num_gt_raw`` (the teacher's), both padded [B, max_gt, 7] with limit_period angles -- the layout
+    sessd_assign_targets reads --, ``selected`` [B, max_gt] (the try each box took, -1 none); and ``transformation`` (host list of dicts).
+    Launches on the current stream and never waits on the device."""
+    B = len(clouds)
+    labeled = [True] * B if labeled is None else [bool(v) for v in labeled]
+    ms = [len(b) if lab else 0 for b, lab in zip(gt_boxes, labeled)]
+    max_gt = max([1] + ms)
+    if max_gt > MAX_GT:
+        raise ValueError("a frame has %d GT boxes > %d" % (max_gt, MAX_GT))
+    ns = [len(c) for c in clouds]
+    off = np.zeros(B + 1, np.int32)
+    off[1:] = np.cumsum(ns)
+    pts = np.concatenate([np.asarray(c, np.float32).reshape(-1, 4) for c in clouds] + [np.zeros((0, 4), np.float32)])
+    boxes = np.zeros((B, max_gt, 7), np.float32)
+    valid = np.zeros((B, max_gt), np.uint8)
+    target = np.zeros((B, max_gt), np.uint8)
+    loc = np.zeros((B, max_gt, NUM_TRY, 3))
+    rot = np.zeros((B, max_gt, NUM_TRY))
+    glob = np.zeros((B, 5), np.float32)
+    perm = np.zeros(len(pts), np.int32)
+    for b in range(B):
+        d = draws.frames[b]
+        if len(d.perm) != ns[b] or d.loc.shape[0] != ms[b]:
+            raise ValueError("frame %d: the draws were made for another frame size" % b)
+        if ns[b] and not (np.bincount(np.asarray(d.perm), minlength=ns[b])[:ns[b]] == 1).all():
+            raise ValueError("frame %d: perm is not a permutation of the frame's points" % b)
+        m = ms[b]
+        if m:
+            boxes[b, :m] = np.asarray(gt_boxes[b], np.float32)
+            names = list(gt_names[b])
+            valid[b, :m] = [n in cfg.class_names for n in names]
+            target[b, :m] = [n in cfg.class_names and cfg.class_names.index(n) + 1 in cfg.target_class_ids for n in names]
+            loc[b, :m], rot[b, :m] = d.loc, d.rot
+        glob[b] = global_row(d)
+        perm[off[b]:off[b + 1]] = d.perm
+    num_gt = np.array(ms, np.int32)
+    lab = np.array(labeled, np.uint8)
+    buf, layout = _pack([pts, off, boxes, num_gt, valid, target, loc, rot, glob, perm, lab])
+    dev = torch.from_numpy(buf).pin_memory().to(device, non_blocking=True)
+    d_pts, d_off, d_boxes, d_num, d_valid, d_target, d_loc, d_rot, d_glob, d_perm, d_lab = _unpack(dev, layout)
+    ctx = cfg.data_aug_with_context
+    sel = ops.noise_per_box(d_boxes, d_num, d_valid, d_loc, d_rot, ctx)
+    raw = None if all(labeled) else d_pts.clone()          # an unlabelled frame has no twin in the reference: its rows keep the input
+    raw, out = ops.augment_points(d_pts, d_off, max(ns + [0]), d_boxes, d_num, d_valid, d_loc, d_rot, sel, d_glob, d_perm, d_lab, ctx,
+                                  points_raw=raw)
+    boxes_raw, num_raw, boxes_out, num_out = ops.augment_boxes(d_boxes, d_num, d_valid, d_target, d_loc, d_rot, sel, d_glob, cfg.range_bev)
+    return dict(points=out, points_raw=raw, frame_off=d_off, gt_boxes=boxes_out, num_gt=num_out, gt_boxes_raw=boxes_raw,
+                num_gt_raw=num_raw, selected=sel, transformation=draws.transformation())
+
+
+
+# ------------------------------------------------------------------------------------------------ collated training batch
+_STATIC = {}
+
+
+def _static(cfg, device):
+    """per-config constants of the batch builder: the augmentation values, the voxeliser config and grid, the anchors on the device and
+    the assigner's thresholds (built once per config object and device)"""
+    key = (id(cfg), str(device))
+    if key not in _STATIC:
+        from det3d.datasets.pipelines import AssignTarget, Voxelization
+        vg = cfg.voxel_generator
+        vox = Voxelization(cfg=vg).voxel_generator
+        at = AssignTarget(cfg=cfg.train_cfg.assigner)
+        if len(at.anchor_dicts_by_task) != 1 or len(at.anchor_dicts_by_task[0]) != 1:
+            raise NotImplementedError("build_train_batch supports the single-class SE-SSD KITTI config")
+        ta = at.target_assigners[0]
+        (ad,) = at.anchor_dicts_by_task[0].values()
+        gen = ta._anchor_generators[0]
+        anchors = torch.from_numpy(np.ascontiguousarray(ad["anchors"].reshape(-1, 7), np.float32)).pin_memory().to(device, non_blocking=True)
+        _STATIC[key] = dict(cfg=cfg, aug=AugmentConfig.from_config(cfg),
+                            vcfg=ops.make_voxel_cfg(vg.voxel_size, vg.range, vg.max_points_in_voxel, vg.max_voxel_num),
+                            grid=np.asarray(vox.grid_size), anchors=anchors, thr=(float(gen.match_threshold), float(gen.unmatch_threshold)))
+    return _STATIC[key]
+
+
+class PendingBatch:
+    """A training batch whose device work has been launched (augmentation, both voxelisations, both target assignments) and whose
+    collated dict is not formed yet.  ``example()`` forms it: the one device-to-host read of the batch (the two branches' voxel totals,
+    which size the exact-count voxel tensors the model reads)."""
+
+    def __init__(self, st, aug, vox, vox_raw, asg, asg_raw, batch, frame_off, num_points_total):
+        self._st, self._aug, self._vox, self._vox_raw, self._asg, self._asg_raw = st, aug, vox, vox_raw, asg, asg_raw
+        self._batch, self._off, self._total = batch, frame_off, num_points_total
+
+    def example(self):
+        B = self._batch
+        totals = torch.stack([self._vox.num_voxels[B], self._vox_raw.num_voxels[B]]).cpu().tolist()      # the one read-back
+        dev = self._off.device
+        counts = self._off[1:] - self._off[:-1]
+        bidx = torch.repeat_interleave(torch.arange(B, dtype=torch.float32, device=dev), counts, output_size=self._total)
+        anchors = [self._st["anchors"].unsqueeze(0).expand(B, -1, -1).contiguous()]
+        shape = np.stack([self._st["grid"]] * B)
+        ex = dict(metadata=[dict(token=i) for i in range(B)], points=torch.cat([bidx[:, None], self._aug["points"]], 1))
+        for sfx, vb, ab, n in (("", self._vox, self._asg, totals[0]), ("_raw", self._vox_raw, self._asg_raw, totals[1])):
+            ex["voxels" + sfx] = vb.voxels[:n]
+            ex["num_points" + sfx] = vb.num_points[:n]
+            ex["coordinates" + sfx] = vb.coors[:n]
+            ex["num_voxels" + sfx] = vb.num_voxels[:B].long()
+            ex["shape" + sfx] = shape
+            ex["anchors" + sfx] = anchors
+            ex["labels" + sfx] = [ab.labels]
+            ex["reg_targets" + sfx] = [ab.bbox_targets]
+        ex["transformation"] = self._aug["transformation"]
+        return ex
+
+
+def launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda"):
+    """Everything of build_train_batch that runs on the device, launched without waiting on it: the draws (host), augment_batch, the
+    voxeliser on the student's points and on the twin, the target assigner on both box sets.  Returns a PendingBatch."""
+    if labeled is not None and not all(labeled):
+        raise ValueError("build_train_batch builds labelled batches (the reference gives unlabelled frames no targets and no twin); "
+                         "augment unlabelled frames with augment_batch(..., labeled=...)")
+    st = _static(cfg, device)
+    B = len(clouds)
+    draws = draw_augmentation(rs, [(len(c), len(b), True) for c, b in zip(clouds, gt_boxes)], st["aug"])
+    aug = augment_batch(st["aug"], clouds, gt_boxes, gt_names, draws, device=device)
+    total = int(sum(len(c) for c in clouds))
+    vox, vox_raw = (ops.VoxelBuffers(st["vcfg"], B, max(total, 1), device) for _ in range(2))
+    ops.voxelize(aug["points"], aug["frame_off"], vox)
+    ops.voxelize(aug["points_raw"], aug["frame_off"], vox_raw)
+    A = st["anchors"].shape[0]
+    asg, asg_raw = (ops.AssignBuffers(A, B, aug["gt_boxes"].shape[1], device) for _ in range(2))
+    ops.assign_targets(st["anchors"], aug["gt_boxes"], aug["num_gt"], asg, *st["thr"])
+    ops.assign_targets(st["anchors"], aug["gt_boxes_raw"], aug["num_gt_raw"], asg_raw, *st["thr"])
+    return PendingBatch(st, aug, vox, vox_raw, asg, asg_raw, B, aug["frame_off"], total)
+
+
+def build_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda"):
+    """A collated SE-SSD training batch with real augmentation: the ``example`` dict batch_processor_inline takes, with the keys of
+    ``synth.train_batch`` (voxels, coordinates with a batch column, num_points, num_voxels, shape, anchors, labels, reg_targets, their
+    ``_raw`` twins for the teacher, points with a batch column, metadata, transformation), all tensors on the device.
+
+    cfg: the loaded det3d Config (train_preprocessor, voxel_generator, train_cfg.assigner); clouds: per frame [N, 4] f32; gt_boxes /
+    gt_names: per frame [M, 7] and [M] (DontCare / ignore dropped); rs: the numpy RandomState the draws come from (draw_augmentation).
+    The student's frame is noised, flipped, rotated, scaled and shuffled; the teacher's twin is the noised frame (Preprocess:131).
+
+    The device work is launched without waiting (launch_train_batch); forming the dict then reads the two branches' voxel totals back
+    once, because the model consumes exact-count voxel tensors."""
+    return launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled, device).example()

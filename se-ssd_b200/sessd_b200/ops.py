@@ -615,3 +615,110 @@ def odiou_loss(head, anchors, labels, reg_targets, losses, grad_head=None, w_odi
     check(lib.sessd_odiou_loss(_p(head), _p(anchors), _p(labels), _p(reg_targets), int(B), int(A), 2, int(head.shape[2]), float(w_odiou),
                                _p(losses), _p(out), _p(grad_head), _p(ws), ws.numel(), _st()), "sessd_odiou_loss")
     return out
+
+
+# ------------------------------------------------------------------------------------------------ training augmentation (csrc/augment.cu)
+def box_collision(boxes, qboxes, out=None):
+    """box_collision_test: boxes [N,4,2], qboxes [K,4,2] fp64 corner sets (device) -> [N,K] uint8 (1 = collide)."""
+    _cuda(boxes, torch.float64, "boxes"); _cuda(qboxes, torch.float64, "qboxes")
+    n, k = boxes.shape[0], qboxes.shape[0]
+    if out is None:
+        out = torch.empty((n, k), dtype=torch.uint8, device=boxes.device)
+    check(lib.sessd_box_collision(_p(boxes), int(n), _p(qboxes), int(k), _p(out), _st()), "sessd_box_collision")
+    return out
+
+
+def _aug_inputs(gt_boxes, num_gt, valid, loc_noise, rot_noise, selected=None):
+    """checks the padded box batch and its draws: gt_boxes [B,M,7] f32, num_gt [B] i32, valid [B,M] u8, loc_noise [B,M,T,3] and
+    rot_noise [B,M,T] f64, selected [B,M] i32 -- contiguous CUDA tensors; returns (B, M, T)"""
+    _cuda(gt_boxes, torch.float32, "gt_boxes"); _cuda(num_gt, torch.int32, "num_gt"); _cuda(valid, torch.uint8, "valid")
+    _cuda(loc_noise, torch.float64, "loc_noise"); _cuda(rot_noise, torch.float64, "rot_noise")
+    B, M = valid.shape
+    T = rot_noise.shape[2]
+    if (tuple(gt_boxes.shape) != (B, M, 7) or num_gt.numel() != B or tuple(loc_noise.shape) != (B, M, T, 3)
+            or tuple(rot_noise.shape) != (B, M, T)):
+        raise ValueError("augmentation inputs: shape mismatch")
+    if selected is not None:
+        _cuda(selected, torch.int32, "selected")
+        if tuple(selected.shape) != (B, M):
+            raise ValueError("selected must be [B, M]")
+    return B, M, T
+
+
+def points_in_boxes(points, boxes, context=-1.0, mask=None):
+    """points [N, >=3] f32, boxes [M, 7] f32 (device) -> [N, M] uint8 membership mask (sessd_points_in_boxes)."""
+    _cuda(points, torch.float32, "points"); _cuda(boxes, torch.float32, "boxes")
+    if points.dim() != 2 or points.shape[1] < 3 or boxes.dim() != 2 or boxes.shape[1] != 7:
+        raise ValueError("points_in_boxes: points [N, >=3], boxes [M, 7]")
+    n, m = points.shape[0], boxes.shape[0]
+    if mask is None:
+        mask = torch.empty((n, m), dtype=torch.uint8, device=points.device)
+    check(lib.sessd_points_in_boxes(_p(points), int(n), int(points.shape[1]), _p(boxes), int(m), float(context), _p(mask), _st()),
+          "sessd_points_in_boxes")
+    return mask
+
+
+def noise_per_box(gt_boxes, num_gt, valid, loc_noise, rot_noise, context=-1.0, selected=None):
+    """noise_per_box over a padded batch: gt_boxes [B,M,7] f32, num_gt [B] i32, valid [B,M] u8, loc_noise [B,M,T,3] / rot_noise [B,M,T]
+    f64 (device) -> selected try per box [B,M] i32 (-1: none)."""
+    B, M, T = _aug_inputs(gt_boxes, num_gt, valid, loc_noise, rot_noise)
+    if selected is None:
+        selected = torch.empty((B, M), dtype=torch.int32, device=gt_boxes.device)
+    _cuda(selected, torch.int32, "selected")
+    check(lib.sessd_noise_per_box(_p(gt_boxes), _p(num_gt), _p(valid), int(B), int(M), _p(loc_noise), _p(rot_noise), int(T),
+                                  float(context), _p(selected), _st()), "sessd_noise_per_box")
+    return selected
+
+
+def augment_points(points, frame_off, max_frame_points, gt_boxes, num_gt, valid, loc_noise, rot_noise, selected, glob, perm, labeled=None,
+                   context=-1.0, points_raw=None, points_out=None):
+    """per-object transform, raw twin, global flip / rotation / scaling and shuffle of a batch of frames (sessd_augment_points).
+    points [P,4] f32 (16-byte aligned rows), frame_off [B+1] i32, glob [B,5] f32 (cos, sin, scale, flip, angle), perm [P] i32 holding a
+    permutation of each frame's rows, labeled [B] u8 or None.  Returns (points_raw, points_out) [P,4] f32."""
+    B, M, T = _aug_inputs(gt_boxes, num_gt, valid, loc_noise, rot_noise, selected)
+    _cuda(points, torch.float32, "points"); _cuda(frame_off, torch.int32, "frame_off"); _cuda(glob, torch.float32, "glob")
+    _cuda(perm, torch.int32, "perm")
+    if labeled is not None:
+        _cuda(labeled, torch.uint8, "labeled")
+        if labeled.numel() != B:
+            raise ValueError("labeled must be [B]")
+    if points.dim() != 2 or points.shape[1] != 4 or frame_off.numel() != B + 1 or perm.numel() != points.shape[0] or tuple(glob.shape) != (B, 5):
+        raise ValueError("augment_points: shape mismatch")
+    if points_raw is None:
+        points_raw = torch.empty_like(points)
+    if points_out is None:
+        points_out = torch.empty_like(points)
+    for name, t in (("points_raw", points_raw), ("points_out", points_out)):
+        _cuda(t, torch.float32, name)
+        if t.shape != points.shape:
+            raise ValueError("%s must be shaped like points" % name)
+    if any(t.data_ptr() % 16 for t in (points, points_raw, points_out)):
+        raise ValueError("augment_points: point rows are read and written as float4 and must be 16-byte aligned")
+    check(lib.sessd_augment_points(_p(points), _p(frame_off), int(B), int(max_frame_points), _p(gt_boxes), _p(num_gt), _p(valid), int(M),
+                                   _p(loc_noise), _p(rot_noise), int(T), _p(selected), float(context), _p(glob), _p(perm), _p(labeled),
+                                   _p(points_raw), _p(points_out), _st()), "sessd_augment_points")
+    return points_raw, points_out
+
+
+def augment_boxes(gt_boxes, num_gt, valid, target, loc_noise, rot_noise, selected, glob, range_bev):
+    """box3d_transform_, valid-box selection, global stages and the Voxelization / AssignTarget bookkeeping (sessd_augment_boxes).
+    target: [B,M] u8 target-class mask or None (all); range_bev: host (x0, y0, x1, y1).  Returns (boxes_raw [B,M,7], num_raw [B],
+    boxes [B,M,7], num [B]) on the device."""
+    B, M, T = _aug_inputs(gt_boxes, num_gt, valid, loc_noise, rot_noise, selected)
+    _cuda(glob, torch.float32, "glob")
+    if tuple(glob.shape) != (B, 5):
+        raise ValueError("glob must be [B, 5]")
+    if target is not None:
+        _cuda(target, torch.uint8, "target")
+        if tuple(target.shape) != (B, M):
+            raise ValueError("target must be [B, M]")
+    dev = gt_boxes.device
+    boxes_raw = torch.empty((B, M, 7), dtype=torch.float32, device=dev)
+    boxes_out = torch.empty((B, M, 7), dtype=torch.float32, device=dev)
+    num_raw = torch.empty((B,), dtype=torch.int32, device=dev)
+    num_out = torch.empty((B,), dtype=torch.int32, device=dev)
+    rg = (C.c_float * 4)(*[float(v) for v in range_bev])
+    check(lib.sessd_augment_boxes(_p(gt_boxes), _p(num_gt), _p(valid), _p(target), int(B), int(M), _p(loc_noise), _p(rot_noise), int(T),
+                                  _p(selected), _p(glob), rg, _p(boxes_raw), _p(num_raw), _p(boxes_out), _p(num_out), _st()),
+          "sessd_augment_boxes")
+    return boxes_raw, num_raw, boxes_out, num_out

@@ -83,3 +83,14 @@ def random_boxes(seed, n=1000, spread=1.0):
     boxes = np.stack([x, y, z, w, l, h, r], 1).astype(np.float32)
     scores = rng.uniform(0.3, 1.0, n).astype(np.float32)
     return boxes, scores
+
+
+def ring_boxes(seed, n_cars=30):
+    """the [n_cars, 7] lidar boxes (x y z w l h r) of the cars ring_cloud(seed, n, n_cars) places: the first draws of its generator
+    (centres, yaw); the car's 3.9 m side lies along its own x axis, which is the box's l (along its y) turned by pi / 2"""
+    rng = np.random.default_rng(seed)
+    cx = rng.uniform(5.0, 65.0, n_cars)
+    cy = rng.uniform(-35.0, 35.0, n_cars)
+    yaw = rng.uniform(-np.pi, np.pi, n_cars)
+    z = np.full(n_cars, -1.73 + 1.56 / 2)
+    return np.stack([cx, cy, z, np.full(n_cars, 1.6), np.full(n_cars, 3.9), np.full(n_cars, 1.56), yaw - np.pi / 2], 1).astype(np.float32)
