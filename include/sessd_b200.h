@@ -408,6 +408,36 @@ int sessd_augment_boxes(const float *d_gt_boxes, const int *d_num_gt, const uint
                         int *d_num_out, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * GT-database sampling (GT-AUG) of the training frames (csrc/gtaug.cu, csrc/augment.cu).  Replaces DataBaseSamplerV2.sample_class_v2's
+ * acceptance (det3d/core/sampler/sample_ops_v2.py:238-276), the point half of sample_all (:133-150) and the paste of Preprocess.__call__
+ * (det3d/datasets/pipelines/preprocess.py:96-110).  Which objects each frame draws is decided on the host (sessd_b200/augment.py,
+ * det3d/core/sampler): the draws and the sampler's resets depend on every earlier frame.
+ * sessd_gtaug_select_host -- HOST buffers, synchronous, no device: h_corners [num_boxes + num_cand, 4, 2] fp64 = the BEV corners of
+ *     center_to_corner_box2d of [boxes so far | candidates] (candidates in sampler order); h_accepted [num_cand] u8 out: candidate c is
+ *     accepted when its corner set collides (box_collision_test, the predicate of sessd_box_collision) with no box, no accepted
+ *     candidate and no later candidate not yet rejected -- the loop of coll_mat[i].any() with rejected rows / columns cleared.  Returns
+ *     the number accepted (>= 0), SESSD_EINVAL for null pointers or negative counts.
+ * sessd_gtaug_paste -- device.  d_points [num_points, 4] f32 with d_frame_off [batch + 1] (the scene points); d_obj_off [batch + 1] i32 and
+ *     d_obj_ids [num_objects] i32: the accepted database objects per frame (CSR, acceptance order); the resident database: d_db_points
+ *     [*, 4] f32 (points relative to the box centre, as the database files hold them), d_db_off / d_db_count [db_size] i32 (first row and
+ *     row count of each object), d_db_boxes [db_size, 7] f64 (box3d_lidar: the centre added back and the box whose points are removed).
+ *     Output d_points_out [capacity, 4] with d_frame_off_out [batch + 1]: per frame, the pasted objects' points (fp32(rel + centre) in
+ *     fp64, acceptance order), then the scene points outside every pasted box (points_in_rbbox, origin 0.5: the fp64 membership frame
+ *     of sessd_points_in_boxes) in their original order.  max_paste_points: the host-known total row count of the accepted objects;
+ *     capacity < num_points + max_paste_points -> SESSD_ECAPACITY, workspace_bytes < sessd_gtaug_paste_workspace_bytes(...) ->
+ *     SESSD_EWORKSPACE.  d_points,
+ *     d_db_points and d_points_out are float4 rows and must be 16-byte aligned (SESSD_EINVAL otherwise).  An object id outside
+ *     [0, db_size) pastes no rows and removes no points (the ids are device memory, so it cannot be reported); no access is ever out of
+ *     bounds.  The new frame offsets stay on the device.
+ * ------------------------------------------------------------------------------------------------ */
+int sessd_gtaug_select_host(const double *h_corners, int num_boxes, int num_cand, uint8_t *h_accepted);
+size_t sessd_gtaug_paste_workspace_bytes(int batch, int num_points, int num_objects);
+int sessd_gtaug_paste(const float *d_points, const int *d_frame_off, int batch, int num_points, const int *d_obj_off, const int *d_obj_ids,
+                      int num_objects, int max_paste_points, const float *d_db_points, const int *d_db_off, const int *d_db_count,
+                      const double *d_db_boxes, int db_size, void *d_workspace, size_t workspace_bytes, float *d_points_out, int capacity,
+                      int *d_frame_off_out, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * SURVEY.md 8(f) row 1, first slice of the training step: the supervised SSD-head loss terms, value AND gradient in one pass.
  * Replaces (for the terms without the teacher model) det3d/models/bbox_heads/mg_head_sessd.py:706-760:
  * prepare_loss_weights/NormByNumPositives (:525-572), SigmoidFocalLoss (det3d/models/losses/losses.py:345-420, gamma = 2),

@@ -20,7 +20,9 @@ LAB = {"bevconv_split.cu"}
 OBJ = os.path.join(HERE, "build")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"] + os.environ.get("SESSD_DEFINES", "").split()
-NO_FMA = {"iou3d.cu", "postproc.cu", "assign.cu", "odiou.cu", "kitti_eval.cu", "augment.cu"}
+NO_FMA = {"iou3d.cu", "postproc.cu", "assign.cu", "odiou.cu", "kitti_eval.cu", "augment.cu", "gtaug.cu"}
+# files whose host code evaluates the collision predicate of csrc/augment.cuh: the host compiler must not contract it into fmas either
+HOST_NO_CONTRACT = {"augment.cu", "gtaug.cu"}
 
 
 def sources():
@@ -43,7 +45,8 @@ def build(force=False, verbose=False):
 
     def compile_one(src):
         obj = os.path.join(OBJ, src[:-3] + ".o")
-        cmd = [nvcc] + ARCH + COMMON + (["-fmad=false"] if src in NO_FMA else []) + ["-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [nvcc] + ARCH + COMMON + (["-fmad=false"] if src in NO_FMA else []) + \
+            (["-Xcompiler", "-ffp-contract=off"] if src in HOST_NO_CONTRACT else []) + ["-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             print(" ".join(cmd))
         subprocess.check_call(cmd)

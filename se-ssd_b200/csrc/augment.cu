@@ -27,15 +27,15 @@
 // augment_points_kernel: one thread per student row (frame = blockIdx.y): reads the permuted source point, finds the first valid box
 // holding it (box-frame test in fp64 against the frame's boxes in shared memory), applies the selected transform (writes the twin), then
 // the global stages.  augment_boxes_kernel: one CTA per frame, one thread per box.
-#include "common.cuh"
+// The collision predicate and the membership frame live in augment.cuh (shared with gtaug.cu); sessd_gtaug_select_host runs the same
+// predicate on the host (this file's host code is compiled with -ffp-contract=off, so it evaluates operation for operation like the device).
+#include "augment.cuh"
 
 namespace sessd {
 
 constexpr int kAugThreads = 256;
 constexpr int kAugMaxGt = 256;     // SESSD_AUGMENT_MAX_GT
 constexpr int kAugMaxTry = 128;    // SESSD_AUGMENT_MAX_TRY
-
-struct Quad { double x[4], y[4]; };
 
 // box2d_to_corner_jit of one (x, y, w, l, r): corners_norm (-.5,-.5) (-.5,.5) (.5,.5) (.5,-.5) times (w, l), rotated, plus the centre
 __device__ __forceinline__ Quad box_corners(double x, double y, double w, double l, double r) {
@@ -48,62 +48,6 @@ __device__ __forceinline__ Quad box_corners(double x, double y, double w, double
         q.x[k] = __dadd_rn(__fma_rn(cy, s, __dmul_rn(cx, c)), x);      // rot_mat_T = [[c, -s], [s, c]]
         q.y[k] = __dadd_rn(__fma_rn(cy, c, __dmul_rn(cx, -s)), y);
     }
-    return q;
-}
-
-// the containment loop of box_collision_test: vec = -(a[k] - a[k+1]) (clockwise); cross = vec.y (a[k].x - p.x) - vec.x (a[k].y - p.y);
-// a corner with cross >= 0 is not inside
-__device__ __forceinline__ bool quad_contains(const Quad &a, const Quad &p) {
-#pragma unroll
-    for (int l = 0; l < 4; ++l)
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const int k1 = (k + 1) & 3;
-            const double vx = -__dsub_rn(a.x[k], a.x[k1]), vy = -__dsub_rn(a.y[k], a.y[k1]);
-            double cross = __dmul_rn(vy, __dsub_rn(a.x[k], p.x[l]));
-            cross = __dsub_rn(cross, __dmul_rn(vx, __dsub_rn(a.y[k], p.y[l])));
-            if (cross >= 0.0) return false;
-        }
-    return true;
-}
-
-// box_collision_test for one (box, qbox) pair, clockwise = True, operation for operation
-__device__ bool quads_collide(const Quad &b, const Quad &q) {
-    double bx0 = b.x[0], bx1 = b.x[0], by0 = b.y[0], by1 = b.y[0], qx0 = q.x[0], qx1 = q.x[0], qy0 = q.y[0], qy1 = q.y[0];
-#pragma unroll
-    for (int k = 1; k < 4; ++k) {
-        bx0 = fmin(bx0, b.x[k]); bx1 = fmax(bx1, b.x[k]); by0 = fmin(by0, b.y[k]); by1 = fmax(by1, b.y[k]);
-        qx0 = fmin(qx0, q.x[k]); qx1 = fmax(qx1, q.x[k]); qy0 = fmin(qy0, q.y[k]); qy1 = fmax(qy1, q.y[k]);
-    }
-    const double iw = __dsub_rn(fmin(bx1, qx1), fmax(bx0, qx0));
-    if (!(iw > 0.0)) return false;
-    const double ih = __dsub_rn(fmin(by1, qy1), fmax(by0, qy0));
-    if (!(ih > 0.0)) return false;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const int k1 = (k + 1) & 3;
-        const double ax = b.x[k], ay = b.y[k], bbx = b.x[k1], bby = b.y[k1];
-#pragma unroll
-        for (int l = 0; l < 4; ++l) {
-            const int l1 = (l + 1) & 3;
-            const double cx = q.x[l], cy = q.y[l], dx = q.x[l1], dy = q.y[l1];
-            const bool acd = __dmul_rn(__dsub_rn(dy, ay), __dsub_rn(cx, ax)) > __dmul_rn(__dsub_rn(cy, ay), __dsub_rn(dx, ax));
-            const bool bcd = __dmul_rn(__dsub_rn(dy, bby), __dsub_rn(cx, bbx)) > __dmul_rn(__dsub_rn(cy, bby), __dsub_rn(dx, bbx));
-            if (acd != bcd) {
-                const bool abc = __dmul_rn(__dsub_rn(cy, ay), __dsub_rn(bbx, ax)) > __dmul_rn(__dsub_rn(bby, ay), __dsub_rn(cx, ax));
-                const bool abd = __dmul_rn(__dsub_rn(dy, ay), __dsub_rn(bbx, ax)) > __dmul_rn(__dsub_rn(bby, ay), __dsub_rn(dx, ax));
-                if (abc != abd) return true;
-            }
-        }
-    }
-    // box contains qbox, then qbox contains box (each corner of one strictly on the inner side of every edge of the other)
-    return quad_contains(b, q) || quad_contains(q, b);
-}
-
-__device__ __forceinline__ Quad load_quad(const double *p) {   // [4][2] (x, y)
-    Quad q;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) { q.x[k] = p[2 * k]; q.y[k] = p[2 * k + 1]; }
     return q;
 }
 
@@ -176,39 +120,10 @@ __global__ void __launch_bounds__(kAugThreads) noise_per_box_kernel(const float 
 }
 
 // ------------------------------------------------------------------------------------------------ points and boxes
-// Per-box constants of the point pass: the membership frame (fp64 of the pre-noise box, w / l enlarged by the context) and the
-// selected try's transform (zero when the try is -1: the reference still applies -c, R(0), +c, +0 to the points it holds).
-// The membership frame of one box: points_in_convex_polygon_3d_jit over the faces of center_to_corner_box3d(origin 0.5) holds the same
-// points as |R^T (p - c)| < dims / 2 everywhere except within rounding of a face; evaluated in fp64 from the fp32 box, w and l enlarged by
-// the context (noise_per_object_v4_'s offset[2:5]).  Shared by the point pass and sessd_points_in_boxes (GT-AUG's points_in_rbbox).
-struct MemberFrame {
-    float cx, cy, cz;
-    double mc, ms;             // cos / sin of the box angle
-    double hx, hy, hz;         // half extents
-};
-
-__device__ __forceinline__ MemberFrame member_frame(const float *p, double add) {
-    MemberFrame f;
-    f.cx = p[0]; f.cy = p[1]; f.cz = p[2];
-    const double r = (double)p[6];
-    f.mc = cos(r); f.ms = sin(r);
-    f.hx = __dmul_rn(__dadd_rn((double)p[3], add), 0.5); f.hy = __dmul_rn(__dadd_rn((double)p[4], add), 0.5);
-    f.hz = __dmul_rn((double)p[5], 0.5);
-    return f;
-}
-
-__device__ __forceinline__ bool in_frame(float x, float y, float z, const MemberFrame &f) {
-    const double dx = __dsub_rn((double)x, (double)f.cx), dy = __dsub_rn((double)y, (double)f.cy);
-    const double dz = __dsub_rn((double)z, (double)f.cz);
-    const double lx = __dsub_rn(__dmul_rn(dx, f.mc), __dmul_rn(dy, f.ms));
-    const double ly = __dadd_rn(__dmul_rn(dx, f.ms), __dmul_rn(dy, f.mc));
-    return fabs(lx) < f.hx && fabs(ly) < f.hy && fabs(dz) < f.hz;
-}
-
 // Per-box constants of the point pass: the membership frame of the pre-noise box and the selected try's transform (zero when the try
 // is -1: the reference still applies -c, R(0), +c, +0 to the points it holds).
 struct AugBox {
-    MemberFrame m;             // its centre is also the fp32 centre points_transform_ subtracts and adds
+    MemberFrame<float> m;             // its centre is also the fp32 centre points_transform_ subtracts and adds
     float rc, rs;              // fp32(cos / sin) of the selected try's angle (rot_mat_T of _rotation_matrix_3d_)
     int valid;
     double lx, ly, lz;         // selected try's translation (fp64, added before the fp32 store)
@@ -385,6 +300,28 @@ extern "C" int sessd_box_collision(const double *d_boxes, int n, const double *d
     const int blocks = (int)std::min<long long>(div_up(total, (long long)kAugThreads), 4096);
     SESSD_LAUNCH(box_collision_kernel, blocks, kAugThreads, 0, (cudaStream_t)stream, d_boxes, n, d_qboxes, k, d_out);
     return last_error();
+}
+
+// sample_class_v2's acceptance loop (sample_ops_v2.py:253-276) on the host: candidate i is rejected when its corner set collides with
+// any box, any accepted earlier candidate or any later candidate (coll_mat[i].any() over the full row, the diagonal and the rows /
+// columns of rejected candidates cleared); a rejected candidate blocks nothing afterwards.  Pairs are evaluated only where needed.
+extern "C" int sessd_gtaug_select_host(const double *h_corners, int num_boxes, int num_cand, uint8_t *h_accepted) {
+    if (!h_corners || !h_accepted || num_boxes < 0 || num_cand < 0) return SESSD_EINVAL;
+    const int n = num_boxes + num_cand;
+    int accepted = 0;
+    for (int c = 0; c < num_cand; ++c) h_accepted[c] = 1;       // undecided candidates still block (their column is set)
+    for (int c = 0; c < num_cand; ++c) {
+        const int i = num_boxes + c;
+        const Quad qi = load_quad(h_corners + 8 * (size_t)i);
+        bool hit = false;
+        for (int j = 0; j < n && !hit; ++j) {
+            if (j == i || (j >= num_boxes && !h_accepted[j - num_boxes])) continue;
+            hit = quads_collide(qi, load_quad(h_corners + 8 * (size_t)j));
+        }
+        h_accepted[c] = hit ? 0 : 1;
+        accepted += hit ? 0 : 1;
+    }
+    return accepted;
 }
 
 extern "C" int sessd_noise_per_box(const float *d_gt_boxes, const int *d_num_gt, const uint8_t *d_valid, int batch, int max_gt,

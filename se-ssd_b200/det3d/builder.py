@@ -34,3 +34,38 @@ def build_anchor_generator(anchor_config):
                                     match_threshold=anchor_config.matched_threshold,
                                     unmatch_threshold=anchor_config.unmatched_threshold, class_name=anchor_config.class_name)
     raise ValueError(" unknown anchor generator type")
+
+
+def build_db_preprocess(db_prep_config, logger=None):
+    """reference det3d/builder.py:67-77"""
+    from det3d.core.sampler import preprocess as prep
+    cfg = db_prep_config
+    if "filter_by_difficulty" in cfg:
+        return prep.DBFilterByDifficulty(cfg["filter_by_difficulty"], logger=logger)
+    elif "filter_by_min_num_points" in cfg:
+        return prep.DBFilterByMinNumPoint(cfg["filter_by_min_num_points"], logger=logger)
+    raise ValueError("unknown database prep type")
+
+
+def build_dbsampler(cfg, logger=None, random_state=None):
+    """reference det3d/builder.py:378-405: the filters in config order, the info pickle, DataBaseSamplerV2.  The database files are read
+    relative to the pickle's directory unless ``sample_all`` is given another root; random_state defaults to the np.random module.
+    ``global_random_rotation_range_per_object`` is read and ignored, as in sample_ops_v2."""
+    import os
+    import pickle
+
+    import numpy as np
+
+    from det3d.core.sampler import DataBasePreprocessor, DataBaseSamplerV2
+    prepors = [build_db_preprocess(c, logger=logger) for c in cfg["db_prep_steps"]]
+    grot_range = list(cfg["global_random_rotation_range_per_object"]) or None
+    if cfg["gt_aug_with_context"] > 0.0:
+        raise NotImplementedError("gt_aug_with_context > 0 is not supported (the SE-SSD car config does not use it)")
+    with open(cfg["db_info_path"], "rb") as f:
+        db_infos = pickle.load(f)
+    sampler = DataBaseSamplerV2(db_infos, cfg["sample_groups"], DataBasePreprocessor(prepors), cfg["rate"], grot_range, logger=logger,
+                                gt_random_drop=cfg["gt_random_drop"], gt_aug_with_context=cfg["gt_aug_with_context"],
+                                gt_aug_similar_type=cfg["gt_aug_similar_type"],
+                                random_state=np.random if random_state is None else random_state)
+    sampler.root_path = os.path.dirname(os.path.abspath(cfg["db_info_path"]))
+    return sampler

@@ -1,8 +1,9 @@
 """The two pipeline transforms that sit on the per-frame hot path (reference: det3d/datasets/pipelines/preprocess.py:178-232 and
 :235-358).  Transforms are ``(res, info) -> (res, info)``.  Dataset I/O and the reference's ``Preprocess`` are not registered here: the
 per-object noise, global flip / rotation / scaling, shuffle and teacher twin run on the device through ``sessd_b200.augment`` (its own entry
-point), and GT-database sampling (GT-AUG) and shape-aware augmentation (SA-DA) are not built -- the reference's ``Preprocess`` always runs
-both, so registering one without them would be a silent difference."""
+point), GT-database sampling (GT-AUG) runs there too when ``build_train_batch`` is given a ``db_sampler`` (det3d.core.sampler), and
+shape-aware augmentation (SA-DA) is not built -- the reference's ``Preprocess`` always runs it, so registering one without it would be a
+silent difference."""
 import numpy as np
 
 from det3d.builder import build_anchor_generator, build_box_coder, build_similarity_metric

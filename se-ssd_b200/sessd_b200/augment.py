@@ -6,10 +6,11 @@ Every random number is drawn on the host by ``draw_augmentation`` with a numpy `
 reference's order; the kernels of csrc/augment.cu are pure functions of the points, the boxes and those draws, so each stage is
 comparable with the reference's own function run on the same seed.
 
-Not built here (see DESIGN §7): GT-database sampling (GT-AUG, before the per-object noise) and shape-aware augmentation (SA-DA,
-``pyramid_augment_v0``, between the global scaling and the shuffle).  The reference's ``Preprocess`` always runs both, so this module
-registers no ``Preprocess`` pipeline; ``build_train_batch`` (the collated batch) and ``augment_batch`` (the augmented points and
-boxes) are their own entry points.
+GT-database sampling (GT-AUG, before the per-object noise) runs when ``build_train_batch`` is given a ``db_sampler``
+(det3d.core.sampler, csrc/gtaug.cu): selection on the host, the paste on the device.  Not built (see DESIGN §7): shape-aware
+augmentation (SA-DA, ``pyramid_augment_v0``, between the global scaling and the shuffle).  The reference's ``Preprocess`` always runs
+it, so this module registers no ``Preprocess`` pipeline; ``build_train_batch`` (the collated batch) and ``augment_batch`` (the augmented
+points and boxes) are their own entry points.
 """
 from dataclasses import dataclass, field
 
@@ -86,8 +87,8 @@ def draw_augmentation(rs, frames, cfg):
     (random_flip_v2), ``uniform`` for the global rotation and for the scale, then ``choice(arange(n), n, replace=False)`` (the shuffle,
     when shuffle_points).  Unlabelled frames: the shuffle first, then flip, rotation and scale.
 
-    GT-AUG (before the noise) and SA-DA (between the scaling and the shuffle) are not built and draw nothing, so a seeded stream matches
-    the reference stage by stage, not over the whole of its Preprocess (which runs both)."""
+    GT-AUG's draws (before the noise) come from the sampler (gtaug_batch interleaves them per frame); SA-DA (between the scaling and
+    the shuffle) is not built and draws nothing, so a seeded stream matches the reference's Preprocess without SA-DA."""
     out = Draws()
     loc_std = np.array(cfg.gt_loc_noise, dtype=np.float32)          # noise_per_object_v4_: np.array(center_noise_std, gt_boxes.dtype)
     for n, m, labeled in frames:
@@ -145,33 +146,24 @@ def _unpack(dev, layout):
     return out
 
 
-def augment_batch(cfg, clouds, gt_boxes, gt_names, draws, labeled=None, device="cuda"):
-    """Augment a batch of frames on the device.  clouds: per frame [N, 4] f32; gt_boxes: per frame [M, 7] (x y z w l h r); gt_names: per
-    frame [M] class names (DontCare / ignore already dropped, as Preprocess does first); draws: draw_augmentation's output for
-    (len(cloud), len(boxes), labeled) of every frame; labeled: per frame, None = all labelled.
-
-    Returns a dict of device tensors: ``points`` (the student's [P, 4]: noised, flipped, rotated, scaled, shuffled), ``points_raw``
-    (the teacher's twin: noised, unshuffled; an unlabelled frame's rows are its input), ``frame_off`` [B+1], ``gt_boxes`` / ``num_gt`` (the student's boxes after the range
-    filter) and ``gt_boxes_raw`` / ``num_gt_raw`` (the teacher's), both padded [B, max_gt, 7] with limit_period angles -- the layout
-    sessd_assign_targets reads --, ``selected`` [B, max_gt] (the try each box took, -1 none); and ``transformation`` (host list of dicts).
-    Launches on the current stream and never waits on the device."""
-    B = len(clouds)
+def _host_inputs(cfg, frame_sizes, gt_boxes, gt_names, draws, labeled):
+    """the host arrays of the augmentation: (None, frame_off), (boxes, num_gt, valid, target, loc, rot, glob, perm, labeled), sizes"""
+    B = len(frame_sizes)
     labeled = [True] * B if labeled is None else [bool(v) for v in labeled]
     ms = [len(b) if lab else 0 for b, lab in zip(gt_boxes, labeled)]
     max_gt = max([1] + ms)
     if max_gt > MAX_GT:
         raise ValueError("a frame has %d GT boxes > %d" % (max_gt, MAX_GT))
-    ns = [len(c) for c in clouds]
+    ns = [int(n) for n in frame_sizes]
     off = np.zeros(B + 1, np.int32)
     off[1:] = np.cumsum(ns)
-    pts = np.concatenate([np.asarray(c, np.float32).reshape(-1, 4) for c in clouds] + [np.zeros((0, 4), np.float32)])
     boxes = np.zeros((B, max_gt, 7), np.float32)
     valid = np.zeros((B, max_gt), np.uint8)
     target = np.zeros((B, max_gt), np.uint8)
     loc = np.zeros((B, max_gt, NUM_TRY, 3))
     rot = np.zeros((B, max_gt, NUM_TRY))
     glob = np.zeros((B, 5), np.float32)
-    perm = np.zeros(len(pts), np.int32)
+    perm = np.zeros(int(off[-1]), np.int32)
     for b in range(B):
         d = draws.frames[b]
         if len(d.perm) != ns[b] or d.loc.shape[0] != ms[b]:
@@ -189,9 +181,40 @@ def augment_batch(cfg, clouds, gt_boxes, gt_names, draws, labeled=None, device="
         perm[off[b]:off[b + 1]] = d.perm
     num_gt = np.array(ms, np.int32)
     lab = np.array(labeled, np.uint8)
-    buf, layout = _pack([pts, off, boxes, num_gt, valid, target, loc, rot, glob, perm, lab])
+    return (None, off), (boxes, num_gt, valid, target, loc, rot, glob, perm, lab), ns
+
+
+def augment_batch(cfg, clouds, gt_boxes, gt_names, draws, labeled=None, device="cuda"):
+    """Augment a batch of frames on the device.  clouds: per frame [N, 4] f32; gt_boxes: per frame [M, 7] (x y z w l h r); gt_names: per
+    frame [M] class names (DontCare / ignore already dropped, as Preprocess does first); draws: draw_augmentation's output for
+    (len(cloud), len(boxes), labeled) of every frame; labeled: per frame, None = all labelled.
+
+    Returns a dict of device tensors: ``points`` (the student's [P, 4]: noised, flipped, rotated, scaled, shuffled), ``points_raw``
+    (the teacher's twin: noised, unshuffled; an unlabelled frame's rows are its input), ``frame_off`` [B+1], ``gt_boxes`` / ``num_gt`` (the student's boxes after the range
+    filter) and ``gt_boxes_raw`` / ``num_gt_raw`` (the teacher's), both padded [B, max_gt, 7] with limit_period angles -- the layout
+    sessd_assign_targets reads --, ``selected`` [B, max_gt] (the try each box took, -1 none); and ``transformation`` (host list of dicts).
+    Launches on the current stream and never waits on the device."""
+    (_, off), rest, ns = _host_inputs(cfg, [len(c) for c in clouds], gt_boxes, gt_names, draws, labeled)
+    pts = np.concatenate([np.asarray(c, np.float32).reshape(-1, 4) for c in clouds] + [np.zeros((0, 4), np.float32)])
+    buf, layout = _pack([pts, off] + list(rest))
     dev = torch.from_numpy(buf).pin_memory().to(device, non_blocking=True)
-    d_pts, d_off, d_boxes, d_num, d_valid, d_target, d_loc, d_rot, d_glob, d_perm, d_lab = _unpack(dev, layout)
+    d = _unpack(dev, layout)
+    return _augment_device(cfg, d[0], d[1], ns, d[2:], draws, labeled)
+
+
+def augment_resident(cfg, d_points, d_frame_off, frame_sizes, gt_boxes, gt_names, draws, device="cuda"):
+    """augment_batch on points already on the device (labelled frames): d_points [P, 4] f32 (16-byte aligned rows) with d_frame_off
+    [B+1] i32, frame_sizes the host's copy of the frame sizes.  Only the boxes and the draws are uploaded (one copy)."""
+    _, rest, ns = _host_inputs(cfg, frame_sizes, gt_boxes, gt_names, draws, None)
+    buf, layout = _pack(list(rest))
+    dev = torch.from_numpy(buf).pin_memory().to(device, non_blocking=True)
+    return _augment_device(cfg, d_points, d_frame_off, ns, _unpack(dev, layout), draws, None)
+
+
+def _augment_device(cfg, d_pts, d_off, ns, rest, draws, labeled):
+    d_boxes, d_num, d_valid, d_target, d_loc, d_rot, d_glob, d_perm, d_lab = rest
+    B = len(ns)
+    labeled = [True] * B if labeled is None else [bool(v) for v in labeled]
     ctx = cfg.data_aug_with_context
     sel = ops.noise_per_box(d_boxes, d_num, d_valid, d_loc, d_rot, ctx)
     raw = None if all(labeled) else d_pts.clone()          # an unlabelled frame has no twin in the reference: its rows keep the input
@@ -200,7 +223,6 @@ def augment_batch(cfg, clouds, gt_boxes, gt_names, draws, labeled=None, device="
     boxes_raw, num_raw, boxes_out, num_out = ops.augment_boxes(d_boxes, d_num, d_valid, d_target, d_loc, d_rot, sel, d_glob, cfg.range_bev)
     return dict(points=out, points_raw=raw, frame_off=d_off, gt_boxes=boxes_out, num_gt=num_out, gt_boxes_raw=boxes_raw,
                 num_gt_raw=num_raw, selected=sel, transformation=draws.transformation())
-
 
 
 # ------------------------------------------------------------------------------------------------ collated training batch
@@ -259,17 +281,99 @@ class PendingBatch:
         return ex
 
 
-def launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda"):
-    """Everything of build_train_batch that runs on the device, launched without waiting on it: the draws (host), augment_batch, the
-    voxeliser on the student's points and on the twin, the target assigner on both box sets.  Returns a PendingBatch."""
+def gtaug_batch(cfg, clouds, gt_boxes, gt_names, rs, db_sampler, device="cuda"):
+    """GT-database sampling of a batch of labelled frames, then the augmentation draws, in the reference's stream order: per frame,
+    the sampler's draws (its shuffles when a class stream runs out) come before the frame's noise / global / shuffle draws, and the
+    shuffle is sized by the frame's point count after the paste.
+
+    Selection runs on the host (db_sampler.select); the paste runs on the device over the resident database (sessd_gtaug_paste).  The
+    host reads the pasted frame offsets back once, before drawing; when db_sampler draws from ``rs`` itself and a class stream has to be
+    reshuffled in a later frame, the frames before it are pasted and drawn first (one more read-back per reshuffle), so the stream
+    stays the reference's.  Returns (d_points [P', 4], d_frame_off [B+1], frame sizes, boxes per frame (gt then sampled, in their
+    dtype), names per frame, Draws, accepted ids per frame)."""
+    db = db_sampler.device_database(device)
+    B = len(clouds)
+    ns = [len(c) for c in clouds]
+    off = np.zeros(B + 1, np.int64)
+    off[1:] = np.cumsum(ns)
+    pts = np.concatenate([np.asarray(c, np.float32).reshape(-1, 4) for c in clouds] + [np.zeros((0, 4), np.float32)])
+    d_pts = torch.from_numpy(pts).pin_memory().to(device, non_blocking=True)
+    ids, boxes, names, frames, groups, pending = [], [], [], [], [], []
+
+    def flush():
+        if not pending:
+            return
+        f0, f1 = pending[0], pending[-1] + 1
+        obj_off = np.zeros(f1 - f0 + 1, np.int32)
+        obj_off[1:] = np.cumsum([len(ids[f]) for f in range(f0, f1)])
+        obj_ids = np.concatenate([ids[f] for f in range(f0, f1)] + [np.zeros(0, np.int64)]).astype(np.int32)
+        sub_off = torch.from_numpy((off[f0:f1 + 1] - off[f0]).astype(np.int32)).to(device)
+        out, fo = ops.gtaug_paste(d_pts[off[f0]:off[f1]], sub_off, obj_off, obj_ids, db["points"], db["off"], db["count"], db["boxes"],
+                                  int(db_sampler.counts[obj_ids].sum()))
+        sizes = np.diff(fo.cpu().numpy())                       # the read-back: each frame's point count after the paste
+        for f, n in zip(range(f0, f1), sizes):
+            frames.append((int(n), len(boxes[f]), True))
+            draws.frames += draw_augmentation(rs, [frames[-1]], cfg).frames
+        groups.append((out, int(sizes.sum())))
+        pending.clear()
+
+    draws = Draws()
+    shared = db_sampler._rs is rs
+    if shared:
+        db_sampler._set_random_state(_FlushOnShuffle(rs, flush))
+    try:
+        for b in range(B):
+            gb = np.asarray(gt_boxes[b]).reshape(-1, 7)
+            acc = db_sampler.select(gb, list(gt_names[b]))
+            ids.append(acc)
+            boxes.append(np.concatenate([gb, db_sampler.boxes[acc]]))
+            names.append(np.concatenate([np.asarray(gt_names[b], dtype=object), db_sampler.names[acc].astype(object)]))
+            pending.append(b)
+        flush()
+    finally:
+        if shared:
+            db_sampler._set_random_state(rs)
+    sizes = [f[0] for f in frames]
+    new_off = np.zeros(B + 1, np.int32)
+    new_off[1:] = np.cumsum(sizes)
+    # the frames' rows (the paste's buffer is sized by its capacity); several groups only when a stream was reshuffled mid-batch
+    d_points = groups[0][0][:groups[0][1]] if len(groups) == 1 else torch.cat([o[:n] for o, n in groups])
+    d_off = torch.from_numpy(new_off).to(device)
+    return d_points, d_off, sizes, boxes, names, draws, ids
+
+
+class _FlushOnShuffle:
+    """the RandomState a sampler sees inside gtaug_batch: before it reshuffles a stream, the frames selected so far are pasted and
+    their augmentation drawn (those draws precede the reshuffle in the reference's stream)"""
+
+    def __init__(self, rs, flush):
+        self._rs, self._flush = rs, flush
+
+    def shuffle(self, x):
+        self._flush()
+        self._rs.shuffle(x)
+
+
+def launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda", db_sampler=None):
+    """Everything of build_train_batch that runs on the device: the draws (host), augment_batch, the voxeliser on the student's points
+    and on the twin, the target assigner on both box sets.  Returns a PendingBatch.
+
+    Without db_sampler nothing waits on the device.  With db_sampler (a det3d.core.sampler DataBaseSamplerV2), GT-database sampling
+    runs first (gtaug_batch): it waits once on the pasted frame offsets before drawing the augmentation, because the shuffle is sized
+    by each frame's point count after the paste and the next frame's draws follow it in the stream."""
     if labeled is not None and not all(labeled):
         raise ValueError("build_train_batch builds labelled batches (the reference gives unlabelled frames no targets and no twin); "
                          "augment unlabelled frames with augment_batch(..., labeled=...)")
     st = _static(cfg, device)
     B = len(clouds)
-    draws = draw_augmentation(rs, [(len(c), len(b), True) for c, b in zip(clouds, gt_boxes)], st["aug"])
-    aug = augment_batch(st["aug"], clouds, gt_boxes, gt_names, draws, device=device)
-    total = int(sum(len(c) for c in clouds))
+    if db_sampler is None:
+        draws = draw_augmentation(rs, [(len(c), len(b), True) for c, b in zip(clouds, gt_boxes)], st["aug"])
+        aug = augment_batch(st["aug"], clouds, gt_boxes, gt_names, draws, device=device)
+        total = int(sum(len(c) for c in clouds))
+    else:
+        d_points, d_off, sizes, boxes, names, draws, _ = gtaug_batch(st["aug"], clouds, gt_boxes, gt_names, rs, db_sampler, device)
+        aug = augment_resident(st["aug"], d_points, d_off, sizes, boxes, names, draws, device)
+        total = int(sum(sizes))
     vox, vox_raw = (ops.VoxelBuffers(st["vcfg"], B, max(total, 1), device) for _ in range(2))
     ops.voxelize(aug["points"], aug["frame_off"], vox)
     ops.voxelize(aug["points_raw"], aug["frame_off"], vox_raw)
@@ -280,15 +384,18 @@ def launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device
     return PendingBatch(st, aug, vox, vox_raw, asg, asg_raw, B, aug["frame_off"], total)
 
 
-def build_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda"):
+def build_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda", db_sampler=None):
     """A collated SE-SSD training batch with real augmentation: the ``example`` dict batch_processor_inline takes, with the keys of
     ``synth.train_batch`` (voxels, coordinates with a batch column, num_points, num_voxels, shape, anchors, labels, reg_targets, their
     ``_raw`` twins for the teacher, points with a batch column, metadata, transformation), all tensors on the device.
 
     cfg: the loaded det3d Config (train_preprocessor, voxel_generator, train_cfg.assigner); clouds: per frame [N, 4] f32; gt_boxes /
     gt_names: per frame [M, 7] and [M] (DontCare / ignore dropped); rs: the numpy RandomState the draws come from (draw_augmentation).
-    The student's frame is noised, flipped, rotated, scaled and shuffled; the teacher's twin is the noised frame (Preprocess:131).
+    db_sampler: None, or the GT-database sampler (det3d.builder.build_dbsampler(cfg.db_sampler)): sampled objects are pasted into each
+    frame first, as Preprocess does.  The student's frame is noised, flipped, rotated, scaled and shuffled; the teacher's twin is the
+    noised frame (Preprocess:131).
 
-    The device work is launched without waiting (launch_train_batch); forming the dict then reads the two branches' voxel totals back
-    once, because the model consumes exact-count voxel tensors."""
-    return launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled, device).example()
+    Without db_sampler the device work is launched without waiting (launch_train_batch); with it, GT-AUG reads the pasted frame sizes
+    back once before drawing.  Forming the dict then reads the two branches' voxel totals back once, because the model consumes
+    exact-count voxel tensors."""
+    return launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled, device, db_sampler).example()

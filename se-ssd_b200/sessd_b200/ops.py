@@ -722,3 +722,62 @@ def augment_boxes(gt_boxes, num_gt, valid, target, loc_noise, rot_noise, selecte
                                   _p(selected), _p(glob), rg, _p(boxes_raw), _p(num_raw), _p(boxes_out), _p(num_out), _st()),
           "sessd_augment_boxes")
     return boxes_raw, num_raw, boxes_out, num_out
+
+
+def gtaug_select_host(corners, num_boxes):
+    """sample_class_v2's acceptance (sessd_gtaug_select_host): corners [num_boxes + K, 4, 2] fp64 (host, center_to_corner_box2d of
+    [boxes so far | candidates]) -> accepted mask [K] bool."""
+    corners = np.ascontiguousarray(corners, np.float64)
+    if corners.ndim != 3 or corners.shape[1:] != (4, 2) or not 0 <= num_boxes <= corners.shape[0]:
+        raise ValueError("gtaug_select_host: corners [num_boxes + K, 4, 2], 0 <= num_boxes <= rows")
+    k = corners.shape[0] - int(num_boxes)
+    acc = np.zeros(max(k, 1), np.uint8)
+    rc = lib.sessd_gtaug_select_host(corners.ctypes.data_as(C.c_void_p), int(num_boxes), int(k), acc.ctypes.data_as(C.c_void_p))
+    if rc < 0:
+        check(rc, "sessd_gtaug_select_host")
+    return acc[:k].astype(bool)
+
+
+def gtaug_paste(points, frame_off, obj_off, obj_ids, db_points, db_off, db_count, db_boxes, max_paste_points, out=None,
+                frame_off_out=None):
+    """Paste the accepted database objects into a batch of frames and drop the scene points inside them (sessd_gtaug_paste).
+    points [P,4] f32 with frame_off [B+1] i32; obj_off [B+1] / obj_ids [K] i32 (CSR, acceptance order); the resident database:
+    db_points [*,4] f32 (relative to the centre), db_off / db_count [N] i32, db_boxes [N,7] f64; max_paste_points: the host-known row
+    total of the accepted objects (sizes the output).  Returns (points_out [P + max_paste_points, 4] f32, frame_off_out [B+1] i32); the
+    rows past frame_off_out[B] are unused.  obj_off / obj_ids given as host numpy arrays are checked here (every id in [0, N), offsets
+    non-decreasing from 0 to K) and uploaded; given as device tensors they are not (an out-of-range id then pastes nothing and removes
+    nothing: the C entry cannot see it)."""
+    _cuda(points, torch.float32, "points"); _cuda(frame_off, torch.int32, "frame_off"); _cuda(db_points, torch.float32, "db_points")
+    _cuda(db_off, torch.int32, "db_off"); _cuda(db_count, torch.int32, "db_count"); _cuda(db_boxes, torch.float64, "db_boxes")
+    B = frame_off.numel() - 1
+    N = db_count.numel()
+    if isinstance(obj_ids, np.ndarray) or isinstance(obj_off, np.ndarray):
+        ids = np.asarray(obj_ids).reshape(-1); off = np.asarray(obj_off).reshape(-1)
+        if ids.size and (ids.min() < 0 or ids.max() >= N):
+            raise ValueError("gtaug_paste: object id out of range [0, %d)" % N)
+        if off.size != B + 1 or off[0] != 0 or off[-1] != ids.size or (np.diff(off) < 0).any():
+            raise ValueError("gtaug_paste: obj_off must be a CSR offset array [B+1] over the ids")
+        host = np.concatenate([off.astype(np.int32), ids.astype(np.int32)])
+        dev_ids = torch.from_numpy(host).to(points.device)
+        obj_off, obj_ids = dev_ids[:B + 1], dev_ids[B + 1:]
+    _cuda(obj_off, torch.int32, "obj_off"); _cuda(obj_ids, torch.int32, "obj_ids")
+    if (B < 1 or points.dim() != 2 or points.shape[1] != 4 or obj_off.numel() != B + 1 or db_points.dim() != 2 or db_points.shape[1] != 4
+            or db_off.numel() != N or tuple(db_boxes.shape) != (N, 7)):
+        raise ValueError("gtaug_paste: shape mismatch")
+    cap = int(points.shape[0]) + int(max_paste_points)
+    dev = points.device
+    if out is None:
+        out = torch.empty((max(cap, 1), 4), dtype=torch.float32, device=dev)
+    if frame_off_out is None:
+        frame_off_out = torch.empty((B + 1,), dtype=torch.int32, device=dev)
+    _cuda(out, torch.float32, "out"); _cuda(frame_off_out, torch.int32, "frame_off_out")
+    if out.dim() != 2 or out.shape[1] != 4 or frame_off_out.numel() != B + 1:
+        raise ValueError("gtaug_paste: out [capacity, 4], frame_off_out [B+1]")
+    if any(t.data_ptr() % 16 for t in (points, db_points, out)):
+        raise ValueError("gtaug_paste: point rows are read and written as float4 and must be 16-byte aligned")
+    K = obj_ids.numel()
+    ws = torch.empty((int(lib.sessd_gtaug_paste_workspace_bytes(B, int(points.shape[0]), K)),), dtype=torch.uint8, device=dev)
+    check(lib.sessd_gtaug_paste(_p(points), _p(frame_off), int(B), int(points.shape[0]), _p(obj_off), _p(obj_ids), int(K),
+                                int(max_paste_points), _p(db_points), _p(db_off), _p(db_count), _p(db_boxes), int(N), _p(ws),
+                                ws.numel(), _p(out), int(out.shape[0]), _p(frame_off_out), _st()), "sessd_gtaug_paste")
+    return out, frame_off_out
