@@ -438,6 +438,61 @@ int sessd_gtaug_paste(const float *d_points, const int *d_frame_off, int batch, 
                       int *d_frame_off_out, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Shape-aware data augmentation (SA-DA) of the training frames (csrc/sada.cu).  Replaces pyramid_augment_v0 and its helpers
+ * (det3d/datasets/utils/sa_da_v2.py): pyramid dropout, farthest-point sparsify and pyramid swap, one frame per call.  Every draw is made
+ * on the host (sessd_b200/sada.py); the entries are pure functions of the points, the pyramids and the lists of pyramids each stage
+ * acts on.  Points are [n, 4] f32 float4 rows and must be 16-byte aligned (SESSD_EINVAL otherwise).  All arithmetic is fp32 and
+ * individually rounded in the reference's order, except the distances of the farthest-point sampling (fp64).
+ * sessd_sada_student_boxes -- device.  The inputs of sessd_augment_boxes (without target and range); output d_boxes_out [batch, max_gt, 7]
+ *     f32: per frame, its class-valid boxes after the noise and the global stages, in index order, before the range filter and
+ *     limit_period (the boxes Preprocess hands to pyramid_augment_v0), zero padded; d_num_out [batch] their count.  max_gt <=
+ *     SESSD_AUGMENT_MAX_GT (SESSD_ECAPACITY above).
+ * sessd_sada_pyramids -- device.  d_boxes [num_boxes, 7] f32 -> d_pyramids [num_boxes * 6, 15] (get_pyramids: the box centre, then the
+ *     four corners of one face of center_to_corner_box3d(origin 0.5), faces box-major) and d_planes [num_boxes * 6, 5, 4] (normal and
+ *     offset of each of the 5 surfaces, as surface_equ_3d_jitv2 computes them).  num_boxes <= SESSD_AUGMENT_MAX_GT; the pointers are
+ *     required even when num_boxes is 0.
+ * sessd_sada_membership -- device.  For the pyramid list d_ids [num_ids] (indices into d_planes [num_pyramids, 5, 4]; num_ids <=
+ *     SESSD_SADA_MAX_IDS): d_bits [n, ceil(num_ids / 32)] u32 (optional, may be null) with bit a of point i set when the point lies
+ *     strictly inside pyramid d_ids[a] (points_in_convex_polygon_3d_jit: a surface sign >= 0 is outside), and d_counts [num_ids] the
+ *     number of points inside each.  An id outside [0, num_pyramids) holds no point.  Integer atomics only: deterministic.
+ * sessd_sada_compact -- device.  Writes the rows of d_points that lie in no listed pyramid a with d_counts[a] > min_count (min_count < 0:
+ *     every listed pyramid) to d_out in their order, and their number to d_num_out [1] (device).  capacity < n -> SESSD_ECAPACITY;
+ *     workspace_bytes < sessd_sada_compact_workspace_bytes(n) -> SESSD_EWORKSPACE.
+ * sessd_sada_fps -- device.  For each listed pyramid a with d_counts[a] > min_count, in list order: its points in row order, then k
+ *     rows by exact farthest-point sampling (start at its first point; each step the point with the largest fp64 distance
+ *     sqrt((dx^2 + dy^2) + dz^2) to its nearest picked point, ties to the first), written in pick order at d_out[*d_num + k * r], r =
+ *     the number of such pyramids before a; *d_num (device, in: rows already in d_out) is advanced by k per such pyramid.  Requires
+ *     min_count >= k - 1 (SESSD_EINVAL), capacity >= n + k * num_ids (SESSD_ECAPACITY) and sessd_sada_fps_workspace_bytes(n, num_ids)
+ *     (SESSD_EWORKSPACE).  A pyramid of up to 4096 points is sampled from shared memory, a larger one from the workspace.
+ * sessd_sada_swap -- device.  d_ids [2 * num_pairs]: to_swap pyramids, then their partners; d_bits / d_counts: sessd_sada_membership
+ *     of that list over d_points; d_pyramids [num_pyramids, 15].  Pair p writes, from row *d_num_in on (device) and after the pairs
+ *     before it, the partner's points in pyramid p's ratio coordinates (get_points_ratio / recover_points_by_ratio) with intensities
+ *     through the min / max ratio (clip(max - min, 1e-6, 1)), then pyramid p's points in the partner's coordinates; *d_num_out is
+ *     the frame's new size.  max_swap_points: the host-known sum of the listed counts; capacity < n + max_swap_points -> SESSD_ECAPACITY.
+ *     A pair with an id outside [0, num_pyramids) writes nothing.
+ * sessd_sada_shuffle -- device.  d_out[off_b + k] = d_points[off_b + d_perm[off_b + k]] for each frame b of d_frame_off [batch + 1];
+ *     a row whose source is outside its frame is left unwritten.
+ * ------------------------------------------------------------------------------------------------ */
+#define SESSD_SADA_MAX_IDS (6 * SESSD_AUGMENT_MAX_GT)
+int sessd_sada_student_boxes(const float *d_gt_boxes, const int *d_num_gt, const uint8_t *d_valid, int batch, int max_gt,
+                             const double *d_loc_noise, const double *d_rot_noise, int num_try, const int *d_selected, const float *d_global,
+                             float *d_boxes_out, int *d_num_out, void *stream);
+int sessd_sada_pyramids(const float *d_boxes, int num_boxes, float *d_pyramids, float *d_planes, void *stream);
+int sessd_sada_membership(const float *d_points, int n, const int *d_n, const float *d_planes, int num_pyramids, const int *d_ids, int num_ids,
+                          uint32_t *d_bits, int *d_counts, void *stream);
+size_t sessd_sada_compact_workspace_bytes(int n);
+int sessd_sada_compact(const float *d_points, int n, const int *d_n, const uint32_t *d_bits, int num_ids, const int *d_counts, int min_count,
+                       void *d_workspace, size_t workspace_bytes, float *d_out, int capacity, int *d_num_out, void *stream);
+size_t sessd_sada_fps_workspace_bytes(int n, int num_ids);
+int sessd_sada_fps(const float *d_points, int n, const int *d_n, const uint32_t *d_bits, int num_ids, const int *d_counts, int min_count, int k,
+                   void *d_workspace, size_t workspace_bytes, float *d_out, int capacity, int *d_num, void *stream);
+int sessd_sada_swap(const float *d_points, int n, const int *d_n, const uint32_t *d_bits, int num_pairs, const int *d_counts, const float *d_pyramids,
+                    int num_pyramids, const int *d_ids, int max_swap_points, float *d_out, int capacity, const int *d_num_in,
+                    int *d_num_out, void *stream);
+int sessd_sada_shuffle(const float *d_points, const int *d_frame_off, int batch, int max_frame_points, const int *d_perm, float *d_out,
+                       void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * SURVEY.md 8(f) row 1, first slice of the training step: the supervised SSD-head loss terms, value AND gradient in one pass.
  * Replaces (for the terms without the teacher model) det3d/models/bbox_heads/mg_head_sessd.py:706-760:
  * prepare_loss_weights/NormByNumPositives (:525-572), SigmoidFocalLoss (det3d/models/losses/losses.py:345-420, gamma = 2),

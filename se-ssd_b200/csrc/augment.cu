@@ -129,14 +129,6 @@ struct AugBox {
     double lx, ly, lz;         // selected try's translation (fp64, added before the fp32 store)
 };
 
-// the fp32 BLAS chain of `p @ [[c, -s, 0], [s, c, 0], [0, 0, 1]]` (1x3 @ 3x3 and N x 3 @ 3x3 gemm, see oracle/augment_ref.py)
-__device__ __forceinline__ void rot32(float &x, float &y, float &z, float c, float s) {
-    const float x0 = x, y0 = y, z0 = z;
-    x = __fmaf_rn(z0, 0.f, __fmaf_rn(y0, s, __fmul_rn(x0, c)));
-    y = __fmaf_rn(z0, 0.f, __fmaf_rn(y0, c, __fmul_rn(x0, -s)));
-    z = __fmaf_rn(z0, 1.f, __fmaf_rn(y0, 0.f, __fmul_rn(x0, 0.f)));
-}
-
 // random_flip_v2 -> global_rotation_v3 -> global_scaling_v3 on one point: g = {cos, sin, scale, flip, angle} (fp32, from the host)
 __device__ __forceinline__ void global32(float &x, float &y, float &z, const float *g) {
     if (g[3] != 0.f) y = -y;
@@ -228,25 +220,14 @@ __global__ void __launch_bounds__(kAugMaxGt) augment_boxes_kernel(
 #pragma unroll
         for (int c = 0; c < 7; ++c) v[c] = gt_boxes[bj * 7 + c];
         if (valid[bj]) {
-            const int t = selected[bj];
-            if (t >= 0) {
-                const double *l = loc_noise + (bj * num_try + t) * 3;
-                v[0] = (float)__dadd_rn((double)v[0], l[0]); v[1] = (float)__dadd_rn((double)v[1], l[1]);
-                v[2] = (float)__dadd_rn((double)v[2], l[2]);
-                v[6] = (float)__dadd_rn((double)v[6], rot_noise[bj * num_try + t]);
-            }
+            box_noise(v, loc_noise, rot_noise, num_try, bj, selected[bj]);
             keep_raw = target == nullptr || target[bj] != 0;
         }
     }
 #pragma unroll
     for (int c = 0; c < 7; ++c) w[c] = v[c];
     const float *g = global + 5 * (size_t)b;
-    const float kPi = 3.14159274101257324f;                  // float32(np.pi)
-    if (g[3] != 0.f) { w[1] = -w[1]; w[6] = __fadd_rn(-w[6], kPi); }
-    rot32(w[0], w[1], w[2], g[0], g[1]);
-    w[6] = __fadd_rn(w[6], g[4]);
-#pragma unroll
-    for (int c = 0; c < 6; ++c) w[c] = __fmul_rn(w[c], g[2]);
+    box_global(w, g);
     if (keep_raw) {
         const float s = sinf(w[6]), c = cosf(w[6]);
         const float nx[4] = {-0.5f, -0.5f, 0.5f, 0.5f}, ny[4] = {-0.5f, 0.5f, 0.5f, -0.5f};

@@ -101,4 +101,31 @@ __device__ __forceinline__ bool in_frame(float x, float y, float z, const Member
     return fabs(lx) < f.hx && fabs(ly) < f.hy && fabs(dz) < f.hz;
 }
 
+// the fp32 BLAS chain of `p @ [[c, -s, 0], [s, c, 0], [0, 0, 1]]` (1x3 @ 3x3 and N x 3 @ 3x3 gemm, see oracle/augment_ref.py)
+__device__ __forceinline__ void rot32(float &x, float &y, float &z, float c, float s) {
+    const float x0 = x, y0 = y, z0 = z;
+    x = __fmaf_rn(z0, 0.f, __fmaf_rn(y0, s, __fmul_rn(x0, c)));
+    y = __fmaf_rn(z0, 0.f, __fmaf_rn(y0, c, __fmul_rn(x0, -s)));
+    z = __fmaf_rn(z0, 1.f, __fmaf_rn(y0, 0.f, __fmul_rn(x0, 0.f)));
+}
+
+// box3d_transform_ of one valid box v [7] (fp32) by its selected try t (-1: unmoved): centre and angle plus the fp64 noise, rounded once
+__device__ __forceinline__ void box_noise(float *v, const double *loc_noise, const double *rot_noise, int num_try, size_t bj, int t) {
+    if (t < 0) return;
+    const double *l = loc_noise + (bj * num_try + t) * 3;
+    v[0] = (float)__dadd_rn((double)v[0], l[0]); v[1] = (float)__dadd_rn((double)v[1], l[1]);
+    v[2] = (float)__dadd_rn((double)v[2], l[2]);
+    v[6] = (float)__dadd_rn((double)v[6], rot_noise[bj * num_try + t]);
+}
+
+// random_flip_v2 -> global_rotation_v3 -> global_scaling_v3 on one box w [7]: g = {cos, sin, scale, flip, angle} (fp32, from the host)
+__device__ __forceinline__ void box_global(float *w, const float *g) {
+    const float kPi = 3.14159274101257324f;                  // float32(np.pi)
+    if (g[3] != 0.f) { w[1] = -w[1]; w[6] = __fadd_rn(-w[6], kPi); }
+    rot32(w[0], w[1], w[2], g[0], g[1]);
+    w[6] = __fadd_rn(w[6], g[4]);
+#pragma unroll
+    for (int c = 0; c < 6; ++c) w[c] = __fmul_rn(w[c], g[2]);
+}
+
 }  // namespace sessd

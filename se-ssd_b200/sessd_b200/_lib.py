@@ -125,6 +125,15 @@ SIGNATURES = {
     "sessd_gtaug_select_host": (_i, [_vp, _i, _i, _vp]),
     "sessd_gtaug_paste_workspace_bytes": (_sz, [_i, _i, _i]),
     "sessd_gtaug_paste": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _sz, _vp, _i, _vp, _vp]),
+    "sessd_sada_student_boxes": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    "sessd_sada_pyramids": (_i, [_vp, _i, _vp, _vp, _vp]),
+    "sessd_sada_membership": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
+    "sessd_sada_compact_workspace_bytes": (_sz, [_i]),
+    "sessd_sada_compact": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _vp, _sz, _vp, _i, _vp, _vp]),
+    "sessd_sada_fps_workspace_bytes": (_sz, [_i, _i]),
+    "sessd_sada_fps": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _i, _vp, _sz, _vp, _i, _vp, _vp]),
+    "sessd_sada_swap": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _vp]),
+    "sessd_sada_shuffle": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
     "sessd_kitti_convert_workspace_bytes": (_sz, [_ll]),
     "sessd_kitti_convert_detections": (_i, [_vp, _vp, _vp, _vp, _i, _ll, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "sessd_kitti_overlaps": (_i, [C.POINTER(KittiFrames), _i, _i, C.c_double, _vp, _vp]),

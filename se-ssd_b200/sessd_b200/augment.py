@@ -7,10 +7,10 @@ reference's order; the kernels of csrc/augment.cu are pure functions of the poin
 comparable with the reference's own function run on the same seed.
 
 GT-database sampling (GT-AUG, before the per-object noise) runs when ``build_train_batch`` is given a ``db_sampler``
-(det3d.core.sampler, csrc/gtaug.cu): selection on the host, the paste on the device.  Not built (see DESIGN §7): shape-aware
-augmentation (SA-DA, ``pyramid_augment_v0``, between the global scaling and the shuffle).  The reference's ``Preprocess`` always runs
-it, so this module registers no ``Preprocess`` pipeline; ``build_train_batch`` (the collated batch) and ``augment_batch`` (the augmented
-points and boxes) are their own entry points.
+(det3d.core.sampler, csrc/gtaug.cu): selection on the host, the paste on the device.  Shape-aware augmentation (SA-DA,
+``pyramid_augment_v0``, between the global scaling and the shuffle) runs when it is given ``sa_da`` (sessd_b200.sada, csrc/sada.cu).  No
+``Preprocess`` pipeline is registered; ``build_train_batch`` (the collated batch) and ``augment_batch`` (the augmented points and boxes)
+are their own entry points.
 """
 from dataclasses import dataclass, field
 
@@ -87,16 +87,14 @@ def draw_augmentation(rs, frames, cfg):
     (random_flip_v2), ``uniform`` for the global rotation and for the scale, then ``choice(arange(n), n, replace=False)`` (the shuffle,
     when shuffle_points).  Unlabelled frames: the shuffle first, then flip, rotation and scale.
 
-    GT-AUG's draws (before the noise) come from the sampler (gtaug_batch interleaves them per frame); SA-DA (between the scaling and
-    the shuffle) is not built and draws nothing, so a seeded stream matches the reference's Preprocess without SA-DA."""
+    GT-AUG's draws (before the noise) come from the sampler (gtaug_batch interleaves them per frame).  SA-DA's draws (between the
+    scaling and the shuffle) depend on the frame's device results, so they are not made here: this is the reference's Preprocess
+    stream without SA-DA; launch_train_batch(sa_da=SadaConfig()) interleaves them frame by frame (sessd_b200.sada)."""
     out = Draws()
-    loc_std = np.array(cfg.gt_loc_noise, dtype=np.float32)          # noise_per_object_v4_: np.array(center_noise_std, gt_boxes.dtype)
     for n, m, labeled in frames:
         n, m = int(n), int(m)
         if labeled:
-            loc = rs.normal(scale=loc_std, size=[m, NUM_TRY, 3])
-            rot = rs.uniform(cfg.gt_rot_noise[0], cfg.gt_rot_noise[1], size=[m, NUM_TRY])
-            flip, rotation, scale = _global_draws(rs, cfg)
+            loc, rot, flip, rotation, scale = _labeled_draws(rs, m, cfg)
             perm = _shuffle(rs, n, cfg)
         else:
             loc, rot = np.zeros((0, NUM_TRY, 3)), np.zeros((0, NUM_TRY))
@@ -104,6 +102,14 @@ def draw_augmentation(rs, frames, cfg):
             flip, rotation, scale = _global_draws(rs, cfg)
         out.frames.append(FrameDraws(loc, rot, flip, rotation, scale, perm))
     return out
+
+
+def _labeled_draws(rs, m, cfg):
+    """a labelled frame's draws before SA-DA and the shuffle: the per-object noise, then flip, rotation and scale"""
+    loc_std = np.array(cfg.gt_loc_noise, dtype=np.float32)          # noise_per_object_v4_: np.array(center_noise_std, gt_boxes.dtype)
+    loc = rs.normal(scale=loc_std, size=[m, NUM_TRY, 3])
+    rot = rs.uniform(cfg.gt_rot_noise[0], cfg.gt_rot_noise[1], size=[m, NUM_TRY])
+    return (loc, rot) + _global_draws(rs, cfg)
 
 
 def _global_draws(rs, cfg):
@@ -202,16 +208,17 @@ def augment_batch(cfg, clouds, gt_boxes, gt_names, draws, labeled=None, device="
     return _augment_device(cfg, d[0], d[1], ns, d[2:], draws, labeled)
 
 
-def augment_resident(cfg, d_points, d_frame_off, frame_sizes, gt_boxes, gt_names, draws, device="cuda"):
+def augment_resident(cfg, d_points, d_frame_off, frame_sizes, gt_boxes, gt_names, draws, device="cuda", student_boxes=False):
     """augment_batch on points already on the device (labelled frames): d_points [P, 4] f32 (16-byte aligned rows) with d_frame_off
-    [B+1] i32, frame_sizes the host's copy of the frame sizes.  Only the boxes and the draws are uploaded (one copy)."""
+    [B+1] i32, frame_sizes the host's copy of the frame sizes.  Only the boxes and the draws are uploaded (one copy).  student_boxes:
+    also return ``sada_boxes`` [B, max_gt, 7], each frame's class-valid boxes after the global stages (sessd_sada_student_boxes)."""
     _, rest, ns = _host_inputs(cfg, frame_sizes, gt_boxes, gt_names, draws, None)
     buf, layout = _pack(list(rest))
     dev = torch.from_numpy(buf).pin_memory().to(device, non_blocking=True)
-    return _augment_device(cfg, d_points, d_frame_off, ns, _unpack(dev, layout), draws, None)
+    return _augment_device(cfg, d_points, d_frame_off, ns, _unpack(dev, layout), draws, None, student_boxes)
 
 
-def _augment_device(cfg, d_pts, d_off, ns, rest, draws, labeled):
+def _augment_device(cfg, d_pts, d_off, ns, rest, draws, labeled, student_boxes=False):
     d_boxes, d_num, d_valid, d_target, d_loc, d_rot, d_glob, d_perm, d_lab = rest
     B = len(ns)
     labeled = [True] * B if labeled is None else [bool(v) for v in labeled]
@@ -221,8 +228,11 @@ def _augment_device(cfg, d_pts, d_off, ns, rest, draws, labeled):
     raw, out = ops.augment_points(d_pts, d_off, max(ns + [0]), d_boxes, d_num, d_valid, d_loc, d_rot, sel, d_glob, d_perm, d_lab, ctx,
                                   points_raw=raw)
     boxes_raw, num_raw, boxes_out, num_out = ops.augment_boxes(d_boxes, d_num, d_valid, d_target, d_loc, d_rot, sel, d_glob, cfg.range_bev)
-    return dict(points=out, points_raw=raw, frame_off=d_off, gt_boxes=boxes_out, num_gt=num_out, gt_boxes_raw=boxes_raw,
-                num_gt_raw=num_raw, selected=sel, transformation=draws.transformation())
+    res = dict(points=out, points_raw=raw, frame_off=d_off, gt_boxes=boxes_out, num_gt=num_out, gt_boxes_raw=boxes_raw,
+               num_gt_raw=num_raw, selected=sel, transformation=draws.transformation())
+    if student_boxes:                                       # the boxes SA-DA takes (sessd_b200.sada)
+        res["sada_boxes"] = ops.sada_student_boxes(d_boxes, d_num, d_valid, d_loc, d_rot, sel, d_glob)[0]
+    return res
 
 
 # ------------------------------------------------------------------------------------------------ collated training batch
@@ -281,7 +291,7 @@ class PendingBatch:
         return ex
 
 
-def gtaug_batch(cfg, clouds, gt_boxes, gt_names, rs, db_sampler, device="cuda"):
+def gtaug_batch(cfg, clouds, gt_boxes, gt_names, rs, db_sampler, device="cuda", frame_hook=None):
     """GT-database sampling of a batch of labelled frames, then the augmentation draws, in the reference's stream order: per frame,
     the sampler's draws (its shuffles when a class stream runs out) come before the frame's noise / global / shuffle draws, and the
     shuffle is sized by the frame's point count after the paste.
@@ -290,7 +300,10 @@ def gtaug_batch(cfg, clouds, gt_boxes, gt_names, rs, db_sampler, device="cuda"):
     host reads the pasted frame offsets back once, before drawing; when db_sampler draws from ``rs`` itself and a class stream has to be
     reshuffled in a later frame, the frames before it are pasted and drawn first (one more read-back per reshuffle), so the stream
     stays the reference's.  Returns (d_points [P', 4], d_frame_off [B+1], frame sizes, boxes per frame (gt then sampled, in their
-    dtype), names per frame, Draws, accepted ids per frame)."""
+    dtype), names per frame, Draws, accepted ids per frame).
+
+    frame_hook: None, or f(frame, d_frame_points, size, boxes, names) -> FrameDraws, called for each pasted frame in stream order in
+    place of draw_augmentation (the SA-DA path runs the frame's device stages there)."""
     db = db_sampler.device_database(device)
     B = len(clouds)
     ns = [len(c) for c in clouds]
@@ -310,10 +323,15 @@ def gtaug_batch(cfg, clouds, gt_boxes, gt_names, rs, db_sampler, device="cuda"):
         sub_off = torch.from_numpy((off[f0:f1 + 1] - off[f0]).astype(np.int32)).to(device)
         out, fo = ops.gtaug_paste(d_pts[off[f0]:off[f1]], sub_off, obj_off, obj_ids, db["points"], db["off"], db["count"], db["boxes"],
                                   int(db_sampler.counts[obj_ids].sum()))
-        sizes = np.diff(fo.cpu().numpy())                       # the read-back: each frame's point count after the paste
+        fo = fo.cpu().numpy()                                   # the read-back: each frame's point count after the paste
+        sizes = np.diff(fo)
         for f, n in zip(range(f0, f1), sizes):
             frames.append((int(n), len(boxes[f]), True))
-            draws.frames += draw_augmentation(rs, [frames[-1]], cfg).frames
+            if frame_hook is None:
+                draws.frames += draw_augmentation(rs, [frames[-1]], cfg).frames
+            else:
+                r0 = int(fo[f - f0])
+                draws.frames.append(frame_hook(f, out[r0:r0 + int(n)], int(n), boxes[f], names[f]))
         groups.append((out, int(sizes.sum())))
         pending.clear()
 
@@ -354,29 +372,99 @@ class _FlushOnShuffle:
         self._rs.shuffle(x)
 
 
-def launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda", db_sampler=None):
+class _SadaFrames:
+    """The SA-DA path of a batch, one labelled frame at a time in the reference's stream order (Preprocess.__call__:113-161): the
+    frame's noise and global draws, its device stages (augment_resident on its rows, perm = identity), its SA-DA (sessd_b200.sada:
+    draws, at most one read-back of the swap counts), one read-back of its new size, then its shuffle draw.  ``assemble`` joins the
+    frames into augment_batch's layout and shuffles them with one gather."""
+
+    def __init__(self, cfg, sa_da, rs, device):
+        self.cfg, self.sa_da, self.rs, self.device = cfg, sa_da, rs, device
+        self.frames = []
+
+    def __call__(self, f, d_points, n, boxes, names):
+        from . import sada
+        cfg, rs = self.cfg, self.rs
+        loc, rot, flip, rotation, scale = _labeled_draws(rs, len(boxes), cfg)
+        fd = FrameDraws(loc, rot, flip, rotation, scale, np.arange(n))
+        d_off = torch.tensor([0, n], dtype=torch.int32).to(self.device)
+        aug = augment_resident(cfg, d_points, d_off, [n], [boxes], [names], Draws([fd]), self.device, student_boxes=True)
+        k = sum(1 for nm in names if nm in cfg.class_names)
+        out, num = sada.sada_frame(aug["points"], aug["sada_boxes"][0], k, rs, self.sa_da)
+        size = int(num.item())                                  # the read-back: the shuffle is sized by the frame after SA-DA
+        fd.perm = _shuffle(rs, size, cfg)
+        self.frames.append((out[:size], aug, fd))
+        return fd
+
+    def assemble(self):
+        B = len(self.frames)
+        dev = self.frames[0][1]["points_raw"].device
+        sizes = [len(o) for o, _, _ in self.frames]
+        raw_sizes = [len(a["points_raw"]) for _, a, _ in self.frames]
+        off = np.zeros(B + 1, np.int32); off[1:] = np.cumsum(sizes)
+        raw_off = np.zeros(B + 1, np.int32); raw_off[1:] = np.cumsum(raw_sizes)
+        perm = np.concatenate([fd.perm for _, _, fd in self.frames] + [np.zeros(0, np.int64)]).astype(np.int32)
+        host = torch.from_numpy(np.concatenate([off, raw_off, perm])).to(dev)
+        d_off, d_raw_off, d_perm = host[:B + 1], host[B + 1:2 * B + 2], host[2 * B + 2:]
+        pts = torch.cat([o for o, _, _ in self.frames] + [torch.empty((0, 4), dtype=torch.float32, device=dev)])
+        points = ops.sada_shuffle(pts, d_off, max(sizes + [0]), d_perm) if len(pts) else pts
+        M = max([1] + [a["gt_boxes"].shape[1] for _, a, _ in self.frames])
+        res = dict(points=points, points_raw=torch.cat([a["points_raw"] for _, a, _ in self.frames]), frame_off=d_off,
+                   frame_off_raw=d_raw_off, transformation=Draws([fd for _, _, fd in self.frames]).transformation())
+        for key, num_key in (("gt_boxes", "num_gt"), ("gt_boxes_raw", "num_gt_raw")):
+            bx = torch.zeros((B, M, 7), dtype=torch.float32, device=dev)
+            for b, (_, a, _) in enumerate(self.frames):
+                bx[b, :a[key].shape[1]] = a[key][0]
+            res[key] = bx
+            res[num_key] = torch.cat([a[num_key] for _, a, _ in self.frames])
+        sel = torch.full((B, M), -1, dtype=torch.int32, device=dev)
+        for b, (_, a, _) in enumerate(self.frames):
+            sel[b, :a["selected"].shape[1]] = a["selected"][0]
+        res["selected"] = sel
+        return res, int(off[-1]), int(raw_off[-1])
+
+
+def launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda", db_sampler=None, sa_da=None):
     """Everything of build_train_batch that runs on the device: the draws (host), augment_batch, the voxeliser on the student's points
     and on the twin, the target assigner on both box sets.  Returns a PendingBatch.
 
     Without db_sampler nothing waits on the device.  With db_sampler (a det3d.core.sampler DataBaseSamplerV2), GT-database sampling
     runs first (gtaug_batch): it waits once on the pasted frame offsets before drawing the augmentation, because the shuffle is sized
-    by each frame's point count after the paste and the next frame's draws follow it in the stream."""
+    by each frame's point count after the paste and the next frame's draws follow it in the stream.
+
+    sa_da: None, or a sessd_b200.sada.SadaConfig: shape-aware augmentation runs between the global scaling and the shuffle, as
+    Preprocess does.  Its draws depend on each frame's device results, so the frames are then built one at a time (_SadaFrames): per
+    frame it waits on the device once for the swap counts, only when a box is swap-selected, and once for the frame's size before the
+    shuffle draw.  The voxelisations and assignments then run batched."""
     if labeled is not None and not all(labeled):
         raise ValueError("build_train_batch builds labelled batches (the reference gives unlabelled frames no targets and no twin); "
                          "augment unlabelled frames with augment_batch(..., labeled=...)")
     st = _static(cfg, device)
     B = len(clouds)
-    if db_sampler is None:
+    if sa_da is not None:
+        frames = _SadaFrames(st["aug"], sa_da, rs, device)
+        if db_sampler is None:
+            pts = np.concatenate([np.asarray(c, np.float32).reshape(-1, 4) for c in clouds] + [np.zeros((0, 4), np.float32)])
+            d_pts = torch.from_numpy(pts).pin_memory().to(device, non_blocking=True)
+            r0 = 0
+            for b in range(B):
+                frames(b, d_pts[r0:r0 + len(clouds[b])], len(clouds[b]), np.asarray(gt_boxes[b]).reshape(-1, 7), list(gt_names[b]))
+                r0 += len(clouds[b])
+        else:
+            gtaug_batch(st["aug"], clouds, gt_boxes, gt_names, rs, db_sampler, device, frame_hook=frames)
+        aug, total, total_raw = frames.assemble()
+    elif db_sampler is None:
         draws = draw_augmentation(rs, [(len(c), len(b), True) for c, b in zip(clouds, gt_boxes)], st["aug"])
         aug = augment_batch(st["aug"], clouds, gt_boxes, gt_names, draws, device=device)
-        total = int(sum(len(c) for c in clouds))
+        total = total_raw = int(sum(len(c) for c in clouds))
     else:
         d_points, d_off, sizes, boxes, names, draws, _ = gtaug_batch(st["aug"], clouds, gt_boxes, gt_names, rs, db_sampler, device)
         aug = augment_resident(st["aug"], d_points, d_off, sizes, boxes, names, draws, device)
-        total = int(sum(sizes))
-    vox, vox_raw = (ops.VoxelBuffers(st["vcfg"], B, max(total, 1), device) for _ in range(2))
+        total = total_raw = int(sum(sizes))
+    vox = ops.VoxelBuffers(st["vcfg"], B, max(total, 1), device)
+    vox_raw = ops.VoxelBuffers(st["vcfg"], B, max(total_raw, 1), device)
     ops.voxelize(aug["points"], aug["frame_off"], vox)
-    ops.voxelize(aug["points_raw"], aug["frame_off"], vox_raw)
+    ops.voxelize(aug["points_raw"], aug.get("frame_off_raw", aug["frame_off"]), vox_raw)
     A = st["anchors"].shape[0]
     asg, asg_raw = (ops.AssignBuffers(A, B, aug["gt_boxes"].shape[1], device) for _ in range(2))
     ops.assign_targets(st["anchors"], aug["gt_boxes"], aug["num_gt"], asg, *st["thr"])
@@ -384,7 +472,7 @@ def launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device
     return PendingBatch(st, aug, vox, vox_raw, asg, asg_raw, B, aug["frame_off"], total)
 
 
-def build_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda", db_sampler=None):
+def build_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda", db_sampler=None, sa_da=None):
     """A collated SE-SSD training batch with real augmentation: the ``example`` dict batch_processor_inline takes, with the keys of
     ``synth.train_batch`` (voxels, coordinates with a batch column, num_points, num_voxels, shape, anchors, labels, reg_targets, their
     ``_raw`` twins for the teacher, points with a batch column, metadata, transformation), all tensors on the device.
@@ -395,7 +483,10 @@ def build_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device=
     frame first, as Preprocess does.  The student's frame is noised, flipped, rotated, scaled and shuffled; the teacher's twin is the
     noised frame (Preprocess:131).
 
-    Without db_sampler the device work is launched without waiting (launch_train_batch); with it, GT-AUG reads the pasted frame sizes
-    back once before drawing.  Forming the dict then reads the two branches' voxel totals back once, because the model consumes
-    exact-count voxel tensors."""
-    return launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled, device, db_sampler).example()
+    sa_da: None, or a sessd_b200.sada.SadaConfig (its defaults are the car values Preprocess passes): shape-aware augmentation of the
+    student's frame between the global scaling and the shuffle.  It leaves the boxes and the teacher's twin as they are.
+
+    Without db_sampler and sa_da the device work is launched without waiting (launch_train_batch); with a db_sampler, GT-AUG reads the
+    pasted frame sizes back once before drawing; with sa_da, each frame waits on the device once or twice (see launch_train_batch).
+    Forming the dict then reads the two branches' voxel totals back once, because the model consumes exact-count voxel tensors."""
+    return launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled, device, db_sampler, sa_da).example()

@@ -781,3 +781,137 @@ def gtaug_paste(points, frame_off, obj_off, obj_ids, db_points, db_off, db_count
                                 int(max_paste_points), _p(db_points), _p(db_off), _p(db_count), _p(db_boxes), int(N), _p(ws),
                                 ws.numel(), _p(out), int(out.shape[0]), _p(frame_off_out), _st()), "sessd_gtaug_paste")
     return out, frame_off_out
+
+
+# ------------------------------------------------------------------------------------------------ shape-aware augmentation (SA-DA)
+SADA_MAX_IDS = 6 * 256                 # SESSD_SADA_MAX_IDS
+
+
+def _rows4(points, name):
+    _cuda(points, torch.float32, name)
+    if points.dim() != 2 or points.shape[1] != 4:
+        raise ValueError("%s must be [N, 4]" % name)
+    if points.data_ptr() % 16:
+        raise ValueError("%s: point rows are read and written as float4 and must be 16-byte aligned" % name)
+    return points
+
+
+def _count(d_n, name="n"):
+    if d_n is not None:
+        _cuda(d_n, torch.int32, name)
+        if d_n.numel() < 1:
+            raise ValueError("%s must hold one count" % name)
+    return d_n
+
+
+def _ids(ids, num_pyramids, device):
+    """a pyramid list: host ids are checked against [0, num_pyramids) and uploaded; device ids are taken as they are"""
+    if not isinstance(ids, torch.Tensor):
+        ids = np.asarray(ids, np.int64).reshape(-1)
+        if ids.size and (ids.min() < 0 or ids.max() >= num_pyramids):
+            raise ValueError("pyramid id out of range [0, %d)" % num_pyramids)
+        if ids.size > SADA_MAX_IDS:
+            raise ValueError("at most %d listed pyramids" % SADA_MAX_IDS)
+        ids = torch.from_numpy(ids.astype(np.int32)).to(device)
+    return _cuda(ids, torch.int32, "ids")
+
+
+def sada_student_boxes(gt_boxes, num_gt, valid, loc_noise, rot_noise, selected, glob):
+    """the class-valid boxes of each frame after the noise and the global stages, before the range filter and limit_period
+    (sessd_sada_student_boxes): the inputs of augment_boxes -> (boxes [B,M,7] f32 compacted, num [B] i32)"""
+    B, M, T = _aug_inputs(gt_boxes, num_gt, valid, loc_noise, rot_noise, selected)
+    _cuda(glob, torch.float32, "glob")
+    if tuple(glob.shape) != (B, 5):
+        raise ValueError("glob must be [B, 5]")
+    boxes = torch.empty((B, M, 7), dtype=torch.float32, device=gt_boxes.device)
+    num = torch.empty((B,), dtype=torch.int32, device=gt_boxes.device)
+    check(lib.sessd_sada_student_boxes(_p(gt_boxes), _p(num_gt), _p(valid), int(B), int(M), _p(loc_noise), _p(rot_noise), int(T),
+                                       _p(selected), _p(glob), _p(boxes), _p(num), _st()), "sessd_sada_student_boxes")
+    return boxes, num
+
+
+def sada_pyramids(boxes):
+    """get_pyramids and their face planes (sessd_sada_pyramids): boxes [K,7] f32 -> (pyramids [6K,15], planes [6K,5,4]) f32"""
+    _cuda(boxes, torch.float32, "boxes")
+    if boxes.dim() != 2 or boxes.shape[1] != 7:
+        raise ValueError("sada_pyramids: boxes [K, 7]")
+    K = boxes.shape[0]
+    pyr = torch.empty((6 * K, 15), dtype=torch.float32, device=boxes.device)
+    planes = torch.empty((6 * K, 5, 4), dtype=torch.float32, device=boxes.device)
+    if K == 0:
+        return pyr, planes
+    check(lib.sessd_sada_pyramids(_p(boxes), int(K), _p(pyr), _p(planes), _st()), "sessd_sada_pyramids")
+    return pyr, planes
+
+
+def sada_membership(points, planes, ids, n=None, with_bits=True):
+    """points_in_pyramids_mask over a pyramid list (sessd_sada_membership): points [N,4] f32, planes [P,5,4] f32, ids [A] (host ids are
+    range-checked), n: optional device row count.  Returns (bits [N, ceil(A/32)] i32 or None, counts [A] i32, ids on the device)."""
+    _rows4(points, "points"); _cuda(planes, torch.float32, "planes"); _count(n)
+    if planes.dim() != 3 or tuple(planes.shape[1:]) != (5, 4):
+        raise ValueError("planes must be [P, 5, 4]")
+    dev = points.device
+    ids = _ids(ids, planes.shape[0], dev)
+    A, N = ids.numel(), points.shape[0]
+    bits = torch.empty((N, max(-(-A // 32), 1)), dtype=torch.int32, device=dev) if with_bits else None
+    counts = torch.zeros((max(A, 1),), dtype=torch.int32, device=dev)
+    check(lib.sessd_sada_membership(_p(points), int(N), _p(n), _p(planes), int(planes.shape[0]), _p(ids), int(A), _p(bits), _p(counts),
+                                    _st()), "sessd_sada_membership")
+    return bits, counts[:A], ids
+
+
+def sada_compact(points, bits, counts, min_count=-1, n=None, out=None):
+    """the rows of points in no listed pyramid whose count exceeds min_count, in order (sessd_sada_compact).  Returns (out [N,4],
+    num [1] i32 on the device)."""
+    _rows4(points, "points"); _cuda(bits, torch.int32, "bits"); _cuda(counts, torch.int32, "counts"); _count(n)
+    N, A = points.shape[0], counts.numel()
+    if bits.shape[0] != N or bits.shape[1] * 32 < A:
+        raise ValueError("sada_compact: bits [N, ceil(A / 32)]")
+    dev = points.device
+    out = _rows4(torch.empty((max(N, 1), 4), dtype=torch.float32, device=dev) if out is None else out, "out")
+    num = torch.empty((1,), dtype=torch.int32, device=dev)
+    ws = torch.empty((max(int(lib.sessd_sada_compact_workspace_bytes(int(N))), 16),), dtype=torch.uint8, device=dev)
+    check(lib.sessd_sada_compact(_p(points), int(N), _p(n), _p(bits), int(A), _p(counts), int(min_count), _p(ws), ws.numel(), _p(out),
+                                 int(out.shape[0]), _p(num), _st()), "sessd_sada_compact")
+    return out, num
+
+
+def sada_fps(points, bits, counts, min_count, k, out, num, n=None):
+    """farthest-point sampling of every listed pyramid whose count exceeds min_count (sessd_sada_fps): k rows each, written after the
+    num[0] rows already in out (capacity >= N + k * A); num is advanced on the device."""
+    _rows4(points, "points"); _cuda(bits, torch.int32, "bits"); _cuda(counts, torch.int32, "counts"); _rows4(out, "out")
+    _count(num, "num"); _count(n)
+    N, A = points.shape[0], counts.numel()
+    if bits.shape[0] != N or bits.shape[1] * 32 < A:
+        raise ValueError("sada_fps: bits [N, ceil(A / 32)]")
+    ws = torch.empty((max(int(lib.sessd_sada_fps_workspace_bytes(int(N), int(A))), 16),), dtype=torch.uint8, device=points.device)
+    check(lib.sessd_sada_fps(_p(points), int(N), _p(n), _p(bits), int(A), _p(counts), int(min_count), int(k), _p(ws), ws.numel(), _p(out),
+                             int(out.shape[0]), _p(num), _st()), "sessd_sada_fps")
+    return out, num
+
+
+def sada_swap(points, bits, counts, pyramids, ids, max_swap_points, out, num_in, n=None):
+    """the pyramid swap of sessd_sada_swap: ids [2 * pairs] (to_swap, then partners) with bits / counts from sada_membership of that
+    list; out already holds num_in[0] kept rows and has room for N + max_swap_points.  Returns (out, num_out [1] i32)."""
+    _rows4(points, "points"); _cuda(bits, torch.int32, "bits"); _cuda(counts, torch.int32, "counts"); _rows4(out, "out")
+    _cuda(pyramids, torch.float32, "pyramids"); _cuda(ids, torch.int32, "ids"); _count(num_in, "num_in"); _count(n)
+    N, A = points.shape[0], ids.numel()
+    if A % 2 or counts.numel() != A or bits.shape[0] != N or bits.shape[1] * 32 < A or pyramids.dim() != 2 or pyramids.shape[1] != 15:
+        raise ValueError("sada_swap: shape mismatch")
+    num_out = torch.empty((1,), dtype=torch.int32, device=points.device)
+    check(lib.sessd_sada_swap(_p(points), int(N), _p(n), _p(bits), int(A // 2), _p(counts), _p(pyramids), int(pyramids.shape[0]), _p(ids),
+                              int(max_swap_points), _p(out), int(out.shape[0]), _p(num_in), _p(num_out), _st()), "sessd_sada_swap")
+    return out, num_out
+
+
+def sada_shuffle(points, frame_off, max_frame_points, perm, out=None):
+    """out[off_b + k] = points[off_b + perm[off_b + k]] per frame (sessd_sada_shuffle); perm [P] i32 frame-local"""
+    _rows4(points, "points"); _cuda(frame_off, torch.int32, "frame_off"); _cuda(perm, torch.int32, "perm")
+    if perm.numel() != points.shape[0]:
+        raise ValueError("sada_shuffle: perm [P]")
+    out = _rows4(torch.empty_like(points) if out is None else out, "out")
+    if out.shape != points.shape:
+        raise ValueError("sada_shuffle: out must be shaped like points")
+    check(lib.sessd_sada_shuffle(_p(points), _p(frame_off), int(frame_off.numel() - 1), int(max_frame_points), _p(perm), _p(out), _st()),
+          "sessd_sada_shuffle")
+    return out
