@@ -391,7 +391,11 @@ int sessd_noise_per_box(const float *d_gt_boxes, const int *d_num_gt, const uint
  *     Voxelization / AssignTarget (pipelines/preprocess.py:200-205, :290-330): both sets keep the boxes that are valid and in d_target
  *     (u8 [batch, max_gt], nullable: all), the student's set also drops the boxes with no BEV corner strictly inside range_bev (HOST
  *     float[4] x0 y0 x1 y1, filter_gt_box_outside_range); angles -> limit_period(r, 0.5, 2 pi); compacted in index order into
- *     d_boxes_raw / d_boxes_out [batch, max_gt, 7] (zero padded) with d_num_raw / d_num_out [batch]: the layout sessd_assign_targets reads. */
+ *     d_boxes_raw / d_boxes_out [batch, max_gt, 7] (zero padded) with d_num_raw / d_num_out [batch]: the layout sessd_assign_targets reads.
+ *     d_boxes_global [batch, max_gt, 7] f32 with d_num_global [batch] (nullable, both or neither: one without the other ->
+ *     SESSD_EINVAL; d_boxes_global may be null when max_gt is 0): per frame, its class-valid boxes after the noise and the global
+ *     stages, in index order, before the range filter and limit_period (the boxes Preprocess hands to pyramid_augment_v0), zero
+ *     padded, with their count. */
 /* sessd_points_in_boxes -- points_in_rbbox / points_in_convex_polygon_3d_jit over center_to_corner_box3d(origin 0.5) faces, as the
  *     point pass tests membership and as GT-AUG's point removal needs it: d_mask [n, m] u8 = point i (d_points rows of point_stride floats,
  *     x y z first) inside box j of d_boxes [m, 7] f32, w and l enlarged by context when it is positive.  The test is |R^T (p - c)| < dims/2
@@ -405,7 +409,7 @@ int sessd_augment_points(const float *d_points, const int *d_frame_off, int batc
 int sessd_augment_boxes(const float *d_gt_boxes, const int *d_num_gt, const uint8_t *d_valid, const uint8_t *d_target, int batch,
                         int max_gt, const double *d_loc_noise, const double *d_rot_noise, int num_try, const int *d_selected,
                         const float *d_global, const float *range_bev, float *d_boxes_raw, int *d_num_raw, float *d_boxes_out,
-                        int *d_num_out, void *stream);
+                        int *d_num_out, float *d_boxes_global, int *d_num_global, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * GT-database sampling (GT-AUG) of the training frames (csrc/gtaug.cu, csrc/augment.cu).  Replaces DataBaseSamplerV2.sample_class_v2's
@@ -442,11 +446,8 @@ int sessd_gtaug_paste(const float *d_points, const int *d_frame_off, int batch, 
  * (det3d/datasets/utils/sa_da_v2.py): pyramid dropout, farthest-point sparsify and pyramid swap, one frame per call.  Every draw is made
  * on the host (sessd_b200/sada.py); the entries are pure functions of the points, the pyramids and the lists of pyramids each stage
  * acts on.  Points are [n, 4] f32 float4 rows and must be 16-byte aligned (SESSD_EINVAL otherwise).  All arithmetic is fp32 and
- * individually rounded in the reference's order, except the distances of the farthest-point sampling (fp64).
- * sessd_sada_student_boxes -- device.  The inputs of sessd_augment_boxes (without target and range); output d_boxes_out [batch, max_gt, 7]
- *     f32: per frame, its class-valid boxes after the noise and the global stages, in index order, before the range filter and
- *     limit_period (the boxes Preprocess hands to pyramid_augment_v0), zero padded; d_num_out [batch] their count.  max_gt <=
- *     SESSD_AUGMENT_MAX_GT (SESSD_ECAPACITY above).
+ * individually rounded in the reference's order, except the distances of the farthest-point sampling (fp64).  The boxes SA-DA acts on
+ * are sessd_augment_boxes's d_boxes_global.
  * sessd_sada_pyramids -- device.  d_boxes [num_boxes, 7] f32 -> d_pyramids [num_boxes * 6, 15] (get_pyramids: the box centre, then the
  *     four corners of one face of center_to_corner_box3d(origin 0.5), faces box-major) and d_planes [num_boxes * 6, 5, 4] (normal and
  *     offset of each of the 5 surfaces, as surface_equ_3d_jitv2 computes them).  num_boxes <= SESSD_AUGMENT_MAX_GT; the pointers are
@@ -474,9 +475,6 @@ int sessd_gtaug_paste(const float *d_points, const int *d_frame_off, int batch, 
  *     a row whose source is outside its frame is left unwritten.
  * ------------------------------------------------------------------------------------------------ */
 #define SESSD_SADA_MAX_IDS (6 * SESSD_AUGMENT_MAX_GT)
-int sessd_sada_student_boxes(const float *d_gt_boxes, const int *d_num_gt, const uint8_t *d_valid, int batch, int max_gt,
-                             const double *d_loc_noise, const double *d_rot_noise, int num_try, const int *d_selected, const float *d_global,
-                             float *d_boxes_out, int *d_num_out, void *stream);
 int sessd_sada_pyramids(const float *d_boxes, int num_boxes, float *d_pyramids, float *d_planes, void *stream);
 int sessd_sada_membership(const float *d_points, int n, const int *d_n, const float *d_planes, int num_pyramids, const int *d_ids, int num_ids,
                           uint32_t *d_bits, int *d_counts, void *stream);

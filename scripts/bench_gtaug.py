@@ -2,7 +2,7 @@
 (2 cars and a pedestrian, so every frame asks the sampler for 13 cars), on a synthetic car database.  Prints one JSON object with the
 card's name and power limit (read in the same run), the database size, and, from CUDA events after warm-up (median, min, max):
   * build_train_batch_ms / build_train_batch_gtaug_ms: sessd_b200.augment.build_train_batch without and with db_sampler;
-  * paste_ms: ops.gtaug_paste on resident inputs (the five kernels of csrc/gtaug.cu plus the wrapper);
+  * paste_ms: ops.gtaug_paste on resident inputs (the kernels of csrc/gtaug.cu and its survivor scan, plus the wrapper);
   * select_host_ms: DataBaseSamplerV2.select for the 8 frames (host, perf_counter);
   * oracle_paste_host_ms: the ORACLE's numpy paste (oracle/gt_aug_ref.py paste: gather + point removal) of the same 8 frames on this
     machine's CPU -- a stand-in for the reference's host path, which is not measured here.

@@ -205,17 +205,19 @@ __global__ void __launch_bounds__(kAugThreads) points_in_boxes_kernel(const floa
 // box3d_transform_ (valid boxes), the valid-box selection and the raw copy, the global stages, then the bookkeeping of
 // Voxelization / AssignTarget: the student's boxes lose those with no BEV corner strictly inside range[4] (filter_gt_box_outside_range,
 // fp32 corners as the host mirror forms them); both sets keep the target-class boxes, get limit_period(r, 0.5, 2 pi) and are compacted.
+// boxes_global (optional): every valid box after the global stages, compacted before the range filter and limit_period (SA-DA's boxes).
 __global__ void __launch_bounds__(kAugMaxGt) augment_boxes_kernel(
     const float *__restrict__ gt_boxes, const int *__restrict__ num_gt, const uint8_t *__restrict__ valid, const uint8_t *__restrict__ target,
     int max_gt, const double *__restrict__ loc_noise, const double *__restrict__ rot_noise, int num_try, const int *__restrict__ selected,
     const float *__restrict__ global, float rx0, float ry0, float rx1, float ry1, float *__restrict__ boxes_raw, int *__restrict__ num_raw,
-    float *__restrict__ boxes_out, int *__restrict__ num_out) {
-    __shared__ unsigned char s_keep_raw[kAugMaxGt], s_keep_out[kAugMaxGt];
+    float *__restrict__ boxes_out, int *__restrict__ num_out, float *__restrict__ boxes_global, int *__restrict__ num_global) {
+    __shared__ unsigned char s_keep_raw[kAugMaxGt], s_keep_out[kAugMaxGt], s_keep_glob[kAugMaxGt];
     const int b = blockIdx.x, j = threadIdx.x;
     const int n = min(max(num_gt[b], 0), max_gt);
     const size_t bj = (size_t)b * max_gt + j;
     float v[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, w[7];
     bool keep_raw = false, keep_out = false;
+    const bool keep_glob = j < n && valid[bj];
     if (j < n) {
 #pragma unroll
         for (int c = 0; c < 7; ++c) v[c] = gt_boxes[bj * 7 + c];
@@ -239,12 +241,21 @@ __global__ void __launch_bounds__(kAugMaxGt) augment_boxes_kernel(
             keep_out |= x > rx0 && x < rx1 && y > ry0 && y < ry1;
         }
     }
-    s_keep_raw[j] = keep_raw; s_keep_out[j] = keep_out;
+    s_keep_raw[j] = keep_raw; s_keep_out[j] = keep_out; s_keep_glob[j] = keep_glob;
     __syncthreads();
-    int pos_raw = 0, pos_out = 0, tot_raw = 0, tot_out = 0;
+    int pos_raw = 0, pos_out = 0, pos_glob = 0, tot_raw = 0, tot_out = 0, tot_glob = 0;
     for (int i = 0; i < max_gt; ++i) {
-        pos_raw += (i < j) & s_keep_raw[i]; pos_out += (i < j) & s_keep_out[i];
-        tot_raw += s_keep_raw[i]; tot_out += s_keep_out[i];
+        pos_raw += (i < j) & s_keep_raw[i]; pos_out += (i < j) & s_keep_out[i]; pos_glob += (i < j) & s_keep_glob[i];
+        tot_raw += s_keep_raw[i]; tot_out += s_keep_out[i]; tot_glob += s_keep_glob[i];
+    }
+    if (boxes_global) {                                       // an invalid box's w is its unnoised global box: the padding is zeros
+        float *glob = boxes_global + (size_t)b * max_gt * 7;
+#pragma unroll
+        for (int c = 0; c < 7; ++c) {
+            if (keep_glob) glob[pos_glob * 7 + c] = w[c];
+            if (j >= tot_glob) glob[j * 7 + c] = 0.f;
+        }
+        if (j == 0) num_global[b] = tot_glob;
     }
     // limit_period(r, 0.5, 2 pi) in fp32 (the period is a Python float: numpy keeps the fp32 array's type)
     const float kTwoPi = 6.28318548202514648f;
@@ -347,20 +358,23 @@ extern "C" int sessd_augment_points(const float *d_points, const int *d_frame_of
 extern "C" int sessd_augment_boxes(const float *d_gt_boxes, const int *d_num_gt, const uint8_t *d_valid, const uint8_t *d_target, int batch,
                                    int max_gt, const double *d_loc_noise, const double *d_rot_noise, int num_try, const int *d_selected,
                                    const float *d_global, const float *range_bev, float *d_boxes_raw, int *d_num_raw, float *d_boxes_out,
-                                   int *d_num_out, void *stream) {
+                                   int *d_num_out, float *d_boxes_global, int *d_num_global, void *stream) {
     if (batch <= 0 || max_gt < 0 || num_try <= 0) return SESSD_EINVAL;
     if (!d_num_gt || !d_global || !range_bev || !d_num_raw || !d_num_out) return SESSD_EINVAL;
-    if (max_gt > 0 && (!d_gt_boxes || !d_valid || !d_loc_noise || !d_rot_noise || !d_selected || !d_boxes_raw || !d_boxes_out))
+    if (d_boxes_global && !d_num_global) return SESSD_EINVAL;
+    if (max_gt > 0 && (!d_gt_boxes || !d_valid || !d_loc_noise || !d_rot_noise || !d_selected || !d_boxes_raw || !d_boxes_out ||
+                       (d_num_global && !d_boxes_global)))
         return SESSD_EINVAL;
     if (max_gt > kAugMaxGt || num_try > kAugMaxTry) return SESSD_ECAPACITY;
     cudaStream_t st = (cudaStream_t)stream;
     if (max_gt == 0) {
         SESSD_CUDA_TRY(cudaMemsetAsync(d_num_raw, 0, sizeof(int) * batch, st));
         SESSD_CUDA_TRY(cudaMemsetAsync(d_num_out, 0, sizeof(int) * batch, st));
+        if (d_num_global) SESSD_CUDA_TRY(cudaMemsetAsync(d_num_global, 0, sizeof(int) * batch, st));
         return SESSD_OK;
     }
     SESSD_LAUNCH(augment_boxes_kernel, batch, max_gt, 0, st, d_gt_boxes, d_num_gt, d_valid, d_target, max_gt, d_loc_noise, d_rot_noise,
                  num_try, d_selected, d_global, range_bev[0], range_bev[1], range_bev[2], range_bev[3], d_boxes_raw, d_num_raw, d_boxes_out,
-                 d_num_out);
+                 d_num_out, d_boxes_global, d_num_global);
     return last_error();
 }

@@ -49,6 +49,17 @@ static inline int persistent_grid(long long work_items, int block, int ctas_per_
     return (int)(need < cap ? need : cap);
 }
 
+// the frame that owns row i of a batch with non-decreasing offsets off [batch + 1]: the largest b < batch with off[b] <= i (0 when none),
+// so an empty frame never owns a row
+__device__ __forceinline__ int find_frame(const int *__restrict__ off, int batch, int i) {
+    int lo = 0, hi = batch;   // off[lo] <= i < off[hi]
+    while (hi - lo > 1) {
+        int mid = (lo + hi) >> 1;
+        if (i >= off[mid]) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
 // ---------------------------------------------------------------------------------------------
 // 64-bit open-addressing hash: slot = key << 24 | value (value < 2^24), empty = all ones.
 // Used by the voxeliser (value = first point index, atomicMin) and the level-0 coordinate index
@@ -100,7 +111,8 @@ __device__ __forceinline__ int hash_lookup(const unsigned long long *__restrict_
 // ---------------------------------------------------------------------------------------------
 // Device-wide exclusive scan of 32-bit counts (three launches, no spin-waits => nothing can hang).
 //   pass 1: per-tile reduce, pass 2: one CTA scans the tile sums, pass 3: per-tile scan + offset.
-// The item count lives in device memory (d_n; nullptr => the host constant n_mul); launches are sized from the capacity.
+// The item count lives in device memory (d_n; nullptr => the host constant n_mul); launches are sized from the capacity, and every
+// kernel clamps the count to [0, capacity], so a device count past the buffer never reads or writes past it.
 // `Load` is a functor int(long long i).  out[i] = sum_{j<i} load(j); out[n] = total.
 // ---------------------------------------------------------------------------------------------
 constexpr int kScanThreads = 256;
@@ -135,11 +147,16 @@ __device__ __forceinline__ int block_excl_scan(int v, int *smem /*>= 9 ints*/, i
     return res;
 }
 
+__device__ __forceinline__ long long scan_count(const int *d_n, long long n_mul, long long cap) {
+    const long long n = d_n ? (long long)(*d_n) * n_mul : n_mul;
+    return n < 0 ? 0 : (n < cap ? n : cap);
+}
+
 template <class Load>
 __global__ void __launch_bounds__(kScanThreads) scan_reduce_kernel(Load load, const int *__restrict__ d_n,
-                                                                   long long n_mul, int *__restrict__ tile_sums) {
+                                                                   long long n_mul, long long cap, int *__restrict__ tile_sums) {
     __shared__ int sm[40];
-    const long long n = d_n ? (long long)(*d_n) * n_mul : n_mul;
+    const long long n = scan_count(d_n, n_mul, cap);
     const long long base = (long long)blockIdx.x * kScanTile;
     if (base >= n) return;
     int s = 0;
@@ -153,11 +170,11 @@ __global__ void __launch_bounds__(kScanThreads) scan_reduce_kernel(Load load, co
     if (threadIdx.x == 0) tile_sums[blockIdx.x] = tot;
 }
 
-static __global__ void __launch_bounds__(1024) scan_tiles_kernel(const int *__restrict__ d_n, long long n_mul,
+static __global__ void __launch_bounds__(1024) scan_tiles_kernel(const int *__restrict__ d_n, long long n_mul, long long cap,
                                                           int *__restrict__ tile_sums, int *__restrict__ d_total) {
     __shared__ int sm[40];
     __shared__ int carry;
-    const long long n = d_n ? (long long)(*d_n) * n_mul : n_mul;
+    const long long n = scan_count(d_n, n_mul, cap);
     const int tiles = (int)((n + kScanTile - 1) / kScanTile);
     if (threadIdx.x == 0) carry = 0;
     __syncthreads();
@@ -178,9 +195,10 @@ static __global__ void __launch_bounds__(1024) scan_tiles_kernel(const int *__re
 // hundred ints) -- saves the one-CTA scan_tiles launch for mid-sized inputs (two launches instead of three); the last tile writes the total.
 template <class Load, class Store, bool SELF_PREFIX>
 __global__ void __launch_bounds__(kScanThreads) scan_apply_kernel(Load load, Store store, const int *__restrict__ d_n,
-                                                                  long long n_mul, const int *__restrict__ tile_sums, int *__restrict__ d_total) {
+                                                                  long long n_mul, long long cap, const int *__restrict__ tile_sums,
+                                                                  int *__restrict__ d_total) {
     __shared__ int sm[40];
-    const long long n = d_n ? (long long)(*d_n) * n_mul : n_mul;
+    const long long n = scan_count(d_n, n_mul, cap);
     const long long base = (long long)blockIdx.x * kScanTile;
     if (SELF_PREFIX && n <= 0 && blockIdx.x == 0 && threadIdx.x == 0 && d_total) *d_total = 0;
     if (base >= n) return;
@@ -223,9 +241,9 @@ constexpr long long kScanSmallMax = 16 * 1024;          // capacity (items) up t
 
 template <class Load, class Store>
 __global__ void __launch_bounds__(kScanSmallThreads) scan_small_kernel(Load load, Store store, const int *__restrict__ d_n, long long n_mul,
-                                                                       int *__restrict__ d_total) {
+                                                                       long long cap, int *__restrict__ d_total) {
     __shared__ int sm[40];
-    const long long n = d_n ? (long long)(*d_n) * n_mul : n_mul;
+    const long long n = scan_count(d_n, n_mul, cap);
     int carry = 0;
     for (long long base = 0; base < n; base += (long long)kScanSmallThreads * kScanItems) {
         int v[kScanItems];
@@ -255,18 +273,20 @@ template <class Load, class Store>
 static inline void device_scan(Load load, Store store, const int *d_n, long long n_mul, long long cap_items,
                                int *scratch, int *d_total, cudaStream_t st) {
     if (cap_items <= kScanSmallMax) {
-        SESSD_LAUNCH((scan_small_kernel<Load, Store>), 1, kScanSmallThreads, 0, st, load, store, d_n, n_mul, d_total);
+        SESSD_LAUNCH((scan_small_kernel<Load, Store>), 1, kScanSmallThreads, 0, st, load, store, d_n, n_mul, cap_items, d_total);
         return;
     }
     int tiles = (int)((cap_items + kScanTile - 1) / kScanTile);
     if (tiles < 1) tiles = 1;
-    SESSD_LAUNCH((scan_reduce_kernel<Load>), tiles, kScanThreads, 0, st, load, d_n, n_mul, scratch);
+    SESSD_LAUNCH((scan_reduce_kernel<Load>), tiles, kScanThreads, 0, st, load, d_n, n_mul, cap_items, scratch);
     if (tiles <= kScanSelfPrefixTiles) {
-        SESSD_LAUNCH((scan_apply_kernel<Load, Store, true>), tiles, kScanThreads, 0, st, load, store, d_n, n_mul, scratch, d_total);
+        SESSD_LAUNCH((scan_apply_kernel<Load, Store, true>), tiles, kScanThreads, 0, st, load, store, d_n, n_mul, cap_items, scratch,
+                     d_total);
         return;
     }
-    SESSD_LAUNCH(scan_tiles_kernel, 1, 1024, 0, st, d_n, n_mul, scratch, d_total);
-    SESSD_LAUNCH((scan_apply_kernel<Load, Store, false>), tiles, kScanThreads, 0, st, load, store, d_n, n_mul, scratch, d_total);
+    SESSD_LAUNCH(scan_tiles_kernel, 1, 1024, 0, st, d_n, n_mul, cap_items, scratch, d_total);
+    SESSD_LAUNCH((scan_apply_kernel<Load, Store, false>), tiles, kScanThreads, 0, st, load, store, d_n, n_mul, cap_items, scratch,
+                     d_total);
 }
 
 static inline size_t scan_scratch_bytes(long long cap_items) {

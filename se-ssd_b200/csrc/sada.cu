@@ -2,15 +2,13 @@
 // pyramid swap of one frame (reference: det3d/datasets/utils/sa_da_v2.py, pyramid_augment_v0, get_pyramids, points_in_pyramids_mask).
 //
 // Every random draw is made on the host (sessd_b200/sada.py); the kernels are pure functions of the points, the pyramids and the lists of
-// pyramids each stage acts on.  The building blocks:
-//   student_boxes_kernel -- the class-valid boxes of each frame after the noise and the global stages (before the range filter and
-//                           limit_period), compacted: the boxes pyramid_augment_v0 receives.
+// pyramids each stage acts on (the boxes pyramid_augment_v0 receives come from sessd_augment_boxes).  The building blocks:
 //   pyramids_kernel      -- get_pyramids (apex = box centre, base = one face of center_to_corner_box3d(origin 0.5)) and the 5 face planes
 //                           of each pyramid as surface_equ_3d_jitv2 computes them, once per pyramid.
 //   member_kernel        -- per point, a bit set over a list of pyramid ids (points_in_convex_polygon_3d_jit: sign >= 0 is outside) and
 //                           the count of each listed pyramid.
-//   keep / plan / scatter -- order-preserving removal of the points inside the listed pyramids whose count passes a threshold (tile,
-//                           scan, scatter as csrc/gtaug.cu; no CTA holds a whole frame).
+//   sessd_sada_compact   -- order-preserving removal of the points inside the listed pyramids whose count passes a threshold: one
+//                           device_scan (common.cuh) of the kept flags whose store writes each kept row.
 //   fps_kernel           -- one CTA per listed pyramid that passes the threshold: its points in row order, exact farthest-point sampling
 //                           (start at row 0, fp64 distances, ties to the lowest row), the picks written in pick order after the kept rows.
 //   swap_kernel          -- one CTA per pair: get_points_ratio / recover_points_by_ratio and the min / max intensity transform.
@@ -28,44 +26,12 @@
 namespace sessd {
 
 constexpr int kSadaThreads = 256;
-constexpr int kSadaRounds = 8;
-constexpr int kSadaTile = kSadaThreads * kSadaRounds;
-constexpr int kSadaPlanThreads = 1024;
 constexpr int kSadaMaxBoxes = 256;             // SESSD_AUGMENT_MAX_GT
 constexpr int kSadaMaxIds = 6 * kSadaMaxBoxes;  // SESSD_SADA_MAX_IDS
 constexpr int kFpsThreads = 512;
 constexpr int kFpsSmemPoints = 4096;           // points a CTA gathers into shared memory (20 B each); larger pyramids stay in global
 
-// ------------------------------------------------------------------------------------------------ boxes and pyramids
-__global__ void __launch_bounds__(kSadaMaxBoxes) student_boxes_kernel(
-    const float *__restrict__ gt_boxes, const int *__restrict__ num_gt, const uint8_t *__restrict__ valid, int max_gt,
-    const double *__restrict__ loc_noise, const double *__restrict__ rot_noise, int num_try, const int *__restrict__ selected,
-    const float *__restrict__ global, float *__restrict__ boxes_out, int *__restrict__ num_out) {
-    __shared__ unsigned char s_keep[kSadaMaxBoxes];
-    const int b = blockIdx.x, j = threadIdx.x;
-    const int n = min(max(num_gt[b], 0), max_gt);
-    const size_t bj = (size_t)b * max_gt + j;
-    float w[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    const bool keep = j < n && valid[bj];
-    if (keep) {
-#pragma unroll
-        for (int c = 0; c < 7; ++c) w[c] = gt_boxes[bj * 7 + c];
-        box_noise(w, loc_noise, rot_noise, num_try, bj, selected[bj]);
-        box_global(w, global + 5 * (size_t)b);
-    }
-    s_keep[j] = keep;
-    __syncthreads();
-    int pos = 0, tot = 0;
-    for (int i = 0; i < max_gt; ++i) { pos += (i < j) & s_keep[i]; tot += s_keep[i]; }
-    float *out = boxes_out + (size_t)b * max_gt * 7;
-    const int row = keep ? pos : j;
-    if (keep || j >= tot) {
-#pragma unroll
-        for (int c = 0; c < 7; ++c) out[row * 7 + c] = w[c];
-    }
-    if (j == 0) num_out[b] = tot;
-}
-
+// ------------------------------------------------------------------------------------------------ pyramids
 // get_pyramids' face orders: corners of center_to_corner_box3d (0 (-,-,-) 1 (-,-,+) 2 (-,+,+) 3 (-,+,-) 4 (+,-,-) 5 (+,-,+) 6 (+,+,+)
 // 7 (+,+,-) in (w, l, h)); points_in_pyramids_mask's surfaces over the 5 pyramid points (0 = apex) are (1 2 0) (2 3 0) (3 4 0) (4 1 0)
 // (4 3 2)
@@ -168,78 +134,21 @@ __device__ __forceinline__ bool removed(const uint32_t *__restrict__ bits, size_
     return false;
 }
 
-struct CompactWs {
-    uint8_t *keep;     // [n]
-    int *tile;         // [tiles + 1]
+// sessd_sada_compact as a device_scan: the flag of a row is "not removed", the store writes each kept row to its rank
+struct NotRemoved {
+    const uint32_t *bits;
+    int words, num_ids, min_count;
+    const int *counts;
+    __device__ __forceinline__ int operator()(long long i) const { return !removed(bits, (size_t)i, words, num_ids, counts, min_count); }
 };
-
-static size_t align16(size_t v) { return (v + 15) & ~(size_t)15; }
-
-static size_t compact_layout(int n, char *base, CompactWs *ws) {
-    size_t off = 0;
-    auto take = [&](size_t bytes) { char *p = base ? base + off : nullptr; off += align16(bytes); return p; };
-    CompactWs w;
-    w.keep = (uint8_t *)take((size_t)n);
-    w.tile = (int *)take(sizeof(int) * ((size_t)div_up(n, kSadaTile) + 1));
-    if (ws) *ws = w;
-    return off;
-}
-
-__global__ void __launch_bounds__(kSadaThreads) keep_kernel(int n, const int *__restrict__ d_n, const uint32_t *__restrict__ bits, int words, int num_ids,
-                                                            const int *__restrict__ counts, int min_count, CompactWs ws) {
-    using Reduce = cub::BlockReduce<int, kSadaThreads>;
-    __shared__ typename Reduce::TempStorage s_red;
-    n = rows_of(n, d_n);
-    int kept = 0;
-#pragma unroll 1
-    for (int r = 0; r < kSadaRounds; ++r) {
-        const int i = blockIdx.x * kSadaTile + r * kSadaThreads + threadIdx.x;
-        if (i >= n) break;
-        const bool keep = !removed(bits, i, words, num_ids, counts, min_count);
-        ws.keep[i] = keep;
-        kept += keep;
+struct StoreKept {
+    const float *points;
+    float *out;
+    int capacity;
+    __device__ __forceinline__ void operator()(long long i, int ex, int v) const {
+        if (v && ex < capacity) reinterpret_cast<float4 *>(out)[ex] = reinterpret_cast<const float4 *>(points)[i];
     }
-    const int total = Reduce(s_red).Sum(kept);
-    if (threadIdx.x == 0) ws.tile[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(kSadaPlanThreads) plan_kernel(int tiles, CompactWs ws, int *__restrict__ num_out) {
-    using Scan = cub::BlockScan<int, kSadaPlanThreads>;
-    __shared__ typename Scan::TempStorage s_scan;
-    __shared__ int s_carry;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    for (int c = 0; c < tiles; c += kSadaPlanThreads) {
-        const int i = c + threadIdx.x;
-        const int v = i < tiles ? ws.tile[i] : 0;
-        int x, tot;
-        Scan(s_scan).ExclusiveSum(v, x, tot);
-        const int carry = s_carry;
-        if (i < tiles) ws.tile[i] = carry + x;
-        __syncthreads();
-        if (threadIdx.x == 0) s_carry = carry + tot;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *num_out = s_carry;
-}
-
-__global__ void __launch_bounds__(kSadaThreads) scatter_kernel(const float *__restrict__ points, int n, const int *__restrict__ d_n, CompactWs ws, float *__restrict__ out,
-                                                               int capacity) {
-    using Scan = cub::BlockScan<int, kSadaThreads>;
-    __shared__ typename Scan::TempStorage s_scan;
-    n = rows_of(n, d_n);
-    int carry = ws.tile[blockIdx.x];
-#pragma unroll 1
-    for (int r = 0; r < kSadaRounds; ++r) {
-        const int i = blockIdx.x * kSadaTile + r * kSadaThreads + threadIdx.x;
-        const int keep = i < n ? ws.keep[i] : 0;
-        int pos, tot;
-        Scan(s_scan).ExclusiveSum(keep, pos, tot);
-        if (keep && carry + pos < capacity) reinterpret_cast<float4 *>(out)[carry + pos] = reinterpret_cast<const float4 *>(points)[i];
-        carry += tot;
-        __syncthreads();
-    }
-}
+};
 
 // ------------------------------------------------------------------------------------------------ members of one listed pyramid, in row order
 // Calls f(rank, row) for every point whose bit a is set, rank = its position among them.  One CTA walks the frame in blockDim rounds.
@@ -435,22 +344,6 @@ using namespace sessd;
 
 static bool misaligned(const void *p) { return ((uintptr_t)p) & 15; }
 
-extern "C" int sessd_sada_student_boxes(const float *d_gt_boxes, const int *d_num_gt, const uint8_t *d_valid, int batch, int max_gt,
-                                        const double *d_loc_noise, const double *d_rot_noise, int num_try, const int *d_selected,
-                                        const float *d_global, float *d_boxes_out, int *d_num_out, void *stream) {
-    if (batch <= 0 || max_gt < 0 || num_try <= 0 || !d_num_gt || !d_global || !d_num_out) return SESSD_EINVAL;
-    if (max_gt > 0 && (!d_gt_boxes || !d_valid || !d_loc_noise || !d_rot_noise || !d_selected || !d_boxes_out)) return SESSD_EINVAL;
-    if (max_gt > kSadaMaxBoxes) return SESSD_ECAPACITY;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (max_gt == 0) {
-        SESSD_CUDA_TRY(cudaMemsetAsync(d_num_out, 0, sizeof(int) * batch, st));
-        return SESSD_OK;
-    }
-    SESSD_LAUNCH(student_boxes_kernel, batch, max_gt, 0, st, d_gt_boxes, d_num_gt, d_valid, max_gt, d_loc_noise, d_rot_noise, num_try,
-                 d_selected, d_global, d_boxes_out, d_num_out);
-    return last_error();
-}
-
 extern "C" int sessd_sada_pyramids(const float *d_boxes, int num_boxes, float *d_pyramids, float *d_planes, void *stream) {
     if (num_boxes < 0 || !d_boxes || !d_pyramids || !d_planes) return SESSD_EINVAL;
     if (num_boxes > kSadaMaxIds / 6) return SESSD_ECAPACITY;
@@ -476,7 +369,7 @@ extern "C" int sessd_sada_membership(const float *d_points, int n, const int *d_
     return last_error();
 }
 
-extern "C" size_t sessd_sada_compact_workspace_bytes(int n) { return n < 0 ? 0 : compact_layout(n, nullptr, nullptr); }
+extern "C" size_t sessd_sada_compact_workspace_bytes(int n) { return n < 0 ? 0 : scan_scratch_bytes(n); }
 
 extern "C" int sessd_sada_compact(const float *d_points, int n, const int *d_n, const uint32_t *d_bits, int num_ids, const int *d_counts, int min_count,
                                   void *d_workspace, size_t workspace_bytes, float *d_out, int capacity, int *d_num_out, void *stream) {
@@ -484,15 +377,11 @@ extern "C" int sessd_sada_compact(const float *d_points, int n, const int *d_n, 
     if ((n > 0 && !d_points) || (n > 0 && num_ids > 0 && (!d_bits || !d_counts))) return SESSD_EINVAL;
     if (misaligned(d_points) || misaligned(d_out)) return SESSD_EINVAL;
     if (num_ids > kSadaMaxIds) return SESSD_ECAPACITY;
-    if (workspace_bytes < compact_layout(n, nullptr, nullptr)) return SESSD_EWORKSPACE;
+    if (workspace_bytes < scan_scratch_bytes(n)) return SESSD_EWORKSPACE;
     if (capacity < n) return SESSD_ECAPACITY;
-    CompactWs ws;
-    compact_layout(n, (char *)d_workspace, &ws);
-    cudaStream_t st = (cudaStream_t)stream;
-    const int tiles = div_up(n, kSadaTile), words = div_up(num_ids, 32);
-    if (tiles > 0) SESSD_LAUNCH(keep_kernel, tiles, kSadaThreads, 0, st, n, d_n, d_bits, words, num_ids, d_counts, min_count, ws);
-    SESSD_LAUNCH(plan_kernel, 1, kSadaPlanThreads, 0, st, tiles, ws, d_num_out);
-    if (tiles > 0) SESSD_LAUNCH(scatter_kernel, tiles, kSadaThreads, 0, st, d_points, n, d_n, ws, d_out, capacity);
+    // the rows: *d_n (clamped to [0, n] by the scan) or n
+    device_scan(NotRemoved{d_bits, div_up(num_ids, 32), num_ids, min_count, d_counts}, StoreKept{d_points, d_out, capacity}, d_n, d_n ? 1 : n,
+                n, (int *)d_workspace, d_num_out, (cudaStream_t)stream);
     return last_error();
 }
 

@@ -33,15 +33,6 @@ struct VoxParams {
     int cap_mask;
 };
 
-__device__ __forceinline__ int find_frame(const int *__restrict__ off, int batch, int i) {
-    int lo = 0, hi = batch;   // off[lo] <= i < off[hi]
-    while (hi - lo > 1) {
-        int mid = (lo + hi) >> 1;
-        if (i >= off[mid]) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 // 1. insert ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) vox_insert_kernel(const float *__restrict__ pts, const int *__restrict__ off,
                                                          VoxParams p, unsigned long long *tbl, int *__restrict__ slot_of) {

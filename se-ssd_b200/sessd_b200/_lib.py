@@ -121,11 +121,10 @@ SIGNATURES = {
     "sessd_noise_per_box": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _i, C.c_double, _vp, _vp]),
     "sessd_points_in_boxes": (_i, [_vp, _i, _i, _vp, _i, C.c_double, _vp, _vp]),
     "sessd_augment_points": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _i, _vp, C.c_double, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "sessd_augment_boxes": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, C.POINTER(C.c_float), _vp, _vp, _vp, _vp, _vp]),
+    "sessd_augment_boxes": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, C.POINTER(C.c_float), _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "sessd_gtaug_select_host": (_i, [_vp, _i, _i, _vp]),
     "sessd_gtaug_paste_workspace_bytes": (_sz, [_i, _i, _i]),
     "sessd_gtaug_paste": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _sz, _vp, _i, _vp, _vp]),
-    "sessd_sada_student_boxes": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "sessd_sada_pyramids": (_i, [_vp, _i, _vp, _vp, _vp]),
     "sessd_sada_membership": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
     "sessd_sada_compact_workspace_bytes": (_sz, [_i]),

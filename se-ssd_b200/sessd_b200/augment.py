@@ -211,7 +211,7 @@ def augment_batch(cfg, clouds, gt_boxes, gt_names, draws, labeled=None, device="
 def augment_resident(cfg, d_points, d_frame_off, frame_sizes, gt_boxes, gt_names, draws, device="cuda", student_boxes=False):
     """augment_batch on points already on the device (labelled frames): d_points [P, 4] f32 (16-byte aligned rows) with d_frame_off
     [B+1] i32, frame_sizes the host's copy of the frame sizes.  Only the boxes and the draws are uploaded (one copy).  student_boxes:
-    also return ``sada_boxes`` [B, max_gt, 7], each frame's class-valid boxes after the global stages (sessd_sada_student_boxes)."""
+    also return ``sada_boxes`` [B, max_gt, 7], each frame's class-valid boxes after the global stages (sessd_augment_boxes)."""
     _, rest, ns = _host_inputs(cfg, frame_sizes, gt_boxes, gt_names, draws, None)
     buf, layout = _pack(list(rest))
     dev = torch.from_numpy(buf).pin_memory().to(device, non_blocking=True)
@@ -227,11 +227,12 @@ def _augment_device(cfg, d_pts, d_off, ns, rest, draws, labeled, student_boxes=F
     raw = None if all(labeled) else d_pts.clone()          # an unlabelled frame has no twin in the reference: its rows keep the input
     raw, out = ops.augment_points(d_pts, d_off, max(ns + [0]), d_boxes, d_num, d_valid, d_loc, d_rot, sel, d_glob, d_perm, d_lab, ctx,
                                   points_raw=raw)
-    boxes_raw, num_raw, boxes_out, num_out = ops.augment_boxes(d_boxes, d_num, d_valid, d_target, d_loc, d_rot, sel, d_glob, cfg.range_bev)
+    boxes = ops.augment_boxes(d_boxes, d_num, d_valid, d_target, d_loc, d_rot, sel, d_glob, cfg.range_bev, global_boxes=student_boxes)
+    boxes_raw, num_raw, boxes_out, num_out = boxes[:4]
     res = dict(points=out, points_raw=raw, frame_off=d_off, gt_boxes=boxes_out, num_gt=num_out, gt_boxes_raw=boxes_raw,
                num_gt_raw=num_raw, selected=sel, transformation=draws.transformation())
     if student_boxes:                                       # the boxes SA-DA takes (sessd_b200.sada)
-        res["sada_boxes"] = ops.sada_student_boxes(d_boxes, d_num, d_valid, d_loc, d_rot, sel, d_glob)[0]
+        res["sada_boxes"] = boxes[4]
     return res
 
 

@@ -700,10 +700,11 @@ def augment_points(points, frame_off, max_frame_points, gt_boxes, num_gt, valid,
     return points_raw, points_out
 
 
-def augment_boxes(gt_boxes, num_gt, valid, target, loc_noise, rot_noise, selected, glob, range_bev):
+def augment_boxes(gt_boxes, num_gt, valid, target, loc_noise, rot_noise, selected, glob, range_bev, global_boxes=False):
     """box3d_transform_, valid-box selection, global stages and the Voxelization / AssignTarget bookkeeping (sessd_augment_boxes).
     target: [B,M] u8 target-class mask or None (all); range_bev: host (x0, y0, x1, y1).  Returns (boxes_raw [B,M,7], num_raw [B],
-    boxes [B,M,7], num [B]) on the device."""
+    boxes [B,M,7], num [B]) on the device; global_boxes=True appends (boxes_global [B,M,7], num_global [B]): the class-valid boxes after
+    the global stages, before the range filter and limit_period (the boxes SA-DA takes)."""
     B, M, T = _aug_inputs(gt_boxes, num_gt, valid, loc_noise, rot_noise, selected)
     _cuda(glob, torch.float32, "glob")
     if tuple(glob.shape) != (B, 5):
@@ -717,11 +718,14 @@ def augment_boxes(gt_boxes, num_gt, valid, target, loc_noise, rot_noise, selecte
     boxes_out = torch.empty((B, M, 7), dtype=torch.float32, device=dev)
     num_raw = torch.empty((B,), dtype=torch.int32, device=dev)
     num_out = torch.empty((B,), dtype=torch.int32, device=dev)
+    boxes_glob = torch.empty((B, M, 7), dtype=torch.float32, device=dev) if global_boxes else None
+    num_glob = torch.empty((B,), dtype=torch.int32, device=dev) if global_boxes else None
     rg = (C.c_float * 4)(*[float(v) for v in range_bev])
     check(lib.sessd_augment_boxes(_p(gt_boxes), _p(num_gt), _p(valid), _p(target), int(B), int(M), _p(loc_noise), _p(rot_noise), int(T),
-                                  _p(selected), _p(glob), rg, _p(boxes_raw), _p(num_raw), _p(boxes_out), _p(num_out), _st()),
-          "sessd_augment_boxes")
-    return boxes_raw, num_raw, boxes_out, num_out
+                                  _p(selected), _p(glob), rg, _p(boxes_raw), _p(num_raw), _p(boxes_out), _p(num_out), _p(boxes_glob),
+                                  _p(num_glob), _st()), "sessd_augment_boxes")
+    res = (boxes_raw, num_raw, boxes_out, num_out)
+    return res + (boxes_glob, num_glob) if global_boxes else res
 
 
 def gtaug_select_host(corners, num_boxes):
@@ -814,20 +818,6 @@ def _ids(ids, num_pyramids, device):
             raise ValueError("at most %d listed pyramids" % SADA_MAX_IDS)
         ids = torch.from_numpy(ids.astype(np.int32)).to(device)
     return _cuda(ids, torch.int32, "ids")
-
-
-def sada_student_boxes(gt_boxes, num_gt, valid, loc_noise, rot_noise, selected, glob):
-    """the class-valid boxes of each frame after the noise and the global stages, before the range filter and limit_period
-    (sessd_sada_student_boxes): the inputs of augment_boxes -> (boxes [B,M,7] f32 compacted, num [B] i32)"""
-    B, M, T = _aug_inputs(gt_boxes, num_gt, valid, loc_noise, rot_noise, selected)
-    _cuda(glob, torch.float32, "glob")
-    if tuple(glob.shape) != (B, 5):
-        raise ValueError("glob must be [B, 5]")
-    boxes = torch.empty((B, M, 7), dtype=torch.float32, device=gt_boxes.device)
-    num = torch.empty((B,), dtype=torch.int32, device=gt_boxes.device)
-    check(lib.sessd_sada_student_boxes(_p(gt_boxes), _p(num_gt), _p(valid), int(B), int(M), _p(loc_noise), _p(rot_noise), int(T),
-                                       _p(selected), _p(glob), _p(boxes), _p(num), _st()), "sessd_sada_student_boxes")
-    return boxes, num
 
 
 def sada_pyramids(boxes):

@@ -141,6 +141,27 @@ def _train_frames(batch, seed):
     return clouds, boxes, names
 
 
+def test_global_boxes_are_the_oracle_global_boxes():
+    """augment_boxes' optional output, the boxes SA-DA takes: per frame the class-valid boxes after the noise and the global stages, in
+    index order, before the range filter and limit_period, zero padded"""
+    from oracle import augment_ref
+    from sessd_b200 import augment, ops
+    acfg = augment.AugmentConfig.from_config(reference_config())
+    clouds, boxes, names = _train_frames(4, 300)
+    draws = augment.draw_augmentation(np.random.RandomState(9), [(len(c), len(b), True) for c, b in zip(clouds, boxes)], acfg)
+    (_, _), rest, _ = augment._host_inputs(acfg, [len(c) for c in clouds], boxes, names, draws, None)
+    d_boxes, d_num, d_valid, _, d_loc, d_rot, d_glob = [_cu(a) for a in rest[:7]]
+    sel = ops.noise_per_box(d_boxes, d_num, d_valid, d_loc, d_rot)
+    sb, sn = ops.augment_boxes(d_boxes, d_num, d_valid, None, d_loc, d_rot, sel, d_glob, acfg.range_bev, global_boxes=True)[4:]
+    sb, sn = sb.cpu().numpy(), sn.cpu().numpy()
+    for b in range(4):
+        valid = np.array([n in acfg.class_names for n in names[b]])
+        f = draws.frames[b]
+        o = augment_ref.augment_frame(clouds[b], boxes[b], valid, dict(loc=f.loc, rot=f.rot, flip=f.flip, rotation=f.rotation,
+                                                                        scale=f.scale, perm=f.perm))
+        assert sn[b] == valid.sum() and np.array_equal(sb[b, :sn[b]], o["boxes"]) and not sb[b, sn[b]:].any()
+
+
 def test_batch_end_to_end_against_the_oracle():
     """8 ring-20k frames with 15 boxes: both branches' voxels bit-exact against the CPU voxeliser on the oracle-augmented points, targets
     bit-exact against assign_v2 on the oracle-augmented boxes, transformation = the draws, and no host synchronisation while building"""
@@ -264,7 +285,7 @@ def test_build_train_batch_feeds_the_training_step():
     assert any(p.grad is not None and torch.isfinite(p.grad).all() for p in model.parameters())
 
 
-def test_error_codes():
+def test_error_codes_and_the_global_box_pair():
     from sessd_b200._lib import lib
     st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     x = torch.zeros(1 << 16, dtype=torch.uint8, device="cuda")
@@ -281,6 +302,8 @@ def test_error_codes():
     assert lib.sessd_points_in_boxes(null, 1, 4, p, 1, -1.0, p, st) == -1
     assert lib.sessd_points_in_boxes(p, 1, 2, p, 1, -1.0, p, st) == -1
     rg = (C.c_float * 4)(0.0, -40.0, 70.4, 40.0)
-    assert lib.sessd_augment_boxes(p, p, p, None, 1, 257, p, p, 100, p, p, rg, p, p, p, p, st) == -2
-    assert lib.sessd_augment_boxes(p, p, p, None, 1, 4, p, p, 100, p, p, None, p, p, p, p, st) == -1
+    assert lib.sessd_augment_boxes(p, p, p, None, 1, 257, p, p, 100, p, p, rg, p, p, p, p, None, None, st) == -2
+    assert lib.sessd_augment_boxes(p, p, p, None, 1, 4, p, p, 100, p, p, None, p, p, p, p, None, None, st) == -1
+    assert lib.sessd_augment_boxes(p, p, p, None, 1, 4, p, p, 100, p, p, rg, p, p, p, p, p, None, st) == -1      # the global pair:
+    assert lib.sessd_augment_boxes(p, p, p, None, 1, 4, p, p, 100, p, p, rg, p, p, p, p, None, p, st) == -1      # both or neither
     torch.cuda.synchronize()

@@ -24,11 +24,11 @@ def _db(z):
                      count=t(z["db_count"], np.int32), boxes=t(z["db_boxes"], np.float64))
 
 
-def _paste_fixture(z, ids_override=None):
+def _paste_fixture(z, ids_override=None, repeat=1):
     from sessd_b200 import ops
     F = int(z["num_frames"])
-    clouds = [z["f%d_in_points" % f] for f in range(F)]
-    ids = [z["f%d_ids" % f] for f in range(F)] if ids_override is None else ids_override
+    clouds = [z["f%d_in_points" % f] for f in range(F)] * repeat
+    ids = ([z["f%d_ids" % f] for f in range(F)] if ids_override is None else ids_override) * repeat
     off = np.concatenate([[0], np.cumsum([len(c) for c in clouds])]).astype(np.int32)
     pts = torch.from_numpy(np.concatenate(clouds).astype(np.float32)).cuda()
     obj_off = np.concatenate([[0], np.cumsum([len(i) for i in ids])]).astype(np.int32)
@@ -62,12 +62,16 @@ def test_select_host_reproduces_the_fixture_acceptance():
 
 
 def test_paste_kernel_reproduces_the_fixture_frames():
+    """the fixture's frames as one batch, then four times over (19.5k scene points: the survivor scan spans several tiles, with empty
+    frames and frame boundaries inside its tiles)"""
     z = load()
-    ops, pts, off, obj_off, obj_ids, db, max_paste = _paste_fixture(z)
-    out, fo = ops.gtaug_paste(pts, off, obj_off, obj_ids, db["points"], db["off"], db["count"], db["boxes"], max_paste)
-    fo = fo.cpu().numpy()
-    for f in range(int(z["num_frames"])):
-        assert np.array_equal(out[fo[f]:fo[f + 1]].cpu().numpy(), z["f%d_points_pasted" % f]), f
+    F = int(z["num_frames"])
+    for repeat in (1, 4):
+        ops, pts, off, obj_off, obj_ids, db, max_paste = _paste_fixture(z, repeat=repeat)
+        out, fo = ops.gtaug_paste(pts, off, obj_off, obj_ids, db["points"], db["off"], db["count"], db["boxes"], max_paste)
+        fo = fo.cpu().numpy()
+        for f in range(F * repeat):
+            assert np.array_equal(out[fo[f]:fo[f + 1]].cpu().numpy(), z["f%d_points_pasted" % (f % F)]), (repeat, f)
 
 
 def test_builder_draws_ids_and_pasted_frames_follow_the_reference_stream(tmp_path):

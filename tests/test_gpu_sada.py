@@ -78,46 +78,35 @@ def _pyramid_cloud(rs, n, dup=0):
     return box, cloud
 
 
-@pytest.mark.parametrize("n,dup", [(51, 0), (700, 0), (4096, 0), (4097, 0), (20000, 0), (300, 120), (6000, 3000)])
-def test_fps_picks_follow_the_contract(n, dup):
-    """shared-memory (<= 4096 points) and global-memory pyramids, and duplicated points (ties)"""
+# (pyramid points, duplicated points, device row count or None): the compaction's one-CTA scan (<= 16k rows), its two-launch scan (up to
+# 1024 scan tiles) and its three-launch scan (more), with a device row count below the buffer's rows and above them (clamped)
+FPS_CASES = [(51, 0, None), (700, 0, None), (4096, 0, None), (4097, 0, None), (20000, 0, None), (300, 120, None), (6000, 3000, None),
+             (2100000, 0, None), (6000, 0, 5000), (700, 0, 1 << 30), (20000, 0, 1 << 30)]
+
+
+@pytest.mark.parametrize("n,dup,rows", FPS_CASES, ids=["%d-%d" % c[:2] + ("" if c[2] is None else "-rows%d" % c[2]) for c in FPS_CASES])
+def test_fps_picks_follow_the_contract(n, dup, rows):
+    """shared-memory (<= 4096 points) and global-memory pyramids, duplicated points (ties), and stages that read a device row count"""
     from sessd_b200 import ops
     rs = np.random.RandomState(n + dup)
     box, cloud = _pyramid_cloud(rs, n, dup)
     pyr, planes = ops.sada_pyramids(_cu(box))
     pts = _cu(cloud)
-    bits, counts, _ = ops.sada_membership(pts, planes, [1])
+    d_n = None if rows is None else _cu(np.array([rows], np.int32))
+    N = len(cloud) if rows is None else min(rows, len(cloud))              # the rows the stages read
+    bits, counts, _ = ops.sada_membership(pts, planes, [1], n=d_n)
     inside = sada_ref.in_pyramids(cloud, sada_ref.pyramids(box)[0, 1:2])[:, 0]
-    assert int(counts.item()) == inside.sum() == n
+    assert inside.sum() == n
+    inside = inside[:N]
+    assert int(counts.item()) == inside.sum()
     out = torch.empty((len(cloud) + 50, 4), dtype=torch.float32, device="cuda")
-    _, num = ops.sada_compact(pts, bits, counts, 50, out=out)
-    ops.sada_fps(pts, bits, counts, 50, 50, out, num)
+    _, num = ops.sada_compact(pts, bits, counts, 50, n=d_n, out=out)
+    ops.sada_fps(pts, bits, counts, 50, 50, out, num, n=d_n)
     torch.cuda.synchronize()
-    mine = cloud[inside]
-    want = np.concatenate([cloud[~inside], mine[sada_ref.fps(mine, 50)]])
+    mine = cloud[:N][inside]
+    want = np.concatenate([cloud[:N][~inside], mine[sada_ref.fps(mine, 50)]])
     assert int(num.item()) == len(want)
     assert np.array_equal(out[:len(want)].cpu().numpy(), want)
-
-
-def test_student_boxes_are_the_oracle_global_boxes():
-    from oracle import augment_ref
-    from sessd_b200 import augment, ops
-    from test_augment_oracle import reference_config
-    from test_gpu_augment import _train_frames
-    acfg = augment.AugmentConfig.from_config(reference_config())
-    clouds, boxes, names = _train_frames(4, 300)
-    draws = augment.draw_augmentation(np.random.RandomState(9), [(len(c), len(b), True) for c, b in zip(clouds, boxes)], acfg)
-    (_, _), rest, _ = augment._host_inputs(acfg, [len(c) for c in clouds], boxes, names, draws, None)
-    d_boxes, d_num, d_valid, _, d_loc, d_rot, d_glob = [_cu(a) for a in rest[:7]]
-    sel = ops.noise_per_box(d_boxes, d_num, d_valid, d_loc, d_rot)
-    sb, sn = ops.sada_student_boxes(d_boxes, d_num, d_valid, d_loc, d_rot, sel, d_glob)
-    sb, sn = sb.cpu().numpy(), sn.cpu().numpy()
-    for b in range(4):
-        valid = np.array([n in acfg.class_names for n in names[b]])
-        f = draws.frames[b]
-        o = augment_ref.augment_frame(clouds[b], boxes[b], valid, dict(loc=f.loc, rot=f.rot, flip=f.flip, rotation=f.rotation,
-                                                                        scale=f.scale, perm=f.perm))
-        assert sn[b] == valid.sum() and np.array_equal(sb[b, :sn[b]], o["boxes"]) and not sb[b, sn[b]:].any()
 
 
 def test_shuffle_gathers_each_frame():
