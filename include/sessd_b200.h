@@ -155,7 +155,8 @@ int sessd_spconv_forward_rows_planes(const float *d_in_feat, int cin, const int 
  * The rulebook is passed as d_tiles = the per-tile pair lists sessd_rulebook_tile_lists() makes from the nbr table (once per rulebook).
  * d_in_planes [plane_rows][2][cp] fp16, x = (hi + lo) / d_in_info[1], d_in_info[0] = abs-max of the input tensor; outputs (each nullable, at
  * least one): fp32 rows [max_out][cout]; planes [>= max_out][2][cout <= 32 ? 32 : 64] with d_out_info = {abs-max of the output (atomicMax; zero
- * it once per frame), S_out}, S_out from the bound d_in_info[0] * gain + shift_max as above.  Supported (cp, cout): (32,32) (32,64) (64,32) (64,64). */
+ * it once per frame), S_out}, S_out from the bound d_in_info[0] * gain + shift_max as above; both outputs are written 16 bytes at a time and
+ * must be 16-byte aligned (SESSD_EINVAL otherwise).  Supported (cp, cout): (32,32) (32,64) (64,32) (64,64). */
 int sessd_spconv_forward_cg(const void *d_in_planes, int cp, int plane_rows, const float *d_in_info, const void *d_tiles, int kvol,
                             const int *d_n_out, int max_out, const void *d_weight_h2, int cout, const float *d_scale, const float *d_shift,
                             int relu, float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, void *stream);

@@ -150,33 +150,6 @@ __device__ __forceinline__ void p2_wgmma_ra(float *d, const uint32_t *a, uint64_
     else wgmma_f16_ra_n256(d, a, db, accumulate);
 }
 
-// 4 x 4 transpose of 2-float pairs inside each quad of lanes (q = lane & 3, the four lanes of one accumulator row): on entry pair g
-// is s[4 g], s[4 g + 1] = channels 8 g + 2 q, + 1 of a 32-channel block; on exit v[0..8) = channels 8 q .. 8 q + 7.  Two xor
-// exchanges, all lanes of the warp take part.
-__device__ __forceinline__ void p2_quad_transpose(const float *s, int q, float v[8]) {
-    const bool odd = q & 1, up = q & 2;
-    float a[2][2][2];      // [k][b][e]: pair of group (q & 1) + 2 k held by lane (q & ~1) | b
-#pragma unroll
-    for (int k = 0; k < 2; ++k)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-            const float even_g = s[4 * (2 * k) + e], odd_g = s[4 * (2 * k + 1) + e];
-            const float keep = odd ? odd_g : even_g;
-            const float recv = __shfl_xor_sync(0xFFFFFFFFu, odd ? even_g : odd_g, 1);
-            a[k][0][e] = odd ? recv : keep;
-            a[k][1][e] = odd ? keep : recv;
-        }
-#pragma unroll
-    for (int b = 0; b < 2; ++b)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-            const float keep = up ? a[1][b][e] : a[0][b][e];
-            const float recv = __shfl_xor_sync(0xFFFFFFFFu, up ? a[0][b][e] : a[1][b][e], 2);
-            v[2 * b + e] = up ? recv : keep;           // from lane b
-            v[2 * (2 + b) + e] = up ? keep : recv;     // from lane 2 + b
-        }
-}
-
 // PROFILE only: clock64() at the start of a timed span, and the span's clocks added to clk (no code otherwise)
 template <bool PROFILE>
 __device__ __forceinline__ long long p2_tick() {
@@ -510,7 +483,7 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
                     const bool row_ok = rows_ok[h];
                     const size_t opix = opixs[h];
                     float v[8], o[8] = {};
-                    p2_quad_transpose(acc + 16 * j + 2 * h, q, v);
+                    quad_transpose8(acc + 16 * j + 2 * h, q, v);
                     const int n = it.n0 + 32 * j + 8 * q;      // this lane's 8 channels; cout % 8 == 0: all exist or none
                     const size_t off = opix * p.cout + n;
                     if (row_ok && n < p.cout) {

@@ -11,10 +11,15 @@
 //   * a stage's missing rows must read as zeros: each producer warp remembers (registers) which of its rows of its stage hold data and
 //     clears (st.shared) only the rows that were valid for the stage's previous offset and are not for the new one -- the stages are
 //     zeroed once per CTA;
-//   * the 32-channel layers stage the weights as [b_hi rows ; b_lo rows] of 64 bytes (SWIZZLE_64B), the 64-channel layers as
-//     [b_hi ; b_lo] tiles of 128-byte rows (SWIZZLE_128B);
-//   * two consumer warpgroups (64 tile rows each) issue the wgmmas of every offset, keep one offset's group in flight while they wait
-//     for the next stage, and run the epilogue from the accumulator registers;
+//   * the 32-channel layers stage the weights as [b_lo rows ; b_hi rows] of 64 bytes (SWIZZLE_64B), the 64-channel layers as
+//     [b_lo ; b_hi] tiles of 128-byte rows (SWIZZLE_128B): per k16, one m64n(2 COUT) over the whole stage computes a_hi b_lo (cross)
+//     and a_hi b_hi (main) with a single shared-memory read of the a_hi tile, and an m64nCOUT adds a_lo b_hi onto the cross half -- two
+//     wgmmas instead of three, the same products in the same order per accumulator (bit-identical to three separate m64nCOUT);
+//   * two consumer warpgroups (64 tile rows each) issue the wgmmas of every offset, wait for them and release the stage at once, so its
+//     next fill starts while the following offset's fill is still in flight (a single frame's layers are bound by this chain of fills,
+//     see DEEP; measurements in DESIGN section 4), and run the epilogue from the accumulator registers: a 4 x 4 transpose inside each
+//     quad of lanes gives every lane 8 whole channels of one row, stored 16 bytes at a time (each warp store covers whole 32-byte
+//     sectors), with the folded BN scale / shift read from shared memory (copied there once per CTA);
 //   * CTAs are persistent (one per SM), so barrier / zero-fill setup is paid once, not per 128 rows;
 //   * the epilogue writes the NEXT layer's operand format directly -- fp16 (hi, lo) planes scaled by a power of two derived from a
 //     rigorous bound |out| <= amax_in * G + max|shift| (G from the weights, host; amax_in measured by the producing layer's epilogue) --
@@ -43,11 +48,11 @@ template <int CP, int COUT, int DEEP = 0>
 struct CgCfg {
     static constexpr bool kWide = (CP == 64);
     static constexpr int kATile = (kWide ? 2 : 1) * kCgBM * 128;              // bytes: [hi tile ; lo tile] (wide) or one [hi | lo] tile
-    static constexpr int kBTile = (kWide ? 2 : 1) * COUT * 128;               // wide: [b_hi ; b_lo] of 128-byte rows; narrow: 64-byte rows
+    static constexpr int kBTile = (kWide ? 2 : 1) * COUT * 128;               // wide: [b_lo ; b_hi] of 128-byte rows; narrow: 64-byte rows
     static constexpr int kStage = kATile + (kBTile + 1023) / 1024 * 1024;
     static constexpr int kStages = (kWide ? 2 : 4) * (DEEP ? 2 : 1);           // must divide the 8 producer warps (one group per stage)
-    static constexpr int kMeta = kCgBM * kCgMaxK * 4 /*lists*/ + kCgMaxK * 16 /*valid*/ + 32 * 4 /*cnt*/ + 33 * 4 /*klist, nact*/ + 32 * 4 /*off*/ +
-                                 3 * kStages * 8 /*barriers*/ + 24;
+    static constexpr int kMeta = kCgBM * kCgMaxK * 4 /*lists*/ + kCgMaxK * 16 /*valid*/ + 2 * COUT * 4 /*scale, shift*/ + 32 * 4 /*cnt*/ +
+                                 33 * 4 /*klist, nact*/ + 32 * 4 /*off*/ + 3 * kStages * 8 /*barriers*/ + 24;
     static constexpr int kSmem = kStages * kStage + kMeta + 1024;
     static constexpr int kCPO = COUT > 32 ? 64 : 32;                          // channels per plane row of the OUTPUT
 };
@@ -75,10 +80,12 @@ __device__ __forceinline__ void cg_sts_zero16(uint32_t saddr) {
     asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};\n" ::"r"(saddr), "r"(0) : "memory");
 }
 
-template <int COUT>
+// N output columns: COUT (one plane of the weight stage) or 2 COUT (the whole [b_lo ; b_hi] stage)
+template <int N>
 __device__ __forceinline__ void cg_wgmma(float *d, uint64_t da, uint64_t db, uint32_t accumulate) {
-    if constexpr (COUT == 32) wgmma_f16_n32(d, da, db, accumulate);
-    else wgmma_f16_n64(d, da, db, accumulate);
+    if constexpr (N == 32) wgmma_f16_n32(d, da, db, accumulate);
+    else if constexpr (N == 64) wgmma_f16_n64(d, da, db, accumulate);
+    else wgmma_f16_n128(d, da, db, accumulate);
 }
 
 template <int CP, int COUT, int DEEP>
@@ -94,7 +101,9 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
     unsigned char *tiles = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint32_t *s_list = (uint32_t *)(tiles + C::kStages * C::kStage);      // [kvol][128]: (input row << 7) | tile row
     uint32_t *s_valid = s_list + kCgBM * kCgMaxK;                        // [kvol][4]: 128-bit row mask per offset
-    int *s_cnt = (int *)(s_valid + kCgMaxK * 4);                         // [32]
+    float *s_scale = (float *)(s_valid + kCgMaxK * 4);                   // [COUT] folded BN scale, 16-byte aligned
+    float *s_shift = s_scale + COUT;                                     // [COUT] folded BN shift (zeros without one)
+    int *s_cnt = (int *)(s_shift + COUT);                                // [32]
     int *s_klist = s_cnt + 32;                                           // [32] + nact
     int *s_nact = s_klist + 32;
     int *s_off = s_nact + 1;                                             // [32] first list entry of every offset
@@ -107,6 +116,10 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
     if (tid == 0) {
         for (int s = 0; s < C::kStages; ++s) { mbar_init(&full_a[s], kCgProdWarps / C::kStages); mbar_init(&full_b[s], 1); mbar_init(&empty[s], kCgMmaWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    }
+    if (tid < COUT) {
+        s_scale[tid] = __ldg(a.scale + tid);
+        s_shift[tid] = a.shift ? __ldg(a.shift + tid) : 0.f;
     }
     // every A tile starts as zeros (the B halves of the stages are always fully overwritten by the TMA)
     for (int s = 0; s < C::kStages; ++s)
@@ -155,7 +168,7 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
         const int nact = *s_nact;
 
         if (warp == kCgWeightWarp) {
-            // ===================== weight tiles (TMA, one elected lane): [b_hi ; b_lo] =====================
+            // ===================== weight tiles (TMA, one elected lane): [b_lo ; b_hi] =====================
             int s = st0;
             uint32_t ph = ph0;
             for (int j = 0; j < nact; ++j) {
@@ -164,8 +177,8 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
                 if (elect_one()) {
                     mbar_expect_tx(&full_b[s], C::kBTile);
                     unsigned char *b_tile = tiles + s * C::kStage + C::kATile;
-                    tma_load_4d(b_tile, &map_w, &full_b[s], 0, 0, 0, k);
-                    tma_load_4d(b_tile + C::kBTile / 2, &map_w, &full_b[s], 0, 0, 1, k);
+                    tma_load_4d(b_tile + C::kBTile / 2, &map_w, &full_b[s], 0, 0, 0, k);      // plane 0 = b_hi
+                    tma_load_4d(b_tile, &map_w, &full_b[s], 0, 0, 1, k);                      // plane 1 = b_lo
                 }
                 __syncwarp();
                 if (++s == C::kStages) { s = 0; ph ^= 1u; }
@@ -174,11 +187,14 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
             // ===================== consumers: wgmma per offset, then the epilogue from the accumulator registers =====================
             const int cw = warp - kCgProdWarps, wg = cw >> 2, wq = cw & 3;
             constexpr int kAcc = COUT / 2;
-            float acc_m[kAcc], acc_c[kAcc];
+            // acc[0, kAcc): cross a_hi x b_lo + a_lo x b_hi, acc[kAcc, COUT): main a_hi x b_hi -- the fragment of an m64n(2 COUT) over the
+            // whole [b_lo ; b_hi] weight stage.  The cross half comes first: ptxas serializes every wgmma of the kernel when one of them
+            // accumulates into a part of another's fragment that does not start at its first register.
+            float acc[COUT];
 #pragma unroll
-            for (int i = 0; i < kAcc; ++i) { acc_m[i] = 0.f; acc_c[i] = 0.f; }
+            for (int i = 0; i < COUT; ++i) acc[i] = 0.f;
             const uint32_t a_rows = (uint32_t)(wg * 64 * 128);   // this warpgroup's 64 rows of the 128-byte-row A tile
-            int s = st0, prev = -1;
+            int s = st0;
             uint32_t ph = ph0;
             for (int j = 0; j < nact; ++j) {
                 mbar_wait(&full_b[s], ph);
@@ -186,67 +202,101 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
                 const uint32_t st = tiles_u32 + (uint32_t)(s * C::kStage);
                 const uint64_t dA = kDescSw128Hi | desc_lo(st + a_rows);
                 const uint32_t first = j != 0 ? 1u : 0u;
+                // per k16: one m64n(2 COUT) over the stacked stage (cross (+)= a_hi x b_lo, main (+)= a_hi x b_hi: a_hi is read once),
+                // then cross += a_lo x b_hi.  Each accumulator sums the same products in the same order as three separate m64nCOUT would.
                 wgmma_fence();
                 if constexpr (C::kWide) {
                     const uint64_t dAl = dA + ((kCgBM * 128) >> 4);
-                    const uint64_t dBh = kDescSw128Hi | desc_lo(st + C::kATile);
-                    const uint64_t dBl = dBh + ((COUT * 128) >> 4);
+                    const uint64_t dBl = kDescSw128Hi | desc_lo(st + C::kATile);
+                    const uint64_t dBh = dBl + ((COUT * 128) >> 4);
 #pragma unroll
-                    for (int kk = 0; kk < 4; ++kk) cg_wgmma<COUT>(acc_m, dA + 2 * kk, dBh + 2 * kk, first | (kk != 0));      // main  += a_hi x b_hi
+                    for (int kk = 0; kk < 4; ++kk) cg_wgmma<2 * COUT>(acc, dA + 2 * kk, dBl + 2 * kk, first | (kk != 0));
 #pragma unroll
-                    for (int kk = 0; kk < 4; ++kk) cg_wgmma<COUT>(acc_c, dA + 2 * kk, dBl + 2 * kk, first | (kk != 0));      // cross += a_hi x b_lo
-#pragma unroll
-                    for (int kk = 0; kk < 4; ++kk) cg_wgmma<COUT>(acc_c, dAl + 2 * kk, dBh + 2 * kk, 1u);                    // cross += a_lo x b_hi
+                    for (int kk = 0; kk < 4; ++kk) cg_wgmma<COUT>(acc, dAl + 2 * kk, dBh + 2 * kk, 1u);
                 } else {
-                    // A line = [hi 32 | lo 32] (SWIZZLE_128B); B stage = [b_hi rows ; b_lo rows] of 64 bytes each (SWIZZLE_64B)
-                    const uint64_t dBh = kDescSw64Hi | desc_lo(st + C::kATile);
-                    const uint64_t dBl = dBh + ((COUT * 64) >> 4);
+                    // A line = [hi 32 | lo 32] (SWIZZLE_128B); B stage = [b_lo rows ; b_hi rows] of 64 bytes each (SWIZZLE_64B)
+                    const uint64_t dBl = kDescSw64Hi | desc_lo(st + C::kATile);
+                    const uint64_t dBh = dBl + ((COUT * 64) >> 4);
 #pragma unroll
-                    for (int kk = 0; kk < 2; ++kk) cg_wgmma<COUT>(acc_m, dA + 2 * kk, dBh + 2 * kk, first | (kk != 0));
+                    for (int kk = 0; kk < 2; ++kk) cg_wgmma<2 * COUT>(acc, dA + 2 * kk, dBl + 2 * kk, first | (kk != 0));
 #pragma unroll
-                    for (int kk = 0; kk < 2; ++kk) cg_wgmma<COUT>(acc_c, dA + 2 * kk, dBl + 2 * kk, first | (kk != 0));
-#pragma unroll
-                    for (int kk = 0; kk < 2; ++kk) cg_wgmma<COUT>(acc_c, dA + 4 + 2 * kk, dBh + 2 * kk, 1u);
+                    for (int kk = 0; kk < 2; ++kk) cg_wgmma<COUT>(acc, dA + 4 + 2 * kk, dBh + 2 * kk, 1u);
                 }
                 wgmma_commit();
-                wgmma_wait<1>();                                 // the previous offset's products are done: its stage may be refilled
-                if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-                prev = s;
+                // release the stage as soon as its own products are done, not one offset later: the producers start its next fill
+                // while this offset's successor is still being filled, so with two stages two fills overlap instead of one.  A
+                // single frame's tiles are bound by this chain of fills; the wait costs little since the next offset's stage is
+                // rarely full by then anyway
+                wgmma_wait<0>();
+                if (lane == 0) mbar_arrive(&empty[s]);
                 if (++s == C::kStages) { s = 0; ph ^= 1u; }
             }
-            wgmma_wait<0>();
-            wgmma_fence_regs<kAcc>(acc_m);
-            wgmma_fence_regs<kAcc>(acc_c);
-            if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-            // BN / ReLU -> planes and / or fp32 rows; this thread holds rows r0 and r0 + 8, two adjacent channels per 8-channel group
+            wgmma_fence_regs<COUT>(acc);
+            // BN / ReLU -> planes and / or fp32 rows.  This thread holds rows r0 and r0 + 8, two adjacent channels of every 8-channel
+            // group; a transpose inside each quad of lanes (one row) gives every lane 8 whole channels, stored 16 bytes at a time
+#pragma unroll
+            for (int i = 0; i < kAcc; ++i) acc[i] = acc[kAcc + i] + acc[i];      // main + cross
+            const int q = lane & 3;
             const int r0 = wg * 64 + wq * 16 + (lane >> 2);
-            const int c2 = 2 * (lane & 3);
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int r = r0 + 8 * h;
-                if (r >= rows) continue;
-                const size_t orow = (size_t)(row0 + r);
+            for (int jb = 0; jb < COUT / 32; ++jb)
 #pragma unroll
-                for (int g = 0; g < COUT / 8; ++g) {
-                    const int n = 8 * g + c2, i = 4 * g + 2 * h;
-                    const float2 sc = __ldg(reinterpret_cast<const float2 *>(a.scale + n));
-                    const float2 sh = a.shift ? __ldg(reinterpret_cast<const float2 *>(a.shift + n)) : make_float2(0.f, 0.f);
-                    float o0 = fmaf((acc_m[i] + acc_c[i]) * inv_act, sc.x, sh.x);
-                    float o1 = fmaf((acc_m[i + 1] + acc_c[i + 1]) * inv_act, sc.y, sh.y);
-                    if (a.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
-                    vmax = fmaxf(vmax, fmaxf(fabsf(o0), fabsf(o1)));
-                    if (a.out_f32) *reinterpret_cast<float2 *>(a.out_f32 + orow * COUT + n) = make_float2(o0, o1);
-                    if (a.out_planes) {
-                        const float x0 = o0 * s_out, x1 = o1 * s_out;
-                        const __half2 hi = __floats2half2_rn(x0, x1);
-                        const float2 f = __half22float2(hi);
-                        const __half2 lo = __floats2half2_rn(x0 - f.x, x1 - f.y);
-                        __half2 *dst = reinterpret_cast<__half2 *>(a.out_planes + orow * (2 * C::kCPO) + n);
-                        dst[0] = hi;
-                        dst[C::kCPO / 2] = lo;
+                for (int h = 0; h < 2; ++h) {
+                    const int r = r0 + 8 * h;
+                    const bool row_ok = r < rows;                // the same in the four lanes of a quad
+                    const size_t orow = (size_t)(row0 + r);
+                    float v[8], o[8];
+                    quad_transpose8(acc + 16 * jb + 2 * h, q, v);
+                    const int n = 32 * jb + 8 * q;               // this lane's 8 channels
+#pragma unroll
+                    for (int t = 0; t < 8; t += 4) {
+                        const float4 sc = *reinterpret_cast<const float4 *>(s_scale + n + t);
+                        const float4 sh = *reinterpret_cast<const float4 *>(s_shift + n + t);
+                        o[t] = fmaf(v[t] * inv_act, sc.x, sh.x);
+                        o[t + 1] = fmaf(v[t + 1] * inv_act, sc.y, sh.y);
+                        o[t + 2] = fmaf(v[t + 2] * inv_act, sc.z, sh.z);
+                        o[t + 3] = fmaf(v[t + 3] * inv_act, sc.w, sh.w);
+                    }
+                    if (a.relu) {
+#pragma unroll
+                        for (int t = 0; t < 8; ++t) o[t] = fmaxf(o[t], 0.f);
+                    }
+                    if (row_ok) {
+#pragma unroll
+                        for (int t = 0; t < 8; ++t) vmax = fmaxf(vmax, fabsf(o[t]));
+                    }
+                    if (a.out_planes && row_ok) {
+                        __align__(16) __half2 hi[4], lo[4];
+#pragma unroll
+                        for (int t = 0; t < 4; ++t) {
+                            const float x0 = o[2 * t] * s_out, x1 = o[2 * t + 1] * s_out;
+                            hi[t] = __floats2half2_rn(x0, x1);
+                            const float2 f = __half22float2(hi[t]);
+                            lo[t] = __floats2half2_rn(x0 - f.x, x1 - f.y);
+                        }
+                        __half *dst = a.out_planes + orow * (2 * C::kCPO) + n;
+                        *reinterpret_cast<uint4 *>(dst) = *reinterpret_cast<const uint4 *>(hi);
+                        *reinterpret_cast<uint4 *>(dst + C::kCPO) = *reinterpret_cast<const uint4 *>(lo);
+                    }
+                    if (a.out_f32) {
+                        // lanes q and q ^ 2 trade half groups, so that each of the two stores of a quad covers 16 whole channels (two whole
+                        // 32-byte sectors): lane q keeps half (q >> 1) of group q and gets the same half of group q ^ 2
+                        const bool up = q & 2;
+                        float keep[4], recv[4];
+#pragma unroll
+                        for (int t = 0; t < 4; ++t) {
+                            keep[t] = up ? o[4 + t] : o[t];
+                            recv[t] = __shfl_xor_sync(0xFFFFFFFFu, up ? o[t] : o[4 + t], 2);
+                        }
+                        const float4 w_lo = up ? make_float4(recv[0], recv[1], recv[2], recv[3]) : make_float4(keep[0], keep[1], keep[2], keep[3]);
+                        const float4 w_hi = up ? make_float4(keep[0], keep[1], keep[2], keep[3]) : make_float4(recv[0], recv[1], recv[2], recv[3]);
+                        float *dst = a.out_f32 + orow * COUT + 32 * jb + 8 * (q & 1) + 4 * (q >> 1);
+                        if (row_ok) {
+                            *reinterpret_cast<float4 *>(dst) = w_lo;
+                            *reinterpret_cast<float4 *>(dst + 16) = w_hi;
+                        }
                     }
                 }
-            }
         } else {
             // ===================== producers: copy the rows that exist, clear the rows that stopped existing =====================
             // One producer GROUP per stage (kStages groups of 8 / kStages warps): a group fills only "its" stage, waits for its own copies
@@ -385,6 +435,7 @@ extern "C" int sessd_spconv_forward_cg(const void *d_in_planes, int cp, int plan
         kvol < 1 || kvol > kCgMaxK || plane_rows < 1 || plane_rows > (1 << 25))
         return SESSD_EINVAL;
     if (d_out_planes && !d_out_info) return SESSD_EINVAL;
+    if (((uintptr_t)d_out_f32 | (uintptr_t)d_out_planes) & 15) return SESSD_EINVAL;     // the epilogue writes 16 bytes at a time
     CgArgs a;
     a.planes = (const __half *)d_in_planes; a.in_info = d_in_info; a.tiles = (const unsigned int *)d_tiles; a.tile_stride = tile_list_stride(kvol); a.d_n_out = d_n_out; a.kvol = kvol; a.max_out = max_out;
     a.relu = relu; a.scale = d_scale; a.shift = d_shift; a.gain = gain; a.shift_max = shift_max; a.out_f32 = d_out_f32;

@@ -103,6 +103,33 @@ __device__ __forceinline__ void wgmma_fence_regs(float *d) {
     for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// 4 x 4 transpose of 2-float pairs inside each quad of lanes (q = lane & 3, the four lanes of one accumulator row): on entry pair g
+// is s[4 g], s[4 g + 1] = channels 8 g + 2 q, + 1 of a 32-channel block; on exit v[0..8) = channels 8 q .. 8 q + 7.  Two xor
+// exchanges, all lanes of the warp take part.  The epilogues use it to store 8 whole channels of a row per lane (16-byte stores).
+__device__ __forceinline__ void quad_transpose8(const float *s, int q, float v[8]) {
+    const bool odd = q & 1, up = q & 2;
+    float a[2][2][2];      // [k][b][e]: pair of group (q & 1) + 2 k held by lane (q & ~1) | b
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const float even_g = s[4 * (2 * k) + e], odd_g = s[4 * (2 * k + 1) + e];
+            const float keep = odd ? odd_g : even_g;
+            const float recv = __shfl_xor_sync(0xFFFFFFFFu, odd ? even_g : odd_g, 1);
+            a[k][0][e] = odd ? recv : keep;
+            a[k][1][e] = odd ? keep : recv;
+        }
+#pragma unroll
+    for (int b = 0; b < 2; ++b)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const float keep = up ? a[1][b][e] : a[0][b][e];
+            const float recv = __shfl_xor_sync(0xFFFFFFFFu, up ? a[0][b][e] : a[1][b][e], 2);
+            v[2 * b + e] = up ? recv : keep;           // from lane b
+            v[2 * (2 + b) + e] = up ? keep : recv;     // from lane 2 + b
+        }
+}
+
 // K-major swizzled shared-memory matrix descriptor (sm_90 GMMA layout):
 //   [0,14) start>>4 | [16,30) LBO>>4 (= 1, unused for swizzled K-major) | [32,46) SBO>>4 (stride between 8-row groups)
 //   [62,64) layout: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B.  The low word (start | LBO) is added to the constant high word.
