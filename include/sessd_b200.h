@@ -492,6 +492,35 @@ int sessd_sada_shuffle(const float *d_points, const int *d_frame_off, int batch,
                        void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * KITTI data preparation (csrc/kitti_prep.cu).  Replaces the membership tests of the reference's data preparation: remove_outside_points
+ * (det3d/core/bbox/box_np_ops.py:981-992) in _create_reduced_point_cloud / _calculate_num_points_in_gt and points_in_rbbox (:1152-1157)
+ * in _calculate_num_points_in_gt / create_groundtruth_database.  Every plane is computed on the host (sessd_b200/kitti_prep.py).  A
+ * polyhedron is six planes [6, 4] fp64 (a, b, c, d); a point is inside when (((x*a) + (y*b)) + (z*c)) + d < 0 for all six, x y z the fp32
+ * coordinates widened to fp64 and each operation rounded on its own (_points_in_convex_polygon_3d_jit: a sign >= 0 is outside).  Points
+ * are [*, 4] f32 float4 rows and must be 16-byte aligned (SESSD_EINVAL otherwise); null pointers and negative counts are SESSD_EINVAL.
+ * sessd_prep_frustum_compact -- device.  d_points [num_points, 4] with d_frame_off [batch + 1], d_planes [batch, 6, 4] (one image frustum
+ *     per frame).  Writes the rows inside their frame's frustum to d_points_out as bit copies in frame order and the new offsets to
+ *     d_frame_off_out [batch + 1] (device).  capacity < num_points -> SESSD_ECAPACITY; workspace_bytes <
+ *     sessd_prep_frustum_compact_workspace_bytes(num_points) -> SESSD_EWORKSPACE.
+ * sessd_prep_box_count -- device.  d_box_planes [num_boxes, 6, 4] with d_box_off [batch + 1] (CSR boxes per frame): d_counts [num_boxes]
+ *     i32 = the points of the box's frame inside the box.  No workspace.
+ * sessd_prep_box_gather -- device.  Same boxes plus d_centres [num_boxes, 3] f64 and d_counts from sessd_prep_box_count.  d_obj_off
+ *     [num_boxes + 1] = the exclusive scan of the counts (device); box k's points, in frame order, go to rows [d_obj_off[k],
+ *     d_obj_off[k + 1]) of d_rows_out as fp32(double(p) - centre) for x y z and the intensity unchanged.  A point inside two boxes is
+ *     written for both.  num_rows: the host-known sum of the counts; capacity < num_rows -> SESSD_ECAPACITY; workspace_bytes <
+ *     sessd_prep_box_gather_workspace_bytes(num_boxes) -> SESSD_EWORKSPACE.  No write is ever past the capacity.
+ * ------------------------------------------------------------------------------------------------ */
+size_t sessd_prep_frustum_compact_workspace_bytes(int num_points);
+int sessd_prep_frustum_compact(const float *d_points, const int *d_frame_off, int batch, int num_points, const double *d_planes,
+                               void *d_workspace, size_t workspace_bytes, float *d_points_out, int capacity, int *d_frame_off_out, void *stream);
+int sessd_prep_box_count(const float *d_points, const int *d_frame_off, int batch, int num_points, const double *d_box_planes,
+                         const int *d_box_off, int num_boxes, int *d_counts, void *stream);
+size_t sessd_prep_box_gather_workspace_bytes(int num_boxes);
+int sessd_prep_box_gather(const float *d_points, const int *d_frame_off, int batch, int num_points, const double *d_box_planes,
+                          const double *d_centres, const int *d_box_off, int num_boxes, const int *d_counts, int num_rows, void *d_workspace,
+                          size_t workspace_bytes, float *d_rows_out, int capacity, int *d_obj_off, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * SURVEY.md 8(f) row 1, first slice of the training step: the supervised SSD-head loss terms, value AND gradient in one pass.
  * Replaces (for the terms without the teacher model) det3d/models/bbox_heads/mg_head_sessd.py:706-760:
  * prepare_loss_weights/NormByNumPositives (:525-572), SigmoidFocalLoss (det3d/models/losses/losses.py:345-420, gamma = 2),

@@ -20,7 +20,7 @@ LAB = {"bevconv_split.cu"}
 OBJ = os.path.join(HERE, "build")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"] + os.environ.get("SESSD_DEFINES", "").split()
-NO_FMA = {"iou3d.cu", "postproc.cu", "assign.cu", "odiou.cu", "kitti_eval.cu", "augment.cu", "gtaug.cu", "sada.cu"}
+NO_FMA = {"iou3d.cu", "postproc.cu", "assign.cu", "odiou.cu", "kitti_eval.cu", "augment.cu", "gtaug.cu", "sada.cu", "kitti_prep.cu"}
 # files whose host code evaluates the collision predicate of csrc/augment.cuh: the host compiler must not contract it into fmas either
 HOST_NO_CONTRACT = {"augment.cu", "gtaug.cu"}
 

@@ -157,3 +157,23 @@ def get_valid_frustum(rect, Trv2c, P2, image_shape):
     frustum = np.linalg.inv(R) @ frustum.T
     frustum = camera_to_lidar(frustum.T, rect, Trv2c)
     return corner_to_surfaces_3d(frustum[np.newaxis, ...])
+
+
+# ------------------------------------------------------------------------------------------------ KITTI data preparation: numpy in and out,
+# membership on the device (sessd_b200.kitti_prep)
+def center_to_corner_box3d(centers, dims, angles=None, origin=(0.5, 0.5, 0.5), axis=2):
+    """[N, 8, 3] box corners (reference :467-509); rotation about z with correctly rounded sin / cos."""
+    from sessd_b200 import kitti_prep
+    return kitti_prep.center_to_corner_box3d(centers, dims, angles, origin, axis)
+
+
+def remove_outside_points(points, rect, Trv2c, P2, image_shape):
+    """The rows of points inside the image frustum, in order (reference :981-992)."""
+    from sessd_b200 import kitti_prep
+    return kitti_prep.remove_outside_points(points, rect, Trv2c, P2, image_shape)
+
+
+def points_in_rbbox(points, rbbox, z_axis=2, origin=(0.5, 0.5, 0.5)):
+    """[N, K] bool membership of points in rotated boxes (reference :1152-1157)."""
+    from sessd_b200 import kitti_prep
+    return kitti_prep.points_in_rbbox(points, rbbox, z_axis, origin)

@@ -133,6 +133,11 @@ SIGNATURES = {
     "sessd_sada_fps": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _i, _vp, _sz, _vp, _i, _vp, _vp]),
     "sessd_sada_swap": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _vp]),
     "sessd_sada_shuffle": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "sessd_prep_frustum_compact_workspace_bytes": (_sz, [_i]),
+    "sessd_prep_frustum_compact": (_i, [_vp, _vp, _i, _i, _vp, _vp, _sz, _vp, _i, _vp, _vp]),
+    "sessd_prep_box_count": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp]),
+    "sessd_prep_box_gather_workspace_bytes": (_sz, [_i]),
+    "sessd_prep_box_gather": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _i, _vp, _sz, _vp, _i, _vp, _vp]),
     "sessd_kitti_convert_workspace_bytes": (_sz, [_ll]),
     "sessd_kitti_convert_detections": (_i, [_vp, _vp, _vp, _vp, _i, _ll, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "sessd_kitti_overlaps": (_i, [C.POINTER(KittiFrames), _i, _i, C.c_double, _vp, _vp]),

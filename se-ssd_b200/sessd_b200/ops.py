@@ -905,3 +905,72 @@ def sada_shuffle(points, frame_off, max_frame_points, perm, out=None):
     check(lib.sessd_sada_shuffle(_p(points), _p(frame_off), int(frame_off.numel() - 1), int(max_frame_points), _p(perm), _p(out), _st()),
           "sessd_sada_shuffle")
     return out
+
+
+# ------------------------------------------------------------------------------------------------ KITTI data preparation
+def _rows16(name, *ts):
+    if any(t is not None and t.data_ptr() % 16 for t in ts):
+        raise ValueError("%s: point rows are read and written as float4 and must be 16-byte aligned" % name)
+
+
+def prep_frustum_compact(points, frame_off, planes, out=None, frame_off_out=None):
+    """The rows of each frame inside its image frustum, bit copies in frame order (sessd_prep_frustum_compact).  points [P,4] f32 with
+    frame_off [B+1] i32, planes [B,6,4] f64.  Returns (out [P,4] f32, frame_off_out [B+1] i32); rows past frame_off_out[B] are unused."""
+    _cuda(points, torch.float32, "points"); _cuda(frame_off, torch.int32, "frame_off"); _cuda(planes, torch.float64, "planes")
+    B = frame_off.numel() - 1
+    P = int(points.shape[0])
+    if B < 1 or points.dim() != 2 or points.shape[1] != 4 or tuple(planes.shape) != (B, 6, 4):
+        raise ValueError("prep_frustum_compact: points [P, 4], frame_off [B+1], planes [B, 6, 4]")
+    dev = points.device
+    if out is None:
+        out = torch.empty((max(P, 1), 4), dtype=torch.float32, device=dev)
+    if frame_off_out is None:
+        frame_off_out = torch.empty((B + 1,), dtype=torch.int32, device=dev)
+    _cuda(out, torch.float32, "out"); _cuda(frame_off_out, torch.int32, "frame_off_out")
+    _rows16("prep_frustum_compact", points, out)
+    ws = torch.empty((max(int(lib.sessd_prep_frustum_compact_workspace_bytes(P)), 16),), dtype=torch.uint8, device=dev)
+    check(lib.sessd_prep_frustum_compact(_p(points), _p(frame_off), int(B), P, _p(planes), _p(ws), ws.numel(), _p(out), int(out.shape[0]),
+                                         _p(frame_off_out), _st()), "sessd_prep_frustum_compact")
+    return out, frame_off_out
+
+
+def prep_box_count(points, frame_off, box_planes, box_off, counts=None):
+    """Points of each box's frame inside the box (sessd_prep_box_count): box_planes [K,6,4] f64, box_off [B+1] i32 (CSR boxes per
+    frame).  Returns counts [K] i32 (device)."""
+    _cuda(points, torch.float32, "points"); _cuda(frame_off, torch.int32, "frame_off"); _cuda(box_planes, torch.float64, "box_planes")
+    _cuda(box_off, torch.int32, "box_off")
+    B = frame_off.numel() - 1
+    K = int(box_planes.shape[0])
+    if B < 1 or points.dim() != 2 or points.shape[1] != 4 or tuple(box_planes.shape[1:]) != (6, 4) or box_off.numel() != B + 1:
+        raise ValueError("prep_box_count: points [P, 4], frame_off [B+1], box_planes [K, 6, 4], box_off [B+1]")
+    if counts is None:
+        counts = torch.empty((max(K, 1),), dtype=torch.int32, device=points.device)
+    _cuda(counts, torch.int32, "counts")
+    _rows16("prep_box_count", points)
+    check(lib.sessd_prep_box_count(_p(points), _p(frame_off), int(B), int(points.shape[0]), _p(box_planes), _p(box_off), K, _p(counts),
+                                   _st()), "sessd_prep_box_count")
+    return counts[:K]
+
+
+def prep_box_gather(points, frame_off, box_planes, centres, box_off, counts, num_rows, out=None, obj_off=None):
+    """Each box's points in frame order as fp32(double(p) - centre) for x y z (sessd_prep_box_gather).  counts: prep_box_count's;
+    num_rows: their host-known sum.  Returns (rows [num_rows, 4] f32, obj_off [K+1] i32 = the exclusive scan of the counts)."""
+    _cuda(points, torch.float32, "points"); _cuda(frame_off, torch.int32, "frame_off"); _cuda(box_planes, torch.float64, "box_planes")
+    _cuda(centres, torch.float64, "centres"); _cuda(box_off, torch.int32, "box_off"); _cuda(counts, torch.int32, "counts")
+    B = frame_off.numel() - 1
+    K = int(box_planes.shape[0])
+    if (B < 1 or points.dim() != 2 or points.shape[1] != 4 or tuple(box_planes.shape[1:]) != (6, 4) or tuple(centres.shape) != (K, 3)
+            or box_off.numel() != B + 1 or counts.numel() < K):
+        raise ValueError("prep_box_gather: shape mismatch")
+    dev = points.device
+    if out is None:
+        out = torch.empty((max(int(num_rows), 1), 4), dtype=torch.float32, device=dev)
+    if obj_off is None:
+        obj_off = torch.empty((K + 1,), dtype=torch.int32, device=dev)
+    _cuda(out, torch.float32, "out"); _cuda(obj_off, torch.int32, "obj_off")
+    _rows16("prep_box_gather", points, out)
+    ws = torch.empty((max(int(lib.sessd_prep_box_gather_workspace_bytes(K)), 16),), dtype=torch.uint8, device=dev)
+    check(lib.sessd_prep_box_gather(_p(points), _p(frame_off), int(B), int(points.shape[0]), _p(box_planes), _p(centres), _p(box_off), K,
+                                    _p(counts), int(num_rows), _p(ws), ws.numel(), _p(out), int(out.shape[0]), _p(obj_off), _st()),
+          "sessd_prep_box_gather")
+    return out[:int(num_rows)], obj_off
