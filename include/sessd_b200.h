@@ -350,7 +350,9 @@ int sessd_nms_sorted(const float *d_boxes, int n, float thresh, int mode, long l
  *   d_bbox_outside_weights [batch,A] (1 on positives), d_pos_anchor / d_pos_gt_id [batch,A]: the first d_num_pos[b]
  *   entries of row b are the positive anchors in ascending order and their GT index (`positive_gt_id`).
  * labels / positive sets are bit-exact against the reference (its mixed fp32/fp64 IoU rounding is reproduced).
- * max_gt <= 1024.  Workspace: sessd_assign_workspace_bytes().
+ * max_gt <= 1024.  Workspace: sessd_assign_workspace_bytes().  num_anchors < 1, batch < 1 or max_gt outside [0, 1024]: SESSD_EINVAL.
+ * A frame uses the first min(d_num_gt[b], max_gt) GT rows: num_gt above max_gt assigns from gt[:max_gt]; num_gt <= 0 (or max_gt 0,
+ * when d_gt_boxes may be null) makes every anchor of the frame background.
  * ------------------------------------------------------------------------------------------------ */
 size_t sessd_assign_workspace_bytes(int num_anchors, int batch, int max_gt);
 int sessd_assign_targets(const float *d_anchors, int num_anchors, const float *d_gt_boxes, const int *d_num_gt, int batch,
@@ -536,7 +538,7 @@ size_t sessd_head_loss_workspace_bytes(int batch);
 /* IoU-prediction term (mg_head_sessd.py:755-768): smooth-L1 of the head's iou output against 2 * aligned-3D-IoU(decoded prediction,
  * decoded target) - 1 on the positives (det3d/core/iou3d/iou3d_utils.py:197-252 as the constant target).  Run AFTER sessd_head_loss on the
  * same stream: reads num_pos from d_losses[b][6], writes the per-frame sum to d_losses[b][5] and d(w_iou * sum / batch) into the iou
- * channels of d_grad_head. */
+ * channels of d_grad_head.  num_anchors must be a multiple of anchors_per_loc (SESSD_EINVAL otherwise, before any launch). */
 /* ODIoU box-regression loss (det3d/models/losses/odious.py:845-900 called from mg_head_sessd.py:770-778; the reference evaluates it with
  * per-box numpy loops on the CPU inside the training step): odiou = 1 - IoU3D + centre distance^2 / (min bounding rectangle diagonal^2 +
  * inter_h^2) + 1.25 (1 - |cos dr|) between the decoded prediction and the decoded target of every positive anchor, weight 1 / num_pos.

@@ -255,8 +255,9 @@ extern "C" size_t sessd_iou_pred_loss_workspace_bytes(int batch) { return batch 
 extern "C" int sessd_iou_pred_loss(const float *d_head, const float *d_anchors, const int *d_labels, const float *d_reg_targets, int batch,
                                    int num_anchors, int anchors_per_loc, int head_stride, float sigma, float w_iou, float *d_losses,
                                    float *d_grad_head, void *workspace, size_t workspace_bytes, void *stream) {
+    // an A that is not a multiple of anchors_per_loc would truncate A / apl in the kernel's row offset and shift every frame after the first
     if (!d_head || !d_anchors || !d_labels || !d_reg_targets || !d_losses || batch < 1 || num_anchors < 1 || anchors_per_loc != 2 ||
-        head_stride < 22 || !(sigma > 0.f))
+        head_stride < 22 || (num_anchors % anchors_per_loc) || !(sigma > 0.f))
         return SESSD_EINVAL;
     if (!workspace || workspace_bytes < sessd_iou_pred_loss_workspace_bytes(batch)) return SESSD_EWORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;

@@ -224,3 +224,89 @@ def assert_tile_lists_match(rec, nbr, n):
             assert np.array_equal(rec[t, pos:pos + len(valid)], want), (t, k)
             pos += len(valid)
         assert not rec[t, kvol:32].any()
+
+
+# ------------------------------------------------------------------------------------------------ assigner edge cases
+F32_PI4 = np.float32(np.pi / 4)
+# GT yaws and anchor yaws where the near-bbox w / l swap (|limit_period(r, 0.5, pi)| > pi / 4) or limit_period's floor changes
+EDGE_YAWS = np.float32([F32_PI4, np.nextafter(F32_PI4, np.float32(1)), np.nextafter(F32_PI4, np.float32(0)), -F32_PI4,
+                        np.float32(3 * np.pi / 4), np.float32(-3 * np.pi / 4),
+                        np.float32(np.pi / 2), np.nextafter(np.float32(np.pi / 2), np.float32(2)),
+                        np.nextafter(np.float32(np.pi / 2), np.float32(0)), np.float32(-np.pi / 2),
+                        np.nextafter(np.float32(-np.pi / 2), np.float32(-2)), np.nextafter(np.float32(-np.pi / 2), np.float32(0))])
+# one GT per frame on the KITTI grid: (anchor, IoU with that anchor under the reference's rounding, GT).  The GT is centred on another
+# anchor (its best), so the forced rule cannot label the listed anchor; found by a search over the GT's x and l with the numpy oracle.
+ASSIGN_THRESHOLD_GTS = (
+    (17600, np.float32(0.6), [0.5999999642372131, -19.799999237060547, -1.0, 1.600000023841858, 3.9000000953674316, 1.559999942779541, 0.0]),
+    (17600, np.nextafter(np.float32(0.6), np.float32(0)),
+     [0.6000000238418579, -19.799999237060547, -1.0, 1.600000023841858, 3.9000000953674316, 1.559999942779541, 0.0]),
+    (17600, np.nextafter(np.float32(0.6), np.float32(1)),
+     [0.5999999046325684, -19.799999237060547, -1.0, 1.600000023841858, 3.9000000953674316, 1.559999942779541, 0.0]),
+    (21120, np.float32(0.45), [0.8068957328796387, -15.800000190734863, -1.0, 1.600000023841858, 3.900005340576172, 1.559999942779541, 0.0]),
+    (21120, np.nextafter(np.float32(0.45), np.float32(0)),
+     [0.8068965673446655, -15.800000190734863, -1.0, 1.600000023841858, 3.9000000953674316, 1.559999942779541, 0.0]),
+    (21120, np.nextafter(np.float32(0.45), np.float32(1)),
+     [0.8068965077400208, -15.800000190734863, -1.0, 1.600000023841858, 3.9000000953674316, 1.559999942779541, 0.0]),
+)
+# (anchor i, anchor j, GT index) pairs with bit-identical IoUs across a CTA boundary (line anchors), and (best, one ulp lower) pairs
+LINE_TIES = ((255, 256, 0), (511, 512, 1))
+LINE_NEAR_TIES = ((255, 256, 0),)
+
+
+def line_anchors(A, near=False):
+    """A custom anchors on a line: x = 0.5 i - 128, y = 0, w 1.5, l 4, h 1.5, yaw 0 -- dyadic, so the IoUs of a GT centred between two
+    anchors are bit-identical; the first len(EDGE_YAWS) anchors take the boundary yaws.  near: anchor 256 one ulp wider, so the GT
+    between 255|256 has its best anchor in CTA 0 and the next best, one ulp lower, in CTA 1."""
+    anc = np.zeros((513, 7), np.float32)
+    anc[:, 0] = np.float32(0.5) * np.arange(513, dtype=np.float32) - np.float32(128)
+    anc[:, 2] = -1.0
+    anc[:, 3:6] = np.float32([1.5, 4.0, 1.5])
+    anc[:len(EDGE_YAWS), 6] = EDGE_YAWS
+    if near:
+        anc[256, 3] = np.nextafter(np.float32(1.5), np.float32(2))
+    return np.ascontiguousarray(anc[:A])
+
+
+def assign_edge_cases():
+    """(name, anchors [A, 7], per-frame GT lists [[M_f, 7]], matched, unmatched) of the assigner's edge cases (tests/golden/
+    assign_edge_cases.npz; the generator asserts every crafted condition in the reference's own overlap matrix)."""
+    from oracle import anchors as oa
+    kitti = oa.create_anchors_3d_range().reshape(-1, 7)
+    f32 = np.float32
+    out = []
+    thr = [np.float32([g]) for _, _, g in ASSIGN_THRESHOLD_GTS]
+    out.append(("thresholds", kitti, thr, 0.6, 0.45))
+    out.append(("thresholds_05_05", kitti, thr, 0.5, 0.5))
+    out.append(("thresholds_07_03", kitti, thr, 0.7, 0.3))
+    # yaw boundaries on GTs over the KITTI grid, in three rows of four
+    yg = np.zeros((len(EDGE_YAWS), 7), f32)
+    for i, r in enumerate(EDGE_YAWS):
+        yg[i] = [10.0 + 6.0 * (i % 4), -20.0 + 12.0 * (i // 4), -1.0, 1.6, 3.9, 1.56, r]
+    out.append(("yaw_boundaries", kitti, [yg], 0.6, 0.45))
+    # line anchors: exact ties across CTAs 0|1 and 1|2, GTs over the boundary-yaw anchors, every anchor count
+    tie = f32([[-0.25, 0, -1, 1.5, 4.0, 1.5, 0], [127.75, 0, -1, 1.5, 4.0, 1.5, 0]])
+    over_yaws = f32([[-128.0 + 0.5 * i + 0.1, 0.3, -1, 1.6, 3.9, 1.5, EDGE_YAWS[(i + 3) % len(EDGE_YAWS)]] for i in range(0, 12, 3)])
+    line = line_anchors(513)
+    # tie IoUs are 0.714: with matched 0.8 / unmatched 0.75 only the forced rule labels the tied anchors positive
+    out.append(("line513", line, [np.concatenate([tie, over_yaws]), f32([[-0.25, 0, -1, 1.5, 4.0, 1.5, 0]])], 0.8, 0.75))
+    out.append(("line513_near_ties", line_anchors(513, near=True), [tie[:1]], 0.8, 0.75))
+    for A in (1, 255, 256, 257):
+        g = f32([[-128.0, 0, -1, 1.5, 4.0, 1.5, 0], [0.5 * (A - 1) - 128.25, 0.2, -1, 1.5, 4.0, 1.5, 0.1],
+                 [0.5 * (A // 2) - 128, 0, -1, 1.5, 4.0, 1.5, EDGE_YAWS[4]]])
+        out.append(("line%d" % A, line_anchors(A), [g], 0.6, 0.45))
+    # KITTI grid, positives only at anchors >= 65 536 (CTAs 256-274): GTs in the rows y >= 35.2
+    hi = f32([[5.0 + 9.0 * i, 36.0 + 1.2 * (i % 3), -1.0, 1.6, 3.9, 1.56, 0.4 * i] for i in range(7)])
+    out.append(("kitti_high", kitti, [hi], 0.6, 0.45))
+    # GT sets: 1024 GTs in one frame (the shared-memory stage's limit), duplicates, a GT without any overlap, a GT equal to an anchor
+    rng = np.random.default_rng(41)
+    many = np.zeros((1024, 7), f32)
+    many[:, 0], many[:, 1] = rng.uniform(0.5, 70, 1024), rng.uniform(-39.5, 39.5, 1024)
+    many[:, 2], many[:, 3:6] = -1.0, rng.uniform([0.5, 0.6, 1.4], [2.0, 4.8, 1.8], (1024, 3))
+    many[:, 6] = rng.uniform(-np.pi, np.pi, 1024)
+    many[1000:1010] = many[500:510]                                       # duplicates: argmax ties resolve to the first
+    many[1010] = [-30.0, 0, -1, 1.6, 3.9, 1.56, 0]                       # no overlap with any anchor
+    many[1011] = kitti[12345]
+    misc = f32([[-30.0, 0, -1, 1.6, 3.9, 1.56, 0], kitti[777], kitti[777], kitti[40001], [30.0, 10.0, -1, 1.6, 3.9, 1.56, 1.0],
+                [30.0, 10.0, -1, 1.6, 3.9, 1.56, 1.0]])
+    out.append(("gt_sets", kitti, [many, misc], 0.6, 0.45))
+    return out

@@ -9,6 +9,7 @@ so only outputs -- or their hashes when large -- are stored):
   voxel_cases.npz      reference numba voxeliser (point_cloud_ops_v2.py) on 7 seeded / edge-case clouds
   iou_cases.npz        reference iou3d_cpu.cpp (compiled in place -> oracle/_ref): overlap / IoU matrices
   anchors_assign.npz   reference AnchorGeneratorRange + TargetAssigner.assign_v2 (12 seeded GT boxes)
+  assign_edge_cases.npz  reference create_target_np on the assigner's edge cases (cases.assign_edge_cases)
   decode_case.npz      reference box_torch_ops.second_box_decode
   ssfa_head_case.npz   reference SSFA + Head modules (rpn_v1.py, mg_head_sessd.py) with seeded state dicts
   vfe_case.npz         reference VoxelFeatureExtractorV3
@@ -203,6 +204,56 @@ def gen_anchors_assign():
     print("decode", dec.shape)
 
 
+def gen_assign_edges():
+    """The assigner's edge cases (cases.assign_edge_cases) through the REFERENCE's create_target_np with its nearest-BEV similarity and
+    second_box_encode, thresholds as the fp32 per-anchor arrays assign_v2 passes.  Every crafted condition is asserted in the reference's
+    own overlap matrix before anything is written; labels are stored as int8, targets for the positives only."""
+    from cases import ASSIGN_THRESHOLD_GTS, EDGE_YAWS, LINE_NEAR_TIES, LINE_TIES, assign_edge_cases
+    bn = sys.modules["det3d.core.bbox.box_np_ops"]
+    rs = sys.modules["det3d.core.bbox.region_similarity"]
+    to = sys.modules["det3d.core.anchor.target_ops_v2"]
+    sim = rs.NearestIouSimilarity()
+
+    def similarity_fn(anchors, gt):
+        return sim.compare(anchors[:, [0, 1, 3, 4, -1]], gt[:, [0, 1, 3, 4, -1]])
+    out = {}
+    for name, anc, frames, matched, unmatched in assign_edge_cases():
+        A = anc.shape[0]
+        out[name + "_inputs_sha"] = sha(np.concatenate([anc.reshape(-1)] + [g.reshape(-1) for g in frames]))
+        for f, gt in enumerate(frames):
+            ov = similarity_fn(anc, gt)
+            if name == "thresholds":
+                a, want, _ = ASSIGN_THRESHOLD_GTS[f]
+                assert ov[a, 0] == want and ov[:, 0].max() > want and ov[:, 0].argmax() != a, (name, f)
+            if name == "line513" and f == 0:
+                for i, j, g in LINE_TIES:
+                    assert ov[i, g] == ov[j, g] == ov[:, g].max() and i // 256 != j // 256, (name, i, j)
+            if name == "line513_near_ties":
+                for i, j, g in LINE_NEAR_TIES:
+                    assert ov[i, g] == ov[:, g].max() and ov[j, g] == np.nextafter(ov[i, g], np.float32(-1)) and i // 256 != j // 256
+            if name == "yaw_boundaries":
+                r = np.abs(bn.limit_period(gt[:, 6], 0.5, np.pi))
+                assert (r > np.pi / 4).any() and (r <= np.pi / 4).any() and np.array_equal(gt[:, 6], EDGE_YAWS)
+            if name == "gt_sets" and f == 0:
+                assert len(gt) == 1024 and ov[:, 1010].max() == 0 and ov[12345, 1011] == 1
+            r = to.create_target_np(anc, gt, similarity_fn, bn.second_box_encode, gt_classes=np.ones(len(gt), np.int32),
+                                    matched_threshold=np.full(A, matched, np.float32), unmatched_threshold=np.full(A, unmatched, np.float32))
+            pos = np.nonzero(r["labels"] > 0)[0]
+            if name == "kitti_high":
+                assert len(pos) and pos.min() >= 65536
+            if name == "line513" and f == 1:
+                assert np.array_equal(pos, [255, 256])
+            if name == "line513_near_ties":
+                assert 255 in pos and 256 not in pos
+            k = "%s_%d_" % (name, f)
+            out[k + "labels"] = r["labels"].astype(np.int8)
+            out[k + "pos_idx"] = pos.astype(np.int32)
+            out[k + "pos_targets"] = r["bbox_targets"][pos]
+            out[k + "positive_gt_id"] = np.asarray(r["positive_gt_id"], np.int32)
+            print("assign edge", name, f, "A", A, "gt", len(gt), "pos", len(pos), "neg", int((r["labels"] == 0).sum()))
+    np.savez_compressed(os.path.join(HERE, "assign_edge_cases.npz"), **out)
+
+
 def gen_wire():
     """KITTI wire format: reference box_np_ops.get_valid_frustum / box_camera_to_lidar / change_box3d_center_ on a synthetic calibration."""
     bn = sys.modules.get("det3d.core.bbox.box_np_ops") or _load("det3d.core.bbox.box_np_ops", "det3d/core/bbox/box_np_ops.py")
@@ -375,6 +426,7 @@ if __name__ == "__main__":
     install_det3d_shims()
     if not only or "assign" in only:
         gen_anchors_assign()
+        gen_assign_edges()
     if not only or "odiou" in only:
         gen_odiou()
     if not only or "loss" in only:

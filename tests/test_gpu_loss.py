@@ -99,30 +99,3 @@ def test_multigrouphead_loss_supervised_from_config():
     np.testing.assert_allclose(float(out["dir_loss_reduced"]), float(0.2 * o["dir"].sum() / 2), rtol=2e-5)
     assert out["grad_head"].shape == preds[0]["_packed"].shape and bool(torch.isfinite(out["grad_head"]).all())
 
-
-def test_iou_prediction_loss_matches_oracle():
-    """IoU-prediction term: decode + aligned rotated 3-D IoU + smooth-L1 on the positives (value, gradient into the iou channels)."""
-    from oracle import anchors as oa, loss_ref
-    from sessd_b200 import ops
-    head, anc, labels, targets = head_loss_case()
-    head = head.copy()
-    head[..., :14] *= 0.2                                    # predictions near the targets' scale => non-trivial IoUs
-    for b in range(2):                                       # half of the positives: prediction = target + noise => IoU ~ 0.5-0.9
-        pos = np.nonzero(labels[b] > 0)[0][::2]
-        hv = head[b].reshape(-1)
-        for a in pos:
-            base = (a // 2) * 24 + 7 * (a % 2)
-            hv[base:base + 7] = targets[b, a] + 0.03 * np.sin(np.arange(7) + a)
-    d = lambda x: torch.from_numpy(np.ascontiguousarray(x)).cuda()   # noqa: E731
-    losses, grad = ops.head_loss(d(head), d(anc), d(labels), d(targets), w_iou=1.0)
-    torch.cuda.synchronize()
-    h = torch.from_numpy(head).clone().requires_grad_(True)
-    box, cls, dr = loss_ref.split_head(h)
-    iou_p = h[..., 20:22].reshape(2, -1)
-    o = loss_ref.iou_pred_loss(iou_p, box, torch.from_numpy(anc), torch.from_numpy(labels).long(), torch.from_numpy(targets))
-    (o.sum() / 2).backward()
-    np.testing.assert_allclose(losses[:, 5].cpu().numpy(), o.detach().numpy(), rtol=1e-4, atol=1e-6)
-    assert float(o.detach().min()) > 0.0
-    G = grad.cpu().numpy()
-    np.testing.assert_allclose(G[..., 20:22], h.grad.numpy()[..., 20:22], rtol=1e-4, atol=1e-8)
-    assert np.abs(G[..., 20:22]).sum() > 0 and not G[..., 22:].any()

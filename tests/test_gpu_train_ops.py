@@ -9,6 +9,8 @@ tests/train_ops_model.py).
 * sessd_axpby / sessd_grad_sqnorm / sessd_adamw_clip_ema_step on plain tensors of sizes that reach the float4 tails and the
   single-chunk norm, against fp64 or the same fp32 expression evaluated by torch.  The C entry points are called on buffers 4-8
   elements longer than n (n = 0 included: a valid pointer, nothing to do), so writes past n would show.
+* sessd_iou_pred_loss: every crafted case of train_ops_model.iou_pred_cases() against the fp64 aligned 3-D IoU reference and the fp32
+  twin, on a NaN-filled gradient; an odd anchor count is refused before any launch.
 * sessd_odiou_loss: where the positives sit (anchor 0, A - 1, past the grid-stride wrap), an empty frame, a clamped prediction and
   accumulation into a pre-filled gradient, against the host twin of odiou.cuh."""
 import numpy as np
@@ -24,7 +26,8 @@ def _d(a):
     return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
-def _head_loss_poisoned(head, anc, labels, targets, cfg, with_grad=True):
+def _head_loss_poisoned(head, anc, labels, targets, cfg, with_grad=True, w_iou=None):
+    """sessd_head_loss (then sessd_iou_pred_loss when w_iou is given) into NaN-filled outputs"""
     from sessd_b200 import _lib, ops
     B, A = labels.shape
     h, a, lab, tg = _d(head), _d(anc), _d(labels), _d(targets)
@@ -36,6 +39,11 @@ def _head_loss_poisoned(head, anc, labels, targets, cfg, with_grad=True):
                                         float(c.dir_offset), float(c.pos_cls_weight), float(c.neg_cls_weight), float(c.w_cls),
                                         float(c.w_loc), float(c.w_dir), ops._p(losses), ops._p(grad), ops._p(ws), ws.numel(), ops._st()),
                "sessd_head_loss")
+    if w_iou is not None:
+        ws2 = torch.empty((_lib.lib.sessd_iou_pred_loss_workspace_bytes(B),), dtype=torch.uint8, device="cuda")
+        _lib.check(_lib.lib.sessd_iou_pred_loss(ops._p(h), ops._p(a), ops._p(lab), ops._p(tg), B, A, 2, head.shape[2], float(c.sigma),
+                                                float(w_iou), ops._p(losses), ops._p(grad), ops._p(ws2), ws2.numel(), ops._st()),
+                   "sessd_iou_pred_loss")
     torch.cuda.synchronize()
     return losses.cpu().numpy(), (grad.cpu().numpy() if with_grad else None)
 
@@ -58,6 +66,65 @@ def test_head_loss_crafted_cases_within_fp64_bounds():
         again, grad2 = _head_loss_poisoned(head, anc, labels, targets, cfg)
         assert np.array_equal(again[:, [0, 1, 2, 3, 4, 6, 7]], losses[:, [0, 1, 2, 3, 4, 6, 7]]) and np.array_equal(grad2, grad), name
     print("head loss: worst error / bound, losses %.3g, gradient %.3g" % tuple(worst))
+
+
+# ------------------------------------------------------------------------------------------------ IoU-prediction loss
+def test_iou_pred_crafted_cases_within_fp64_bounds():
+    """sessd_iou_pred_loss behind sessd_head_loss on every case of train_ops_model.iou_pred_cases() (degenerate pairs, knee residuals,
+    positives at anchor 0, A - 1 and past the grid-stride wrap, an empty frame, a ragged batch of 5, strides 22 / 24 / 32, sigma 3 / 1,
+    w_iou 1 / 0.5), into a NaN-filled gradient: the iou channels of the positives within iou_pred_bounds of the fp64 reference and within
+    twice that of the fp32 twin, those of every other anchor exactly 0; every other gradient channel and every other loss column
+    bit-identical to the run without the IoU term; losses[:, 5] within the sum bound; two runs bitwise equal."""
+    worst = [0.0, 0.0, 0.0]
+    keep = [0, 1, 2, 3, 4, 6, 7]
+    for name, head, anc, labels, targets, sigma, w_iou in tm.iou_pred_cases():
+        cfg = tm.HeadCfg(sigma=sigma)
+        rs, rg, info = tm.iou_pred_ref(head, anc, labels, targets, sigma, w_iou)
+        sb, gb = tm.iou_pred_bounds(info)
+        es, eg = tm.iou_pred_emul(head, anc, labels, targets, sigma, w_iou)
+        base, gbase = _head_loss_poisoned(head, anc, labels, targets, cfg)
+        losses, grad = _head_loss_poisoned(head, anc, labels, targets, cfg, w_iou=w_iou)
+        assert np.isfinite(grad).all() and np.isfinite(losses).all(), name
+        pos = labels > 0
+        assert not grad[..., 20:22].reshape(labels.shape)[~pos].any(), name
+        other = np.ones(head.shape[2], bool)
+        other[20:22] = False
+        assert np.array_equal(grad[..., other], gbase[..., other]), name
+        assert np.array_equal(losses[:, keep], base[:, keep]), name
+        assert (losses[~pos.any(1), 5] == 0).all(), name
+        g_iou = np.zeros_like(grad)
+        sel = (info["b"], info["a"] // 2, 20 + info["r"])
+        g_iou[sel] = grad[sel]
+        rv, rgr = tm.iou_pred_violations(losses[:, 5], g_iou, rs, rg, sb, gb)
+        assert rv <= 1.0 and rgr <= 1.0, (name, rv, rgr)
+        ts, tg_ = tm.iou_pred_violations(losses[:, 5], g_iou, es.astype(np.float64), eg.astype(np.float64), sb, gb, scale=2.0)
+        assert ts <= 1.0 and tg_ <= 1.0, (name, ts, tg_)
+        worst = [max(worst[0], rv), max(worst[1], rgr), max(worst[2], ts, tg_)]
+        again, grad2 = _head_loss_poisoned(head, anc, labels, targets, cfg, w_iou=w_iou)
+        assert np.array_equal(again, losses) and np.array_equal(grad2, grad), name
+    print("iou prediction device: worst error / bound, sums %.3g, gradient vs fp64 %.3g, vs twin (2x bound) %.3g" % tuple(worst))
+
+
+def test_iou_pred_refuses_odd_anchor_count():
+    """num_anchors not a multiple of anchors_per_loc: SESSD_EINVAL before any launch (the outputs keep their fill)"""
+    from sessd_b200 import _lib, ops
+    B, A, S = 2, 7, 24
+    h = torch.zeros((B, A // 2 + 1, S), device="cuda")
+    a = torch.zeros((A + 1, 7), device="cuda")
+    lab = torch.ones((B, A + 1), dtype=torch.int32, device="cuda")
+    tg = torch.zeros((B, A + 1, 7), device="cuda")
+    losses = torch.full((B, 8), 7.0, device="cuda")
+    grad = torch.full_like(h, 7.0)
+    ws = torch.empty((_lib.lib.sessd_iou_pred_loss_workspace_bytes(B),), dtype=torch.uint8, device="cuda")
+    rc = _lib.lib.sessd_iou_pred_loss(ops._p(h), ops._p(a), ops._p(lab), ops._p(tg), B, A, 2, S, 3.0, 1.0, ops._p(losses), ops._p(grad),
+                                      ops._p(ws), ws.numel(), ops._st())
+    torch.cuda.synchronize()
+    assert rc == -1                                                              # SESSD_EINVAL
+    assert bool((losses == 7.0).all()) and bool((grad == 7.0).all())
+    rc = _lib.lib.sessd_iou_pred_loss(ops._p(h), ops._p(a), ops._p(lab), ops._p(tg), B, A + 1, 2, S, 3.0, 1.0, ops._p(losses), ops._p(grad),
+                                      ops._p(ws), ws.numel(), ops._st())
+    torch.cuda.synchronize()
+    assert rc == 0
 
 
 # ------------------------------------------------------------------------------------------------ optimiser kernels

@@ -326,3 +326,22 @@ def test_neck_dgrad_restatement_equals_autograd():
     G = rnd(*y.shape)
     (y * G).sum().backward()
     torch.testing.assert_close(BG.deconv_dgrad(G, wd), x.grad, rtol=1e-12, atol=1e-12)
+
+
+def test_assign_oracle_matches_reference_edge_golden(golden_dir):
+    """oracle.anchors.assign_targets (which other GPU tests use as their reference) equals the reference's create_target_np bit for bit on
+    the assigner's edge cases: IoUs exactly on fp32(0.6) / fp32(0.45) and one ulp either side, pi/4 and limit_period yaw boundaries on
+    GTs and anchors, ties across CTAs, A = 1 / 255 / 256 / 257 / 513, positives past anchor 65 536, 1024 GTs, non-default thresholds"""
+    from cases import assign_edge_cases
+    from oracle import anchors as oa
+    g = np.load(os.path.join(golden_dir, "assign_edge_cases.npz"))
+    for name, anc, frames, matched, unmatched in assign_edge_cases():
+        assert np.array_equal(g[name + "_inputs_sha"], sha(np.concatenate([anc.reshape(-1)] + [x.reshape(-1) for x in frames]))), name
+        for f, gt in enumerate(frames):
+            r = oa.assign_targets(anc, gt, np.float32(matched), np.float32(unmatched))
+            k = "%s_%d_" % (name, f)
+            pos = np.nonzero(r["labels"] > 0)[0]
+            assert np.array_equal(r["labels"], g[k + "labels"]), k
+            assert np.array_equal(pos, g[k + "pos_idx"]), k
+            assert np.array_equal(r["bbox_targets"][pos], g[k + "pos_targets"]), k
+            assert np.array_equal(r["positive_gt_id"], g[k + "positive_gt_id"]), k

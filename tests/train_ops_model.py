@@ -1,5 +1,5 @@
-"""fp64 references, fp32 numpy emulations and error bounds of the SE-SSD supervised head loss (csrc/headloss.cu)
-and the ODIoU loss (csrc/odiou.cuh, odiou.cu); shared by tests/test_train_ops_model.py (CPU) and tests/test_gpu_train_ops.py.
+"""fp64 references, fp32 numpy emulations and error bounds of the SE-SSD supervised head loss (csrc/headloss.cu), the IoU-prediction
+loss (csrc/iou3d.cu) and the ODIoU loss (csrc/odiou.cuh, odiou.cu); shared by tests/test_train_ops_model.py (CPU) and tests/test_gpu_train_ops.py.
 
 Notation: u = 2^-24 (fp32 unit roundoff); an fp32 operation rounds its exact result r to r (1 + e), |e| <= u; one ulp of r is at most
 2u |r|.  expf / logf / log1pf / sinf / cosf of CUDA (and numpy's float32 versions in the emulations) are within 2 ulp = 4u relative.
@@ -43,6 +43,37 @@ per-frame sums: each partial sum the kernel forms is a sum of a subset of the te
 steps per thread at A <= 74 * 256 * 4, + 7 box components, 5 shuffle levels, 8 warps, 74 block partials => D = 98 and
         |d S| <= sum_a E_a + D u sum_a |term_a|.
 The iou and padding channels of the gradient are written as exact zeros; counts are exact.
+
+IoU-prediction loss (sessd_iou_pred_loss, iou_pred_loss_kernel in csrc/iou3d.cu), per positive, against iou_pred_ref
+---------------------------------------------------------------------------------------------------------------------
+iou_pred_ref decodes the prediction and the target in fp64 (second_box_decode), builds the BEV rectangles [x -+ w/2, y -+ l/2] rotated
+clockwise by r as rb_spin does (not the ODIoU corner convention), takes their exact convex intersection (_od_inter_area), the height
+overlap about the z centres and the union clamped at 1e-7, then smooth-L1 of the iou head value h against the constant 2 IoU - 1 with
+weight rw = 1 / max(num_pos, 1); the gradient into channel 20 + r is scaled by w_iou / B.  With R = the largest |x|, |y| of the two
+centres and the anchor's plus half the larger BEV diagonal:
+  * decode: diag = sqrtf(l^2 + w^2) (2 products, the add, sqrtf: 3u), x = e diag + x_a: 4u |e diag| + u |x| <= 9u R; w = expf(e) w_a:
+    5u relative; r = e + r_a: u |r|.
+  * corners: x -+ w/2, the recomputed centre, p - c, cosf / sinf (2 ulp each, argument error u |r|), two products, the sum and + c: the
+    absolute error of every corner coordinate is a cancellation between centres up to ~70 m and offsets of 0.25-2 m, counted on R:
+        E_p = u R (24 + |r_q| + |r_g|).
+  * area: the intersection of two convex polygons whose edges each move by <= E_p changes by <= E_p per unit length of its boundary, and
+    that boundary is no longer than the smaller perimeter P_min; a crossing of two nearly parallel edges is ill-conditioned along the
+    edges (~ 1 / sin of the angle) but moves inside the thin wedge between them, so it stays within the same band.  rb_inside admits a
+    corner up to m = 1e-5 outside the other rectangle (its margin), which adds at most m x P_min -- counted only where some corner lies
+    within m + 2 E_p of the other rectangle's boundary.  The shoelace fan sums <= 24 cross products of differences <= D (the smaller
+    BEV diagonal): 72u D^2.
+        E_A = (2 E_p + [near] m) P_min + 72u D^2.
+  * height: z -+ h/2 per box (decode of z and h, the half, the add): E_zb = u (2 |z| + |z_a| + 3h); E_ih = 2 max(E_zb) + u ih.
+  * ov3 = ov ih: E_ov3 = E_A ih + ov E_ih + E_A E_ih + u ov ih; volumes (three 5u dimensions, two products): 17u v; the union's two adds:
+    E_Un = 19u (v_q + v_g) + E_ov3; the quotient: E_I = (E_ov3 + IoU E_Un) / (Un - E_Un) + u IoU; the target 2 IoU - 1: E_t = 2 E_I + u.
+  * smooth-L1 of d = h - t: E_d = E_t + u |d|.  The gradient sigma^2 d or sign(d) is continuous at the knee k = 1 / sigma^2 (fp32(k) in
+    the kernel: + u k) but its sign flips at d = 0, so the bar is absolute:
+        |d g| <= rw (w_iou / B) sigma^2 (E_d + u k) + 4u |g|,     value: rw (min(sigma^2 |d|, 1) E_d + sigma^2 E_d^2 + u k) + 4u |f|.
+  * per-frame sums: <= ceil(A / 18 944) grid-stride steps per thread (74 CTAs x 256), 5 shuffle levels, 8 warps, 74 block partials:
+        |d S| <= sum E_f + (ceil(A / 18 944) + 87) u sum |f|.
+A disjoint pair or a pair without height overlap has IoU exactly 0 in both fp32 and fp64 (target exactly -1); an encoded dimension of
+-104 underflows expf to a zero-size box (target -1 up to the shoelace term).  The fp32 twin iou_pred_emul (the C oracle's decode and
+overlap) passes these bounds; IP_MUTANTS are the planted mistakes each of which fails at least one crafted case.
 
 ODIoU: odiou_ref (fp64 restatement of odiou.cuh) and odiou_bounds, derived in its docstring.  The optimiser kernels' references and
 bounds sit beside their tests (tests/test_gpu_train_ops.py).
@@ -349,7 +380,7 @@ def _od_corners(x, y, w, l, r):
 
 
 def _od_inter_area(clip, subj, zero):
-    """Sutherland-Hodgman clip of subj against the clockwise rectangle clip, shoelace area"""
+    """Sutherland-Hodgman clip of subj against the clockwise rectangle clip, shoelace area (torch or numpy scalars)"""
     a = list(subj)
     for e in range(4):
         if not a:
@@ -374,7 +405,7 @@ def _od_inter_area(clip, subj, zero):
     for i in range(len(a)):
         p, q = a[i], a[(i + 1) % len(a)]
         s2 = s2 + (p[0] * q[1] - q[0] * p[1])
-    return torch.abs(s2) * 0.5
+    return abs(s2) * 0.5
 
 
 def _od_mbr_diag(pts, zero):
@@ -484,3 +515,290 @@ def odiou_bounds(gboxes, qboxes, grad_ref):
     S = np.minimum(np.minimum(gc[:, 3], gc[:, 4]), np.minimum(qc[:, 3], qc[:, 4]))
     k = (R / S) ** 2
     return ODIOU_C_VAL * U * k, ODIOU_C_GRAD * U * k * (np.abs(grad_ref).max(1) + 1.0 / S)
+
+
+# ------------------------------------------------------------------------------------------------ IoU prediction (iou_pred_loss_kernel)
+IP_CTA_SPAN = 74 * 256                                            # anchors one grid-stride step of iou_pred_loss_kernel covers
+IP_MARGIN = 1e-5                                                  # rb_inside's margin (rotbox.cuh)
+
+
+def _ip_decode64(e, an):
+    """second_box_decode in fp64 of fp32 encodings e [n, 7] against fp32 anchors an [n, 7]"""
+    e, an = e.astype(np.float64), an.astype(np.float64)
+    diag = np.sqrt(an[:, 4] ** 2 + an[:, 3] ** 2)
+    return np.stack([e[:, 0] * diag + an[:, 0], e[:, 1] * diag + an[:, 1], e[:, 2] * an[:, 5] + an[:, 2], np.exp(e[:, 3]) * an[:, 3],
+                     np.exp(e[:, 4]) * an[:, 4], np.exp(e[:, 5]) * an[:, 5], e[:, 6] + an[:, 6]], 1)
+
+
+def _ip_corners(b):
+    """the BEV rectangle [x -+ w/2, y -+ l/2] rotated clockwise by r about its centre (rb_spin), corners in rb_spin's order"""
+    x, y, w, l, r = (np.float64(b[k]) for k in (0, 1, 3, 4, 6))
+    c, s = np.cos(r), np.sin(r)
+    out = []
+    for px, py in ((-w / 2, -l / 2), (w / 2, -l / 2), (w / 2, l / 2), (-w / 2, l / 2)):
+        out.append((px * c + py * s + x, -px * s + py * c + y))
+    return out
+
+
+def _ip_outside(p, b):
+    """Chebyshev distance by which point p lies outside rectangle b in b's own frame (negative: inside), as rb_inside measures it"""
+    c, s = np.cos(b[6]), np.sin(b[6])
+    dx, dy = p[0] - b[0], p[1] - b[1]
+    lx, ly = dx * c - dy * s, dx * s + dy * c                     # undo the clockwise rotation
+    return max(abs(lx) - b[3] / 2, abs(ly) - b[4] / 2)
+
+
+def iou3d_aligned_ref(q, g):
+    """fp64 aligned 3-D IoU of box rows q, g [n, 7] (decoded): exact convex BEV intersection of the rb_spin rectangles, the height
+    overlap about the z centres, the union clamped at 1e-7 (iou3d_utils.py:197-252).  Returns (iou [n], bev overlap [n], ih [n])."""
+    n = len(q)
+    iou, ov, ih = np.zeros(n), np.zeros(n), np.zeros(n)
+    for i in range(n):
+        cg = _ip_corners(g[i])[::-1]                               # rb_spin's order is counter-clockwise; the clip wants clockwise
+        ov[i] = _od_inter_area(cg, _ip_corners(q[i]), np.float64(0))
+        ih[i] = max(min(q[i, 2] + q[i, 5] / 2, g[i, 2] + g[i, 5] / 2) - max(q[i, 2] - q[i, 5] / 2, g[i, 2] - g[i, 5] / 2), 0.0)
+        ov3 = ov[i] * ih[i]
+        iou[i] = ov3 / max(q[i, 3] * q[i, 4] * q[i, 5] + g[i, 3] * g[i, 4] * g[i, 5] - ov3, 1e-7)
+    return iou, ov, ih
+
+
+def _ip_positives(head, labels):
+    """(frame, anchor, slot) index arrays of the positives, in frame-major ascending-anchor order"""
+    b, a = np.nonzero(labels > 0)
+    return b, a, a % 2
+
+
+def iou_pred_ref(head, anchors, labels, targets, sigma=3.0, w_iou=1.0):
+    """fp64 reference of sessd_iou_pred_loss on the fp32 inputs: (sums [B], grad [B, P, S], per-positive details for iou_pred_bounds).
+    grad holds d (w_iou * sum / B) / d head in the iou channels 20 + r of the positives and zero elsewhere."""
+    B, P, S = head.shape
+    bi, ai, ri = _ip_positives(head, labels)
+    an = anchors[ai]
+    e = np.stack([head[bi, ai // 2, 7 * ri + k] for k in range(7)], 1)
+    q, g = _ip_decode64(e, an), _ip_decode64(targets[bi, ai], an)
+    iou, ov, ih = iou3d_aligned_ref(q, g)
+    h = head[bi, ai // 2, 20 + ri].astype(np.float64)
+    t = 2.0 * iou - 1.0
+    d = h - t
+    k, s2 = 1.0 / sigma ** 2, sigma ** 2
+    npos = np.maximum((labels > 0).sum(1), 1).astype(np.float64)
+    rw = 1.0 / npos[bi]
+    f = np.where(np.abs(d) <= k, 0.5 * s2 * d * d, np.abs(d) - 0.5 * k) * rw
+    fp = np.where(np.abs(d) <= k, s2 * d, np.sign(d)) * rw * w_iou / B
+    sums = np.zeros(B)
+    np.add.at(sums, bi, f)
+    grad = np.zeros((B, P, S))
+    grad[bi, ai // 2, 20 + ri] = fp
+    info = dict(b=bi, a=ai, r=ri, an=an.astype(np.float64), q=q, g=g, iou=iou, ov=ov, ih=ih, d=d, f=f, fp=fp, rw=rw, sigma=sigma,
+                w_iou=w_iou, B=B, A=labels.shape[1], shape=head.shape)
+    return sums, grad, info
+
+
+def iou_pred_bounds(info):
+    """(sum bound [B], gradient bound [B, P, S]) of the module docstring's IoU-prediction section, from iou_pred_ref's details"""
+    u = U
+    q, g, an = info["q"], info["g"], info["an"]
+    n = len(q)
+    R = np.maximum.reduce([np.abs(q[:, 0]), np.abs(q[:, 1]), np.abs(g[:, 0]), np.abs(g[:, 1]), np.abs(an[:, 0]), np.abs(an[:, 1])]) \
+        + 0.5 * np.maximum(np.hypot(q[:, 3], q[:, 4]), np.hypot(g[:, 3], g[:, 4]))
+    Ep = u * R * (24 + np.abs(q[:, 6]) + np.abs(g[:, 6]))
+    Pmin = np.minimum(2 * (q[:, 3] + q[:, 4]), 2 * (g[:, 3] + g[:, 4]))
+    D2 = np.minimum(q[:, 3] ** 2 + q[:, 4] ** 2, g[:, 3] ** 2 + g[:, 4] ** 2)
+    near = np.zeros(n, bool)                                      # a corner within the margin (+ rounding) of the other rectangle
+    for i in range(n):
+        dist = [_ip_outside(p, g[i]) for p in _ip_corners(q[i])] + [_ip_outside(p, q[i]) for p in _ip_corners(g[i])]
+        near[i] = min(abs(x) for x in dist) <= IP_MARGIN + 2 * Ep[i]
+    EA = (2 * Ep + np.where(near, IP_MARGIN, 0.0)) * Pmin + 72 * u * D2
+    Ezb = lambda b: u * (2 * np.abs(b[:, 2]) + np.abs(an[:, 2]) + 3 * b[:, 5])           # noqa: E731
+    Eih = 2 * np.maximum(Ezb(q), Ezb(g)) + u * info["ih"]
+    ov, ih, iou = info["ov"], info["ih"], info["iou"]
+    Eov3 = EA * ih + ov * Eih + EA * Eih + u * ov * ih
+    vq, vg = q[:, 3] * q[:, 4] * q[:, 5], g[:, 3] * g[:, 4] * g[:, 5]
+    Un = vq + vg - ov * ih
+    EUn = 19 * u * (vq + vg) + Eov3
+    EI = (Eov3 + iou * EUn) / np.maximum(Un - EUn, 1e-7) + u * iou
+    Et = 2 * EI + u
+    sigma, d, rw = info["sigma"], info["d"], info["rw"]
+    s2, k = sigma ** 2, 1.0 / sigma ** 2
+    Ed = Et + u * np.abs(d)
+    fb = rw * (np.minimum(s2 * np.abs(d), 1) * Ed + s2 * Ed ** 2 + u * k) + 4 * u * np.abs(info["f"])
+    gb = rw * info["w_iou"] / info["B"] * s2 * (Ed + u * k) + 4 * u * np.abs(info["fp"])
+    B, A = info["B"], info["A"]
+    depth = -(-A // IP_CTA_SPAN) + 5 + 8 + 74
+    sb = np.zeros(B)
+    np.add.at(sb, info["b"], fb + depth * u * np.abs(info["f"]))
+    grad_b = np.zeros(info["shape"])
+    grad_b[info["b"], info["a"] // 2, 20 + info["r"]] = gb
+    return sb, grad_b
+
+
+IP_MUTANTS = ("angle_neg", "wl_swap", "z_bottom", "no_batch_div", "wrong_slot", "iou_target")
+
+
+def iou_pred_emul(head, anchors, labels, targets, sigma=3.0, w_iou=1.0, mutant=None):
+    """fp32 twin of iou_pred_loss_kernel: the C oracle's decode and rotated BEV overlap (oracle/csrc/oracle.c, the reference's iou3d_cpu
+    arithmetic), the rest in numpy fp32 in the kernel's operation order.  `mutant` plants one of IP_MUTANTS, or "no_npos_clamp".
+    Returns (sums [B] float32, grad [B, P, S] float32 with the iou channels of the positives, zero elsewhere)."""
+    from oracle import cpu as ocpu
+    f = np.float32
+    B, P, S = head.shape
+    bi, ai, ri = _ip_positives(head, labels)
+    an = anchors[ai]
+    e = np.stack([head[bi, ai // 2, 7 * ri + k] for k in range(7)], 1)
+    q, g = ocpu.box_decode(e, an), ocpu.box_decode(targets[bi, ai], an)
+    two = f(2)
+
+    def rect(b):
+        x = b.copy()
+        if mutant == "wl_swap":
+            x[:, [3, 4]] = x[:, [4, 3]]
+        if mutant == "angle_neg":
+            x[:, 6] = -x[:, 6]
+        return ocpu.boxes3d_to_bev(x)
+    rq, rg = rect(q), rect(g)
+    ov = np.array([ocpu.boxes_overlap_bev(rq[i:i + 1], rg[i:i + 1])[0, 0] for i in range(len(q))], f)
+    if mutant == "z_bottom":
+        lo, hi = np.maximum(q[:, 2], g[:, 2]), np.minimum(q[:, 2] + q[:, 5], g[:, 2] + g[:, 5])
+    else:
+        lo = np.maximum(q[:, 2] - q[:, 5] / two, g[:, 2] - g[:, 5] / two)
+        hi = np.minimum(q[:, 2] + q[:, 5] / two, g[:, 2] + g[:, 5] / two)
+    ov3 = ov * np.maximum(hi - lo, f(0))
+    iou = ov3 / np.maximum(q[:, 3] * q[:, 4] * q[:, 5] + g[:, 3] * g[:, 4] * g[:, 5] - ov3, f(1e-7))
+    target = iou if mutant == "iou_target" else two * iou - f(1)
+    slot = 1 - ri if mutant == "wrong_slot" else ri
+    d = head[bi, ai // 2, 20 + slot] - target
+    cnt = (labels > 0).sum(1).astype(f)
+    with np.errstate(divide="ignore"):
+        rw_frame = f(1) / (cnt if mutant == "no_npos_clamp" else np.maximum(cnt, f(1)))
+    rw = rw_frame[bi]
+    sig = f(sigma)
+    inv_s2 = f(1) / (sig * sig)
+    ad = np.abs(d)
+    small = ad <= inv_s2
+    sd = ad * sig
+    term = np.where(small, f(0.5) * sd * sd, ad - f(0.5) * inv_s2) * rw
+    inv_b = f(1) if mutant == "no_batch_div" else f(B)
+    gv = np.where(small, sig * sig * d, np.sign(d).astype(f)) * rw * f(w_iou) / inv_b
+    sums = np.zeros(B, f)
+    for b in range(B):
+        sums[b] = term[bi == b].sum(dtype=f)
+    grad = np.zeros((B, P, S), f)
+    grad[bi, ai // 2, 20 + ri] = gv
+    return sums, grad
+
+
+def iou_pred_violations(sums, grad, ref_sums, ref_grad, sb, gb, scale=1.0):
+    """(worst |got - ref| / (scale * bound) over the sums, over the iou channels of the positives); non-finite counts as infinite"""
+    def ratio(got, ref, bound):
+        got = got.astype(np.float64)
+        err = np.abs(got - ref)
+        r = np.where(err == 0, 0.0, err / np.maximum(scale * bound, 1e-300))
+        r[~np.isfinite(got)] = np.inf
+        return float(r.max()) if r.size else 0.0
+    return ratio(sums, ref_sums, sb), ratio(grad, ref_grad, gb)
+
+
+# crafted (prediction, target) pairs in decoded form, centres relative to the anchor's: (name, q [7], g [7])
+def iou_pred_pairs():
+    pi = np.pi
+    car = [0.15, -0.2, 0.05, 1.7, 4.1, 1.5, 0.3]
+    out = []
+    add = lambda name, q, g: out.append((name, np.float64(q), np.float64(g)))       # noqa: E731
+    add("identical", car, car)
+    add("yaw_plus_pi", car[:6] + [car[6] + pi], car)
+    add("yaw_plus_half_pi_wl_swapped", car[:3] + [car[4], car[3], car[5], car[6] + pi / 2], car)
+    add("disjoint_bev", [6.5] + car[1:], car)                                          # target exactly -1
+    add("no_height_overlap", car[:2] + [car[2] + 1.6] + car[3:], car)                  # target exactly -1
+    ax = [0.0, 0.0, 0.0, 1.6, 3.9, 1.56, 0.0]
+    add("touching_faces", [1.6] + ax[1:], ax)                                          # x faces touch: zero area
+    add("contained", [0.1, 0.3, 0.0, 0.8, 2.0, 1.0, 0.4], ax)
+    s = 1.2                                                                            # a square rotated by pi/4: its corner on ax's x face
+    add("corner_on_edge", [0.8 + s / np.sqrt(2), 0.5, 0.0, s, s, 1.5, pi / 4], ax)
+    add("corner_poking_in", [0.8 + s / np.sqrt(2) - 0.1, 0.5, 0.0, s, s, 1.5, pi / 4], ax)
+    add("pedestrian", [0.1, 0.05, 0.1, 0.6, 0.8, 1.73, 0.2], [0.0, 0.0, 0.0, 0.55, 0.9, 1.7, -0.1])
+    add("enc_dims_plus5", car, car)                                                    # dims of q re-encoded below
+    add("enc_dims_minus5", car, car)
+    add("enc_dims_minus104", car, car)                                                 # expf underflows: zero-size box, target -1
+    rng = np.random.default_rng(17)
+    for i in range(6):                                                                 # generic: rotated, offset in x and y, heights differ
+        gq = [rng.uniform(-0.5, 0.5), rng.uniform(-0.5, 0.5), rng.uniform(-0.3, 0.3), rng.uniform(1.4, 1.9), rng.uniform(3.4, 4.4),
+              rng.uniform(1.3, 1.8), rng.uniform(-pi, pi)]
+        gg = [rng.uniform(-0.5, 0.5), rng.uniform(-0.5, 0.5), rng.uniform(-0.3, 0.3), rng.uniform(1.4, 1.9), rng.uniform(3.4, 4.4),
+              rng.uniform(1.3, 1.8), gq[6] + rng.uniform(-0.6, 0.6)]
+        add("generic%d" % i, gq, gg)
+    return out
+
+
+IP_EXACT_MINUS_ONE = ("disjoint_bev", "no_height_overlap")          # pairs whose target is exactly -1 in fp32 and in fp64
+
+
+def _ip_encode(box, anc):
+    """second_box_encode in fp64 of a decoded box against one anchor, rounded to fp32"""
+    diag = np.sqrt(np.float64(anc[4]) ** 2 + np.float64(anc[3]) ** 2)
+    a = anc.astype(np.float64)
+    return np.float32([(box[0] - a[0]) / diag, (box[1] - a[1]) / diag, (box[2] - a[2]) / a[5], np.log(box[3] / a[3]), np.log(box[4] / a[4]),
+                       np.log(box[5] / a[5]), box[6] - a[6]])
+
+
+def _ip_head_values(sigma):
+    """iou head values around the exact target -1: target -+ knee, one ulp either side of each, and d = 0"""
+    k = np.float32(1.0) / (np.float32(sigma) * np.float32(sigma))
+    m1 = np.float32(-1)
+    vals = [m1, m1 + k, m1 - k]
+    for v in (m1 + k, m1 - k):
+        vals += [np.nextafter(v, np.float32(2)), np.nextafter(v, np.float32(-2))]
+    return np.float32(vals)
+
+
+def make_iou_pred_case(B, A, stride, seed, sigma, frames):
+    """head [B, A/2, stride], anchors [A, 7], labels [B, A], targets [B, A, 7].  frames: per frame "all", "empty", "edges" (only the
+    positives at anchor 0, A - 1 and past the grid-stride wrap) or "shifted" (every placement, the pairs rotated by 5)."""
+    rng = np.random.default_rng(seed)
+    P = A // 2
+    anc = _anchors(A)
+    head = (rng.standard_normal((B, P, stride)) * 0.5).astype(np.float32)
+    labels = rng.choice(np.int32([-1, 0]), (B, A), p=[0.2, 0.8]).astype(np.int32)
+    targets = (rng.standard_normal((B, A, 7)) * 0.3).astype(np.float32)
+    pairs = iou_pred_pairs()
+    hv = _ip_head_values(sigma)
+    jobs = [(i, None) for i in range(len(pairs))]
+    jobs += [(i, v) for i, (n, _, _) in enumerate(pairs) if n in IP_EXACT_MINUS_ONE for v in hv]
+    edges = [0, 1, A - 2, A - 1, IP_CTA_SPAN - 1, IP_CTA_SPAN, IP_CTA_SPAN + 1, 350, 351]          # 350 / 351: x = 70.2, y = -39.8
+    edges += [x for x in (2 * IP_CTA_SPAN + 3, 3 * IP_CTA_SPAN + 8) if x < A]
+    mid = [(100 * 176 + 40) * 2 + i for i in range(max(0, len(jobs) - len(edges)) + 4)]
+    slots = edges + mid
+    for b, kind in enumerate(frames):
+        if kind == "empty":
+            labels[b] = np.minimum(labels[b], 0)
+            continue
+        use = edges if kind == "edges" else slots
+        rot = 5 if kind == "shifted" else 0
+        for n, a in enumerate(use):
+            i, v = jobs[(n + rot) % len(jobs)]
+            name, qd, gd = pairs[i]
+            labels[b, a] = 1
+            qa, ga = qd.copy(), gd.copy()
+            qa[:3] += anc[a, :3]
+            ga[:3] += anc[a, :3]
+            eq, eg = _ip_encode(qa, anc[a]), _ip_encode(ga, anc[a])
+            if name == "enc_dims_plus5":
+                eq[3:6] = 5
+            elif name == "enc_dims_minus5":
+                eq[3:6] = -5
+            elif name == "enc_dims_minus104":
+                eq[3] = -104
+            r = a % 2
+            head[b, a // 2, 7 * r:7 * r + 7] = eq
+            targets[b, a] = eg
+            head[b, a // 2, 20 + r] = v if v is not None else np.float32(rng.uniform(-1, 1))
+    return head, anc, labels, targets
+
+
+def iou_pred_cases():
+    """(name, head, anchors, labels, targets, sigma, w_iou) of the crafted IoU-prediction cases"""
+    A1, A2 = 37890, 70400
+    return [
+        ("a37890_s22_ragged5", *make_iou_pred_case(5, A1, 22, 31, 3.0, ["all", "empty", "edges", "shifted", "all"]), 3.0, 1.0),
+        ("a70400_s24_sig1", *make_iou_pred_case(2, A2, 24, 32, 1.0, ["shifted", "all"]), 1.0, 0.5),
+        ("a70400_s32_empty", *make_iou_pred_case(3, A2, 32, 33, 3.0, ["edges", "empty", "all"]), 3.0, 0.5),
+    ]
