@@ -14,7 +14,7 @@ from spconv import SparseConv3d, SubMConv3d
 from torch import nn
 
 from sessd_b200 import sparse_grad
-from sessd_b200.runners import SPMIDDLE_LAYERS, SpMiddleRunner
+from sessd_b200.runners import SPMIDDLE_LAYERS, RunnerCache, SpMiddleRunner
 
 from ..registry import BACKBONES
 from ..utils import build_norm_layer
@@ -37,9 +37,7 @@ class SpMiddleFHD(nn.Module):
             mods.append(nn.ReLU())
             cin = cout
         self.middle_conv = spconv.SparseSequential(*mods)
-        self._runner = None
-        self._runner_key = None
-        self._weights_key = None
+        self._runner = RunnerCache()
 
     def init_weights(self, pretrained=None):
         if isinstance(pretrained, str):       # reference convention (e.g. rpn.py / resnet): a checkpoint path
@@ -70,18 +68,13 @@ class SpMiddleFHD(nn.Module):
         coors = coors.int().contiguous()
         n = int(coors.shape[0])
         cap = max(4096, -(-n // 4096) * 4096)
-        key = (int(batch_size), cap, tuple(grid_xyz), str(coors.device))
-        if self._runner is None or self._runner_key != key:
-            self._runner = SpMiddleRunner(int(batch_size), cap, grid_xyz, self.middle_conv[0].in_channels, coors.device)
-            self._runner_key, self._weights_key = key, None
-        wkey = tuple((p.data_ptr(), p._version) for p in self.parameters()) + tuple((b.data_ptr(), b._version) for b in self.buffers())
-        if wkey != self._weights_key:
-            self._runner.load_weights(self._layers())
-            self._weights_key = wkey
+        runner = self._runner.get(self, (int(batch_size), cap, tuple(grid_xyz), str(coors.device)),
+                                  lambda: SpMiddleRunner(int(batch_size), cap, grid_xyz, self.middle_conv[0].in_channels, coors.device),
+                                  lambda r: r.load_weights(self._layers()))
         feats = voxel_features.detach().float().contiguous()
         n_dev = torch.tensor([n], dtype=torch.int32, device=coors.device)
-        dense = self._runner.forward(feats, coors, n_dev)                 # NHWC [B, 200, 176, 128]
-        if int(self._runner.status.item()) != 0:
+        dense = runner.forward(feats, coors, n_dev)                       # NHWC [B, 200, 176, 128]
+        if int(runner.status.item()) != 0:
             raise RuntimeError("SpMiddleFHD: active-site capacity exceeded")
         # logical NCHW, channels-last memory; a fresh tensor per call (the runner's dense buffer is overwritten by the next forward)
         return dense.permute(0, 3, 1, 2).clone()

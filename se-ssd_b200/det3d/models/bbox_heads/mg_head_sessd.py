@@ -18,7 +18,7 @@ from torch import nn
 
 from det3d.core.bbox.geometry import frustum_planes
 from sessd_b200 import bev_grad, ops
-from sessd_b200.runners import HeadRunner
+from sessd_b200.runners import HeadRunner, RunnerCache
 
 from ..builder import build_loss
 from ..registry import HEADS
@@ -49,9 +49,7 @@ class Head(nn.Module):
         self.trans_conv = None
         if self.use_dir:
             self.conv_dir = nn.Conv2d(num_input, num_dir, 1)
-        self._runner = None
-        self._runner_key = None
-        self._weights_key = None
+        self._runner = RunnerCache()
 
     def packed_forward(self, x):
         """x logical NCHW [B,128,H,W] -> packed NHWC [B,H,W,24] = [box 14 | cls 2 | dir 4 | iou 2 | pad 2]."""
@@ -60,15 +58,9 @@ class Head(nn.Module):
         if self.training:       # differentiable w.r.t. x and the four convs' weights and biases (sessd_b200.bev_grad); a fresh tensor
             return bev_grad.head_forward(self, x)
         b, c, h, w = x.shape
-        key = (b, h, w, str(x.device))
-        if self._runner is None or self._runner_key != key:
-            self._runner = HeadRunner(b, (h, w), x.device)
-            self._runner_key, self._weights_key = key, None
-        wkey = tuple((p.data_ptr(), p._version) for p in self.parameters())
-        if wkey != self._weights_key:
-            self._runner.load_state({k: v.detach() for k, v in self.state_dict().items()}, prefix="")
-            self._weights_key = wkey
-        return self._runner.forward(x.detach().float().permute(0, 2, 3, 1).contiguous())
+        runner = self._runner.get(self, (b, h, w, str(x.device)), lambda: HeadRunner(b, (h, w), x.device),
+                                  lambda r: r.load_state({k: v.detach() for k, v in self.state_dict().items()}, prefix=""))
+        return runner.forward(x.detach().float().permute(0, 2, 3, 1).contiguous())
 
     def forward(self, x):
         # a fresh tensor per call (like the reference): the runner's output buffer is overwritten by the next forward, and the SE-SSD

@@ -9,7 +9,7 @@ the convs on the same kernels through an autograd Function, BatchNorm2d with bat
 from torch import nn
 
 from sessd_b200 import bev_grad
-from sessd_b200.runners import SSFAPlanesRunner
+from sessd_b200.runners import RunnerCache, SSFAPlanesRunner
 
 from ..registry import NECKS
 from ..utils import build_norm_layer
@@ -52,9 +52,7 @@ class SSFA(nn.Module):
         self.conv_1 = S(*_cbr(128, 128, 3, norm_cfg))
         self.w_1 = S(*_cbr(128, 1, 1, norm_cfg, relu=False))
         logger.info("Finish RPN Initialization")
-        self._runner = None
-        self._runner_key = None
-        self._weights_key = None
+        self._runner = RunnerCache()
 
     def init_weights(self):
         for m in self.modules():
@@ -65,16 +63,13 @@ class SSFA(nn.Module):
         if self.training:       # the reference forward layer by layer, differentiable (sessd_b200.bev_grad); BatchNorm2d with batch statistics
             return bev_grad.ssfa_forward(self, x)
         b, c, h, w = x.shape
-        key = (b, h, w, str(x.device))
-        if self._runner is None or self._runner_key != key:
-            self._runner = SSFAPlanesRunner(b, (h, w), x.device)
-            self._runner_key, self._weights_key = key, None
-        wkey = tuple((p.data_ptr(), p._version) for p in self.parameters()) + tuple((t.data_ptr(), t._version) for t in self.buffers())
-        if wkey != self._weights_key:
+
+        def load(runner):
             eps = {float(m.eps) for m in self.modules() if isinstance(m, nn.modules.batchnorm._BatchNorm)}
             assert len(eps) == 1, "SSFA: all BatchNorm layers must share one eps"
-            self._runner.load_state({k: v.detach() for k, v in self.state_dict().items()}, bn_eps=eps.pop())
-            self._weights_key = wkey
+            runner.load_state({k: v.detach() for k, v in self.state_dict().items()}, bn_eps=eps.pop())
+
+        runner = self._runner.get(self, (b, h, w, str(x.device)), lambda: SSFAPlanesRunner(b, (h, w), x.device), load)
         x_nhwc = x.detach().float().permute(0, 2, 3, 1).contiguous()     # no copy when x is channels-last already
-        out, _ = self._runner.forward(x_nhwc)
+        out, _ = runner.forward(x_nhwc)
         return out.permute(0, 3, 1, 2).clone()        # fresh tensor per call: the runner buffer is overwritten by the next forward

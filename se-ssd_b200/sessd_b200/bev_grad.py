@@ -22,7 +22,7 @@ import torch.nn.functional as F
 from sessd_data.layers import SSFA_LAUNCHES, ssfa_extents
 
 from . import ops
-from .runners import _cout_pad, _pack_conv
+from .runners import _cout_pad, _pack_conv, conv_taps, head_weight, launch_desc, launch_weight
 from .train import conv2d_s1_dgrad_weight
 
 HEAD = SSFA_LAUNCHES[-1]
@@ -39,12 +39,9 @@ def split(x):
     return planes, info
 
 
-def conv_taps(k):
-    """taps (dy, dx) of a k x k conv padded by k // 2, relative to the output pixel (times the input stride), in _pack_conv order"""
-    return [(dy - k // 2, dx - k // 2) for dy in range(k) for dx in range(k)]
-
-
 def conv_desc(batch, in_hw, cin, out_hw, cout, k, stride):
+    """ConvDesc of a data- or weight-gradient launch, whose input and output swap roles against the forward launch's: the taps of
+    runners.conv_taps, no ReLU"""
     return ops.conv_desc(batch, in_hw, cin, out_hw, cout, out_hw, conv_taps(k), in_stride=stride, relu=False)
 
 
@@ -85,13 +82,10 @@ class BevConvFunction(torch.autograd.Function):
     def forward(ctx, x, weight, bias, L, in_hw, out_hw):
         b = int(x.shape[0])
         planes, info = split(x.detach().float())
-        w = weight.detach().float()
+        wp, taps = launch_weight(L, weight.detach().float())
         out = torch.empty((b,) + tuple(out_hw) + (L.cout,), dtype=torch.float32, device=x.device)
         shift = None if bias is None else bias.detach().float().contiguous()
-        if L.kind == "conv":
-            _run("conv", planes, info, _pack_conv(w)[0], shift, out, conv_desc(b, in_hw, L.cin, out_hw, L.cout, L.k, L.stride))
-        else:
-            _run("deconv", planes, info, w.permute(2, 3, 0, 1).reshape(9, L.cin, L.cout), shift, out)
+        _run(L.kind, planes, info, wp, shift, out, launch_desc(L, b, in_hw, out_hw, taps, relu=False) if L.kind == "conv" else None)
         # through save_for_backward: an in-place change of the weight or of the input planes between forward and backward raises
         ctx.save_for_backward(weight, planes, info)
         ctx.L, ctx.in_hw, ctx.out_hw, ctx.has_bias = L, tuple(in_hw), tuple(out_hw), bias is not None
@@ -164,12 +158,7 @@ def _attention_logit(seq, o):
 
 def head_forward(head, x):
     """the four 1x1 convs of a Head (mg_head_sessd.py:202-230) as one BevConvFunction on x [B, 128, H, W] -> packed NHWC [B, H, W, 24] =
-    [box 14 | cls 2 | dir 4 | iou 2 | pad 2] (runners.pack_head's layout), with a graph to x and every conv's weight and bias"""
-    convs = (head.conv_box, head.conv_cls, head.conv_dir, head.conv_iou)
-    w = torch.cat([c.weight for c in convs], 0)
-    bias = torch.cat([c.bias for c in convs], 0)
-    pad = HEAD.cout - w.shape[0]
-    w = torch.cat([w, w.new_zeros((pad,) + tuple(w.shape[1:]))], 0)
-    bias = torch.cat([bias, bias.new_zeros((pad,))], 0)
+    [box 14 | cls 2 | dir 4 | iou 2 | pad 2] (runners.head_weight's layout), with a graph to x and every conv's weight and bias"""
+    w, bias = head_weight(head.get_parameter)
     hw = tuple(x.shape[2:])
     return BevConvFunction.apply(x.permute(0, 2, 3, 1), w, bias, HEAD, hw, hw)

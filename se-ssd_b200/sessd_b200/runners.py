@@ -4,6 +4,7 @@ data-dependent count stays on the device -- so a whole frame can be captured in 
 
 Layer tables mirror det3d/models/backbones/scn.py:106-149 (SpMiddleFHD) and det3d/models/necks/rpn_v1.py:135-235 (SSFA).
 """
+import itertools
 import math
 
 import torch
@@ -204,6 +205,32 @@ class SpMiddleRunner:
 
 
 # ---------------------------------------------------------------------------------------------------------------
+class RunnerCache:
+    """The stage runner of an eval-mode module (SpMiddleFHD, SSFA, Head): built anew when its key (shapes, device) changes, and its
+    weights reloaded when the (data_ptr, _version) of any parameter or buffer of the module changes."""
+
+    def __init__(self):
+        self.runner = self.key = self.weights = None
+
+    def get(self, module, key, build, load):
+        """the runner for ``key``: build() makes a new one, load(runner) loads the module's weights into it"""
+        if self.runner is None or key != self.key:
+            self.runner, self.key, self.weights = build(), key, None
+        weights = tuple((t.data_ptr(), t._version) for t in itertools.chain(module.parameters(), module.buffers()))
+        if weights != self.weights:
+            load(self.runner)
+            self.weights = weights
+        return self.runner
+
+
+_SSFA = {L.name: L for L in SSFA_LAUNCHES}
+
+
+def conv_taps(k):
+    """taps (dy, dx) of a k x k conv padded by k // 2, relative to the output pixel (times the input stride), in _pack_conv order"""
+    return [(dy - k // 2, dx - k // 2) for dy in range(k) for dx in range(k)]
+
+
 def _pack_conv(w):
     """nn.Conv2d weight [Cout,Cin,kh,kw] -> ([kh*kw, Cin, Cout], taps (dy,dx) relative to the unpadded origin)."""
     cout, cin, kh, kw = w.shape
@@ -211,17 +238,33 @@ def _pack_conv(w):
     return packed, [(ky, kx) for ky in range(kh) for kx in range(kw)]
 
 
-def pack_head(head_sd, prefix, device, stride=24):
-    """Four 1x1 head convs (mg_head_sessd.py:202-215) -> one [1,128,stride] GEMM weight + bias, channel layout
-    [box 14 | cls 2 | dir 4 | iou 2 | zero pad]."""
-    hw = torch.zeros((1, 128, stride), dtype=torch.float32, device=device)
-    hb = torch.zeros((stride,), dtype=torch.float32, device=device)
-    o = 0
-    for nm, c in (("conv_box", 14), ("conv_cls", 2), ("conv_dir", 4), ("conv_iou", 2)):
-        hw[0, :, o:o + c] = head_sd[prefix + nm + ".weight"].to(device, torch.float32).reshape(c, 128).t()
-        hb[o:o + c] = head_sd[prefix + nm + ".bias"].to(device, torch.float32)
-        o += c
-    return hw.contiguous(), hb.contiguous()
+def launch_weight(L, w):
+    """(weight [taps, Cin, Cout], taps) of launch L from its weight in the module's layout: a conv's Conv2d weight [Cout, Cin, k, k] (the
+    head's from head_weight) in the packing of _pack_conv with the taps of conv_taps; a deconv's ConvTranspose2d weight
+    [Cin, Cout, 3, 3] in the plain 9-tap packing of W[cin][cout][ky][kx], taps None"""
+    if L.kind == "deconv":
+        return w.permute(2, 3, 0, 1).reshape(9, L.cin, L.cout).contiguous(), None
+    return _pack_conv(w)[0], conv_taps(L.k)
+
+
+def launch_desc(L, batch, in_hw, out_hw, taps, relu=None):
+    """ConvDesc of conv launch L on a batch of its ssfa_extents (in_hw, out_hw), with the taps of launch_weight's packing and the fused
+    ReLU of L unless relu says otherwise"""
+    return ops.conv_desc(batch, in_hw, L.cin, out_hw, L.cout, out_hw, taps, in_stride=L.stride, relu=L.relu if relu is None else relu)
+
+
+def head_weight(param):
+    """The four 1x1 head convs (mg_head_sessd.py:202-215) as the module-layout weight [24, 128, 1, 1] and bias [24] of the head launch,
+    channel layout [box 14 | cls 2 | dir 4 | iou 2 | zero pad].  param(name) returns a conv's tensor ("conv_box.weight"); the result is
+    built with torch ops, so it keeps the autograd graph of module parameters."""
+    w, b = (torch.cat([param(c + s) for c in ("conv_box", "conv_cls", "conv_dir", "conv_iou")], 0) for s in (".weight", ".bias"))
+    pad = _SSFA["head"].cout - w.shape[0]
+    return torch.cat([w, w.new_zeros((pad,) + tuple(w.shape[1:]))], 0), torch.cat([b, b.new_zeros((pad,))], 0)
+
+
+def pack_head(head_sd, prefix, device):
+    """head_weight from a state dict"""
+    return head_weight(lambda name: head_sd[prefix + name].to(device, torch.float32))
 
 
 def fold_ssfa_bn(sd, conv_name, device, eps=BN_EPS):
@@ -231,13 +274,13 @@ def fold_ssfa_bn(sd, conv_name, device, eps=BN_EPS):
     return fold_bn(*(sd[b + k].to(device, torch.float32) for k in ("weight", "bias", "running_mean", "running_var")), eps=eps)
 
 
-def pack_h2(wp, scale, shift, cout_pad):
-    """[taps, Cin, Cout] weight + folded BN (scale None: 1) -> the fp16-split launch parameters of bev_conv_p2 / _h2: weight planes,
-    epilogue scale (BN scale x the planes' 2^-e[n]), shift, and gain / shift_max of the output bound"""
-    planes, inv = ops.pack_weight_h2(wp, cout_pad)
+def pack_h2(wp, taps, scale, shift):
+    """launch_weight's (weight [taps, Cin, Cout], taps) + folded BN (scale None: 1) -> the fp16-split launch parameters of bev_conv_p2 /
+    _h2: weight planes, epilogue scale (BN scale x the planes' 2^-e[n]), shift, gain / shift_max of the output bound, and the taps"""
+    planes, inv = ops.pack_weight_h2(wp, _cout_pad(wp.shape[2]))
     scale = torch.ones(wp.shape[2], device=wp.device) if scale is None else scale
     return dict(w=planes, scale=(scale * inv[:scale.numel()]).contiguous(), shift=shift.contiguous(), gain=ops.conv_gain(wp, scale),
-                shift_max=float(shift.abs().max()))
+                shift_max=float(shift.abs().max()), taps=taps)
 
 
 def _cout_pad(cout):
@@ -247,22 +290,15 @@ def _cout_pad(cout):
 
 
 def ssfa_weights(ssfa_sd, head_sd, head_prefix, device, bn_eps=BN_EPS):
-    """yields (launch, weight [taps, Cin, Cout], taps, BN scale, BN shift) in SSFA_LAUNCHES order: convs in the tap-list packing (taps
-    (dy, dx) relative to the output pixel), deconvs in the plain 9-tap packing of W[cin][cout][ky][kx] (taps None), the head (only with
-    head_sd) with scale None and its bias as the shift"""
+    """yields (launch, weight [taps, Cin, Cout], taps, BN scale, BN shift) in SSFA_LAUNCHES order, weight and taps from launch_weight;
+    the head (only with head_sd) with scale None and its bias as the shift"""
     for L in SSFA_LAUNCHES:
-        if L.name == "head":
-            if head_sd is not None:
-                hw, hb = pack_head(head_sd, head_prefix, device, L.cout)
-                yield L, hw, [(0, 0)], None, hb
-            continue
-        wt = ssfa_sd[L.name + ".weight"].to(device, torch.float32)
-        if L.kind == "conv":
-            wp, taps = _pack_conv(wt)
-            taps = [(dy - L.k // 2, dx - L.k // 2) for dy, dx in taps]
-        else:
-            wp, taps = wt.permute(2, 3, 0, 1).reshape(9, L.cin, L.cout).contiguous(), None
-        yield (L, wp, taps) + fold_ssfa_bn(ssfa_sd, L.name, device, bn_eps)
+        if L.name != "head":
+            wp, taps = launch_weight(L, ssfa_sd[L.name + ".weight"].to(device, torch.float32))
+            yield (L, wp, taps) + fold_ssfa_bn(ssfa_sd, L.name, device, bn_eps)
+        elif head_sd is not None:
+            w, bias = pack_head(head_sd, head_prefix, device)
+            yield (L, *launch_weight(L, w), None, bias)
 
 
 def ssfa_fuse_weights(ssfa_sd, device, bn_eps=BN_EPS):
@@ -276,35 +312,6 @@ def ssfa_fuse_weights(ssfa_sd, device, bn_eps=BN_EPS):
 
 # {abs-max, scale} slot of every SSFA tensor: the neck input, the launch outputs kept as planes, the fused map, then the fp32 outputs
 SSFA_SLOT = {n: i for i, n in enumerate(["x"] + [L.dst for L in SSFA_LAUNCHES if not L.f32] + ["out"] + [L.dst for L in SSFA_LAUNCHES if L.f32])}
-_SSFA = {L.name: L for L in SSFA_LAUNCHES}
-
-
-class HeadRunner:
-    """The fused head GEMM alone (MultiGroupHead.forward) on the fp16-split tensor-core conv (csrc/bevconv_p2.cu; the fp32 input is
-    split into planes first)."""
-
-    def __init__(self, batch, hw, device="cuda", stride=24):
-        self.batch, self.h, self.w, self.stride = batch, int(hw[0]), int(hw[1]), stride
-        self.out = torch.zeros((batch, self.h, self.w, stride), dtype=torch.float32, device=device)
-        self.device = torch.device(device)
-        self.params = None
-        self.x_planes = ops.alloc_bev_planes(batch, self.h, self.w, 128, self.device)
-        self.info = torch.zeros((2, 2), dtype=torch.float32, device=self.device)     # {abs-max, scale} of the input / the output
-
-    def load_state(self, head_sd, prefix=""):
-        w, bias = pack_head(head_sd, prefix, self.device, self.stride)
-        self.params = pack_h2(w, None, bias, _cout_pad(self.stride))
-
-    def forward(self, x):
-        H = (self.h, self.w)
-        d = ops.conv_desc(self.batch, H, 128, H, self.stride, H, [(0, 0)], relu=False)
-        q = self.params
-        self.info.zero_()
-        ops.absmax(x, self.info[0, 0:1])
-        ops.bev_split_planes(x, self.info[0], self.x_planes)
-        ops.bev_conv_p2(self.x_planes, self.info[0], q["w"], q["scale"], q["shift"], None, None, q["gain"], q["shift_max"], self.out, None,
-                        self.info[1], d)
-        return self.out
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -341,9 +348,15 @@ class SSFAPlanesRunner:
     def load_state(self, ssfa_sd, head_sd=None, head_prefix="tasks.0.", bn_eps=BN_EPS):
         """bn_eps: eps of the neck's BatchNorm2d layers (rpn_v1.py:131-132 uses 1e-3; pass the module's own value otherwise)."""
         P = ssfa_fuse_weights(ssfa_sd, self.device, bn_eps)
-        for L, wp, taps, sc, sh in ssfa_weights(ssfa_sd, head_sd, head_prefix, self.device, bn_eps):
-            P[L.name] = dict(pack_h2(wp, sc, sh, _cout_pad(L.cout)), taps=taps)
+        for L, *weight in ssfa_weights(ssfa_sd, head_sd, head_prefix, self.device, bn_eps):
+            P[L.name] = pack_h2(*weight)
         self.params = P
+
+    def _split(self, x, name):
+        """zero the info slots, then split the fp32 NHWC x into the planes of tensor ``name`` and its info slot"""
+        self.info.zero_()
+        ops.absmax(x, self._info(name)[0:1])
+        ops.bev_split_planes(x, self._info(name), self.planes[name])
 
     def _launch(self, L, skip=False):
         """launch L from its input planes into its output planes or fp32 buffer.  skip: run the work items of this launch's skip-plan
@@ -354,8 +367,7 @@ class SSFAPlanesRunner:
         i = self.SKIP_LAUNCHES.index(L.name)
         rec = self.skip.record(i) if skip else None
         if L.kind == "conv":
-            in_hw, out_hw = ssfa_extents(L, self.h, self.w)
-            d = ops.conv_desc(self.batch, in_hw, L.cin, out_hw, L.cout, out_hw, q["taps"], in_stride=L.stride, relu=L.relu)
+            d = launch_desc(L, self.batch, *ssfa_extents(L, self.h, self.w), q["taps"])
             ops.bev_conv_p2(self.planes[L.src], self._info(L.src), q["w"], q["scale"], q["shift"], resid, resid_info, q["gain"],
                             q["shift_max"], out_f32, out_planes, self._info(L.dst), d, items=rec)
         else:
@@ -372,9 +384,7 @@ class SSFAPlanesRunner:
         assert self.params is not None, "load_state first"
         mark = mark or (lambda label: None)
         if x is not None:
-            self.info.zero_()
-            ops.absmax(x, self.info[0, 0:1])
-            ops.bev_split_planes(x, self.info[0], self.planes["x"])
+            self._split(x, "x")
         skip = self.skip_constant and occupancy is not None
         if skip:
             index, grid = occupancy
@@ -413,3 +423,23 @@ class SSFAPlanesRunner:
             self._launch(_SSFA[name]._replace(src="x0", dst="b0b"))
 
         return launch, "bev_conv_p2_kernel (fp16 wgmma from pre-split fp16 planes, two-term split)"
+
+
+class HeadRunner(SSFAPlanesRunner):
+    """The fused head GEMM alone (MultiGroupHead.forward): only the buffers of the head launch (its input planes, the info slots, its
+    output), launched by SSFAPlanesRunner.head after the fp32 input is split into planes."""
+
+    def __init__(self, batch, hw, device="cuda"):
+        self.batch, self.h, self.w, self.device = batch, int(hw[0]), int(hw[1]), torch.device(device)
+        self.planes = dict(out=ops.alloc_bev_planes(batch, self.h, self.w, 128, self.device))
+        self.buf = dict(head=torch.zeros((batch, self.h, self.w, self.HEAD_STRIDE), dtype=torch.float32, device=self.device))
+        self.info = torch.zeros((len(self.SLOT), 2), dtype=torch.float32, device=self.device)
+        self.params = None
+
+    def load_state(self, head_sd, prefix=""):
+        w, bias = pack_head(head_sd, prefix, self.device)
+        self.params = {"head": pack_h2(*launch_weight(_SSFA["head"], w), None, bias)}
+
+    def forward(self, x):
+        self._split(x, "out")
+        return self.head()
