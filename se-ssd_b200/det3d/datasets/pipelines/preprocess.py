@@ -2,8 +2,8 @@
 :235-358).  Transforms are ``(res, info) -> (res, info)``.  Dataset I/O and the reference's ``Preprocess`` are not registered here: the
 per-object noise, global flip / rotation / scaling, shuffle and teacher twin run on the device through ``sessd_b200.augment`` (its own entry
 point), GT-database sampling (GT-AUG) runs there too when ``build_train_batch`` is given a ``db_sampler`` (det3d.core.sampler), and
-shape-aware augmentation (SA-DA) when it is given ``sa_da`` (sessd_b200.sada).  No ``Preprocess`` is registered: frame loading is not
-mirrored, and a DataLoader worker cannot hold the CUDA context those stages need."""
+shape-aware augmentation (SA-DA) when it is given ``sa_da`` (sessd_b200.sada).  No ``Preprocess`` is registered: KittiDataset runs only the
+host loaders, and the device loader (det3d.datasets.loader.build_dataloader) runs these stages per batch, on the device."""
 import numpy as np
 
 from det3d.builder import build_anchor_generator, build_box_coder, build_similarity_metric

@@ -1,4 +1,4 @@
-"""Dataset-side registries (``DATASETS`` is only named by configs here: dataset I/O is outside the hot path; ``PIPELINES`` holds the per-frame transforms)."""
+"""Dataset-side registries: ``DATASETS`` (build_dataset) and ``PIPELINES`` (the per-frame transforms)."""
 from det3d.utils import Registry
 
 DATASETS, PIPELINES = (Registry(kind) for kind in ("dataset", "pipeline"))

@@ -1,6 +1,14 @@
-"""Teacher / student bookkeeping of the SE-SSD trainer (reference: det3d/torchie/trainer/trainer_sessd.py:250-275, 302-318).  Only the
-pieces that sit on the per-step path are mirrored: the consistency-weight ramp and the teacher's exponential moving average (one kernel
-launch over the flat parameter arenas, sessd_b200.train)."""
+"""The SE-SSD trainer (reference: det3d/torchie/trainer/trainer_sessd.py): the epoch loop with the teacher / student step, validation,
+checkpoints and resume, the consistency-weight ramp and the teacher's exponential moving average (one kernel launch over the flat
+parameter arenas, sessd_b200.train).  Over an ArenaAdamW and a teacher ParamArena the gradient clip, the AdamW update and the teacher
+EMA run as one fused device pass per step."""
+import logging
+import os
+import os.path as osp
+import sys
+import time
+from collections import OrderedDict
+
 import numpy as np
 
 from sessd_b200 import train as _train
@@ -114,3 +122,237 @@ def merge_label_unlabel_data(data_batch, data_batch_unlabel):
     flag[:n_lab] = 1
     merged["ssl_labeled"] = flag
     return merged
+
+
+# ---------------------------------------------------------------------------------------------------------------- the loop
+class Trainer:
+    """The reference's Trainer with its SE-SSD semantics, single-GPU.  ``batch_processor`` has batch_processor_inline's signature.
+    ``register_training_hooks`` takes the config's optimizer / checkpoint / log entries in place of the reference's hook objects."""
+
+    def __init__(self, model, model_ema, batch_processor, optimizer=None, lr_scheduler=None, work_dir=None, log_level=logging.INFO,
+                 logger=None):
+        assert callable(batch_processor)
+        self.model, self.model_ema, self.batch_processor = model, model_ema, batch_processor
+        self.optimizer, self.lr_scheduler = optimizer, lr_scheduler
+        self.work_dir = None if work_dir is None else osp.abspath(work_dir)
+        if self.work_dir is not None:
+            os.makedirs(self.work_dir, exist_ok=True)
+        self.timestamp = time.strftime("%Y%m%d_%H%M%S", time.localtime())
+        self.logger = logger if logger is not None else self.init_logger(self.work_dir, log_level)
+        self.optimizer_config, self.checkpoint_config, self.log_config = {}, {}, None
+        self.mode, self.data_loader, self.outputs = None, None, None
+        self._epoch = self._iter = self._inner_iter = self._max_epochs = self._max_iters = 0
+
+    epoch = property(lambda self: self._epoch)
+    iter = property(lambda self: self._iter)
+    inner_iter = property(lambda self: self._inner_iter)
+    max_epochs = property(lambda self: self._max_epochs)
+    max_iters = property(lambda self: self._max_iters)
+
+    def init_logger(self, log_dir=None, level=logging.INFO):
+        """a logger writing to stderr and, with a work dir, to ``<work_dir>/<timestamp>.log``"""
+        logger = logging.getLogger("det3d.trainer.%x" % id(self))
+        logger.setLevel(level)
+        logger.propagate = False
+        fmt = logging.Formatter("%(asctime)s - %(levelname)s - %(message)s")
+        handlers = [logging.StreamHandler(sys.stderr)]
+        if log_dir:
+            handlers.append(logging.FileHandler(osp.join(log_dir, "%s.log" % self.timestamp), "w"))
+        for h in handlers:
+            h.setFormatter(fmt)
+            h.setLevel(level)
+            logger.addHandler(h)
+        return logger
+
+    def register_training_hooks(self, lr_config, optimizer_config=None, checkpoint_config=None, log_config=None):
+        if lr_config is not None:
+            raise NotImplementedError("lr_config hooks: the one-cycle schedule is passed to the Trainer as lr_scheduler")
+        self.optimizer_config = dict(optimizer_config or {})
+        self.checkpoint_config = dict(checkpoint_config or {})
+        self.log_config = log_config
+
+    def current_lr(self):
+        return [self.optimizer.lr]
+
+    # ------------------------------------------------------------------------------------------------ train / val
+    def _fused(self):
+        """the teacher's ParamArena when clip, AdamW and EMA can run as one ArenaAdamW pass, else None"""
+        from .hooks.optimizer import _owns_gradients
+        ema = getattr(self.model_ema, "_arena", None)
+        clip = self.optimizer_config.get("grad_clip")
+        if not isinstance(ema, _train.ParamArena) or (clip is not None and clip.get("norm_type", 2) != 2):
+            return None
+        return ema if _owns_gradients(self.optimizer, self.model.parameters()) else None
+
+    def _step(self, global_step):
+        ema = self._fused()
+        if ema is not None:
+            clip = self.optimizer_config.get("grad_clip")
+            self.optimizer.zero_grad()
+            self.outputs["loss"].backward()
+            self.optimizer.step(max_grad_norm=None if clip is None else clip["max_norm"], ema=ema, global_step=global_step)
+            return
+        from .hooks.optimizer import OptimizerHook
+        OptimizerHook(self.optimizer_config.get("grad_clip")).after_train_iter(self)
+        update_ema_variables(self.model, self.model_ema, global_step)
+
+    def train(self, data_loader, data_loader_unlabel=None, epoch=None, **kwargs):
+        """One epoch (trainer_sessd.py:320-360).  ``data_loader_unlabel`` is accepted and not drawn from: the reference's merge of
+        unlabelled batches is commented out."""
+        self.model_ema.train()
+        self.model.train()
+        self.mode, self.data_loader = "train", data_loader
+        self.length = len(data_loader)
+        self._max_iters = self._max_epochs * self.length
+        base_step = self.epoch * self.length
+        if hasattr(data_loader, "set_epoch"):
+            data_loader.set_epoch(self.epoch)
+        consistency_weight = 1.0 * sigmoid_rampup(self.epoch, self._max_epochs)
+        log = _LogBuffer()
+        interval = self.log_config["interval"] if self.log_config else 0
+        t_end = time.time()
+        for i, data_batch in enumerate(data_loader):
+            t_data = time.time()
+            global_step = base_step + i
+            if self.lr_scheduler is not None:
+                self.lr_scheduler.step(global_step)
+            self._inner_iter = i
+            outputs = self.batch_processor(self.model, self.model_ema, data_batch, consistency_weight, train_mode=True)
+            if not isinstance(outputs, dict):
+                raise TypeError("batch_processor() must return a dict")
+            self.outputs = outputs
+            self._step(global_step)
+            self._iter += 1
+            now = time.time()
+            log.update(outputs["log_vars"], outputs["num_samples"], time=now - t_end, data_time=t_data - t_end)
+            t_end = now
+            if interval and (i + 1) % interval == 0:
+                self._log_train(log)
+        if self.work_dir and (self.epoch + 1) % self.checkpoint_config.get("interval", 1) == 0:
+            self.save_checkpoint(self.work_dir, save_optimizer=self.checkpoint_config.get("save_optimizer", True),
+                                 meta=dict(self.checkpoint_config.get("meta") or {}))
+        self._epoch += 1
+
+    def _log_train(self, log):
+        avg = log.average()
+        head = "Epoch [%d/%d][%d/%d]\tlr: %.5f, time: %.3f, data_time: %.3f, " % (
+            self.epoch + 1, self._max_epochs, self._inner_iter + 1, self.length, self.current_lr()[0], avg.pop("time"),
+            avg.pop("data_time"))
+        self.logger.info(head + ", ".join("%s: %s" % (k, _fmt(v)) for k, v in avg.items()))
+        log.clear()
+
+    def val(self, data_loader, **kwargs):
+        """Evaluate the student (trainer_sessd.py:362-415): predictions keyed by token, ``dataset.evaluation``, the official AP strings
+        logged.  Returns the results dict."""
+        self.mode, self.data_loader = "val", data_loader
+        self.logger.info("work dir: %s", self.work_dir)
+        result_dict, _ = data_loader.dataset.evaluation(compute_on_dataset(self.model, data_loader), output_dir=self.work_dir)
+        self.logger.info("\n")
+        for k, v in list(result_dict["results"].items()) + list(result_dict["results_2"].items()):
+            self.logger.info("Evaluation %s: %s", k, v)
+        return result_dict
+
+    def run(self, data_loaders, workflow, max_epochs, **kwargs):
+        """Train from the current epoch to ``max_epochs`` on ``data_loaders[0]``, then validate once on ``data_loaders[-1]``, the order
+        of the reference's run() (trainer_sessd.py:430-470) for workflow [("train", N), ("val", 1)].  Returns the validation results,
+        or None when the workflow has no val phase."""
+        assert isinstance(data_loaders, list)
+        self._max_epochs = max_epochs
+        self.logger.info("Start running, work_dir: %s", self.work_dir)
+        self.logger.info("workflow: %s, max: %d epochs", workflow, max_epochs)
+        results = None
+        while self.epoch < max_epochs:
+            for mode, epochs in workflow:
+                if mode not in ("train", "val"):
+                    raise ValueError("Trainer has no method named '{}' to run an epoch".format(mode))
+                for _ in range(epochs):
+                    if mode == "train" and self.epoch > max_epochs:
+                        return results
+                    if mode == "train" and self.epoch == max_epochs:
+                        return self.val(data_loaders[-1]) if len(workflow) > 1 else results
+                    if mode == "val":
+                        results = self.val(data_loaders[-1])
+                    else:
+                        self.train(data_loaders[0], None, self.epoch)
+        return results
+
+    # ------------------------------------------------------------------------------------------------ checkpoints
+    def save_checkpoint(self, out_dir, filename_tmpl="epoch_{}.pth", save_optimizer=True, meta=None):
+        """``epoch_{n}.pth`` (student) and ``epoch_{n}_ema.pth`` (teacher), both with the optimiser state and meta = {epoch, iter} plus
+        ``meta``; relative symlinks latest.pth / latest_ema.pth (trainer_sessd.py:228-248)"""
+        from .checkpoint import save_checkpoint
+        meta = dict(meta or {})
+        meta.update(epoch=self.epoch + 1, iter=self.iter)
+        filename = filename_tmpl.format(self.epoch + 1)
+        optimizer = self.optimizer if save_optimizer else None
+        filename_ema = osp.splitext(filename)[0] + "_ema.pth"
+        for model, name, link in ((self.model, filename, "latest.pth"), (self.model_ema, filename_ema, "latest_ema.pth")):
+            save_checkpoint(model, osp.join(out_dir, name), optimizer=optimizer, meta=meta)
+            _symlink(name, osp.join(out_dir, link))
+
+    def load_checkpoint(self, filename, map_location="cpu", strict=False):
+        """the student from ``filename``, the teacher from its ``_ema`` twin, the optimiser state"""
+        from .checkpoint import load_checkpoint
+        self.logger.info("load checkpoint from %s", filename)
+        ckpt = load_checkpoint(self.model, filename, map_location, strict, self.logger)
+        load_checkpoint(self.model_ema, osp.splitext(filename)[0] + "_ema.pth", map_location, strict, self.logger)
+        self.optimizer.load_state_dict(ckpt["optimizer"])
+        return ckpt
+
+    def load_checkpoint_from_scratch(self, filename, map_location="cpu", strict=False):
+        """student and teacher from the same checkpoint, and its optimiser state (the ``load_from`` of SE-SSD's SSL stage)"""
+        from .checkpoint import load_checkpoint
+        self.logger.info("load checkpoint from %s", filename)
+        ckpt = load_checkpoint(self.model, filename, map_location, strict, self.logger)
+        load_checkpoint(self.model_ema, filename, map_location, strict, self.logger)
+        self.optimizer.load_state_dict(ckpt["optimizer"])
+        return ckpt
+
+    def resume(self, checkpoint, resume_optimizer=True, map_location="default"):
+        if map_location == "default":
+            import torch
+            map_location = "cuda:%d" % torch.cuda.current_device() if torch.cuda.is_available() else "cpu"
+        ckpt = self.load_checkpoint(checkpoint, map_location=map_location)
+        self._epoch, self._iter = ckpt["meta"]["epoch"], ckpt["meta"]["iter"]
+        self.logger.info("resumed epoch %d, iter %d", self.epoch, self.iter)
+
+
+def compute_on_dataset(model, data_loader):
+    """the model's detections on every batch of ``data_loader`` in eval mode, keyed by token, tensors on the host (tools/test.py)"""
+    import torch
+    model.eval()
+    detections = {}
+    with torch.no_grad():
+        for example in data_loader:
+            for output in model(example, return_loss=False):
+                detections[output["metadata"]["token"]] = {k: (v if k == "metadata" else v.cpu()) for k, v in output.items()}
+    return detections
+
+
+def _symlink(src, dst):
+    if osp.lexists(dst):
+        os.remove(dst)
+    os.symlink(src, dst)
+
+
+def _fmt(v):
+    return "%.4f" % v if np.ndim(v) == 0 else str(np.round(np.asarray(v, np.float64), 4).tolist())
+
+
+class _LogBuffer:
+    """averages of the logged values over the iterations since the last log line, weighted by the batch's sample count"""
+
+    def __init__(self):
+        self.clear()
+
+    def clear(self):
+        self.values, self.counts = OrderedDict(), []
+
+    def update(self, log_vars, count, **times):
+        for k, v in list(times.items()) + list(log_vars.items()):
+            self.values.setdefault(k, []).append(np.asarray(v, np.float64))
+        self.counts.append(count)
+
+    def average(self):
+        w = np.asarray(self.counts, np.float64)
+        return OrderedDict((k, np.average(np.stack(v), axis=0, weights=w)) for k, v in self.values.items())

@@ -261,6 +261,14 @@ def _static(cfg, device):
     return _STATIC[key]
 
 
+def voxel_example(st, vb, batch, total, sfx=""):
+    """the model-input keys of one voxelised branch (``sfx`` "" or "_raw"): the exact-count voxels / num_points / coordinates (the first
+    ``total`` rows of the VoxelBuffers ``vb``, read back by the caller), num_voxels, shape and the per-task anchors"""
+    return {"voxels" + sfx: vb.voxels[:total], "num_points" + sfx: vb.num_points[:total], "coordinates" + sfx: vb.coors[:total],
+            "num_voxels" + sfx: vb.num_voxels[:batch].long(), "shape" + sfx: np.stack([st["grid"]] * batch),
+            "anchors" + sfx: [st["anchors"].unsqueeze(0).expand(batch, -1, -1).contiguous()]}
+
+
 class PendingBatch:
     """A training batch whose device work has been launched (augmentation, both voxelisations, both target assignments) and whose
     collated dict is not formed yet.  ``example()`` forms it: the one device-to-host read of the batch (the two branches' voxel totals,
@@ -276,16 +284,9 @@ class PendingBatch:
         dev = self._off.device
         counts = self._off[1:] - self._off[:-1]
         bidx = torch.repeat_interleave(torch.arange(B, dtype=torch.float32, device=dev), counts, output_size=self._total)
-        anchors = [self._st["anchors"].unsqueeze(0).expand(B, -1, -1).contiguous()]
-        shape = np.stack([self._st["grid"]] * B)
         ex = dict(metadata=[dict(token=i) for i in range(B)], points=torch.cat([bidx[:, None], self._aug["points"]], 1))
         for sfx, vb, ab, n in (("", self._vox, self._asg, totals[0]), ("_raw", self._vox_raw, self._asg_raw, totals[1])):
-            ex["voxels" + sfx] = vb.voxels[:n]
-            ex["num_points" + sfx] = vb.num_points[:n]
-            ex["coordinates" + sfx] = vb.coors[:n]
-            ex["num_voxels" + sfx] = vb.num_voxels[:B].long()
-            ex["shape" + sfx] = shape
-            ex["anchors" + sfx] = anchors
+            ex.update(voxel_example(self._st, vb, B, n, sfx))
             ex["labels" + sfx] = [ab.labels]
             ex["reg_targets" + sfx] = [ab.bbox_targets]
         ex["transformation"] = self._aug["transformation"]
