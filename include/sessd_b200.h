@@ -608,7 +608,8 @@ int sessd_adamw_clip_ema_step(float *d_param, float *d_grad, float *d_exp_avg, f
  *     [n, 2] = (class code, difficulty 0-2) with d_min_overlap [n].  Outputs per config: d_thresholds / d_precision / d_aos [n, 41]
  *     (zero past d_num_thresholds[c]), d_map [n, 4] = R11 precision, R40 precision, R11 AOS, R40 AOS (get_mAP / get_mAP_v2, in
  *     percent).  A config with no valid ground truth has no thresholds and AP 0.  max_frame_dt: the largest dt_off[f+1] - dt_off[f]
- *     (SESSD_ECAPACITY above 1024).  total_gt = gt_off[F]; overlap_elems = ov_off[F].  Bitwise deterministic run to run.  The
+ *     (SESSD_ECAPACITY above 1024).  This is the frame's capacity, not dt_cnt[f]: a frame of 1025 input detections is refused
+ *     even when the conversion kept 1024 or fewer.  total_gt = gt_off[F]; overlap_elems = ov_off[F].  Bitwise deterministic run to run.  The
  *     workspace holds the overlaps, 2 x num_configs x total_gt fp64 scores and, with compute_aos, one fp64 similarity per (config,
  *     threshold, frame) for the frame-ordered sum: num_configs x 41 x F doubles (133 MB for 108 configs over 3769 frames).
  * ------------------------------------------------------------------------------------------------ */
