@@ -162,6 +162,9 @@ int sessd_spconv_forward_cg(const void *d_in_planes, int cp, int plane_rows, con
                             int relu, float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, void *stream);
 /* 1: deep pipeline (twice the stages) for launches with fewer tiles than SMs (single frames); 0 (default): the shorter ring */
 void sessd_set_sp_cg_deep(int on);
+/* CTAs of sessd_spconv_forward_cg's (cp, cout, deep) kernel resident on one SM of the current device; its persistent grid is at most that
+ * many per SM.  SESSD_EINVAL for an unsupported (cp, cout), -cudaError on a CUDA error. */
+int sessd_spconv_cg_blocks_per_sm(int cp, int cout, int deep);
 /* *d_amax = max(*d_amax, max |d_feat[i]|) over the first *d_n rows of a [max_rows, channels] fp32 tensor */
 int sessd_absmax_rows(const float *d_feat, const int *d_n, int max_rows, int channels, float *d_amax, void *stream);
 

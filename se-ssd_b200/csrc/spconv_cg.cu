@@ -6,28 +6,29 @@
 // a_hi b_lo + a_lo b_hi into the cross accumulator, both fp32), summed in RN fp32 by the epilogue.
 //   * the rulebook is regrouped ONCE per build (sessd_rulebook_tile_lists; a SubM rulebook serves 2-3 layers) into per-tile, per-offset
 //     lists of (input row, tile row) pairs + row masks; a tile's record (~3-8 KB) is copied to shared memory;
-//   * eight producer warps copy the listed rows with 16-byte cp.async (global/L2 -> shared, no registers) straight into the K-major
+//   * four producer warps copy the listed rows with 16-byte cp.async (global/L2 -> shared, no registers) straight into the K-major
 //     SWIZZLE_128B layout the wgmma descriptors address; rows without a neighbour are never touched;
-//   * a stage's missing rows must read as zeros: each producer warp remembers (registers) which of its rows of its stage hold data and
+//   * a stage's missing rows must read as zeros: each producer warp remembers (registers) which of its rows of its stages hold data and
 //     clears (st.shared) only the rows that were valid for the stage's previous offset and are not for the new one -- the stages are
 //     zeroed once per CTA;
 //   * the 32-channel layers stage the weights as [b_lo rows ; b_hi rows] of 64 bytes (SWIZZLE_64B), the 64-channel layers as
-//     [b_lo ; b_hi] tiles of 128-byte rows (SWIZZLE_128B): per k16, one m64n(2 COUT) over the whole stage computes a_hi b_lo (cross)
-//     and a_hi b_hi (main) with a single shared-memory read of the a_hi tile, and an m64nCOUT adds a_lo b_hi onto the cross half -- two
-//     wgmmas instead of three, the same products in the same order per accumulator (bit-identical to three separate m64nCOUT);
+//     [b_lo ; b_hi] tiles of 128-byte rows (SWIZZLE_128B); per k16, three m64nCOUT compute a_hi b_lo and a_lo b_hi into the cross
+//     accumulator and a_hi b_hi into the main one;
 //   * two consumer warpgroups (64 tile rows each) issue the wgmmas of every offset, wait for them and release the stage at once, so its
 //     next fill starts while the following offset's fill is still in flight (a single frame's layers are bound by this chain of fills,
 //     see DEEP; measurements in DESIGN section 4), and run the epilogue from the accumulator registers: a 4 x 4 transpose inside each
 //     quad of lanes gives every lane 8 whole channels of one row, stored 16 bytes at a time (each warp store covers whole 32-byte
 //     sectors), with the folded BN scale / shift read from shared memory (copied there once per CTA);
-//   * CTAs are persistent (one per SM), so barrier / zero-fill setup is paid once, not per 128 rows;
+//   * CTAs are persistent, so barrier / zero-fill setup is paid once, not per 128 rows; two fit on an SM (384 threads, <= 113 KB of
+//     shared memory), so one tile's chain of fills runs while the other CTA's wgmmas or epilogue do;
 //   * the epilogue writes the NEXT layer's operand format directly -- fp16 (hi, lo) planes scaled by a power of two derived from a
 //     rigorous bound |out| <= amax_in * G + max|shift| (G from the weights, host; amax_in measured by the producing layer's epilogue) --
 //     and raises the output's abs-max: no separate split kernel.
-// Each stage has its own producer group (8 / kStages warps): the group copies, waits for ITS copies (cp.async.wait_all), makes them and
-// the clears visible to the async proxy (fence.proxy.async by the writing threads) and arrives on the stage's mbarrier, while the other
-// groups' fills are in flight.
-// Warps: 0-7 producers, 8-15 consumers (warpgroups 2 and 3), 16 weight-tile TMA.
+// Stages are owned by producer groups (2 stages: two groups of 2 warps; 4 stages: one warp each; 8 stages: two per warp): after the
+// stage's empty wait the group loads its weight tile with TMA from one lane, copies the A rows, waits for ITS copies (cp.async.wait_all),
+// makes them and the clears visible to the async proxy (fence.proxy.async by the writing threads) and arrives on the stage's mbarrier,
+// while the other groups' fills are in flight.
+// Warps: 0-3 producers (warpgroup 0, 48 registers), 4-11 consumers (warpgroups 1 and 2, 96 registers).
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -37,10 +38,12 @@ namespace sessd {
 
 constexpr int kCgBM = 128;
 constexpr int kCgMaxK = 27;
-constexpr int kCgProdWarps = 8;
+constexpr int kCgProdWarps = 4;
 constexpr int kCgMmaWarps = 8;
-constexpr int kCgWeightWarp = kCgProdWarps + kCgMmaWarps;
-constexpr int kCgThreads = (kCgWeightWarp + 1) * 32;
+constexpr int kCgThreads = (kCgProdWarps + kCgMmaWarps) * 32;
+// 80 registers per thread at launch fit two CTAs on an SM; setmaxnreg then moves them from the producers to the consumers'
+// accumulators: 128 x 48 + 256 x 96 = 384 x 80
+constexpr int kCgRegsProducer = 48, kCgRegsConsumer = 96;
 
 // DEEP = 1: twice the stages -- for launches whose tiles do not fill the machine (a single frame: ~100 tiles on 132 SMs), where the
 // layer's time is the serial chain of a tile's fills (latency-bound): more fills in flight shorten it
@@ -50,7 +53,11 @@ struct CgCfg {
     static constexpr int kATile = (kWide ? 2 : 1) * kCgBM * 128;              // bytes: [hi tile ; lo tile] (wide) or one [hi | lo] tile
     static constexpr int kBTile = (kWide ? 2 : 1) * COUT * 128;               // wide: [b_lo ; b_hi] of 128-byte rows; narrow: 64-byte rows
     static constexpr int kStage = kATile + (kBTile + 1023) / 1024 * 1024;
-    static constexpr int kStages = (kWide ? 2 : 4) * (DEEP ? 2 : 1);           // must divide the 8 producer warps (one group per stage)
+    static constexpr int kStages = (kWide ? 2 : 4) * (DEEP ? 2 : 1);
+    // producer groups: group g owns stages g, g + kGroups, ... and fills them in ring order
+    static constexpr int kGroups = kStages < kCgProdWarps ? kStages : kCgProdWarps;
+    static constexpr int kGroupWarps = kCgProdWarps / kGroups;                // 2 or 1
+    static constexpr int kGroupStages = kStages / kGroups;                    // 1 or 2
     static constexpr int kMeta = kCgBM * kCgMaxK * 4 /*lists*/ + kCgMaxK * 16 /*valid*/ + 2 * COUT * 4 /*scale, shift*/ + 32 * 4 /*cnt*/ +
                                  33 * 4 /*klist, nact*/ + 32 * 4 /*off*/ + 3 * kStages * 8 /*barriers*/ + 24;
     static constexpr int kSmem = kStages * kStage + kMeta + 1024;
@@ -80,22 +87,24 @@ __device__ __forceinline__ void cg_sts_zero16(uint32_t saddr) {
     asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};\n" ::"r"(saddr), "r"(0) : "memory");
 }
 
-// N output columns: COUT (one plane of the weight stage) or 2 COUT (the whole [b_lo ; b_hi] stage)
+// N = COUT output columns: one plane of the weight stage
 template <int N>
 __device__ __forceinline__ void cg_wgmma(float *d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    static_assert(N == 32 || N == 64, "COUT is 32 or 64");
     if constexpr (N == 32) wgmma_f16_n32(d, da, db, accumulate);
-    else if constexpr (N == 64) wgmma_f16_n64(d, da, db, accumulate);
-    else wgmma_f16_n128(d, da, db, accumulate);
+    else wgmma_f16_n64(d, da, db, accumulate);
 }
 
 template <int CP, int COUT, int DEEP>
-__global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_constant__ CUtensorMap map_w, const CgArgs a) {
+__global__ void __launch_bounds__(kCgThreads, 2) spconv_cg_kernel(const __grid_constant__ CUtensorMap map_w, const CgArgs a) {
     using C = CgCfg<CP, COUT, DEEP>;
+    static_assert(DEEP || C::kSmem <= 113 * 1024, "two CTAs per SM: 228 KB of shared memory less 1 KB reserved per CTA");
+    static_assert(kCgProdWarps * 32 * kCgRegsProducer + kCgMmaWarps * 32 * kCgRegsConsumer <= kCgThreads * 80, "setmaxnreg budget");
     const int n_out = min(*a.d_n_out, a.max_out);
     const int ntiles = (n_out + kCgBM - 1) / kCgBM;
     if ((int)blockIdx.x >= ntiles) return;                       // whole CTA leaves together (before any barrier use)
     const int kvol = a.kvol;
-    if (threadIdx.x == kCgWeightWarp * 32) prefetch_tensormap(&map_w);      // the weight-TMA warp's first load finds the descriptor cached
+    if (threadIdx.x == 0) prefetch_tensormap(&map_w);            // the producers' first weight load finds the descriptor cached
 
     extern __shared__ unsigned char smem_raw[];
     unsigned char *tiles = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -114,7 +123,11 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
     const uint32_t tiles_u32 = smem_u32(tiles);
 
     if (tid == 0) {
-        for (int s = 0; s < C::kStages; ++s) { mbar_init(&full_a[s], kCgProdWarps / C::kStages); mbar_init(&full_b[s], 1); mbar_init(&empty[s], kCgMmaWarps); }
+        for (int s = 0; s < C::kStages; ++s) {
+            mbar_init(&full_a[s], C::kGroupWarps);
+            mbar_init(&full_b[s], 1);
+            mbar_init(&empty[s], kCgMmaWarps);
+        }
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
     }
     if (tid < COUT) {
@@ -127,90 +140,176 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
     cg_fence_proxy_async();
     __syncthreads();
 
-    const float amax_in = __ldg(a.in_info), s_in = __ldg(a.in_info + 1);
-    const float inv_act = 1.f / s_in;                            // exact: power of two
-    const float s_out = pow2_scale_for_bound(amax_in * a.gain + a.shift_max);
-    if (blockIdx.x == 0 && tid == 0 && a.out_info) a.out_info[1] = s_out;
-    float vmax = 0.f;
-    uint32_t dirty[4] = {0u, 0u, 0u, 0u};                        // rows of this warp's share of its stage that hold data (producer warps)
-    int st0 = 0;                                                 // stage of this tile's first fill (all roles advance it alike)
-    uint32_t ph0 = 0;                                            // phase bit of stage st0
-
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const int row0 = tile * kCgBM;
-        const int rows = min(kCgBM, n_out - row0);
-        // ---------------------------------------------------------------- the tile's per-offset pair lists (built once per rulebook by
-        // sessd_rulebook_tile_lists: counts, row masks, (input row << 7 | tile row) entries grouped by offset) -> shared memory
-        {
-            const unsigned int *rec = a.tiles + (size_t)tile * (size_t)a.tile_stride;
-            const int c = (int)__ldg(rec + lane);                        // every warp ranks the 32 counts itself: no extra block-wide sync
-            // the first list entries are requested together with the counts (one L2 round trip instead of two for most tiles; the record
-            // is tile_list_stride(kvol) words long, so the speculative reads stay inside it)
-            unsigned int spec[4];
+    // The tile's per-offset pair lists (built once per rulebook by sessd_rulebook_tile_lists: counts, row masks, (input row << 7 | tile
+    // row) entries grouped by offset) -> shared memory.  Every thread of both roles runs it at the head of a tile, then a __syncthreads.
+    auto load_lists = [&](int tile) {
+        const unsigned int *rec = a.tiles + (size_t)tile * (size_t)a.tile_stride;
+        const int c = (int)__ldg(rec + lane);                    // every warp ranks the 32 counts itself: no extra block-wide sync
+        // the first list entries are requested together with the counts (one L2 round trip instead of two for most tiles; the record
+        // is tile_list_stride(kvol) words long, so the speculative reads stay inside it)
+        unsigned int spec[4];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) spec[u] = (tid + u * kCgThreads < kTlRows * kvol) ? __ldg(rec + kTlHeader + tid + u * kCgThreads) : 0u;
-            const int incl = warp_incl_scan(c, lane);
-            const int total = __shfl_sync(0xffffffffu, incl, 31);
-            if (warp == 0) {
-                s_cnt[lane] = c;
-                s_off[lane] = incl - c;
-                const unsigned int m = __ballot_sync(0xffffffffu, c > 0);
-                if (c > 0) s_klist[__popc(m & ((1u << lane) - 1u))] = lane;
-                if (lane == 0) *s_nact = __popc(m);
-            }
-            if (tid < kvol * 4) s_valid[tid] = __ldg(rec + kTlMask + tid);
-#pragma unroll
-            for (int u = 0; u < 4; ++u)
-                if (tid + u * kCgThreads < total) s_list[tid + u * kCgThreads] = spec[u];
-            for (int e = tid + 4 * kCgThreads; e < total; e += kCgThreads) s_list[e] = __ldg(rec + kTlHeader + e);
+        for (int u = 0; u < 4; ++u) spec[u] = (tid + u * kCgThreads < kTlRows * kvol) ? __ldg(rec + kTlHeader + tid + u * kCgThreads) : 0u;
+        const int incl = warp_incl_scan(c, lane);
+        const int total = __shfl_sync(0xffffffffu, incl, 31);
+        if (warp == 0) {
+            s_cnt[lane] = c;
+            s_off[lane] = incl - c;
+            const unsigned int m = __ballot_sync(0xffffffffu, c > 0);
+            if (c > 0) s_klist[__popc(m & ((1u << lane) - 1u))] = lane;
+            if (lane == 0) *s_nact = __popc(m);
         }
-        __syncthreads();
-        const int nact = *s_nact;
+        if (tid < kvol * 4) s_valid[tid] = __ldg(rec + kTlMask + tid);
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+            if (tid + u * kCgThreads < total) s_list[tid + u * kCgThreads] = spec[u];
+        for (int e = tid + 4 * kCgThreads; e < total; e += kCgThreads) s_list[e] = __ldg(rec + kTlHeader + e);
+    };
+    // Ring position of a tile's first fill: stage st0, phase bit ph0.  Both roles advance it alike by each tile's nact fills.
+    int st0 = 0;
+    uint32_t ph0 = 0;
+    auto advance_ring = [&](int nact) {
+        const int adv = st0 + nact;
+        ph0 ^= (uint32_t)(adv / C::kStages) & 1u;
+        st0 = adv % C::kStages;
+    };
 
-        if (warp == kCgWeightWarp) {
-            // ===================== weight tiles (TMA, one elected lane): [b_lo ; b_hi] =====================
-            int s = st0;
-            uint32_t ph = ph0;
-            for (int j = 0; j < nact; ++j) {
+    if (warp < kCgProdWarps) {
+        setmaxnreg_dec<kCgRegsProducer>();
+        // ===================== producers: weight tile (TMA), copy the rows that exist, clear the rows that stopped existing ============
+        // Group grp fills the ring positions p = grp (mod kGroups), i.e. its stages grp, grp + kGroups, ... in turn; it waits for its
+        // own copies (cp.async.wait_all), fences them into the async proxy and arrives, while the other groups' fills are in flight.
+        constexpr int kGroups = C::kGroups, kGroupWarps = C::kGroupWarps, kGroupStages = C::kGroupStages;
+        constexpr int kGroupThreads = kGroupWarps * 32;
+        constexpr int kOwnRows = kCgBM / kGroupWarps;                // rows of a stage whose zero state this warp maintains: 128 or 64
+        constexpr int kOwnWords = kOwnRows / 32;
+        constexpr int kLanesPerRow = C::kWide ? 16 : 8;
+        constexpr int kRowsPerPass = kGroupThreads / kLanesPerRow;
+        const int grp = warp / kGroupWarps, gw = warp % kGroupWarps;
+        const int gtid = tid - grp * kGroupThreads;
+        const int slot = gtid / kLanesPerRow;
+        const int c = gtid % kLanesPerRow;
+        const int half = c >> 3, cc = c & 7;                         // wide: chunk c of the 256-byte row = (hi | lo tile, 16-byte chunk)
+        // rows of this warp's share of each of its stages that hold data; dirty[0] is the stage of the group's next fill
+        uint32_t dirty[kGroupStages][kOwnWords];
+#pragma unroll
+        for (int g = 0; g < kGroupStages; ++g)
+#pragma unroll
+            for (int w = 0; w < kOwnWords; ++w) dirty[g][w] = 0u;
+        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+            load_lists(tile);
+            __syncthreads();
+            const int nact = *s_nact;
+            for (int j = (grp - st0 % kGroups + kGroups) % kGroups; j < nact; j += kGroups) {
+                const int pos = st0 + j;                             // the phase bit of fill j follows the ring position
+                const int s = pos % C::kStages;
+                const uint32_t ph = ph0 ^ ((uint32_t)(pos / C::kStages) & 1u);
                 const int k = s_klist[j];
-                mbar_wait(&empty[s], ph ^ 1u);
-                if (elect_one()) {
-                    mbar_expect_tx(&full_b[s], C::kBTile);
-                    unsigned char *b_tile = tiles + s * C::kStage + C::kATile;
-                    tma_load_4d(b_tile + C::kBTile / 2, &map_w, &full_b[s], 0, 0, 0, k);      // plane 0 = b_hi
-                    tma_load_4d(b_tile, &map_w, &full_b[s], 0, 0, 1, k);                      // plane 1 = b_lo
+                const uint32_t a_base = tiles_u32 + (uint32_t)(s * C::kStage);
+                if (lane == 0) {
+                    mbar_wait<true>(&empty[s], ph ^ 1u);
+                    if (gw == 0) {                                   // weight tile [b_lo ; b_hi]
+                        mbar_expect_tx(&full_b[s], C::kBTile);
+                        unsigned char *b_tile = tiles + s * C::kStage + C::kATile;
+                        tma_load_4d(b_tile + C::kBTile / 2, &map_w, &full_b[s], 0, 0, 0, k);      // plane 0 = b_hi
+                        tma_load_4d(b_tile, &map_w, &full_b[s], 0, 0, 1, k);                      // plane 1 = b_lo
+                    }
                 }
                 __syncwarp();
-                if (++s == C::kStages) { s = 0; ph ^= 1u; }
-            }
-        } else if (warp >= kCgProdWarps) {
-            // ===================== consumers: wgmma per offset, then the epilogue from the accumulator registers =====================
-            const int cw = warp - kCgProdWarps, wg = cw >> 2, wq = cw & 3;
-            constexpr int kAcc = COUT / 2;
-            // acc[0, kAcc): cross a_hi x b_lo + a_lo x b_hi, acc[kAcc, COUT): main a_hi x b_hi -- the fragment of an m64n(2 COUT) over the
-            // whole [b_lo ; b_hi] weight stage.  The cross half comes first: ptxas serializes every wgmma of the kernel when one of them
-            // accumulates into a part of another's fragment that does not start at its first register.
-            float acc[COUT];
 #pragma unroll
-            for (int i = 0; i < COUT; ++i) acc[i] = 0.f;
-            const uint32_t a_rows = (uint32_t)(wg * 64 * 128);   // this warpgroup's 64 rows of the 128-byte-row A tile
+                for (int w = 0; w < kOwnWords; ++w) {
+                    const uint32_t vs = s_valid[k * 4 + gw * kOwnWords + w];
+                    const uint32_t z = dirty[0][w] & ~vs;    // rows that hold data of the stage's previous offset and get none now
+                    dirty[0][w] = vs;
+                    if (z) {
+#pragma unroll
+                        for (int q4 = 0; q4 < 8; ++q4) {
+                            const int r32 = q4 * 4 + (lane >> 3);
+                            if ((z >> r32) & 1u) {
+                                const uint32_t dst = a_base + (uint32_t)((gw * kOwnRows + w * 32 + r32) * 128 + (lane & 7) * 16);
+                                cg_sts_zero16(dst);
+                                if constexpr (C::kWide) cg_sts_zero16(dst + kCgBM * 128);
+                            }
+                        }
+                    }
+                }
+                const int n = s_cnt[k];
+                const uint32_t *lst = s_list + s_off[k];
+                auto copy_row = [&](uint32_t e) {
+                    const uint32_t r = tl_tile_row(e);
+                    const size_t src = (size_t)tl_in_row(e);
+                    if constexpr (C::kWide)
+                        cg_cp_async16(a_base + (uint32_t)half * (kCgBM * 128) + r * 128u + (((uint32_t)cc ^ (r & 7u)) << 4),
+                                      a.planes + src * 128 + half * 64 + cc * 8);
+                    else
+                        cg_cp_async16(a_base + r * 128u + (((uint32_t)cc ^ (r & 7u)) << 4), a.planes + src * 64 + cc * 8);
+                };
+                // four list entries per round: the shared-memory reads of a round are in flight together
+                int i = slot;
+                for (; i + 3 * kRowsPerPass < n; i += 4 * kRowsPerPass) {
+                    const uint32_t e0 = lst[i], e1 = lst[i + kRowsPerPass], e2 = lst[i + 2 * kRowsPerPass], e3 = lst[i + 3 * kRowsPerPass];
+                    copy_row(e0); copy_row(e1); copy_row(e2); copy_row(e3);
+                }
+                for (; i < n; i += kRowsPerPass) copy_row(lst[i]);
+                asm volatile("cp.async.wait_all;\n" ::: "memory");
+                cg_fence_proxy_async();                              // copies and clears (generic proxy) -> visible to the tensor core
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&full_a[s]);
+                if constexpr (kGroupStages > 1) {                    // the group's next fill lands in its next stage
+#pragma unroll
+                    for (int w = 0; w < kOwnWords; ++w) {
+                        const uint32_t d = dirty[0][w];
+#pragma unroll
+                        for (int g = 0; g + 1 < kGroupStages; ++g) dirty[g][w] = dirty[g + 1][w];
+                        dirty[kGroupStages - 1][w] = d;
+                    }
+                }
+            }
+            advance_ring(nact);
+            __syncthreads();                                         // lists are rebuilt next; every role is done reading them
+        }
+    } else {
+        setmaxnreg_inc<kCgRegsConsumer>();
+        // ===================== consumers: wgmma per offset, then the epilogue from the accumulator registers =====================
+        const int cw = warp - kCgProdWarps, wg = cw >> 2, wq = cw & 3;
+        constexpr int kAcc = COUT / 2;
+        const float amax_in = __ldg(a.in_info), s_in = __ldg(a.in_info + 1);
+        const float inv_act = 1.f / s_in;                        // exact: power of two
+        const float s_out = pow2_scale_for_bound(amax_in * a.gain + a.shift_max);
+        if (blockIdx.x == 0 && cw == 0 && lane == 0 && a.out_info) a.out_info[1] = s_out;
+        float vmax = 0.f;
+        const uint32_t a_rows = (uint32_t)(wg * 64 * 128);       // this warpgroup's 64 rows of the 128-byte-row A tile
+        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+            load_lists(tile);
+            __syncthreads();
+            const int nact = *s_nact;
+            const int row0 = tile * kCgBM;
+            const int rows = min(kCgBM, n_out - row0);
+            // m64nCOUT fragments: cross a_hi x b_lo + a_lo x b_hi, main a_hi x b_hi
+            float acc[kAcc], acc_main[kAcc];
+#pragma unroll
+            for (int i = 0; i < kAcc; ++i) acc[i] = acc_main[i] = 0.f;
             int s = st0;
             uint32_t ph = ph0;
             for (int j = 0; j < nact; ++j) {
-                mbar_wait(&full_b[s], ph);
-                mbar_wait(&full_a[s], ph);
+                mbar_wait<true>(&full_b[s], ph);
+                mbar_wait<true>(&full_a[s], ph);
                 const uint32_t st = tiles_u32 + (uint32_t)(s * C::kStage);
                 const uint64_t dA = kDescSw128Hi | desc_lo(st + a_rows);
                 const uint32_t first = j != 0 ? 1u : 0u;
-                // per k16: one m64n(2 COUT) over the stacked stage (cross (+)= a_hi x b_lo, main (+)= a_hi x b_hi: a_hi is read once),
-                // then cross += a_lo x b_hi.  Each accumulator sums the same products in the same order as three separate m64nCOUT would.
+                // per k16: cross (+)= a_hi x b_lo and main (+)= a_hi x b_hi, then cross += a_lo x b_hi.  Each accumulator sums the same
+                // products in the same order as one m64n(2 COUT) over the stacked stage followed by an m64nCOUT would; that wider form
+                // needs more registers than a consumer has with two CTAs on an SM (ptxas then ignores setmaxnreg or fails at 80).
                 wgmma_fence();
                 if constexpr (C::kWide) {
                     const uint64_t dAl = dA + ((kCgBM * 128) >> 4);
                     const uint64_t dBl = kDescSw128Hi | desc_lo(st + C::kATile);
                     const uint64_t dBh = dBl + ((COUT * 128) >> 4);
 #pragma unroll
-                    for (int kk = 0; kk < 4; ++kk) cg_wgmma<2 * COUT>(acc, dA + 2 * kk, dBl + 2 * kk, first | (kk != 0));
+                    for (int kk = 0; kk < 4; ++kk) {
+                        cg_wgmma<COUT>(acc, dA + 2 * kk, dBl + 2 * kk, first | (kk != 0));
+                        cg_wgmma<COUT>(acc_main, dA + 2 * kk, dBh + 2 * kk, first | (kk != 0));
+                    }
 #pragma unroll
                     for (int kk = 0; kk < 4; ++kk) cg_wgmma<COUT>(acc, dAl + 2 * kk, dBh + 2 * kk, 1u);
                 } else {
@@ -218,7 +317,10 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
                     const uint64_t dBl = kDescSw64Hi | desc_lo(st + C::kATile);
                     const uint64_t dBh = dBl + ((COUT * 64) >> 4);
 #pragma unroll
-                    for (int kk = 0; kk < 2; ++kk) cg_wgmma<2 * COUT>(acc, dA + 2 * kk, dBl + 2 * kk, first | (kk != 0));
+                    for (int kk = 0; kk < 2; ++kk) {
+                        cg_wgmma<COUT>(acc, dA + 2 * kk, dBl + 2 * kk, first | (kk != 0));
+                        cg_wgmma<COUT>(acc_main, dA + 2 * kk, dBh + 2 * kk, first | (kk != 0));
+                    }
 #pragma unroll
                     for (int kk = 0; kk < 2; ++kk) cg_wgmma<COUT>(acc, dA + 4 + 2 * kk, dBh + 2 * kk, 1u);
                 }
@@ -231,11 +333,12 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
                 if (lane == 0) mbar_arrive(&empty[s]);
                 if (++s == C::kStages) { s = 0; ph ^= 1u; }
             }
-            wgmma_fence_regs<COUT>(acc);
+            wgmma_fence_regs<kAcc>(acc);
+            wgmma_fence_regs<kAcc>(acc_main);
             // BN / ReLU -> planes and / or fp32 rows.  This thread holds rows r0 and r0 + 8, two adjacent channels of every 8-channel
             // group; a transpose inside each quad of lanes (one row) gives every lane 8 whole channels, stored 16 bytes at a time
 #pragma unroll
-            for (int i = 0; i < kAcc; ++i) acc[i] = acc[kAcc + i] + acc[i];      // main + cross
+            for (int i = 0; i < kAcc; ++i) acc[i] = acc_main[i] + acc[i];        // main + cross
             const int q = lane & 3;
             const int r0 = wg * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
@@ -297,93 +400,40 @@ __global__ void __launch_bounds__(kCgThreads, 1) spconv_cg_kernel(const __grid_c
                         }
                     }
                 }
-        } else {
-            // ===================== producers: copy the rows that exist, clear the rows that stopped existing =====================
-            // One producer GROUP per stage (kStages groups of 8 / kStages warps): a group fills only "its" stage, waits for its own copies
-            // (cp.async.wait_all), fences them into the async proxy and arrives; the other groups' fills are in flight meanwhile.
-            constexpr int kGroupWarps = kCgProdWarps / C::kStages;       // 1, 2 or 4
-            constexpr int kGroupThreads = kGroupWarps * 32;
-            constexpr int kOwnRows = kCgBM / kGroupWarps;                // rows of the stage whose zero state this warp maintains: 128, 64 or 32
-            constexpr int kOwnWords = kOwnRows / 32;
-            constexpr int kLanesPerRow = C::kWide ? 16 : 8;
-            constexpr int kRowsPerPass = kGroupThreads / kLanesPerRow;
-            const int grp = warp / kGroupWarps, gw = warp % kGroupWarps;
-            const int gtid = tid - grp * kGroupThreads;
-            const int slot = gtid / kLanesPerRow;
-            const int c = gtid % kLanesPerRow;
-            const int half = c >> 3, cc = c & 7;                         // wide: chunk c of the 256-byte row = (hi | lo tile, 16-byte chunk)
-            const uint32_t a_base = tiles_u32 + (uint32_t)(grp * C::kStage);
-            // this tile's fills that land in stage `grp`: j = j0, j0 + kStages, ...; the phase bit of fill j follows the ring position
-            for (int j = (grp - st0 + C::kStages) % C::kStages; j < nact; j += C::kStages) {
-                const uint32_t ph = ph0 ^ ((uint32_t)((st0 + j) / C::kStages) & 1u);
-                const int k = s_klist[j];
-                if (lane == 0) mbar_wait(&empty[grp], ph ^ 1u);
-                __syncwarp();
-#pragma unroll
-                for (int w = 0; w < kOwnWords; ++w) {
-                    const uint32_t vs = s_valid[k * 4 + gw * kOwnWords + w];
-                    const uint32_t z = dirty[w] & ~vs;                     // rows that hold data of the stage's previous offset and get none now
-                    dirty[w] = vs;
-                    if (z) {
-#pragma unroll
-                        for (int q4 = 0; q4 < 8; ++q4) {
-                            const int r32 = q4 * 4 + (lane >> 3);
-                            if ((z >> r32) & 1u) {
-                                const uint32_t dst = a_base + (uint32_t)((gw * kOwnRows + w * 32 + r32) * 128 + (lane & 7) * 16);
-                                cg_sts_zero16(dst);
-                                if constexpr (C::kWide) cg_sts_zero16(dst + kCgBM * 128);
-                            }
-                        }
-                    }
-                }
-                const int n = s_cnt[k];
-                const uint32_t *lst = s_list + s_off[k];
-                auto copy_row = [&](uint32_t e) {
-                    const uint32_t r = tl_tile_row(e);
-                    const size_t src = (size_t)tl_in_row(e);
-                    if constexpr (C::kWide)
-                        cg_cp_async16(a_base + (uint32_t)half * (kCgBM * 128) + r * 128u + (((uint32_t)cc ^ (r & 7u)) << 4),
-                                      a.planes + src * 128 + half * 64 + cc * 8);
-                    else
-                        cg_cp_async16(a_base + r * 128u + (((uint32_t)cc ^ (r & 7u)) << 4), a.planes + src * 64 + cc * 8);
-                };
-                // four list entries per round: the shared-memory reads of a round are in flight together
-                int i = slot;
-                for (; i + 3 * kRowsPerPass < n; i += 4 * kRowsPerPass) {
-                    const uint32_t e0 = lst[i], e1 = lst[i + kRowsPerPass], e2 = lst[i + 2 * kRowsPerPass], e3 = lst[i + 3 * kRowsPerPass];
-                    copy_row(e0); copy_row(e1); copy_row(e2); copy_row(e3);
-                }
-                for (; i < n; i += kRowsPerPass) copy_row(lst[i]);
-                asm volatile("cp.async.wait_all;\n" ::: "memory");
-                cg_fence_proxy_async();                                  // copies and clears (generic proxy) -> visible to the tensor core
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&full_a[grp]);
-            }
+            advance_ring(nact);
+            __syncthreads();                                         // lists are rebuilt next; every role is done reading them
         }
-        {   // advance the ring position by this tile's fills
-            const int adv = st0 + nact;
-            ph0 ^= (uint32_t)(adv / C::kStages) & 1u;
-            st0 = adv % C::kStages;
+        if (a.out_info) {
+            const unsigned m = __reduce_max_sync(0xFFFFFFFFu, __float_as_uint(vmax));     // non-negative floats order like their bits
+            if (lane == 0 && m != 0u) atomicMax(reinterpret_cast<unsigned *>(a.out_info), m);
         }
-        __syncthreads();                                         // lists are rebuilt next; every role is done reading them
-    }
-    if (warp >= kCgProdWarps && warp < kCgWeightWarp && a.out_info) {
-        const unsigned m = __reduce_max_sync(0xFFFFFFFFu, __float_as_uint(vmax));     // non-negative floats order like their bits
-        if (lane == 0 && m != 0u) atomicMax(reinterpret_cast<unsigned *>(a.out_info), m);
     }
 }
 
 static int g_cg_deep = 0;          // 1: deep pipeline (sessd_set_sp_cg_deep)
 
+// CTAs of spconv_cg_kernel<CP, COUT, DEEP> that are resident on one SM at once (registers, shared memory, threads).  The first call also
+// raises the kernel's dynamic shared-memory limit.
+template <int CP, int COUT, int DEEP>
+static cudaError_t cg_blocks_per_sm(int *blocks) {
+    using C = CgCfg<CP, COUT, DEEP>;
+    static int cached = 0;
+    if (!cached) {
+        cudaError_t e = cudaFuncSetAttribute(spconv_cg_kernel<CP, COUT, DEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem);
+        if (e == cudaSuccess)
+            e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cached, spconv_cg_kernel<CP, COUT, DEEP>, kCgThreads, C::kSmem);
+        if (e != cudaSuccess) { cached = 0; return e; }
+        if (!cached) return cudaErrorInvalidConfiguration;
+    }
+    *blocks = cached;
+    return cudaSuccess;
+}
+
 template <int CP, int COUT, int DEEP>
 static int launch_spconv_cg(const CgArgs &a, const void *w_h2, cudaStream_t st) {
     using C = CgCfg<CP, COUT, DEEP>;
-    static bool attr_done = false;
-    if (!attr_done) {
-        cudaError_t e = cudaFuncSetAttribute(spconv_cg_kernel<CP, COUT, DEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem);
-        if (e != cudaSuccess) return (int)e;
-        attr_done = true;
-    }
+    int blocks_per_sm = 0;
+    SESSD_CUDA_TRY((cg_blocks_per_sm<CP, COUT, DEEP>(&blocks_per_sm)));
     CUtensorMap map_w;
     int rc;
     if (C::kWide) {       // [kvol][2 (hi|lo)][Cout][64]
@@ -409,7 +459,7 @@ static int launch_spconv_cg(const CgArgs &a, const void *w_h2, cudaStream_t st) 
         SESSD_CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
     }
     const int tiles = div_up(a.max_out, kCgBM);
-    const int grid = tiles < num_sms ? tiles : num_sms;                          // persistent, one CTA per SM
+    const int grid = tiles < blocks_per_sm * num_sms ? tiles : blocks_per_sm * num_sms;     // persistent, every CTA resident at once
     SESSD_LAUNCH((spconv_cg_kernel<CP, COUT, DEEP>), grid, kCgThreads, C::kSmem, st, map_w, a);
     return last_error();
 }
@@ -421,6 +471,23 @@ using namespace sessd;
 // 1: twice the stages (launches with fewer tiles than SMs, e.g. single frames: the serial fill chain of a tile is latency-bound);
 // 0 (default): the shorter ring (many tiles: throughput)
 extern "C" void sessd_set_sp_cg_deep(int on) { sessd::g_cg_deep = on ? 1 : 0; }
+
+template <int CP, int COUT>
+static int cg_blocks_per_sm_or_error(int deep) {
+    int blocks = 0;
+    const cudaError_t e = deep ? cg_blocks_per_sm<CP, COUT, 1>(&blocks) : cg_blocks_per_sm<CP, COUT, 0>(&blocks);
+    return e == cudaSuccess ? blocks : -(int)e;
+}
+
+// CTAs of the (cp, cout, deep) instantiation resident on one SM of the current device (the grid is that many per SM at most);
+// SESSD_EINVAL for an unsupported (cp, cout), -cudaError on a CUDA error
+extern "C" int sessd_spconv_cg_blocks_per_sm(int cp, int cout, int deep) {
+    if (cp == 32 && cout == 32) return cg_blocks_per_sm_or_error<32, 32>(deep);
+    if (cp == 32 && cout == 64) return cg_blocks_per_sm_or_error<32, 64>(deep);
+    if (cp == 64 && cout == 32) return cg_blocks_per_sm_or_error<64, 32>(deep);
+    if (cp == 64 && cout == 64) return cg_blocks_per_sm_or_error<64, 64>(deep);
+    return SESSD_EINVAL;
+}
 
 // S4 (scn.py:106-149), pair-proportional tensor-core path.  d_in_planes [plane_rows][2][cp] fp16 with d_in_info = {abs-max, scale};
 // weights / d_scale from ops.pack_weight_sp_h2 (cp = 64: [kvol][2][Cout][64], cp = 32: [kvol][2][Cout][32]; d_scale = BN scale *

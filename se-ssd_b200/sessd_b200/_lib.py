@@ -70,6 +70,7 @@ SIGNATURES = {
     "sessd_spconv_forward_rows_planes": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _f, _f, _vp, _vp, _i, _vp, _vp]),
     "sessd_spconv_forward_cg": (_i, [_vp, _i, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _f, _f, _vp, _vp, _vp, _vp]),
     "sessd_set_sp_cg_deep": (None, [_i]),
+    "sessd_spconv_cg_blocks_per_sm": (_i, [_i, _i, _i]),
     "sessd_absmax_rows": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
     "sessd_rulebook_transpose": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp]),
     "sessd_sparse_split_planes": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _vp]),

@@ -235,6 +235,13 @@ def set_sp_cg_deep(on):
     lib.sessd_set_sp_cg_deep(int(on))
 
 
+def spconv_cg_blocks_per_sm(cp, cout, deep=0):
+    """CTAs of spconv_forward_cg's (cp, cout, deep) kernel resident on one SM of the current device"""
+    n = int(lib.sessd_spconv_cg_blocks_per_sm(int(cp), int(cout), int(deep)))
+    check(min(n, 0), "sessd_spconv_cg_blocks_per_sm")
+    return n
+
+
 # ---- backward of the sparse convs (csrc/spconv_grad.cu) -------------------------------------------------------------------------
 def rulebook_transpose(nbr, n_out, max_out, max_in, nbr_t=None):
     """nbr [max_out, kvol] -> nbr_t [max_in, kvol]: nbr_t[i, k] = o where nbr[o, k] = i, else -1 (strided layers' data gradient)"""
