@@ -280,6 +280,20 @@ int sessd_absmax(const float *d_x, long long n, float *d_amax, void *stream);
  * head layout per pixel: [box 2x7 | cls 2 | dir 2x2 | iou 2] = 22 floats, row stride head_stride (22, or 24 when the
  * fused 128->22 head GEMM pads its output to a multiple of 4 channels).
  * ------------------------------------------------------------------------------------------------ */
+
+/* DI-NMS (IoU-weighted rotated NMS, nms_cpu.h:173-384 with box_torch_ops.rotate_weighted_nms's centerness) constants; the SE-SSD /
+ * CIA-SSD head's values (mg_head_sessd.py:1001-1018) in brackets. */
+typedef struct {
+    float cnt_thresh;          /* 2.6: a pick is emitted when sum over same-label j with IoU > 0 of IoU * q_j exceeds this */
+    float dist_edge[4];        /* 0, 20, 40, 60: band b = [dist_edge[b], dist_edge[b+1]) of the pick's distance to the origin */
+    float sigma2[3];           /* 0.0009, 0.009, 0.1: weight exp(-(1 - IoU)^2 / sigma2[b]); no band (>= dist_edge[3]): weight 0 */
+    float suppressed_thresh;   /* 0.3: members have IoU > thr; IoU >= thr suppresses */
+    float centerness_pow;      /* 2 */
+    int centerness;            /* 1: score *= (1 - softmax_k(|centre - anchor centre|))^centerness_pow before the loop */
+} sessd_dinms_cfg;
+
+#define SESSD_DINMS_MAX_PRE 4096   /* DI-NMS keeps a dense [pre_max, pre_max] fp32 IoU matrix per frame: 64 MB at the cap */
+
 typedef struct {
     int batch;
     int num_anchors;           /* per frame (70400) */
@@ -293,6 +307,8 @@ typedef struct {
     float post_range[6];       /* 0,-40,-5,70.4,40,5 */
     float direction_offset;    /* 0 */
     int use_frustum;           /* apply the calib frustum filter (mg_head_sessd.py:1024-1030) */
+    int nms_mode;              /* 0: rotate_nms (greedy, nms_iou_thresh, nms_ge); 1: DI-NMS (rotate_weighted_nms, constants below) */
+    sessd_dinms_cfg dinms;     /* read in nms_mode 1 only: a zero-initialised config keeps rotate_nms */
 } sessd_post_cfg;
 
 size_t sessd_postprocess_workspace_bytes(const sessd_post_cfg *cfg);
@@ -301,7 +317,10 @@ size_t sessd_postprocess_workspace_bytes(const sessd_post_cfg *cfg);
  * d_frustum [batch, 6, 4] plane (a,b,c,d) per surface (nullable unless use_frustum);
  * outputs: d_boxes [batch, post_max, 7], d_scores [batch, post_max], d_labels [batch, post_max] i32,
  * d_count [batch] i32, d_aux [batch, 4] i32 (candidates, pre-NMS count, NMS-selected count, reserved),
- * d_sel_anchor [batch, post_max] i32 (anchor index of each NMS-selected box, before frustum/range masks). */
+ * d_sel_anchor [batch, post_max] i32 (anchor index of each NMS-selected box, before frustum/range masks).
+ * nms_mode 1 (DI-NMS): nms_pre_max <= SESSD_DINMS_MAX_PRE, and every "post_max" above is nms_pre_max (DI-NMS applies no post_max);
+ * the boxes are the clusters' weighted averages, d_sel_anchor holds each emitted cluster's pick, d_aux[2] the emitted clusters and
+ * d_aux[3] the loop's picks. */
 int sessd_postprocess(const float *d_head, const float *d_anchors, const float *d_frustum,
                       const sessd_post_cfg *cfg, float *d_boxes, float *d_scores, int *d_labels, int *d_count,
                       int *d_aux, int *d_sel_anchor, void *workspace, size_t workspace_bytes, void *stream);
@@ -324,6 +343,20 @@ size_t sessd_rotate_nms_workspace_bytes(int max_boxes, int pre_max);
 int sessd_rotate_nms(const float *d_boxes5, const float *d_scores, const int *d_n, int max_boxes, int pre_max,
                      int post_max, float iou_thresh, int ge, int *d_keep, int *d_num_keep, void *workspace,
                      size_t workspace_bytes, void *stream);
+
+/* stand-alone DI-NMS: box_torch_ops.rotate_weighted_nms (box_torch_ops.py:552-621) with the C core nms_cpu.h:173-384.
+ * Inputs, n = min(*d_n, max_boxes) rows: d_boxes7 [n,7] (averaged and distance-tested), d_boxes5 [n,5] (x,y,w,l,r: the IoU
+ * geometry), d_scores [n] (>= 0), d_iou_preds [n] (the rectified q = (iou + 1) / 2), d_labels [n] i32, d_dirs [n] i32, d_anchors
+ * [n,7] (read when cfg->centerness; nullable otherwise).  Top-k = min(n, pre_max) by score (equal scores: lower index first), then
+ * the loop.  Outputs, one row per emitted cluster in pick order: d_out_boxes [pre_max,7], d_out_scores, d_out_labels,
+ * d_out_dirs, d_keep (the pick's top-k position), d_selected (the pick's input index); d_count [2] = emitted clusters, picks.
+ * Rows beyond the count are left unwritten.  pre_max <= SESSD_DINMS_MAX_PRE. */
+size_t sessd_rotate_weighted_nms_workspace_bytes(int max_boxes, int pre_max);
+int sessd_rotate_weighted_nms(const float *d_boxes7, const float *d_boxes5, const float *d_scores, const float *d_iou_preds,
+                              const int *d_labels, const int *d_dirs, const float *d_anchors, const int *d_n, int max_boxes,
+                              int pre_max, const sessd_dinms_cfg *cfg, float *d_out_boxes, float *d_out_scores, int *d_out_labels,
+                              int *d_out_dirs, int *d_keep, int *d_selected, int *d_count, void *workspace, size_t workspace_bytes,
+                              void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * I1/I2: the iou3d_cuda extension.  Replaces det3d/core/iou3d/src/iou3d.cpp:34-281 (+ iou3d_kernel.cu

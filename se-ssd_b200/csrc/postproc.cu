@@ -20,6 +20,10 @@
 //                 IoU >= thr (nms_cpu.h:155; '>' selectable for iou3d nms_gpu semantics).
 //   5. finalize : greedy scan (stops at nms_post_max), frustum planes, direction flip (mg_head_sessd.py:1035-1037),
 //                 post-centre range mask (:1040-1045), ordered compaction into the fixed-size outputs.
+// DI-NMS (cfg.nms_mode 1, mg_head_sessd.py:999-1018 -> box_torch_ops.py:552-621 -> nms_cpu.h:173-384) replaces 4 and the scan of 5:
+//   4'. overlap : the dense k x k BEV IoU matrix of each frame, on the 32x32 upper-triangle tiles of stage 4.
+//   4''. cluster: one CTA per frame: the centerness softmax, then one pick per iteration (block argmax, a pass over the pick's
+//                 matrix row, block reductions); emitted clusters feed the frustum / flip / range / compaction of stage 5.
 // Compiled with -fmad=false (rotbox.cuh).
 #include "common.cuh"
 #include "rotbox.cuh"
@@ -39,12 +43,22 @@ struct PostWs {
     float *sscore;                 // [B, K]
     int *sdir;                     // [B, K]
     unsigned long long *mask;      // [B, K, K/64]
+    // DI-NMS only (null in rotate_nms mode, which carves exactly the buffers above)
+    float *iou;                    // [B, K, K] BEV IoU matrix
+    float *sq;                     // [B, K] rectified IoU prediction q = (iou + 1) / 2
+    int *slab;                     // [B, K] labels: stand-alone entry only (null on the head path: one class, label 0)
+    float *obox;                   // [B, K, 7] emitted clusters (head path): averaged box
+    float *oscore;                 // [B, K]
+    int *odir;                     // [B, K]
+    int *osel;                     // [B, K] anchor index of the pick
+    int *ostat;                    // [B, 2] emitted clusters, picks
     size_t bytes;
 };
 
 static inline size_t al(size_t x) { return (x + 255) & ~(size_t)255; }
 
-static PostWs post_carve(void *base, int batch, int anchors, int k) {
+// dinms: carve the DI-NMS buffers; labels: also the per-candidate labels, which only the stand-alone entry fills
+static PostWs post_carve(void *base, int batch, int anchors, int k, bool dinms = false, bool labels = false) {
     PostWs w;
     char *p = (char *)base;
     size_t o = 0;
@@ -60,6 +74,14 @@ static PostWs post_carve(void *base, int batch, int anchors, int k) {
     w.sscore = (float *)take(sizeof(float) * (size_t)batch * k);
     w.sdir = (int *)take(sizeof(int) * (size_t)batch * k);
     w.mask = (unsigned long long *)take(sizeof(unsigned long long) * (size_t)batch * k * cb);
+    w.iou = dinms ? (float *)take(sizeof(float) * (size_t)batch * k * k) : nullptr;
+    w.sq = dinms ? (float *)take(sizeof(float) * (size_t)batch * k) : nullptr;
+    w.slab = (dinms && labels) ? (int *)take(sizeof(int) * (size_t)batch * k) : nullptr;
+    w.obox = dinms ? (float *)take(sizeof(float) * (size_t)batch * k * 7) : nullptr;
+    w.oscore = dinms ? (float *)take(sizeof(float) * (size_t)batch * k) : nullptr;
+    w.odir = dinms ? (int *)take(sizeof(int) * (size_t)batch * k) : nullptr;
+    w.osel = dinms ? (int *)take(sizeof(int) * (size_t)batch * k) : nullptr;
+    w.ostat = dinms ? (int *)take(sizeof(int) * (size_t)batch * 2) : nullptr;
     w.bytes = o;
     return w;
 }
@@ -205,6 +227,7 @@ __global__ void __launch_bounds__(128) post_prepare_kernel(const float *__restri
         w.sscore[o] = key_score(key);
         const float *d = h + 7 * apl + apl + 2 * r;
         w.sdir[o] = (d[1] > d[0]) ? 1 : 0;                           // torch.max(dim=-1)[1]: first max wins
+        if (w.sq) w.sq[o] = (h[7 * apl + apl + 2 * apl + r] + 1.0f) * 0.5f;   // DI-NMS: (iou + 1) * 0.5 (:971)
     }
 }
 
@@ -293,6 +316,278 @@ __global__ void __launch_bounds__(kMaskThreads) post_mask_kernel(PostWs w, int K
     }
 }
 
+// 4'. overlap (DI-NMS) --------------------------------------------------------------------------------------------
+// The loop reads the pick's whole row, every box of the frame included (nms_cpu.h:244-320 clips the pick against all j), so each frame
+// gets a dense k x k matrix.  Same tiles and polygon clips as post_mask_kernel: a tile of the upper triangle computes its pairs once and
+// writes them twice, the mirrored block through a shared-memory transpose, so the matrix is exactly symmetric like the reference's
+// (boost clips (i, j) and (j, i) to the same polygon).  A pair whose stand-up boxes do not overlap gets 0 without a clip.
+// Identical rectangles (the diagonal, duplicate candidates) get exactly 1, as boost's intersection of a ring with itself gives: the
+// clip is not asked to decide that degenerate case.
+__device__ __forceinline__ bool same_rect(const RotBox &a, const RotBox &b) {
+    return a.x1 == b.x1 && a.y1 == b.y1 && a.x2 == b.x2 && a.y2 == b.y2 && a.c == b.c && a.s == b.s;
+}
+
+__global__ void __launch_bounds__(kMaskThreads) dinms_iou_kernel(PostWs w, int K) {
+    const int b = blockIdx.z;
+    const int rb = blockIdx.y, cb = blockIdx.x;
+    const int m = min(w.ncand[b], K);
+    if (cb < rb || rb * kMaskTile >= m || cb * kMaskTile >= m) return;
+    __shared__ RotBox s_col[kMaskTile];
+    __shared__ RotBox s_row[kMaskTile];
+    __shared__ float s_csu[kMaskTile * 4];
+    __shared__ float s_rsu[kMaskTile * 4];
+    __shared__ float s_t[kMaskTile][kMaskTile + 1];
+    const int ncol = min(m - cb * kMaskTile, kMaskTile), nrow = min(m - rb * kMaskTile, kMaskTile);
+    const size_t fb = (size_t)b * K;
+    if ((int)threadIdx.x < kMaskTile) {
+        const int t = threadIdx.x;
+        if (t < ncol) {
+            s_col[t] = w.srot[fb + cb * kMaskTile + t];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) s_csu[t * 4 + k] = w.ssu[(fb + cb * kMaskTile + t) * 4 + k];
+        }
+    } else if (threadIdx.x < 2 * kMaskTile) {
+        const int t = threadIdx.x - kMaskTile;
+        if (t < nrow) {
+            s_row[t] = w.srot[fb + rb * kMaskTile + t];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) s_rsu[t * 4 + k] = w.ssu[(fb + rb * kMaskTile + t) * 4 + k];
+        }
+    }
+    __syncthreads();
+    float *mat = w.iou + fb * K;
+    const int lane = threadIdx.x & 31;
+    for (int r0 = 0; r0 < kMaskTile; r0 += kMaskThreads / 32) {
+        const int r = r0 + (threadIdx.x >> 5), j = lane;
+        if (r < nrow && j < ncol && (rb != cb || j >= r)) {
+            float v = 0.f;
+            if ((rb == cb && j == r) || same_rect(s_row[r], s_col[j])) v = 1.f;
+            else if (standup_iou_pos(s_rsu + r * 4, s_csu + j * 4) > 0.0f) v = rot_iou_bev_pre(s_row[r], s_col[j]);
+            mat[(size_t)(rb * kMaskTile + r) * K + cb * kMaskTile + j] = v;
+            s_t[r][j] = v;
+        }
+    }
+    __syncthreads();
+    // mirrored block: element (row c, column r) = s_t[r][c]; one warp per mirrored row, lanes along its columns
+    for (int c0 = 0; c0 < kMaskTile; c0 += kMaskThreads / 32) {
+        const int c = c0 + (threadIdx.x >> 5), r = lane;
+        if (c < ncol && r < nrow && (rb != cb || c > r)) mat[(size_t)(cb * kMaskTile + c) * K + rb * kMaskTile + r] = s_t[r][c];
+    }
+}
+
+// 4''. cluster loop (DI-NMS) ---------------------------------------------------------------------------------------
+// One CTA per frame; candidate j (top-k position) is owned by thread j % kClusterThreads for the whole kernel, so its state needs no
+// barrier between the pass that writes it and the next pass.  Shared memory: adjusted score, q, label and state of every candidate;
+// state -1 = live, -2 = picked (suppressed for good), it >= 0 = suppressed by pick `it` (its recover list, nms_cpu.h:308-313, 357-360).
+// Per pick: one pass over the pick's matrix row and one block reduction of cnt, wsum, avg[7], score_box and two argmax keys (best live
+// box, best box of this pick's recover list), so the next pick is known without another pass.  The only serial term is the pick count.
+constexpr int kClusterThreads = 512;
+
+struct DinmsOut {
+    float *box;       // [B, K, 7]
+    float *score;     // [B, K]
+    int *label;       // [B, K] nullable
+    int *dir;         // [B, K]
+    int *pos;         // [B, K] nullable: top-k position of the pick
+    int *sel;         // [B, K] anchor / input index of the pick
+    int *stat;        // [B, 2] emitted clusters, picks
+};
+
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        const unsigned long long u = __shfl_xor_sync(0xffffffffu, v, o);
+        v = u > v ? u : v;
+    }
+    return v;
+}
+// block-wide sum or max of one float (all threads get the result); s_tmp: [kClusterThreads / 32 + 1] floats
+__device__ __forceinline__ float block_reduce(float v, bool is_max, float *s_tmp) {
+    constexpr int NW = kClusterThreads / 32;
+    v = is_max ? warp_max(v) : warp_sum(v);
+    if ((threadIdx.x & 31) == 0) s_tmp[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        float u = (threadIdx.x < NW) ? s_tmp[threadIdx.x] : (is_max ? -INFINITY : 0.f);
+        u = is_max ? warp_max(u) : warp_sum(u);
+        if (threadIdx.x == 0) s_tmp[NW] = u;
+    }
+    __syncthreads();
+    const float r = s_tmp[NW];
+    __syncthreads();
+    return r;
+}
+
+__global__ void __launch_bounds__(kClusterThreads) dinms_cluster_kernel(PostWs w, int K, const float *__restrict__ anchors,
+                                                                         sessd_dinms_cfg c, DinmsOut o) {
+    constexpr int NW = kClusterThreads / 32;
+    extern __shared__ float cdyn[];
+    float *s_adj = cdyn;
+    float *s_q = s_adj + K;
+    int *s_lab = (int *)(s_q + K);
+    int *s_state = s_lab + K;
+    __shared__ float s_tmp[NW + 1];
+    __shared__ float s_red[NW][10];
+    __shared__ unsigned long long s_key[NW][2];
+    __shared__ unsigned long long s_next;
+    __shared__ int s_kept;
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const int m = min(w.ncand[b], K);
+    const size_t fb = (size_t)b * K;
+    const float *sbox = w.sbox + fb * 7;
+
+    // centerness (box_torch_ops.py:584-588): d = |centre - anchor centre|, m = softmax(d) over the k candidates,
+    // score *= (1 - m)^pow; d is parked in s_adj until the softmax is known
+    float dmax = -INFINITY;
+    for (int i = tid; i < m; i += kClusterThreads) {
+        const float *an = anchors ? anchors + (size_t)key_index(w.sel[fb + i]) * 7 : nullptr;
+        float d = 0.f;
+        if (c.centerness) {
+            const float dx = fabsf(sbox[i * 7] - an[0]), dy = fabsf(sbox[i * 7 + 1] - an[1]);
+            d = sqrtf(dx * dx + dy * dy);
+        }
+        s_adj[i] = d;
+        dmax = fmaxf(dmax, d);
+    }
+    dmax = block_reduce(dmax, true, s_tmp);
+    float se = 0.f;
+    if (c.centerness)
+        for (int i = tid; i < m; i += kClusterThreads) se += expf(s_adj[i] - dmax);
+    se = block_reduce(se, false, s_tmp);
+    float smax = -INFINITY;
+    unsigned long long best = 0;
+    for (int i = tid; i < m; i += kClusterThreads) {
+        float s = w.sscore[fb + i];
+        if (c.centerness) {
+            const float t = 1.0f - expf(s_adj[i] - dmax) / se;
+            s *= (c.centerness_pow == 2.0f) ? t * t : powf(t, c.centerness_pow);   // torch.pow(x, 2) is x * x
+        }
+        s_adj[i] = s;
+        s_q[i] = w.sq[fb + i];
+        s_lab[i] = w.slab ? w.slab[fb + i] : 0;
+        s_state[i] = -1;
+        smax = fmaxf(smax, s);
+        const unsigned long long key = make_key(s, i);
+        best = key > best ? key : best;
+    }
+    smax = block_reduce(smax, true, s_tmp);          // score_max4norm (nms_cpu.h:226-235)
+    best = warp_max_u64(best);
+    if (lane == 0) s_key[wid][0] = best;
+    __syncthreads();
+    if (tid < 32) {
+        unsigned long long u = tid < NW ? s_key[tid][0] : 0ull;
+        u = warp_max_u64(u);
+        if (tid == 0) s_next = u;
+    }
+    __syncthreads();
+
+    int nout = 0, picks = 0;
+    for (int it = 0;; ++it) {
+        const unsigned long long next = s_next;
+        if (next == 0ull) break;                      // every candidate suppressed
+        const int idx = key_index(next);             // argmax of the adjusted score, strict '>': the first position wins a tie
+        // sigma^2 band of the pick's distance to the origin (sqrt of the fp64 sum, stored as fp32, nms_cpu.h:255)
+        const float px = sbox[idx * 7], py = sbox[idx * 7 + 1];
+        const float dist = (float)sqrt((double)px * (double)px + (double)py * (double)py);
+        float s2 = 0.f;
+        bool band = false;
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+            if (dist >= c.dist_edge[k] && dist < c.dist_edge[k + 1]) { s2 = c.sigma2[k]; band = true; }
+        const float *row = w.iou + (fb + idx) * K;
+        const int li = s_lab[idx];
+        float cnt = 0.f, wsum = 0.f, sb = -1.f, av[7];
+#pragma unroll
+        for (int k = 0; k < 7; ++k) av[k] = 0.f;
+        unsigned long long best_live = 0, best_rec = 0;
+        for (int j = tid; j < m; j += kClusterThreads) {
+            const float ov = row[j];
+            int st = (j == idx) ? -2 : s_state[j];
+            if (s_lab[j] == li) {
+                const float qj = s_q[j];
+                if (ov > 0.f) cnt += ov * qj;
+                if (ov > c.suppressed_thresh) {                                 // member (nms_cpu.h:284-301)
+                    sb = fmaxf(sb, s_adj[j] / smax);
+                    // no band (distance >= the last edge): weight 0, so wsum = 0 and a kept cluster's box is NaN, as in the reference
+                    const float wt = band ? (float)exp(-((double)(1.f - ov) * (double)(1.f - ov)) / (double)s2) : 0.f;
+                    const float wq = wt * qj;
+#pragma unroll
+                    for (int k = 0; k < 7; ++k) av[k] += wq * sbox[j * 7 + k];
+                    wsum += wq;
+                }
+            }
+            // suppression (nms_cpu.h:303-309) also requires overlapping stand-up boxes; IoU >= thr > 0 implies that, so it is not tested
+            if (st == -1 && ov >= c.suppressed_thresh) st = it;
+            s_state[j] = st;
+            const unsigned long long key = make_key(s_adj[j], j);
+            if (st == -1) best_live = key > best_live ? key : best_live;
+            else if (st == it) best_rec = key > best_rec ? key : best_rec;
+        }
+        cnt = warp_sum(cnt);
+        wsum = warp_sum(wsum);
+        sb = warp_max(sb);
+#pragma unroll
+        for (int k = 0; k < 7; ++k) av[k] = warp_sum(av[k]);
+        best_live = warp_max_u64(best_live);
+        best_rec = warp_max_u64(best_rec);
+        if (lane == 0) {
+            s_red[wid][0] = cnt; s_red[wid][1] = wsum; s_red[wid][2] = sb;
+#pragma unroll
+            for (int k = 0; k < 7; ++k) s_red[wid][3 + k] = av[k];
+            s_key[wid][0] = best_live; s_key[wid][1] = best_rec;
+        }
+        __syncthreads();
+        if (tid < 32) {
+            float v[10];
+#pragma unroll
+            for (int k = 0; k < 10; ++k) v[k] = tid < NW ? s_red[tid][k] : (k == 2 ? -1.f : 0.f);
+            unsigned long long kl = tid < NW ? s_key[tid][0] : 0ull, kr = tid < NW ? s_key[tid][1] : 0ull;
+            v[0] = warp_sum(v[0]);
+            v[1] = warp_sum(v[1]);
+            v[2] = warp_max(v[2]);
+#pragma unroll
+            for (int k = 3; k < 10; ++k) v[k] = warp_sum(v[k]);
+            kl = warp_max_u64(kl);
+            kr = warp_max_u64(kr);
+            if (tid == 0) {
+                ++picks;
+                const bool kept = v[0] > c.cnt_thresh;
+                if (kept) {
+                    const size_t r = fb + nout;
+#pragma unroll
+                    for (int k = 0; k < 7; ++k) o.box[r * 7 + k] = v[3 + k] / v[1];
+                    o.score[r] = v[2] * smax;
+                    o.dir[r] = w.sdir[fb + idx];
+                    if (o.label) o.label[r] = li;
+                    if (o.pos) o.pos[r] = idx;
+                    o.sel[r] = key_index(w.sel[fb + idx]);
+                    ++nout;
+                }
+                s_kept = kept;
+                s_next = kept ? kl : (kl > kr ? kl : kr);
+            }
+        }
+        __syncthreads();
+        if (!s_kept)                                  // recover this pick's list (nms_cpu.h:357-360)
+            for (int j = tid; j < m; j += kClusterThreads)
+                if (s_state[j] == it) s_state[j] = -1;
+    }
+    if (tid == 0) {
+        o.stat[2 * b] = nout;
+        o.stat[2 * b + 1] = picks;
+    }
+}
+
 // 5. finalize ------------------------------------------------------------------------------------------------
 // greedy scan shared by the detection path and the stand-alone NMS; returns kept positions (into the sorted list)
 // in s_keep[0..nkeep).  One CTA (256 threads) per frame.
@@ -347,12 +642,15 @@ struct PostPack {
     const int *status;         // [1] nullable
 };
 
+// kDI: the rows come from the DI-NMS cluster loop (w.obox / oscore / odir / osel, w.ostat) instead of the greedy scan over the mask,
+// and the capacity P is nms_pre_max
+template <bool kDI>
 __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post_cfg cfg, const float *__restrict__ frustum,
                                                             float *__restrict__ out_boxes, float *__restrict__ out_scores,
                                                             int *__restrict__ out_labels, int *__restrict__ out_count,
                                                             int *__restrict__ out_aux, int *__restrict__ out_sel_anchor, PostPack pk) {
     extern __shared__ unsigned long long dyn[];
-    const int K = cfg.nms_pre_max, P = cfg.nms_post_max;
+    const int K = cfg.nms_pre_max, P = kDI ? cfg.nms_pre_max : cfg.nms_post_max;
     const int col_blocks = (K + 63) / 64;
     unsigned long long *remv = dyn;
     unsigned long long *diag = dyn + col_blocks;
@@ -364,12 +662,19 @@ __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post
     const int n = w.ncand[b];
     const int m = min(n, K);
     const size_t fb = (size_t)b * K;
-    const int nk = greedy_scan(w.mask + fb * col_blocks, m, col_blocks, P, remv, diag, s_keep, s_misc, &s_kb);
+    int nk;
+    if constexpr (kDI) nk = w.ostat[2 * b];
+    else nk = greedy_scan(w.mask + fb * col_blocks, m, col_blocks, P, remv, diag, s_keep, s_misc, &s_kb);
+    // row t of the kept list: its box, score, direction label and anchor index
+    auto row_box = [&](int t) -> const float * { return kDI ? w.obox + (fb + t) * 7 : w.sbox + (fb + s_keep[t]) * 7; };
+    auto row_score = [&](int t) { return kDI ? w.oscore[fb + t] : w.sscore[fb + s_keep[t]]; };
+    auto row_dir = [&](int t) { return kDI ? w.odir[fb + t] : w.sdir[fb + s_keep[t]]; };
+    auto row_anchor = [&](int t) { return kDI ? w.osel[fb + t] : key_index(w.sel[fb + s_keep[t]]); };
     // per kept box: frustum test + range mask (the direction fix happens before the range test but only touches r)
     for (int t = threadIdx.x; t < P; t += blockDim.x) {
         int ok = 0;
         if (t < nk) {
-            const float *bx = w.sbox + (fb + s_keep[t]) * 7;
+            const float *bx = row_box(t);
             ok = 1;
             if (cfg.use_frustum && frustum) {
                 const float *pl = frustum + (size_t)b * 24;
@@ -380,7 +685,7 @@ __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post
             }
             for (int j = 0; j < 3; ++j)
                 if (!(bx[j] >= cfg.post_range[j] && bx[j] <= cfg.post_range[3 + j])) ok = 0;
-            out_sel_anchor[(size_t)b * P + t] = key_index(w.sel[fb + s_keep[t]]);
+            out_sel_anchor[(size_t)b * P + t] = row_anchor(t);
         } else {
             out_sel_anchor[(size_t)b * P + t] = -1;
         }
@@ -395,7 +700,7 @@ __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post
         out_aux[b * 4 + 0] = n;
         out_aux[b * 4 + 1] = m;
         out_aux[b * 4 + 2] = nk;
-        out_aux[b * 4 + 3] = 0;
+        out_aux[b * 4 + 3] = kDI ? w.ostat[2 * b + 1] : 0;
         s_misc[1] = c;
         if (pk.meta) {
             int *mt = pk.meta + (size_t)b * (8 + P);
@@ -410,23 +715,24 @@ __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post
     for (int t = threadIdx.x; t < P; t += blockDim.x) {
         const int dst = s_flag[t];
         if (dst >= 0) {
-            const size_t src = fb + s_keep[t];
+            const float *bx = row_box(t);
             float *ob = out_boxes + ((size_t)b * P + dst) * 7;
 #pragma unroll
-            for (int j = 0; j < 6; ++j) ob[j] = w.sbox[src * 7 + j];
-            float r = w.sbox[src * 7 + 6];
-            const bool opp = ((r - cfg.direction_offset) > 0.f) != (w.sdir[src] == 1);   // :1035-1037
+            for (int j = 0; j < 6; ++j) ob[j] = bx[j];
+            float r = bx[6];
+            const bool opp = ((r - cfg.direction_offset) > 0.f) != (row_dir(t) == 1);   // :1035-1037
             if (opp) r += 3.14159265358979323846f;   // torch.tensor(np.pi).type_as(fp32)
             ob[6] = r;
-            out_scores[(size_t)b * P + dst] = w.sscore[src];
+            const float sc = row_score(t);
+            out_scores[(size_t)b * P + dst] = sc;
             out_labels[(size_t)b * P + dst] = 0;
             if (pk.packed) {
                 float *pp = pk.packed + ((size_t)b * P + dst) * 8;
 #pragma unroll
                 for (int j = 0; j < 6; ++j) pp[j] = ob[j];
                 pp[6] = r;
-                pp[7] = w.sscore[src];
-                pk.meta[(size_t)b * (8 + P) + 8 + dst] = key_index(w.sel[src]);
+                pp[7] = sc;
+                pk.meta[(size_t)b * (8 + P) + 8 + dst] = row_anchor(t);
             }
         }
     }
@@ -463,7 +769,24 @@ using namespace sessd;
 
 extern "C" size_t sessd_postprocess_workspace_bytes(const sessd_post_cfg *cfg) {
     if (!cfg) return 0;
-    return post_carve(nullptr, cfg->batch, cfg->num_anchors, cfg->nms_pre_max).bytes;
+    return post_carve(nullptr, cfg->batch, cfg->num_anchors, cfg->nms_pre_max, cfg->nms_mode == 1).bytes;
+}
+
+static bool dinms_cfg_ok(const sessd_dinms_cfg &c) {
+    return c.suppressed_thresh > 0.f && c.sigma2[0] > 0.f && c.sigma2[1] > 0.f && c.sigma2[2] > 0.f;
+}
+
+static size_t cluster_smem(int K) { return (sizeof(float) * 2 + sizeof(int) * 2) * (size_t)K; }
+
+// overlap matrix + cluster loop of B frames whose candidates stage 3 (or dinms_prepare_kernel) has laid out in w
+static int dinms_launch(PostWs w, int B, int K, const float *d_anchors, const sessd_dinms_cfg &c, DinmsOut o, cudaStream_t st) {
+    const int cb = (K + kMaskTile - 1) / kMaskTile;
+    dim3 g(cb, cb, B);
+    SESSD_LAUNCH(dinms_iou_kernel, g, kMaskThreads, 0, st, w, K);
+    const size_t sm = cluster_smem(K);
+    if (sm > 48 * 1024) SESSD_CUDA_TRY(cudaFuncSetAttribute(dinms_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    SESSD_LAUNCH(dinms_cluster_kernel, B, kClusterThreads, sm, st, w, K, d_anchors, c, o);
+    return 0;
 }
 
 static size_t finalize_smem(int K, int P) {
@@ -480,10 +803,13 @@ static int postprocess_impl(const float *d_head, const float *d_anchors, const f
         cfg->nms_pre_max < 1 || cfg->nms_post_max < 1 || cfg->nms_post_max > 4096 || cfg->nms_pre_max > 16384)
         return SESSD_EINVAL;
     if (cfg->anchors_per_loc != 2 || cfg->head_stride < 22) return SESSD_EINVAL;   // head layout is fixed at 22 channels
-    PostWs w = post_carve(workspace, cfg->batch, cfg->num_anchors, cfg->nms_pre_max);
+    if (cfg->nms_mode != 0 && cfg->nms_mode != 1) return SESSD_EINVAL;
+    const bool dinms = cfg->nms_mode == 1;
+    if (dinms && (cfg->nms_pre_max > SESSD_DINMS_MAX_PRE || !dinms_cfg_ok(cfg->dinms))) return SESSD_EINVAL;
+    PostWs w = post_carve(workspace, cfg->batch, cfg->num_anchors, cfg->nms_pre_max, dinms);
     if (!workspace || w.bytes > workspace_bytes) return SESSD_EWORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;
-    const int B = cfg->batch, A = cfg->num_anchors, K = cfg->nms_pre_max, P = cfg->nms_post_max;
+    const int B = cfg->batch, A = cfg->num_anchors, K = cfg->nms_pre_max, P = dinms ? K : cfg->nms_post_max;
     SESSD_CUDA_TRY(cudaMemsetAsync(w.ncand, 0, sizeof(int) * B, st));
     dim3 g1(div_up(A, 256), B);
     SESSD_LAUNCH(post_score_kernel, g1, 256, 0, st, d_head, *cfg, w.cand, w.ncand);
@@ -491,12 +817,22 @@ static int postprocess_impl(const float *d_head, const float *d_anchors, const f
     SESSD_LAUNCH(post_select_kernel, g2, 256, 0, st, w.cand, w.ncand, A, K, w.sel);
     dim3 g3(div_up(K, 128), B);
     SESSD_LAUNCH(post_prepare_kernel, g3, 128, 0, st, d_head, d_anchors, *cfg, w);
+    const size_t sm = finalize_smem(K, P);
+    if (dinms) {
+        DinmsOut o = {w.obox, w.oscore, nullptr, w.odir, nullptr, w.osel, w.ostat};
+        const int rc = dinms_launch(w, B, K, d_anchors, cfg->dinms, o, st);
+        if (rc) return rc;
+        if (sm > 48 * 1024)
+            SESSD_CUDA_TRY(cudaFuncSetAttribute(post_finalize_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+        SESSD_LAUNCH(post_finalize_kernel<true>, B, 256, sm, st, w, *cfg, d_frustum, d_boxes, d_scores, d_labels, d_count, d_aux,
+                     d_sel_anchor, pk);
+        return last_error();
+    }
     const int cb = (K + kMaskTile - 1) / kMaskTile;
     dim3 g4(cb, cb, B);
     SESSD_LAUNCH(post_mask_kernel, g4, kMaskThreads, 0, st, w, K, cfg->nms_iou_thresh, cfg->nms_ge);
-    const size_t sm = finalize_smem(K, P);
-    if (sm > 48 * 1024) SESSD_CUDA_TRY(cudaFuncSetAttribute(post_finalize_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    SESSD_LAUNCH(post_finalize_kernel, B, 256, sm, st, w, *cfg, d_frustum, d_boxes, d_scores, d_labels, d_count, d_aux, d_sel_anchor, pk);
+    if (sm > 48 * 1024) SESSD_CUDA_TRY(cudaFuncSetAttribute(post_finalize_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    SESSD_LAUNCH(post_finalize_kernel<false>, B, 256, sm, st, w, *cfg, d_frustum, d_boxes, d_scores, d_labels, d_count, d_aux, d_sel_anchor, pk);
     return last_error();
 }
 
@@ -542,5 +878,55 @@ extern "C" int sessd_rotate_nms(const float *d_boxes5, const float *d_scores, co
     const size_t sm = finalize_smem(pre_max, post_max);
     if (sm > 48 * 1024) SESSD_CUDA_TRY(cudaFuncSetAttribute(nms_finalize_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
     SESSD_LAUNCH(nms_finalize_kernel, 1, 256, sm, st, w, pre_max, post_max, d_keep, d_num_keep);
+    return last_error();
+}
+
+// ---------------------------------------------------------------------------------------------------------------- stand-alone DI-NMS
+// gather the top-k rows of the caller's arrays into the layout the overlap stage and the cluster loop read
+__global__ void __launch_bounds__(128) dinms_prepare_kernel(const float *__restrict__ boxes7, const float *__restrict__ boxes5,
+                                                            const float *__restrict__ scores, const float *__restrict__ iou_preds,
+                                                            const int *__restrict__ labels, const int *__restrict__ dirs, int K, PostWs w) {
+    const int m = min(w.ncand[0], K);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+        const int src = key_index(w.sel[i]);
+        const float *q = boxes5 + (size_t)src * 5;
+        float box[7] = {q[0], q[1], 0.f, q[2], q[3], 0.f, q[4]};
+        nms_geometry(box, w.sbev + (size_t)i * 5, w.ssu + (size_t)i * 4);
+        const float *bv = w.sbev + (size_t)i * 5;
+        w.srot[i] = rot_prepare(bv[0], bv[1], bv[2], bv[3], bv[4]);
+#pragma unroll
+        for (int j = 0; j < 7; ++j) w.sbox[(size_t)i * 7 + j] = boxes7[(size_t)src * 7 + j];
+        w.sscore[i] = scores[src];
+        w.sq[i] = iou_preds[src];
+        w.slab[i] = labels[src];
+        w.sdir[i] = dirs[src];
+    }
+}
+
+extern "C" size_t sessd_rotate_weighted_nms_workspace_bytes(int max_boxes, int pre_max) {
+    if (max_boxes < 1 || pre_max < 1) return 0;
+    return post_carve(nullptr, 1, max_boxes, pre_max, true, true).bytes;
+}
+
+extern "C" int sessd_rotate_weighted_nms(const float *d_boxes7, const float *d_boxes5, const float *d_scores, const float *d_iou_preds,
+                                         const int *d_labels, const int *d_dirs, const float *d_anchors, const int *d_n, int max_boxes,
+                                         int pre_max, const sessd_dinms_cfg *cfg, float *d_out_boxes, float *d_out_scores,
+                                         int *d_out_labels, int *d_out_dirs, int *d_keep, int *d_selected, int *d_count, void *workspace,
+                                         size_t workspace_bytes, void *stream) {
+    if (!d_boxes7 || !d_boxes5 || !d_scores || !d_iou_preds || !d_labels || !d_dirs || !d_n || !cfg || !d_out_boxes || !d_out_scores ||
+        !d_out_labels || !d_out_dirs || !d_keep || !d_selected || !d_count || max_boxes < 1 || pre_max < 1 ||
+        pre_max > SESSD_DINMS_MAX_PRE || !dinms_cfg_ok(*cfg) || (cfg->centerness && !d_anchors))
+        return SESSD_EINVAL;
+    PostWs w = post_carve(workspace, 1, max_boxes, pre_max, true, true);
+    if (!workspace || w.bytes > workspace_bytes) return SESSD_EWORKSPACE;
+    cudaStream_t st = (cudaStream_t)stream;
+    SESSD_LAUNCH(keys_from_scores_kernel, persistent_grid(max_boxes, 256), 256, 0, st, d_scores, d_n, max_boxes, w.cand, w.ncand);
+    dim3 g2(div_up(max_boxes, 256), 1);
+    SESSD_LAUNCH(post_select_kernel, g2, 256, 0, st, w.cand, w.ncand, max_boxes, pre_max, w.sel);
+    SESSD_LAUNCH(dinms_prepare_kernel, div_up(pre_max, 128), 128, 0, st, d_boxes7, d_boxes5, d_scores, d_iou_preds, d_labels, d_dirs,
+                 pre_max, w);
+    DinmsOut o = {d_out_boxes, d_out_scores, d_out_labels, d_out_dirs, d_keep, d_selected, d_count};
+    const int rc = dinms_launch(w, 1, pre_max, d_anchors, *cfg, o, st);
+    if (rc) return rc;
     return last_error();
 }

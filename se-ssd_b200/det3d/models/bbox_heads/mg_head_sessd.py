@@ -345,14 +345,17 @@ class MultiGroupHead(nn.Module):
             fr = fr.cpu().numpy() if isinstance(fr, torch.Tensor) else np.asarray(fr)
             planes = np.stack([frustum_planes(fr[i])[0] for i in range(batch)], 0)          # [B, 6, 4]
             frustum = torch.from_numpy(np.ascontiguousarray(planes, np.float32)).to(packed.device)
+        # "rotate_weighted_nms" selects DI-NMS with the head's constants (mg_head_sessd.py:999-1018 of the reference, where the choice is
+        # a local variable); a config without the key keeps rotate_nms
+        nms_type = nms.get("nms_type", "rotate_nms") if hasattr(nms, "get") else getattr(nms, "nms_type", "rotate_nms")
         key = (batch, int(anc.shape[0]), float(self.thresh), int(nms["nms_pre_max_size"]), int(nms["nms_post_max_size"]),
-               float(nms["nms_iou_threshold"]), frustum is not None, str(packed.device))
+               float(nms["nms_iou_threshold"]), frustum is not None, str(packed.device), nms_type)
         if self._post is None or self._post_key != key:
             cfg = ops.make_post_cfg(batch=batch, num_anchors=int(anc.shape[0]), anchors_per_loc=self.num_anchor_per_locs[0],
                                     head_stride=24, score_thresh=self.thresh, nms_pre_max=nms["nms_pre_max_size"],
                                     nms_post_max=nms["nms_post_max_size"], nms_iou_thresh=nms["nms_iou_threshold"], nms_ge=True,
                                     post_range=self.post_center_range, direction_offset=getattr(self, "direction_offset", 0.0),
-                                    use_frustum=frustum is not None)
+                                    use_frustum=frustum is not None, nms_type=nms_type)
             self._post, self._post_key = ops.PostBuffers(cfg, packed.device), key
         buf = ops.postprocess(packed.contiguous(), anc, frustum, self._post)
         counts = buf.count.cpu().tolist()                       # the one host sync of the frame

@@ -32,11 +32,16 @@ class ConvDesc(C.Structure):
                 ("ntaps", C.c_int), ("tap_dy", C.c_int * 16), ("tap_dx", C.c_int * 16), ("relu", C.c_int)]
 
 
+class DinmsCfg(C.Structure):
+    _fields_ = [("cnt_thresh", C.c_float), ("dist_edge", C.c_float * 4), ("sigma2", C.c_float * 3), ("suppressed_thresh", C.c_float),
+                ("centerness_pow", C.c_float), ("centerness", C.c_int)]
+
+
 class PostCfg(C.Structure):
     _fields_ = [("batch", C.c_int), ("num_anchors", C.c_int), ("anchors_per_loc", C.c_int), ("head_stride", C.c_int),
                 ("score_thresh", C.c_float), ("nms_pre_max", C.c_int), ("nms_post_max", C.c_int),
                 ("nms_iou_thresh", C.c_float), ("nms_ge", C.c_int), ("post_range", C.c_float * 6),
-                ("direction_offset", C.c_float), ("use_frustum", C.c_int)]
+                ("direction_offset", C.c_float), ("use_frustum", C.c_int), ("nms_mode", C.c_int), ("dinms", DinmsCfg)]
 
 
 class KittiFrames(C.Structure):
@@ -98,6 +103,9 @@ SIGNATURES = {
     "sessd_postprocess_packed": (_i, [_vp, _vp, _vp, C.POINTER(PostCfg), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "sessd_rotate_nms_workspace_bytes": (_sz, [_i, _i]),
     "sessd_rotate_nms": (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _i, _vp, _vp, _vp, _sz, _vp]),
+    "sessd_rotate_weighted_nms_workspace_bytes": (_sz, [_i, _i]),
+    "sessd_rotate_weighted_nms": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, C.POINTER(DinmsCfg), _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                       _vp, _sz, _vp]),
     "sessd_boxes_overlap_bev": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
     "sessd_boxes_aligned_overlap_bev": (_i, [_vp, _vp, _i, _vp, _vp]),
     "sessd_boxes_iou_bev": (_i, [_vp, _i, _vp, _i, _vp, _vp]),

@@ -38,7 +38,7 @@ class FrameEngine:
         pk.update(post_kwargs or {})
         self.pcfg = ops.make_post_cfg(**pk)
         self.post = ops.PostBuffers(self.pcfg, dev)
-        P = self.pcfg.nms_post_max
+        P = ops.post_capacity(self.pcfg)
         # packed result block (written by post_finalize_kernel): [B,P,8] = box 7 | score; meta [B, 8+P] = count, candidates, pre-NMS,
         # NMS-selected, voxels, capacity status, 0, 0, anchor index of every returned detection
         self.d_result = torch.zeros((self.batch, P, 8), dtype=torch.float32, device=dev)

@@ -9,7 +9,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import ConvDesc, Grid, PostCfg, VoxelCfg, check, lib
+from ._lib import ConvDesc, DinmsCfg, Grid, PostCfg, VoxelCfg, check, lib
 
 
 def _p(t):
@@ -469,9 +469,33 @@ def absmax(x, amax):
 
 
 # ------------------------------------------------------------------------------------------------ post-processing
+NMS_TYPES = ("rotate_nms", "rotate_weighted_nms")
+DINMS_MAX_PRE = 4096          # SESSD_DINMS_MAX_PRE
+
+
+def make_dinms_cfg(nms_cnt_thresh=2.6, nms_sigma_dist_interval=(0, 20, 40, 60), nms_sigma_square=(0.0009, 0.009, 0.1, 1),
+                   suppressed_thresh=0.3, centerness_pow=2, enable_centerness=True):
+    """DI-NMS constants; the defaults are the values get_task_detections passes (mg_head_sessd.py:1001-1018).  The fourth sigma^2
+    of the reference's tuple belongs to no band and is never read."""
+    if len(nms_sigma_dist_interval) != 4 or len(nms_sigma_square) < 3:
+        raise ValueError("DI-NMS takes four distance edges (three bands) and their three sigma^2")
+    d = DinmsCfg()
+    d.cnt_thresh, d.suppressed_thresh, d.centerness_pow = float(nms_cnt_thresh), float(suppressed_thresh), float(centerness_pow)
+    for j in range(4):
+        d.dist_edge[j] = float(nms_sigma_dist_interval[j])
+    for j in range(3):
+        d.sigma2[j] = float(nms_sigma_square[j])
+    d.centerness = int(bool(enable_centerness))
+    return d
+
+
 def make_post_cfg(batch, num_anchors=70400, anchors_per_loc=2, head_stride=24, score_thresh=0.3, nms_pre_max=1000, nms_post_max=100,
                   nms_iou_thresh=0.01, nms_ge=True, post_range=(0, -40.0, -5.0, 70.4, 40.0, 5.0), direction_offset=0.0,
-                  use_frustum=False):
+                  use_frustum=False, nms_type="rotate_nms"):
+    """nms_type "rotate_nms" (greedy rotated NMS) or "rotate_weighted_nms" (DI-NMS with the head's constants, make_dinms_cfg();
+    it keeps up to nms_pre_max detections and ignores nms_post_max, nms_iou_thresh and nms_ge, as the reference does)"""
+    if nms_type not in NMS_TYPES:
+        raise ValueError("nms_type must be one of %s, not %r" % (NMS_TYPES, nms_type))
     c = PostCfg()
     c.batch, c.num_anchors, c.anchors_per_loc, c.head_stride = int(batch), int(num_anchors), int(anchors_per_loc), int(head_stride)
     c.score_thresh, c.nms_pre_max, c.nms_post_max = float(score_thresh), int(nms_pre_max), int(nms_post_max)
@@ -479,13 +503,20 @@ def make_post_cfg(batch, num_anchors=70400, anchors_per_loc=2, head_stride=24, s
     for j in range(6):
         c.post_range[j] = float(post_range[j])
     c.direction_offset, c.use_frustum = float(direction_offset), int(bool(use_frustum))
+    if nms_type == "rotate_weighted_nms":
+        c.nms_mode, c.dinms = 1, make_dinms_cfg()
     return c
+
+
+def post_capacity(cfg):
+    """detections per frame the post-processing outputs hold: nms_post_max, or nms_pre_max under DI-NMS"""
+    return cfg.nms_pre_max if cfg.nms_mode == 1 else cfg.nms_post_max
 
 
 class PostBuffers:
     def __init__(self, cfg, device):
         self.cfg = cfg
-        b, p = cfg.batch, cfg.nms_post_max
+        b, p = cfg.batch, post_capacity(cfg)
         self.boxes = torch.zeros((b, p, 7), dtype=torch.float32, device=device)
         self.scores = torch.zeros((b, p), dtype=torch.float32, device=device)
         self.labels = torch.zeros((b, p), dtype=torch.int32, device=device)
@@ -517,6 +548,33 @@ def rotate_nms(boxes5, scores, n, max_boxes, pre_max, post_max, iou_thresh, ge=T
     check(lib.sessd_rotate_nms(_p(boxes5), _p(scores), _p(n), int(max_boxes), int(pre_max), int(post_max), float(iou_thresh),
                                int(bool(ge)), _p(keep), _p(num), _p(ws), ws.numel(), _st()), "sessd_rotate_nms")
     return keep, num
+
+
+def rotate_weighted_nms(boxes7, boxes5, scores, iou_preds, labels, dirs, anchors, n, max_boxes, pre_max, dinms_cfg, ws=None):
+    """Stand-alone DI-NMS (sessd_rotate_weighted_nms).  boxes7 [N,7], boxes5 [N,5], scores [N], iou_preds [N] (rectified q) f32,
+    labels / dirs [N] i32, anchors [N,7] f32 (or None without centerness), n [1] i32 on the device.  Returns (boxes [pre_max,7],
+    scores, labels, dirs, keep = top-k position of each pick, selected = its input index, count [2] = emitted clusters, picks);
+    rows beyond count[0] are unspecified.  ws: a uint8 CUDA workspace of at least
+    sessd_rotate_weighted_nms_workspace_bytes(max_boxes, pre_max) bytes to reuse across calls (allocated per call when None)."""
+    dev = scores.device
+    for t, dt, name in ((boxes7, torch.float32, "boxes7"), (boxes5, torch.float32, "boxes5"), (scores, torch.float32, "scores"),
+                        (iou_preds, torch.float32, "iou_preds"), (labels, torch.int32, "labels"), (dirs, torch.int32, "dirs"),
+                        (n, torch.int32, "n")):
+        _cuda(t, dt, name)
+    if anchors is not None:
+        _cuda(anchors, torch.float32, "anchors")
+    p = int(pre_max)
+    out = dict(boxes=torch.empty((p, 7), dtype=torch.float32, device=dev), scores=torch.empty((p,), dtype=torch.float32, device=dev),
+               labels=torch.empty((p,), dtype=torch.int32, device=dev), dirs=torch.empty((p,), dtype=torch.int32, device=dev),
+               keep=torch.empty((p,), dtype=torch.int32, device=dev), selected=torch.empty((p,), dtype=torch.int32, device=dev),
+               count=torch.zeros((2,), dtype=torch.int32, device=dev))
+    if ws is None:
+        ws = torch.empty((max(lib.sessd_rotate_weighted_nms_workspace_bytes(int(max_boxes), p), 1),), dtype=torch.uint8, device=dev)
+    check(lib.sessd_rotate_weighted_nms(_p(boxes7), _p(boxes5), _p(scores), _p(iou_preds), _p(labels), _p(dirs), _p(anchors), _p(n),
+                                        int(max_boxes), p, C.byref(dinms_cfg), _p(out["boxes"]), _p(out["scores"]), _p(out["labels"]),
+                                        _p(out["dirs"]), _p(out["keep"]), _p(out["selected"]), _p(out["count"]), _p(ws), ws.numel(),
+                                        _st()), "sessd_rotate_weighted_nms")
+    return out
 
 
 # ------------------------------------------------------------------------------------------------ iou3d family
