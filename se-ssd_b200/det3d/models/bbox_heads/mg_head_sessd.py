@@ -6,6 +6,7 @@
 * ``predict``  : decode -> sigmoid -> threshold -> IoU-rectified score -> top-k -> rotated NMS -> frustum filter -> direction fix
   -> range mask in five kernels with no host round trip (sessd_postprocess); the reference syncs to the host twice per frame
   (box_torch_ops.py:536, mg_head_sessd.py:1026) and clips polygons on one CPU thread.
+* ``loss_ciassd``: the CIA-SSD pre-training loss (supervised terms only, smooth-L1 box loss in the sum and the gradient).
 * ``loss``     : the assembled SE-SSD head loss (supervised terms + ODIoU on the device, consistency loss against the teacher); value and
   gradient w.r.t. the packed head tensor.  In train mode the packed tensor carries a graph to the head's input and its convs' weights
   and biases (sessd_b200.bev_grad), so ``loss.backward()`` reaches the neck and the encoder below it."""
@@ -144,16 +145,17 @@ class MultiGroupHead(nn.Module):
             return (torch.as_tensor(example["ssl_labeled"]) == 1).to(device)
         return torch.ones(batch, dtype=torch.bool, device=device)
 
-    def _supervised_terms(self, example, preds_dict, keys, with_odiou):
+    def _supervised_terms(self, example, preds_dict, keys, with_odiou, with_loc=False):
         """One pass of the supervised terms over the supervised frames of ``preds_dict``: (values dict, loss scalar wired to the packed head
         tensor through ``_HeadLossFn``).  ``keys`` = the example entries to read (anchors, labels, reg_targets -- or their ``_raw`` twins for
-        the teacher, mg_head_sessd.py:810-830)."""
+        the teacher, mg_head_sessd.py:810-830).  ``with_loc``: the smooth-L1 box term is part of the loss and its gradient (CIA-SSD)."""
         k_anc, k_lab, k_reg = keys
         packed = preds_dict["_packed"]
         mask = self._supervision_mask(example, packed.shape[0], packed.device)
         sel = packed if bool(mask.all()) else packed[mask]
         ex = dict(anchors=[example[k_anc][0][mask.to(example[k_anc][0].device)]], labels=[example[k_lab][0]], reg_targets=[example[k_reg][0]])
-        out = self.loss_supervised(ex, [dict(_packed=sel.detach())], with_grad=True, with_odiou=with_odiou)
+        out = self.loss_supervised(ex, [dict(_packed=sel.detach())], with_grad=True, with_odiou=with_odiou,
+                                   w_loc=float(self.loss_reg._loss_weight) if with_loc else 0.0)
         b = sel.shape[0]
         labels = ex["labels"][0]
         head = sel.detach().reshape(b, -1, sel.shape[-1])
@@ -164,6 +166,8 @@ class MultiGroupHead(nn.Module):
         d = torch.cat([box[..., :-1] - tgt[..., :-1], torch.sin(box[..., -1:]) * torch.cos(tgt[..., -1:]) - torch.cos(box[..., -1:]) * torch.sin(tgt[..., -1:])], -1)
         elem = (self._smooth_l1(d, float(self.loss_reg._sigma)) * w[..., None]).sum((0, 1)) / b      # analysis only (:752)
         value = out["cls_loss_reduced"] + out["dir_loss_reduced"] + out["iou_pred_loss"]
+        if with_loc:
+            value = out["loc_loss_reduced"] + value
         if with_odiou:
             value = value + out["ious_loss"]
         grad = out["grad_head"]
@@ -199,6 +203,22 @@ class MultiGroupHead(nn.Module):
             for k, v in self.get_model_ema_loss(example, preds_ema).items():
                 merged[k] = [v[0]]
         return merged
+
+    def loss_ciassd(self, example, preds_dicts, **kwargs):
+        """The CIA-SSD head loss, the supervised loss SE-SSD's detector is pre-trained with (reference mg_head_ciassd.py:567-673),
+        single-task car head: ``loss`` = focal cls + smooth-L1 box loss on the sin-difference residuals (weight ``loss_bbox.loss_weight``)
+        + direction CE (weight ``loss_aux.loss_weight``) + IoU-prediction smooth-L1, with no ODIoU, consistency or teacher terms.  Value and
+        gradient w.r.t. the packed head tensor come from one device pass (csrc/headloss.cu, box-channel gradient included); ``loss`` hands
+        that gradient to ``preds_dicts[0]['_packed']``'s graph.  As in the reference, ``dir_loss_reduced`` is reported without its weight
+        while ``loss`` sums the weighted term.  Returns the reference's key -> [per-task value] dict."""
+        if len(preds_dicts) != 1:
+            raise NotImplementedError("the fused loss kernels are built for the single-task (car) head")
+        out, loss = self._supervised_terms(example, preds_dicts[0], ("anchors", "labels", "reg_targets"), with_odiou=False, with_loc=True)
+        cpu = lambda v: v.detach().cpu()                                                     # noqa: E731
+        return dict(loss=[loss], cls_loss_reduced=[cpu(out["cls_loss_reduced"])], loc_loss_reduced=[cpu(out["loc_loss_reduced"])],
+                    dir_loss_reduced=[cpu(out["dir_loss"])], iou_pred_loss=[cpu(out["iou_pred_loss"])], loc_loss_elem=[out["loc_loss_elem"]],
+                    cls_pos_loss=[cpu(out["cls_pos_loss"])], cls_neg_loss=[cpu(out["cls_neg_loss"])], num_pos=[out["num_pos"]],
+                    num_neg=[out["num_neg"]])
 
     def get_model_ema_loss(self, example, preds_dicts):
         """The teacher's supervised terms on the un-augmented targets (``labels_raw`` / ``reg_targets_raw`` / ``anchors_raw``), reported only
@@ -293,12 +313,13 @@ class MultiGroupHead(nn.Module):
             total = total + box_loss + score_loss + iou_loss
         return total / batch
 
-    def loss_supervised(self, example, preds_dicts, with_grad=True, with_odiou=False):
+    def loss_supervised(self, example, preds_dicts, with_grad=True, with_odiou=False, w_loc=0.0):
         """Supervised terms of ``loss`` (reference mg_head_sessd.py:706-768 without the teacher / ODIoU parts) for the
         single-task car head, value and gradient w.r.t. the fused head tensor in one device pass (csrc/headloss.cu).
         ``example``: ``anchors`` [[B,A,7]], ``labels`` [[B,A]], ``reg_targets`` [[B,A,7]] (device tensors, e.g. from
-        TargetAssigner.assign_batch_gpu).  Returns the reference's reduced values (loss_weight * batch total / batch_size) and the gradient
-        of ``cls_loss_reduced + dir_loss_reduced + iou_pred_loss`` (the reference's total does not include the smooth-L1 term)."""
+        TargetAssigner.assign_batch_gpu).  Returns the reference's reduced values (loss_weight * batch total / batch_size), ``dir_loss``
+        (the direction term without its weight) and the gradient of ``cls_loss_reduced + dir_loss_reduced + iou_pred_loss`` (the SE-SSD
+        total does not include the smooth-L1 term) plus ``w_loc`` times the smooth-L1 term's batch mean (CIA-SSD passes its loss weight)."""
         from sessd_b200 import ops
         packed = preds_dicts[0]["_packed"]
         b = packed.shape[0]
@@ -309,13 +330,14 @@ class MultiGroupHead(nn.Module):
         w_cls, w_dir = float(self.loss_cls._loss_weight), float(self.loss_aux._loss_weight)
         losses, grad = ops.head_loss(head, anchors, labels, reg_targets, alpha=float(self.loss_cls._alpha), sigma=float(self.loss_reg._sigma),
                                      dir_offset=float(self.direction_offset), pos_cls_weight=float(self.loss_norm["pos_cls_weight"]),
-                                     neg_cls_weight=float(self.loss_norm["neg_cls_weight"]), w_cls=w_cls, w_loc=0.0, w_dir=w_dir,
+                                     neg_cls_weight=float(self.loss_norm["neg_cls_weight"]), w_cls=w_cls, w_loc=float(w_loc), w_dir=w_dir,
                                      w_iou=1.0, with_grad=with_grad)
         tot = losses.sum(0) / b
         ious_loss = None
         if with_odiou:          # ODIoU box loss (odious.py:845-900): 2.0 * batch total / batch_size, gradient added to the box channels
             ious_loss = 2.0 * ops.odiou_loss(head, anchors, labels, reg_targets, losses, grad, w_odiou=2.0).sum() / b
         return dict(cls_loss_reduced=w_cls * tot[0], loc_loss_reduced=float(self.loss_reg._loss_weight) * tot[1], dir_loss_reduced=w_dir * tot[2],
+                    dir_loss=tot[2],
                     cls_pos_loss=tot[3] / float(self.loss_norm["pos_cls_weight"]), cls_neg_loss=tot[4] / float(self.loss_norm["neg_cls_weight"]),
                     iou_pred_loss=tot[5], ious_loss=ious_loss, num_pos=losses[0, 6], num_neg=losses[0, 7], grad_head=None if grad is None else grad.view_as(packed))
 

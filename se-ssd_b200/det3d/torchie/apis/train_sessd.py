@@ -28,6 +28,18 @@ def _create_learning_rate_scheduler(optimizer, lr_config, total_steps):
     return lsf.OneCycle(optimizer, total_steps, lr_config["lr_max"], list(lr_config["moms"]), lr_config["div_factor"], lr_config["pct_start"])
 
 
+def build_loaders(dataset, cfg, twin=True):
+    """the device loaders of ``dataset`` = [train, (unlabelled,) val] without the unlabelled one: ``cfg.data.samples_per_gpu`` frames per
+    batch, random streams from ``cfg.seed`` (0 when unset); ``twin`` as kitti_loader.DeviceLoader takes it"""
+    from det3d.datasets import build_dataloader
+    datasets = list(dataset) if isinstance(dataset, (list, tuple)) else [dataset]
+    if len(datasets) == 3:
+        datasets = [datasets[0], datasets[2]]
+    seed = cfg.get("seed") or 0
+    return [build_dataloader(ds, cfg.data.samples_per_gpu, cfg.data.workers_per_gpu, dist=False, cfg=cfg, seed=seed, twin=twin)
+            for ds in datasets]
+
+
 def train_detector(model, dataset, cfg, distributed=False, validate=False, logger=None):
     """Train ``model`` on ``dataset`` = [train, (unlabelled,) val] as the reference's train_detector does, single-GPU, and return the
     final validation's results dict (None without a val phase).
@@ -36,17 +48,10 @@ def train_detector(model, dataset, cfg, distributed=False, validate=False, logge
     ``cfg.data.samples_per_gpu`` frames and draws from ``cfg.seed`` (0 when unset).  With ``my_paras.enable_ssl`` the reference also
     builds an unlabelled dataset but never draws from it (its merge is commented out, trainer_sessd.py:334-339): it is accepted and not
     iterated here."""
-    from det3d.datasets import build_dataloader
-
     from ..trainer.trainer_sessd import Trainer, batch_processor_inline
     if distributed:
         raise NotImplementedError("distributed training is not implemented")
-    datasets = list(dataset) if isinstance(dataset, (list, tuple)) else [dataset]
-    if len(datasets) == 3:
-        datasets = [datasets[0], datasets[2]]
-    seed = cfg.get("seed") or 0
-    loaders = [build_dataloader(ds, cfg.data.samples_per_gpu, cfg.data.workers_per_gpu, dist=False, cfg=cfg, seed=seed)
-               for ds in datasets]
+    loaders = build_loaders(dataset, cfg)
     model = model.cuda()
     model_ema = copy.deepcopy(model)
     for p in model_ema.parameters():

@@ -201,13 +201,19 @@ class Trainer:
         unlabelled batches is commented out."""
         self.model_ema.train()
         self.model.train()
+        consistency_weight = 1.0 * sigmoid_rampup(self.epoch, self._max_epochs)
+        self._train_epoch(data_loader, lambda batch: self.batch_processor(self.model, self.model_ema, batch, consistency_weight,
+                                                                          train_mode=True))
+
+    def _train_epoch(self, data_loader, process):
+        """the epoch loop: per batch the schedule step, ``process(batch)`` (the batch processor's outputs), the optimiser step, the log;
+        then the checkpoint"""
         self.mode, self.data_loader = "train", data_loader
         self.length = len(data_loader)
         self._max_iters = self._max_epochs * self.length
         base_step = self.epoch * self.length
         if hasattr(data_loader, "set_epoch"):
             data_loader.set_epoch(self.epoch)
-        consistency_weight = 1.0 * sigmoid_rampup(self.epoch, self._max_epochs)
         log = _LogBuffer()
         interval = self.log_config["interval"] if self.log_config else 0
         t_end = time.time()
@@ -217,7 +223,7 @@ class Trainer:
             if self.lr_scheduler is not None:
                 self.lr_scheduler.step(global_step)
             self._inner_iter = i
-            outputs = self.batch_processor(self.model, self.model_ema, data_batch, consistency_weight, train_mode=True)
+            outputs = process(data_batch)
             if not isinstance(outputs, dict):
                 raise TypeError("batch_processor() must return a dict")
             self.outputs = outputs
@@ -273,29 +279,34 @@ class Trainer:
                     if mode == "val":
                         results = self.val(data_loaders[-1])
                     else:
-                        self.train(data_loaders[0], None, self.epoch)
+                        self.train(data_loaders[0], epoch=self.epoch)
         return results
 
     # ------------------------------------------------------------------------------------------------ checkpoints
+    def _checkpointed(self):
+        """(model, file-name suffix) of every model a checkpoint holds: the student, then the teacher"""
+        return ((self.model, ""), (self.model_ema, "_ema"))
+
     def save_checkpoint(self, out_dir, filename_tmpl="epoch_{}.pth", save_optimizer=True, meta=None):
         """``epoch_{n}.pth`` (student) and ``epoch_{n}_ema.pth`` (teacher), both with the optimiser state and meta = {epoch, iter} plus
         ``meta``; relative symlinks latest.pth / latest_ema.pth (trainer_sessd.py:228-248)"""
         from .checkpoint import save_checkpoint
         meta = dict(meta or {})
         meta.update(epoch=self.epoch + 1, iter=self.iter)
-        filename = filename_tmpl.format(self.epoch + 1)
+        stem = osp.splitext(filename_tmpl.format(self.epoch + 1))[0]
         optimizer = self.optimizer if save_optimizer else None
-        filename_ema = osp.splitext(filename)[0] + "_ema.pth"
-        for model, name, link in ((self.model, filename, "latest.pth"), (self.model_ema, filename_ema, "latest_ema.pth")):
+        for model, sfx in self._checkpointed():
+            name = stem + sfx + ".pth"
             save_checkpoint(model, osp.join(out_dir, name), optimizer=optimizer, meta=meta)
-            _symlink(name, osp.join(out_dir, link))
+            _symlink(name, osp.join(out_dir, "latest" + sfx + ".pth"))
 
     def load_checkpoint(self, filename, map_location="cpu", strict=False):
         """the student from ``filename``, the teacher from its ``_ema`` twin, the optimiser state"""
         from .checkpoint import load_checkpoint
         self.logger.info("load checkpoint from %s", filename)
         ckpt = load_checkpoint(self.model, filename, map_location, strict, self.logger)
-        load_checkpoint(self.model_ema, osp.splitext(filename)[0] + "_ema.pth", map_location, strict, self.logger)
+        for model, sfx in self._checkpointed()[1:]:
+            load_checkpoint(model, osp.splitext(filename)[0] + sfx + ".pth", map_location, strict, self.logger)
         self.optimizer.load_state_dict(ckpt["optimizer"])
         return ckpt
 

@@ -190,7 +190,7 @@ def _host_inputs(cfg, frame_sizes, gt_boxes, gt_names, draws, labeled):
     return (None, off), (boxes, num_gt, valid, target, loc, rot, glob, perm, lab), ns
 
 
-def augment_batch(cfg, clouds, gt_boxes, gt_names, draws, labeled=None, device="cuda"):
+def augment_batch(cfg, clouds, gt_boxes, gt_names, draws, labeled=None, device="cuda", twin=True):
     """Augment a batch of frames on the device.  clouds: per frame [N, 4] f32; gt_boxes: per frame [M, 7] (x y z w l h r); gt_names: per
     frame [M] class names (DontCare / ignore already dropped, as Preprocess does first); draws: draw_augmentation's output for
     (len(cloud), len(boxes), labeled) of every frame; labeled: per frame, None = all labelled.
@@ -199,34 +199,37 @@ def augment_batch(cfg, clouds, gt_boxes, gt_names, draws, labeled=None, device="
     (the teacher's twin: noised, unshuffled; an unlabelled frame's rows are its input), ``frame_off`` [B+1], ``gt_boxes`` / ``num_gt`` (the student's boxes after the range
     filter) and ``gt_boxes_raw`` / ``num_gt_raw`` (the teacher's), both padded [B, max_gt, 7] with limit_period angles -- the layout
     sessd_assign_targets reads --, ``selected`` [B, max_gt] (the try each box took, -1 none); and ``transformation`` (host list of dicts).
+    twin=False (labelled frames): no teacher copy of the points is written and ``points_raw`` is None.
     Launches on the current stream and never waits on the device."""
     (_, off), rest, ns = _host_inputs(cfg, [len(c) for c in clouds], gt_boxes, gt_names, draws, labeled)
     pts = np.concatenate([np.asarray(c, np.float32).reshape(-1, 4) for c in clouds] + [np.zeros((0, 4), np.float32)])
     buf, layout = _pack([pts, off] + list(rest))
     dev = torch.from_numpy(buf).pin_memory().to(device, non_blocking=True)
     d = _unpack(dev, layout)
-    return _augment_device(cfg, d[0], d[1], ns, d[2:], draws, labeled)
+    return _augment_device(cfg, d[0], d[1], ns, d[2:], draws, labeled, twin=twin)
 
 
-def augment_resident(cfg, d_points, d_frame_off, frame_sizes, gt_boxes, gt_names, draws, device="cuda", student_boxes=False):
+def augment_resident(cfg, d_points, d_frame_off, frame_sizes, gt_boxes, gt_names, draws, device="cuda", student_boxes=False, twin=True):
     """augment_batch on points already on the device (labelled frames): d_points [P, 4] f32 (16-byte aligned rows) with d_frame_off
     [B+1] i32, frame_sizes the host's copy of the frame sizes.  Only the boxes and the draws are uploaded (one copy).  student_boxes:
-    also return ``sada_boxes`` [B, max_gt, 7], each frame's class-valid boxes after the global stages (sessd_augment_boxes)."""
+    also return ``sada_boxes`` [B, max_gt, 7], each frame's class-valid boxes after the global stages (sessd_augment_boxes).
+    twin=False: no teacher copy of the points is written (``points_raw`` is None)."""
     _, rest, ns = _host_inputs(cfg, frame_sizes, gt_boxes, gt_names, draws, None)
     buf, layout = _pack(list(rest))
     dev = torch.from_numpy(buf).pin_memory().to(device, non_blocking=True)
-    return _augment_device(cfg, d_points, d_frame_off, ns, _unpack(dev, layout), draws, None, student_boxes)
+    return _augment_device(cfg, d_points, d_frame_off, ns, _unpack(dev, layout), draws, None, student_boxes, twin)
 
 
-def _augment_device(cfg, d_pts, d_off, ns, rest, draws, labeled, student_boxes=False):
+def _augment_device(cfg, d_pts, d_off, ns, rest, draws, labeled, student_boxes=False, twin=True):
     d_boxes, d_num, d_valid, d_target, d_loc, d_rot, d_glob, d_perm, d_lab = rest
     B = len(ns)
     labeled = [True] * B if labeled is None else [bool(v) for v in labeled]
     ctx = cfg.data_aug_with_context
     sel = ops.noise_per_box(d_boxes, d_num, d_valid, d_loc, d_rot, ctx)
-    raw = None if all(labeled) else d_pts.clone()          # an unlabelled frame has no twin in the reference: its rows keep the input
+    # an unlabelled frame has no twin in the reference: its rows keep the input
+    raw = None if not twin or all(labeled) else d_pts.clone()
     raw, out = ops.augment_points(d_pts, d_off, max(ns + [0]), d_boxes, d_num, d_valid, d_loc, d_rot, sel, d_glob, d_perm, d_lab, ctx,
-                                  points_raw=raw)
+                                  points_raw=raw, with_raw=twin)
     boxes = ops.augment_boxes(d_boxes, d_num, d_valid, d_target, d_loc, d_rot, sel, d_glob, cfg.range_bev, global_boxes=student_boxes)
     boxes_raw, num_raw, boxes_out, num_out = boxes[:4]
     res = dict(points=out, points_raw=raw, frame_off=d_off, gt_boxes=boxes_out, num_gt=num_out, gt_boxes_raw=boxes_raw,
@@ -270,9 +273,9 @@ def voxel_example(st, vb, batch, total, sfx=""):
 
 
 class PendingBatch:
-    """A training batch whose device work has been launched (augmentation, both voxelisations, both target assignments) and whose
-    collated dict is not formed yet.  ``example()`` forms it: the one device-to-host read of the batch (the two branches' voxel totals,
-    which size the exact-count voxel tensors the model reads)."""
+    """A training batch whose device work has been launched (augmentation, both voxelisations, both target assignments; the student's
+    only when ``vox_raw`` is None) and whose collated dict is not formed yet.  ``example()`` forms it: the one device-to-host read of the
+    batch (the branches' voxel totals, which size the exact-count voxel tensors the model reads)."""
 
     def __init__(self, st, aug, vox, vox_raw, asg, asg_raw, batch, frame_off, num_points_total):
         self._st, self._aug, self._vox, self._vox_raw, self._asg, self._asg_raw = st, aug, vox, vox_raw, asg, asg_raw
@@ -280,12 +283,13 @@ class PendingBatch:
 
     def example(self):
         B = self._batch
-        totals = torch.stack([self._vox.num_voxels[B], self._vox_raw.num_voxels[B]]).cpu().tolist()      # the one read-back
+        branches = [("", self._vox, self._asg)] + ([("_raw", self._vox_raw, self._asg_raw)] if self._vox_raw is not None else [])
+        totals = torch.stack([vb.num_voxels[B] for _, vb, _ in branches]).cpu().tolist()                 # the one read-back
         dev = self._off.device
         counts = self._off[1:] - self._off[:-1]
         bidx = torch.repeat_interleave(torch.arange(B, dtype=torch.float32, device=dev), counts, output_size=self._total)
         ex = dict(metadata=[dict(token=i) for i in range(B)], points=torch.cat([bidx[:, None], self._aug["points"]], 1))
-        for sfx, vb, ab, n in (("", self._vox, self._asg, totals[0]), ("_raw", self._vox_raw, self._asg_raw, totals[1])):
+        for (sfx, vb, ab), n in zip(branches, totals):
             ex.update(voxel_example(self._st, vb, B, n, sfx))
             ex["labels" + sfx] = [ab.labels]
             ex["reg_targets" + sfx] = [ab.bbox_targets]
@@ -380,8 +384,8 @@ class _SadaFrames:
     draws, at most one read-back of the swap counts), one read-back of its new size, then its shuffle draw.  ``assemble`` joins the
     frames into augment_batch's layout and shuffles them with one gather."""
 
-    def __init__(self, cfg, sa_da, rs, device):
-        self.cfg, self.sa_da, self.rs, self.device = cfg, sa_da, rs, device
+    def __init__(self, cfg, sa_da, rs, device, twin=True):
+        self.cfg, self.sa_da, self.rs, self.device, self.twin = cfg, sa_da, rs, device, twin
         self.frames = []
 
     def __call__(self, f, d_points, n, boxes, names):
@@ -390,7 +394,7 @@ class _SadaFrames:
         loc, rot, flip, rotation, scale = _labeled_draws(rs, len(boxes), cfg)
         fd = FrameDraws(loc, rot, flip, rotation, scale, np.arange(n))
         d_off = torch.tensor([0, n], dtype=torch.int32).to(self.device)
-        aug = augment_resident(cfg, d_points, d_off, [n], [boxes], [names], Draws([fd]), self.device, student_boxes=True)
+        aug = augment_resident(cfg, d_points, d_off, [n], [boxes], [names], Draws([fd]), self.device, student_boxes=True, twin=self.twin)
         k = sum(1 for nm in names if nm in cfg.class_names)
         out, num = sada.sada_frame(aug["points"], aug["sada_boxes"][0], k, rs, self.sa_da)
         size = int(num.item())                                  # the read-back: the shuffle is sized by the frame after SA-DA
@@ -400,9 +404,9 @@ class _SadaFrames:
 
     def assemble(self):
         B = len(self.frames)
-        dev = self.frames[0][1]["points_raw"].device
+        dev = self.frames[0][1]["frame_off"].device
         sizes = [len(o) for o, _, _ in self.frames]
-        raw_sizes = [len(a["points_raw"]) for _, a, _ in self.frames]
+        raw_sizes = [len(a["points_raw"]) if self.twin else 0 for _, a, _ in self.frames]
         off = np.zeros(B + 1, np.int32); off[1:] = np.cumsum(sizes)
         raw_off = np.zeros(B + 1, np.int32); raw_off[1:] = np.cumsum(raw_sizes)
         perm = np.concatenate([fd.perm for _, _, fd in self.frames] + [np.zeros(0, np.int64)]).astype(np.int32)
@@ -411,7 +415,7 @@ class _SadaFrames:
         pts = torch.cat([o for o, _, _ in self.frames] + [torch.empty((0, 4), dtype=torch.float32, device=dev)])
         points = ops.sada_shuffle(pts, d_off, max(sizes + [0]), d_perm) if len(pts) else pts
         M = max([1] + [a["gt_boxes"].shape[1] for _, a, _ in self.frames])
-        res = dict(points=points, points_raw=torch.cat([a["points_raw"] for _, a, _ in self.frames]), frame_off=d_off,
+        res = dict(points=points, points_raw=torch.cat([a["points_raw"] for _, a, _ in self.frames]) if self.twin else None, frame_off=d_off,
                    frame_off_raw=d_raw_off, transformation=Draws([fd for _, _, fd in self.frames]).transformation())
         for key, num_key in (("gt_boxes", "num_gt"), ("gt_boxes_raw", "num_gt_raw")):
             bx = torch.zeros((B, M, 7), dtype=torch.float32, device=dev)
@@ -426,9 +430,13 @@ class _SadaFrames:
         return res, int(off[-1]), int(raw_off[-1])
 
 
-def launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda", db_sampler=None, sa_da=None):
+def launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda", db_sampler=None, sa_da=None, twin=True):
     """Everything of build_train_batch that runs on the device: the draws (host), augment_batch, the voxeliser on the student's points
     and on the twin, the target assigner on both box sets.  Returns a PendingBatch.
+
+    twin=False builds the student's branch only (a single-model batch, as CIA-SSD pre-training reads): no teacher copy of the points,
+    no second voxelisation or assignment, no ``*_raw`` keys.  The draws and the RandomState stream are those of twin=True, so every
+    student key is bit-identical to the twin batch of the same stream.
 
     Without db_sampler nothing waits on the device.  With db_sampler (a det3d.core.sampler DataBaseSamplerV2), GT-database sampling
     runs first (gtaug_batch): it waits once on the pasted frame offsets before drawing the augmentation, because the shuffle is sized
@@ -444,7 +452,7 @@ def launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device
     st = _static(cfg, device)
     B = len(clouds)
     if sa_da is not None:
-        frames = _SadaFrames(st["aug"], sa_da, rs, device)
+        frames = _SadaFrames(st["aug"], sa_da, rs, device, twin)
         if db_sampler is None:
             pts = np.concatenate([np.asarray(c, np.float32).reshape(-1, 4) for c in clouds] + [np.zeros((0, 4), np.float32)])
             d_pts = torch.from_numpy(pts).pin_memory().to(device, non_blocking=True)
@@ -457,24 +465,27 @@ def launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device
         aug, total, total_raw = frames.assemble()
     elif db_sampler is None:
         draws = draw_augmentation(rs, [(len(c), len(b), True) for c, b in zip(clouds, gt_boxes)], st["aug"])
-        aug = augment_batch(st["aug"], clouds, gt_boxes, gt_names, draws, device=device)
+        aug = augment_batch(st["aug"], clouds, gt_boxes, gt_names, draws, device=device, twin=twin)
         total = total_raw = int(sum(len(c) for c in clouds))
     else:
         d_points, d_off, sizes, boxes, names, draws, _ = gtaug_batch(st["aug"], clouds, gt_boxes, gt_names, rs, db_sampler, device)
-        aug = augment_resident(st["aug"], d_points, d_off, sizes, boxes, names, draws, device)
+        aug = augment_resident(st["aug"], d_points, d_off, sizes, boxes, names, draws, device, twin=twin)
         total = total_raw = int(sum(sizes))
-    vox = ops.VoxelBuffers(st["vcfg"], B, max(total, 1), device)
-    vox_raw = ops.VoxelBuffers(st["vcfg"], B, max(total_raw, 1), device)
-    ops.voxelize(aug["points"], aug["frame_off"], vox)
-    ops.voxelize(aug["points_raw"], aug.get("frame_off_raw", aug["frame_off"]), vox_raw)
     A = st["anchors"].shape[0]
-    asg, asg_raw = (ops.AssignBuffers(A, B, aug["gt_boxes"].shape[1], device) for _ in range(2))
+    vox = ops.VoxelBuffers(st["vcfg"], B, max(total, 1), device)
+    ops.voxelize(aug["points"], aug["frame_off"], vox)
+    asg = ops.AssignBuffers(A, B, aug["gt_boxes"].shape[1], device)
     ops.assign_targets(st["anchors"], aug["gt_boxes"], aug["num_gt"], asg, *st["thr"])
-    ops.assign_targets(st["anchors"], aug["gt_boxes_raw"], aug["num_gt_raw"], asg_raw, *st["thr"])
+    vox_raw = asg_raw = None
+    if twin:
+        vox_raw = ops.VoxelBuffers(st["vcfg"], B, max(total_raw, 1), device)
+        ops.voxelize(aug["points_raw"], aug.get("frame_off_raw", aug["frame_off"]), vox_raw)
+        asg_raw = ops.AssignBuffers(A, B, aug["gt_boxes"].shape[1], device)
+        ops.assign_targets(st["anchors"], aug["gt_boxes_raw"], aug["num_gt_raw"], asg_raw, *st["thr"])
     return PendingBatch(st, aug, vox, vox_raw, asg, asg_raw, B, aug["frame_off"], total)
 
 
-def build_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda", db_sampler=None, sa_da=None):
+def build_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device="cuda", db_sampler=None, sa_da=None, twin=True):
     """A collated SE-SSD training batch with real augmentation: the ``example`` dict batch_processor_inline takes, with the keys of
     ``synth.train_batch`` (voxels, coordinates with a batch column, num_points, num_voxels, shape, anchors, labels, reg_targets, their
     ``_raw`` twins for the teacher, points with a batch column, metadata, transformation), all tensors on the device.
@@ -490,5 +501,7 @@ def build_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled=None, device=
 
     Without db_sampler and sa_da the device work is launched without waiting (launch_train_batch); with a db_sampler, GT-AUG reads the
     pasted frame sizes back once before drawing; with sa_da, each frame waits on the device once or twice (see launch_train_batch).
-    Forming the dict then reads the two branches' voxel totals back once, because the model consumes exact-count voxel tensors."""
-    return launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled, device, db_sampler, sa_da).example()
+    Forming the dict then reads the two branches' voxel totals back once, because the model consumes exact-count voxel tensors.
+
+    twin=False: the student's branch only, without the ``*_raw`` keys (see launch_train_batch)."""
+    return launch_train_batch(cfg, clouds, gt_boxes, gt_names, rs, labeled, device, db_sampler, sa_da, twin).example()

@@ -39,10 +39,11 @@ def restart_sampler(db_sampler, rs):
 class DeviceLoader:
     """Iterable of ``example`` dicts whose tensors are on ``device``; ``len()`` batches per epoch (the last one partial).  The dataset's
     mode (its pipeline's Preprocess mode) chooses the train or the val / test batch.  Train mode shuffles the frames; val / test mode keeps the info order (predictions are keyed by token, so the order does not change a result).
-    Each ``iter()`` runs epoch ``self.epoch`` and advances it; ``set_epoch`` chooses the epoch, as a resumed run does."""
+    Each ``iter()`` runs epoch ``self.epoch`` and advances it; ``set_epoch`` chooses the epoch, as a resumed run does.
+    twin=False: training batches carry the student's branch only (no ``*_raw`` keys), as single-model (CIA-SSD) training reads them."""
 
-    def __init__(self, dataset, batch_size, cfg, seed=0, device=None):
-        self.dataset, self.batch_size, self.cfg, self.seed = dataset, int(batch_size), cfg, int(seed)
+    def __init__(self, dataset, batch_size, cfg, seed=0, device=None, twin=True):
+        self.dataset, self.batch_size, self.cfg, self.seed, self.twin = dataset, int(batch_size), cfg, int(seed), bool(twin)
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self.train = dataset.mode == "train"
         self.epoch = 0
@@ -85,7 +86,7 @@ class DeviceLoader:
         lidar = [f["lidar"] for f in frames]
         pending = augment.launch_train_batch(self.cfg, [l["points"] for l in lidar], [l["gt_boxes"] for l in lidar],
                                              [l["gt_names"] for l in lidar], rs, device=self.device, db_sampler=self.db_sampler,
-                                             sa_da=SadaConfig())
+                                             sa_da=SadaConfig(), twin=self.twin)
         ex = pending.example()
         ex["metadata"] = [f["metadata"] for f in frames]
         return ex
@@ -109,12 +110,12 @@ class DeviceLoader:
         return ex
 
 
-def build_dataloader(dataset, batch_size, workers_per_gpu, num_gpus=1, dist=False, cfg=None, seed=0, **kwargs):
+def build_dataloader(dataset, batch_size, workers_per_gpu, num_gpus=1, dist=False, cfg=None, seed=0, twin=True, **kwargs):
     """The reference's loader entry point.  ``cfg`` (the loaded config) carries the augmentation, voxeliser, assigner and db_sampler
     values; ``seed`` the random streams.  ``workers_per_gpu`` is accepted for the reference's signature: one reader thread reads ahead,
-    the rest of the work is on the device.  Multi-GPU loading (dist=True) is not implemented."""
+    the rest of the work is on the device.  ``twin``: see DeviceLoader.  Multi-GPU loading (dist=True) is not implemented."""
     if dist or num_gpus != 1:
         raise NotImplementedError("distributed / multi-GPU loading is not implemented")
     if cfg is None:
         raise ValueError("build_dataloader needs the loaded config (cfg=...): the batches are built from its stage values")
-    return DeviceLoader(dataset, batch_size, cfg, seed)
+    return DeviceLoader(dataset, batch_size, cfg, seed, twin=twin)

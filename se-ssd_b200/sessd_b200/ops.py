@@ -736,10 +736,11 @@ def noise_per_box(gt_boxes, num_gt, valid, loc_noise, rot_noise, context=-1.0, s
 
 
 def augment_points(points, frame_off, max_frame_points, gt_boxes, num_gt, valid, loc_noise, rot_noise, selected, glob, perm, labeled=None,
-                   context=-1.0, points_raw=None, points_out=None):
+                   context=-1.0, points_raw=None, points_out=None, with_raw=True):
     """per-object transform, raw twin, global flip / rotation / scaling and shuffle of a batch of frames (sessd_augment_points).
     points [P,4] f32 (16-byte aligned rows), frame_off [B+1] i32, glob [B,5] f32 (cos, sin, scale, flip, angle), perm [P] i32 holding a
-    permutation of each frame's rows, labeled [B] u8 or None.  Returns (points_raw, points_out) [P,4] f32."""
+    permutation of each frame's rows, labeled [B] u8 or None.  Returns (points_raw, points_out) [P,4] f32; with_raw=False writes no twin
+    and returns (None, points_out)."""
     B, M, T = _aug_inputs(gt_boxes, num_gt, valid, loc_noise, rot_noise, selected)
     _cuda(points, torch.float32, "points"); _cuda(frame_off, torch.int32, "frame_off"); _cuda(glob, torch.float32, "glob")
     _cuda(perm, torch.int32, "perm")
@@ -749,15 +750,18 @@ def augment_points(points, frame_off, max_frame_points, gt_boxes, num_gt, valid,
             raise ValueError("labeled must be [B]")
     if points.dim() != 2 or points.shape[1] != 4 or frame_off.numel() != B + 1 or perm.numel() != points.shape[0] or tuple(glob.shape) != (B, 5):
         raise ValueError("augment_points: shape mismatch")
-    if points_raw is None:
+    if not with_raw:
+        points_raw = None
+    elif points_raw is None:
         points_raw = torch.empty_like(points)
     if points_out is None:
         points_out = torch.empty_like(points)
-    for name, t in (("points_raw", points_raw), ("points_out", points_out)):
+    written = (("points_raw", points_raw), ("points_out", points_out)) if with_raw else (("points_out", points_out),)
+    for name, t in written:
         _cuda(t, torch.float32, name)
         if t.shape != points.shape:
             raise ValueError("%s must be shaped like points" % name)
-    if any(t.data_ptr() % 16 for t in (points, points_raw, points_out)):
+    if any(t.data_ptr() % 16 for t in (points, points_out) + ((points_raw,) if with_raw else ())):
         raise ValueError("augment_points: point rows are read and written as float4 and must be 16-byte aligned")
     check(lib.sessd_augment_points(_p(points), _p(frame_off), int(B), int(max_frame_points), _p(gt_boxes), _p(num_gt), _p(valid), int(M),
                                    _p(loc_noise), _p(rot_noise), int(T), _p(selected), float(context), _p(glob), _p(perm), _p(labeled),
