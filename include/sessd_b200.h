@@ -73,7 +73,6 @@ int sessd_voxelize_host(const float *h_points, int num_points, const sessd_voxel
  * S3: rulebook ("indice pairs") construction.  Replaces spconv 1.x's indice-pair builders that
  * det3d/models/backbones/scn.py:106-149,182-183 trigger (4 SubM keys + 4 strided convs per forward).
  * The rulebook is kept output-major: nbr[o, k] = input row feeding output o through kernel offset k, or -1.
- * The canonical spconv form (per offset: pairs sorted by output index) is sessd_rulebook_pairs().
  *
  * An "index" is either a hash table over given coordinates (any row order: the voxeliser's first-appearance
  * order at level 0) or a rank bitmap (rows in ascending linear index: what strided convs emit).
@@ -110,10 +109,6 @@ int sessd_strided_rulebook(const int *d_in_coors, const int *d_n_in, int max_in,
  * (input row << 7) | tile row, ascending tile row (deterministic).  d_tiles: uint32 [ceil(max_out / 128)][stride].  kvol <= 27. */
 int sessd_tile_list_stride(int kvol);
 int sessd_rulebook_tile_lists(const int *d_nbr, int kvol, const int *d_n_out, int max_out, void *d_tiles, void *stream);
-/* canonical spconv-style pairs from a nbr table: pairs_in/out [kvol, max_rows], pair_num [kvol] */
-size_t sessd_rulebook_pairs_workspace_bytes(int max_rows, int kvol);
-int sessd_rulebook_pairs(const int *d_nbr, const int *d_n_out, int max_rows, int kvol, int *d_pairs_in,
-                         int *d_pairs_out, int *d_pair_num, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * S4/S5: sparse convolution (gather -> GEMM -> fused BN(eval)+ReLU epilogue, output-stationary) and dense().

@@ -5,8 +5,8 @@
 // lists with global atomic counters (nondeterministic order).  Here the rulebook is OUTPUT-MAJOR and deterministic:
 //     nbr[o, k] = row of the input voxel at  pos_o * stride - pad + k   (or -1),
 // which is exactly what the output-stationary gather-GEMM in spconv.cu consumes (no scatter-add, no atomics on
-// features), and from which the canonical spconv form (per offset, pairs sorted by output index) follows by an
-// ordered compaction (sessd_rulebook_pairs: warp ballots + shared-memory histogram).
+// features), and which the tensor-core conv (spconv_cg.cu) reads regrouped into per-tile pair lists
+// (sessd_rulebook_tile_lists, at the end of this file).
 //
 // Two coordinate indices:
 //   * hash   : 64-bit open addressing over linear cell index -> row, for coordinates given in arbitrary order
@@ -222,72 +222,6 @@ __global__ void __launch_bounds__(256) enumerate_kernel(uint2 *__restrict__ bitm
     }
 }
 
-// canonical pairs: per kernel offset, (in, out) sorted by out.  Pass 1 histogram, pass 2 ordered write.
-constexpr int kPairRows = 256;
-
-__global__ void __launch_bounds__(kPairRows) pair_count_kernel(const int *__restrict__ nbr, const int *__restrict__ d_n, int max_rows,
-                                                               int kvol, int *__restrict__ block_counts /*[nblocks, kvol]*/) {
-    extern __shared__ int s_hist[];   // [kvol]
-    const int n = min(*d_n, max_rows);
-    const int base = blockIdx.x * kPairRows;
-    if (base >= n) return;
-    for (int k = threadIdx.x; k < kvol; k += blockDim.x) s_hist[k] = 0;
-    __syncthreads();
-    const int o = base + threadIdx.x;
-    const int lane = threadIdx.x & 31;
-    for (int k = 0; k < kvol; ++k) {
-        const bool f = (o < n) && (nbr[(size_t)o * kvol + k] >= 0);
-        const unsigned int bal = __ballot_sync(0xffffffffu, f);
-        if (lane == 0 && bal) atomicAdd(&s_hist[k], __popc(bal));
-    }
-    __syncthreads();
-    for (int k = threadIdx.x; k < kvol; k += blockDim.x) block_counts[(size_t)blockIdx.x * kvol + k] = s_hist[k];
-}
-
-__global__ void __launch_bounds__(32) pair_offsets_kernel(const int *__restrict__ d_n, int max_rows, int kvol,
-                                                          int *__restrict__ block_counts, int *__restrict__ pair_num) {
-    // one warp per kernel offset: exclusive scan of the per-block counts (serial over block chunks of 32)
-    const int n = min(*d_n, max_rows);
-    const int nblk = (n + kPairRows - 1) / kPairRows;
-    const int k = blockIdx.x;
-    const int lane = threadIdx.x;
-    int carry = 0;
-    for (int b0 = 0; b0 < nblk; b0 += 32) {
-        const int b = b0 + lane;
-        const int v = (b < nblk) ? block_counts[(size_t)b * kvol + k] : 0;
-        const int incl = warp_incl_scan(v, lane);
-        if (b < nblk) block_counts[(size_t)b * kvol + k] = carry + incl - v;
-        carry += __shfl_sync(0xffffffffu, incl, 31);
-    }
-    if (lane == 0) pair_num[k] = carry;
-}
-
-__global__ void __launch_bounds__(kPairRows) pair_write_kernel(const int *__restrict__ nbr, const int *__restrict__ d_n, int max_rows,
-                                                               int kvol, const int *__restrict__ block_offsets,
-                                                               int *__restrict__ pairs_in, int *__restrict__ pairs_out) {
-    __shared__ int s_warp[kPairRows / 32];
-    const int n = min(*d_n, max_rows);
-    const int base = blockIdx.x * kPairRows;
-    if (base >= n) return;
-    const int o = base + threadIdx.x;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int k = 0; k < kvol; ++k) {
-        const int src = (o < n) ? nbr[(size_t)o * kvol + k] : -1;
-        const bool f = src >= 0;
-        const unsigned int bal = __ballot_sync(0xffffffffu, f);
-        if (lane == 0) s_warp[warp] = __popc(bal);
-        __syncthreads();
-        int woff = 0;
-        for (int w2 = 0; w2 < warp; ++w2) woff += s_warp[w2];
-        if (f) {
-            const int pos = block_offsets[(size_t)blockIdx.x * kvol + k] + woff + __popc(bal & ((1u << lane) - 1u));
-            pairs_in[(size_t)k * max_rows + pos] = src;
-            pairs_out[(size_t)k * max_rows + pos] = o;
-        }
-        __syncthreads();
-    }
-}
-
 static GridDims to_dims(sessd_grid g) { GridDims d; d.B = g.batch; d.D = g.shape[0]; d.H = g.shape[1]; d.W = g.shape[2]; return d; }
 
 
@@ -497,24 +431,6 @@ extern "C" int sessd_sparse_to_dense_planes(const float *d_feat, int max_rows, c
     if (total >= (1ll << 31)) return SESSD_ECAPACITY;
     SESSD_LAUNCH(dense_gather_kernel<true>, persistent_grid(total, 256), 256, 0, stream, d_feat, idx, g, channels, max_rows, nullptr, d_amax,
                  d_info, (__half *)d_planes, total * 4);
-    return last_error();
-}
-
-extern "C" size_t sessd_rulebook_pairs_workspace_bytes(int max_rows, int kvol) {
-    if (max_rows < 1 || kvol < 1) return 0;
-    return sizeof(int) * (size_t)div_up(max_rows, kPairRows) * kvol;
-}
-
-extern "C" int sessd_rulebook_pairs(const int *d_nbr, const int *d_n_out, int max_rows, int kvol, int *d_pairs_in, int *d_pairs_out,
-                                    int *d_pair_num, void *workspace, size_t workspace_bytes, void *stream) {
-    if (!d_nbr || !d_n_out || !d_pairs_in || !d_pairs_out || !d_pair_num || max_rows < 1 || kvol < 1 || kvol > 1024) return SESSD_EINVAL;
-    if (!workspace || workspace_bytes < sessd_rulebook_pairs_workspace_bytes(max_rows, kvol)) return SESSD_EWORKSPACE;
-    cudaStream_t st = (cudaStream_t)stream;
-    const int nblk = div_up(max_rows, kPairRows);
-    int *block_counts = (int *)workspace;   // per-block histograms -> exclusive offsets
-    SESSD_LAUNCH(pair_count_kernel, nblk, kPairRows, sizeof(int) * kvol, st, d_nbr, d_n_out, max_rows, kvol, block_counts);
-    SESSD_LAUNCH(pair_offsets_kernel, kvol, 32, 0, st, d_n_out, max_rows, kvol, block_counts, d_pair_num);
-    SESSD_LAUNCH(pair_write_kernel, nblk, kPairRows, 0, st, d_nbr, d_n_out, max_rows, kvol, block_counts, d_pairs_in, d_pairs_out);
     return last_error();
 }
 

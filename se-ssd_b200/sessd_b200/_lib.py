@@ -68,8 +68,6 @@ SIGNATURES = {
     "sessd_strided_rulebook": (_i, [_vp, _vp, _i, Grid, _i, _vp, _i, _I3, _I3, _I3, Grid, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     "sessd_tile_list_stride": (_i, [_i]),
     "sessd_rulebook_tile_lists": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
-    "sessd_rulebook_pairs_workspace_bytes": (_sz, [_i, _i]),
-    "sessd_rulebook_pairs": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "sessd_spconv_forward": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _vp]),
     "sessd_spconv_forward_rows": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "sessd_spconv_forward_rows_planes": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _f, _f, _vp, _vp, _i, _vp, _vp]),

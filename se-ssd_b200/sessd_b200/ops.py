@@ -134,17 +134,6 @@ def strided_rulebook(in_coors, n_in, max_in, in_grid, in_index_kind, in_index, k
                                      int(max_out), _p(nbr), _p(status), _st()), "sessd_strided_rulebook")
 
 
-def rulebook_pairs(nbr, n, max_rows, kvol):
-    dev = nbr.device
-    pin = torch.full((kvol, max_rows), -1, dtype=torch.int32, device=dev)
-    pout = torch.full((kvol, max_rows), -1, dtype=torch.int32, device=dev)
-    num = torch.zeros((kvol,), dtype=torch.int32, device=dev)
-    ws = torch.empty((lib.sessd_rulebook_pairs_workspace_bytes(int(max_rows), int(kvol)),), dtype=torch.uint8, device=dev)
-    check(lib.sessd_rulebook_pairs(_p(nbr), _p(n), int(max_rows), int(kvol), _p(pin), _p(pout), _p(num), _p(ws), ws.numel(), _st()),
-          "sessd_rulebook_pairs")
-    return pin, pout, num
-
-
 # ------------------------------------------------------------------------------------------------ sparse conv
 def spconv_forward(in_feat, nbr, n_out, max_out, weight, scale, shift, relu, out=None):
     """in_feat [*,Cin]; nbr [max_out,kvol]; weight [kvol,Cin,Cout]; scale/shift [Cout] or None."""

@@ -15,7 +15,6 @@ kernel, and the CPU tests check that each changes at least one crafted expectati
   "cut_off_by_one"               the max_voxels cut lets one voxel too many through
   "keep_last"                    a voxel keeps its last max_points points instead of its first
   "no_frame_key"                 the voxel key misses the frame index (frames share cells)
-  "pairs_by_input"               canonical pairs ordered by input row instead of output row
 """
 import numpy as np
 
@@ -199,19 +198,6 @@ def level_table(sites, rows, shape, out_coors, ksize, stride, padding):
     idx = coors_of(keys, shape)
     idx[keys < 0] = (-(1 << 20), 0, 0, 0)                      # holes: an impossible frame, never matched
     return neighbor_table(idx, shape, out_coors, ksize, stride, padding)
-
-
-def pairs_from_nbr(nbr, mut=()):
-    """canonical pairs: per kernel offset (in, out) sorted by out"""
-    out = []
-    for k in range(nbr.shape[1]):
-        o = np.nonzero(nbr[:, k] >= 0)[0]
-        i = nbr[o, k].astype(np.int64)
-        if "pairs_by_input" in mut:
-            s = np.argsort(i, kind="stable")
-            i, o = i[s], o[s]
-        out.append((i, o.astype(np.int64)))
-    return out
 
 
 # ------------------------------------------------------------------------------------------------------------ voxeliser

@@ -316,22 +316,6 @@ def test_strided_rulebook_refusals():
         ops.strided_rulebook(d, n_dev, len(coors), big, 0, table, (1, 1, 1), (1, 1, 1), (0, 0, 0), big, buf, buf, buf, _n(0), 16, buf, _n(0))
 
 
-@pytest.mark.parametrize("kvol", [1, 3, 27, 125])
-def test_rulebook_pairs(kvol):
-    from sessd_b200 import ops
-    rng = np.random.default_rng(kvol)
-    for n in (0, 255, 256, 257, 9000):
-        nbr = np.where(rng.random((n + 5, kvol)) < 0.5, rng.integers(0, max(n, 1), (n + 5, kvol)), -1).astype(np.int32)
-        d = _i32(nbr)
-        pin, pout, num = ops.rulebook_pairs(d, _n(n), n + 5, kvol)
-        pin, pout, num = _np(pin), _np(pout), _np(num)
-        for k, (i, o) in enumerate(S.pairs_from_nbr(nbr[:n])):
-            assert num[k] == len(i), (n, k)
-            assert np.array_equal(pin[k, :num[k]], i) and np.array_equal(pout[k, :num[k]], o), (n, k)
-        again = ops.rulebook_pairs(d, _n(n), n + 5, kvol)
-        assert np.array_equal(_np(again[0]), pin)
-
-
 # ------------------------------------------------------------------------------------------------------------ overflow
 def _frame_coors(cloud):
     from oracle import cpu as ocpu
