@@ -48,8 +48,9 @@ def _encoder_outputs(feat, coors, deep):
 
 @gpu
 def test_cg_deep_pipeline_matches_default_bitwise_on_a_uniform_frame():
-    """uniform-20k frame (531-808 tiles per cg layer: every CTA of the two-per-SM grid runs several tiles and carries its ring state
-    between them): each layer's output and the dense BEV tensor bitwise equal at deep 0 and deep 1"""
+    """uniform-20k frame (531-808 tiles per cg layer: on 132 SMs each CTA of the 264-CTA default grid runs 2 or 3 tiles and of the
+    132-CTA deep grid 4 to 7, carrying its ring state between them): each layer's output and the dense BEV tensor bitwise equal at deep 0
+    and deep 1.  The ring state at each tile boundary is checked on crafted tables in test_gpu_spconv_cg_grid."""
     from oracle import cpu as ocpu
     from sessd_b200 import synth
     v, c, num = ocpu.points_to_voxel(synth.uniform_cloud(0, 20000), synth.VOXEL_SIZE, synth.PC_RANGE, 5, 20000)

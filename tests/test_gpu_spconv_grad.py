@@ -114,9 +114,14 @@ def test_split_planes_bound_and_untouched_rows():
                                                 ("cg", 64, 64, True), ("cg", 64, 64, False)])
 def test_dgrad_matches_fp64(impl, cin, cout, subm):
     """the data gradient through SparseConvFunction (forward kernel, re-packed weights, same / transposed table) vs conv_backward_from_nbr"""
+    check_dgrad(impl, cin, cout, subm)
+
+
+def check_dgrad(impl, cin, cout, subm, n_in=3000, n_out=2500):
+    """test_dgrad_matches_fp64 on n_in input rows (and n_out output rows of a strided table)"""
     from sessd_b200 import sparse_grad
     rng = np.random.default_rng(cin + cout + subm)
-    n_in, kvol = 3000, 27
+    kvol = 27
     if subm:
         # a point-symmetric table: nbr[o, k] = i  <=>  nbr[i, K-1-k] = o
         nbr = np.full((n_in, kvol), -1, np.int64)
@@ -128,7 +133,6 @@ def test_dgrad_matches_fp64(impl, cin, cout, subm):
         nbr[:, kvol // 2] = np.arange(n_in)
         n_out = n_in
     else:
-        n_out = 2500
         nbr = _strided_nbr(n_out, n_in, kvol, cin)
     x = rng.standard_normal((n_in, cin)).astype(np.float32)
     w = (rng.standard_normal((3, 3, 3, cin, cout)) / np.sqrt(27 * cin)).astype(np.float32)

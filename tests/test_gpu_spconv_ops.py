@@ -31,26 +31,33 @@ planes outputs (fp16 (hi, lo) [rows][2][cpo] at the scale S = pow2_scale_for_bou
   |(hi + lo) / S - o| <= 2^-9 / S <= 2^-23 bound; checked at 2^-22 bound.
 
 Each tolerance is shown to catch a subtly wrong kernel on the CPU (negative controls): the emulation without the cross products, with one
-(row, offset) pair dropped, with a row's product taken from the previous offset of its stage (a missed dirty-row clear), with two
-offsets' weights swapped, and the fp64 result with one pair dropped.  Smallest ratio of error to bound of each control over the control
-cases (cg vs emulation bound / cg vs fp64 bound): no cross products 9.1 / 4.1, missed dirty-row clear 71 / 36, one pair dropped
-1190 / 740, two offsets' weights swapped 9230 / 5000; fp64 with one pair dropped vs the fp32 bound 540.
+(row, offset) pair dropped, with a row's product taken from the previous offset of its stage within a tile (a missed dirty-row clear),
+with two offsets' weights swapped, and the fp64 result with one pair dropped.  The staging faults that carry stale rows from tile to
+tile (dirty masks reset at each tile, a two-warp group's second warp never clearing, a two-stage warp not rotating its masks) are
+replayed by cg_ring_model on the tables of test_gpu_spconv_cg_grid, which is where they are flagged.  Smallest ratio of error to bound
+of each control over the control cases (cg vs emulation bound / cg vs fp64 bound): no cross products 9.1 / 4.1, missed dirty-row clear
+71 / 36, one pair dropped 1190 / 740, two offsets' weights swapped 9230 / 5000; fp64 with one pair dropped vs the fp32 bound 540.
 Largest ratios measured on one H100 80GB HBM3 (400 W power limit), the same at deep 0 and deep 1: cg vs emulation 0.46 (single-pair
 rows: the wgmma accumulation is not round-to-nearest, ~1 ulp per step), cg vs fp64 0.03, rows and SIMT vs fp64 0.55, planes 0.1.
+With (64,32) added and `single` sized against the device grid, the largest cg ratios measured on an H100 (132 SMs) over all eight
+instantiations were 0.49 vs the emulation, 0.05 vs fp64 and 0.051 for the planes.
 """
 import numpy as np
 import pytest
 import torch
 
+from cg_ring_model import NACTS, CgLayout, cg_grid, replay, tile_ring
 from oracle.spconv_ref import conv_from_nbr
 
 U = 2.0 ** -24
 CG_C = 2.0                                     # wgmma accumulation: ulps per k=16 step (module docstring)
-NUM_SMS = 132                                  # H100 SXM: persistent grids of the cg kernel are min(tiles, SMs) CTAs
-BIG = 3 * NUM_SMS * 128 + 77                   # every persistent CTA runs >= 3 tiles
-SWEEP = 8 * NUM_SMS * 128 + 50                 # nact_sweep: enough tiles per CTA to meet every ring position
-NACTS = (1, 2, 3, 4, 5, 7, 8, 9, 27)           # kStages - 1, kStages, kStages + 1 for kStages 2, 4, 8; 1 and 27
+BIG = 3 * 132 * 128 + 77                       # `single` for the fp32 kernels: 397 tiles (the cg cases size it against the device grid)
+SWEEP = 8 * 132 * 128 + 50                     # nact_sweep: 1057 tiles, >= 4 per CTA at 264 CTAs, >= 8 at 132 (ring_positions)
 NACT_SCHEDULE_SEED = 2
+# grids of spconv_cg (cg_ring_model.cg_grid: min(tiles, blocks_per_sm x SMs)) with the ring lengths that run at them: the default
+# pipeline (2 CTAs per SM; 2 stages at Cp 64, 4 at Cp 32) and the deep one (1 CTA per SM; 4 and 8 stages), on 132- and 114-SM parts.
+# The deep grids are checked at 2 stages too.
+GRID_RINGS = ((264, (2, 4)), (228, (2, 4)), (132, (2, 4, 8)), (114, (2, 4, 8)))
 SLACK = 3                                      # sentinel rows past max_out in every output buffer
 PATTERNS = ("full", "single", "flip", "nact_sweep", "empty_tiles", "duplicates", "high_rows")
 F32_SENTINEL = -1234.5
@@ -74,7 +81,9 @@ def crafted_nbr(pattern, n, kvol, n_in, seed):
     elif pattern == "single":              # one offset per row, rotating: a stage's consecutive fills (k, k + kStages) hit disjoint rows
         k = (r + r // 128) % kvol
         nbr[r, k] = rand[r, k]
-    elif pattern == "flip":                # valid iff (r + k) even: every row's validity flips between consecutive offsets
+    elif pattern == "flip":                # valid iff (r + k) even: every row's validity flips between consecutive offsets.  A stage's
+        # fills k and k + kStages share their parity at every (even) ring length, so within a tile no dirty row is ever cleared; the
+        # clears across tiles are test_gpu_spconv_cg_grid's
         ok = (r[:, None] + np.arange(kvol)[None, :]) % 2 == 0
         nbr[ok] = rand[ok]
     elif pattern == "nact_sweep":          # tiles with exactly nact active offsets, nact from NACTS (<= kvol)
@@ -108,16 +117,19 @@ def crafted_nbr(pattern, n, kvol, n_in, seed):
 
 class Case:
     """One crafted layer: nbr [max_out, kvol] (rows >= n_eff hold valid-looking entries the kernels must ignore), device row count n_dev,
-    the input rows actually used (in_rows) with their fp32 features x, weights, folded BN."""
+    the input rows actually used (in_rows) with their fp32 features x, weights, folded BN.  live: the first n_eff rows of the table
+    (default: crafted_nbr(pattern, ...))."""
 
-    def __init__(self, pattern, n, kvol, cin, cout, seed, n_in=None, max_out=None, n_dev=None, relu=True, shift=True):
+    def __init__(self, pattern, n, kvol, cin, cout, seed, n_in=None, max_out=None, n_dev=None, relu=True, shift=True, live=None):
         rng = np.random.default_rng(seed + 1000)
         self.pattern, self.kvol, self.cin, self.cout, self.relu = pattern, kvol, cin, cout, relu
         self.max_out = n + 40 if max_out is None else max_out
         self.n_dev = n if n_dev is None else n_dev
         self.n_eff = min(self.n_dev, self.max_out)
         self.n_in = n_in if n_in is not None else max(64, n // 2)
-        live = crafted_nbr(pattern, self.n_eff, kvol, self.n_in, seed)
+        if live is None:
+            live = crafted_nbr(pattern, self.n_eff, kvol, self.n_in, seed)
+        assert live.shape == (self.n_eff, kvol)
         self.nbr = rng.integers(0, self.n_in, (self.max_out, kvol))
         self.nbr[:self.n_eff] = live
         self.in_rows = np.unique(live[live >= 0])
@@ -283,31 +295,23 @@ def check_planes(hi, lo, cout, s, bound, f32):
     return ratio(back, f32.astype(np.float64), np.full(f32.shape, 2.0 ** -22 * bound))
 
 
-def ring_positions(nbr, n, stages, num_ctas=NUM_SMS):
-    """(nact, st0, ph0) of every tile of a persistent cg launch: tile t runs on CTA t % grid after that CTA's earlier tiles"""
-    ntiles = -(-n // 128)
-    grid = min(ntiles, num_ctas)
-    nact = [int((nbr[t * 128:(t + 1) * 128] >= 0).any(0).sum()) for t in range(ntiles)]
-    seen = set()
-    for b in range(grid):
-        st0 = ph0 = 0
-        for t in range(b, ntiles, grid):
-            seen.add((nact[t], st0, ph0))
-            adv = st0 + nact[t]
-            ph0 ^= (adv // stages) & 1
-            st0 = adv % stages
-    return seen
+def ring_positions(nbr, n, stages, grid):
+    """(nact, st0, ph0) of every tile of a persistent cg launch of `grid` CTAs: tile t runs on CTA t % grid after that CTA's earlier
+    tiles (cg_ring_model.tile_ring)"""
+    _cta, _round, p, nact = tile_ring(nbr, n, grid)
+    return set(zip(nact.tolist(), (p % stages).tolist(), ((p // stages) & 1).tolist()))
 
 
 # ================================================================================================================== CPU section
 def test_nact_sweep_reaches_every_ring_position():
     """The nact_sweep rulebook of the GPU tests meets every active-offset count of NACTS at every ring position (st0, phase) a persistent
-    CTA can carry in, for all four ring lengths (2 and 4 stages at Cp 64, 4 and 8 at Cp 32)."""
+    CTA can carry in, for the ring lengths that run at each grid (GRID_RINGS: 264 and 132 CTAs on 132 SMs, 228 and 114 on 114)."""
     nbr = crafted_nbr("nact_sweep", SWEEP, 27, 4000, 11)
-    for stages in (2, 4, 8):
-        seen = ring_positions(nbr, SWEEP, stages)
-        want = {(a, s, p) for a in NACTS for s in range(stages) for p in (0, 1)}
-        assert want <= seen, sorted(want - seen)[:5]
+    for grid, rings in GRID_RINGS:
+        for stages in rings:
+            seen = ring_positions(nbr, SWEEP, stages, grid)
+            want = {(a, s, p) for a in NACTS for s in range(stages) for p in (0, 1)}
+            assert want <= seen, (grid, stages, sorted(want - seen)[:5])
 
 
 @pytest.mark.parametrize("pattern", PATTERNS)
@@ -323,6 +327,8 @@ def test_crafted_rulebooks_have_their_shape(pattern):
         assert all(valid[t * 128:(t + 1) * 128].any(0).all() for t in range(n // 128))      # full tiles fill every offset
     if pattern == "flip":
         assert (valid[:, 1:] != valid[:, :-1]).all()
+        for cp, deep in ((32, 0), (64, 0), (32, 1)):                # ring lengths 4, 2, 8, one tile per CTA: no clear
+            assert not replay(nbr, n, n, -(-n // 128), CgLayout(cp, 32, deep)).clears
     if pattern == "nact_sweep":
         nact = [int(valid[t * 128:(t + 1) * 128].any(0).sum()) for t in range(-(-n // 128))]
         assert set(nact) <= set(NACTS)
@@ -540,15 +546,16 @@ def test_tile_lists_regroup_crafted_tables_exactly(kvol):
 
 
 def _cg_specs():
-    """every pattern meets every instantiation (each spec runs at deep 0 and 1); ReLU, shift and the outputs rotate over the cases"""
+    """every pattern meets every instantiation (each spec runs at deep 0 and 1); ReLU, shift and the outputs rotate over the cases.
+    `single` is sized at run time against the device grid (None here), the others are fixed."""
     specs = []
-    sizes = {"full": (1, 128, 129), "single": (BIG,) * 3, "flip": (127, 129, 128), "nact_sweep": (SWEEP,) * 3,
-             "empty_tiles": (10 * 128 + 37,) * 3, "duplicates": (300, 300, 300), "high_rows": (200, 200, 200)}
-    for ii, (cp, cout) in enumerate(((32, 32), (32, 64), (64, 64))):
+    sizes = {"full": (1, 128, 129, 127), "single": (None,) * 4, "flip": (127, 129, 128, 255), "nact_sweep": (SWEEP,) * 4,
+             "empty_tiles": (10 * 128 + 37,) * 4, "duplicates": (300, 300, 300, 300), "high_rows": (200, 200, 200, 200)}
+    for ii, (cp, cout) in enumerate(((32, 32), (32, 64), (64, 64), (64, 32))):
         for pi, pattern in enumerate(PATTERNS):
             i = 7 * ii + pi
             n = sizes[pattern][ii]
-            max_out, n_dev = n + (i % 3) * 40, n
+            max_out, n_dev = (None, None) if n is None else (n + (i % 3) * 40, n)
             if pattern == "duplicates" and cout == 64 and cp == 32:
                 max_out, n_dev = 260, 300                        # device count above the capacity: the kernel clamps
             specs.append(dict(cp=cp, cout=cout, pattern=pattern, n=n, max_out=max_out, n_dev=n_dev, relu=(i // 2) % 2 == 0,
@@ -614,12 +621,17 @@ def _check_cg(case, emu, plane_rows, label, sp_cg_deep, first_output=2):
 @gpu
 @pytest.mark.parametrize("spec", _cg_specs(), ids=_cg_id)
 def test_cg_kernel_matches_emulation_and_fp64(spec, sp_cg_deep):
-    """spconv_forward_cg, all six instantiations ((32,32), (32,64), (64,64) x deep 0 / 1) on every crafted pattern, ReLU, shift and the
-    outputs rotating: fp32 rows within the accumulation bound of the fp64 emulation and within that plus the split's error of fp64,
-    planes within 2^-22 bound, out_info exact, run to run and deep 0 vs deep 1 bitwise, rows past the device count untouched.  The
-    single and nact_sweep cases run several tiles per persistent CTA, so the ring state carried between tiles (stage, phase, dirty
-    rows) is exercised at all four ring lengths."""
+    """spconv_forward_cg, all eight instantiations ((32,32), (32,64), (64,64), (64,32) x deep 0 / 1) on every crafted pattern, ReLU, shift
+    and the outputs rotating: fp32 rows within the accumulation bound of the fp64 emulation and within that plus the split's error of
+    fp64, planes within 2^-22 bound, out_info exact, run to run and deep 0 vs deep 1 bitwise, rows past the device count untouched.
+    nact_sweep meets every (active offsets, st0, phase) a CTA can carry into a tile at the ring lengths of both grids
+    (test_nact_sweep_reaches_every_ring_position) and `single`, 3 grid + 1 tiles at the device's default grid, gives every CTA three
+    tiles or more (six at deep 1).  Whether each dirty-row clear across tiles is reached is left to the cases of
+    test_gpu_spconv_cg_grid, which are built against the grid and assert it."""
     s = spec
+    if s["n"] is None:
+        n = 3 * cg_grid(s["cp"], s["cout"], 0, 1 << 30) * 128 + 77
+        s = dict(s, n=n, max_out=n + (s["seed"] - 100) % 3 * 40, n_dev=n)
     case = Case(s["pattern"], min(s["n_dev"], s["max_out"]), 27, s["cp"], s["cout"], s["seed"], n_in=s["n_in"], max_out=s["max_out"],
                 n_dev=s["n_dev"], relu=s["relu"], shift=s["shift"])
     _check_cg(case, CgEmu(case, s["cp"]), case.n_in + 1, _cg_id(s), sp_cg_deep, s["outputs"])
