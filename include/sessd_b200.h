@@ -222,21 +222,26 @@ typedef struct {
 int sessd_bev_conv_p2(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                       const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                       float *d_out_f32, void *d_out_planes, float *d_out_info, const sessd_conv_desc *desc, const int *d_items,
-                      void *stream);
+                      const int *d_segs, void *stream);
 int sessd_bev_deconv_p2(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                         const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                         float *d_out_f32, void *d_out_planes, float *d_out_info, int batch, int in_h, int in_w, int cin, int cout,
-                        int relu, const int *d_items, void *stream);
+                        int relu, const int *d_items, const int *d_segs, void *stream);
 /* Constant-region skipping of the SSFA neck + head (csrc/bevskip.cu).  Where the last sparse level has no site, dense() writes exact
  * zeros; every neck pixel whose receptive field lies in that empty space (and inside the map) then holds, bit for bit, the same value
  * as every other such pixel of its output-parity class.  sessd_bev_skip_plan derives from the level's bitmap index, per neck launch
  * (SKIP_LAUNCHES order of runners.SSFAPlanesRunner), the work items that must run plus one representative of the skipped ones, all on
  * the device.  The conv / deconv run the list (d_items = the launch's record); sessd_bev_skip_fill then copies the representative's
  * output into the skipped tiles.  sessd_bev_skip_plan_words: int32 words of the plan of a [batch, h, w] neck; offsets[13] <- the
- * word offset of every launch record. */
+ * word offset of every launch record.  The same plan also lists, in d_segs, the live segments (8 pixels along the launch's u in one
+ * v row) of every stride-1 launch, packed 16 to a work item: the conv / deconv run them (d_segs = the launch's segment record) and
+ * sessd_bev_skip_fill_segs fills the other segments.  sessd_bev_skip_seg_words: int32 words of d_segs; offsets[13] <- the word offset
+ * of every segment record, -1 for the stride-2 launch (tiles only). */
 long long sessd_bev_skip_plan_words(int batch, int h, int w, int *offsets);
-int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, int *d_plan, void *stream);
+long long sessd_bev_skip_seg_words(int batch, int h, int w, int *offsets);
+int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, int *d_plan, int *d_segs, void *stream);
 int sessd_bev_skip_fill(const int *d_record, float *d_out_f32, void *d_out_planes, int cout, void *stream);
+int sessd_bev_skip_fill_segs(const int *d_seg_record, float *d_out_f32, void *d_out_planes, int cout, void *stream);
 /* Weight gradient of a BEV conv (csrc/bevgrad.cu; training of the neck and head, rpn_v1.py:135-210, mg_head_sessd.py:202-215):
  *    d_gw[t][ci][co] = sum_{b, y, x} in[b, y*is + dy[t], x*is + dx[t], ci] * g[b, y, x, co]     (zero outside the input)
  * for the tap list, stride and extents of the forward's descriptor (out_stride 1, no offset, grid = the output extent; relu ignored).

@@ -26,18 +26,18 @@ int sessd_bev_deconv_h2(const float *d_in, const void *d_weight_h2, int cout_pad
                         const float *d_shift, const float *d_residual, float *d_out, int batch, int in_h, int in_w,
                         int cin, int cout, int relu, const float *d_amax_in, float *d_amax_out, void *stream);
 
-/* Stall profile of the product's planes conv / deconv (sessd_bev_conv_p2 / sessd_bev_deconv_p2, same arguments and results): the
- * kernel's clock counters are written to d_prof, int64 [grid][16] with grid = min(work items, SMs); word order in csrc/bevconv_p2.cuh
+/* Stall profile of the product's planes conv / deconv (sessd_bev_conv_p2 / sessd_bev_deconv_p2, same arguments and results, d_prof
+ * between d_segs and the stream): the kernel's clock counters are written to d_prof, int64 [grid][16] with grid = min(work items, SMs); word order in csrc/bevconv_p2.cuh
  * (P2Prof).  For measurement only: the counters cost clocks of their own. */
 int sessd_bev_conv_p2_profile(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
                               const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
                               float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info,
-                              const sessd_conv_desc *desc, const int *d_items, long long *d_prof, void *stream);
+                              const sessd_conv_desc *desc, const int *d_items, const int *d_segs, long long *d_prof, void *stream);
 int sessd_bev_deconv_p2_profile(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
                                 const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
                                 float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, int batch,
-                                int in_h, int in_w, int cin, int cout, int relu, const int *d_items, long long *d_prof,
-                                void *stream);
+                                int in_h, int in_w, int cin, int cout, int relu, const int *d_items, const int *d_segs,
+                                long long *d_prof, void *stream);
 
 /* Loader-only probe of sessd_bev_conv_p2_profile's launch: the two TMA producer warps run unchanged, the consumers wait on the full
  * barriers and release them without issuing wgmma or an epilogue, so the launch's time is what the loads alone take (no output is
@@ -47,6 +47,11 @@ int sessd_bev_conv_p2_loads(const void *d_in_planes, const float *d_in_info, con
                             const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
                             float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info,
                             const sessd_conv_desc *desc, const int *d_items, int smem_a, long long *d_prof, void *stream);
+/* The same probe on a segment record of sessd_bev_skip_plan (d_segs, required; stride-1 conv): the patch layout of segment windows. */
+int sessd_bev_conv_p2_seg_loads(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
+                                const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
+                                float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info,
+                                const sessd_conv_desc *desc, const int *d_segs, long long *d_prof, void *stream);
 
 /* The launch plan of the conv desc (deconv != 0: of the deconv of desc's batch, in_h, in_w, cin and cout) as sessd_bev_conv_p2 (split 0;
  * smem_a as for sessd_bev_conv_p2_loads) or sessd_bev_conv_h2 (split != 0) would launch it, without launching: plan[19] =

@@ -10,10 +10,12 @@ b_full / patch_full / wgmma_wait and in the epilogue, the producers' shares wait
 per tap step against the tensor-core floor (6 * n_tile clocks: 128 px x 32 cin x 3 n_tile fp16 FMA at 2048 FMA/clk/SM).  The card's
 name, power limit and SM clocks are read in the same run.  The counters cost clocks of their own: the µs here are not bench numbers.
 
---loads adds the L2 -> SM ceiling of the 3x3 128 -> 128 launch: the launch alone and dense through the loader-only probe
-(sessd_bev_conv_p2_loads: the TMA producers run unchanged, the consumers only wait on the full barriers and release them), once with
-the three patch copies shared-memory A descriptors would need and once with the single copy the register-fed A reads.  Bytes are counted
-from the shapes (per item and 32-channel chunk: the patch boxes plus nine 16 KB weight stages); reported per clock and SM and as TB/s.
+--loads adds the L2 -> SM ceiling of the 3x3 128 -> 128 launch: the launch alone through the loader-only probe
+(sessd_bev_conv_p2_loads: the TMA producers run unchanged, the consumers only wait on the full barriers and release them), dense once
+with the three patch copies shared-memory A descriptors would need and once with the single copy the register-fed A reads, then on the
+frame's segment record (sessd_bev_conv_p2_seg_loads: one 3 x 10-row window per segment).  Bytes are counted from the shapes (per item
+and 32-channel chunk: the patch boxes plus nine 16 KB weight stages; segments: the windows of the item's segments); reported per clock
+and SM and as TB/s.
 
     python scripts/p2_stall_profile.py --out FILE [--reps 20] [--engines 12] [--frames 8] [--loads]
 """
@@ -52,7 +54,9 @@ class Profiler:
         from sessd_b200 import ops
         self.torch, self.ops, self.device, self.num_sms = torch, ops, device, num_sms
         self.bufs, self.key = {}, None
-        self.loads_smem_a = None      # 0 / 1: route conv() to the loader-only probe with that patch plan, counters filed under self.key
+        # 0 / 1: route conv() to the loader-only probe with that patch plan ("segs": on the launch's segment record), counters filed
+        # under self.key
+        self.loads_smem_a = None
         ops.bev_conv_p2, ops.bev_deconv_p2 = self.conv, self.deconv
 
     def buf(self):
@@ -61,8 +65,14 @@ class Profiler:
         return self.bufs[self.key]
 
     def conv(self, in_planes, in_info, weight_h2, scale, shift, residual, resid_info, gain, shift_max, out_f32, out_planes, out_info, desc,
-             items=None):
+             items=None, segs=None):
         o = self.ops
+        if self.loads_smem_a == "segs":
+            o.check(o.lib.sessd_bev_conv_p2_seg_loads(o._p(in_planes), o._p(in_info), o._p(weight_h2), int(weight_h2.shape[2]), o._p(scale),
+                                                      o._p(shift), o._p(residual), o._p(resid_info), float(gain), float(shift_max),
+                                                      o._p(out_f32), o._p(out_planes), o._p(out_info), C.byref(desc), o._p(segs),
+                                                      o._p(self.buf()), o._st()), "sessd_bev_conv_p2_seg_loads")
+            return
         if self.loads_smem_a is not None:
             o.check(o.lib.sessd_bev_conv_p2_loads(o._p(in_planes), o._p(in_info), o._p(weight_h2), int(weight_h2.shape[2]), o._p(scale),
                                                   o._p(shift), o._p(residual), o._p(resid_info), float(gain), float(shift_max), o._p(out_f32),
@@ -71,18 +81,20 @@ class Profiler:
             return
         o.check(o.lib.sessd_bev_conv_p2_profile(o._p(in_planes), o._p(in_info), o._p(weight_h2), int(weight_h2.shape[2]), o._p(scale),
                                                 o._p(shift), o._p(residual), o._p(resid_info), float(gain), float(shift_max), o._p(out_f32),
-                                                o._p(out_planes), o._p(out_info), C.byref(desc), o._p(items), o._p(self.buf()), o._st()),
+                                                o._p(out_planes), o._p(out_info), C.byref(desc), o._p(items), o._p(segs), o._p(self.buf()),
+                                                o._st()),
                 "sessd_bev_conv_p2_profile")
 
     def deconv(self, in_planes, in_info, weight_h2, scale, shift, residual, resid_info, gain, shift_max, out_f32, out_planes, out_info,
-               relu=True, items=None):
+               relu=True, items=None, segs=None):
         o = self.ops
         _two, b, h, w, cin = in_planes.shape
         cout = (out_f32 if out_f32 is not None else out_planes).shape[-1]
         o.check(o.lib.sessd_bev_deconv_p2_profile(o._p(in_planes), o._p(in_info), o._p(weight_h2), int(weight_h2.shape[2]), o._p(scale),
                                                   o._p(shift), o._p(residual), o._p(resid_info), float(gain), float(shift_max),
                                                   o._p(out_f32), o._p(out_planes), o._p(out_info), int(b), int(h), int(w), int(cin), int(cout),
-                                                  int(bool(relu)), o._p(items), o._p(self.buf()), o._st()), "sessd_bev_deconv_p2_profile")
+                                                  int(bool(relu)), o._p(items), o._p(segs), o._p(self.buf()), o._st()),
+                "sessd_bev_deconv_p2_profile")
 
     def tag(self, eng_id, neck):
         """every launch of this engine's neck files its counters under (eng_id, launch name, dense | skip)"""
@@ -172,23 +184,29 @@ def main():
             # 64 B, plus 9 weight stages of 2 x 128 rows of 64 B
             L = next(L for L in SSFA_LAUNCHES if L.kind == "conv" and L.cin == 128 and L.cout == 128 and L.k == 3 and L.stride == 1)
             res["loads"] = dict(launch=L.name)
-            for smem_a, patch in ((1, 3 * 2 * 18 * 8 * 64), (0, 2 * 18 * 10 * 64)):
+            # segments: 2 planes x 3 x 10 rows of 64 B per segment of the item
+            seg_rec = eng.neck.skip.seg_record(eng.neck.SKIP_LAUNCHES.index(L.name)).cpu().numpy()
+            groups = seg_rec[32:32 + 16 * int(seg_rec[2])]
+            seg_patch = 2 * 3 * 10 * 64 * float((groups >= 0).sum()) / max(len(groups) // 16, 1)
+            for smem_a, patch, name in ((1, 3 * 2 * 18 * 8 * 64, "smem_a"), (0, 2 * 18 * 10 * 64, "reg_a"), ("segs", seg_patch, "segs")):
                 prof.loads_smem_a = smem_a
-                prof.key = (0, L.name, "loads%d" % smem_a)
+                prof.key = (0, L.name, "loads_%s" % name)
+                skip = smem_a == "segs"
                 for _ in range(3):
-                    eng.neck._launch(L, False)
+                    eng.neck._launch(L, skip)
                 t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 t0.record(eng.stream)
                 for _ in range(a.reps):
-                    eng.neck._launch(L, False)
+                    eng.neck._launch(L, skip)
                 t1.record(eng.stream)
                 eng.stream.synchronize()
                 us = t0.elapsed_time(t1) * 1000.0 / a.reps
                 r = prof.bufs[prof.key].cpu().numpy().astype(np.float64)
                 item_bytes = (L.cin // 32) * (patch + 9 * 2 * 128 * 64)
                 act = r[:, ITEMS] > 0
-                res["loads"]["smem_a" if smem_a else "reg_a"] = dict(
+                res["loads"][name] = dict(
                     us=us, items=int(r[:, ITEMS].sum()), bytes_per_item=item_bytes, patch_bytes_per_chunk=patch,
+                    bytes_per_step=item_bytes / (9 * (L.cin // 32)),
                     bytes_per_clk_per_sm=float((r[act, ITEMS] * item_bytes / r[act, CTA]).mean()),
                     tb_per_s=float(r[:, ITEMS].sum() * item_bytes / (us * 1e-6) / 1e12))
             prof.loads_smem_a = None
@@ -253,10 +271,11 @@ def main():
             k, t["clk_per_step_main"], t["floor_clk_per_step"], t["clk_per_step_with_epilogue"],
             {x: round(v, 3) for x, v in t["consumer_share"].items()}, {x: round(v, 3) for x, v in t["producer_share"].items()}))
     if a.loads:
-        for k in ("smem_a", "reg_a"):
+        for k in ("smem_a", "reg_a", "segs"):
             r = res["loads"][k]
-            print("  loader-only %-6s %s: %.1f us, %d B per item, %.1f B/clk/SM, %.2f TB/s" % (
-                k, res["loads"]["launch"], r["us"], r["bytes_per_item"], r["bytes_per_clk_per_sm"], r["tb_per_s"]))
+            print("  loader-only %-6s %s: %.1f us, %d items, %d B per item, %d B per step, %.1f B/clk/SM, %.2f TB/s" % (
+                k, res["loads"]["launch"], r["us"], r["items"], r["bytes_per_item"], r["bytes_per_step"], r["bytes_per_clk_per_sm"],
+                r["tb_per_s"]))
     print("  alone totals (us): %s; concurrent frames/s while profiled: %.0f" % (res["alone_total_us"], res["concurrent_frames_per_s_profiled"]))
 
 

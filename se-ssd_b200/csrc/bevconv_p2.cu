@@ -33,13 +33,14 @@ using namespace sessd;
 //   gain, shift_max: |out| <= amax_in * gain + shift_max (+ amax_resid), see the header;
 //   outputs: d_out_f32 (fp32 NHWC) and / or d_out_planes (__half [2][batch][out_h][out_w][cout], scale written to d_out_info[1]);
 //   d_out_info[0] is atomically raised to max|out| (zero it once per frame).
-//   d_items (nullable): a launch record of sessd_bev_skip_plan -- only the work items it lists run (same grid, same per-item work).
+//   d_items (nullable): a launch record of sessd_bev_skip_plan -- only the work items it lists run (same grid, same per-item work);
+//   d_segs (nullable, stride 1 only, not with d_items): a launch's segment record of sessd_bev_skip_plan -- only its segments run.
 extern "C" int sessd_bev_conv_p2(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                                  const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                                  float *d_out_f32, void *d_out_planes, float *d_out_info, const sessd_conv_desc *desc, const int *d_items,
-                                 void *stream) {
+                                 const int *d_segs, void *stream) {
     return p2_conv<kP2Planes>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
-                              d_out_f32, d_out_planes, d_out_info, desc, stream, d_items);
+                              d_out_f32, d_out_planes, d_out_info, desc, stream, d_items, nullptr, false, d_segs);
 }
 
 // ConvTranspose2d(k3, s2, p1, op1) + BN + ReLU (+ residual), four output-parity classes in one launch; weights [2][9][cout_pad][cin],
@@ -47,9 +48,9 @@ extern "C" int sessd_bev_conv_p2(const void *d_in_planes, const float *d_in_info
 extern "C" int sessd_bev_deconv_p2(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                                    const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                                    float *d_out_f32, void *d_out_planes, float *d_out_info, int batch, int in_h, int in_w, int cin, int cout,
-                                   int relu, const int *d_items, void *stream) {
+                                   int relu, const int *d_items, const int *d_segs, void *stream) {
     return p2_deconv<kP2Planes>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
-                                d_out_f32, d_out_planes, d_out_info, batch, in_h, in_w, cin, cout, relu, stream, d_items);
+                                d_out_f32, d_out_planes, d_out_info, batch, in_h, in_w, cin, cout, relu, stream, d_items, nullptr, d_segs);
 }
 
 // fp32 [n] (n % 4 == 0, 16-byte aligned) -> planes [2][n] fp16 scaled by the power of two that maps d_info[0] (the tensor's abs-max,

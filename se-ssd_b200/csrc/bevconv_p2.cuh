@@ -50,6 +50,11 @@ constexpr int kP2MaxSmem = 227 * 1024;
 constexpr int kP2Chunk = 32;                              // input channels per K stage: one 64-byte fp16 operand row
 // optional device item list (bevskip.cu): int32 record, word 0 = number of items to run, the item indices from word kP2ItemsHeader on
 constexpr int kP2ItemsHeader = 32;
+// optional device segment list (bevskip.cu, register-A launches only): word 0 = number of items to run, the groups from word
+// kP2SegHeader on.  A group is kP2SegSlots = 16 segments of kP2TileU pixels along u in one v row, one int32 each: class << 24 | segment
+// index ((b * grid_v + v) * tiles_u + u / 8), -1 for an empty slot (only after the group's last segment); item k runs group
+// k / nblocks on n-block k % nblocks.  Slot s takes the place of tile v row s: rows 8 s .. 8 s + 7 of the item.
+constexpr int kP2SegHeader = 32, kP2SegSlots = kP2TileV;
 // operand source of the A side: pre-split fp16 planes (TMA straight into the operand layout), or an fp32 NHWC input that TMA stages in
 // shared memory and the consumer warpgroups split there into fp16 (hi, lo) with the power-of-two scale of its abs-max
 enum { kP2Planes = 0, kP2SplitF16 = 1 };
@@ -84,6 +89,8 @@ struct P2Params {
     float *out_info;                   // [2] = {running abs-max of the output (atomicMax), S_out}
     long long out_plane_stride;        // elements between the hi and the lo plane of the output
     const int *items;                  // nullable: run only the listed work items (count + indices, see kP2ItemsHeader), else all p.total
+    const int *segs;                   // nullable (REGA only): run the listed segment groups (see kP2SegHeader) instead of tiles
+    int slot_rows;                     // REGA: patch rows from one tile v row (segment slot) to the next: pitch_u (segments: a slot)
     long long *prof;                   // probe instantiations only: [grid][kP2ProfWords] clock counters (P2Prof)
 };
 
@@ -106,7 +113,7 @@ enum P2Prof {
 };
 
 // number of work items this launch runs and the k-th of them (every warp role walks the same sequence)
-__device__ __forceinline__ int p2_item_count(const P2Params &p) { return p.items ? __ldg(p.items) : p.total; }
+__device__ __forceinline__ int p2_item_count(const P2Params &p) { return p.segs ? __ldg(p.segs) : p.items ? __ldg(p.items) : p.total; }
 __device__ __forceinline__ int p2_item(const P2Params &p, int k) { return p.items ? __ldg(p.items + kP2ItemsHeader + k) : k; }
 
 // work item g -> (class rank in the heavy-first order, n-block, pixel tile): the item encoding of the kernel and of the skip planner
@@ -130,6 +137,16 @@ __device__ __forceinline__ P2Item p2_decode(const P2Params &p, int g) {
     it.u0 = tu * kP2TileU; it.v0 = tv * kP2TileV;
     it.ntaps = p.cls_ntaps[it.cls];
     return it;
+}
+
+// segment list: the 16 entries of item k's group, and one entry's frame, first pixel along u and v row
+__device__ __forceinline__ const int *p2_seg_group(const P2Params &p, int k) {
+    return p.segs + kP2SegHeader + (k / p.nblocks) * kP2SegSlots;
+}
+struct P2Seg { int b, u0, v; };
+__device__ __forceinline__ P2Seg p2_seg(const P2Params &p, int e) {
+    const int s = e & 0xFFFFFF, rest = s / p.tiles_u;
+    return {rest / p.grid_v, (s - rest * p.tiles_u) * kP2TileU, rest % p.grid_v};
 }
 
 // N output columns: NT (one plane of the weight stage) or 2 NT (the whole [b_lo ; b_hi] stage)
@@ -237,6 +254,24 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
             uint32_t pph = 0;
             const uint32_t patches_u32 = smem_u32(patches);
             for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
+                if (REGA && p.segs) {
+                    // one window [rows][pitch_u] per segment and plane into its slot: lane l loads plane l & 1 of slot l / 2
+                    const int e = __ldg(p2_seg_group(p, k) + (lane >> 1));
+                    const P2Seg sg = p2_seg(p, e);
+                    const uint32_t bytes = (uint32_t)__popc(__ballot_sync(0xFFFFFFFFu, e >= 0)) * (uint32_t)p.load_bytes;
+                    const uint32_t dst0 = patches_u32 + (uint32_t)((lane & 1) * p.copy_bytes + (lane >> 1) * p.slot_rows * 64);
+                    for (int cc = 0; cc < nchunks; ++cc) {
+                        { const long long t0 = p2_tick<PROFILE>(); mbar_wait<REGA>(&patch_empty[pb], pph ^ 1u); p2_tock<PROFILE>(clk[kProfPatchEmpty], t0); }
+                        if (elect_one()) mbar_expect_tx(&patch_full[pb], bytes);
+                        __syncwarp();
+                        if (e >= 0)
+                            tma_load_5d(dst0 + (uint32_t)(pb * p.patch_bytes), &map_a, &patch_full[pb], cc * kP2Chunk, sg.u0 + p.copy_u[0],
+                                        sg.v + p.copy_v[0], sg.b, lane & 1);
+                        __syncwarp();
+                        if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
+                    }
+                    continue;
+                }
                 const P2Item it = p2_decode(p, p2_item(p, k));
                 const int bu = it.u0 * p.in_stride, bv = it.v0 * p.in_stride;
                 for (int cc = 0; cc < nchunks; ++cc) {
@@ -271,7 +306,14 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
             int S = 0;
             uint32_t bph = 0;
             for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
-                const P2Item it = p2_decode(p, p2_item(p, k));
+                P2Item it;
+                if (REGA && p.segs) {
+                    it.cls = __ldg(p2_seg_group(p, k)) >> 24;
+                    it.n0 = (k % p.nblocks) * p.n_tile;
+                    it.ntaps = p.cls_ntaps[it.cls];
+                } else {
+                    it = p2_decode(p, p2_item(p, k));
+                }
                 for (int cc = 0; cc < nchunks; ++cc)
                     for (int tap = 0; tap < it.ntaps; ++tap) {
                         { const long long t0 = p2_tick<PROFILE>(); mbar_wait<REGA>(&b_empty[S], bph ^ 1u); p2_tock<PROFILE>(clk[kProfBEmpty], t0); }
@@ -304,7 +346,8 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
         const uint32_t copy_lo = (uint32_t)(p.copy_bytes >> 4), patch_sz = (uint32_t)(p.patch_bytes >> 4);
         // REGA: lane l gives ldmatrix the address of row l % 8 of matrix l / 8 -- matrices 0, 1 = tile rows 0-7, 8-15 of this warp's
         // 16 (one v row of 8 u each), matrices 2, 3 the same rows 16 bytes on.  Its patch row before the tap's shift, and 16-byte chunk:
-        const uint32_t a_row = (uint32_t)((wg * 8 + wq * 2 + ((lane >> 3) & 1)) * p.pitch_u + (lane & 7)), a_chunk = (uint32_t)(lane >> 4);
+        // (segments: the first row of slot v instead of tile v row v)
+        const uint32_t a_row = (uint32_t)((wg * 8 + wq * 2 + ((lane >> 3) & 1)) * p.slot_rows + (lane & 7)), a_chunk = (uint32_t)(lane >> 4);
         const uint32_t patches_u32 = smem_u32(patches);
         float amax_in = 0.f, s_in = 1.f;
         if constexpr (MODE == kP2Planes) { amax_in = __ldg(p.in_info); s_in = __ldg(p.in_info + 1); }
@@ -321,7 +364,8 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
         for (int k = blockIdx.x; k < nitems; k += gridDim.x) {
             const long long t_item = p2_tick<PROFILE>();
             const int g = p2_item(p, k);
-            const int cls = p.cls_order[g / per_cls];
+            const int *grp = REGA && p.segs ? p2_seg_group(p, k) : nullptr;
+            const int cls = grp ? __ldg(grp) >> 24 : p.cls_order[g / per_cls];
             const int ntaps = p.cls_ntaps[cls];
             const uint32_t *aoff = s_aoff + cls * 9;
             // acc[0, kAcc): cross a_hi x b_lo + a_lo x b_hi, acc[kAcc, NT): main a_hi x b_hi -- the fragment of an m64n(2 NT) over the
@@ -450,6 +494,9 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
                     if (++pb == p.npatch) { pb = 0; pph ^= 1u; }
                 }
             }
+            // segments: the entries of this thread's two slots (rows r0 and r0 + 8 below), loaded while the last wgmmas drain
+            int seg_e[2] = {-1, -1};
+            if (grp) { seg_e[0] = __ldg(grp + wg * 8 + wq * 2); seg_e[1] = __ldg(grp + wg * 8 + wq * 2 + 1); }
             { const long long t0 = p2_tick<PROFILE>(); wgmma_wait<0>(); p2_tock<PROFILE>(clk[kProfMmaWait], t0); }
             const long long t_epi = p2_tick<PROFILE>();
             wgmma_fence_regs<NT>(acc);
@@ -461,7 +508,7 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
             // each quad of lanes (one row) gives every lane 8 whole channels, stored 16 bytes at a time
 #pragma unroll
             for (int i = 0; i < kAcc; ++i) acc[i] = acc[kAcc + i] + acc[i];      // main + cross
-            const P2Item it = p2_decode(p, g);
+            P2Item it = grp ? P2Item{cls, (k % p.nblocks) * p.n_tile, 0, 0, 0, ntaps} : p2_decode(p, g);
             const int q = lane & 3;
             const int r0 = wg * 64 + wq * 16 + (lane >> 2);
             bool rows_ok[2];
@@ -470,6 +517,10 @@ __global__ void __launch_bounds__(REGA ? kP2ThreadsRegA : kP2Threads, 1) bev_con
             for (int h = 0; h < 2; ++h) {
                 const int r = r0 + 8 * h;
                 const int lv = r / kP2TileU, lu = r % kP2TileU;
+                if (grp) {      // slot lv holds segment seg_e[h]: its pixels along u are this item's rows 8 lv .. 8 lv + 7
+                    const P2Seg sg = p2_seg(p, seg_e[h]);
+                    it.b = seg_e[h] >= 0 ? sg.b : p.batch; it.u0 = sg.u0; it.v0 = sg.v - lv;
+                }
                 const int gu = it.u0 + lu, gv = it.v0 + lv;
                 rows_ok[h] = it.b < p.batch && gu < p.grid_u && gv < p.grid_v;      // the same in the four lanes of a quad
                 const int ou = gu * p.out_stride + p.cls_off_u[it.cls], ov = gv * p.out_stride + p.cls_off_v[it.cls];
@@ -624,8 +675,12 @@ static int p2_geometry(P2Geometry &g, int batch, int grid_h, int grid_w, int cou
 // The launch plan: work-item geometry (p2_geometry), the patch copies and every (class, tap)'s copy, row and weight tap, and the
 // shared-memory split between the patch buffers and the weight-stage ring.  Reads p.batch, p.cin, p.cout and p.in_stride, fills the
 // plan fields of p and *smem (dynamic shared memory bytes), or returns SESSD_EINVAL for a launch the kernel cannot run.  Host only.
-static int p2_plan(P2Params &p, const P2Taps *cls, int nclass, int grid_h, int grid_w, int cout_pad, int mode, bool reg_a, int *smem) {
+// segs (register A only): the items are segment groups (kP2SegHeader): each of the 16 slots gets its own window of the taps' v extent
+// x pitch_u rows, padded to whole 512-byte swizzle periods, and the launch always keeps two patch buffers.
+static int p2_plan(P2Params &p, const P2Taps *cls, int nclass, int grid_h, int grid_w, int cout_pad, int mode, bool reg_a, int *smem,
+                   bool segs = false) {
     if (reg_a && (mode != kP2Planes || p.in_stride != 1)) return SESSD_EINVAL;
+    if (segs && !reg_a) return SESSD_EINVAL;
     if (p.cin < 64 || p.cin % 64) return SESSD_EINVAL;      // whole 64-channel groups
     P2Geometry g;
     if (p2_geometry(g, p.batch, grid_h, grid_w, p.cout, cout_pad, cls, nclass)) return SESSD_EINVAL;
@@ -682,15 +737,22 @@ static int p2_plan(P2Params &p, const P2Taps *cls, int nclass, int grid_h, int g
         }
     }
     p.copy_bytes = (p.rows_v * p.pitch_u * 64 + 511) & ~511;      // whole 512-byte swizzle periods: every copy starts one
+    p.slot_rows = p.pitch_u;
+    if (segs) {
+        const int win = (p.rows_v - kP2TileV + 1) * p.pitch_u;       // rows of one segment's window
+        p.slot_rows = (win + 7) & ~7;
+        p.copy_bytes = kP2SegSlots * p.slot_rows * 64;
+    }
     p.patch_bytes = p.ncopies * 2 * p.copy_bytes;
     // fp32 staging (split mode): 32 channels = 128-byte rows
     p.staging_bytes = mode == kP2Planes ? 0 : p.ncopies * p.rows_v * kP2TileU * kP2Chunk * 4;
     p.load_bytes = mode == kP2Planes ? p.ncopies * 2 * p.rows_v * p.pitch_u * 64 : p.staging_bytes;
+    if (segs) p.load_bytes = (p.rows_v - kP2TileV + 1) * p.pitch_u * 64;      // one window of one plane
     const int per_buf = p.patch_bytes + p.staging_bytes, bstage = 2 * p.n_tile * 64;
     // after the ring and the patch buffers: barriers and tap offsets (1536 B with the 1 KB alignment slack), then scale / shift
     const int tail = 1536 + 16 + 2 * 4 * p.cout;
     // two patch buffers when kP2BStages weight stages fit next to them, else one; then every stage that fits (>= 2), up to kP2MaxBStages
-    p.npatch = (kP2BStages * bstage + tail + 2 * per_buf <= kP2MaxSmem) ? 2 : 1;
+    p.npatch = (segs || kP2BStages * bstage + tail + 2 * per_buf <= kP2MaxSmem) ? 2 : 1;
     p.bstage_bytes = bstage;
     p.bstages = min((kP2MaxSmem - tail - p.npatch * per_buf) / bstage, kP2MaxBStages);
     if (p.bstages < 2) return SESSD_EINVAL;
@@ -713,9 +775,12 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
     if (((uintptr_t)d_scale | (uintptr_t)d_shift | (uintptr_t)d_residual | (uintptr_t)d_out_f32 | (uintptr_t)d_out_planes) & 15)
         return SESSD_EINVAL;
     int smem = 0;
-    if (p2_plan(p, cls, nclass, grid_h, grid_w, cout_pad, MODE, reg_a, &smem)) return SESSD_EINVAL;
+    if (p.items && p.segs) return SESSD_EINVAL;
+    if (p2_plan(p, cls, nclass, grid_h, grid_w, cout_pad, MODE, reg_a, &smem, p.segs != nullptr)) return SESSD_EINVAL;
     // a skip-plan record numbers the items of the width the runner packs: any other width decodes them to other classes / n-blocks
-    if (p.items && cout_pad != div_up(p.cout, p.n_tile) * p.n_tile) return SESSD_EINVAL;
+    if ((p.items || p.segs) && cout_pad != div_up(p.cout, p.n_tile) * p.n_tile) return SESSD_EINVAL;
+    // segment entries hold the segment index in 24 bits
+    if (p.segs && (long long)p.batch * p.grid_v * p.tiles_u >= (1 << 24)) return SESSD_EINVAL;
     const int s = p.in_stride;
     CUtensorMap map_a, map_b;
     if (MODE != kP2Planes) {   // fp32 NHWC [B][H][W][C] viewed as {C, U, V, B, 1}, staged unswizzled
@@ -734,7 +799,9 @@ static int launch_p2(const void *d_in_planes, int in_h, int in_w, const float *d
                                     (cuuint64_t)p.batch, 2};
         const cuuint64_t strides[4] = {p.u_is_x ? row_w : row_h, p.u_is_x ? row_h : row_w, (cuuint64_t)in_h * in_w * p.cin * 2,
                                        (cuuint64_t)p.batch * in_h * in_w * p.cin * 2};
-        const cuuint32_t box[5] = {(cuuint32_t)kP2Chunk, (cuuint32_t)(p.pitch_u * s), (cuuint32_t)(p.rows_v * s), 1, 1};
+        // segments: one window of the taps' v extent per box
+        const int box_v = p.segs ? p.rows_v - kP2TileV + 1 : p.rows_v;
+        const cuuint32_t box[5] = {(cuuint32_t)kP2Chunk, (cuuint32_t)(p.pitch_u * s), (cuuint32_t)(box_v * s), 1, 1};
         const cuuint32_t estr[5] = {1, (cuuint32_t)s, (cuuint32_t)s, 1, 1};
         int rc = encode_map_nd(&map_a, d_in_planes, 5, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_64B);
         if (rc) return rc;
@@ -805,13 +872,14 @@ template <int MODE, int PROBE = kP2NoProbe>
 static int p2_conv(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                    const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                    float *d_out_f32, void *d_out_planes, float *d_out_info, const sessd_conv_desc *desc, void *stream,
-                   const int *d_items = nullptr, long long *d_prof = nullptr, bool smem_a = false) {
+                   const int *d_items = nullptr, long long *d_prof = nullptr, bool smem_a = false, const int *d_segs = nullptr) {
     if (!desc || (PROBE != kP2NoProbe && !d_prof)) return SESSD_EINVAL;
     const sessd_conv_desc &d = *desc;
     P2Params p;
     P2Taps t;
     if (p2_conv_params(d, p, t)) return SESSD_EINVAL;
     p.items = d_items;
+    p.segs = d_segs;
     p.prof = d_prof;
     return launch_p2<MODE, PROBE>(d_in_planes, d.in_h, d.in_w, d_in_info, d_weight_h2, d.ntaps, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
                      shift_max, d_out_f32, d_out_planes, d_out_info, p, &t, 1, d.grid_h, d.grid_w, MODE == kP2Planes && d.in_stride == 1 && !smem_a,
@@ -822,12 +890,13 @@ template <int MODE, int PROBE = kP2NoProbe>
 static int p2_deconv(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad, const float *d_scale,
                      const float *d_shift, const float *d_residual, const float *d_resid_info, float gain, float shift_max,
                      float *d_out_f32, void *d_out_planes, float *d_out_info, int batch, int in_h, int in_w, int cin, int cout,
-                     int relu, void *stream, const int *d_items = nullptr, long long *d_prof = nullptr) {
+                     int relu, void *stream, const int *d_items = nullptr, long long *d_prof = nullptr, const int *d_segs = nullptr) {
     if (PROBE != kP2NoProbe && !d_prof) return SESSD_EINVAL;
     P2Params p;
     P2Taps cls[4];
     p2_deconv_params(batch, in_h, in_w, cin, cout, relu, p, cls);
     p.items = d_items;
+    p.segs = d_segs;
     p.prof = d_prof;
     return launch_p2<MODE, PROBE>(d_in_planes, in_h, in_w, d_in_info, d_weight_h2, 9, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain, shift_max,
                      d_out_f32, d_out_planes, d_out_info, p, cls, 4, in_h, in_w, MODE == kP2Planes, stream);

@@ -32,19 +32,20 @@ extern "C" int sessd_bev_deconv_h2(const float *d_in, const void *d_weight_h2, i
 extern "C" int sessd_bev_conv_p2_profile(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
                                          const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
                                          float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info,
-                                         const sessd_conv_desc *desc, const int *d_items, long long *d_prof, void *stream) {
+                                         const sessd_conv_desc *desc, const int *d_items, const int *d_segs, long long *d_prof,
+                                         void *stream) {
     return p2_conv<kP2Planes, kP2ProbeClocks>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
-                                              shift_max, d_out_f32, d_out_planes, d_out_info, desc, stream, d_items, d_prof);
+                                              shift_max, d_out_f32, d_out_planes, d_out_info, desc, stream, d_items, d_prof, false, d_segs);
 }
 
 extern "C" int sessd_bev_deconv_p2_profile(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
                                            const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
                                            float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info, int batch,
-                                           int in_h, int in_w, int cin, int cout, int relu, const int *d_items, long long *d_prof,
-                                           void *stream) {
+                                           int in_h, int in_w, int cin, int cout, int relu, const int *d_items, const int *d_segs,
+                                           long long *d_prof, void *stream) {
     return p2_deconv<kP2Planes, kP2ProbeClocks>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
                                                 shift_max, d_out_f32, d_out_planes, d_out_info, batch, in_h, in_w, cin, cout, relu, stream,
-                                                d_items, d_prof);
+                                                d_items, d_prof, d_segs);
 }
 
 // The loader-only probe: the launch of sessd_bev_conv_p2_profile with consumers that wait on the full barriers and release them,
@@ -56,6 +57,16 @@ extern "C" int sessd_bev_conv_p2_loads(const void *d_in_planes, const float *d_i
                                        const sessd_conv_desc *desc, const int *d_items, int smem_a, long long *d_prof, void *stream) {
     return p2_conv<kP2Planes, kP2ProbeLoads>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
                                              shift_max, d_out_f32, d_out_planes, d_out_info, desc, stream, d_items, d_prof, smem_a != 0);
+}
+
+// The loader-only probe on a segment record (d_segs, sessd_bev_skip_plan): the segment windows' patch layout of a stride-1 conv.
+extern "C" int sessd_bev_conv_p2_seg_loads(const void *d_in_planes, const float *d_in_info, const void *d_weight_h2, int cout_pad,
+                                           const float *d_scale, const float *d_shift, const float *d_residual, const float *d_resid_info,
+                                           float gain, float shift_max, float *d_out_f32, void *d_out_planes, float *d_out_info,
+                                           const sessd_conv_desc *desc, const int *d_segs, long long *d_prof, void *stream) {
+    if (!d_segs) return SESSD_EINVAL;
+    return p2_conv<kP2Planes, kP2ProbeLoads>(d_in_planes, d_in_info, d_weight_h2, cout_pad, d_scale, d_shift, d_residual, d_resid_info, gain,
+                                             shift_max, d_out_f32, d_out_planes, d_out_info, desc, stream, nullptr, d_prof, false, d_segs);
 }
 
 // The plan p2_conv / p2_deconv would launch with (p2_plan), word order in sessd_b200_lab.h.  No device call.

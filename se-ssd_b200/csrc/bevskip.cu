@@ -14,6 +14,17 @@
 //   * the skipped (class, tile) pairs are listed.
 // sessd_bev_skip_fill copies, after the launch, the representative's pixel at the same tile position into every skipped pixel.  Tile
 // origins are multiples of 8 (u) and 16 (v) along the class grid, so that pixel has the same parity.
+//
+// Most pixels of the tiles that run are constant too, so the stride-1 launches (the register-A path of bev_conv_p2, which addresses
+// A per 8-row matrix) run segments instead: 8 pixels along u in one v row.  The plan kernel copies every frame's bit maps into the
+// segment buffer (a separate record per launch, next to the tile record, which stays as it is); bev_skip_seg_kernel then, one CTA per
+// launch so that the work runs in parallel rather than on the plan kernel's single CTA:
+//   * flags every segment that holds a non-constant pixel or leaves the map;
+//   * picks two representatives per class, the first all-constant segment of each v parity (a segment starts at a multiple of 8 along u,
+//     but at any v, and the maps after the deconvs have period 2);
+//   * packs the live segments and the representatives 16 to a group, per class in the launcher's heavy-first order, by ascending segment
+//     index (a class's last group is padded with -1);
+//   * lists the skipped (class, segment) pairs, which sessd_bev_skip_fill_segs fills from the representative of their v parity.
 #include "bevconv_p2.cuh"
 
 namespace sessd {
@@ -22,6 +33,13 @@ namespace sessd {
 enum {
     kRecCount = 0, kRecSkipped = 1, kRecNclass = 2, kRecTiles = 3, kRecTilesU = 4, kRecTilesV = 5, kRecUisX = 6, kRecOutStride = 7,
     kRecOutH = 8, kRecOutW = 9, kRecBatch = 10, kRecOffY = 11, kRecOffX = 15, kRecRep = 19, kRecSkipOff = 23, kRecFlagOff = 24
+};
+// segment record header (int32 words; the groups start at kP2SegHeader, where bev_conv_p2_kernel reads them, then the skipped
+// (class * segments + segment) entries and the per-(class, segment) flags); representatives at kSegRep + 2 class + v parity
+enum {
+    kSegCount = 0, kSegSkipped = 1, kSegGroups = 2, kSegNclass = 3, kSegPerClass = 4, kSegTilesU = 5, kSegGridV = 6, kSegUisX = 7,
+    kSegOutStride = 8, kSegOutH = 9, kSegOutW = 10, kSegBatch = 11, kSegOffY = 12, kSegOffX = 16, kSegRep = 20, kSegSkipOff = 28,
+    kSegFlagOff = 29
 };
 
 // bit maps of the plan kernel: the neck input, every layer output (t0 = x0 and t1 = x1 pixel for pixel: 1x1 convs) and two scratch maps
@@ -34,10 +52,15 @@ struct SkipLaunch : P2Geometry {             // the launcher's work items (p2_ge
     int map;                                   // bit map of the launch's output
     int out_stride, out_h, out_w;
     int rec;                                   // word offset of the launch record
+    int seg;                                   // word offset of the segment record, -1: tiles only (the stride-2 conv)
+    int nseg, max_groups;                      // segments per class (batch * grid_v * tiles_u), groups of a record at most
 };
 
 struct SkipPlan {
     int batch, depth, h, w, h2, w2, nwf, nwh;  // nwf / nwh: 32-bit words per row of a full / half resolution map
+    long long seg_words;                       // int32 words of the segment records and, from map_off, of every frame's bit maps
+    long long map_off;
+    int frame_words;                           // words of one frame's bit maps (the plan kernel's shared memory, same layout)
     SkipLaunch l[kSkipLaunches];
 };
 
@@ -73,10 +96,19 @@ static long long skip_plan(SkipPlan &P, int batch, int h, int w) {
                  | skip_launch(L[11], kMO1, batch, h, w, h, w, 128, false)     // conv_1.0
                  | skip_launch(L[12], kMOut, batch, h, w, h, w, 24, false);    // head (1x1 on the fused map)
     long long words = 0;
+    P.seg_words = 0;
     for (int i = 0; i < kSkipLaunches; ++i) {
         L[i].rec = (int)words;
         words += kP2ItemsHeader + L[i].total + 2LL * L[i].nclass * L[i].tiles;
+        L[i].nseg = batch * L[i].grid_v * L[i].tiles_u;
+        L[i].max_groups = L[i].nclass * div_up(L[i].nseg, kP2SegSlots);
+        L[i].seg = i == 3 ? -1 : (int)P.seg_words;
+        if (L[i].seg >= 0) P.seg_words += kP2SegHeader + (long long)kP2SegSlots * L[i].max_groups + 2LL * L[i].nclass * L[i].nseg;
     }
+    P.frame_words = kNumFullMaps * h * P.nwf + (kNumMaps - kNumFullMaps) * P.h2 * P.nwh;
+    P.map_off = P.seg_words;
+    P.seg_words += (long long)batch * P.frame_words;
+    if (P.seg_words >= (1LL << 31) || L[0].nseg >= (1 << 24)) return 0;
     return rc ? 0 : words;
 }
 
@@ -152,7 +184,8 @@ __device__ int skip_compact(int n, Pred pred, int *out, int *s_scan) {
     return base;
 }
 
-__global__ void __launch_bounds__(kSkipThreads) bev_skip_plan_kernel(const uint2 *__restrict__ bitmap, int *__restrict__ plan, SkipPlan P) {
+__global__ void __launch_bounds__(kSkipThreads) bev_skip_plan_kernel(const uint2 *__restrict__ bitmap, int *__restrict__ plan,
+                                                                    int *__restrict__ segs, SkipPlan P) {
     extern __shared__ uint32_t s_bits[];
     __shared__ int s_scan[33], s_rep[4];
     BitMap m[kNumMaps];
@@ -230,6 +263,8 @@ __global__ void __launch_bounds__(kSkipThreads) bev_skip_plan_kernel(const uint2
                 flags[c * L.tiles + b * per_frame + tf] = run ? 1 : 0;
             }
         }
+        // the frame's maps, for bev_skip_seg_kernel to flag the segments from (in parallel, off this CTA)
+        for (int i = threadIdx.x; i < P.frame_words; i += blockDim.x) segs[P.map_off + (long long)b * P.frame_words + i] = (int)s_bits[i];
         __syncthreads();
     }
     // per launch: representatives, the item list, the skipped list, the header
@@ -263,6 +298,121 @@ __global__ void __launch_bounds__(kSkipThreads) bev_skip_plan_kernel(const uint2
             rec[kRecFlagOff] = kP2ItemsHeader + L.total + L.nclass * L.tiles;
         }
         __syncthreads();
+    }
+}
+
+// one CTA per launch with a segment record: the flags from the plan kernel's maps, representatives, the groups, the skipped list, the
+// header
+__global__ void __launch_bounds__(kSkipThreads) bev_skip_seg_kernel(int *__restrict__ segs, SkipPlan P) {
+    __shared__ int s_scan[33], s_rep[8];
+    const SkipLaunch &L = P.l[blockIdx.x];
+    if (L.seg < 0) return;
+    int *rec = segs + L.seg;
+    int *groups = rec + kP2SegHeader, *skipped = groups + kP2SegSlots * L.max_groups;
+    int *flags = skipped + L.nclass * L.nseg;
+    const int nseg = L.nseg;
+    // flags: a segment runs when it holds a non-constant pixel or leaves the map
+    const bool full = L.map < kNumFullMaps;
+    const int map_word = full ? L.map * P.h * P.nwf : kNumFullMaps * P.h * P.nwf + (L.map - kNumFullMaps) * P.h2 * P.nwh;
+    const int seg_frame = L.grid_v * L.tiles_u;
+    for (int b = 0; b < P.batch; ++b) {
+        const BitMap o{reinterpret_cast<uint32_t *>(segs + P.map_off + (long long)b * P.frame_words + map_word), full ? P.h : P.h2,
+                       full ? P.w : P.w2, full ? P.nwf : P.nwh};
+        for (int idx = threadIdx.x; idx < L.nclass * seg_frame; idx += blockDim.x) {
+            const int c = idx / seg_frame, sf = idx - c * seg_frame;
+            const int v = sf / L.tiles_u, u0 = (sf - v * L.tiles_u) * kP2TileU;
+            bool live = u0 + kP2TileU > L.grid_u;                        // partial segment
+            if (!live && L.out_stride == 1 && L.u_is_x) {                // one aligned 8-bit field
+                live = (o.w[v * o.nw + (u0 >> 5)] >> (u0 & 31)) & 0xFFu;
+            } else {
+                for (int i = 0; i < kP2TileU && !live; ++i) {
+                    const int ou = (u0 + i) * L.out_stride + L.off_u[c], ov = v * L.out_stride + L.off_v[c];
+                    live = L.u_is_x ? o.get(ov, ou) : o.get(ou, ov);
+                }
+            }
+            flags[c * nseg + b * seg_frame + sf] = live ? 1 : 0;
+        }
+    }
+    __syncthreads();
+    auto parity = [&](int s) { return (s / L.tiles_u) % L.grid_v & 1; };
+    if (threadIdx.x < 8) s_rep[threadIdx.x] = 0x7FFFFFFF;
+    __syncthreads();
+    for (int e = threadIdx.x; e < L.nclass * nseg; e += blockDim.x)
+        if (!flags[e]) {
+            const int c = e / nseg, s = e - c * nseg;
+            atomicMin(&s_rep[2 * c + parity(s)], s);
+        }
+    __syncthreads();
+    int ngroups = 0;
+    for (int rank = 0; rank < L.nclass; ++rank) {
+        const int c = L.order[rank];
+        int *g = groups + kP2SegSlots * ngroups;
+        const int n = skip_compact(nseg, [&](int s) {
+            return flags[c * nseg + s] != 0 || s == s_rep[2 * c] || s == s_rep[2 * c + 1];
+        }, g, s_scan);
+        const int ng = (n + kP2SegSlots - 1) / kP2SegSlots;
+        for (int j = threadIdx.x; j < ng * kP2SegSlots; j += blockDim.x) g[j] = j < n ? (c << 24) | g[j] : -1;
+        ngroups += ng;
+        __syncthreads();
+    }
+    const int nskip = skip_compact(L.nclass * nseg, [&](int e) {
+        const int c = e / nseg, s = e - c * nseg;
+        return flags[e] == 0 && s != s_rep[2 * c + parity(s)];
+    }, skipped, s_scan);
+    if (threadIdx.x == 0) {
+        rec[kSegCount] = ngroups * L.nblocks; rec[kSegSkipped] = nskip; rec[kSegGroups] = ngroups;
+        rec[kSegNclass] = L.nclass; rec[kSegPerClass] = nseg; rec[kSegTilesU] = L.tiles_u; rec[kSegGridV] = L.grid_v;
+        rec[kSegUisX] = L.u_is_x; rec[kSegOutStride] = L.out_stride; rec[kSegOutH] = L.out_h; rec[kSegOutW] = L.out_w;
+        rec[kSegBatch] = P.batch;
+        for (int c = 0; c < 4; ++c) {
+            rec[kSegOffY + c] = L.u_is_x ? L.off_v[c] : L.off_u[c]; rec[kSegOffX + c] = L.u_is_x ? L.off_u[c] : L.off_v[c];
+            for (int par = 0; par < 2; ++par)
+                rec[kSegRep + 2 * c + par] = c < L.nclass && s_rep[2 * c + par] != 0x7FFFFFFF ? s_rep[2 * c + par] : -1;
+        }
+        rec[kSegSkipOff] = kP2SegHeader + kP2SegSlots * L.max_groups;
+        rec[kSegFlagOff] = kP2SegHeader + kP2SegSlots * L.max_groups + L.nclass * nseg;
+    }
+}
+
+// every pixel of a skipped segment <- the pixel at the same position of the representative of its class and v parity
+__global__ void __launch_bounds__(256) bev_skip_fill_segs_kernel(const int *__restrict__ rec, float *__restrict__ out_f32,
+                                                                 __half *__restrict__ out_planes, int cout) {
+    const int nskip = __ldg(rec + kSegSkipped);
+    const int nseg = __ldg(rec + kSegPerClass), tiles_u = __ldg(rec + kSegTilesU), grid_v = __ldg(rec + kSegGridV);
+    const int u_is_x = __ldg(rec + kSegUisX), os = __ldg(rec + kSegOutStride), out_h = __ldg(rec + kSegOutH), out_w = __ldg(rec + kSegOutW);
+    const long long plane_stride = (long long)__ldg(rec + kSegBatch) * out_h * out_w * cout;
+    const int *skipped = rec + __ldg(rec + kSegSkipOff);
+    // (destination, source) pixel of position lu of skipped entry e
+    auto pixels = [&](int e, int lu, size_t &dst, size_t &src) {
+        const int ent = __ldg(skipped + e), c = ent / nseg, s = ent - c * nseg;
+        const int oy0 = __ldg(rec + kSegOffY + c), ox0 = __ldg(rec + kSegOffX + c);
+        auto pixel = [&](int ss) -> size_t {
+            const int rest = ss / tiles_u, v = rest % grid_v, b = rest / grid_v, gu = (ss - rest * tiles_u) * kP2TileU + lu;
+            const int gy = u_is_x ? v : gu, gx = u_is_x ? gu : v;
+            return ((size_t)b * out_h + (size_t)(gy * os + oy0)) * out_w + (size_t)(gx * os + ox0);
+        };
+        dst = pixel(s);
+        src = pixel(__ldg(rec + kSegRep + 2 * c + ((s / tiles_u) % grid_v & 1)));
+    };
+    const int stride = gridDim.x * blockDim.x, tid = blockIdx.x * blockDim.x + threadIdx.x;
+    if (out_f32) {
+        const int q = cout / 4, n = nskip * kP2TileU * q;
+        for (int i = tid; i < n; i += stride) {
+            const int px = i / q, j = i - px * q;
+            size_t dst, src;
+            pixels(px / kP2TileU, px % kP2TileU, dst, src);
+            reinterpret_cast<float4 *>(out_f32 + dst * cout)[j] = reinterpret_cast<const float4 *>(out_f32 + src * cout)[j];
+        }
+    }
+    if (out_planes) {
+        const int q = cout / 8, n = nskip * kP2TileU * q;
+        for (int i = tid; i < 2 * n; i += stride) {
+            const int pl = i / n, k = i - pl * n, px = k / q, j = k - px * q;
+            size_t dst, src;
+            pixels(px / kP2TileU, px % kP2TileU, dst, src);
+            reinterpret_cast<uint4 *>(out_planes + pl * plane_stride + dst * cout)[j] =
+                reinterpret_cast<const uint4 *>(out_planes + pl * plane_stride + src * cout)[j];
+        }
     }
 }
 
@@ -317,20 +467,30 @@ extern "C" long long sessd_bev_skip_plan_words(int batch, int h, int w, int *off
     return words;
 }
 
-// d_bitmap_index: the last sparse level's bitmap index (grid = that level: shape = {D, h, w}); d_plan: sessd_bev_skip_plan_words(B, h, w)
-extern "C" int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, int *d_plan, void *stream) {
-    if (!d_bitmap_index || !d_plan || grid.shape[0] < 1) return SESSD_EINVAL;
+extern "C" long long sessd_bev_skip_seg_words(int batch, int h, int w, int *offsets) {
+    SkipPlan P;
+    if (!skip_plan(P, batch, h, w)) return 0;
+    if (offsets)
+        for (int i = 0; i < kSkipLaunches; ++i) offsets[i] = P.l[i].seg;
+    return P.seg_words;
+}
+
+// d_bitmap_index: the last sparse level's bitmap index (grid = that level: shape = {D, h, w}); d_plan: sessd_bev_skip_plan_words(B, h, w),
+// d_segs: sessd_bev_skip_seg_words(B, h, w)
+extern "C" int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, int *d_plan, int *d_segs, void *stream) {
+    if (!d_bitmap_index || !d_plan || !d_segs || grid.shape[0] < 1) return SESSD_EINVAL;
     SkipPlan P;
     if (!skip_plan(P, grid.batch, grid.shape[1], grid.shape[2])) return SESSD_EINVAL;
     P.depth = grid.shape[0];
-    const int smem = 4 * (kNumFullMaps * P.h * P.nwf + (kNumMaps - kNumFullMaps) * P.h2 * P.nwh);
+    const int smem = 4 * P.frame_words;
     if (smem > 200 * 1024) return SESSD_EINVAL;
     static int attr_smem = 48 * 1024;     // opt in to what the maps need (the static shared memory counts against the same limit)
     if (smem > attr_smem) {
         SESSD_CUDA_TRY(cudaFuncSetAttribute(bev_skip_plan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         attr_smem = smem;
     }
-    SESSD_LAUNCH(bev_skip_plan_kernel, 1, kSkipThreads, smem, (cudaStream_t)stream, (const uint2 *)d_bitmap_index, d_plan, P);
+    SESSD_LAUNCH(bev_skip_plan_kernel, 1, kSkipThreads, smem, (cudaStream_t)stream, (const uint2 *)d_bitmap_index, d_plan, d_segs, P);
+    SESSD_LAUNCH(bev_skip_seg_kernel, kSkipLaunches, kSkipThreads, 0, (cudaStream_t)stream, d_segs, P);
     return last_error();
 }
 
@@ -338,5 +498,12 @@ extern "C" int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, 
 extern "C" int sessd_bev_skip_fill(const int *d_record, float *d_out_f32, void *d_out_planes, int cout, void *stream) {
     if (!d_record || (!d_out_f32 && !d_out_planes) || cout < 8 || cout % 8) return SESSD_EINVAL;
     SESSD_LAUNCH(bev_skip_fill_kernel, 2 * kNumSMs, 256, 0, (cudaStream_t)stream, d_record, d_out_f32, (__half *)d_out_planes, cout);
+    return last_error();
+}
+
+// after the launch that ran d_seg_record's segments: fill its skipped segments in d_out_f32 [B][H][W][cout] and / or d_out_planes
+extern "C" int sessd_bev_skip_fill_segs(const int *d_seg_record, float *d_out_f32, void *d_out_planes, int cout, void *stream) {
+    if (!d_seg_record || (!d_out_f32 && !d_out_planes) || cout < 8 || cout % 8) return SESSD_EINVAL;
+    SESSD_LAUNCH(bev_skip_fill_segs_kernel, 2 * kNumSMs, 256, 0, (cudaStream_t)stream, d_seg_record, d_out_f32, (__half *)d_out_planes, cout);
     return last_error();
 }

@@ -84,11 +84,13 @@ SIGNATURES = {
     "sessd_spconv_wgrad_cg": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
     "sessd_sparse_to_dense_indexed": (_i, [_vp, _i, _vp, _i, Grid, _vp, _vp]),
     "sessd_sparse_to_dense": (_i, [_vp, _vp, _vp, _i, _i, Grid, _vp, _vp]),
-    "sessd_bev_conv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp]),
-    "sessd_bev_deconv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "sessd_bev_conv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp, _vp]),
+    "sessd_bev_deconv_p2": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "sessd_bev_skip_plan_words": (_ll, [_i, _i, _i, _I3]),
-    "sessd_bev_skip_plan": (_i, [_vp, Grid, _vp, _vp]),
+    "sessd_bev_skip_seg_words": (_ll, [_i, _i, _i, _I3]),
+    "sessd_bev_skip_plan": (_i, [_vp, Grid, _vp, _vp, _vp]),
     "sessd_bev_skip_fill": (_i, [_vp, _vp, _vp, _i, _vp]),
+    "sessd_bev_skip_fill_segs": (_i, [_vp, _vp, _vp, _i, _vp]),
     "sessd_bev_wgrad_items": (_i, [C.POINTER(ConvDesc)]),
     "sessd_bev_wgrad_workspace_bytes": (_sz, [C.POINTER(ConvDesc)]),
     "sessd_bev_wgrad": (_i, [_vp, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp, _sz, _vp]),
@@ -159,10 +161,13 @@ SIGNATURES = {
 LAB_SIGNATURES = {
     "sessd_bev_conv_h2": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp, _vp]),
     "sessd_bev_deconv_h2": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
-    "sessd_bev_conv_p2_profile": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp, _vp]),
+    "sessd_bev_conv_p2_profile": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp, _vp,
+                                       _vp]),
     "sessd_bev_deconv_p2_profile": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp,
-                                         _vp]),
+                                         _vp, _vp]),
     "sessd_bev_conv_p2_loads": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _i, _vp, _vp]),
+    "sessd_bev_conv_p2_seg_loads": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, C.POINTER(ConvDesc), _vp, _vp,
+                                         _vp]),
     "sessd_bev_p2_plan": (_i, [C.POINTER(ConvDesc), _i, _i, _i, _i, _I3]),
 }
 

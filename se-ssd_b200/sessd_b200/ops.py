@@ -366,46 +366,59 @@ def conv_gain(wp, scale):
 
 
 def bev_conv_p2(in_planes, in_info, weight_h2, scale, shift, residual, resid_info, gain, shift_max, out_f32, out_planes, out_info, desc,
-                items=None):
-    """items: optional launch record of a skip plan (BevSkipPlan.record): only the work items it lists run"""
+                items=None, segs=None):
+    """items: optional launch record of a skip plan (BevSkipPlan.record): only the work items it lists run; segs (stride 1, instead of
+    items): optional segment record (BevSkipPlan.seg_record): only the segments it lists run"""
     check(lib.sessd_bev_conv_p2(_p(in_planes), _p(in_info), _p(weight_h2), int(weight_h2.shape[2]), _p(scale), _p(shift), _p(residual),
                                 _p(resid_info), float(gain), float(shift_max), _p(out_f32), _p(out_planes), _p(out_info), C.byref(desc),
-                                _p(items), _st()), "sessd_bev_conv_p2")
+                                _p(items), _p(segs), _st()), "sessd_bev_conv_p2")
 
 
 def bev_deconv_p2(in_planes, in_info, weight_h2, scale, shift, residual, resid_info, gain, shift_max, out_f32, out_planes, out_info, relu=True,
-                  items=None):
+                  items=None, segs=None):
     _two, b, h, w, cin = in_planes.shape
     cout = (out_f32 if out_f32 is not None else out_planes).shape[-1]
     check(lib.sessd_bev_deconv_p2(_p(in_planes), _p(in_info), _p(weight_h2), int(weight_h2.shape[2]), _p(scale), _p(shift), _p(residual),
                                   _p(resid_info), float(gain), float(shift_max), _p(out_f32), _p(out_planes), _p(out_info), int(b), int(h),
-                                  int(w), int(cin), int(cout), int(bool(relu)), _p(items), _st()), "sessd_bev_deconv_p2")
+                                  int(w), int(cin), int(cout), int(bool(relu)), _p(items), _p(segs), _st()), "sessd_bev_deconv_p2")
 
 
 class BevSkipPlan:
     """Device buffer of the SSFA neck's constant-region skip plan (sessd_bev_skip_plan): one int32 record per neck launch, in the
     order of runners.SSFAPlanesRunner.SKIP_LAUNCHES.  Record layout (csrc/bevskip.cu): header of 32 words (0: items to run, 1: skipped
-    tiles, then the launch geometry), the work items to run, the skipped (class, tile) entries, the per-(class, tile) flags."""
+    tiles, then the launch geometry), the work items to run, the skipped (class, tile) entries, the per-(class, tile) flags.
+    Segment records (seg_buf, every launch but the stride-2 conv): header of 32 words (0: items to run, 1: skipped segments, 2: groups,
+    then the geometry and the representatives), groups of 16 segment entries, the skipped (class, segment) entries, the flags."""
 
     LAUNCHES = 13
 
     def __init__(self, batch, h, w, device):
-        offs = (C.c_int * self.LAUNCHES)()
+        offs, seg_offs = (C.c_int * self.LAUNCHES)(), (C.c_int * self.LAUNCHES)()
         words = lib.sessd_bev_skip_plan_words(int(batch), int(h), int(w), offs)
-        if words <= 0:
+        seg_words = lib.sessd_bev_skip_seg_words(int(batch), int(h), int(w), seg_offs)
+        if words <= 0 or seg_words <= 0:
             raise ValueError("no skip plan for a [%d, %d, %d] neck" % (batch, h, w))
-        self.offsets = list(offs)
+        self.offsets, self.seg_offsets = list(offs), list(seg_offs)
         self.buf = torch.zeros((int(words),), dtype=torch.int32, device=device)
+        self.seg_buf = torch.zeros((int(seg_words),), dtype=torch.int32, device=device)
 
     def record(self, i):
         return self.buf[self.offsets[i]:]
 
+    def seg_record(self, i):
+        """launch i's segment record, or None (the stride-2 conv runs tiles)"""
+        return self.seg_buf[self.seg_offsets[i]:] if self.seg_offsets[i] >= 0 else None
+
     def build(self, bitmap_index, grid):
         """bitmap_index / grid: the last sparse level's index (SpMiddleRunner.levels[-1]) -- grid.shape = (D, h, w)"""
-        check(lib.sessd_bev_skip_plan(_p(bitmap_index), grid, _p(self.buf), _st()), "sessd_bev_skip_plan")
+        check(lib.sessd_bev_skip_plan(_p(bitmap_index), grid, _p(self.buf), _p(self.seg_buf), _st()), "sessd_bev_skip_plan")
 
     def fill(self, i, out_f32, out_planes, cout):
         check(lib.sessd_bev_skip_fill(_p(self.record(i)), _p(out_f32), _p(out_planes), int(cout), _st()), "sessd_bev_skip_fill")
+
+    def fill_segs(self, i, out_f32, out_planes, cout):
+        check(lib.sessd_bev_skip_fill_segs(_p(self.seg_record(i)), _p(out_f32), _p(out_planes), int(cout), _st()),
+              "sessd_bev_skip_fill_segs")
 
 
 def bev_split_planes(x, info, planes):

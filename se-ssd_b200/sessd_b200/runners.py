@@ -320,7 +320,7 @@ class SSFAPlanesRunner:
     activations travel between the layers as fp16 (hi, lo) planes written by the producing epilogue (the main loops are pure
     TMA -> wgmma).  14 launches per forward: 13 convs (the stride-2 conv included)
     + the attention fusion; + abs-max and split when the input arrives as fp32 (module API) instead of planes (FrameEngine).
-    With skip_constant and the sparse occupancy (FrameEngine): + one skip-plan launch and one fill launch after each conv / deconv."""
+    With skip_constant and the sparse occupancy (FrameEngine): + the skip plan's two launches and one fill launch after each conv / deconv."""
 
     HEAD_STRIDE = 24
     # info slots (each {abs-max, scale}); the whole table is zeroed once per forward
@@ -359,21 +359,24 @@ class SSFAPlanesRunner:
         ops.bev_split_planes(x, self._info(name), self.planes[name])
 
     def _launch(self, L, skip=False):
-        """launch L from its input planes into its output planes or fp32 buffer.  skip: run the work items of this launch's skip-plan
-        record, then fill the skipped tiles"""
+        """launch L from its input planes into its output planes or fp32 buffer.  skip: run the segments of this launch's segment
+        record (the stride-2 conv: the work items of its tile record), then fill the skipped segments (tiles)"""
         q = self.params[L.name]
         out_f32, out_planes = (self.buf[L.dst], None) if L.f32 else (None, self.planes[L.dst])
         resid, resid_info = (self.buf[L.residual], self._info(L.residual)) if L.residual else (None, None)
         i = self.SKIP_LAUNCHES.index(L.name)
-        rec = self.skip.record(i) if skip else None
+        segs = self.skip.seg_record(i) if skip else None
+        rec = self.skip.record(i) if skip and segs is None else None
         if L.kind == "conv":
             d = launch_desc(L, self.batch, *ssfa_extents(L, self.h, self.w), q["taps"])
             ops.bev_conv_p2(self.planes[L.src], self._info(L.src), q["w"], q["scale"], q["shift"], resid, resid_info, q["gain"],
-                            q["shift_max"], out_f32, out_planes, self._info(L.dst), d, items=rec)
+                            q["shift_max"], out_f32, out_planes, self._info(L.dst), d, items=rec, segs=segs)
         else:
             ops.bev_deconv_p2(self.planes[L.src], self._info(L.src), q["w"], q["scale"], q["shift"], resid, resid_info, q["gain"],
-                              q["shift_max"], out_f32, out_planes, self._info(L.dst), L.relu, items=rec)
-        if skip:
+                              q["shift_max"], out_f32, out_planes, self._info(L.dst), L.relu, items=rec, segs=segs)
+        if segs is not None:
+            self.skip.fill_segs(i, out_f32, out_planes, L.cout)
+        elif skip:
             self.skip.fill(i, out_f32, out_planes, L.cout)
 
     def forward(self, x=None, mark=None, occupancy=None):
