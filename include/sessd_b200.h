@@ -236,10 +236,14 @@ int sessd_bev_deconv_p2(const void *d_in_planes, const float *d_in_info, const v
  * word offset of every launch record.  The same plan also lists, in d_segs, the live segments (8 pixels along the launch's u in one
  * v row) of every stride-1 launch, packed 16 to a work item: the conv / deconv run them (d_segs = the launch's segment record) and
  * sessd_bev_skip_fill_segs fills the other segments.  sessd_bev_skip_seg_words: int32 words of d_segs; offsets[13] <- the word offset
- * of every segment record, -1 for the stride-2 launch (tiles only). */
+ * of every segment record, -1 for the stride-2 launch (tiles only).  These three plan the one-task head (24 channels); the _head
+ * variants plan a head launch of head_cout channels (24 per task of a multi-task head, a multiple of 8). */
 long long sessd_bev_skip_plan_words(int batch, int h, int w, int *offsets);
 long long sessd_bev_skip_seg_words(int batch, int h, int w, int *offsets);
 int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, int *d_plan, int *d_segs, void *stream);
+long long sessd_bev_skip_plan_words_head(int batch, int h, int w, int head_cout, int *offsets);
+long long sessd_bev_skip_seg_words_head(int batch, int h, int w, int head_cout, int *offsets);
+int sessd_bev_skip_plan_head(const void *d_bitmap_index, sessd_grid grid, int head_cout, int *d_plan, int *d_segs, void *stream);
 int sessd_bev_skip_fill(const int *d_record, float *d_out_f32, void *d_out_planes, int cout, void *stream);
 int sessd_bev_skip_fill_segs(const int *d_seg_record, float *d_out_f32, void *d_out_planes, int cout, void *stream);
 /* Weight gradient of a BEV conv (csrc/bevgrad.cu; training of the neck and head, rpn_v1.py:135-210, mg_head_sessd.py:202-215):
@@ -309,7 +313,11 @@ typedef struct {
     int use_frustum;           /* apply the calib frustum filter (mg_head_sessd.py:1024-1030) */
     int nms_mode;              /* 0: rotate_nms (greedy, nms_iou_thresh, nms_ge); 1: DI-NMS (rotate_weighted_nms, constants below) */
     sessd_dinms_cfg dinms;     /* read in nms_mode 1 only: a zero-initialised config keeps rotate_nms */
+    int num_tasks;             /* T: one-class tasks of a MultiGroupHead (Car, Pedestrian, Cyclist); 0 or 1 = one task */
+    int task_stride;           /* T > 1: floats between two tasks' 22-float blocks in a pixel row (24) */
 } sessd_post_cfg;
+
+#define SESSD_POST_MAX_TASKS 64
 
 size_t sessd_postprocess_workspace_bytes(const sessd_post_cfg *cfg);
 
@@ -320,7 +328,15 @@ size_t sessd_postprocess_workspace_bytes(const sessd_post_cfg *cfg);
  * d_sel_anchor [batch, post_max] i32 (anchor index of each NMS-selected box, before frustum/range masks).
  * nms_mode 1 (DI-NMS): nms_pre_max <= SESSD_DINMS_MAX_PRE, and every "post_max" above is nms_pre_max (DI-NMS applies no post_max);
  * the boxes are the clusters' weighted averages, d_sel_anchor holds each emitted cluster's pick, d_aux[2] the emitted clusters and
- * d_aux[3] the loop's picks. */
+ * d_aux[3] the loop's picks.
+ * Several tasks (num_tasks = T > 1; one class and anchors_per_loc anchors per location each): task t's head floats start at
+ * t * task_stride of the pixel row (head_stride >= (T - 1) * task_stride + 22), its anchors at d_anchors + t * num_anchors * 7
+ * (d_anchors [T, num_anchors, 7]).  Every frame and task is one slot (b * T + t) of the same launches; each slot takes its own top
+ * nms_pre_max and runs NMS within its task only (no suppression across classes) and keeps nms_post_max; score threshold, frustum,
+ * direction fix and range mask are shared.  Layouts with P the per-task capacity above: d_boxes [batch, T * P, 7], d_scores and
+ * d_labels [batch, T * P]: the tasks' detections concatenated in task order, label t; d_count [batch] = the frame total;
+ * d_aux [batch * T, 4] per slot; d_sel_anchor [batch, T * P], task t's block at t * P, holding indices t * num_anchors + a into the
+ * concatenated anchors.  The workspace carries one staging copy of each slot's detections. */
 int sessd_postprocess(const float *d_head, const float *d_anchors, const float *d_frustum,
                       const sessd_post_cfg *cfg, float *d_boxes, float *d_scores, int *d_labels, int *d_count,
                       int *d_aux, int *d_sel_anchor, void *workspace, size_t workspace_bytes, void *stream);
@@ -329,7 +345,8 @@ int sessd_postprocess(const float *d_head, const float *d_anchors, const float *
  * scores and labels to the host separately and syncs twice per frame: box_torch_ops.py:536, mg_head_sessd.py:1026):
  * d_packed [batch, post_max, 8] = box 7 | score; d_meta [batch, 8 + post_max] i32 = count, candidates, pre-NMS count,
  * NMS-selected count, d_num_voxels[b] (0 if null), *d_status (0 if null), 0, 0, then the anchor index of every returned
- * detection (-1 beyond count). */
+ * detection (-1 beyond count).  Several tasks: d_packed [batch, T * P, 8] and d_meta [batch, 8 + T * P] follow the concatenated
+ * order; the counts of the header are summed over the tasks, and the anchor index t * num_anchors + a gives the label t. */
 int sessd_postprocess_packed(const float *d_head, const float *d_anchors, const float *d_frustum,
                              const sessd_post_cfg *cfg, float *d_boxes, float *d_scores, int *d_labels, int *d_count,
                              int *d_aux, int *d_sel_anchor, float *d_packed, int *d_meta, const int *d_num_voxels,

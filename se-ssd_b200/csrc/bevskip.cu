@@ -75,8 +75,9 @@ static int skip_launch(SkipLaunch &L, int map, int batch, int grid_h, int grid_w
     return p2_geometry(L, batch, grid_h, grid_w, cout, div_up(cout, p2_n_tile(cout)) * p2_n_tile(cout), cls, deconv ? 4 : 1);
 }
 
-// the SSFAPlanesRunner launch sequence (runners.SSFAPlanesRunner.SKIP_LAUNCHES); returns the plan's int32 words, or 0
-static long long skip_plan(SkipPlan &P, int batch, int h, int w) {
+// the SSFAPlanesRunner launch sequence (runners.SSFAPlanesRunner.SKIP_LAUNCHES) with a head of head_cout channels (24 per task);
+// returns the plan's int32 words, or 0
+static long long skip_plan(SkipPlan &P, int batch, int h, int w, int head_cout) {
     if (batch < 1 || h < 4 || w < 4 || (h & 1) || (w & 1)) return 0;
     P.batch = batch; P.h = h; P.w = w; P.h2 = h / 2; P.w2 = w / 2;
     P.nwf = div_up(w, 32); P.nwh = div_up(P.w2, 32);
@@ -94,7 +95,7 @@ static long long skip_plan(SkipPlan &P, int batch, int h, int w) {
                  | skip_launch(L[9], kMM1, batch, h2, w2, h, w, 128, true)     // deconv_block_1.0
                  | skip_launch(L[10], kMO0, batch, h, w, h, w, 128, false)     // conv_0.0
                  | skip_launch(L[11], kMO1, batch, h, w, h, w, 128, false)     // conv_1.0
-                 | skip_launch(L[12], kMOut, batch, h, w, h, w, 24, false);    // head (1x1 on the fused map)
+                 | skip_launch(L[12], kMOut, batch, h, w, h, w, head_cout, false);   // head (1x1 on the fused map)
     long long words = 0;
     P.seg_words = 0;
     for (int i = 0; i < kSkipLaunches; ++i) {
@@ -459,28 +460,37 @@ __global__ void __launch_bounds__(256) bev_skip_fill_kernel(const int *__restric
 
 using namespace sessd;
 
-extern "C" long long sessd_bev_skip_plan_words(int batch, int h, int w, int *offsets) {
+extern "C" long long sessd_bev_skip_plan_words_head(int batch, int h, int w, int head_cout, int *offsets) {
     SkipPlan P;
-    const long long words = skip_plan(P, batch, h, w);
+    const long long words = skip_plan(P, batch, h, w, head_cout);
     if (words && offsets)
         for (int i = 0; i < kSkipLaunches; ++i) offsets[i] = P.l[i].rec;
     return words;
 }
 
-extern "C" long long sessd_bev_skip_seg_words(int batch, int h, int w, int *offsets) {
+extern "C" long long sessd_bev_skip_seg_words_head(int batch, int h, int w, int head_cout, int *offsets) {
     SkipPlan P;
-    if (!skip_plan(P, batch, h, w)) return 0;
+    if (!skip_plan(P, batch, h, w, head_cout)) return 0;
     if (offsets)
         for (int i = 0; i < kSkipLaunches; ++i) offsets[i] = P.l[i].seg;
     return P.seg_words;
 }
 
-// d_bitmap_index: the last sparse level's bitmap index (grid = that level: shape = {D, h, w}); d_plan: sessd_bev_skip_plan_words(B, h, w),
-// d_segs: sessd_bev_skip_seg_words(B, h, w)
-extern "C" int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, int *d_plan, int *d_segs, void *stream) {
+extern "C" long long sessd_bev_skip_plan_words(int batch, int h, int w, int *offsets) {
+    return sessd_bev_skip_plan_words_head(batch, h, w, 24, offsets);
+}
+
+extern "C" long long sessd_bev_skip_seg_words(int batch, int h, int w, int *offsets) {
+    return sessd_bev_skip_seg_words_head(batch, h, w, 24, offsets);
+}
+
+// d_bitmap_index: the last sparse level's bitmap index (grid = that level: shape = {D, h, w}); d_plan: sessd_bev_skip_plan_words_head(B, h,
+// w, head_cout), d_segs: sessd_bev_skip_seg_words_head(B, h, w, head_cout)
+extern "C" int sessd_bev_skip_plan_head(const void *d_bitmap_index, sessd_grid grid, int head_cout, int *d_plan, int *d_segs,
+                                        void *stream) {
     if (!d_bitmap_index || !d_plan || !d_segs || grid.shape[0] < 1) return SESSD_EINVAL;
     SkipPlan P;
-    if (!skip_plan(P, grid.batch, grid.shape[1], grid.shape[2])) return SESSD_EINVAL;
+    if (!skip_plan(P, grid.batch, grid.shape[1], grid.shape[2], head_cout)) return SESSD_EINVAL;
     P.depth = grid.shape[0];
     const int smem = 4 * P.frame_words;
     if (smem > 200 * 1024) return SESSD_EINVAL;
@@ -492,6 +502,10 @@ extern "C" int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, 
     SESSD_LAUNCH(bev_skip_plan_kernel, 1, kSkipThreads, smem, (cudaStream_t)stream, (const uint2 *)d_bitmap_index, d_plan, d_segs, P);
     SESSD_LAUNCH(bev_skip_seg_kernel, kSkipLaunches, kSkipThreads, 0, (cudaStream_t)stream, d_segs, P);
     return last_error();
+}
+
+extern "C" int sessd_bev_skip_plan(const void *d_bitmap_index, sessd_grid grid, int *d_plan, int *d_segs, void *stream) {
+    return sessd_bev_skip_plan_head(d_bitmap_index, grid, 24, d_plan, d_segs, stream);
 }
 
 // after the launch that ran d_record's items: fill its skipped tiles in d_out_f32 [B][H][W][cout] and / or d_out_planes [2][B][H][W][cout]

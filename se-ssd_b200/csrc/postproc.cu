@@ -24,13 +24,21 @@
 //   4'. overlap : the dense k x k BEV IoU matrix of each frame, on the 32x32 upper-triangle tiles of stage 4.
 //   4''. cluster: one CTA per frame: the centerness softmax, then one pick per iteration (block argmax, a pass over the pick's
 //                 matrix row, block reductions); emitted clusters feed the frustum / flip / range / compaction of stage 5.
+// Tasks (cfg.num_tasks = T > 1, MultiGroupHead with one class per task): every stage runs over B*T slots s = b*T + t in the same
+// launches.  Slot (b, t) reads head floats at pix*head_stride + t*task_stride and anchors at d_anchors + t*A*7, frame b's frustum, and its
+// own candidate / top-k / mask workspace, so top-k, NMS and nms_post_max are per task (no suppression across classes).  The finalize
+// stage compacts each slot into a staging area and post_merge_kernel concatenates the tasks of a frame in task order with label t.
 // Compiled with -fmad=false (rotbox.cuh).
 #include "common.cuh"
 #include "rotbox.cuh"
 
 namespace sessd {
 
-// head layout per pixel: [box 2x7 | cls 2 | dir 2x2 | iou 2] = 22 floats, row stride cfg.head_stride (>= 22)
+// head layout per pixel and task: [box 2x7 | cls 2 | dir 2x2 | iou 2] = 22 floats at t*task_stride, row stride cfg.head_stride
+
+// tasks of a post-processing config (num_tasks 0 means one) and the head floats between them
+__host__ __device__ __forceinline__ int post_tasks(const sessd_post_cfg &c) { return c.num_tasks > 1 ? c.num_tasks : 1; }
+__host__ __device__ __forceinline__ int post_task_stride(const sessd_post_cfg &c) { return c.num_tasks > 1 ? c.task_stride : 0; }
 
 struct PostWs {
     unsigned long long *cand;      // [B, A] candidate keys
@@ -52,13 +60,19 @@ struct PostWs {
     int *odir;                     // [B, K]
     int *osel;                     // [B, K] anchor index of the pick
     int *ostat;                    // [B, 2] emitted clusters, picks
+    // several tasks only: each slot's compacted detections before post_merge_kernel concatenates a frame's tasks
+    float *fbox;                   // [B, P, 7]
+    float *fscore;                 // [B, P]
+    int *fanchor;                  // [B, P] anchor index into the concatenated anchors (t*A + a)
+    int *fcount;                   // [B]
     size_t bytes;
 };
 
 static inline size_t al(size_t x) { return (x + 255) & ~(size_t)255; }
 
-// dinms: carve the DI-NMS buffers; labels: also the per-candidate labels, which only the stand-alone entry fills
-static PostWs post_carve(void *base, int batch, int anchors, int k, bool dinms = false, bool labels = false) {
+// batch: slots (frames x tasks); dinms: carve the DI-NMS buffers; labels: also the per-candidate labels, which only the stand-alone entry
+// fills; stage_p > 0: the staging rows of several tasks, stage_p per slot
+static PostWs post_carve(void *base, int batch, int anchors, int k, bool dinms = false, bool labels = false, int stage_p = 0) {
     PostWs w;
     char *p = (char *)base;
     size_t o = 0;
@@ -82,6 +96,11 @@ static PostWs post_carve(void *base, int batch, int anchors, int k, bool dinms =
     w.odir = dinms ? (int *)take(sizeof(int) * (size_t)batch * k) : nullptr;
     w.osel = dinms ? (int *)take(sizeof(int) * (size_t)batch * k) : nullptr;
     w.ostat = dinms ? (int *)take(sizeof(int) * (size_t)batch * 2) : nullptr;
+    const bool st = stage_p > 0;
+    w.fbox = st ? (float *)take(sizeof(float) * (size_t)batch * stage_p * 7) : nullptr;
+    w.fscore = st ? (float *)take(sizeof(float) * (size_t)batch * stage_p) : nullptr;
+    w.fanchor = st ? (int *)take(sizeof(int) * (size_t)batch * stage_p) : nullptr;
+    w.fcount = st ? (int *)take(sizeof(int) * (size_t)batch) : nullptr;
     w.bytes = o;
     return w;
 }
@@ -119,7 +138,8 @@ __device__ __forceinline__ void append_key(unsigned long long *list, int *count,
 // 1. score ---------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) post_score_kernel(const float *__restrict__ head, sessd_post_cfg cfg,
                                                          unsigned long long *__restrict__ cand, int *__restrict__ ncand) {
-    const int b = blockIdx.y;
+    const int s = blockIdx.y, T = post_tasks(cfg);                   // slot = frame * T + task
+    const int b = s / T, toff = (s - b * T) * post_task_stride(cfg);
     const int apl = cfg.anchors_per_loc;
     const int A = cfg.num_anchors;
     const int a_pad = (A + 31) & ~31;   // keep whole warps in the loop for the ballot
@@ -128,7 +148,7 @@ __global__ void __launch_bounds__(256) post_score_kernel(const float *__restrict
         unsigned long long key = 0;
         if (a < A) {
             const int pix = a / apl, r = a - pix * apl;
-            const float *h = head + ((size_t)b * (A / apl) + pix) * cfg.head_stride;
+            const float *h = head + ((size_t)b * (A / apl) + pix) * cfg.head_stride + toff;
             const float logit = h[7 * apl + r];
             const float s = 1.0f / (1.0f + expf(-logit));          // torch.sigmoid
             keep = s >= cfg.score_thresh;                          // mg_head_sessd.py:965-969
@@ -138,7 +158,7 @@ __global__ void __launch_bounds__(256) post_score_kernel(const float *__restrict
                 key = make_key(s * (q2 * q2), a);                  // score * pow(q, 4)              (:972)
             }
         }
-        append_key(cand + (size_t)b * A, ncand + b, keep, key);
+        append_key(cand + (size_t)s * A, ncand + s, keep, key);
     }
 }
 
@@ -199,15 +219,17 @@ __device__ __forceinline__ void nms_geometry(const float *box7, float *bev, floa
 
 __global__ void __launch_bounds__(128) post_prepare_kernel(const float *__restrict__ head, const float *__restrict__ anchors,
                                                            sessd_post_cfg cfg, PostWs w) {
-    const int b = blockIdx.y;
+    const int s = blockIdx.y, T = post_tasks(cfg);                   // slot = frame * T + task
+    const int b = s / T, t_ = s - b * T;
     const int K = cfg.nms_pre_max;
-    const int m = min(w.ncand[b], K);
+    const int m = min(w.ncand[s], K);
     const int apl = cfg.anchors_per_loc;
+    anchors += (size_t)t_ * cfg.num_anchors * 7;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
-        const unsigned long long key = w.sel[(size_t)b * K + i];
+        const unsigned long long key = w.sel[(size_t)s * K + i];
         const int a = key_index(key);
         const int pix = a / apl, r = a - pix * apl;
-        const float *h = head + ((size_t)b * (cfg.num_anchors / apl) + pix) * cfg.head_stride;
+        const float *h = head + ((size_t)b * (cfg.num_anchors / apl) + pix) * cfg.head_stride + t_ * post_task_stride(cfg);
         const float *t = h + 7 * r;
         const float *an = anchors + (size_t)a * 7;
         float box[7];
@@ -219,7 +241,7 @@ __global__ void __launch_bounds__(128) post_prepare_kernel(const float *__restri
         box[4] = expf(t[4]) * an[4];
         box[5] = expf(t[5]) * an[5];
         box[6] = t[6] + an[6];
-        const size_t o = (size_t)b * K + i;
+        const size_t o = (size_t)s * K + i;
 #pragma unroll
         for (int j = 0; j < 7; ++j) w.sbox[o * 7 + j] = box[j];
         nms_geometry(box, w.sbev + o * 5, w.ssu + o * 4);
@@ -428,8 +450,9 @@ __device__ __forceinline__ float block_reduce(float v, bool is_max, float *s_tmp
     return r;
 }
 
-__global__ void __launch_bounds__(kClusterThreads) dinms_cluster_kernel(PostWs w, int K, const float *__restrict__ anchors,
-                                                                         sessd_dinms_cfg c, DinmsOut o) {
+// anchors: slot b reads anchors + (b % tasks) * task_anchors * 7 (its task's anchors)
+__global__ void __launch_bounds__(kClusterThreads) dinms_cluster_kernel(PostWs w, int K, const float *__restrict__ anchors, int tasks,
+                                                                         int task_anchors, sessd_dinms_cfg c, DinmsOut o) {
     constexpr int NW = kClusterThreads / 32;
     extern __shared__ float cdyn[];
     float *s_adj = cdyn;
@@ -445,6 +468,7 @@ __global__ void __launch_bounds__(kClusterThreads) dinms_cluster_kernel(PostWs w
     const int m = min(w.ncand[b], K);
     const size_t fb = (size_t)b * K;
     const float *sbox = w.sbox + fb * 7;
+    if (anchors) anchors += (size_t)(b % tasks) * task_anchors * 7;
 
     // centerness (box_torch_ops.py:584-588): d = |centre - anchor centre|, m = softmax(d) over the k candidates,
     // score *= (1 - m)^pow; d is parked in s_adj until the softmax is known
@@ -643,7 +667,9 @@ struct PostPack {
 };
 
 // kDI: the rows come from the DI-NMS cluster loop (w.obox / oscore / odir / osel, w.ostat) instead of the greedy scan over the mask,
-// and the capacity P is nms_pre_max
+// and the capacity P is nms_pre_max.  One CTA per slot (frame b, task t).  One task: the CTA writes the frame's outputs.  Several
+// tasks: d_sel_anchor and d_aux are written per slot ([B, T*P] with task t's block at t*P, and [B*T, 4]); the compacted rows go to the
+// slot's staging rows (w.fbox / fscore / fanchor / fcount), which post_merge_kernel concatenates.
 template <bool kDI>
 __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post_cfg cfg, const float *__restrict__ frustum,
                                                             float *__restrict__ out_boxes, float *__restrict__ out_scores,
@@ -658,18 +684,22 @@ __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post
     int *s_flag = s_keep + P;
     __shared__ int s_misc[4];
     __shared__ unsigned long long s_kb;
-    const int b = blockIdx.x;
-    const int n = w.ncand[b];
+    const int slot = blockIdx.x, T = post_tasks(cfg);
+    const int b = slot / T, task = slot - b * T;
+    const bool staged = T > 1;
+    const int n = w.ncand[slot];
     const int m = min(n, K);
-    const size_t fb = (size_t)b * K;
+    const size_t fb = (size_t)slot * K;
+    const int abase = task * cfg.num_anchors;                        // index into the concatenated anchors [T, A, 7]
     int nk;
-    if constexpr (kDI) nk = w.ostat[2 * b];
+    if constexpr (kDI) nk = w.ostat[2 * slot];
     else nk = greedy_scan(w.mask + fb * col_blocks, m, col_blocks, P, remv, diag, s_keep, s_misc, &s_kb);
     // row t of the kept list: its box, score, direction label and anchor index
     auto row_box = [&](int t) -> const float * { return kDI ? w.obox + (fb + t) * 7 : w.sbox + (fb + s_keep[t]) * 7; };
     auto row_score = [&](int t) { return kDI ? w.oscore[fb + t] : w.sscore[fb + s_keep[t]]; };
     auto row_dir = [&](int t) { return kDI ? w.odir[fb + t] : w.sdir[fb + s_keep[t]]; };
-    auto row_anchor = [&](int t) { return kDI ? w.osel[fb + t] : key_index(w.sel[fb + s_keep[t]]); };
+    auto row_anchor = [&](int t) { return abase + (kDI ? w.osel[fb + t] : key_index(w.sel[fb + s_keep[t]])); };
+    int *sel_out = out_sel_anchor + ((size_t)b * T + task) * P;
     // per kept box: frustum test + range mask (the direction fix happens before the range test but only touches r)
     for (int t = threadIdx.x; t < P; t += blockDim.x) {
         int ok = 0;
@@ -685,9 +715,9 @@ __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post
             }
             for (int j = 0; j < 3; ++j)
                 if (!(bx[j] >= cfg.post_range[j] && bx[j] <= cfg.post_range[3 + j])) ok = 0;
-            out_sel_anchor[(size_t)b * P + t] = row_anchor(t);
+            sel_out[t] = row_anchor(t);
         } else {
-            out_sel_anchor[(size_t)b * P + t] = -1;
+            sel_out[t] = -1;
         }
         s_flag[t] = ok;
     }
@@ -696,13 +726,14 @@ __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post
     if (threadIdx.x == 0) {
         int c = 0;
         for (int t = 0; t < P; ++t) { int f = s_flag[t]; s_flag[t] = f ? c : -1; c += f; }
-        out_count[b] = c;
-        out_aux[b * 4 + 0] = n;
-        out_aux[b * 4 + 1] = m;
-        out_aux[b * 4 + 2] = nk;
-        out_aux[b * 4 + 3] = kDI ? w.ostat[2 * b + 1] : 0;
+        out_aux[slot * 4 + 0] = n;
+        out_aux[slot * 4 + 1] = m;
+        out_aux[slot * 4 + 2] = nk;
+        out_aux[slot * 4 + 3] = kDI ? w.ostat[2 * slot + 1] : 0;
+        if (staged) w.fcount[slot] = c;
+        else out_count[b] = c;
         s_misc[1] = c;
-        if (pk.meta) {
+        if (pk.meta && !staged) {
             int *mt = pk.meta + (size_t)b * (8 + P);
             mt[0] = c; mt[1] = n; mt[2] = m; mt[3] = nk;
             mt[4] = pk.num_voxels ? pk.num_voxels[b] : 0;
@@ -716,7 +747,7 @@ __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post
         const int dst = s_flag[t];
         if (dst >= 0) {
             const float *bx = row_box(t);
-            float *ob = out_boxes + ((size_t)b * P + dst) * 7;
+            float *ob = (staged ? w.fbox : out_boxes) + ((size_t)slot * P + dst) * 7;
 #pragma unroll
             for (int j = 0; j < 6; ++j) ob[j] = bx[j];
             float r = bx[6];
@@ -724,8 +755,13 @@ __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post
             if (opp) r += 3.14159265358979323846f;   // torch.tensor(np.pi).type_as(fp32)
             ob[6] = r;
             const float sc = row_score(t);
+            if (staged) {
+                w.fscore[(size_t)slot * P + dst] = sc;
+                w.fanchor[(size_t)slot * P + dst] = row_anchor(t);
+                continue;
+            }
             out_scores[(size_t)b * P + dst] = sc;
-            out_labels[(size_t)b * P + dst] = 0;
+            out_labels[(size_t)b * P + dst] = task;
             if (pk.packed) {
                 float *pp = pk.packed + ((size_t)b * P + dst) * 8;
 #pragma unroll
@@ -736,6 +772,7 @@ __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post
             }
         }
     }
+    if (staged) return;
     for (int t = total + threadIdx.x; t < P; t += blockDim.x) {
         float *ob = out_boxes + ((size_t)b * P + t) * 7;
         for (int j = 0; j < 7; ++j) ob[j] = 0.f;
@@ -745,6 +782,60 @@ __global__ void __launch_bounds__(256) post_finalize_kernel(PostWs w, sessd_post
             float *pp = pk.packed + ((size_t)b * P + t) * 8;
             for (int j = 0; j < 8; ++j) pp[j] = 0.f;
             pk.meta[(size_t)b * (8 + P) + 8 + t] = -1;
+        }
+    }
+}
+
+// several tasks: one CTA per frame concatenates its slots' staged detections in task order into the [B, T*P] outputs, label = task,
+// count = the frame total, the packed block's meta header summed over the tasks; rows beyond the total as in post_finalize_kernel
+__global__ void __launch_bounds__(256) post_merge_kernel(PostWs w, sessd_post_cfg cfg, int P, float *__restrict__ out_boxes,
+                                                         float *__restrict__ out_scores, int *__restrict__ out_labels,
+                                                         int *__restrict__ out_count, const int *__restrict__ out_aux, PostPack pk) {
+    const int b = blockIdx.x, T = post_tasks(cfg), TP = T * P;
+    const size_t ob0 = (size_t)b * TP;
+    int off = 0;
+    for (int t = 0; t < T; ++t) {
+        const int slot = b * T + t, c = w.fcount[slot];
+        for (int i = threadIdx.x; i < c; i += blockDim.x) {
+            const size_t src = (size_t)slot * P + i, dst = ob0 + off + i;
+            const float *bx = w.fbox + src * 7;
+            float *o = out_boxes + dst * 7;
+#pragma unroll
+            for (int j = 0; j < 7; ++j) o[j] = bx[j];
+            out_scores[dst] = w.fscore[src];
+            out_labels[dst] = t;
+            if (pk.packed) {
+                float *pp = pk.packed + dst * 8;
+#pragma unroll
+                for (int j = 0; j < 7; ++j) pp[j] = bx[j];
+                pp[7] = w.fscore[src];
+                pk.meta[(size_t)b * (8 + TP) + 8 + off + i] = w.fanchor[src];
+            }
+        }
+        off += c;
+    }
+    for (int t = off + threadIdx.x; t < TP; t += blockDim.x) {
+        float *o = out_boxes + (ob0 + t) * 7;
+        for (int j = 0; j < 7; ++j) o[j] = 0.f;
+        out_scores[ob0 + t] = 0.f;
+        out_labels[ob0 + t] = -1;
+        if (pk.packed) {
+            float *pp = pk.packed + (ob0 + t) * 8;
+            for (int j = 0; j < 8; ++j) pp[j] = 0.f;
+            pk.meta[(size_t)b * (8 + TP) + 8 + t] = -1;
+        }
+    }
+    if (threadIdx.x == 0) {
+        out_count[b] = off;
+        if (pk.meta) {
+            int sum[3] = {0, 0, 0};
+            for (int t = 0; t < T; ++t)
+                for (int j = 0; j < 3; ++j) sum[j] += out_aux[(b * T + t) * 4 + j];
+            int *mt = pk.meta + (size_t)b * (8 + TP);
+            mt[0] = off; mt[1] = sum[0]; mt[2] = sum[1]; mt[3] = sum[2];
+            mt[4] = pk.num_voxels ? pk.num_voxels[b] : 0;
+            mt[5] = pk.status ? *pk.status : 0;
+            mt[6] = 0; mt[7] = 0;
         }
     }
 }
@@ -767,9 +858,18 @@ __global__ void __launch_bounds__(256) nms_finalize_kernel(PostWs w, int K, int 
 
 using namespace sessd;
 
+// per-frame capacity of one task: nms_post_max, nms_pre_max under DI-NMS
+static int post_slot_capacity(const sessd_post_cfg &c) { return c.nms_mode == 1 ? c.nms_pre_max : c.nms_post_max; }
+
+// the workspace of a config: slots = frames x tasks, plus the staging rows when there are several tasks
+static PostWs post_carve_cfg(void *base, const sessd_post_cfg &c) {
+    const int T = post_tasks(c);
+    return post_carve(base, c.batch * T, c.num_anchors, c.nms_pre_max, c.nms_mode == 1, false, T > 1 ? post_slot_capacity(c) : 0);
+}
+
 extern "C" size_t sessd_postprocess_workspace_bytes(const sessd_post_cfg *cfg) {
     if (!cfg) return 0;
-    return post_carve(nullptr, cfg->batch, cfg->num_anchors, cfg->nms_pre_max, cfg->nms_mode == 1).bytes;
+    return post_carve_cfg(nullptr, *cfg).bytes;
 }
 
 static bool dinms_cfg_ok(const sessd_dinms_cfg &c) {
@@ -779,13 +879,15 @@ static bool dinms_cfg_ok(const sessd_dinms_cfg &c) {
 static size_t cluster_smem(int K) { return (sizeof(float) * 2 + sizeof(int) * 2) * (size_t)K; }
 
 // overlap matrix + cluster loop of B frames whose candidates stage 3 (or dinms_prepare_kernel) has laid out in w
-static int dinms_launch(PostWs w, int B, int K, const float *d_anchors, const sessd_dinms_cfg &c, DinmsOut o, cudaStream_t st) {
+// B: slots; slot b reads the anchors of task b % tasks (task_anchors rows each)
+static int dinms_launch(PostWs w, int B, int K, const float *d_anchors, int tasks, int task_anchors, const sessd_dinms_cfg &c, DinmsOut o,
+                        cudaStream_t st) {
     const int cb = (K + kMaskTile - 1) / kMaskTile;
     dim3 g(cb, cb, B);
     SESSD_LAUNCH(dinms_iou_kernel, g, kMaskThreads, 0, st, w, K);
     const size_t sm = cluster_smem(K);
     if (sm > 48 * 1024) SESSD_CUDA_TRY(cudaFuncSetAttribute(dinms_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    SESSD_LAUNCH(dinms_cluster_kernel, B, kClusterThreads, sm, st, w, K, d_anchors, c, o);
+    SESSD_LAUNCH(dinms_cluster_kernel, B, kClusterThreads, sm, st, w, K, d_anchors, tasks, task_anchors, c, o);
     return 0;
 }
 
@@ -804,12 +906,17 @@ static int postprocess_impl(const float *d_head, const float *d_anchors, const f
         return SESSD_EINVAL;
     if (cfg->anchors_per_loc != 2 || cfg->head_stride < 22) return SESSD_EINVAL;   // head layout is fixed at 22 channels
     if (cfg->nms_mode != 0 && cfg->nms_mode != 1) return SESSD_EINVAL;
+    // several tasks: each one's 22 floats at t * task_stride inside the pixel row
+    if (cfg->num_tasks < 0 || cfg->num_tasks > SESSD_POST_MAX_TASKS) return SESSD_EINVAL;
+    const int T = post_tasks(*cfg);
+    if (T > 1 && (cfg->task_stride < 22 || (long long)(T - 1) * cfg->task_stride + 22 > cfg->head_stride)) return SESSD_EINVAL;
     const bool dinms = cfg->nms_mode == 1;
     if (dinms && (cfg->nms_pre_max > SESSD_DINMS_MAX_PRE || !dinms_cfg_ok(cfg->dinms))) return SESSD_EINVAL;
-    PostWs w = post_carve(workspace, cfg->batch, cfg->num_anchors, cfg->nms_pre_max, dinms);
+    PostWs w = post_carve_cfg(workspace, *cfg);
     if (!workspace || w.bytes > workspace_bytes) return SESSD_EWORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;
-    const int B = cfg->batch, A = cfg->num_anchors, K = cfg->nms_pre_max, P = dinms ? K : cfg->nms_post_max;
+    // B: slots (frame b, task t) = b * T + t; every stage below runs over all of them
+    const int B = cfg->batch * T, A = cfg->num_anchors, K = cfg->nms_pre_max, P = post_slot_capacity(*cfg);
     SESSD_CUDA_TRY(cudaMemsetAsync(w.ncand, 0, sizeof(int) * B, st));
     dim3 g1(div_up(A, 256), B);
     SESSD_LAUNCH(post_score_kernel, g1, 256, 0, st, d_head, *cfg, w.cand, w.ncand);
@@ -820,12 +927,13 @@ static int postprocess_impl(const float *d_head, const float *d_anchors, const f
     const size_t sm = finalize_smem(K, P);
     if (dinms) {
         DinmsOut o = {w.obox, w.oscore, nullptr, w.odir, nullptr, w.osel, w.ostat};
-        const int rc = dinms_launch(w, B, K, d_anchors, cfg->dinms, o, st);
+        const int rc = dinms_launch(w, B, K, d_anchors, T, A, cfg->dinms, o, st);
         if (rc) return rc;
         if (sm > 48 * 1024)
             SESSD_CUDA_TRY(cudaFuncSetAttribute(post_finalize_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
         SESSD_LAUNCH(post_finalize_kernel<true>, B, 256, sm, st, w, *cfg, d_frustum, d_boxes, d_scores, d_labels, d_count, d_aux,
                      d_sel_anchor, pk);
+        if (T > 1) SESSD_LAUNCH(post_merge_kernel, cfg->batch, 256, 0, st, w, *cfg, P, d_boxes, d_scores, d_labels, d_count, d_aux, pk);
         return last_error();
     }
     const int cb = (K + kMaskTile - 1) / kMaskTile;
@@ -833,6 +941,7 @@ static int postprocess_impl(const float *d_head, const float *d_anchors, const f
     SESSD_LAUNCH(post_mask_kernel, g4, kMaskThreads, 0, st, w, K, cfg->nms_iou_thresh, cfg->nms_ge);
     if (sm > 48 * 1024) SESSD_CUDA_TRY(cudaFuncSetAttribute(post_finalize_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
     SESSD_LAUNCH(post_finalize_kernel<false>, B, 256, sm, st, w, *cfg, d_frustum, d_boxes, d_scores, d_labels, d_count, d_aux, d_sel_anchor, pk);
+    if (T > 1) SESSD_LAUNCH(post_merge_kernel, cfg->batch, 256, 0, st, w, *cfg, P, d_boxes, d_scores, d_labels, d_count, d_aux, pk);
     return last_error();
 }
 
@@ -926,7 +1035,7 @@ extern "C" int sessd_rotate_weighted_nms(const float *d_boxes7, const float *d_b
     SESSD_LAUNCH(dinms_prepare_kernel, div_up(pre_max, 128), 128, 0, st, d_boxes7, d_boxes5, d_scores, d_iou_preds, d_labels, d_dirs,
                  pre_max, w);
     DinmsOut o = {d_out_boxes, d_out_scores, d_out_labels, d_out_dirs, d_keep, d_selected, d_count};
-    const int rc = dinms_launch(w, 1, pre_max, d_anchors, *cfg, o, st);
+    const int rc = dinms_launch(w, 1, pre_max, d_anchors, 1, max_boxes, *cfg, o, st);
     if (rc) return rc;
     return last_error();
 }

@@ -9,7 +9,12 @@
 * ``loss_ciassd``: the CIA-SSD pre-training loss (supervised terms only, smooth-L1 box loss in the sum and the gradient).
 * ``loss``     : the assembled SE-SSD head loss (supervised terms + ODIoU on the device, consistency loss against the teacher); value and
   gradient w.r.t. the packed head tensor.  In train mode the packed tensor carries a graph to the head's input and its convs' weights
-  and biases (sessd_b200.bev_grad), so ``loss.backward()`` reaches the neck and the encoder below it."""
+  and biases (sessd_b200.bev_grad), so ``loss.backward()`` reaches the neck and the encoder below it.
+
+Several tasks (one class each, e.g. the KITTI Car / Pedestrian / Cyclist config) run in eval mode only: ``forward`` is ONE 128 -> 24 T
+GEMM over every task's convs, and ``predict`` one post-processing pass over all (frame, task) slots, whose detections come out
+concatenated in task order with the task as the label, as the reference's per-task loop and concatenation give.  Training stays
+single-task."""
 import logging
 import math
 
@@ -23,6 +28,8 @@ from sessd_b200.runners import HeadRunner, RunnerCache
 
 from ..builder import build_loss
 from ..registry import HEADS
+
+TRAIN_SINGLE_TASK = "training is single-task: the fused loss kernels are built for one one-class (car) head, not %d tasks"
 
 
 class _HeadLossFn(torch.autograd.Function):
@@ -52,10 +59,13 @@ class Head(nn.Module):
             self.conv_dir = nn.Conv2d(num_input, num_dir, 1)
         self._runner = RunnerCache()
 
-    def packed_forward(self, x):
-        """x logical NCHW [B,128,H,W] -> packed NHWC [B,H,W,24] = [box 14 | cls 2 | dir 4 | iou 2 | pad 2]."""
+    def _check_layout(self):
         if not (self.use_dir and self.conv_box.out_channels == 14 and self.conv_cls.out_channels == 2 and self.conv_dir.out_channels == 4):
             raise NotImplementedError("the fused head kernel is built for the car head: 2 anchors x (7 box, 1 cls, 2 dir, 1 iou)")
+
+    def packed_forward(self, x):
+        """x logical NCHW [B,128,H,W] -> packed NHWC [B,H,W,24] = [box 14 | cls 2 | dir 4 | iou 2 | pad 2]."""
+        self._check_layout()
         if self.training:       # differentiable w.r.t. x and the four convs' weights and biases (sessd_b200.bev_grad); a fresh tensor
             return bev_grad.head_forward(self, x)
         b, c, h, w = x.shape
@@ -123,6 +133,7 @@ class MultiGroupHead(nn.Module):
         self.thresh = 0.3                                                # and this (:486)
         self._post = None
         self._post_key = None
+        self._runner = RunnerCache()     # the one head GEMM of several tasks (eval mode)
 
     def init_weights(self, pretrained=None):
         if isinstance(pretrained, str):
@@ -137,8 +148,37 @@ class MultiGroupHead(nn.Module):
                 if m.bias is not None:
                     nn.init.constant_(m.bias, 0)
 
+    def _check_multitask(self):
+        """several tasks: each has one class and two anchors per location (the fused kernels' layout)"""
+        if any(n != 1 for n in self.num_classes):
+            raise NotImplementedError("multi-task inference takes one class per task, got classes per task %s" % (self.num_classes,))
+        if any(a != 2 for a in self.num_anchor_per_locs):
+            raise NotImplementedError("multi-task inference takes 2 anchors per location, got %s" % (self.num_anchor_per_locs,))
+
     def forward(self, x):
-        return [task(x) for task in self.tasks]
+        T = len(self.tasks)
+        if T == 1:
+            return [task(x) for task in self.tasks]
+        if self.training:
+            raise NotImplementedError(TRAIN_SINGLE_TASK % T)
+        self._check_multitask()
+        for task in self.tasks:
+            task._check_layout()
+        # eval mode: every task's four convs in one head GEMM (runners.HeadRunner over all tasks); task t's dict holds slices of its
+        # 24-channel block of the one packed tensor, which predict() reads whole
+        b, c, h, w = x.shape
+        prefixes = ["tasks.%d." % t for t in range(T)]
+        runner = self._runner.get(self, (b, h, w, str(x.device), T), lambda: HeadRunner(b, (h, w), x.device, num_tasks=T),
+                                  lambda r: r.load_state({k: v.detach() for k, v in self.state_dict().items() if k.startswith("tasks.")},
+                                                         prefixes))
+        packed = runner.forward(x.detach().float().permute(0, 2, 3, 1).contiguous()).clone()
+        out = []
+        for t in range(T):
+            o = 24 * t
+            d = {"box_preds": packed[..., o:o + 14], "cls_preds": packed[..., o + 14:o + 16], "dir_cls_preds": packed[..., o + 16:o + 20],
+                 "iou_preds": packed[..., o + 20:o + 22], "_packed": packed, "_task": t}
+            out.append(d)
+        return out
 
     def _supervision_mask(self, example, batch, device):
         if "ssl_labeled" in example:
@@ -189,7 +229,7 @@ class MultiGroupHead(nn.Module):
         ``box_preds / cls_preds / iou_preds`` by torch autograd.  Returns the reference's key -> [per-task value] dict.  A head tensor
         produced by ``Head.forward`` in train mode carries the graph of the head, the neck and the encoder (in eval mode none)."""
         if len(preds_dicts) != 1:
-            raise NotImplementedError("the fused loss kernels are built for the single-task (car) head")
+            raise NotImplementedError(TRAIN_SINGLE_TASK % len(preds_dicts))
         merged = {}
         if preds_ema is not None:
             merged["consistency_loss"] = [self.consistency_loss(preds_dicts, preds_ema, example)]
@@ -212,7 +252,7 @@ class MultiGroupHead(nn.Module):
         that gradient to ``preds_dicts[0]['_packed']``'s graph.  As in the reference, ``dir_loss_reduced`` is reported without its weight
         while ``loss`` sums the weighted term.  Returns the reference's key -> [per-task value] dict."""
         if len(preds_dicts) != 1:
-            raise NotImplementedError("the fused loss kernels are built for the single-task (car) head")
+            raise NotImplementedError(TRAIN_SINGLE_TASK % len(preds_dicts))
         out, loss = self._supervised_terms(example, preds_dicts[0], ("anchors", "labels", "reg_targets"), with_odiou=False, with_loc=True)
         cpu = lambda v: v.detach().cpu()                                                     # noqa: E731
         return dict(loss=[loss], cls_loss_reduced=[cpu(out["cls_loss_reduced"])], loc_loss_reduced=[cpu(out["loc_loss_reduced"])],
@@ -343,20 +383,28 @@ class MultiGroupHead(nn.Module):
 
     # ------------------------------------------------------------------------------------------------------------------
     def predict(self, example, preds_dicts, test_cfg, **kwargs):
-        if len(preds_dicts) != 1:
-            raise NotImplementedError("the fused post-processing is built for the single-task (car) head")
-        preds = preds_dicts[0]
+        """Detections per frame.  Several tasks: every task is decoded against its own anchors (``example["anchors"][t]``), takes its
+        own top-k, NMS and post_max, and the frame's detections are the tasks' concatenated in task order, ``label_preds`` = the task
+        (the reference's class offset of one-class tasks, mg_head_sessd.py:923-943), all in one post-processing pass."""
+        T = len(preds_dicts)
+        if T != len(self.tasks):
+            raise ValueError("%d prediction dicts for a %d-task head" % (T, len(self.tasks)))
+        if T > 1:
+            self._check_multitask()
         anchors = example["anchors"][0]
         batch = int(anchors.shape[0])
-        anc = anchors[0].reshape(-1, self.box_n_dim).float().contiguous()
-        if not anc.is_cuda:
-            anc = anc.cuda()
-        packed = preds.get("_packed")
-        if packed is None:
-            b, h, w, _ = preds["box_preds"].shape
-            packed = torch.zeros((b, h, w, 24), dtype=torch.float32, device=preds["box_preds"].device)
-            packed[..., 0:14], packed[..., 14:16] = preds["box_preds"], preds["cls_preds"]
-            packed[..., 16:20], packed[..., 20:22] = preds["dir_cls_preds"], preds["iou_preds"]
+        anc = torch.cat([example["anchors"][t][0].reshape(-1, self.box_n_dim).float() for t in range(T)], 0)
+        anc = (anc if anc.is_cuda else anc.cuda()).contiguous()
+        num_anchors = int(anc.shape[0]) // T
+        packed = preds_dicts[0].get("_packed")
+        if packed is None or packed.shape[-1] != 24 * T:
+            p0 = preds_dicts[0]
+            b, h, w, _ = p0["box_preds"].shape
+            packed = torch.zeros((b, h, w, 24 * T), dtype=torch.float32, device=p0["box_preds"].device)
+            for t, preds in enumerate(preds_dicts):
+                o = 24 * t
+                packed[..., o:o + 14], packed[..., o + 14:o + 16] = preds["box_preds"], preds["cls_preds"]
+                packed[..., o + 16:o + 20], packed[..., o + 20:o + 22] = preds["dir_cls_preds"], preds["iou_preds"]
         nms = test_cfg.nms if hasattr(test_cfg, "nms") else test_cfg["nms"]
         if test_cfg["score_threshold"] <= 0.0:
             raise NotImplementedError("score_threshold must be positive (the reference path thresholds before NMS)")
@@ -370,14 +418,14 @@ class MultiGroupHead(nn.Module):
         # "rotate_weighted_nms" selects DI-NMS with the head's constants (mg_head_sessd.py:999-1018 of the reference, where the choice is
         # a local variable); a config without the key keeps rotate_nms
         nms_type = nms.get("nms_type", "rotate_nms") if hasattr(nms, "get") else getattr(nms, "nms_type", "rotate_nms")
-        key = (batch, int(anc.shape[0]), float(self.thresh), int(nms["nms_pre_max_size"]), int(nms["nms_post_max_size"]),
-               float(nms["nms_iou_threshold"]), frustum is not None, str(packed.device), nms_type)
+        key = (batch, num_anchors, float(self.thresh), int(nms["nms_pre_max_size"]), int(nms["nms_post_max_size"]),
+               float(nms["nms_iou_threshold"]), frustum is not None, str(packed.device), nms_type, T)
         if self._post is None or self._post_key != key:
-            cfg = ops.make_post_cfg(batch=batch, num_anchors=int(anc.shape[0]), anchors_per_loc=self.num_anchor_per_locs[0],
-                                    head_stride=24, score_thresh=self.thresh, nms_pre_max=nms["nms_pre_max_size"],
+            cfg = ops.make_post_cfg(batch=batch, num_anchors=num_anchors, anchors_per_loc=self.num_anchor_per_locs[0],
+                                    head_stride=24 * T, score_thresh=self.thresh, nms_pre_max=nms["nms_pre_max_size"],
                                     nms_post_max=nms["nms_post_max_size"], nms_iou_thresh=nms["nms_iou_threshold"], nms_ge=True,
                                     post_range=self.post_center_range, direction_offset=getattr(self, "direction_offset", 0.0),
-                                    use_frustum=frustum is not None, nms_type=nms_type)
+                                    use_frustum=frustum is not None, nms_type=nms_type, num_tasks=T, task_stride=24)
             self._post, self._post_key = ops.PostBuffers(cfg, packed.device), key
         buf = ops.postprocess(packed.contiguous(), anc, frustum, self._post)
         counts = buf.count.cpu().tolist()                       # the one host sync of the frame

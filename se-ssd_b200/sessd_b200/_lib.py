@@ -41,7 +41,8 @@ class PostCfg(C.Structure):
     _fields_ = [("batch", C.c_int), ("num_anchors", C.c_int), ("anchors_per_loc", C.c_int), ("head_stride", C.c_int),
                 ("score_thresh", C.c_float), ("nms_pre_max", C.c_int), ("nms_post_max", C.c_int),
                 ("nms_iou_thresh", C.c_float), ("nms_ge", C.c_int), ("post_range", C.c_float * 6),
-                ("direction_offset", C.c_float), ("use_frustum", C.c_int), ("nms_mode", C.c_int), ("dinms", DinmsCfg)]
+                ("direction_offset", C.c_float), ("use_frustum", C.c_int), ("nms_mode", C.c_int), ("dinms", DinmsCfg),
+                ("num_tasks", C.c_int), ("task_stride", C.c_int)]
 
 
 class KittiFrames(C.Structure):
@@ -89,6 +90,9 @@ SIGNATURES = {
     "sessd_bev_skip_plan_words": (_ll, [_i, _i, _i, _I3]),
     "sessd_bev_skip_seg_words": (_ll, [_i, _i, _i, _I3]),
     "sessd_bev_skip_plan": (_i, [_vp, Grid, _vp, _vp, _vp]),
+    "sessd_bev_skip_plan_words_head": (_ll, [_i, _i, _i, _i, _I3]),
+    "sessd_bev_skip_seg_words_head": (_ll, [_i, _i, _i, _i, _I3]),
+    "sessd_bev_skip_plan_head": (_i, [_vp, Grid, _i, _vp, _vp, _vp]),
     "sessd_bev_skip_fill": (_i, [_vp, _vp, _vp, _i, _vp]),
     "sessd_bev_skip_fill_segs": (_i, [_vp, _vp, _vp, _i, _vp]),
     "sessd_bev_wgrad_items": (_i, [C.POINTER(ConvDesc)]),

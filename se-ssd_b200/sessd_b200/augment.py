@@ -243,24 +243,39 @@ def _augment_device(cfg, d_pts, d_off, ns, rest, draws, labeled, student_boxes=F
 _STATIC = {}
 
 
-def _static(cfg, device):
-    """per-config constants of the batch builder: the augmentation values, the voxeliser config and grid, the anchors on the device and
-    the assigner's thresholds (built once per config object and device)"""
-    key = (id(cfg), str(device))
+def _device_anchors(a, device):
+    return torch.from_numpy(np.ascontiguousarray(a.reshape(-1, 7), np.float32)).pin_memory().to(device, non_blocking=True)
+
+
+def _static_eval(cfg, device):
+    """per-config constants of an evaluation batch: the voxeliser config and grid, the assigner and every task's anchors on the device
+    (AssignTarget's, in task order; any number of one-class tasks).  Built once per config object and device."""
+    key = ("eval", id(cfg), str(device))
     if key not in _STATIC:
         from det3d.datasets.pipelines import AssignTarget, Voxelization
         vg = cfg.voxel_generator
         vox = Voxelization(cfg=vg).voxel_generator
         at = AssignTarget(cfg=cfg.train_cfg.assigner)
-        if len(at.anchor_dicts_by_task) != 1 or len(at.anchor_dicts_by_task[0]) != 1:
-            raise NotImplementedError("build_train_batch supports the single-class SE-SSD KITTI config")
-        ta = at.target_assigners[0]
-        (ad,) = at.anchor_dicts_by_task[0].values()
-        gen = ta._anchor_generators[0]
-        anchors = torch.from_numpy(np.ascontiguousarray(ad["anchors"].reshape(-1, 7), np.float32)).pin_memory().to(device, non_blocking=True)
-        _STATIC[key] = dict(cfg=cfg, aug=AugmentConfig.from_config(cfg),
-                            vcfg=ops.make_voxel_cfg(vg.voxel_size, vg.range, vg.max_points_in_voxel, vg.max_voxel_num),
-                            grid=np.asarray(vox.grid_size), anchors=anchors, thr=(float(gen.match_threshold), float(gen.unmatch_threshold)))
+        if any(len(d) != 1 for d in at.anchor_dicts_by_task):
+            raise NotImplementedError("evaluation batches take one class per task")
+        anchors = [_device_anchors(d[at.target_class_names[t]]["anchors"], device) for t, d in enumerate(at.anchor_dicts_by_task)]
+        _STATIC[key] = dict(cfg=cfg, vcfg=ops.make_voxel_cfg(vg.voxel_size, vg.range, vg.max_points_in_voxel, vg.max_voxel_num),
+                            grid=np.asarray(vox.grid_size), assigner=at, task_anchors=anchors)
+    return _STATIC[key]
+
+
+def _static(cfg, device):
+    """per-config constants of the training batch builder: _static_eval's, the augmentation values, the one task's anchors and the
+    assigner's thresholds (built once per config object and device).  Training is single-task, single-class."""
+    key = (id(cfg), str(device))
+    if key not in _STATIC:
+        tasks = cfg.train_cfg.assigner.target_assigner.tasks
+        if len(tasks) != 1 or int(tasks[0]["num_class"]) != 1:
+            raise NotImplementedError("build_train_batch supports the single-class SE-SSD KITTI config (training is single-task)")
+        ev = _static_eval(cfg, device)
+        gen = ev["assigner"].target_assigners[0]._anchor_generators[0]
+        _STATIC[key] = dict(ev, aug=AugmentConfig.from_config(cfg), anchors=ev["task_anchors"][0],
+                            thr=(float(gen.match_threshold), float(gen.unmatch_threshold)))
     return _STATIC[key]
 
 
@@ -269,7 +284,7 @@ def voxel_example(st, vb, batch, total, sfx=""):
     ``total`` rows of the VoxelBuffers ``vb``, read back by the caller), num_voxels, shape and the per-task anchors"""
     return {"voxels" + sfx: vb.voxels[:total], "num_points" + sfx: vb.num_points[:total], "coordinates" + sfx: vb.coors[:total],
             "num_voxels" + sfx: vb.num_voxels[:batch].long(), "shape" + sfx: np.stack([st["grid"]] * batch),
-            "anchors" + sfx: [st["anchors"].unsqueeze(0).expand(batch, -1, -1).contiguous()]}
+            "anchors" + sfx: [a.unsqueeze(0).expand(batch, -1, -1).contiguous() for a in st["task_anchors"]]}
 
 
 class PendingBatch:

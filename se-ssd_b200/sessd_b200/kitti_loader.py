@@ -94,7 +94,7 @@ class DeviceLoader:
     def val_batch(self, frames):
         """the collated evaluation batch of ``frames``: the keys the model's eval forward and MultiGroupHead.predict read"""
         from det3d.torchie.parallel import collate_kitti
-        st = augment._static(self.cfg, self.device)
+        st = augment._static_eval(self.cfg, self.device)
         B = len(frames)
         clouds = [np.asarray(f["lidar"]["points"], np.float32).reshape(-1, 4) for f in frames]
         off = np.zeros(B + 1, np.int32)

@@ -392,10 +392,12 @@ class BevSkipPlan:
 
     LAUNCHES = 13
 
-    def __init__(self, batch, h, w, device):
+    def __init__(self, batch, h, w, device, head_cout=24):
+        """head_cout: channels of the head launch (24 per task)"""
+        self.head_cout = int(head_cout)
         offs, seg_offs = (C.c_int * self.LAUNCHES)(), (C.c_int * self.LAUNCHES)()
-        words = lib.sessd_bev_skip_plan_words(int(batch), int(h), int(w), offs)
-        seg_words = lib.sessd_bev_skip_seg_words(int(batch), int(h), int(w), seg_offs)
+        words = lib.sessd_bev_skip_plan_words_head(int(batch), int(h), int(w), self.head_cout, offs)
+        seg_words = lib.sessd_bev_skip_seg_words_head(int(batch), int(h), int(w), self.head_cout, seg_offs)
         if words <= 0 or seg_words <= 0:
             raise ValueError("no skip plan for a [%d, %d, %d] neck" % (batch, h, w))
         self.offsets, self.seg_offsets = list(offs), list(seg_offs)
@@ -411,7 +413,8 @@ class BevSkipPlan:
 
     def build(self, bitmap_index, grid):
         """bitmap_index / grid: the last sparse level's index (SpMiddleRunner.levels[-1]) -- grid.shape = (D, h, w)"""
-        check(lib.sessd_bev_skip_plan(_p(bitmap_index), grid, _p(self.buf), _p(self.seg_buf), _st()), "sessd_bev_skip_plan")
+        check(lib.sessd_bev_skip_plan_head(_p(bitmap_index), grid, self.head_cout, _p(self.buf), _p(self.seg_buf), _st()),
+              "sessd_bev_skip_plan_head")
 
     def fill(self, i, out_f32, out_planes, cout):
         check(lib.sessd_bev_skip_fill(_p(self.record(i)), _p(out_f32), _p(out_planes), int(cout), _st()), "sessd_bev_skip_fill")
@@ -493,9 +496,12 @@ def make_dinms_cfg(nms_cnt_thresh=2.6, nms_sigma_dist_interval=(0, 20, 40, 60), 
 
 def make_post_cfg(batch, num_anchors=70400, anchors_per_loc=2, head_stride=24, score_thresh=0.3, nms_pre_max=1000, nms_post_max=100,
                   nms_iou_thresh=0.01, nms_ge=True, post_range=(0, -40.0, -5.0, 70.4, 40.0, 5.0), direction_offset=0.0,
-                  use_frustum=False, nms_type="rotate_nms"):
+                  use_frustum=False, nms_type="rotate_nms", num_tasks=1, task_stride=24):
     """nms_type "rotate_nms" (greedy rotated NMS) or "rotate_weighted_nms" (DI-NMS with the head's constants, make_dinms_cfg();
-    it keeps up to nms_pre_max detections and ignores nms_post_max, nms_iou_thresh and nms_ge, as the reference does)"""
+    it keeps up to nms_pre_max detections and ignores nms_post_max, nms_iou_thresh and nms_ge, as the reference does).
+    num_tasks > 1: the head rows hold one 22-float block per one-class task, task_stride floats apart, num_anchors is per task and the
+    anchors are [num_tasks, num_anchors, 7]; each task takes its own top-k, NMS and post_max, and the frame's detections are the tasks'
+    concatenated in task order with label = task (see sessd_postprocess)"""
     if nms_type not in NMS_TYPES:
         raise ValueError("nms_type must be one of %s, not %r" % (NMS_TYPES, nms_type))
     c = PostCfg()
@@ -507,12 +513,21 @@ def make_post_cfg(batch, num_anchors=70400, anchors_per_loc=2, head_stride=24, s
     c.direction_offset, c.use_frustum = float(direction_offset), int(bool(use_frustum))
     if nms_type == "rotate_weighted_nms":
         c.nms_mode, c.dinms = 1, make_dinms_cfg()
+    if int(num_tasks) < 1:
+        raise ValueError("num_tasks must be at least 1")
+    if int(num_tasks) > 1:                  # one task keeps both fields zero: the single-task layout
+        c.num_tasks, c.task_stride = int(num_tasks), int(task_stride)
     return c
 
 
+def post_tasks(cfg):
+    """tasks of a post-processing config (num_tasks 0 means one)"""
+    return max(int(cfg.num_tasks), 1)
+
+
 def post_capacity(cfg):
-    """detections per frame the post-processing outputs hold: nms_post_max, or nms_pre_max under DI-NMS"""
-    return cfg.nms_pre_max if cfg.nms_mode == 1 else cfg.nms_post_max
+    """detections per frame the post-processing outputs hold: nms_post_max, or nms_pre_max under DI-NMS, per task"""
+    return post_tasks(cfg) * (cfg.nms_pre_max if cfg.nms_mode == 1 else cfg.nms_post_max)
 
 
 class PostBuffers:
@@ -523,7 +538,7 @@ class PostBuffers:
         self.scores = torch.zeros((b, p), dtype=torch.float32, device=device)
         self.labels = torch.zeros((b, p), dtype=torch.int32, device=device)
         self.count = torch.zeros((b,), dtype=torch.int32, device=device)
-        self.aux = torch.zeros((b, 4), dtype=torch.int32, device=device)
+        self.aux = torch.zeros((b * post_tasks(cfg), 4), dtype=torch.int32, device=device)     # per (frame, task)
         self.sel_anchor = torch.zeros((b, p), dtype=torch.int32, device=device)
         self.ws = torch.empty((lib.sessd_postprocess_workspace_bytes(C.byref(cfg)),), dtype=torch.uint8, device=device)
 

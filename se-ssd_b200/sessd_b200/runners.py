@@ -253,18 +253,36 @@ def launch_desc(L, batch, in_hw, out_hw, taps, relu=None):
     return ops.conv_desc(batch, in_hw, L.cin, out_hw, L.cout, out_hw, taps, in_stride=L.stride, relu=L.relu if relu is None else relu)
 
 
-def head_weight(param):
+HEAD_TASK_STRIDE = _SSFA["head"].cout      # channels of one task's block in the head launch: [box 14 | cls 2 | dir 4 | iou 2 | pad 2]
+
+
+def head_weight(param, prefixes=("",)):
     """The four 1x1 head convs (mg_head_sessd.py:202-215) as the module-layout weight [24, 128, 1, 1] and bias [24] of the head launch,
     channel layout [box 14 | cls 2 | dir 4 | iou 2 | zero pad].  param(name) returns a conv's tensor ("conv_box.weight"); the result is
-    built with torch ops, so it keeps the autograd graph of module parameters."""
-    w, b = (torch.cat([param(c + s) for c in ("conv_box", "conv_cls", "conv_dir", "conv_iou")], 0) for s in (".weight", ".bias"))
-    pad = _SSFA["head"].cout - w.shape[0]
-    return torch.cat([w, w.new_zeros((pad,) + tuple(w.shape[1:]))], 0), torch.cat([b, b.new_zeros((pad,))], 0)
+    built with torch ops, so it keeps the autograd graph of module parameters.  Several prefixes (one per task, "tasks.0." ...): the
+    tasks' blocks stacked, task t at channels 24 t ... 24 t + 23 of a [24 T, 128, 1, 1] weight."""
+    ws, bs = [], []
+    for p in prefixes:
+        w, b = (torch.cat([param(p + c + s) for c in ("conv_box", "conv_cls", "conv_dir", "conv_iou")], 0) for s in (".weight", ".bias"))
+        pad = HEAD_TASK_STRIDE - w.shape[0]
+        ws += [w, w.new_zeros((pad,) + tuple(w.shape[1:]))]
+        bs += [b, b.new_zeros((pad,))]
+    return torch.cat(ws, 0), torch.cat(bs, 0)
+
+
+def head_prefixes(prefix):
+    """the task prefixes of a head state dict: one prefix ("tasks.0.") or a list of them, one per task"""
+    return (prefix,) if isinstance(prefix, str) else tuple(prefix)
 
 
 def pack_head(head_sd, prefix, device):
-    """head_weight from a state dict"""
-    return head_weight(lambda name: head_sd[prefix + name].to(device, torch.float32))
+    """head_weight from a state dict; prefix: one task's key prefix or a list of them (head_prefixes)"""
+    return head_weight(lambda name: head_sd[name].to(device, torch.float32), head_prefixes(prefix))
+
+
+def head_launch(num_tasks=1):
+    """the head launch of a head with num_tasks one-class tasks: 24 channels per task"""
+    return _SSFA["head"]._replace(cout=HEAD_TASK_STRIDE * int(num_tasks))
 
 
 def fold_ssfa_bn(sd, conv_name, device, eps=BN_EPS):
@@ -291,7 +309,7 @@ def _cout_pad(cout):
 
 def ssfa_weights(ssfa_sd, head_sd, head_prefix, device, bn_eps=BN_EPS):
     """yields (launch, weight [taps, Cin, Cout], taps, BN scale, BN shift) in SSFA_LAUNCHES order, weight and taps from launch_weight;
-    the head (only with head_sd) with scale None and its bias as the shift"""
+    the head (only with head_sd; head_prefix: one prefix or one per task) with scale None and its bias as the shift"""
     for L in SSFA_LAUNCHES:
         if L.name != "head":
             wp, taps = launch_weight(L, ssfa_sd[L.name + ".weight"].to(device, torch.float32))
@@ -316,7 +334,8 @@ SSFA_SLOT = {n: i for i, n in enumerate(["x"] + [L.dst for L in SSFA_LAUNCHES if
 
 # ---------------------------------------------------------------------------------------------------------------
 class SSFAPlanesRunner:
-    """SSFA neck (rpn_v1.py:220-235) + the fused 128->22(+2 pad) head GEMM (mg_head_sessd.py:202-230) on csrc/bevconv_p2.cu:
+    """SSFA neck (rpn_v1.py:220-235) + the fused 128->22(+2 pad) head GEMM (mg_head_sessd.py:202-230) on csrc/bevconv_p2.cu, one 24-channel
+    block per task of a multi-task head (num_tasks one-class tasks: one 128 -> 24 T GEMM, HEAD_STRIDE = 24 T):
     activations travel between the layers as fp16 (hi, lo) planes written by the producing epilogue (the main loops are pure
     TMA -> wgmma).  14 launches per forward: 13 convs (the stride-2 conv included)
     + the attention fusion; + abs-max and split when the input arrives as fp32 (module API) instead of planes (FrameEngine).
@@ -328,10 +347,12 @@ class SSFAPlanesRunner:
     # the conv / deconv launches of one forward, in the order of the skip plan's records (csrc/bevskip.cu)
     SKIP_LAUNCHES = tuple(L.name for L in SSFA_LAUNCHES)
 
-    def __init__(self, batch, hw=(200, 176), device="cuda", skip_constant=False):
+    def __init__(self, batch, hw=(200, 176), device="cuda", skip_constant=False, num_tasks=1):
         """skip_constant: when forward() gets the occupancy of the last sparse level, run only the work items whose output can differ
-        from the empty-space constant of its class and fill the others with it (bit-identical to the dense neck, csrc/bevskip.cu)"""
+        from the empty-space constant of its class and fill the others with it (bit-identical to the dense neck, csrc/bevskip.cu).
+        num_tasks: tasks of the head; load_state then takes one head prefix per task"""
         self.batch, self.h, self.w, self.device = batch, int(hw[0]), int(hw[1]), torch.device(device)
+        self._set_tasks(num_tasks)
         pl = lambda hw_, c: ops.alloc_bev_planes(batch, hw_[0], hw_[1], c, self.device)     # noqa: E731
         z = lambda hw_, c: torch.zeros((batch,) + hw_ + (c,), dtype=torch.float32, device=self.device)  # noqa: E731
         H, ext = (self.h, self.w), lambda L: ssfa_extents(L, self.h, self.w)[1]     # noqa: E731
@@ -340,13 +361,26 @@ class SSFAPlanesRunner:
         self.info = torch.zeros((16, 2), dtype=torch.float32, device=self.device)
         self.params = None
         self.skip_constant = bool(skip_constant)
-        self.skip = ops.BevSkipPlan(batch, self.h, self.w, self.device) if self.skip_constant else None
+        self.skip = ops.BevSkipPlan(batch, self.h, self.w, self.device, self.HEAD_STRIDE) if self.skip_constant else None
+
+    def _set_tasks(self, num_tasks):
+        self.num_tasks = int(num_tasks)
+        if self.num_tasks < 1:
+            raise ValueError("num_tasks must be at least 1")
+        self.head_launch = head_launch(self.num_tasks)
+        self.HEAD_STRIDE = self.head_launch.cout
+
+    def _check_prefixes(self, prefix):
+        if len(head_prefixes(prefix)) != self.num_tasks:
+            raise ValueError("a %d-task head needs %d head prefixes, got %r" % (self.num_tasks, self.num_tasks, prefix))
 
     def _info(self, name):
         return self.info[self.SLOT[name]]
 
     def load_state(self, ssfa_sd, head_sd=None, head_prefix="tasks.0.", bn_eps=BN_EPS):
         """bn_eps: eps of the neck's BatchNorm2d layers (rpn_v1.py:131-132 uses 1e-3; pass the module's own value otherwise)."""
+        if head_sd is not None:
+            self._check_prefixes(head_prefix)
         P = ssfa_fuse_weights(ssfa_sd, self.device, bn_eps)
         for L, *weight in ssfa_weights(ssfa_sd, head_sd, head_prefix, self.device, bn_eps):
             P[L.name] = pack_h2(*weight)
@@ -381,7 +415,7 @@ class SSFAPlanesRunner:
 
     def forward(self, x=None, mark=None, occupancy=None):
         """x: NHWC fp32 [B,200,176,128] (converted to planes here) or None when self.planes['x'] / info slot 'x' were filled by the
-        producer (FrameEngine: dense() writes the planes directly).  Returns (neck out NHWC fp32, head NHWC fp32 [B,200,176,24]).
+        producer (FrameEngine: dense() writes the planes directly).  Returns (neck out NHWC fp32, head NHWC fp32 [B,200,176,24 T]).
         occupancy: (bitmap index, grid) of the last sparse level whose dense() made the input (FrameEngine); with skip_constant, the
         launches then skip the tiles of the empty space (the input must be exactly zero wherever that level has no site)."""
         assert self.params is not None, "load_state first"
@@ -409,7 +443,7 @@ class SSFAPlanesRunner:
         return self.buf["out"], self.buf["head"]
 
     def head(self, skip=False):
-        self._launch(SSFA_LAUNCHES[-1], skip)
+        self._launch(self.head_launch, skip)
         return self.buf["head"]
 
     def activation(self, name):
@@ -430,18 +464,22 @@ class SSFAPlanesRunner:
 
 class HeadRunner(SSFAPlanesRunner):
     """The fused head GEMM alone (MultiGroupHead.forward): only the buffers of the head launch (its input planes, the info slots, its
-    output), launched by SSFAPlanesRunner.head after the fp32 input is split into planes."""
+    output), launched by SSFAPlanesRunner.head after the fp32 input is split into planes.  num_tasks > 1: every task of a MultiGroupHead
+    in the one launch, task t at channels 24 t ... 24 t + 23 of the output."""
 
-    def __init__(self, batch, hw, device="cuda"):
+    def __init__(self, batch, hw, device="cuda", num_tasks=1):
         self.batch, self.h, self.w, self.device = batch, int(hw[0]), int(hw[1]), torch.device(device)
+        self._set_tasks(num_tasks)
         self.planes = dict(out=ops.alloc_bev_planes(batch, self.h, self.w, 128, self.device))
         self.buf = dict(head=torch.zeros((batch, self.h, self.w, self.HEAD_STRIDE), dtype=torch.float32, device=self.device))
         self.info = torch.zeros((len(self.SLOT), 2), dtype=torch.float32, device=self.device)
         self.params = None
 
     def load_state(self, head_sd, prefix=""):
+        """prefix: the key prefix of the head's convs, or one prefix per task"""
+        self._check_prefixes(prefix)
         w, bias = pack_head(head_sd, prefix, self.device)
-        self.params = {"head": pack_h2(*launch_weight(_SSFA["head"], w), None, bias)}
+        self.params = {"head": pack_h2(*launch_weight(self.head_launch, w), None, bias)}
 
     def forward(self, x):
         self._split(x, "out")

@@ -153,3 +153,33 @@ def bench_detector_state(cloud="ring", seed=0, alpha=None, gains=None):
     head["tasks.0.conv_iou.weight"] = head["tasks.0.conv_iou.weight"].float() * IOU_HEAD_SCALE
     head["tasks.0.conv_iou.bias"] = torch.full((2,), 0.5)
     return layers, ssfa, apply_cls_calibration(head, alpha)
+
+
+def task_anchors(target_assigner, feature_size=(1, 200, 176), dtype=np.float32):
+    """Per-task anchors [A, 7] of a config's ``target_assigner`` (its ``anchor_generators``, one per one-class task, in task order),
+    by the grid arithmetic of kitti_car_anchors with each generator's sizes, anchor_ranges and rotations -- what
+    AnchorGeneratorRange / TargetAssigner.generate_anchors_dict give.  The list FrameEngine.load_weights takes for a multi-class head."""
+    gens = target_assigner["anchor_generators"]
+    tasks = target_assigner.get("tasks") if hasattr(target_assigner, "get") else None
+    if tasks is not None and any(int(t["num_class"]) != 1 for t in tasks):
+        raise NotImplementedError("multi-class inference takes one class per task")
+    out = []
+    for g in gens:
+        if g.get("type", "anchor_generator_range") != "anchor_generator_range":
+            raise NotImplementedError("anchor generator %r: only anchor_generator_range is supported" % g.get("type"))
+        out.append(kitti_car_anchors(feature_size, anchor_range=tuple(g["anchor_ranges"]), sizes=tuple(g["sizes"]),
+                                     rotations=tuple(g["rotations"]), dtype=dtype))
+    return out
+
+
+def add_task_heads(sd, num_tasks, seed=1, cls_bias=None):
+    """Adds seeded heads ``bbox_head.tasks.1.`` ... ``tasks.{num_tasks-1}.`` (same shapes and scales as random_detector_state's
+    ``tasks.0.``) to a detector state dict, for a model with num_tasks one-class tasks; ``tasks.0.`` and everything else is kept."""
+    g = torch.Generator().manual_seed(seed)
+    for t in range(1, int(num_tasks)):
+        for nm, co in (("conv_box", 14), ("conv_cls", 2), ("conv_iou", 2), ("conv_dir", 4)):
+            sd["bbox_head.tasks.%d.%s.weight" % (t, nm)] = torch.randn((co, 128, 1, 1), generator=g) * math.sqrt(1.0 / 128)
+            sd["bbox_head.tasks.%d.%s.bias" % (t, nm)] = 0.1 * torch.randn(co, generator=g)
+        if cls_bias is not None:
+            sd["bbox_head.tasks.%d.conv_cls.bias" % t] = torch.full((2,), float(cls_bias))
+    return sd
